@@ -10,6 +10,11 @@ update, sequenced by the native host code (convnet_b200/host, the mirror of the 
 ConvNet::TrainOneBatch) through the C ABI of libconvnet_b200.so.  Nothing is skipped: dropout,
 bias, ReLU, softmax/CE and the optimizer run inside the timed region.
 
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step computed: DIR/output.npy (the net's output
+layer), DIR/params.npy and DIR/grads.npy (the parameters after its update and its gradients), float32; arrays longer than
+DUMP_SAMPLE elements are a fixed, seeded sample of it.  Inputs and initial parameters are seeded, so two builds run with
+the same arguments can be compared output for output.
+
 Prints ONE JSON line (rank 0).  `value` = images/s with the batch already resident in HBM;
 `e2e` = the same step fed from pinned HOST buffers (H2D of images+labels and D2H of the loss inside
 the timed region).  `--impl reference` times the reference's own CPU implementation of the same
@@ -34,11 +39,28 @@ WORKLOAD = ("examples/imagenet CLS_net_20140801232522 (AlexNet-style, 19 edges, 
             "batch %d per GPU, synthetic 224x224x3" % PER_GPU_BATCH)
 
 
+DUMP_SAMPLE = 1 << 22          # --dump-outputs: elements kept of a longer array (16 MiB of float32)
+
+
 def measured_peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # NVIDIA H100 SXM data sheet (dense, 700 W card): a bound, not a rate this machine was measured at
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data-sheet"
+
+
+def dump_outputs(torch, net, out_dir):
+    """what the last timed step computed, as float32 .npy files (see the module docstring)"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    for name, t in (("output", net.output_tensor()), ("params", net.params_tensor()), ("grads", net.grads_tensor())):
+        flat = t.reshape(-1).float()
+        if flat.numel() > DUMP_SAMPLE:
+            idx = np.unique(np.random.RandomState(0).randint(0, flat.numel(), DUMP_SAMPLE))
+            flat = flat[torch.from_numpy(idx).to(flat.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), flat.cpu().numpy().astype(np.float32))
 
 
 class ClockSampler:
@@ -124,7 +146,7 @@ def run_reference(args, rank, world):
 
 
 def conv_roofline(torch, lib, peaks, peak_kind, iters=10):
-    """the dominant kernel family of the step: tcgen05 implicit-GEMM conv.  Timed live (CUDA events on the
+    """the dominant kernel family of the step: the tensor-core implicit-GEMM conv.  Timed live (CUDA events on the
     launching stream) on the BASELINE headline layer: 3x3 conv fprop at batch 256 (conv4: 14x14x768 -> 384)."""
     from convnet_b200 import conv_gemm as cg
     from convnet_b200.abi import GetConvDesc
@@ -134,7 +156,7 @@ def conv_roofline(torch, lib, peaks, peak_kind, iters=10):
     x = CUDAMatrix(N, W * W * Cin, (N, W, W, Cin)); x.storage.normal_()
     w = CUDAMatrix(Cout, k * k * Cin, (Cout, k, k, Cin)); w.storage.normal_().mul_(0.02)
     y = CUDAMatrix(N, W * W * Cout, (N, W, W, Cout))
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")       # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")       # > 50 MB L2
     L = lib.load()
 
     def timed_call(flush_l2=True):
@@ -152,12 +174,12 @@ def conv_roofline(torch, lib, peaks, peak_kind, iters=10):
     ms_call = timed_call()                 # the plain ABI call: in bf16 mode it holds the two staging passes + the kernel
     path = lib.last_conv_path()
     ms = ms_call
-    if path == "tcgen05-bf16":
+    if path == "tc-bf16":
         # what the training host does (EdgeWithWeight::StageForUp): operands staged once, the call is the kernel alone
         L.convnet_b200_bf16_stage(x.ptr, x.storage.numel())
         L.convnet_b200_bf16_stage(w.ptr, w.storage.numel())
         ms = timed_call()
-        try:       # informational: back-to-back launches, no flush (the 159 MB working set already exceeds the 126 MB L2)
+        try:       # informational: back-to-back launches, no flush (the 159 MB working set already exceeds the 50 MB L2)
             ms_warm = timed_call(flush_l2=False)
         except Exception:
             ms_warm = None
@@ -165,22 +187,16 @@ def conv_roofline(torch, lib, peaks, peak_kind, iters=10):
     flops = 2.0 * N * W * W * Cout * k * k * Cin
     achieved = flops / (ms * 1e-3) / 1e12
     peak = peaks["bf16_tflops"]
-    traffic = None                          # DRAM bytes per launch from the committed ncu --set full capture of this kernel
-    if path == "tcgen05-bf16":
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "r2_conv4_fprop_fast_ncu.json")))["traffic_bytes_per_launch"]
-        except Exception:
-            traffic = None
     return {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-            "traffic": traffic, "kernel": "tc_fast_kernel<fprop, pair> (%s)" % path,
+            "kernel": "tc_conv_kernel<fprop> (%s)" % path,
             "shape": "conv4 fprop 3x3 s1 p1, 14x14x768 -> 384, batch 256 (266.3 GFLOP)", "ms_per_launch": ms,
             "back_to_back": None if not ms_warm else {"ms": ms_warm, "tflops": flops / (ms_warm * 1e-3) / 1e12,
                                                      "note": "same staged launch without the L2 flush between launches"},
             "unstaged_call": {"ms": ms_call, "tflops": flops / (ms_call * 1e-3) / 1e12,
                               "note": "same conv call with the fp32 -> bf16 staging passes of both operands inside it"},
-            "peak_source": "%s bf16 burst peak (cuBLAS); %s" % (peak_kind, {
-                "tcgen05-bf16": "bf16 operands staged beforehand (convnet_b200_bf16_stage, as the training step does), fp32 accumulate",
-                "tcgen05-tf32": "the kernel multiplies in tf32, whose tensor peak is half of bf16"}.get(path, path))}
+            "peak_source": "%s bf16 peak; %s" % (peak_kind, {
+                "tc-bf16": "bf16 operands staged beforehand (convnet_b200_bf16_stage, as the training step does), fp32 accumulate",
+                "tc-tf32": "the kernel multiplies in tf32 (mma.sync), whose tensor peak is half of bf16"}.get(path, path))}
 
 
 def main():
@@ -196,6 +212,7 @@ def main():
     ap.add_argument("--no-prefetch", action="store_true", help="e2e: copy each batch synchronously instead of one step ahead")
     ap.add_argument("--bucket-mb", type=float, default=128.0, help="gradient all-reduce bucket size")
     ap.add_argument("--no-cfg3", action="store_true", help="N > 1: skip the extra 256-images-per-GPU measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -293,6 +310,8 @@ def main():
     ms_total = timed(step_resident, args.steps)
     sampler.window(t0, time.time())
     launches = int(L.convnet_b200_launch_count())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(torch, net, args.dump_outputs)
     ev_consumed.record()
     prefetch()                                               # the first timed step's batch
     for _ in range(2):
@@ -348,9 +367,9 @@ def main():
             "vs_baseline": None, "dtype": {"tf32": "tf32", "bf16": "bf16", "fp32": "f32"}[args.precision], "data": "synthetic",
             "config": {"workload": WORKLOAD if args.model == "alexnet" else args.model, "global_batch": args.batch * world,
                        "per_gpu_batch": args.batch, "parallelism": "dp%d" % world,
-                       "arithmetic": "fp32 storage and master weights; conv/1x1/fc multiply in %s on tcgen05 with fp32 accumulate "
+                       "arithmetic": "fp32 storage and master weights; conv/1x1/fc multiply in %s on the tensor cores with fp32 accumulate "
                                      "(conv1, Cin=3, always tf32); pool/rnorm/elementwise fp32" % args.precision,
-                       "l2": "no flush needed: one step streams >3 GB of activations/weights through the 126 MB L2",
+                       "l2": "no flush needed: one step streams >3 GB of activations/weights through the 50 MB L2",
                        "sync": ("NCCL all-reduce(avg) of the flat gradient buffer in buckets of >= %.0f MB cut at layer boundaries, on "
                                 "its own stream as soon as a bucket's last wgrad is done, each followed by that bucket's SGD step on the "
                                 "optimizer stream; NCCL width %s CTAs = SMs the conv grids leave free meanwhile"

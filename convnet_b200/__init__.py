@@ -1,4 +1,4 @@
-"""convnet_b200 — B200-native (sm_100a) conv / pool / response-norm / gradient-sync hot path of
+"""convnet_b200 — H100-native (sm_90a) conv / pool / response-norm / gradient-sync hot path of
 TorontoDeepLearning/convnet behind the reference's own C ABI.
 
 The product is the C-ABI shared library convnet_b200/lib/libconvnet_b200.so

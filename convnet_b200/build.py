@@ -1,4 +1,4 @@
-"""Build convnet_b200/lib/libconvnet_b200.so in-tree with nvcc for sm_100a.
+"""Build convnet_b200/lib/libconvnet_b200.so in-tree with nvcc for sm_90a (H100).
 
 One shared object exports both reference symbol sets (ABI-1 `*Gemm`, ABI-2) plus the
 extension API.  cudart is linked statically and the driver API (cuTensorMapEncodeTiled)
@@ -16,7 +16,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libconvnet_b200.so")
 SOURCES = ["abi.cu", "ext.cu", "stage.cu", "conv_simt.cu", "conv_tc.cu", "pool.cu", "rnorm.cu", "elementwise.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
          "-ccbin", "g++"]
 # no --use_fast_math: softmax / cross-entropy / avg-pool division / the fp32 conv path are IEEE-compliant; the kernels

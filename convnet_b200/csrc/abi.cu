@@ -322,7 +322,7 @@ void ResponseNormCrossMap3DUndoGemm(cudamat* outGrads, cudamat* inputs, cudamat*
 }
 
 // =============================== ABI-2 (cudamat_conv.cuh) ====================================
-void SetupTexture(cudamat*) {}   // texture-object cache of cudamat_conv_util.cu: nothing to do on sm_100a
+void SetupTexture(cudamat*) {}   // texture-object cache of cudamat_conv_util.cu: nothing to do on sm_90a
 
 void convUp(cudamat* images, cudamat* filters, cudamat* targets, Shape4D* is, Shape4D* fs, Shape4D* ts, ConvDesc d,
             float scaleTargets) {

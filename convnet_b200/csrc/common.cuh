@@ -1,4 +1,4 @@
-// common.cuh — library-wide state and helpers (sm_100a only).
+// common.cuh — library-wide state and helpers (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -48,7 +48,7 @@ namespace cnb {
 
 // programmatic dependent launch: this CTA does not mind the NEXT kernel of the stream being placed on the machine already
 // (only kernels launched with the PDL attribute use it, and those wait for this grid's completion before their first
-// global access — conv_tc.cu: launch_fast); a no-op for every other successor
+// global access — conv_tc.cu: launch); a no-op for every other successor
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 // ... and the other half: block until every kernel this one depends on has completed and its writes are visible.  First
 // statement of every kernel that launch_pdl() starts; a no-op when the launch carried no programmatic dependency.

@@ -18,7 +18,7 @@ void simt_conv_outp(const ConvGeom& g, const float* images, const float* derivs,
 void scale_buffer(float* a, long long n, float s);
 void reduce_partials(const float* part, float* out, long long elems, int groups, int per, float st, float so);
 
-// conv_tc.cu — tcgen05 / TMA implicit GEMM (sm_100a tensor cores)
+// conv_tc.cu — TMA-fed implicit GEMM on the sm_90a tensor cores (wgmma bf16, mma.sync tf32)
 bool tc_conv_up(const ConvGeom& g, const float* images, const float* filters, float* targets,
                 float scaleTargets, float scaleOutput, const Fuse& fuse);
 int extract_patches(const float* images, float* patches, const float* width_offset, const float* height_offset, const float* flip,

@@ -259,7 +259,7 @@ __global__ void scale_kernel(float* a, long long n, float s) {
 void scale_buffer(float* a, long long n, float s) {
   if (s == 1.f || n <= 0) return;
   if (s == 0.f) { CNB_CUDA_CHECK(cudaMemsetAsync(a, 0, sizeof(float) * n, state().stream)); return; }
-  const int blocks = (int)std::min<long long>(ceil_div<long long>(n, 256), 4 * 148);
+  const int blocks = (int)std::min<long long>(ceil_div<long long>(n, 256), 4 * num_sms());
   scale_kernel<<<blocks, 256, 0, state().stream>>>(a, n, s);
   count_launch();
   CNB_LAUNCH_CHECK("scale");
@@ -303,7 +303,7 @@ void reduce_partials(const float* part, float* out, long long elems, int groups,
     return;
   }
   const long long total = elems * groups;
-  const int blocks = (int)std::min<long long>(ceil_div<long long>(total, 256), 8 * 148);
+  const int blocks = (int)std::min<long long>(ceil_div<long long>(total, 256), 8 * num_sms());
   reduce_partials_kernel<<<blocks, 256, 0, state().stream>>>(part, out, elems, groups, per, st, so);
   count_launch();
   CNB_LAUNCH_CHECK("reduce_partials");

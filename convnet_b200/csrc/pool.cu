@@ -197,8 +197,8 @@ __global__ void __launch_bounds__(256) pool_undo_kernel(PoolGeom g, const float*
 
 
 // ---- 2-D fast paths: one output ROW per block iteration ---------------------------------------------
-// The flat-index kernels above spend ~300-400 instructions per 16-byte result on index arithmetic (ncu: issue-bound at
-// 75 % issue slots, 2.8 TB/s).  Here everything that depends on the row (window rows, row base pointers) is computed
+// The flat-index kernels above spend ~300-400 instructions per 16-byte result on index arithmetic, which makes them
+// issue-bound.  Here everything that depends on the row (window rows, row base pointers) is computed
 // once per block iteration from blockIdx (uniform), the stride is a template constant (S = 0: run time), the image
 // index is a shift when N/VEC is a power of two, and per-thread offsets are 32-bit.
 template <int S> __device__ __forceinline__ int div_s(int a, int s) { return S > 0 ? a / S : a / s; }
@@ -463,8 +463,8 @@ __global__ void __launch_bounds__(256) pool_undo_masked_kernel(PoolGeom g, const
 // The same undo for stride 2, windows up to 3 x 3, organised by PATCHES: the 2 x 2 input elements whose offset from the
 // padded origin is (2*mx + a, 2*my + b) are covered by the same 2 x 2 windows {mx-1, mx} x {my-1, my}, so one thread loads
 // those four (gradient, mask) pairs once and writes four outputs.  The per-element kernel above is bound by instruction
-// issue (75 % of cycles, DRAM at 2.8 TB/s: profiles/r2_membound_kernels.md) — every element loads, unpacks and tests its
-// covering windows again; here that work is shared by the patch: 1.46x fewer instructions, 1.46x faster on pool1.  Sums run
+// issue — every element loads, unpacks and tests its covering windows again; here that work is shared by the patch (about a
+// third fewer instructions per element).  Sums run
 // over the windows in the same ascending (y, x) order as the per-element kernels: results are bit-identical to them.
 template <int VEC>
 __global__ void __launch_bounds__(256, 4) pool_undo_masked_patch_kernel(PoolGeom g, const float* __restrict__ grads,

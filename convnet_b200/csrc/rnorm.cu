@@ -28,7 +28,7 @@ namespace cnb {
 constexpr int RN_THREADS = 128;
 
 // VEC consecutive locations per thread (16-byte accesses when VEC == 4): the scalar version spent ~70 instructions per
-// channel step on one float (ncu: issue-bound at 76 % of the issue slots, 2.4 TB/s); the vector version shares the ring
+// channel step on one float, which makes it issue-bound; the vector version shares the ring
 // bookkeeping, branches and address arithmetic between four values.
 template <int VEC> __device__ __forceinline__ void rld(const float* p, float (&v)[VEC]);
 template <> __device__ __forceinline__ void rld<4>(const float* p, float (&v)[4]) {
@@ -228,8 +228,8 @@ __global__ void __launch_bounds__(RN_THREADS) rnorm_undo_kernel(const float* __r
 // ------------------------------------------------------------------------------------------------
 // Tile kernels (the default whenever one tile fits in shared memory).
 //
-// The channel walk above is a serial dependency chain per location with its loads inside the chain: ncu showed the
-// backward pass issue/latency-bound at 0.30 of the HBM peak.  Here a CTA owns a tile of TL consecutive locations x ALL
+// The channel walk above is a serial dependency chain per location with its loads inside the chain, which leaves the
+// backward pass issue/latency-bound well below the HBM bandwidth.  Here a CTA owns a tile of TL consecutive locations x ALL
 // channels and works in phases that are either fully parallel or touch shared memory only:
 //   1. the whole x (and dy) tile is fetched with 16-byte cp.async — every load of the tile is in flight at once;
 //   2. an exclusive prefix sum of x^2 along the channels is built in shared memory (a thread per (location, channel

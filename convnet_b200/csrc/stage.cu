@@ -119,7 +119,7 @@ Staged* acquire_slot(const float* ptr, long long n, int kind = 0) {
 // ---- dgrad weight banks ---------------------------------------------------------------------------------------------
 // dgrad is a stride-1 correlation of the output derivative with the flipped filters — one per stride phase (a, b) of the
 // input pixel (x = sx*i + a, y = sy*j + b), each phase seeing only the taps congruent to (a + pad) mod stride.  Run in that
-// form it uses the fprop kernel (CTA pairs, MN-major B), which needs the filters of a phase as [c fastest][tap''][o]:
+// form it uses the fprop kernel (MN-major B), which needs the filters of a phase as [c fastest][tap''][o]:
 //   bank(a,b)[c + Cin*((u' + ku*v') + ku*kv*o)] = w[o, tx = ra + sx*(ku-1-u'), ty = rb + sy*(kv-1-v'), c]
 // (reference semantics: cudamat_conv_gemm.cu:684-825, convDown = Sgemm + kContract).  The banks are a permutation of the
 // filter tensor (every tap belongs to exactly one phase), built by one small kernel and cached like a bf16 copy.

@@ -154,8 +154,8 @@ bool DataParallelSync::Init(int rank, int world, const char idbytes[128]) {
   // not the launcher (torch.distributed) initialised NCCL and its environment cache first — and the conv grids leave that
   // many SMs free while a collective is in flight (convnet_b200_reserve_sms).  0: NCCL's default width, nothing reserved.
   const char* e = getenv("CONVNET_B200_NCCL_CTAS");
-  // measured on 2 / 4 / 8 B200s (profiles/r2_scaling_timeline.md): 16 CTAs hide AlexNet's 417 MB exchange under the backward
-  // pass up to 4 ranks; at 8 ranks 16 leave the last bucket exposed and 24 do not
+  // the widths chosen to hide AlexNet's 417 MB exchange under the backward pass: 16 CTAs up to 4 ranks, 24 above (not yet
+  // retuned on H100s: ConvNet::TraceStep shows each bucket's exchange window)
   nccl_ctas_ = e ? atoi(e) : (world <= 4 ? 16 : 24);
   if (nccl_ctas_ < 0) nccl_ctas_ = 0;
   ncclComm_t c;

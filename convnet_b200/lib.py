@@ -126,7 +126,7 @@ def load():
 
 
 PRECISION = {"fp32": 0, "tf32": 1, "bf16": 2}
-PATH_NAME = {-1: "none", 0: "cuda-core-fp32", 1: "tcgen05-tf32", 2: "tcgen05-bf16"}
+PATH_NAME = {-1: "none", 0: "cuda-core-fp32", 1: "tc-tf32", 2: "tc-bf16"}
 
 
 def set_precision(mode):

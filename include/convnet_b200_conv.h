@@ -2,7 +2,7 @@
  * builds with USE_GEMM_KERNELS=no (libcudamat_conv.so), declared in
  * cudamat/cudamat_conv.cuh:8-78.  Same math as ABI-1, different signatures for
  * pooling (no scale args), response-norm undo (takes `acts`) and wgrad
- * (partial sums).  Implemented here on the SAME sm_100a kernels as ABI-1, so the
+ * (partial sums).  Implemented here on the SAME sm_90a kernels as ABI-1, so the
  * reference's own restrictions (square kernels, Cin<=3 or %4, Cout%16, batch
  * multiple of 32 — cudamat_conv_filteracts.cu:1222-1240) are NOT imposed.
  */
@@ -19,7 +19,7 @@ extern "C" {
 #pragma GCC visibility push(default)   /* the library is built with -fvisibility=hidden */
 #endif
 
-/* cudamat_conv_util.cu (texture-object cache): nothing to set up on sm_100a; no-op. */
+/* cudamat_conv_util.cu (texture-object cache): nothing to set up on sm_90a; no-op. */
 void SetupTexture(cudamat* mat);
 
 /* replaces cudamat_conv_filteracts.cu:2085 (convUp) / :2093 (localUp). */

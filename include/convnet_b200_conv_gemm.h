@@ -1,5 +1,5 @@
 /* convnet_b200_conv_gemm.h — ABI-1: the reference's DEFAULT conv library surface
- * (USE_GEMM_KERNELS=yes, libcudamat_conv_gemm.so), re-implemented for sm_100a.
+ * (USE_GEMM_KERNELS=yes, libcudamat_conv_gemm.so), re-implemented for sm_90a.
  *
  * Every entry point below replaces the reference symbol of the same name and
  * signature declared in cudamat/cudamat_conv_gemm.cuh:36-138 (definitions in

@@ -26,16 +26,16 @@ void* convnet_b200_get_stream(void);
 /* Arithmetic of the three conv ops (pool / response-norm are always fp32):
  *   0  FP32  fp32 FMA on CUDA cores (the DEFAULT: a drop-in caller gets the reference's arithmetic); meets the
  *            reference's own 1e-4 kernel test tolerance (py/test_conv.py:387); what run_grad_check uses
- *   1  TF32  tcgen05 kind::tf32 on the caller's fp32 buffers, fp32 accumulate;
+ *   1  TF32  tensor-core tf32 (mma.sync) on the caller's fp32 buffers, fp32 accumulate;
  *            Diff <= 5e-3 (operands truncated to 10 mantissa bits by the tensor core)
- *   2  BF16  tcgen05 kind::f16 on bf16 copies, fp32 accumulate; Diff <= 2e-2
+ *   2  BF16  tensor-core bf16 (wgmma) on bf16 copies, fp32 accumulate; Diff <= 2e-2
  * Shapes the tensor-core path does not take fall through to FP32.  The tensor-core modes are opt-in: this call, or
  * CONVNET_B200_PRECISION={fp32,tf32,bf16} in the environment before first use (host/ConvNet and bench.py opt in). */
 void convnet_b200_set_conv_precision(int mode);
 int convnet_b200_get_conv_precision(void);
 
-/* Which path the most recent conv call took: 0 CUDA-core fp32, 1 tcgen05 tf32,
- * 2 tcgen05 bf16, -1 none yet.  (tests assert the tensor path really ran) */
+/* Which path the most recent conv call took: 0 CUDA-core fp32, 1 tensor-core tf32,
+ * 2 tensor-core bf16, -1 none yet.  (tests assert the tensor path really ran) */
 int convnet_b200_last_conv_path(void);
 
 /* Number of kernels this library has launched since the last reset. */
@@ -68,8 +68,8 @@ void convnet_b200_pool_cache_next(void);
  * the generator of cnb_dropout — element i of the target is kept iff hash(seed + i) >= dropprob, kept values are multiplied
  * by `scale` — exactly as if cnb_dropout(target, mask, n, dropprob, scale, seed) followed the call, except that NO mask
  * tensor is written: the caller's backward pass must not need one (for a ReLU layer the kept units are the non-zero ones:
- * convnet_b200_fuse_next_scale on the dgrad that produces this layer's derivative).  The bf16 lean kernels apply it in
- * the epilogue; every other path runs one trailing pass inside the call. */
+ * convnet_b200_fuse_next_scale on the dgrad that produces this layer's derivative).  The tensor-core fprop applies it in
+ * its epilogue; every other path runs one trailing pass inside the call. */
 void convnet_b200_fuse_next_dropout(float dropprob, float scale, unsigned long long seed);
 
 /* One-shot request for the next convDown* call: do not compute anything, only prepare on the current stream what that call
@@ -79,7 +79,7 @@ void convnet_b200_fuse_next_dropout(float dropprob, float scale, unsigned long l
  * convDown finds the banks ready instead of rebuilding them on the critical path. */
 void convnet_b200_prestage_next(void);
 
-/* The conv kernels are persistent: one CTA (or CTA pair) per SM, each owning most of the SM's shared memory.  A kernel
+/* The conv kernels are persistent: one CTA per SM, each owning most of the SM's shared memory.  A kernel
  * of another library that must run CONCURRENTLY (an NCCL collective on a side stream) cannot co-reside with them and
  * would otherwise wait for — or push out — a whole wave.  convnet_b200_reserve_sms(n) makes the persistent grids leave
  * n SMs free until it is called again with 0.  (host/convnet.cc reserves the SMs of the gradient all-reduce while it

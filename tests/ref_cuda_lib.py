@@ -1,8 +1,9 @@
 """ctypes door onto oracle/_ref/libcudamat_conv_gemm_ref.so (TEST INFRASTRUCTURE).
 
 That file is the reference's own CUDA implementation of the path — cudamat/cudamat_conv_gemm.cu and
-cudamat_conv3d_gemm.cu compiled UNMODIFIED for sm_100 by oracle/Makefile — so on the GPU box it is
-"the reference on the same inputs" at BASELINE sizes, where the CPU oracle would take hours.
+cudamat_conv3d_gemm.cu compiled UNMODIFIED for sm_90 by oracle/Makefile — so on the GPU it is
+"the reference on the same inputs" at BASELINE sizes, where the CPU oracle would take hours (tests record its outputs
+into tests/golden/ref_cuda_samples.npz, see tests/test_gpu_vs_reference_cuda.py).
 It exports the same ABI-1 symbols as the product, so the product's python surface
 (convnet_b200.conv_gemm.Binding) is simply bound to it.  Only tests/ may import this module.
 """

@@ -1,4 +1,4 @@
-"""CPU-only: the C-ABI library builds for sm_100a, loads without a GPU, and exports every symbol
+"""CPU-only: the C-ABI library builds for sm_90a, loads without a GPU, and exports every symbol
 that include/*.h declares (no compute calls)."""
 import ctypes as ct
 import os
@@ -62,9 +62,9 @@ def test_abi_struct_sizes_match_reference_layout():
     assert cudamat.data_device.offset == 8 and cudamat.size.offset == 24 and cudamat.tex_obj.offset == 40
 
 
-def test_sass_is_sm100a(libpath):
+def test_sass_is_sm90a(libpath):
     out = subprocess.run(["cuobjdump", "-lelf", libpath], capture_output=True, text=True).stdout
-    assert "sm_100a" in out, out
+    assert "sm_90a" in out, out
 
 
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):

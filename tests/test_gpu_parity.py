@@ -1,13 +1,13 @@
-"""GPU parity tests (run with -m gpu on the B200 box): every C-ABI entry point of
+"""GPU parity tests (run with -m gpu on an H100): every C-ABI entry point of
 libconvnet_b200.so against the CPU oracle and the committed golden vectors.
 
 Metric: the reference's own Diff = max|a-b| / mean|a+b| (py/test_conv.py:382-385).
 Tolerances (stated once, used everywhere):
   FP32 mode (CUDA-core fp32)            : 1e-4  — the reference's own bar (py/test_conv.py:387)
-  TF32 mode (tcgen05 kind::tf32)        : 5e-3  — the tensor core reads the fp32 operands' top 19 bits
-                                                   (10-bit mantissa, truncated), fp32 accumulate; measured 2-3.5e-3
-  BF16 mode (tcgen05 kind::f16, bf16)   : 2.5e-2 — operands rounded to bf16 (8-bit mantissa, nearest even) by the
-                                                   staging pass, fp32 accumulate; measured 0.6-1.1e-2
+  TF32 mode (mma.sync tf32)             : 5e-3  — the tensor core reads the fp32 operands' top 19 bits
+                                                   (10-bit mantissa, truncated), fp32 accumulate
+  BF16 mode (wgmma, bf16 operands)      : 2.5e-2 — operands rounded to bf16 (8-bit mantissa, nearest even) by the
+                                                   staging pass, fp32 accumulate
   max-pool values                       : bit-exact
   avg-pool / pool-undo / response-norm  : 1e-4  (rnorm uses __powf like the reference GPU build)
 """
@@ -196,23 +196,23 @@ def test_conv_vs_oracle(gpu, oracle, case, mode):
 
 
 def test_tensor_core_path_is_taken(gpu):
-    """In TF32 mode the AlexNet 3x3 layers must run on tcgen05, not fall through."""
+    """In TF32 mode the AlexNet 3x3 layers must run on the tensor cores, not fall through."""
     gpu.lib.set_precision("tf32")
     d, ish, fsh, tsh, images, filters, derivs = _conv_case(CONV_CASES["alex_conv3"])
     gi, gf, gd = gpu.up(images, ish), gpu.up(filters, fsh), gpu.up(derivs, tsh)
     out = gpu.new(ish[0], derivs.shape[1], tsh); gpu.cg.convUp(gi, gf, out, d)
-    assert gpu.lib.last_conv_path() == "tcgen05-tf32"
+    assert gpu.lib.last_conv_path() == "tc-tf32"
     out = gpu.new(*images.shape, ish); gpu.cg.convDown(gd, gf, out, d)
-    assert gpu.lib.last_conv_path() == "tcgen05-tf32"
+    assert gpu.lib.last_conv_path() == "tc-tf32"
     out = gpu.new(*filters.shape, fsh); gpu.cg.convOutp(gi, gd, out, d)
-    assert gpu.lib.last_conv_path() == "tcgen05-tf32"
+    assert gpu.lib.last_conv_path() == "tc-tf32"
     gpu.lib.set_precision("bf16")
     out = gpu.new(ish[0], derivs.shape[1], tsh); gpu.cg.convUp(gi, gf, out, d)
-    assert gpu.lib.last_conv_path() == "tcgen05-bf16"
+    assert gpu.lib.last_conv_path() == "tc-bf16"
     out = gpu.new(*images.shape, ish); gpu.cg.convDown(gd, gf, out, d)
-    assert gpu.lib.last_conv_path() == "tcgen05-bf16"
+    assert gpu.lib.last_conv_path() == "tc-bf16"
     out = gpu.new(*filters.shape, fsh); gpu.cg.convOutp(gi, gd, out, d)
-    assert gpu.lib.last_conv_path() == "tcgen05-bf16"
+    assert gpu.lib.last_conv_path() == "tc-bf16"
 
 
 @pytest.mark.parametrize("mode", ["fp32", "tf32", "bf16"])

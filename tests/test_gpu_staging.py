@@ -70,7 +70,7 @@ def test_library_writes_keep_copies_coherent():
         assert staged(x) == 1
         # conv output: requested -> staged, and the copy equals a conversion of the fp32 output
         L.convnet_b200_emit_bf16_next(); cg.convUp(x, w, y, d)
-        assert lib.last_conv_path() == "tcgen05-bf16" and staged(y) == 1
+        assert lib.last_conv_path() == "tc-bf16" and staged(y) == 1
         y2 = CUDAMatrix(N, W * W * Cout, (N, W, W, Cout)); cg.convUp(x, w, y2, d)
         assert staged(y2) == 0
         # consumer results with the emitted copy == results with an explicit conversion
@@ -181,7 +181,7 @@ def test_fused_dropout_equals_the_separate_pass(precision, k, pad):
         L.convnet_b200_fuse_next(b.data_ptr(), 1, None); L.convnet_b200_fuse_next_dropout(prob, scale, seed)
         L.convnet_b200_emit_bf16_next(); cg.convUp(x, w, out, d)
         if precision == "bf16":
-            assert lib.last_conv_path() == "tcgen05-bf16"
+            assert lib.last_conv_path() == "tc-bf16"
             assert L.convnet_b200_launch_count() == 1             # bias, ReLU, dropout and the bf16 twin all in its epilogue
         assert torch.equal(out.storage, ref.storage)
         kept = (out.storage != 0).float().mean().item()
@@ -223,7 +223,7 @@ def test_prestaged_dgrad_banks_are_used_and_dropped_on_weight_writes():
         dx0 = CUDAMatrix(N, W * W * Cin, (N, W, W, Cin)); dx1 = CUDAMatrix(N, W * W * Cin, (N, W, W, Cin))
         dx1.storage.fill_(7.0)
         cg.convDown(dy, w, dx0, d)                                 # builds the banks on first use
-        assert lib.last_conv_path() == "tcgen05-bf16"
+        assert lib.last_conv_path() == "tc-bf16"
         L.convnet_b200_bf16_invalidate(None)
         L.convnet_b200_reset_launch_count()
         L.convnet_b200_prestage_next(); cg.convDown(dy, w, dx1, d)

@@ -57,7 +57,7 @@ def test_bucket_plan_partitions_the_flat_buffer(host, model, bucket):
 
 def test_default_bucket_plan_of_the_bench(host):
     """bench.py's default (--bucket-mb 128) on AlexNet: three exchanges per step — {fc8, fc7, fc6} as soon as fc6's
-    gradient exists, {conv5 ... conv2}, and conv1 alone (DESIGN.md §5, profiles/r2_scaling_timeline.md)."""
+    gradient exists, {conv5 ... conv2}, and conv1 alone (DESIGN.md §5)."""
     sizes = host.model_edge_params("alexnet")
     plan, total = host.plan_buckets(sizes, int(128 * (1 << 20) / 4))
     assert [trig for _, _, trig in plan] == [16, 3, 0]         # lowest edge of each bucket: fc6, conv2, conv1

@@ -2,11 +2,15 @@
 to the reference's own CPU implementation (eigenmat/eigenmat.cc:2046-2090), the C-ABI's argument checks, and (GPU) the
 kernel against the oracle, bit for bit."""
 import ctypes as ct
+import hashlib
+import os
 
 import numpy as np
 import pytest
 
 from oracle_lib import Oracle, RefLib
+
+GOLDEN_PATCHES = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_patches.npz")
 
 CASES = [  # N, C, W, H, pw, ph
     (5, 3, 12, 10, 7, 6),
@@ -43,11 +47,19 @@ def test_oracle_equals_the_formula_and_the_reference_cpu_code(case):
     got = np.asfortranarray(np.full(N * C * pw * ph, np.nan, np.float32))
     assert Oracle().extract_patches(images, got, wo, ho, flip, N, C, W, H, pw, ph) == 0
     assert np.array_equal(got, _numpy_reference(images, wo, ho, flip, N, C, W, H, pw, ph))
-    if not RefLib.available() or not hasattr(RefLib().lib, "ref_extract_patches"):
-        pytest.skip("oracle/_ref/libeigenmat_ref.so (with the extract_patches door) not built")
-    ref = np.asfortranarray(np.full(N * C * pw * ph, np.nan, np.float32))
-    assert RefLib().extract_patches(images, ref, wo, ho, flip, N, C, W, H, pw, ph) == 0
-    assert np.array_equal(got, ref)
+    # the reference's CPU code (eigenmat.cc extract_patches): its output's SHA-256 is stored in tests/golden/ref_patches.npz;
+    # CONVNET_B200_RECORD_REF_PATCHES=1 with oracle/_ref/libeigenmat_ref.so built compares live and re-records the file
+    key = "_".join(map(str, case))
+    digest = hashlib.sha256(got.tobytes(order="F")).hexdigest()
+    if os.environ.get("CONVNET_B200_RECORD_REF_PATCHES"):
+        assert RefLib.available() and hasattr(RefLib().lib, "ref_extract_patches"), "recording needs oracle/_ref/libeigenmat_ref.so"
+        ref = np.asfortranarray(np.full(N * C * pw * ph, np.nan, np.float32))
+        assert RefLib().extract_patches(images, ref, wo, ho, flip, N, C, W, H, pw, ph) == 0
+        assert np.array_equal(got, ref)
+        stored = dict(np.load(GOLDEN_PATCHES)) if os.path.exists(GOLDEN_PATCHES) else {}
+        stored[key] = np.array(hashlib.sha256(ref.tobytes(order="F")).hexdigest())
+        np.savez_compressed(GOLDEN_PATCHES, **stored)
+    assert digest == str(np.load(GOLDEN_PATCHES)[key][()])
 
 
 def test_argument_checks_return_the_reference_error_code():

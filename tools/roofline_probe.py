@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Run bench.py's conv roofline leg alone (conv4 fprop, batch 256, operands staged in bf16 mode) — the target of the
-`ncu --set full -k regex:tc_conv_kernel --launch-skip 19 --launch-count 1` capture under profiles/."""
+`ncu --set full -k regex:tc_conv_kernel --launch-skip 19 --launch-count 1` capture."""
 import json
 import os
 import sys

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Run ONE AlexNet training step (batch 128) between cudaProfilerStart/Stop, after two warm-up steps.
-For `ncu --profile-from-start off ...` launch lists and full captures (profiles/)."""
+For `ncu --profile-from-start off ...` launch lists and full captures."""
 import os
 import sys
 

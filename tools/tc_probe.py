@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Debug aid: run conv fprop/dgrad/wgrad in TF32 (tcgen05) mode and compare with the FP32 CUDA-core
+"""Debug aid: run conv fprop/dgrad/wgrad in TF32 (tensor-core) mode and compare with the FP32 CUDA-core
 path of the same library on the GPU (fast; the oracle-based parity lives in tests/)."""
 import os
 import sys

@@ -63,12 +63,8 @@ __host__ __device__ __forceinline__ float dropout_keep(unsigned long long x, flo
   return hash_u32(x) * (1.0f / 4294967296.0f) >= dropprob ? scale : 0.f;
 }
 
-// launch with programmatic stream serialization allowed (CONVNET_B200_NO_PDL=1: plain launch).  ONLY for kernels that
-// execute pdl_wait() before their first global access.
-inline bool pdl_enabled() {
-  static const bool on = !(getenv("CONVNET_B200_NO_PDL") && getenv("CONVNET_B200_NO_PDL")[0] == '1');
-  return on;
-}
+// launch with programmatic stream serialization allowed.  ONLY for kernels that execute pdl_wait() before their first
+// global access.
 template <typename... KArgs, typename... Args>
 inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
@@ -76,7 +72,7 @@ inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.attrs = attr; cfg.numAttrs = 1;
   CNB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...));
 }
 

@@ -634,12 +634,6 @@ void launch(const CUtensorMap& a, const CUtensorMap& b, TcParams& p) {
   CNB_LAUNCH_CHECK("tc_conv");
 }
 
-bool tc_enabled() {
-  static int en = -1;
-  if (en < 0) { const char* e = getenv("CONVNET_B200_DISABLE_TC"); en = (e && e[0] == '1') ? 0 : 1; }
-  return en == 1 && state().precision >= kPrecTF32;
-}
-
 void fill_common(TcParams& p, const ConvGeom& g, const Elem& e) {
   p.bf16 = e.bf16; p.chunk = e.chunk; p.chunk_shift = e.shift; p.cpt = BM / e.chunk; p.bk = e.bk;
   p.N = g.N; p.nb = ceil_div(g.N, 32); p.nbc = ceil_div(g.N, e.chunk);
@@ -861,7 +855,7 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
 }
 bool tc_conv_up(const ConvGeom& g, const float* images, const float* filters, float* targets, float st, float so,
                 const Fuse& fuse) {
-  if (!tc_enabled() || !g.conv) return false;
+  if (!g.conv) return false;
   if (want_bf16() && tc_conv_up_impl(g, images, filters, targets, st, so, fuse, true)) return true;
   return tc_conv_up_impl(g, images, filters, targets, st, so, fuse, false);
 }
@@ -885,7 +879,7 @@ static bool dgrad_as_fprop_eligible(const ConvGeom& g, const float* derivs, cons
 
 void tc_conv_down_prestage(const ConvGeom& g, const float* derivs, const float* filters) {
   DgradBanks banks;
-  if (!tc_enabled() || !g.conv || !want_bf16() || !dgrad_as_fprop_eligible(g, derivs, filters, &banks)) return;
+  if (!g.conv || !want_bf16() || !dgrad_as_fprop_eligible(g, derivs, filters, &banks)) return;
   dgrad_weights(filters, g, banks);
 }
 
@@ -1015,7 +1009,7 @@ static bool tc_conv_down_impl(const ConvGeom& g, const float* derivs, const floa
 }
 bool tc_conv_down(const ConvGeom& g, const float* derivs, const float* filters, float* targets, float st, float so,
                   const Fuse& fuse) {
-  if (!tc_enabled() || !g.conv) return false;
+  if (!g.conv) return false;
   if (want_bf16() && st == 0.f && tc_conv_down_as_fprop(g, derivs, filters, targets, so, fuse)) return true;
   if (want_bf16() && tc_conv_down_impl(g, derivs, filters, targets, st, so, fuse, true)) return true;
   return tc_conv_down_impl(g, derivs, filters, targets, st, so, fuse, false);
@@ -1104,7 +1098,7 @@ static bool tc_conv_outp_impl(const ConvGeom& g, const float* images, const floa
   return true;
 }
 bool tc_conv_outp(const ConvGeom& g, const float* images, const float* derivs, float* targets, float st, float so) {
-  if (!tc_enabled() || !g.conv) return false;
+  if (!g.conv) return false;
   if (want_bf16() && tc_conv_outp_impl(g, images, derivs, targets, st, so, true)) return true;
   return tc_conv_outp_impl(g, images, derivs, targets, st, so, false);
 }

@@ -374,98 +374,16 @@ __global__ void __launch_bounds__(256) pool_undo_rows_kernel(PoolGeom g, const f
   }
 }
 
-// max-pool undo from the tie masks the forward kernel recorded (convnet_b200_pool_cache_next): for an input element,
-// every covering window contributes its gradient iff the mask says this element equalled the window's maximum — the same
-// sum as pool_undo_rows_kernel<MAX>, without loading the pool input or output.  POSITIVE_ONLY: the fused ReLU' mask is the
-// pool input itself and that input is a ReLU output (>= 0): an element passes the mask iff its value — the window maximum
-// it equals — is > 0, which is bit 15.
-template <int VEC, int Q, int S, int K>
-__global__ void __launch_bounds__(256) pool_undo_masked_kernel(PoolGeom g, const float* __restrict__ grads,
-                                                               const uint16_t* __restrict__ tie_masks, float* targets,
-                                                               float st, float so, int positive_only, int nv_shift,
-                                                               __nv_bfloat16* __restrict__ targets16, float* __restrict__ rowsum) {
-  pdl_wait();
-  pdl_trigger();
-  const unsigned NV = g.N / VEC;
-  const unsigned rowlen = NV * g.W;
-  const long long in_plane = (long long)g.N * g.W * g.H * blockIdx.y, out_plane = (long long)g.N * g.modX * g.modY * blockIdx.y;
-  const float* gr_p = grads + out_plane;
-  const uint16_t* mk_p = tie_masks + out_plane;
-  float* out = targets + in_plane;
-  __nv_bfloat16* out16 = targets16 ? targets16 + in_plane : nullptr;
-  const int sx = S > 0 ? S : g.sx, sy = S > 0 ? S : g.sy;
-  float total = 0.f;
-  for (int Y = blockIdx.x; Y < g.H; Y += gridDim.x) {
-    int y0, y1;
-    cover_s<S>(Y, g.sy, g.py, g.ky, g.modY, y0, y1);
-    for (unsigned t = threadIdx.x; t < rowlen; t += blockDim.x) {
-      const unsigned X = nv_shift >= 0 ? (t >> nv_shift) : t / NV;
-      const unsigned nv = t - X * NV;
-      const unsigned idx = (unsigned)(Y * rowlen + t) * VEC;
-      int x0, x1;
-      cover_s<S>((int)X, g.sx, g.px, g.kx, g.modX, x0, x1);
-      float acc[VEC], old[VEC];
-#pragma unroll
-      for (int v = 0; v < VEC; v++) { acc[v] = 0.f; old[v] = 0.f; }
-      if (st != 0.f) vload<VEC>(out + idx, old);
-      float gr[Q * Q][VEC];
-      uint16_t mk[Q * Q][VEC];
-      bool ok[Q * Q];
-#pragma unroll
-      for (int j = 0; j < Q; j++)
-#pragma unroll
-        for (int i = 0; i < Q; i++) {
-          const int mx = x0 + i, my = y0 + j;
-          ok[j * Q + i] = mx <= x1 && my <= y1;
-          if (ok[j * Q + i]) {
-            const unsigned off = (unsigned)((my * g.modX + mx) * g.N) + nv * VEC;
-            vload<VEC>(gr_p + off, gr[j * Q + i]);
-            if (VEC == 4) {
-              const uint2 m = __ldg(reinterpret_cast<const uint2*>(mk_p + off));
-              mk[j * Q + i][0] = (uint16_t)(m.x & 0xFFFF); mk[j * Q + i][1 % VEC] = (uint16_t)(m.x >> 16);
-              mk[j * Q + i][2 % VEC] = (uint16_t)(m.y & 0xFFFF); mk[j * Q + i][3 % VEC] = (uint16_t)(m.y >> 16);
-            } else mk[j * Q + i][0] = __ldg(mk_p + off);
-          }
-        }
-#pragma unroll
-      for (int j = 0; j < Q; j++)
-#pragma unroll
-        for (int i = 0; i < Q; i++)
-          if (ok[j * Q + i]) {
-            const int bit = ((int)X - ((x0 + i) * sx + g.px)) + K * (Y - ((y0 + j) * sy + g.py));     // element's place in that window
-            const uint16_t need = (uint16_t)((1u << bit) | (positive_only ? 0x8000u : 0u));
-#pragma unroll
-            for (int v = 0; v < VEC; v++) acc[v] += ((mk[j * Q + i][v] & need) == need) ? so * gr[j * Q + i][v] : 0.f;
-          }
-#pragma unroll
-      for (int v = 0; v < VEC; v++) acc[v] += st * old[v];
-      vstore<VEC>(out + idx, acc);
-      if (out16) vemit<VEC>(out16 + idx, acc);
-      if (rowsum) {
-#pragma unroll
-        for (int v = 0; v < VEC; v++) total += acc[v];
-      }
-    }
-  }
-  if (rowsum) {
-    __shared__ float sh[8];
-    for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = total;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      float s = 0.f;
-      for (int w = 0; w < 8; w++) s += sh[w];
-      rowsum[(size_t)blockIdx.x * gridDim.y + blockIdx.y] = s;
-    }
-  }
-}
-
-// The same undo for stride 2, windows up to 3 x 3, organised by PATCHES: the 2 x 2 input elements whose offset from the
-// padded origin is (2*mx + a, 2*my + b) are covered by the same 2 x 2 windows {mx-1, mx} x {my-1, my}, so one thread loads
-// those four (gradient, mask) pairs once and writes four outputs.  The per-element kernel above is bound by instruction
-// issue — every element loads, unpacks and tests its covering windows again; here that work is shared by the patch (about a
-// third fewer instructions per element).  Sums run
-// over the windows in the same ascending (y, x) order as the per-element kernels: results are bit-identical to them.
+// max-pool undo from the tie masks the forward kernel recorded (convnet_b200_pool_cache_next), stride 2, windows up to
+// 3 x 3: every window covering an input element contributes its gradient iff the mask says this element equalled the
+// window's maximum — the same sum as pool_undo_rows_kernel<MAX>, without loading the pool input or output.  positive_only:
+// the fused ReLU' mask is the pool input itself and that input is a ReLU output (>= 0): an element passes the mask iff its
+// value — the window maximum it equals — is > 0, which is bit 15.
+// Organised by PATCHES: the 2 x 2 input elements whose offset from the padded origin is (2*mx + a, 2*my + b) are covered by
+// the same 2 x 2 windows {mx-1, mx} x {my-1, my}, so one thread loads those four (gradient, mask) pairs once and writes
+// four outputs.  The undo is bound by instruction issue; sharing the loads, unpacking and tests of the covering windows
+// across a patch saves about a third of the instructions per element.  Sums run over the windows in the same ascending
+// (y, x) order as the compare-based kernels: results are bit-identical to them.
 template <int VEC>
 __global__ void __launch_bounds__(256, 4) pool_undo_masked_patch_kernel(PoolGeom g, const float* __restrict__ grads,
                                                                      const uint16_t* __restrict__ tie_masks, float* targets,
@@ -670,14 +588,12 @@ static unsigned long long pool_sig(const PoolGeom& g) {
   for (int v : {g.N, g.W, g.H, g.C, g.modX, g.modY, g.kx, g.ky, g.sx, g.sy, g.px, g.py}) sig = (sig ^ (unsigned)v) * 1099511628211ULL;
   return sig;
 }
-// CONVNET_B200_POOL_PATCH=0: the per-element undo kernels instead of the patch kernels (A/B measurements)
-static bool pool_patch_enabled() {
-  static const bool on = !(getenv("CONVNET_B200_POOL_PATCH") && getenv("CONVNET_B200_POOL_PATCH")[0] == '0');
-  return on;
-}
-
-static bool masks_supported(const PoolGeom& g) {      // the row kernels, windows up to 3 x 3 (9 tie bits + the sign bit)
-  return g.kt == 1 && g.T == 1 && g.modT == 1 && std::max(g.kx, g.ky) <= 3 && g.sx == g.sy && (long long)g.N * g.W * g.H < (1LL << 31);
+// the geometry of the patch kernels: 2-D, stride 2, windows up to 3 x 3 with a side of 3 (at most 2 x 2 covering windows),
+// padding offsets in [-2, 0], in-plane offsets in 32 bits.  The forward pass records tie masks (pool_fwd_rows_kernel<K = 3>
+// bit layout) for exactly this geometry, the only one whose undo reads them.
+static bool patch_geometry(const PoolGeom& g) {
+  return g.kt == 1 && g.T == 1 && g.modT == 1 && std::max(g.kx, g.ky) == 3 && g.sx == 2 && g.sy == 2 && g.px <= 0 &&
+         g.py <= 0 && g.px >= -2 && g.py >= -2 && (long long)g.N * g.W * g.H < (1LL << 31);
 }
 
 template <int VEC, bool MAX>
@@ -711,9 +627,9 @@ bool pool_forward(const PoolGeom& g, bool is_max, const float* images, float* ta
                   bool cache_masks) {
   const bool v4 = (g.N % 4 == 0) && aligned16(images) && aligned16(targets);
   const long long outs = (long long)g.modX * g.modY * g.C * g.modT;
-  // tie masks for the matching undo: only from the row kernels with K == 3 bit layout (k <= 3), unscaled outputs
+  // tie masks for the matching undo: unscaled outputs only
   uint16_t* masks = nullptr;
-  if (cache_masks && is_max && so == 1.f && masks_supported(g) && std::max(g.kx, g.ky) == 3)
+  if (cache_masks && is_max && so == 1.f && patch_geometry(g))
     masks = pool_masks_slot(targets, outs * g.N, images, (long long)g.N * g.W * g.H * g.C, pool_sig(g));
   bool emitted;
   if (v4) {
@@ -744,36 +660,22 @@ static bool launch_undo(const PoolGeom& g, const float* images, const float* gra
     const dim3 rgrid((unsigned)g.H, planes);
     const int sh = pow2_shift(g.N / VEC);
     const int S = (g.sx == g.sy && g.sx <= 2) ? g.sx : 0;
-    // the forward pass left tie masks for exactly this (input, output) pair and nothing wrote either since: no need to
-    // reload and compare them.  A fused ReLU' mask is only expressible when it IS the pool input (bit 15 = maximum > 0).
-    // (with scaleTargets != 0 the compare path also zeroes the OLD target where the mask fails; the tie masks cannot say
-    // that for elements that are no window's maximum, so that combination stays on the compare path)
-    if (MAX && q == 2 && std::max(g.kx, g.ky) == 3 && masks_supported(g) && (mask == nullptr || (mask == images && st == 0.f))) {
-      const uint16_t* tm = pool_masks_find(acts, (long long)g.N * g.modX * g.modY * g.C, images, pool_sig(g));
-      if (tm) {
-        const int pos = mask != nullptr ? 1 : 0;
-        if (S == 2 && g.px <= 0 && g.py <= 0 && g.px >= -2 && g.py >= -2 && pool_patch_enabled()) {
-          // patches: element X belongs to patch (X - px) / 2; the first patch holds X = 0, the last X = W - 1
-          const int PX = (g.W - 1 - g.px) / 2 + 1, PY = (g.H - 1 - g.py) / 2 + 1;
-          const int shp = pow2_shift(g.N / VEC);
-          if (colsum && colsum_slices) *colsum_slices = PY;
-          launch_pdl(pool_undo_masked_patch_kernel<VEC>, dim3((unsigned)PY, planes), dim3(256), 0, s, g, grads, tm, targets, st, so, pos,
-                     shp, t16, colsum, PX, PY);
-          return t16 != nullptr;
-        }
-        if (colsum && colsum_slices) *colsum_slices = g.H;
-        if (S == 2) pool_undo_masked_kernel<VEC, 2, 2, 3><<<rgrid, 256, 0, s>>>(g, grads, tm, targets, st, so, pos, sh, t16, colsum);
-        else if (S == 1) pool_undo_masked_kernel<VEC, 2, 1, 3><<<rgrid, 256, 0, s>>>(g, grads, tm, targets, st, so, pos, sh, t16, colsum);
-        else pool_undo_masked_kernel<VEC, 2, 0, 3><<<rgrid, 256, 0, s>>>(g, grads, tm, targets, st, so, pos, sh, t16, colsum);
-        return t16 != nullptr;
-      }
-    }
-    if (MAX && S == 2 && q == 2 && std::max(g.kx, g.ky) <= 3 && g.px <= 0 && g.py <= 0 && g.px >= -2 && g.py >= -2 &&
-        pool_patch_enabled()) {
+    if (MAX && patch_geometry(g)) {
+      // patches: element X belongs to patch (X - px) / 2; the first patch holds X = 0, the last X = W - 1
       const int PX = (g.W - 1 - g.px) / 2 + 1, PY = (g.H - 1 - g.py) / 2 + 1;
       if (colsum && colsum_slices) *colsum_slices = PY;
-      launch_pdl(pool_undo_patch_kernel<VEC>, dim3((unsigned)PY, planes), dim3(256), 0, s, g, images, grads, acts, targets, st, so, mask,
-                 sh, t16, colsum, PX, PY);
+      // the forward pass left tie masks for exactly this (input, output) pair and nothing wrote either since: no need to
+      // reload and compare them.  A fused ReLU' mask is only expressible when it IS the pool input (bit 15 = maximum > 0).
+      // (with scaleTargets != 0 the compare path also zeroes the OLD target where the mask fails; the tie masks cannot say
+      // that for elements that are no window's maximum, so that combination stays on the compare path)
+      const uint16_t* tm = mask == nullptr || (mask == images && st == 0.f)
+                               ? pool_masks_find(acts, (long long)g.N * g.modX * g.modY * g.C, images, pool_sig(g)) : nullptr;
+      if (tm)
+        launch_pdl(pool_undo_masked_patch_kernel<VEC>, dim3((unsigned)PY, planes), dim3(256), 0, s, g, grads, tm, targets, st, so,
+                   mask != nullptr ? 1 : 0, sh, t16, colsum, PX, PY);
+      else
+        launch_pdl(pool_undo_patch_kernel<VEC>, dim3((unsigned)PY, planes), dim3(256), 0, s, g, images, grads, acts, targets, st,
+                   so, mask, sh, t16, colsum, PX, PY);
       return t16 != nullptr;
     }
     if (colsum && colsum_slices) *colsum_slices = g.H;

@@ -119,12 +119,13 @@ __global__ void __launch_bounds__(RN_THREADS) rnorm_fwd_kernel(const float* __re
   }
 }
 
-template <bool BLOCKED, int VEC>
+template <bool BLOCKED>
 __global__ void __launch_bounds__(RN_THREADS) rnorm_undo_kernel(const float* __restrict__ dy, const float* __restrict__ x,
                                                                  float* __restrict__ dx, long long L, int F, int k,
                                                                  float alpha, float beta, float* gring, long long gstride,
                                                                  int seg) {
   // three rings of k entries per thread: x, t = dy*x*denom, p = dy*denom^(beta/(beta+1))
+  constexpr int VEC = 1;                                 // one location per thread (launch_undo)
   extern __shared__ __align__(16) float sring[];
   const long long loc = (blockIdx.x * (long long)RN_THREADS + threadIdx.x) * VEC;
   if (loc >= L) return;
@@ -169,7 +170,7 @@ __global__ void __launch_bounds__(RN_THREADS) rnorm_undo_kernel(const float* __r
   const int Qend = f1 + a + b;                           // last output f1-1 needs t up to f1-1+a, i.e. q up to f1-1+a+b
   // ring slots of q, i = q - b and j = i - a, advanced with wrap instead of three `% k` per channel
   int slot_q = q0 % k, slot_i = ((q0 - b) % k + k) % k, slot_j = ((q0 - b - a) % k + k) % k;
-  constexpr int U = VEC == 4 ? 2 : 4;
+  constexpr int U = 4;
   for (int qb = q0; qb < Qend; qb += U) {
     float xv[U][VEC], gv[U][VEC];
 #pragma unroll
@@ -394,8 +395,6 @@ __global__ void __launch_bounds__(RN_THREADS) rnorm_undo_tile_kernel(const float
 // share an SM, else the widest that fits at all; 0 = no tile kernel (window walk with the ring instead)
 static int pick_tile(int F, int arrays, size_t* smem_out) {
   auto bytes = [&](int tl) { return sizeof(float) * ((size_t)arrays * (F + 1) * tl + RN_THREADS); };
-  static const int forced = getenv("CONVNET_B200_RNORM_TL") ? atoi(getenv("CONVNET_B200_RNORM_TL")) : 0;     // experiments
-  if ((forced == 32 || forced == 64) && bytes(forced) <= 220 * 1024) { *smem_out = bytes(forced); return forced; }
   // a CTA works in phases (load everything, scan, compute, store): the loads of one CTA only overlap the arithmetic of
   // ANOTHER one on the same SM, so prefer the width that leaves room for >= 3 resident CTAs, then 2, then whatever fits
   const size_t sm = 224 * 1024;
@@ -404,20 +403,15 @@ static int pick_tile(int F, int arrays, size_t* smem_out) {
       if (bytes(tl) + 1024 <= sm / per_sm) { *smem_out = bytes(tl); return tl; }
   return 0;
 }
-static bool rn_tile_enabled() {
-  static const bool off = getenv("CONVNET_B200_RNORM_NO_TILE") && getenv("CONVNET_B200_RNORM_NO_TILE")[0] == '1';
-  return !off;
-}
 
 static constexpr size_t kMaxRingSmem = 160 * 1024;
 
 // channel segments per location: 1 unless the location count cannot fill the GPU
-static int pick_segments(long long L, int F, int k, bool blocked) {
+static int pick_segments(long long L, int F, int k) {
   const long long blocks = ceil_div<long long>(L, RN_THREADS);
   const long long want = ceil_div<long long>(2LL * num_sms(), blocks);
   int segs = (int)std::min<long long>(want, std::max(1, F / std::max(k, 1)));      // segment >= k: halo <= 2x / 3x reads
   if (segs < 1) segs = 1;
-  (void)blocked;
   return segs;
 }
 
@@ -427,7 +421,7 @@ template <int VEC>
 static void launch_fwd(const float* images, float* targets, long long L, int F, int k, float alpha, float beta, bool blocked) {
   const long long owners = L / VEC;                      // threads needed
   const int blocks = (int)ceil_div<long long>(owners, RN_THREADS);
-  int segs = pick_segments(owners, F, k, blocked);
+  int segs = pick_segments(owners, F, k);
   int seg = ceil_div(F, segs);
   if (blocked) seg = ceil_div(seg, k) * k;
   segs = ceil_div(F, seg);
@@ -470,7 +464,7 @@ void rnorm_forward(const float* images, float* targets, long long L, int F, int 
                    bool blocked, bool relu, __nv_bfloat16* targets_bf16) {
   CNB_REQUIRE(k >= 1 && F >= 1, "ResponseNormCrossMap");
   size_t tsmem = 0;
-  const int tl = rn_tile_enabled() && L < (1LL << 31) * 32 ? pick_tile(F, 2, &tsmem) : 0;
+  const int tl = L < (1LL << 31) * 32 ? pick_tile(F, 2, &tsmem) : 0;
   if (tl) {
     const bool vec = L % 4 == 0 && rn_aligned16(images) && rn_aligned16(targets) &&
                      (!targets_bf16 || (reinterpret_cast<uintptr_t>(targets_bf16) & 7) == 0);
@@ -491,30 +485,31 @@ void rnorm_forward(const float* images, float* targets, long long L, int F, int 
   CNB_LAUNCH_CHECK("rnorm_forward");
 }
 
-template <int VEC>
+// one location per thread: the backward walk carries three rings and two dependent stages per channel, so it is
+// latency-bound, and a version with four locations per thread (a quarter of the threads, 4x the shared memory per block)
+// was slower when measured before the port to the H100
 static void launch_undo(const float* outGrads, const float* inputs, float* targets, long long L, int F, int k, float alpha,
                         float beta, bool blocked) {
-  const long long owners = L / VEC;
-  const int blocks = (int)ceil_div<long long>(owners, RN_THREADS);
-  int segs = pick_segments(owners, F, k, blocked);
+  const int blocks = (int)ceil_div<long long>(L, RN_THREADS);
+  int segs = pick_segments(L, F, k);
   int seg = ceil_div(F, segs);
   if (blocked) seg = ceil_div(seg, k) * k;
   segs = ceil_div(F, seg);
-  size_t smem = sizeof(float) * 3 * (size_t)k * RN_THREADS * VEC;
+  size_t smem = sizeof(float) * 3 * (size_t)k * RN_THREADS;
   float* gring = nullptr;
   if (smem > kMaxRingSmem) { gring = (float*)workspace(sizeof(float) * 3 * (size_t)k * L * segs); smem = 0; }
-  auto kern = blocked ? rnorm_undo_kernel<true, VEC> : rnorm_undo_kernel<false, VEC>;
+  auto kern = blocked ? rnorm_undo_kernel<true> : rnorm_undo_kernel<false>;
   if (smem > 48 * 1024) CNB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<dim3(blocks, segs), RN_THREADS, smem, state().stream>>>(outGrads, inputs, targets, L, F, k, alpha, beta, gring, L, seg);
 }
 
-bool rnorm_can_fuse(int F) { size_t b; return rn_tile_enabled() && pick_tile(F, 2, &b) != 0; }
+bool rnorm_can_fuse(int F) { size_t b; return pick_tile(F, 2, &b) != 0; }
 
 void rnorm_undo(const float* outGrads, const float* inputs, float* targets, long long L, int F, int k,
                 float alpha, float beta, bool blocked) {
   CNB_REQUIRE(k >= 1 && F >= 1, "ResponseNormCrossMapUndo");
   size_t tsmem = 0;
-  const int tl = rn_tile_enabled() ? pick_tile(F, 4, &tsmem) : 0;
+  const int tl = pick_tile(F, 4, &tsmem);
   if (tl) {
     const bool vec = L % 4 == 0 && rn_aligned16(outGrads) && rn_aligned16(inputs) && rn_aligned16(targets);
     if (tl == 64) launch_undo_tile<64>(outGrads, inputs, targets, L, F, k, alpha, beta, blocked, tsmem, vec);
@@ -523,12 +518,7 @@ void rnorm_undo(const float* outGrads, const float* inputs, float* targets, long
     CNB_LAUNCH_CHECK("rnorm_undo(tile)");
     return;
   }
-  // the backward walk carries three rings and two dependent stages per channel: it is latency-bound, and the vector
-  // version (a quarter of the threads, 4x the shared memory per block) measured SLOWER (210 -> 333 us); opt-in only
-  static const bool wide_undo = getenv("CONVNET_B200_RNORM_UNDO_VEC4") && getenv("CONVNET_B200_RNORM_UNDO_VEC4")[0] == '1';
-  if (wide_undo && L % 4 == 0 && rn_aligned16(outGrads) && rn_aligned16(inputs) && rn_aligned16(targets))
-    launch_undo<4>(outGrads, inputs, targets, L, F, k, alpha, beta, blocked);
-  else launch_undo<1>(outGrads, inputs, targets, L, F, k, alpha, beta, blocked);
+  launch_undo(outGrads, inputs, targets, L, F, k, alpha, beta, blocked);
   count_launch();
   CNB_LAUNCH_CHECK("rnorm_undo");
 }

@@ -193,8 +193,6 @@ namespace {
 bool want_bf16() { return state().precision == kPrecBF16; }
 
 void to_bf16(const float* src, __nv_bfloat16* dst, long long n) {
-  static const int dbg = getenv("CONVNET_B200_TC_DEBUG") ? atoi(getenv("CONVNET_B200_TC_DEBUG")) : 0;
-  if (dbg & 4) return;
   const long long n8 = n >> 3;
   const int grid = (int)std::min<long long>(std::max<long long>(ceil_div<long long>(n8, 256), 1), 8LL * num_sms());
   cvt_bf16_kernel<<<grid, 256, 0, state().stream>>>(src, dst, n);

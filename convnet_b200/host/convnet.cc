@@ -204,15 +204,12 @@ ConvNet::ConvNet(const ModelConfig& model, int batch_size) : model_(model), batc
     edges_.push_back(e);
   }
   // epilogue fusion of the Layer-side ReLU / ReLU' into the neighbouring edges (SURVEY.md 8(f) rank 2)
-  const char* nf = getenv("CONVNET_B200_NO_FUSE");
-  if (!(nf && nf[0] == '1')) {
-    for (size_t i = 0; i < edges_.size(); i++) {
-      Layer *src = layers_[i], *dst = layers_[i + 1];
-      if (dst->GetActivation() == RECTIFIED_LINEAR) {
-        edges_[i]->SetFuseReLU(true);              // honoured only where CanFuseReLU() (checked after SetImageSize below)
-      }
-      if (!src->IsInput() && src->GetActivation() == RECTIFIED_LINEAR) edges_[i]->SetFuseMask(true);
+  for (size_t i = 0; i < edges_.size(); i++) {
+    Layer *src = layers_[i], *dst = layers_[i + 1];
+    if (dst->GetActivation() == RECTIFIED_LINEAR) {
+      edges_[i]->SetFuseReLU(true);                // honoured only where CanFuseReLU() (checked after SetImageSize below)
     }
+    if (!src->IsInput() && src->GetActivation() == RECTIFIED_LINEAR) edges_[i]->SetFuseMask(true);
   }
   // SetImageSize propagation (convnet.cc:226-268)
   const LayerConfig& in = model.layer.front();
@@ -291,13 +288,10 @@ void ConvNet::AllocateMemory() {
   HOST_CUDA_CHECK(cudaEventCreateWithFlags(&ev_main_, cudaEventDisableTiming));
   HOST_CUDA_CHECK(cudaEventCreateWithFlags(&ev_side_, cudaEventDisableTiming));
   SetBucketFloats((size_t)8 << 20);
-  static const bool no_lane = getenv("CONVNET_B200_NO_SIDE_BIAS_GRAD") && getenv("CONVNET_B200_NO_SIDE_BIAS_GRAD")[0] == '1';
-  if (!no_lane) {
-    lane_.stream = side_;
-    HOST_CUDA_CHECK(cudaEventCreateWithFlags(&lane_.ready, cudaEventDisableTiming));
-    for (Edge* e : edges_)
-      if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(e)) w->SetSideLane(&lane_);
-  }
+  lane_.stream = side_;
+  HOST_CUDA_CHECK(cudaEventCreateWithFlags(&lane_.ready, cudaEventDisableTiming));
+  for (Edge* e : edges_)
+    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(e)) w->SetSideLane(&lane_);
 }
 
 void ConvNet::Fprop(bool train) {                            // convnet.cc:377-388
@@ -380,8 +374,7 @@ void ConvNet::Bprop() {                                      // convnet.cc:390-4
       const bool drop_pass = in->HasDropout() && !fold;
       e->SetEmitDown(want_in && !drop_pass && !in->HasSeparateDerivPass());
       // the kernel that writes in's derivative LAST can also sum its channels: that is the bias gradient of the edge below
-      static const bool no_bg = getenv("CONVNET_B200_NO_FUSED_BIAS_GRAD") && getenv("CONVNET_B200_NO_FUSED_BIAS_GRAD")[0] == '1';
-      if (!no_bg && i >= 2 && e->CanProduceBiasGrad() && !drop_pass && !in->HasSeparateDerivPass()) {
+      if (i >= 2 && e->CanProduceBiasGrad() && !drop_pass && !in->HasSeparateDerivPass()) {
         Edge::BiasGradTarget t;
         if (edges_[i - 2]->OfferFusedBiasGrad(&t)) e->SetBiasGradRequest(t);
       }
@@ -459,11 +452,10 @@ void ConvNet::TrainOneBatch(float* loss_out) {               // convnet.cc:475-4
   if (loss_out) {                                            // GetLoss: one scalar D2H per step, like the reference
     cnb_sum(OutputLayer().GetLossPerImage(), loss_sum_.GetDevData(), batch_size_);
   }
-  static const bool no_eager = getenv("CONVNET_B200_NO_EAGER_UPDATE") && getenv("CONVNET_B200_NO_EAGER_UPDATE")[0] == '1';
-  eager_update_ = !no_eager;
+  eager_update_ = true;
   Bprop();
   if (trace_.on) HOST_CUDA_CHECK(cudaEventRecord(trace_.bwd, Matrix::Stream()));
-  updated_in_bprop_ = eager_update_;
+  updated_in_bprop_ = true;
   eager_update_ = false;
   UpdateWeights();
   if (trace_.on) HOST_CUDA_CHECK(cudaEventRecord(trace_.end, Matrix::Stream()));

@@ -84,7 +84,6 @@ void EdgeWithWeight::StageForBprop(Matrix& deriv_output) {
   if (bf_outer_ == 1 || bf_down_ == 1) convnet_b200_bf16_ensure(deriv_output.GetDevData(), (long long)deriv_output.GetNumEls());
 }
 void EdgeWithWeight::SumBiasRows(Matrix& deriv_output, float scale_targets, float scale) {
-  if (!side_ || !side_->stream) { deriv_output.SumRows(grad_bias_, scale_targets, scale); return; }
   cudaEventRecord(side_->ready, Matrix::Stream());            // the derivative is final on the main stream
   cudaStreamWaitEvent(side_->stream, side_->ready, 0);
   void* main_stream = convnet_b200_get_stream();

@@ -142,7 +142,7 @@ class Edge {
 
 // The side stream of ConvNet::TrainOneBatch (all-reduce + optimizer, see convnet.h): bias-gradient column sums are
 // memory-bound passes over a derivative that is already final, so they run there, beside the tensor-bound wgrad / dgrad
-// kernels of the main stream.  Null stream: everything stays on the main stream.
+// kernels of the main stream.  ConvNet::AllocateMemory gives every weighted edge the lane together with its gradient memory.
 struct SideLane { cudaStream_t stream = nullptr; cudaEvent_t ready = nullptr; bool used = false; };
 
 class EdgeWithWeight : public Edge {
@@ -181,7 +181,7 @@ class EdgeWithWeight : public Edge {
  protected:
   void StageForUp(Matrix& input);
   void StageForBprop(Matrix& deriv_output);
-  void SumBiasRows(Matrix& deriv_output, float scale_targets, float scale);      // SumRows on the side lane when there is one
+  void SumBiasRows(Matrix& deriv_output, float scale_targets, float scale);      // SumRows on the side lane
   SideLane* side_ = nullptr;
   void NoteUp();
   void NoteDown();

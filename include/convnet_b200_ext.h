@@ -61,7 +61,8 @@ void convnet_b200_fuse_next_scale(float scale);
  * memory-bound pass of the step, bit-identical results (ties duplicate the gradient exactly as kMaxPoolUndo's `==` test
  * does, cudamat_conv_gemm.cu:262-300).  The masks go stale, and the undo falls back to comparing, as soon as any entry
  * point of this library writes either tensor; a caller that overwrites them by other means between the two calls must
- * not use this request (or must call convnet_b200_bf16_invalidate(NULL)).  2-D windows up to 3 x 3. */
+ * not use this request (or must call convnet_b200_bf16_invalidate(NULL)).  2-D windows up to 3 x 3 with a side of 3,
+ * stride 2, padding up to 2; other pools ignore the request. */
 void convnet_b200_pool_cache_next(void);
 
 /* One-shot request for the next convUp* call (after its bias / ReLU, if those are requested too): dropout of the result with

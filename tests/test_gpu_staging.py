@@ -92,13 +92,13 @@ def test_library_writes_keep_copies_coherent():
         lib.set_precision("fp32")
 
 
-@pytest.mark.parametrize("pad", [1, 0])
+@pytest.mark.parametrize("pad", [1, 0, 3])
 @pytest.mark.parametrize("shape", [(128, 27, 27, 64), (32, 110, 110, 8), (7, 9, 9, 5), (4, 8, 8, 3)])
 def test_max_pool_undo_from_tie_masks_is_bit_identical(shape, pad):
     """convnet_b200_pool_cache_next: the undo fed by the forward pass's tie masks equals the compare-based undo bit for bit —
     with ties (quantised inputs), with scaleTargets, with the fused ReLU' mask that is the pool input (that mask together
-    with scaleTargets != 0 stays on the compare path), odd and even widths, with and without padding — and it falls back
-    as soon as the library writes one of the two tensors."""
+    with scaleTargets != 0 stays on the compare path), odd and even widths, with and without padding (padding 3 records no
+    masks: both undos compare) — and it falls back as soon as the library writes one of the two tensors."""
     import torch
     from convnet_b200 import conv_gemm as cg
     from convnet_b200 import lib

@@ -2,6 +2,7 @@
 // (bias add, bias gradient, ReLU, SGD).  See include/convnet_b200_ext.h for the reference
 // call sites they correspond to.  All are single-pass, float4-vectorised where aligned.
 #include <algorithm>
+#include <vector>
 
 #include <cuda_bf16.h>
 
@@ -104,46 +105,172 @@ __global__ void relu_deriv_kernel(float* dx, const float* __restrict__ y, long l
   }
   for (long long i = 4 * n4 + tid; i < n; i += nt) dx[i] = y[i] > 0.f ? dx[i] : 0.f;
 }
-// Multi-tensor SGD with momentum and L2 decay: ONE launch updates every tensor of a batch (an all-reduce bucket, or the
-// whole net).  A block owns kSgdChunk consecutive elements of one tensor; the block -> tensor map is a prefix table that
-// travels in the kernel parameters (no device-side descriptor to keep coherent).  Tensors whose staged bf16 copy exists
-// (conv weights in bf16 mode) get it refreshed from the same registers.
-constexpr int kSgdMaxTensors = 48, kSgdChunk = 4096;
-struct SgdItem { float* w; float* h; const float* g; __nv_bfloat16* w16; long long n; float lr, mom, l2; int vec; };
-struct SgdBatch { int count; int first_block[kSgdMaxTensors + 1]; SgdItem t[kSgdMaxTensors]; };
+// Multi-tensor SGD (SGDOptimizer::Optimize, src/optimizer.cc:174-200): ONE launch updates every tensor of a batch (an
+// all-reduce bucket, or the whole net).  The block -> tensor map is a prefix table that travels in the kernel parameters
+// (no device-side descriptor to keep coherent).  Tensors whose staged bf16 copy exists (conv weights in bf16 mode) get it
+// refreshed from the same registers.
+//   Plain tensors: a block owns kSgdChunk consecutive elements.
+//   Row-norm tensors (weight_norm_limit / weight_norm_constraint): the tensor is [rows x K] with the rows fastest, row r =
+//   the elements r + rows*k (one output unit's incoming weights, DESIGN.md §3).  A block owns a tile of up to 128 rows x
+//   (8192 / tile rows) columns, and while it stores the updated weights it also sums their squares per row; the tile's
+//   per-row sums go to part[slab * rows + r] (slab = the tile's column range) in a fixed order — no atomics, so the
+//   result is bit-reproducible.  norm_rescale_kernel then finishes the norms and rescales the rows that need it.
+constexpr int kSgdMaxTensors = 48, kSgdChunk = 4096, kNormTile = 8192, kNormRescaleRows = 32;
+enum { kNormNone = 0, kNormLimit = 1, kNormConstraint = 2 };
+struct SgdItem {
+  float* w; float* h; const float* g; __nv_bfloat16* w16; float* part;   // part: row-norm partial sums (norm tensors)
+  long long n; float lr, mom, l2, clip, norm; int rows, mode, vec;
+};
+struct SgdBatch { int count; int first_block[kSgdMaxTensors + 1]; SgdItem t[kSgdMaxTensors]; };   // <= 4 KB of parameters
 
-__global__ void __launch_bounds__(256) sgd_multi_kernel(const __grid_constant__ SgdBatch b) {
+__device__ __forceinline__ int batch_item(const SgdBatch& b) {
   int ti = 0;
   while (ti + 1 < b.count && (int)blockIdx.x >= b.first_block[ti + 1]) ti++;      // <= 48 uniform steps
-  const SgdItem& t = b.t[ti];
-  const long long e0 = (long long)((int)blockIdx.x - b.first_block[ti]) * kSgdChunk;
+  return ti;
+}
+// one element: g += l2*w; clip g to [-clip, clip]; h = mom*h + lr*g; w -= h.  Written out with explicit roundings so that
+// every tensor, and every block mapping, computes the same bits (the fused l2 term and the h update are single FMAs).
+__device__ __forceinline__ void sgd1(float& w, float& h, float g, const SgdItem& t) {
+  float d = __fmaf_rn(t.l2, w, g);
+  if (t.clip > 0.f) d = d > t.clip ? t.clip : (d < -t.clip ? -t.clip : d);     // UpperBoundMod (keeps NaN)
+  h = __fmaf_rn(t.mom, h, __fmul_rn(t.lr, d));
+  w = __fsub_rn(w, h);
+}
+__host__ __device__ inline int norm_tile_rows(int rows) {                      // power of two <= 128
+  int r = 1;
+  while (r < rows && r < 128) r <<= 1;
+  return r;
+}
+__host__ __device__ inline long long norm_slabs(const SgdItem& t) {
+  return ceil_div<long long>(t.n / t.rows, kNormTile / norm_tile_rows(t.rows));
+}
+
+__device__ void sgd_chunk(const SgdItem& t, int block) {
+  const long long e0 = (long long)block * kSgdChunk;
   const long long e1 = min(t.n, e0 + kSgdChunk);
   if (t.vec) {                                                                     // all pointers 16-byte aligned
     for (long long i = e0 + 4 * threadIdx.x; i < e1; i += 4 * 256) {
       if (i + 4 <= e1) {
         float4 w = *reinterpret_cast<const float4*>(t.w + i), h = *reinterpret_cast<const float4*>(t.h + i);
         const float4 g = __ldg(reinterpret_cast<const float4*>(t.g + i));
-        h.x = t.mom * h.x + t.lr * (g.x + t.l2 * w.x); w.x -= h.x;
-        h.y = t.mom * h.y + t.lr * (g.y + t.l2 * w.y); w.y -= h.y;
-        h.z = t.mom * h.z + t.lr * (g.z + t.l2 * w.z); w.z -= h.z;
-        h.w = t.mom * h.w + t.lr * (g.w + t.l2 * w.w); w.w -= h.w;
+        sgd1(w.x, h.x, g.x, t); sgd1(w.y, h.y, g.y, t); sgd1(w.z, h.z, g.z, t); sgd1(w.w, h.w, g.w, t);
         *reinterpret_cast<float4*>(t.h + i) = h;
         *reinterpret_cast<float4*>(t.w + i) = w;
         emit4(t.w16, i >> 2, w);
       } else {
         for (long long j = i; j < e1; j++) {
-          const float wi = t.w[j], hi = t.mom * t.h[j] + t.lr * (t.g[j] + t.l2 * wi);
-          t.h[j] = hi; t.w[j] = wi - hi;
-          if (t.w16) t.w16[j] = __float2bfloat16_rn(wi - hi);
+          float wi = t.w[j], hi = t.h[j];
+          sgd1(wi, hi, t.g[j], t);
+          t.h[j] = hi; t.w[j] = wi;
+          if (t.w16) t.w16[j] = __float2bfloat16_rn(wi);
         }
       }
     }
   } else {
     for (long long i = e0 + threadIdx.x; i < e1; i += 256) {
-      const float wi = t.w[i], hi = t.mom * t.h[i] + t.lr * (t.g[i] + t.l2 * wi);
-      t.h[i] = hi; t.w[i] = wi - hi;
-      if (t.w16) t.w16[i] = __float2bfloat16_rn(wi - hi);
+      float wi = t.w[i], hi = t.h[i];
+      sgd1(wi, hi, t.g[i], t);
+      t.h[i] = hi; t.w[i] = wi;
+      if (t.w16) t.w16[i] = __float2bfloat16_rn(wi);
     }
+  }
+}
+
+// a row-norm tile.  vec (rows % 4 == 0, tile of 128 rows, aligned): lane = 4 consecutive rows (512 contiguous bytes per
+// column and warp), warp = every 8th column of the tile's 64.  Otherwise: thread = one row and every (256 / tile rows)-th
+// column.  Either way each thread holds the sums of its rows over its columns; red[] combines them in lane order.
+__device__ void sgd_norm_tile(const SgdItem& t, int block, float* red) {
+  const int R = norm_tile_rows(t.rows), C = kNormTile / R;
+  const long long K = t.n / t.rows;
+  const int strips = (int)ceil_div<long long>(t.rows, R);
+  const int strip = block % strips;
+  const long long slab = block / strips;
+  const int r0 = strip * R;
+  const long long c0 = slab * C, c1 = min(K, c0 + C);
+  const int lanes = t.vec ? 8 : 256 / R;
+  if (t.vec) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, r = r0 + 4 * lane;
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (r < t.rows) {
+      for (long long k = c0 + warp; k < c1; k += 8) {
+        const long long i = r + (long long)t.rows * k;
+        float4 w = *reinterpret_cast<const float4*>(t.w + i), h = *reinterpret_cast<const float4*>(t.h + i);
+        const float4 g = __ldg(reinterpret_cast<const float4*>(t.g + i));
+        sgd1(w.x, h.x, g.x, t); sgd1(w.y, h.y, g.y, t); sgd1(w.z, h.z, g.z, t); sgd1(w.w, h.w, g.w, t);
+        *reinterpret_cast<float4*>(t.h + i) = h;
+        *reinterpret_cast<float4*>(t.w + i) = w;
+        emit4(t.w16, i >> 2, w);
+        s.x = __fmaf_rn(w.x, w.x, s.x); s.y = __fmaf_rn(w.y, w.y, s.y);
+        s.z = __fmaf_rn(w.z, w.z, s.z); s.w = __fmaf_rn(w.w, w.w, s.w);
+      }
+    }
+    reinterpret_cast<float4*>(red)[warp * 32 + lane] = s;                        // red[warp * 128 + row in tile]
+  } else {
+    const int rr = threadIdx.x % R, lane = threadIdx.x / R, r = r0 + rr;
+    float s = 0.f;
+    if (r < t.rows) {
+      for (long long k = c0 + lane; k < c1; k += lanes) {
+        const long long i = r + (long long)t.rows * k;
+        float wi = t.w[i], hi = t.h[i];
+        sgd1(wi, hi, t.g[i], t);
+        t.h[i] = hi; t.w[i] = wi;
+        if (t.w16) t.w16[i] = __float2bfloat16_rn(wi);
+        s = __fmaf_rn(wi, wi, s);
+      }
+    }
+    red[lane * R + rr] = s;
+  }
+  __syncthreads();
+  if ((int)threadIdx.x < R && r0 + (int)threadIdx.x < t.rows) {
+    float s = 0.f;
+    for (int l = 0; l < lanes; l++) s += red[l * R + threadIdx.x];
+    t.part[slab * t.rows + r0 + threadIdx.x] = s;
+  }
+}
+
+__global__ void __launch_bounds__(256) sgd_multi_kernel(const __grid_constant__ SgdBatch b) {
+  __shared__ __align__(16) float red[1024];
+  const int ti = batch_item(b);
+  const SgdItem& t = b.t[ti];
+  const int block = (int)blockIdx.x - b.first_block[ti];
+  if (t.mode == kNormNone) sgd_chunk(t, block);
+  else sgd_norm_tile(t, block, red);
+}
+
+// Second pass, norm tensors only: a block owns kNormRescaleRows rows.  It adds up each row's partial sums in slab order
+// (warp w takes every 8th slab, then the 8 warp sums in warp order), takes the reference's scale (kNormLimitRowwise,
+// cudamat_kernels.cu:1549-1569: c/|w| under a constraint, L/|w| where |w| > L under a limit) and rewrites the weights and
+// their bf16 twin only in rows whose scale is not 1.  A limit no row exceeds costs the read of the partial sums.
+// Deviation: under a constraint a row of norm 0 stays 0 (the reference writes 0 * inf = NaN there).
+__global__ void __launch_bounds__(256) norm_rescale_kernel(const __grid_constant__ SgdBatch b) {
+  __shared__ float red[8][kNormRescaleRows];
+  __shared__ float scale[kNormRescaleRows];
+  const int ti = batch_item(b);
+  const SgdItem& t = b.t[ti];
+  const int r0 = ((int)blockIdx.x - b.first_block[ti]) * kNormRescaleRows;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, r = r0 + lane;
+  const long long slabs = norm_slabs(t), K = t.n / t.rows;
+  float s = 0.f;
+  if (r < t.rows)
+    for (long long j = warp; j < slabs; j += 8) s += t.part[j * t.rows + r];
+  red[warp][lane] = s;
+  __syncthreads();
+  if (warp == 0) {
+    float ss = 0.f;
+    for (int k = 0; k < 8; k++) ss += red[k][lane];
+    const float nrm = sqrtf(ss);
+    float sc = 1.f;
+    if (r < t.rows && nrm > 0.f && (t.mode == kNormConstraint || nrm > t.norm)) sc = t.norm / nrm;
+    scale[lane] = sc;
+  }
+  if (!__syncthreads_or(warp == 0 && scale[lane] != 1.f)) return;
+  const float sc = scale[lane];
+  if (r >= t.rows || sc == 1.f) return;
+  for (long long k = warp; k < K; k += 8) {
+    const long long i = r + (long long)t.rows * k;
+    const float v = t.w[i] * sc;
+    t.w[i] = v;
+    if (t.w16) t.w16[i] = __float2bfloat16_rn(v);
   }
 }
 
@@ -300,25 +427,31 @@ void cnb_add_channel_bias_relu(float* acts, const float* bias, long long rows, i
   bias_launch<true>(acts, bias, rows, cols);
   end_write(acts, rows * cols, emit, nullptr);
 }
-// partial sums of the bias gradient live in their OWN scratch, not in the shared workspace: a host may run this pass on a
-// side stream beside conv kernels that are using the workspace (host/convnet.cc does)
-static float* colsum_scratch(size_t floats) {
-  static float* buf = nullptr; static size_t cap = 0; static int dev = -1;
-  const int cur = current_device();
-  if (buf && (cap < floats || dev != cur)) {
-    CNB_CUDA_CHECK(cudaDeviceSynchronize());
-    if (dev != cur) CNB_CUDA_CHECK(cudaSetDevice(dev));
-    CNB_CUDA_CHECK(cudaFree(buf));
-    if (dev != cur) CNB_CUDA_CHECK(cudaSetDevice(cur));
-    buf = nullptr; cap = 0;
+// A device buffer that grows on demand.  The partial sums of the bias gradient and those of the SGD row norms each have
+// their OWN, not the shared workspace: a host may run those passes on side streams beside conv kernels that are using the
+// workspace, and beside each other (host/convnet.cc does).
+struct GrowingScratch {
+  float* buf = nullptr; size_t cap = 0; int dev = -1;
+  float* get(size_t floats) {
+    const int cur = current_device();
+    if (buf && (cap < floats || dev != cur)) {
+      CNB_CUDA_CHECK(cudaDeviceSynchronize());
+      if (dev != cur) CNB_CUDA_CHECK(cudaSetDevice(dev));
+      CNB_CUDA_CHECK(cudaFree(buf));
+      if (dev != cur) CNB_CUDA_CHECK(cudaSetDevice(cur));
+      buf = nullptr; cap = 0;
+    }
+    if (!buf) {
+      const size_t want = std::max<size_t>(floats, (size_t)1 << 18);
+      CNB_CUDA_CHECK(cudaMalloc((void**)&buf, want * sizeof(float)));
+      cap = want; dev = cur;
+    }
+    return buf;
   }
-  if (!buf) {
-    const size_t want = std::max<size_t>(floats, (size_t)1 << 18);
-    CNB_CUDA_CHECK(cudaMalloc((void**)&buf, want * sizeof(float)));
-    cap = want; dev = cur;
-  }
-  return buf;
-}
+};
+static float* colsum_scratch(size_t floats) { static GrowingScratch s; return s.get(floats); }
+// one buffer for every update call: calls are ordered on one stream (the optimizer's), so each may reuse it from the start
+static float* sgd_norm_scratch(size_t floats) { static GrowingScratch s; return s.get(floats); }
 void cnb_channel_bias_grad(const float* derivs, float* grad_bias, long long rows, int cols, float st, float so) {
   if (cols <= 0) return;
   int slices = (int)std::max<long long>(1, std::min<long long>(64, (4LL * num_sms()) / cols));
@@ -383,34 +516,71 @@ void cnb_sum(const float* a, float* out, int n) {
   sum_kernel<<<1, 256, 0, state().stream>>>(a, out, n);
   count_launch(); CNB_LAUNCH_CHECK("sum");
 }
-void cnb_sgd_momentum_multi(const CnbSgdTensor* tensors, int count) {
+void cnb_sgd_update_multi(const CnbOptTensor* tensors, int count) {
+  // partial sums of every norm tensor of the call, laid out one after the other (slabs x rows each)
+  size_t part_floats = 0;
+  for (int i = 0; i < count; i++) {
+    const CnbOptTensor& s = tensors[i];
+    if (s.n <= 0 || s.norm_mode == CNB_NORM_NONE) continue;
+    CNB_REQUIRE(s.norm_mode == CNB_NORM_LIMIT || s.norm_mode == CNB_NORM_CONSTRAINT, "cnb_sgd_update_multi");
+    CNB_REQUIRE(s.rows > 0 && s.n % s.rows == 0 && s.norm_value > 0.f, "cnb_sgd_update_multi");
+    SgdItem t; t.n = s.n; t.rows = s.rows;
+    part_floats += (size_t)norm_slabs(t) * s.rows;
+  }
+  float* part = part_floats ? sgd_norm_scratch(part_floats) : nullptr;
   for (int base = 0; base < count; base += kSgdMaxTensors) {
-    SgdBatch b;
-    b.count = 0;
-    int blocks = 0;
-    for (int i = base; i < count && b.count < kSgdMaxTensors; i++) {
-      const CnbSgdTensor& s = tensors[i];
+    SgdBatch b, nb;                                                 // update pass; rescale pass (norm tensors)
+    b.count = 0; nb.count = 0;
+    int blocks = 0, nblocks = 0;
+    for (int i = base; i < count && i < base + kSgdMaxTensors; i++) {
+      const CnbOptTensor& s = tensors[i];
       if (s.n <= 0) continue;
       SgdItem& t = b.t[b.count];
       t.w = s.w; t.h = s.hist; t.g = s.grad; t.n = s.n; t.lr = s.lr; t.mom = s.momentum; t.l2 = s.l2;
+      t.clip = s.clip > 0.f ? s.clip : 0.f;
+      t.mode = s.norm_mode; t.norm = s.norm_value; t.rows = s.norm_mode ? s.rows : 1; t.part = nullptr;
       t.vec = (aligned16(s.w) && aligned16(s.hist) && aligned16(s.grad)) ? 1 : 0;
+      if (t.mode) t.vec = t.vec && t.rows % 4 == 0 && norm_tile_rows(t.rows) == 128;
       // the weights change: a staged bf16 copy of exactly this tensor is refreshed in the same pass, any other overlap dropped
       const bool had_copy = bf16_staged(s.w, s.n) != nullptr;      // only a copy somebody keeps valid is worth refreshing
       bf16_note_write(s.w, s.n);                    // every derived copy (bf16 twin, dgrad banks) goes stale ...
       t.w16 = had_copy ? bf16_refresh_slot(s.w, s.n) : nullptr;    // ... and the bf16 twin is rewritten by this kernel
       b.first_block[b.count] = blocks;
-      blocks += (int)ceil_div<long long>(s.n, kSgdChunk);
+      if (t.mode) {
+        const long long slabs = norm_slabs(t);
+        t.part = part;
+        part += slabs * t.rows;
+        blocks += (int)(ceil_div<long long>(t.rows, norm_tile_rows(t.rows)) * slabs);
+        nb.t[nb.count] = t;
+        nb.first_block[nb.count] = nblocks;
+        nblocks += (int)ceil_div<long long>(t.rows, kNormRescaleRows);
+        nb.count++;
+      } else {
+        blocks += (int)ceil_div<long long>(s.n, kSgdChunk);
+      }
       b.count++;
     }
     if (b.count == 0) continue;
     b.first_block[b.count] = blocks;
     sgd_multi_kernel<<<blocks, 256, 0, state().stream>>>(b);
-    count_launch(); CNB_LAUNCH_CHECK("sgd_momentum_multi");
+    count_launch(); CNB_LAUNCH_CHECK("sgd_update_multi");
+    if (nb.count == 0) continue;
+    nb.first_block[nb.count] = nblocks;
+    norm_rescale_kernel<<<nblocks, 256, 0, state().stream>>>(nb);
+    count_launch(); CNB_LAUNCH_CHECK("sgd_norm_rescale");
   }
 }
+void cnb_sgd_momentum_multi(const CnbSgdTensor* tensors, int count) {
+  std::vector<CnbOptTensor> t(count > 0 ? count : 0);
+  for (int i = 0; i < count; i++) {
+    const CnbSgdTensor& s = tensors[i];
+    t[i] = CnbOptTensor{s.w, s.hist, s.grad, s.n, s.lr, s.momentum, s.l2, 0.f, 1, CNB_NORM_NONE, 0.f};
+  }
+  cnb_sgd_update_multi(t.data(), count);
+}
 void cnb_sgd_momentum(float* w, float* hist, const float* grad, long long n, float lr, float momentum, float l2) {
-  CnbSgdTensor t = {w, hist, grad, n, lr, momentum, l2};
-  cnb_sgd_momentum_multi(&t, 1);
+  const CnbOptTensor t = {w, hist, grad, n, lr, momentum, l2, 0.f, 1, CNB_NORM_NONE, 0.f};
+  cnb_sgd_update_multi(&t, 1);
 }
 
 }  // extern "C"

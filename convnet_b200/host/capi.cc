@@ -1,5 +1,7 @@
 // capi.cc — plain C doors onto the host C++ (ConvNet / GradChecker / DataParallelSync) for ctypes.
+#include <cstdio>
 #include <cstring>
+#include <stdexcept>
 
 #include "convnet.h"
 #include "data.h"
@@ -14,8 +16,16 @@ struct NetHandle {
   DataParallelSync* dp = nullptr;
 };
 
+// BuildModel for the C API: an unknown name gives false and the reason on stderr instead of an exception
+static bool TryBuildModel(const char* name, ModelConfig* m) {
+  try { *m = BuildModel(name); return true; }
+  catch (const std::invalid_argument& e) { fprintf(stderr, "convnet_b200 host: %s\n", e.what()); return false; }
+}
+
+// NULL: unknown model name (the reason is printed on stderr)
 API void* cnb_net_create(const char* model, int batch_size, unsigned seed, int grad_checker) {
-  ModelConfig m = BuildModel(model);
+  ModelConfig m;
+  if (!TryBuildModel(model, &m)) return nullptr;
   m.seed = seed;
   NetHandle* h = new NetHandle;
   if (grad_checker) { h->checker = new GradChecker(m, batch_size); h->net = h->checker; }
@@ -51,6 +61,36 @@ API float* cnb_net_device_loss(void* p) { return ((NetHandle*)p)->net->DeviceLos
 API void cnb_net_fprop(void* p, int train) { ((NetHandle*)p)->net->Fprop(train != 0); }
 API void cnb_net_bprop(void* p) { ((NetHandle*)p)->net->ComputeDeriv(); ((NetHandle*)p)->net->Bprop(); }
 API void cnb_net_update(void* p) { ((NetHandle*)p)->net->UpdateWeights(); }
+API void cnb_net_reduce_learning_rate(void* p, float factor) { ((NetHandle*)p)->net->ReduceLearningRate(factor); }
+
+// ---- optimizer settings (edge.h OptimizerConfig: proto Optimizer, SGD fields).  which: 0 the weights, 1 the bias.
+static EdgeWithWeight* WeightedEdge(void* p, int edge) {
+  std::vector<Edge*>& e = ((NetHandle*)p)->net->Edges();
+  return edge >= 0 && edge < (int)e.size() ? dynamic_cast<EdgeWithWeight*>(e[edge]) : nullptr;
+}
+// replaces the settings of one optimizer (its step count and momentum history stay).  0 ok, -1 no such weighted edge,
+// -2 a config the SGD path cannot run (see OptimizerConfigError, printed on stderr)
+API int cnb_net_set_optimizer(void* p, int edge, int which, const OptimizerConfig* c) {
+  EdgeWithWeight* e = WeightedEdge(p, edge);
+  if (!e || which < 0 || which > 1) return -1;
+  if (const char* err = OptimizerConfigError(*c)) { fprintf(stderr, "convnet_b200 host: %s\n", err); return -2; }
+  e->Optimizer(which) = *c;
+  return 0;
+}
+// the step count of one optimizer and the (epsilon, momentum) its next update uses.  0 ok, -1 no such weighted edge
+API int cnb_net_get_optimizer_state(void* p, int edge, int which, long long* step, float* epsilon, float* momentum) {
+  EdgeWithWeight* e = WeightedEdge(p, edge);
+  if (!e || which < 0 || which > 1) return -1;
+  *step = e->OptimizerStep(which);
+  OptimizerSchedule(e->Optimizer(which), *step, epsilon, momentum);
+  return 0;
+}
+// pure host logic: (epsilon, momentum) of the update after `step` earlier ones.  0 ok, -2 invalid config
+API int cnb_optimizer_schedule(const OptimizerConfig* c, long long step, float* epsilon, float* momentum) {
+  if (OptimizerConfigError(*c)) return -2;
+  OptimizerSchedule(*c, step, epsilon, momentum);
+  return 0;
+}
 API float cnb_net_loss(void* p) { return ((NetHandle*)p)->net->GetLoss(); }
 // one training step; *loss (may be NULL) receives the summed cross-entropy of the batch (one scalar D2H, like GetLoss)
 API void cnb_net_train_step(void* p, float* loss) { ((NetHandle*)p)->net->TrainOneBatch(loss); }
@@ -98,11 +138,23 @@ API int cnb_plan_buckets(int n_edges, const long long* offsets, const long long*
 }
 // static description of a model (no device memory): per-edge parameter count, for planning / reporting
 API int cnb_model_edge_params(const char* model, int batch, int cap, long long* sizes) {
-  ModelConfig m = BuildModel(model);
+  ModelConfig m;
+  if (!TryBuildModel(model, &m)) return -1;
   ConvNet net(m, batch);
   int n = 0;
   for (Edge* e : net.Edges()) { if (n >= cap) break; sizes[n++] = (long long)e->GetParameterMemoryRequirement(); }
   return n;
+}
+// static description of a model: the optimizer config of edge `edge` (which: 0 weights, 1 bias).  0 ok, -1 unknown model,
+// -2 edge out of range or without parameters
+API int cnb_model_edge_optimizer(const char* model, int edge, int which, OptimizerConfig* out) {
+  ModelConfig m;
+  if (!TryBuildModel(model, &m)) return -1;
+  if (edge < 0 || edge >= (int)m.edge.size() || which < 0 || which > 1) return -2;
+  const EdgeConfig& e = m.edge[edge];
+  if (e.edge_type == MAXPOOL || e.edge_type == AVGPOOL || e.edge_type == RESPONSE_NORM || (which == 1 && e.has_no_bias)) return -2;
+  *out = which ? e.bias_optimizer : e.weight_optimizer;
+  return 0;
 }
 
 // ---- the device side of the input pipeline (data.h): a GPU-resident chunk + per-minibatch crop / mirror into the net's input

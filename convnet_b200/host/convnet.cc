@@ -396,7 +396,7 @@ void ConvNet::Bprop() {                                      // convnet.cc:390-4
 // queued on the side stream so far, and the compute stream's last read of the bucket's weights in this step.  Its own
 // stream: an all-reduce waits for the side stream's bias gradients, and must not queue behind an earlier bucket's SGD step
 void ConvNet::IssueBucketUpdate(const Bucket& b) {
-  std::vector<CnbSgdTensor> tensors;
+  std::vector<CnbOptTensor> tensors;
   for (int i = b.trigger; i <= b.last; i++)
     if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i])) w->AppendSgdTensors(tensors);
   if (tensors.empty()) return;
@@ -406,7 +406,9 @@ void ConvNet::IssueBucketUpdate(const Bucket& b) {
   HOST_CUDA_CHECK(cudaStreamWaitEvent(opt_, ev_side_, 0));
   void* main_stream = convnet_b200_get_stream();
   convnet_b200_set_stream(opt_);
-  cnb_sgd_momentum_multi(tensors.data(), (int)tensors.size());
+  // the update, and the rescale of the rows of norm-limited tensors: both before the banks below are rebuilt from the weights
+  // (PlanBuckets splits at edge boundaries, so every row of a tensor is updated in this one call)
+  cnb_sgd_update_multi(tensors.data(), (int)tensors.size());
   // what the next step's dgrad derives from these weights alone (bf16 filter banks): rebuilt here, behind the update
   static const bool no_prestage = getenv("CONVNET_B200_NO_PRESTAGE") && getenv("CONVNET_B200_NO_PRESTAGE")[0] == '1';
   if (!no_prestage)
@@ -438,10 +440,15 @@ void ConvNet::UpdateWeights() {                              // convnet.cc:440-4
   WaitSide();                                                // replaces Accumulate + Broadcast (MPI through host memory)
   if (updated_in_bprop_) { updated_in_bprop_ = false; return; }        // TrainOneBatch: every bucket was updated on the side stream
   // one multi-tensor SGD launch for every weight and bias matrix of the net (the reference loops edges: optimizer.cc:174-200)
-  std::vector<CnbSgdTensor> tensors;
+  std::vector<CnbOptTensor> tensors;
   for (Edge* e : edges_)
     if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(e)) w->AppendSgdTensors(tensors);
-  cnb_sgd_momentum_multi(tensors.data(), (int)tensors.size());
+  cnb_sgd_update_multi(tensors.data(), (int)tensors.size());
+}
+
+void ConvNet::ReduceLearningRate(float factor) {             // convnet.cc:820-825
+  for (Edge* e : edges_)
+    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(e)) w->ReduceLearningRate(factor);
 }
 
 void ConvNet::TrainOneBatch(float* loss_out) {               // convnet.cc:475-485 (GetBatch is the caller's H2D copy)

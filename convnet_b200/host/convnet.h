@@ -114,6 +114,7 @@ class ConvNet {
   virtual void Fprop(bool train);                               // convnet.cc:377-388
   virtual void Bprop();                                         // convnet.cc:390-405
   virtual void UpdateWeights();                                 // convnet.cc:440-450
+  void ReduceLearningRate(float factor);                        // base epsilon of every weight and bias optimizer *= factor
   void ComputeDeriv();
   void TrainOneBatch(float* loss_out);                          // convnet.cc:475-485
   float GetLoss();                                              // sum of per-image CE (synchronises)

@@ -1,6 +1,7 @@
 // models.cc — ModelConfig builders for the BASELINE configs (the reference reads these from pbtxt).
 #include <cstdio>
 #include <cstdlib>
+#include <stdexcept>
 
 #include "convnet.h"
 
@@ -12,8 +13,8 @@ LayerConfig L(const char* name, int ch, Activation act = LINEAR, float dropprob 
 }
 EdgeConfig E(EdgeType t, int k = 1, int s = 1, int p = 0) {
   EdgeConfig e; e.edge_type = t; e.kernel_size = k; e.stride = s; e.padding = p;
-  e.weight_optimizer.epsilon = 0.01f; e.weight_optimizer.momentum = 0.9f;
-  e.bias_optimizer.epsilon = 0.01f; e.bias_optimizer.momentum = 0.9f;
+  e.weight_optimizer.epsilon = 0.01f; e.weight_optimizer.final_momentum = 0.9f;
+  e.bias_optimizer.epsilon = 0.01f; e.bias_optimizer.final_momentum = 0.9f;
   return e;
 }
 EdgeConfig Conv(int k, int s, int p, float l2 = 0.f) { EdgeConfig e = E(CONVOLUTIONAL, k, s, p); e.weight_optimizer.l2_decay = l2; return e; }
@@ -63,7 +64,7 @@ ModelConfig BuildLeNet() {
              L("hidden2_conv", 128, RECTIFIED_LINEAR), L("hidden2_maxpool", 128), L("output", 10, SOFTMAX)};
   m.layer.back().is_output = true;
   m.edge = {Conv(4, 1, 0, 0.0005f), Pool(4, 2, 0), Conv(4, 1, 0, 0.0005f), Pool(4, 2, 0), E(FC)};
-  for (EdgeConfig& e : m.edge) { e.weight_optimizer.momentum = 0.95f; e.bias_optimizer.momentum = 0.95f; }
+  for (EdgeConfig& e : m.edge) { e.weight_optimizer.final_momentum = 0.95f; e.bias_optimizer.final_momentum = 0.95f; }
   finish(m);
   return m;
 }
@@ -114,7 +115,41 @@ ModelConfig BuildGradCheckNet() {
   return m;
 }
 
+// "<model>+ref-optimizer": the optimizer blocks of the model's pbtxt exactly (BuildAlexNet / BuildLeNet keep the constant
+// momentum and leave out the norm rules and the FC l2_decay)
+static void UseReferenceOptimizers(const std::string& base, ModelConfig& m) {
+  OptimizerConfig o;                                        // every weight and bias optimizer of both files
+  o.epsilon = 0.01f;
+  if (base == "alexnet") {        // examples/imagenet/CLS_net_20140801232522.pbtxt:148-505
+    o.initial_momentum = 0.5f; o.final_momentum = 0.9f; o.momentum_transition_timescale = 2000;
+    for (EdgeConfig& e : m.edge) {
+      const float l2 = e.weight_optimizer.l2_decay;        // conv3-5: 0.0005, as BuildAlexNet has it
+      e.weight_optimizer = o; e.bias_optimizer = o;
+      e.weight_optimizer.l2_decay = l2;
+      if (e.edge_type == CONV_ONETOONE) e.weight_optimizer.weight_norm_constraint = 1.f;
+      if (e.edge_type == FC) { e.weight_optimizer.weight_norm_limit = 4.f; e.weight_optimizer.l2_decay = 0.0005f; }
+    }
+  } else {                        // examples/mnist-conv/net.pbtxt:60-127
+    OptimizerConfig w = o, b = o;
+    w.initial_momentum = 0.5f; w.final_momentum = 0.95f; w.l2_decay = 0.0005f;    // no transition timescale: 0.95 throughout
+    b.final_momentum = 0.95f;
+    for (EdgeConfig& e : m.edge) {
+      e.weight_optimizer = w; e.bias_optimizer = b;
+      if (e.edge_type == FC) e.weight_optimizer.weight_norm_limit = 4.f;
+    }
+  }
+}
+
 ModelConfig BuildModel(const std::string& name) {
+  const std::string ref = "+ref-optimizer";
+  if (name.size() > ref.size() && name.compare(name.size() - ref.size(), ref.size(), ref) == 0) {
+    const std::string base = name.substr(0, name.size() - ref.size());
+    if (base != "alexnet" && base != "lenet")
+      throw std::invalid_argument("model '" + name + "': +ref-optimizer is defined for alexnet and lenet only");
+    ModelConfig m = BuildModel(base);
+    UseReferenceOptimizers(base, m);
+    return m;
+  }
   // "<model>+gradcheck": the model with run_grad_check's edge flags as BASELINE config 1 states them
   // (grad_check_num_params: 10, grad_check_epsilon: [1e-2, 1e-3, 1e-4]; src/grad_check.cc:20-61)
   const std::string suffix = "+gradcheck";
@@ -128,8 +163,7 @@ ModelConfig BuildModel(const std::string& name) {
   if (name == "lenet") return BuildLeNet();
   if (name == "c3d") return BuildC3D();
   if (name == "tiny") return BuildTinyNet();
-  fprintf(stderr, "unknown model '%s'\n", name.c_str());
-  exit(1);
+  throw std::invalid_argument("unknown model '" + name + "'");
 }
 
 }  // namespace cnbhost

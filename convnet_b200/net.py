@@ -6,6 +6,36 @@ import os
 
 from . import lib as _lib
 
+
+class OptimizerConfig(ct.Structure):
+    """host/edge.h OptimizerConfig: the SGD fields of the reference's proto Optimizer (proto/convnet_config.proto:64-113),
+    same names, same defaults, same order as the C struct."""
+    _fields_ = [("epsilon", ct.c_float), ("epsilon_decay", ct.c_int), ("epsilon_decay_timescale", ct.c_int),
+                ("minimum_epsilon", ct.c_float), ("decay_factor", ct.c_float), ("initial_momentum", ct.c_float),
+                ("final_momentum", ct.c_float), ("momentum_transition_timescale", ct.c_int), ("l2_decay", ct.c_float),
+                ("gradient_clip", ct.c_float), ("start_optimization_after", ct.c_int), ("weight_norm_limit", ct.c_float),
+                ("weight_norm_constraint", ct.c_float)]
+    DEFAULTS = {"decay_factor": 1.0, "gradient_clip": -1.0}
+    DECAY = {"NONE": 0, "INVERSE_T": 1, "EXPONENTIAL": 2, "LINEAR": 3, "EXPONENTIAL_STEP": 4}
+
+    @classmethod
+    def from_dict(cls, d):
+        """an optimizer block as a dict of proto field names (epsilon_decay also by name); unset fields take the proto's
+        defaults.  Fields outside the SGD path (Nesterov, Adagrad, RMSProp, LBFGS, shared prior) are not supported."""
+        c = cls(**cls.DEFAULTS)
+        names = [f[0] for f in cls._fields_]
+        for k, v in d.items():
+            if k not in names:
+                raise KeyError("unsupported optimizer field %r (known: %s)" % (k, ", ".join(names)))
+            if k == "epsilon_decay" and isinstance(v, str):
+                v = cls.DECAY[v]
+            setattr(c, k, v)
+        return c
+
+    def to_dict(self):
+        return {f[0]: getattr(self, f[0]) for f in self._fields_}
+
+
 HOST_LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "libconvnet_b200_host.so")
 _host = None
 
@@ -37,6 +67,11 @@ def load_host():
             "cnb_dp_unique_id": ([ct.c_char_p], i), "cnb_net_dp_init": ([vp, i, i, ct.c_char_p, ll], i),
             "cnb_plan_buckets": ([i, ct.POINTER(ll), ct.POINTER(ll), ll, i, ct.POINTER(ll), ct.POINTER(ll), ct.POINTER(i)], i),
             "cnb_model_edge_params": ([ct.c_char_p, i, i, ct.POINTER(ll)], i),
+            "cnb_net_reduce_learning_rate": ([vp, f], None),
+            "cnb_net_set_optimizer": ([vp, i, i, ct.POINTER(OptimizerConfig)], i),
+            "cnb_net_get_optimizer_state": ([vp, i, i, ct.POINTER(ll), ct.POINTER(f), ct.POINTER(f)], i),
+            "cnb_optimizer_schedule": ([ct.POINTER(OptimizerConfig), ll, ct.POINTER(f), ct.POINTER(f)], i),
+            "cnb_model_edge_optimizer": ([ct.c_char_p, i, i, ct.POINTER(OptimizerConfig)], i),
             "cnb_net_grad_check": ([vp, ct.c_uint, i, ct.c_char_p, ct.POINTER(f), ct.POINTER(f), ct.POINTER(f)], i),
         }
         for name, (args, res) in sig.items():
@@ -47,11 +82,14 @@ def load_host():
 
 
 class Net:
-    """A chain ConvNet built natively ("alexnet" | "lenet" | "c3d" | "tiny")."""
+    """A chain ConvNet built natively ("alexnet" | "lenet" | "c3d" | "tiny"; "alexnet+ref-optimizer" and
+    "lenet+ref-optimizer" train with the optimizer blocks of the reference's pbtxt files)."""
 
     def __init__(self, model, batch_size, seed=42, grad_checker=False):
         self.H = load_host()
         self.h = self.H.cnb_net_create(model.encode(), batch_size, seed, int(grad_checker))
+        if not self.h:
+            raise ValueError("cannot build model %r (see stderr)" % model)
         self.batch_size = batch_size
         self.model = model
 
@@ -115,6 +153,42 @@ class Net:
     def loss(self):
         return self.H.cnb_net_loss(self.h)
 
+    # --- optimizer (SGDOptimizer, src/optimizer.cc): one for the weights and one for the bias of every weighted edge
+    def _edge_index(self, edge):
+        if isinstance(edge, str):
+            names = [e[0] for e in self.edges()]
+            if edge not in names:
+                raise KeyError("no edge %r (edges: %s)" % (edge, ", ".join(names)))
+            return names.index(edge)
+        return int(edge)
+
+    def set_optimizer(self, edge, weights=None, bias=None):
+        """replace the settings of the weight and / or bias optimizer of `edge` (index or name) with the optimizer block
+        `weights` / `bias` (dicts of proto field names, unset fields at the proto's defaults).  Step counts and momentum
+        histories are kept."""
+        i = self._edge_index(edge)
+        for which, d in ((0, weights), (1, bias)):
+            if d is None:
+                continue
+            rc = self.H.cnb_net_set_optimizer(self.h, i, which, ct.byref(OptimizerConfig.from_dict(d)))
+            if rc != 0:
+                raise ValueError("set_optimizer(%r, %s): %s" % (edge, ("weights", "bias")[which],
+                                 "no such weighted edge" if rc == -1 else "config not supported (see stderr)"))
+
+    def optimizer_state(self, edge):
+        """{"weights": {...}, "bias": {...}}: updates counted so far ("step") and the epsilon / momentum of the next one"""
+        i, out = self._edge_index(edge), {}
+        for which, key in ((0, "weights"), (1, "bias")):
+            step, eps, mom = ct.c_longlong(0), ct.c_float(0), ct.c_float(0)
+            if self.H.cnb_net_get_optimizer_state(self.h, i, which, ct.byref(step), ct.byref(eps), ct.byref(mom)) != 0:
+                raise ValueError("edge %r has no parameters" % (edge,))
+            out[key] = {"step": step.value, "epsilon": eps.value, "momentum": mom.value}
+        return out
+
+    def reduce_learning_rate(self, factor):
+        """multiply the base epsilon of every optimizer by `factor` (ConvNet::ReduceLearningRate)"""
+        self.H.cnb_net_reduce_learning_rate(self.h, factor)
+
     def train_step(self, want_loss=True):
         if want_loss:
             v = ct.c_float(0)
@@ -156,7 +230,27 @@ def model_edge_params(model, batch=1):
     H = load_host()
     buf = (ct.c_longlong * 64)()
     n = H.cnb_model_edge_params(model.encode(), batch, 64, buf)
+    if n < 0:
+        raise ValueError("unknown model %r (see stderr)" % model)
     return [buf[k] for k in range(n)]
+
+
+def model_edge_optimizer(model, edge, which="weights"):
+    """the optimizer config (dict of proto field names) a model gives edge `edge` (host-only); None for an edge without
+    parameters"""
+    c = OptimizerConfig()
+    rc = load_host().cnb_model_edge_optimizer(model.encode(), edge, {"weights": 0, "bias": 1}[which], ct.byref(c))
+    if rc == -1:
+        raise ValueError("unknown model %r (see stderr)" % model)
+    return c.to_dict() if rc == 0 else None
+
+
+def optimizer_schedule(config, step):
+    """(epsilon, momentum) of the update after `step` earlier ones under the optimizer block `config` (a dict)"""
+    eps, mom = ct.c_float(0), ct.c_float(0)
+    if load_host().cnb_optimizer_schedule(ct.byref(OptimizerConfig.from_dict(config)), step, ct.byref(eps), ct.byref(mom)):
+        raise ValueError("optimizer config not supported: %r" % (config,))
+    return eps.value, mom.value
 
 
 def plan_buckets(edge_sizes, bucket_floats):

@@ -154,16 +154,38 @@ void cnb_softmax_ce_deriv(const float* probs, const int* labels, float* deriv, f
 /* *out = sum(a[0..n)) on the device (no host sync) */
 void cnb_sum(const float* a, float* out, int n);
 /* SGD with momentum and L2 decay, one fused pass (src/optimizer.cc:174-200):
- *   g' = lr*(g + l2*w);  h = momentum*h + g';  w -= h */
+ *   g' = lr*(g + l2*w);  h = momentum*h + g';  w -= h
+ * (cnb_sgd_update_multi with one tensor, no clip and no norm) */
 void cnb_sgd_momentum(float* w, float* hist, const float* grad, long long n, float lr,
                       float momentum, float l2);
 /* the same update for `count` tensors in ONE launch (one call per all-reduce bucket / per net instead of one per
  * weight and bias matrix).  `tensors` is a host array.  In bf16 mode a staged copy of a weight tensor is refreshed
- * by the same pass (see convnet_b200_bf16_stage). */
+ * by the same pass (see convnet_b200_bf16_stage).  (cnb_sgd_update_multi without clip and norms) */
 typedef struct CnbSgdTensor {
   float* w; float* hist; const float* grad; long long n; float lr, momentum, l2;
 } CnbSgdTensor;
 void cnb_sgd_momentum_multi(const CnbSgdTensor* tensors, int count);
+
+/* The whole SGD step of SGDOptimizer::Optimize (src/optimizer.cc:174-200) for `count` tensors, in this order:
+ *   g += l2*w;  g = clamp(g, -clip, clip) if clip > 0 (gradient_clip);  h = momentum*h + lr*g;  w -= h;
+ *   then the row-norm rule (Optimizer::ApplyConstraints, optimizer.cc:75-81) on the updated w.
+ * The caller supplies this step's lr and momentum (the schedules are host logic).  Row norms: the tensor is
+ * [rows x n/rows] with the rows fastest — row r is the elements r + rows*k, one output unit's incoming weights in this
+ * library's filter layout; a bias is one row.  CNB_NORM_LIMIT rescales the rows whose norm exceeds norm_value to
+ * norm_value (weight_norm_limit), CNB_NORM_CONSTRAINT rescales every row to norm_value (weight_norm_constraint); a row of
+ * norm 0 is left at 0 (the reference divides by 0 there).  One launch for the update — which also sums the squares of
+ * the weights it stores, per row, into library scratch — plus one for the rescale when any tensor has a norm rule; no
+ * atomics, so results are bit-reproducible.  Calls must be ordered on one stream (the scratch is shared between calls).
+ * A tensor with clip <= 0 and no norm rule gets exactly the bits of cnb_sgd_momentum_multi. */
+enum { CNB_NORM_NONE = 0, CNB_NORM_LIMIT = 1, CNB_NORM_CONSTRAINT = 2 };
+typedef struct CnbOptTensor {
+  float* w; float* hist; const float* grad; long long n; float lr, momentum, l2;
+  float clip;          /* > 0: gradient clip */
+  int rows;            /* norm groups (n % rows == 0); read only with a norm rule */
+  int norm_mode;       /* CNB_NORM_* */
+  float norm_value;    /* > 0 with a norm rule */
+} CnbOptTensor;
+void cnb_sgd_update_multi(const CnbOptTensor* tensors, int count);
 
 /* ---- input pipeline, device side (SURVEY.md §8 f4) -------------------------------------------------------------------
  * The reference keeps a chunk of the data set on the GPU, one image per COLUMN (pixel index = col + W*(row + H*color)),

@@ -57,23 +57,88 @@ static void bias_launch(float* acts, const float* bias, long long rows, int cols
   CNB_LAUNCH_CHECK("add_channel_bias");
 }
 
-// column sums of a column-major [rows x cols] matrix; one block per (column, row-slice)
-__global__ void colsum_partial_kernel(const float* __restrict__ a, float* __restrict__ part, long long rows, int cols,
-                                      int slices) {
+// Column reductions of a column-major [rows x cols] matrix (a column = one channel of a 2-D layer, DESIGN.md §3): one
+// block per (column, row slice), a fixed summation order, no atomics.  Op accumulates Op::K quantities per element; slice
+// s of column c leaves quantity k in part[(k * slices + s) * cols + c], and a small per-column kernel adds the slices up
+// in slice order.  VEC (rows % 4 == 0, 16-byte aligned operands): float4 loads, slice boundaries on multiples of 4.
+//   SumOp      the column sum: the bias gradient (scalar, the order it has always had) and the batch-norm mean
+//   SqDevOp    sum of (x - mu[c])^2: the batch-norm variance, taken about the mean
+//   BnGradOp   sum of d and of d * (x - mu[c]) / sigma[c]: the batch-norm backward pass
+__device__ __forceinline__ float4 ldg4(const float* p, long long i4) { return __ldg(reinterpret_cast<const float4*>(p) + i4); }
+struct SumOp {
+  static constexpr int K = 1;
+  const float* a;
+  struct Col { const float* p; };
+  __device__ Col column(int c, long long rows) const { return {a + (long long)c * rows}; }
+  __device__ void add(const Col& k, long long r, float* s) const { s[0] += __ldg(k.p + r); }
+  __device__ void add4(const Col& k, long long r, float* s) const {
+    const float4 v = ldg4(k.p, r);
+    s[0] += (v.x + v.y) + (v.z + v.w);
+  }
+};
+struct SqDevOp {
+  static constexpr int K = 1;
+  const float* a; const float* mu;
+  struct Col { const float* p; float m; };
+  __device__ Col column(int c, long long rows) const { return {a + (long long)c * rows, __ldg(mu + c)}; }
+  __device__ void add(const Col& k, long long r, float* s) const { const float d = __ldg(k.p + r) - k.m; s[0] = __fmaf_rn(d, d, s[0]); }
+  __device__ void add4(const Col& k, long long r, float* s) const {
+    const float4 v = ldg4(k.p, r);
+    const float a = v.x - k.m, b = v.y - k.m, c = v.z - k.m, d = v.w - k.m;
+    s[0] += __fmaf_rn(a, a, b * b) + __fmaf_rn(c, c, d * d);
+  }
+};
+struct BnGradOp {
+  static constexpr int K = 2;
+  const float* d; const float* x; const float* mu; const float* sigma;
+  struct Col { const float* pd; const float* px; float m, inv; };
+  __device__ Col column(int c, long long rows) const {
+    return {d + (long long)c * rows, x + (long long)c * rows, __ldg(mu + c), 1.f / __ldg(sigma + c)};
+  }
+  __device__ void add(const Col& k, long long r, float* s) const {
+    const float g = __ldg(k.pd + r), xh = (__ldg(k.px + r) - k.m) * k.inv;
+    s[0] += g; s[1] = __fmaf_rn(g, xh, s[1]);
+  }
+  __device__ void add4(const Col& k, long long r, float* s) const {
+    const float4 g = ldg4(k.pd, r), v = ldg4(k.px, r);
+    s[0] += (g.x + g.y) + (g.z + g.w);
+    s[1] += __fmaf_rn(g.x, (v.x - k.m) * k.inv, g.y * ((v.y - k.m) * k.inv)) +
+            __fmaf_rn(g.z, (v.z - k.m) * k.inv, g.w * ((v.w - k.m) * k.inv));
+  }
+};
+
+template <class Op, bool VEC>
+__global__ void __launch_bounds__(256) colsum_partial_kernel(const Op op, float* __restrict__ part, long long rows, int cols,
+                                                             int slices) {
+  constexpr int K = Op::K;
   const int col = blockIdx.x, slice = blockIdx.y;
-  const long long per = ceil_div<long long>(rows, slices);
-  const long long r0 = slice * per, r1 = min(rows, r0 + per);
-  const float* p = a + (long long)col * rows;
-  float s = 0.f;
-  for (long long r = r0 + threadIdx.x; r < r1; r += blockDim.x) s += __ldg(p + r);
-  __shared__ float sh[32];
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = s;
+  const typename Op::Col k = op.column(col, rows);
+  float s[K];
+#pragma unroll
+  for (int q = 0; q < K; q++) s[q] = 0.f;
+  if (VEC) {
+    const long long rv = rows / 4, per = ceil_div<long long>(rv, slices);
+    const long long r0 = slice * per, r1 = min(rv, r0 + per);
+    for (long long r = r0 + threadIdx.x; r < r1; r += blockDim.x) op.add4(k, r, s);
+  } else {
+    const long long per = ceil_div<long long>(rows, slices);
+    const long long r0 = slice * per, r1 = min(rows, r0 + per);
+    for (long long r = r0 + threadIdx.x; r < r1; r += blockDim.x) op.add(k, r, s);
+  }
+  __shared__ float sh[K][32];
+#pragma unroll
+  for (int q = 0; q < K; q++) {
+    for (int o = 16; o > 0; o >>= 1) s[q] += __shfl_xor_sync(0xffffffffu, s[q], o);
+    if ((threadIdx.x & 31) == 0) sh[q][threadIdx.x >> 5] = s[q];
+  }
   __syncthreads();
   if (threadIdx.x < 32) {
-    s = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.f;
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (threadIdx.x == 0) part[(long long)slice * cols + col] = s;
+#pragma unroll
+    for (int q = 0; q < K; q++) {
+      float t = threadIdx.x < (blockDim.x >> 5) ? sh[q][threadIdx.x] : 0.f;
+      for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+      if (threadIdx.x == 0) part[((long long)q * slices + slice) * cols + col] = t;
+    }
   }
 }
 __global__ void colsum_final_kernel(const float* __restrict__ part, float* out, int cols, int slices, float st, float so) {
@@ -311,6 +376,115 @@ __global__ void mult_kernel(float* a, const float* __restrict__ b, long long n, 
   for (long long i = 4 * n4 + tid; i < n; i += nt) { const float v = a[i] * b[i]; a[i] = v; if (out16) out16[i] = __float2bfloat16_rn(v); }
 }
 
+// ---- batch normalisation (Layer::ApplyBatchNormalization / ApplyDerivativeofBatchNormalization, src/layer.cc:452-510)
+// The per-channel statistics are column reductions (colsum_partial_kernel); these kernels finish them per channel and
+// run the two elementwise passes.  An elementwise block works inside one channel (blockIdx.y): it reads that channel's
+// parameters once and walks the channel's n values with a grid stride over blockIdx.x.
+__global__ void bn_mean_final_kernel(const float* __restrict__ part, float* mu, int cols, int slices, float inv_n) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= cols) return;
+  float s = 0.f;
+  for (int j = 0; j < slices; j++) s += part[(long long)j * cols + c];
+  mu[c] = s * inv_n;
+}
+// sigma = sqrt(mean((x - mu)^2) + eps); the running averages (layer.cc:468-471) when run_mu is given
+__global__ void bn_sigma_final_kernel(const float* __restrict__ part, const float* __restrict__ mu, float* sigma, float* run_mu,
+                                      float* run_sigma, int cols, int slices, float inv_n, float eps, float f) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= cols) return;
+  float s = 0.f;
+  for (int j = 0; j < slices; j++) s += part[(long long)j * cols + c];
+  const float sg = sqrtf(s * inv_n + eps);
+  sigma[c] = sg;
+  if (run_mu) {
+    run_mu[c] = __fmaf_rn(1.f - f, mu[c], f * run_mu[c]);
+    run_sigma[c] = __fmaf_rn(1.f - f, sg, f * run_sigma[c]);
+  }
+}
+// grad_beta = mean(d), grad_gamma = mean(d * xhat) (the reference's 1/n scaling, layer.cc:493-496)
+__global__ void bn_grad_final_kernel(const float* __restrict__ part, float* grad_gamma, float* grad_beta, int cols, int slices,
+                                     float inv_n) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= cols) return;
+  float s0 = 0.f, s1 = 0.f;
+  for (int j = 0; j < slices; j++) { s0 += part[(long long)j * cols + c]; s1 += part[(long long)(slices + j) * cols + c]; }
+  grad_beta[c] = s0 * inv_n;
+  grad_gamma[c] = s1 * inv_n;
+}
+
+// y = gamma * (x - mu) / sigma + beta [, max(., 0)], with the bf16 twin of y when out16 is given.  vec: n % 4 == 0 and
+// x, y 16-byte aligned (a float4 never straddles two channels)
+template <bool RELU>
+__global__ void __launch_bounds__(256) bn_apply_kernel(const float* __restrict__ x, float* __restrict__ y, long long n, int vec,
+                                                       const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                       const float* __restrict__ mu, const float* __restrict__ sigma,
+                                                       __nv_bfloat16* out16) {
+  const int c = blockIdx.y;
+  const float m = __ldg(mu + c), a = __ldg(gamma + c) / __ldg(sigma + c), b = __ldg(beta + c);
+  const long long stride = (long long)gridDim.x * blockDim.x, base = (long long)c * n;
+  auto f = [&](float v) { const float r = __fmaf_rn(v - m, a, b); return RELU ? fmaxf(r, 0.f) : r; };
+  if (vec) {
+    const long long n4 = n / 4, b4 = base / 4;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += stride) {
+      float4 v = ldg4(x, b4 + i);
+      v.x = f(v.x); v.y = f(v.y); v.z = f(v.z); v.w = f(v.w);
+      reinterpret_cast<float4*>(y)[b4 + i] = v;
+      emit4(out16, b4 + i, v);
+    }
+  } else {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += stride) {
+      const float v = f(__ldg(x + base + i));
+      y[base + i] = v;
+      if (out16) out16[base + i] = __float2bfloat16_rn(v);
+    }
+  }
+}
+// in place: d = gamma / sigma * (d - mean(d) - xhat * mean(d * xhat)), xhat = (x - mu) / sigma; mean(d) and mean(d * xhat)
+// are grad_beta and grad_gamma (bn_grad_final_kernel).  train == 0: d = gamma / sigma * d (the running statistics are
+// constants of the test-mode transform)
+__global__ void __launch_bounds__(256) bn_backward_kernel(float* dx, const float* __restrict__ x, long long n, int vec,
+                                                          const float* __restrict__ gamma, const float* __restrict__ mu,
+                                                          const float* __restrict__ sigma, const float* __restrict__ grad_gamma,
+                                                          const float* __restrict__ grad_beta, int train, __nv_bfloat16* out16) {
+  const int c = blockIdx.y;
+  const float m = __ldg(mu + c), inv = 1.f / __ldg(sigma + c), a = __ldg(gamma + c) * inv;
+  const float md = train ? __ldg(grad_beta + c) : 0.f, mdx = train ? __ldg(grad_gamma + c) : 0.f;
+  const long long stride = (long long)gridDim.x * blockDim.x, base = (long long)c * n;
+  auto f = [&](float d, float v) { return a * __fmaf_rn(-(v - m) * inv, mdx, d - md); };
+  if (vec) {
+    const long long n4 = n / 4, b4 = base / 4;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += stride) {
+      float4 d = reinterpret_cast<const float4*>(dx)[b4 + i];
+      const float4 v = ldg4(x, b4 + i);
+      d.x = f(d.x, v.x); d.y = f(d.y, v.y); d.z = f(d.z, v.z); d.w = f(d.w, v.w);
+      reinterpret_cast<float4*>(dx)[b4 + i] = d;
+      emit4(out16, b4 + i, d);
+    }
+  } else {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += stride) {
+      const float v = f(dx[base + i], __ldg(x + base + i));
+      dx[base + i] = v;
+      if (out16) out16[base + i] = __float2bfloat16_rn(v);
+    }
+  }
+}
+
+int bn_slices(long long n, int channels) {
+  const long long want = ceil_div<long long>(8LL * num_sms(), channels), most = std::max<long long>(1, n / 2048);
+  return (int)std::max<long long>(1, std::min<long long>(std::min(want, most), 1024));
+}
+bool bn_vec(long long n, const void* a, const void* b) { return n % 4 == 0 && aligned16(a) && aligned16(b); }
+dim3 bn_grid(long long n, int channels, bool vec) {
+  const long long per = ceil_div<long long>(vec ? n / 4 : n, 256), fill = ceil_div<long long>(16LL * num_sms(), channels);
+  return dim3((unsigned)std::max<long long>(1, std::min(per, fill)), (unsigned)channels);
+}
+template <class Op>
+void bn_reduce(const Op& op, float* part, long long n, int channels, int slices, bool vec) {
+  if (vec) colsum_partial_kernel<Op, true><<<dim3(channels, slices), 256, 0, state().stream>>>(op, part, n, channels, slices);
+  else colsum_partial_kernel<Op, false><<<dim3(channels, slices), 256, 0, state().stream>>>(op, part, n, channels, slices);
+  count_launch(); CNB_LAUNCH_CHECK("bn_reduce");
+}
+
 // softmax over classes of a column-major [rows x cols] matrix: one block per 32 images; lane = image (coalesced
 // along rows), the block's warps split the classes; max and sum combined through shared memory.
 __global__ void __launch_bounds__(256) softmax_kernel(float* x, int rows, int cols) {
@@ -457,7 +631,7 @@ void cnb_channel_bias_grad(const float* derivs, float* grad_bias, long long rows
   int slices = (int)std::max<long long>(1, std::min<long long>(64, (4LL * num_sms()) / cols));
   slices = (int)std::min<long long>(slices, std::max<long long>(1, rows / 1024));
   float* part = colsum_scratch((size_t)slices * cols);
-  colsum_partial_kernel<<<dim3(cols, slices), 256, 0, state().stream>>>(derivs, part, rows, cols, slices);
+  colsum_partial_kernel<SumOp, false><<<dim3(cols, slices), 256, 0, state().stream>>>(SumOp{derivs}, part, rows, cols, slices);
   colsum_final_kernel<<<ceil_div(cols, 128), 128, 0, state().stream>>>(part, grad_bias, cols, slices, st, so);
   count_launch(2);
   CNB_LAUNCH_CHECK("channel_bias_grad");
@@ -581,6 +755,62 @@ void cnb_sgd_momentum_multi(const CnbSgdTensor* tensors, int count) {
 void cnb_sgd_momentum(float* w, float* hist, const float* grad, long long n, float lr, float momentum, float l2) {
   const CnbOptTensor t = {w, hist, grad, n, lr, momentum, l2, 0.f, 1, CNB_NORM_NONE, 0.f};
   cnb_sgd_update_multi(&t, 1);
+}
+
+// ---- batch normalisation.  The reductions fill the machine at both ends of the layer shapes: a few channels of ~1.5 M
+// values (row slices, about 8 blocks per SM in all) and thousands of channels of 128 values (one block per channel).
+static float* bn_scratch(size_t floats) { static GrowingScratch s; return s.get(floats); }   // ordered on the caller's stream
+void cnb_bn_stats(const float* x, long long n, int channels, float eps, float bn_f, float* batch_mu, float* batch_sigma,
+                  float* run_mu, float* run_sigma) {
+  if (n <= 0 || channels <= 0) return;
+  CNB_REQUIRE(channels <= 65535 && (run_mu == nullptr) == (run_sigma == nullptr), "cnb_bn_stats");
+  for (float* v : {batch_mu, batch_sigma, run_mu, run_sigma}) bf16_note_write(v, channels);
+  const int slices = bn_slices(n, channels);
+  const bool vec = n % 4 == 0 && aligned16(x);
+  float* part = bn_scratch((size_t)slices * channels);
+  const float inv_n = 1.f / (float)n;
+  bn_reduce(SumOp{x}, part, n, channels, slices, vec);
+  bn_mean_final_kernel<<<ceil_div(channels, 128), 128, 0, state().stream>>>(part, batch_mu, channels, slices, inv_n);
+  count_launch(); CNB_LAUNCH_CHECK("bn_mean");
+  bn_reduce(SqDevOp{x, batch_mu}, part, n, channels, slices, vec);
+  bn_sigma_final_kernel<<<ceil_div(channels, 128), 128, 0, state().stream>>>(part, batch_mu, batch_sigma, run_mu, run_sigma,
+                                                                              channels, slices, inv_n, eps, bn_f);
+  count_launch(); CNB_LAUNCH_CHECK("bn_sigma");
+}
+void cnb_bn_apply(const float* x, float* y, long long n, int channels, const float* gamma, const float* beta, const float* mu,
+                  const float* sigma, int relu) {
+  const bool emit = take_fuse().emit_bf16 != 0;
+  if (n <= 0 || channels <= 0) return;
+  CNB_REQUIRE(channels <= 65535, "cnb_bn_apply");
+  const long long total = n * channels;
+  const bool vec = bn_vec(n, x, y);
+  __nv_bfloat16* o16 = begin_write(y, total, emit, true);
+  const dim3 grid = bn_grid(n, channels, vec);
+  if (relu) bn_apply_kernel<true><<<grid, 256, 0, state().stream>>>(x, y, n, vec, gamma, beta, mu, sigma, o16);
+  else bn_apply_kernel<false><<<grid, 256, 0, state().stream>>>(x, y, n, vec, gamma, beta, mu, sigma, o16);
+  count_launch(); CNB_LAUNCH_CHECK("bn_apply");
+  end_write(y, total, emit, o16);
+}
+void cnb_bn_backward(float* deriv, const float* x, long long n, int channels, const float* gamma, const float* mu,
+                     const float* sigma, int train, float* grad_gamma, float* grad_beta) {
+  const bool emit = take_fuse().emit_bf16 != 0;
+  if (n <= 0 || channels <= 0) return;
+  CNB_REQUIRE(channels <= 65535, "cnb_bn_backward");
+  const long long total = n * channels;
+  const bool vec = bn_vec(n, x, deriv);
+  bf16_note_write(grad_gamma, channels);
+  bf16_note_write(grad_beta, channels);
+  const int slices = bn_slices(n, channels);
+  float* part = bn_scratch((size_t)2 * slices * channels);
+  bn_reduce(BnGradOp{deriv, x, mu, sigma}, part, n, channels, slices, vec);
+  bn_grad_final_kernel<<<ceil_div(channels, 128), 128, 0, state().stream>>>(part, grad_gamma, grad_beta, channels, slices,
+                                                                             1.f / (float)n);
+  count_launch(); CNB_LAUNCH_CHECK("bn_grad");
+  __nv_bfloat16* o16 = begin_write(deriv, total, emit, true);
+  bn_backward_kernel<<<bn_grid(n, channels, vec), 256, 0, state().stream>>>(deriv, x, n, vec, gamma, mu, sigma, grad_gamma,
+                                                                            grad_beta, train, o16);
+  count_launch(); CNB_LAUNCH_CHECK("bn_backward");
+  end_write(deriv, total, emit, o16);
 }
 
 }  // extern "C"

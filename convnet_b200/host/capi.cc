@@ -22,14 +22,20 @@ static bool TryBuildModel(const char* name, ModelConfig* m) {
   catch (const std::invalid_argument& e) { fprintf(stderr, "convnet_b200 host: %s\n", e.what()); return false; }
 }
 
-// NULL: unknown model name (the reason is printed on stderr)
+// NULL: unknown model name, or a model the host cannot run (the reason is printed on stderr)
 API void* cnb_net_create(const char* model, int batch_size, unsigned seed, int grad_checker) {
   ModelConfig m;
   if (!TryBuildModel(model, &m)) return nullptr;
   m.seed = seed;
   NetHandle* h = new NetHandle;
-  if (grad_checker) { h->checker = new GradChecker(m, batch_size); h->net = h->checker; }
-  else h->net = new ConvNet(m, batch_size);
+  try {
+    if (grad_checker) { h->checker = new GradChecker(m, batch_size); h->net = h->checker; }
+    else h->net = new ConvNet(m, batch_size);
+  } catch (const std::invalid_argument& e) {
+    fprintf(stderr, "convnet_b200 host: %s\n", e.what());
+    delete h;
+    return nullptr;
+  }
   h->net->AllocateMemory();
   return h;
 }
@@ -91,6 +97,44 @@ API int cnb_optimizer_schedule(const OptimizerConfig* c, long long step, float* 
   OptimizerSchedule(*c, step, epsilon, momentum);
   return 0;
 }
+
+// ---- batch normalisation (convnet.h Layer).  layer: index into the chain (0 = input).  which: 0 gamma, 1 beta.
+static Layer* BnLayer(void* p, int layer) {
+  std::vector<Layer*>& l = ((NetHandle*)p)->net->Layers();
+  return layer >= 0 && layer < (int)l.size() && l[layer]->BatchNormalize() ? l[layer] : nullptr;
+}
+API const char* cnb_net_layer_name(void* p, int i) { return ((NetHandle*)p)->net->Layers()[i]->GetName().c_str(); }
+API int cnb_net_layer_channels(void* p, int i) { return ((NetHandle*)p)->net->Layers()[i]->GetNumChannels(); }
+// offset of the layer's [gamma | beta] (2 x channels floats) in the flat parameter / gradient buffers; -1: not batch-normalised
+API long long cnb_net_bn_offset(void* p, int layer) { return BnLayer(p, layer) ? ((NetHandle*)p)->net->BnOffsets()[layer] : -1; }
+// device vector of `channels` floats: which 0 running mean, 1 running sigma, 2 batch mean, 3 batch sigma (of the last
+// training-mode forward pass); NULL: not batch-normalised
+API float* cnb_net_bn_stat(void* p, int layer, int which) {
+  Layer* l = BnLayer(p, layer);
+  return l && which >= 0 && which < 4 ? l->BnStat(which) : nullptr;
+}
+// replaces the settings of the gamma or beta optimizer (its step count and momentum history stay).  0 ok, -1 not a
+// batch-normalised layer, -2 a config gamma / beta cannot train with (BnOptimizerConfigError, printed on stderr)
+API int cnb_net_set_bn_optimizer(void* p, int layer, int which, const OptimizerConfig* c) {
+  Layer* l = BnLayer(p, layer);
+  if (!l || which < 0 || which > 1) return -1;
+  if (const char* err = BnOptimizerConfigError(*c)) { fprintf(stderr, "convnet_b200 host: %s\n", err); return -2; }
+  l->BnOptimizer(which) = *c;
+  return 0;
+}
+API int cnb_net_get_bn_optimizer_state(void* p, int layer, int which, long long* step, float* epsilon, float* momentum) {
+  Layer* l = BnLayer(p, layer);
+  if (!l || which < 0 || which > 1) return -1;
+  *step = l->BnOptimizerStep(which);
+  OptimizerSchedule(l->BnOptimizer(which), *step, epsilon, momentum);
+  return 0;
+}
+// pure host logic: 0 if `c` can train gamma / beta, -2 if not (the reason on stderr)
+API int cnb_bn_optimizer_check(const OptimizerConfig* c) {
+  if (const char* err = BnOptimizerConfigError(*c)) { fprintf(stderr, "convnet_b200 host: %s\n", err); return -2; }
+  return 0;
+}
+
 API float cnb_net_loss(void* p) { return ((NetHandle*)p)->net->GetLoss(); }
 // one training step; *loss (may be NULL) receives the summed cross-entropy of the batch (one scalar D2H, like GetLoss)
 API void cnb_net_train_step(void* p, float* loss) { ((NetHandle*)p)->net->TrainOneBatch(loss); }
@@ -136,14 +180,50 @@ API int cnb_plan_buckets(int n_edges, const long long* offsets, const long long*
   for (const Bucket& k : b) { if (n >= cap) break; lo[n] = (long long)k.lo; hi[n] = (long long)k.hi; trigger[n] = k.trigger; n++; }
   return n;
 }
+// a host-only ConvNet (no device memory) of a model, or nullptr with the reason on stderr
+static ConvNet* TryBuildNet(const char* model, int batch) {
+  ModelConfig m;
+  if (!TryBuildModel(model, &m)) return nullptr;
+  try { return new ConvNet(m, batch); }
+  catch (const std::invalid_argument& e) { fprintf(stderr, "convnet_b200 host: %s\n", e.what()); return nullptr; }
+}
 // static description of a model (no device memory): per-edge parameter count, for planning / reporting
 API int cnb_model_edge_params(const char* model, int batch, int cap, long long* sizes) {
+  ConvNet* net = TryBuildNet(model, batch);
+  if (!net) return -1;
+  int n = 0;
+  for (Edge* e : net->Edges()) { if (n >= cap) break; sizes[n++] = (long long)e->GetParameterMemoryRequirement(); }
+  delete net;
+  return n;
+}
+// static description of a model: the flat parameter buffer (ConvNet::PlanParameters).  Returns the number of edges E
+// (-1: unknown model); fills edge_offsets[0, E) and, per layer, bn_offsets[0, E] (-1: not batch-normalised), each up to
+// `cap` entries, and *total (floats, padding included)
+API int cnb_model_param_layout(const char* model, int batch, int cap, long long* edge_offsets, long long* bn_offsets,
+                               long long* total) {
+  ConvNet* net = TryBuildNet(model, batch);
+  if (!net) return -1;
+  net->PlanParameters();
+  const int n = (int)net->Edges().size();
+  for (int i = 0; i < n && i < cap; i++) edge_offsets[i] = (long long)net->EdgeOffsets()[i];
+  for (int i = 0; i <= n && i < cap; i++) bn_offsets[i] = net->BnOffsets()[i];
+  *total = (long long)net->NumParameters();
+  delete net;
+  return n;
+}
+// static description of a model's layer `layer`: 1 batch-normalised (then *channels, *bn_f, *bn_epsilon and the gamma /
+// beta optimizers are filled), 0 not, -1 unknown model, -2 layer out of range.  name: 64 bytes, the layer's name
+API int cnb_model_bn_layer(const char* model, int layer, char* name, int* channels, float* bn_f, float* bn_epsilon,
+                           OptimizerConfig* gamma, OptimizerConfig* beta) {
   ModelConfig m;
   if (!TryBuildModel(model, &m)) return -1;
-  ConvNet net(m, batch);
-  int n = 0;
-  for (Edge* e : net.Edges()) { if (n >= cap) break; sizes[n++] = (long long)e->GetParameterMemoryRequirement(); }
-  return n;
+  if (layer < 0 || layer >= (int)m.layer.size()) return -2;
+  const LayerConfig& l = m.layer[layer];
+  strncpy(name, l.name.c_str(), 63); name[63] = 0;
+  if (!l.batch_normalize) return 0;
+  *channels = l.num_channels; *bn_f = l.bn_f; *bn_epsilon = l.bn_epsilon;
+  *gamma = l.gamma_optimizer; *beta = l.beta_optimizer;
+  return 1;
 }
 // static description of a model: the optimizer config of edge `edge` (which: 0 weights, 1 bias).  0 ok, -1 unknown model,
 // -2 edge out of range or without parameters

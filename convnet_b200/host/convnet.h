@@ -25,7 +25,15 @@ struct LayerConfig {
   Activation activation = LINEAR;
   int image_size_y = 0, image_size_x = 0, image_size_t = 1;   // input layer only
   float dropprob = 0.f;
+  // batch normalisation between the incoming edge and the activation (proto/convnet_config.proto:56-61)
+  bool batch_normalize = false;
+  float bn_f = 0.98f;                      // running averages: mu = bn_f*mu + (1-bn_f)*batch mean (likewise sigma)
+  float bn_epsilon = 1e-5f;                // sigma = sqrt(biased variance + bn_epsilon)
+  OptimizerConfig gamma_optimizer, beta_optimizer;
 };
+
+// nullptr if `c` can train gamma or beta, else why not: OptimizerConfigError, or a norm rule (refused, DESIGN.md §5)
+const char* BnOptimizerConfigError(const OptimizerConfig& c);
 
 struct ModelConfig {
   std::string name;
@@ -67,10 +75,30 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   void SetDerivFused(bool v) { deriv_fused_ = v; }                // the outgoing edge applies ReLU' in its epilogue
   ~Layer();
 
+  // ---- batch normalisation (layer.cc:452-510).  The incoming edge writes the pre-normalisation input x into its own
+  // buffer (GetPreBN); the forward pass (statistics, then gamma/beta and the activation) writes the state from it.  The
+  // backward pass reads x, not the state: the state has been through the ReLU and the dropout.
+  bool BatchNormalize() const { return config_.batch_normalize; }
+  Matrix& GetPreBN() { return pre_bn_; }
+  // gamma | beta: 2 * channels floats of the flat parameter, gradient and history buffers (ConvNet::PlanParameters)
+  void SetBnMemory(Matrix& params, Matrix& grads, Matrix& hist);
+  void InitializeBn();                                          // gamma = 1, beta = 0, mu = 0, sigma = 1 (layer.cc:271-278)
+  void ApplyBatchNormalization(bool train, bool emit_bf16);     // activation included (its own pass is switched off)
+  void ApplyDerivativeofBatchNormalization(bool emit_bf16);     // of the transform the last ApplyBatchNormalization applied
+  void AppendBnSgdTensors(std::vector<CnbOptTensor>& out);      // gamma and beta; advances both step counts
+  OptimizerConfig& BnOptimizer(int which) { return which ? config_.beta_optimizer : config_.gamma_optimizer; }   // 0 gamma, 1 beta
+  long long BnOptimizerStep(int which) const { return which ? beta_step_ : gamma_step_; }
+  // device vectors of `channels` floats: 0 running mean, 1 running sigma, 2 batch mean, 3 batch sigma
+  float* BnStat(int which) { return bn_stats_.GetDevData() + (size_t)which * config_.num_channels; }
+  long long BnPixels() const { return (long long)image_size_y_ * image_size_x_; }
+
  private:
   LayerConfig config_;
   int image_size_y_, image_size_x_, image_size_t_;
   Matrix state_, deriv_, loss_per_image_, dropout_mask_;
+  Matrix pre_bn_, bn_stats_, gamma_, beta_, grad_gamma_, grad_beta_, hist_gamma_, hist_beta_;
+  bool bn_train_ = false;                       // the last ApplyBatchNormalization used the batch statistics
+  long long gamma_step_ = 0, beta_step_ = 0;
   int* labels_ = nullptr;
   bool activation_fused_ = false, deriv_fused_ = false, dropout_deriv_folded_ = false;
 };
@@ -108,8 +136,11 @@ std::vector<Bucket> PlanBuckets(const std::vector<size_t>& edge_offset, const st
 
 class ConvNet {
  public:
-  ConvNet(const ModelConfig& model, int batch_size);
+  ConvNet(const ModelConfig& model, int batch_size);            // std::invalid_argument: a model this class cannot run
   virtual ~ConvNet();
+  // the layout of the flat parameter buffer (host only): each edge's slice padded to 128 floats, followed by the
+  // [gamma | beta] slice, also padded, of the layer the edge writes when that layer is batch-normalised
+  void PlanParameters();
   void AllocateMemory();                                        // convnet.cc:272-298: ONE flat parameter / gradient buffer
   virtual void Fprop(bool train);                               // convnet.cc:377-388
   virtual void Bprop();                                         // convnet.cc:390-405
@@ -135,6 +166,7 @@ class ConvNet {
   double FlopsTrainStep() const;                                // fprop + wgrad for every weighted edge + dgrad except into the input
   const std::vector<size_t>& EdgeOffsets() const { return edge_offset_; }
   const std::vector<size_t>& EdgeSizes() const { return edge_size_; }
+  const std::vector<long long>& BnOffsets() const { return bn_offset_; }     // per layer: offset of [gamma | beta], -1 none
   float* DeviceLoss() { return loss_sum_.GetDevData(); }
   // One traced TrainOneBatch: device times (ms since the step began) of the pipeline's milestones, for the scaling report:
   // {fprop_end, bprop_compute_end, step_end, n_buckets, then per bucket {MB, exchange_begin, exchange_end, sgd_end}}.
@@ -148,6 +180,8 @@ class ConvNet {
   std::vector<Edge*> edges_;                    // edges_[i]: layers_[i] -> layers_[i+1]
   Matrix parameters_, grad_parameters_, history_, loss_sum_;
   std::vector<size_t> edge_offset_, edge_size_;
+  std::vector<size_t> edge_span_;               // edge slice + the [gamma | beta] slice of its destination, both padded
+  std::vector<long long> bn_offset_;
   size_t num_params_ = 0;
   // Side-stream pipeline of TrainOneBatch: as soon as a bucket's gradients are final its all-reduce (data parallel) is
   // enqueued on side_, and once the bucket's edges have finished their dgrad the multi-tensor SGD step of that bucket

@@ -44,6 +44,10 @@ struct OptimizerConfig {
 const char* OptimizerConfigError(const OptimizerConfig& c);
 // (epsilon, momentum) of the update after `step` earlier ones: GetDecayedEpsilon / GetMomentum, optimizer.cc:83-104,158-165
 void OptimizerSchedule(const OptimizerConfig& c, long long step, float* epsilon, float* momentum);
+// one tensor's update under optimizer `o` (SGDOptimizer::Optimize, optimizer.cc:174-200), appended to `out` unless the
+// optimizer is still before start_optimization_after; advances `step` either way.  `rows`: the norm groups of the tensor
+void AppendOptTensor(const OptimizerConfig& o, long long& step, float* w, float* hist, const float* grad, long long n, int rows,
+                     std::vector<CnbOptTensor>& out);
 
 struct EdgeConfig {
   std::string name, source, dest;

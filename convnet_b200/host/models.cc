@@ -140,7 +140,33 @@ static void UseReferenceOptimizers(const std::string& base, ModelConfig& m) {
   }
 }
 
+// "<model>+bn": batch_normalize on every hidden layer written by a conv, 1x1 or FC edge.  gamma trains with the writing
+// edge's weight optimizer and beta with its bias optimizer, both without L2 decay and norm rules (a per-channel scale and
+// shift are not weights of a unit; the reference's norm rules would not apply to a [1 x channels] row anyway)
+static void UseBatchNorm(const std::string& name, ModelConfig& m) {
+  if (m.layer.front().image_size_t > 1)
+    throw std::invalid_argument("model '" + name + "': batch normalisation is not supported on 3-D layers (image_size_t > 1)");
+  for (size_t i = 0; i < m.edge.size(); i++) {
+    const EdgeConfig& e = m.edge[i];
+    LayerConfig& l = m.layer[i + 1];
+    if (l.is_output || (e.edge_type != CONVOLUTIONAL && e.edge_type != CONV_ONETOONE && e.edge_type != FC)) continue;
+    if (l.batch_normalize) throw std::invalid_argument("model '" + name + "': +bn is given twice");
+    l.batch_normalize = true;
+    l.gamma_optimizer = e.weight_optimizer;
+    l.beta_optimizer = e.bias_optimizer;
+    for (OptimizerConfig* o : {&l.gamma_optimizer, &l.beta_optimizer}) {
+      o->l2_decay = 0.f; o->weight_norm_limit = 0.f; o->weight_norm_constraint = 0.f;
+    }
+  }
+}
+
 ModelConfig BuildModel(const std::string& name) {
+  const std::string bn = "+bn";
+  if (name.size() > bn.size() && name.compare(name.size() - bn.size(), bn.size(), bn) == 0) {
+    ModelConfig m = BuildModel(name.substr(0, name.size() - bn.size()));
+    UseBatchNorm(name, m);
+    return m;
+  }
   const std::string ref = "+ref-optimizer";
   if (name.size() > ref.size() && name.compare(name.size() - ref.size(), ref.size(), ref) == 0) {
     const std::string base = name.substr(0, name.size() - ref.size());

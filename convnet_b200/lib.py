@@ -99,6 +99,9 @@ SIGNATURES = {
     "cnb_softmax": [FP, I, I],
     "cnb_softmax_ce_deriv": [FP, FP, FP, FP, I, I],
     "cnb_sum": [FP, FP, I],
+    "cnb_bn_stats": [FP, ct.c_longlong, I, F, F, FP, FP, FP, FP],
+    "cnb_bn_apply": [FP, FP, ct.c_longlong, I, FP, FP, FP, FP, I],
+    "cnb_bn_backward": [FP, FP, ct.c_longlong, I, FP, FP, FP, I, FP, FP],
 }
 RESTYPES = {
     "convnet_b200_version": I, "convnet_b200_get_stream": ct.c_void_p,

@@ -73,6 +73,14 @@ def load_host():
             "cnb_optimizer_schedule": ([ct.POINTER(OptimizerConfig), ll, ct.POINTER(f), ct.POINTER(f)], i),
             "cnb_model_edge_optimizer": ([ct.c_char_p, i, i, ct.POINTER(OptimizerConfig)], i),
             "cnb_net_grad_check": ([vp, ct.c_uint, i, ct.c_char_p, ct.POINTER(f), ct.POINTER(f), ct.POINTER(f)], i),
+            "cnb_net_layer_name": ([vp, i], ct.c_char_p), "cnb_net_layer_channels": ([vp, i], i),
+            "cnb_net_bn_offset": ([vp, i], ll), "cnb_net_bn_stat": ([vp, i, i], vp),
+            "cnb_net_set_bn_optimizer": ([vp, i, i, ct.POINTER(OptimizerConfig)], i),
+            "cnb_net_get_bn_optimizer_state": ([vp, i, i, ct.POINTER(ll), ct.POINTER(f), ct.POINTER(f)], i),
+            "cnb_bn_optimizer_check": ([ct.POINTER(OptimizerConfig)], i),
+            "cnb_model_param_layout": ([ct.c_char_p, i, i, ct.POINTER(ll), ct.POINTER(ll), ct.POINTER(ll)], i),
+            "cnb_model_bn_layer": ([ct.c_char_p, i, ct.c_char_p, ct.POINTER(i), ct.POINTER(f), ct.POINTER(f),
+                                    ct.POINTER(OptimizerConfig), ct.POINTER(OptimizerConfig)], i),
         }
         for name, (args, res) in sig.items():
             fn = getattr(H, name)
@@ -82,8 +90,12 @@ def load_host():
 
 
 class Net:
-    """A chain ConvNet built natively ("alexnet" | "lenet" | "c3d" | "tiny"; "alexnet+ref-optimizer" and
-    "lenet+ref-optimizer" train with the optimizer blocks of the reference's pbtxt files)."""
+    """A chain ConvNet built natively ("alexnet" | "lenet" | "c3d" | "tiny" | "gradcheck").  Suffixes:
+    "+ref-optimizer" (alexnet and lenet): train with the optimizer blocks of the reference's pbtxt files.
+    "+bn": batch normalisation on every hidden layer written by a conv, 1x1 or FC edge; gamma / beta train with that
+    edge's weight / bias optimizer, without L2 decay and norm rules ("tiny+bn", "lenet+bn", "alexnet+bn", "gradcheck+bn",
+    "alexnet+ref-optimizer+bn"; not "c3d+bn": 3-D layers are not supported).
+    "+gradcheck": run_grad_check's edge flags (e.g. "tiny+bn+gradcheck")."""
 
     def __init__(self, model, batch_size, seed=42, grad_checker=False):
         self.H = load_host()
@@ -189,6 +201,52 @@ class Net:
         """multiply the base epsilon of every optimizer by `factor` (ConvNet::ReduceLearningRate)"""
         self.H.cnb_net_reduce_learning_rate(self.h, factor)
 
+    # --- batch normalisation (Layer::ApplyBatchNormalization, src/layer.cc:452-510)
+    def bn_layers(self):
+        """[(layer index, name, channels, offset of [gamma | beta] in params_tensor())] of the batch-normalised layers"""
+        out = []
+        for i in range(self.H.cnb_net_num_layers(self.h)):
+            off = self.H.cnb_net_bn_offset(self.h, i)
+            if off >= 0:
+                out.append((i, self.H.cnb_net_layer_name(self.h, i).decode(), self.H.cnb_net_layer_channels(self.h, i), off))
+        return out
+
+    def _bn_layer(self, layer):
+        for entry in self.bn_layers():
+            if layer in (entry[0], entry[1]):
+                return entry
+        raise KeyError("layer %r is not batch-normalised (those that are: %s)" % (layer, [e[1] for e in self.bn_layers()]))
+
+    def bn_state(self, layer):
+        """the tensors of a batch-normalised layer (index or name), as zero-copy views: gamma / beta (into params_tensor()),
+        grad_gamma / grad_beta (into grads_tensor(): mean over the layer's N * pixels values, the reference's scaling),
+        running_mean / running_sigma, and batch_mean / batch_sigma of the last training-mode fprop"""
+        i, _, c, off = self._bn_layer(layer)
+        p, g = self.params_tensor(), self.grads_tensor()
+        stat = [self._view(self.H.cnb_net_bn_stat(self.h, i, k), c, "f") for k in range(4)]
+        return {"gamma": p[off:off + c], "beta": p[off + c:off + 2 * c], "grad_gamma": g[off:off + c],
+                "grad_beta": g[off + c:off + 2 * c], "running_mean": stat[0], "running_sigma": stat[1],
+                "batch_mean": stat[2], "batch_sigma": stat[3]}
+
+    def set_bn_optimizer(self, layer, gamma=None, beta=None):
+        """replace the settings of the gamma and / or beta optimizer of a batch-normalised layer (optimizer blocks as for
+        set_optimizer; norm rules are refused).  Step counts and momentum histories are kept."""
+        i = self._bn_layer(layer)[0]
+        for which, d in ((0, gamma), (1, beta)):
+            if d is None:
+                continue
+            if self.H.cnb_net_set_bn_optimizer(self.h, i, which, ct.byref(OptimizerConfig.from_dict(d))) != 0:
+                raise ValueError("set_bn_optimizer(%r, %s): config not supported (see stderr)" % (layer, ("gamma", "beta")[which]))
+
+    def bn_optimizer_state(self, layer):
+        """{"gamma": {...}, "beta": {...}}: updates counted so far ("step") and the epsilon / momentum of the next one"""
+        i, out = self._bn_layer(layer)[0], {}
+        for which, key in ((0, "gamma"), (1, "beta")):
+            step, eps, mom = ct.c_longlong(0), ct.c_float(0), ct.c_float(0)
+            self.H.cnb_net_get_bn_optimizer_state(self.h, i, which, ct.byref(step), ct.byref(eps), ct.byref(mom))
+            out[key] = {"step": step.value, "epsilon": eps.value, "momentum": mom.value}
+        return out
+
     def train_step(self, want_loss=True):
         if want_loss:
             v = ct.c_float(0)
@@ -243,6 +301,42 @@ def model_edge_optimizer(model, edge, which="weights"):
     if rc == -1:
         raise ValueError("unknown model %r (see stderr)" % model)
     return c.to_dict() if rc == 0 else None
+
+
+def model_bn_layers(model):
+    """the batch-normalised layers of a model (host-only): [{"layer", "name", "channels", "bn_f", "bn_epsilon",
+    "gamma_optimizer", "beta_optimizer"}] in chain order"""
+    H, out, i = load_host(), [], 0
+    while True:
+        name, ch, f_, eps = ct.create_string_buffer(64), ct.c_int(0), ct.c_float(0), ct.c_float(0)
+        g, b = OptimizerConfig(), OptimizerConfig()
+        rc = H.cnb_model_bn_layer(model.encode(), i, name, ct.byref(ch), ct.byref(f_), ct.byref(eps), ct.byref(g), ct.byref(b))
+        if rc == -1:
+            raise ValueError("unknown model %r (see stderr)" % model)
+        if rc == -2:
+            return out
+        if rc == 1:
+            out.append({"layer": i, "name": name.value.decode(), "channels": ch.value, "bn_f": f_.value,
+                        "bn_epsilon": eps.value, "gamma_optimizer": g.to_dict(), "beta_optimizer": b.to_dict()})
+        i += 1
+
+
+def model_param_layout(model, batch=1):
+    """the flat parameter buffer of a model (host-only): {"edge_offsets": [...], "bn_offsets": per layer (None: not
+    batch-normalised), "total": floats with padding}"""
+    cap = 256
+    eo, bo, total = (ct.c_longlong * cap)(), (ct.c_longlong * cap)(), ct.c_longlong(0)
+    n = load_host().cnb_model_param_layout(model.encode(), batch, cap, eo, bo, ct.byref(total))
+    if n < 0:
+        raise ValueError("cannot build model %r (see stderr)" % model)
+    return {"edge_offsets": [eo[k] for k in range(n)], "bn_offsets": [bo[k] if bo[k] >= 0 else None for k in range(n + 1)],
+            "total": total.value}
+
+
+def check_bn_optimizer(config):
+    """raise ValueError if the optimizer block `config` (a dict) cannot train gamma / beta"""
+    if load_host().cnb_bn_optimizer_check(ct.byref(OptimizerConfig.from_dict(config))) != 0:
+        raise ValueError("optimizer config not supported for gamma / beta: %r (see stderr)" % (config,))
 
 
 def optimizer_schedule(config, step):

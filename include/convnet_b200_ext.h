@@ -187,6 +187,29 @@ typedef struct CnbOptTensor {
 } CnbOptTensor;
 void cnb_sgd_update_multi(const CnbOptTensor* tensors, int count);
 
+/* ---- batch normalisation over the channels of a 2-D layer (Layer::ApplyBatchNormalization and
+ * ApplyDerivativeofBatchNormalization, src/layer.cc:452-510).  x, y and deriv hold `channels` contiguous blocks of n
+ * floats: channel c is [c*n, (c+1)*n), n = images * pixels (the layout of a layer state, DESIGN.md §3).  Per-channel
+ * vectors hold `channels` floats.  Reductions use a fixed order and no atomics: results are bit-reproducible.  Calls must
+ * be ordered on one stream (they share a library scratch buffer).
+ *
+ * cnb_bn_stats: batch_mu = mean(x), batch_sigma = sqrt(mean((x - batch_mu)^2) + eps) (two passes: the variance is taken
+ *   about the mean); when run_mu / run_sigma are given (both or neither), the running averages
+ *   run_mu = bn_f*run_mu + (1-bn_f)*batch_mu and run_sigma = bn_f*run_sigma + (1-bn_f)*batch_sigma (sigma, not the variance).
+ * cnb_bn_apply: y = gamma*(x - mu)/sigma + beta, then max(y, 0) if relu.  mu / sigma are the batch statistics (training)
+ *   or the running ones (test).  Honours convnet_b200_emit_bf16_next for y.
+ * cnb_bn_backward: with xhat = (x - mu)/sigma,
+ *   grad_beta = mean(deriv), grad_gamma = mean(deriv * xhat)            (1/n scaling, layer.cc:493-496), then in place
+ *   deriv = gamma/sigma * (deriv - grad_beta - xhat * grad_gamma)     train != 0 (mu / sigma: the batch statistics)
+ *   deriv = gamma/sigma * deriv                                       train == 0 (mu / sigma: the running statistics)
+ *   Honours convnet_b200_emit_bf16_next for deriv. */
+void cnb_bn_stats(const float* x, long long n, int channels, float eps, float bn_f, float* batch_mu, float* batch_sigma,
+                  float* run_mu, float* run_sigma);
+void cnb_bn_apply(const float* x, float* y, long long n, int channels, const float* gamma, const float* beta,
+                  const float* mu, const float* sigma, int relu);
+void cnb_bn_backward(float* deriv, const float* x, long long n, int channels, const float* gamma, const float* mu,
+                     const float* sigma, int train, float* grad_gamma, float* grad_beta);
+
 /* ---- input pipeline, device side (SURVEY.md §8 f4) -------------------------------------------------------------------
  * The reference keeps a chunk of the data set on the GPU, one image per COLUMN (pixel index = col + W*(row + H*color)),
  * and cuts every minibatch out of it with a random crop and mirror per image while transposing it into the image-fastest

@@ -180,26 +180,79 @@ __global__ void relu_deriv_kernel(float* dx, const float* __restrict__ y, long l
 //   (8192 / tile rows) columns, and while it stores the updated weights it also sums their squares per row; the tile's
 //   per-row sums go to part[slab * rows + r] (slab = the tile's column range) in a fixed order — no atomics, so the
 //   result is bit-reproducible.  norm_rescale_kernel then finishes the norms and rescales the rows that need it.
+// Each tensor has a rule (Adagrad / RMSProp: AdagradSGDOptimizer / RMSPropSGDOptimizer::Optimize, optimizer.cc:202-279),
+// uniform over its blocks; the adaptive rules also read and write a per-element state s.  The batch is larger than the
+// classic 4 KB parameter limit: sm_70+ with CUDA 12.1+ takes up to 32 KB of kernel parameters.
 constexpr int kSgdMaxTensors = 48, kSgdChunk = 4096, kNormTile = 8192, kNormRescaleRows = 32;
 enum { kNormNone = 0, kNormLimit = 1, kNormConstraint = 2 };
+enum { kRuleSgd = 0, kRuleAdagrad = 1, kRuleRmsProp = 2, kRuleAdagradState = 3 };   // the last: s only, w and h untouched
 struct SgdItem {
   float* w; float* h; const float* g; __nv_bfloat16* w16; float* part;   // part: row-norm partial sums (norm tensors)
-  long long n; float lr, mom, l2, clip, norm; int rows, mode, vec;
+  float* s;                                                              // adaptive rules: the state
+  long long n; float lr, mom, l2, clip, norm;
+  float rp, scale;                                                       // Adagrad: delta, sqrt(step + 1); RMSProp: factor
+  int rows, mode, vec, rule;
 };
-struct SgdBatch { int count; int first_block[kSgdMaxTensors + 1]; SgdItem t[kSgdMaxTensors]; };   // <= 4 KB of parameters
+struct SgdBatch { int count; int first_block[kSgdMaxTensors + 1]; SgdItem t[kSgdMaxTensors]; };
+static_assert(sizeof(SgdBatch) <= 32764, "kernel parameter limit");
 
 __device__ __forceinline__ int batch_item(const SgdBatch& b) {
   int ti = 0;
   while (ti + 1 < b.count && (int)blockIdx.x >= b.first_block[ti + 1]) ti++;      // <= 48 uniform steps
   return ti;
 }
-// one element: g += l2*w; clip g to [-clip, clip]; h = mom*h + lr*g; w -= h.  Written out with explicit roundings so that
-// every tensor, and every block mapping, computes the same bits (the fused l2 term and the h update are single FMAs).
-__device__ __forceinline__ void sgd1(float& w, float& h, float g, const SgdItem& t) {
+// x / s, and 0 where x is 0: the reference's 0 / 0 (Adagrad with delta 0, RMSProp with factor 0 and a zero gradient) is NaN
+__device__ __forceinline__ float safe_div(float x, float s) { return x == 0.f ? 0.f : __fdiv_rn(x, s); }
+// One element, in this order.  Every operation is rounded to nearest and written with an intrinsic, so nothing is
+// contracted and every tensor and block mapping computes the same bits; fma() is the one fused operation.
+//   Adagrad:  e = s - delta;  s = delta + sqrt(e*e + g*g);  g = safe_div(g, s) * scale   (state only: stop here)
+//   all:      d = fma(l2, w, g);  d = clamp(d, -clip, clip) if clip > 0
+//   RMSProp:  s = sqrt((f*s)*s + ((1-f)*d)*d);  d = safe_div(d, s)
+//   all:      h = fma(mom, h, lr*d);  w = w - h
+// The SGD rule is exactly the update this kernel has always computed.
+template <int R>
+__device__ __forceinline__ void opt1(float& w, float& h, float& s, float g, const SgdItem& t) {
+  if (R == kRuleAdagrad || R == kRuleAdagradState) {
+    const float e = __fsub_rn(s, t.rp);
+    s = __fadd_rn(t.rp, __fsqrt_rn(__fadd_rn(__fmul_rn(e, e), __fmul_rn(g, g))));
+    if (R == kRuleAdagradState) return;
+    g = __fmul_rn(safe_div(g, s), t.scale);
+  }
   float d = __fmaf_rn(t.l2, w, g);
   if (t.clip > 0.f) d = d > t.clip ? t.clip : (d < -t.clip ? -t.clip : d);     // UpperBoundMod (keeps NaN)
+  if (R == kRuleRmsProp) {
+    s = __fsqrt_rn(__fadd_rn(__fmul_rn(__fmul_rn(t.rp, s), s), __fmul_rn(__fmul_rn(__fsub_rn(1.f, t.rp), d), d)));
+    d = safe_div(d, s);
+  }
   h = __fmaf_rn(t.mom, h, __fmul_rn(t.lr, d));
   w = __fsub_rn(w, h);
+}
+// element i of a tensor: load what rule R reads, update, store what it writes (and the bf16 twin of w)
+template <int R>
+__device__ __forceinline__ float opt_at(const SgdItem& t, long long i) {
+  constexpr bool S = R != kRuleSgd, W = R != kRuleAdagradState;
+  float w = W ? t.w[i] : 0.f, h = W ? t.h[i] : 0.f, s = S ? t.s[i] : 0.f;
+  opt1<R>(w, h, s, t.g[i], t);
+  if (S) t.s[i] = s;
+  if (W) { t.h[i] = h; t.w[i] = w; if (t.w16) t.w16[i] = __float2bfloat16_rn(w); }
+  return w;
+}
+// four elements from i (16-byte aligned operands)
+template <int R>
+__device__ __forceinline__ float4 opt_at4(const SgdItem& t, long long i) {
+  constexpr bool S = R != kRuleSgd, W = R != kRuleAdagradState;
+  const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+  float4 w = W ? *reinterpret_cast<const float4*>(t.w + i) : z, h = W ? *reinterpret_cast<const float4*>(t.h + i) : z;
+  float4 s = S ? *reinterpret_cast<const float4*>(t.s + i) : z;
+  const float4 g = __ldg(reinterpret_cast<const float4*>(t.g + i));
+  opt1<R>(w.x, h.x, s.x, g.x, t); opt1<R>(w.y, h.y, s.y, g.y, t); opt1<R>(w.z, h.z, s.z, g.z, t); opt1<R>(w.w, h.w, s.w, g.w, t);
+  if (S) *reinterpret_cast<float4*>(t.s + i) = s;
+  if (W) {
+    *reinterpret_cast<float4*>(t.h + i) = h;
+    *reinterpret_cast<float4*>(t.w + i) = w;
+    emit4(t.w16, i >> 2, w);
+  }
+  return w;
 }
 __host__ __device__ inline int norm_tile_rows(int rows) {                      // power of two <= 128
   int r = 1;
@@ -210,40 +263,24 @@ __host__ __device__ inline long long norm_slabs(const SgdItem& t) {
   return ceil_div<long long>(t.n / t.rows, kNormTile / norm_tile_rows(t.rows));
 }
 
+template <int R>
 __device__ void sgd_chunk(const SgdItem& t, int block) {
   const long long e0 = (long long)block * kSgdChunk;
   const long long e1 = min(t.n, e0 + kSgdChunk);
   if (t.vec) {                                                                     // all pointers 16-byte aligned
     for (long long i = e0 + 4 * threadIdx.x; i < e1; i += 4 * 256) {
-      if (i + 4 <= e1) {
-        float4 w = *reinterpret_cast<const float4*>(t.w + i), h = *reinterpret_cast<const float4*>(t.h + i);
-        const float4 g = __ldg(reinterpret_cast<const float4*>(t.g + i));
-        sgd1(w.x, h.x, g.x, t); sgd1(w.y, h.y, g.y, t); sgd1(w.z, h.z, g.z, t); sgd1(w.w, h.w, g.w, t);
-        *reinterpret_cast<float4*>(t.h + i) = h;
-        *reinterpret_cast<float4*>(t.w + i) = w;
-        emit4(t.w16, i >> 2, w);
-      } else {
-        for (long long j = i; j < e1; j++) {
-          float wi = t.w[j], hi = t.h[j];
-          sgd1(wi, hi, t.g[j], t);
-          t.h[j] = hi; t.w[j] = wi;
-          if (t.w16) t.w16[j] = __float2bfloat16_rn(wi);
-        }
-      }
+      if (i + 4 <= e1) opt_at4<R>(t, i);
+      else for (long long j = i; j < e1; j++) opt_at<R>(t, j);
     }
   } else {
-    for (long long i = e0 + threadIdx.x; i < e1; i += 256) {
-      float wi = t.w[i], hi = t.h[i];
-      sgd1(wi, hi, t.g[i], t);
-      t.h[i] = hi; t.w[i] = wi;
-      if (t.w16) t.w16[i] = __float2bfloat16_rn(wi);
-    }
+    for (long long i = e0 + threadIdx.x; i < e1; i += 256) opt_at<R>(t, i);
   }
 }
 
 // a row-norm tile.  vec (rows % 4 == 0, tile of 128 rows, aligned): lane = 4 consecutive rows (512 contiguous bytes per
 // column and warp), warp = every 8th column of the tile's 64.  Otherwise: thread = one row and every (256 / tile rows)-th
 // column.  Either way each thread holds the sums of its rows over its columns; red[] combines them in lane order.
+template <int RULE>
 __device__ void sgd_norm_tile(const SgdItem& t, int block, float* red) {
   const int R = norm_tile_rows(t.rows), C = kNormTile / R;
   const long long K = t.n / t.rows;
@@ -258,13 +295,7 @@ __device__ void sgd_norm_tile(const SgdItem& t, int block, float* red) {
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
     if (r < t.rows) {
       for (long long k = c0 + warp; k < c1; k += 8) {
-        const long long i = r + (long long)t.rows * k;
-        float4 w = *reinterpret_cast<const float4*>(t.w + i), h = *reinterpret_cast<const float4*>(t.h + i);
-        const float4 g = __ldg(reinterpret_cast<const float4*>(t.g + i));
-        sgd1(w.x, h.x, g.x, t); sgd1(w.y, h.y, g.y, t); sgd1(w.z, h.z, g.z, t); sgd1(w.w, h.w, g.w, t);
-        *reinterpret_cast<float4*>(t.h + i) = h;
-        *reinterpret_cast<float4*>(t.w + i) = w;
-        emit4(t.w16, i >> 2, w);
+        const float4 w = opt_at4<RULE>(t, r + (long long)t.rows * k);
         s.x = __fmaf_rn(w.x, w.x, s.x); s.y = __fmaf_rn(w.y, w.y, s.y);
         s.z = __fmaf_rn(w.z, w.z, s.z); s.w = __fmaf_rn(w.w, w.w, s.w);
       }
@@ -275,11 +306,7 @@ __device__ void sgd_norm_tile(const SgdItem& t, int block, float* red) {
     float s = 0.f;
     if (r < t.rows) {
       for (long long k = c0 + lane; k < c1; k += lanes) {
-        const long long i = r + (long long)t.rows * k;
-        float wi = t.w[i], hi = t.h[i];
-        sgd1(wi, hi, t.g[i], t);
-        t.h[i] = hi; t.w[i] = wi;
-        if (t.w16) t.w16[i] = __float2bfloat16_rn(wi);
+        const float wi = opt_at<RULE>(t, r + (long long)t.rows * k);
         s = __fmaf_rn(wi, wi, s);
       }
     }
@@ -298,8 +325,20 @@ __global__ void __launch_bounds__(256) sgd_multi_kernel(const __grid_constant__ 
   const int ti = batch_item(b);
   const SgdItem& t = b.t[ti];
   const int block = (int)blockIdx.x - b.first_block[ti];
-  if (t.mode == kNormNone) sgd_chunk(t, block);
-  else sgd_norm_tile(t, block, red);
+  if (t.mode == kNormNone) {
+    switch (t.rule) {
+      case kRuleSgd: sgd_chunk<kRuleSgd>(t, block); break;
+      case kRuleAdagrad: sgd_chunk<kRuleAdagrad>(t, block); break;
+      case kRuleRmsProp: sgd_chunk<kRuleRmsProp>(t, block); break;
+      default: sgd_chunk<kRuleAdagradState>(t, block); break;
+    }
+  } else {
+    switch (t.rule) {                                       // (a state-only tensor never has a norm rule: no update)
+      case kRuleSgd: sgd_norm_tile<kRuleSgd>(t, block, red); break;
+      case kRuleAdagrad: sgd_norm_tile<kRuleAdagrad>(t, block, red); break;
+      default: sgd_norm_tile<kRuleRmsProp>(t, block, red); break;
+    }
+  }
 }
 
 // Second pass, norm tensors only: a block owns kNormRescaleRows rows.  It adds up each row's partial sums in slab order
@@ -690,14 +729,18 @@ void cnb_sum(const float* a, float* out, int n) {
   sum_kernel<<<1, 256, 0, state().stream>>>(a, out, n);
   count_launch(); CNB_LAUNCH_CHECK("sum");
 }
-void cnb_sgd_update_multi(const CnbOptTensor* tensors, int count) {
+void cnb_opt_update_multi(const CnbOptTensorEx* tensors, int count) {
   // partial sums of every norm tensor of the call, laid out one after the other (slabs x rows each)
   size_t part_floats = 0;
   for (int i = 0; i < count; i++) {
-    const CnbOptTensor& s = tensors[i];
-    if (s.n <= 0 || s.norm_mode == CNB_NORM_NONE) continue;
-    CNB_REQUIRE(s.norm_mode == CNB_NORM_LIMIT || s.norm_mode == CNB_NORM_CONSTRAINT, "cnb_sgd_update_multi");
-    CNB_REQUIRE(s.rows > 0 && s.n % s.rows == 0 && s.norm_value > 0.f, "cnb_sgd_update_multi");
+    const CnbOptTensorEx& x = tensors[i];
+    const CnbOptTensor& s = x.t;
+    CNB_REQUIRE(x.rule == CNB_RULE_SGD || x.rule == CNB_RULE_ADAGRAD || x.rule == CNB_RULE_RMSPROP, "cnb_opt_update_multi");
+    CNB_REQUIRE(x.rule == CNB_RULE_SGD || s.n <= 0 || x.state != nullptr, "cnb_opt_update_multi");
+    CNB_REQUIRE(!x.state_only || x.rule == CNB_RULE_ADAGRAD, "cnb_opt_update_multi");
+    if (s.n <= 0 || s.norm_mode == CNB_NORM_NONE || x.state_only) continue;
+    CNB_REQUIRE(s.norm_mode == CNB_NORM_LIMIT || s.norm_mode == CNB_NORM_CONSTRAINT, "cnb_opt_update_multi");
+    CNB_REQUIRE(s.rows > 0 && s.n % s.rows == 0 && s.norm_value > 0.f, "cnb_opt_update_multi");
     SgdItem t; t.n = s.n; t.rows = s.rows;
     part_floats += (size_t)norm_slabs(t) * s.rows;
   }
@@ -707,18 +750,29 @@ void cnb_sgd_update_multi(const CnbOptTensor* tensors, int count) {
     b.count = 0; nb.count = 0;
     int blocks = 0, nblocks = 0;
     for (int i = base; i < count && i < base + kSgdMaxTensors; i++) {
-      const CnbOptTensor& s = tensors[i];
+      const CnbOptTensorEx& x = tensors[i];
+      const CnbOptTensor& s = x.t;
       if (s.n <= 0) continue;
       SgdItem& t = b.t[b.count];
       t.w = s.w; t.h = s.hist; t.g = s.grad; t.n = s.n; t.lr = s.lr; t.mom = s.momentum; t.l2 = s.l2;
       t.clip = s.clip > 0.f ? s.clip : 0.f;
-      t.mode = s.norm_mode; t.norm = s.norm_value; t.rows = s.norm_mode ? s.rows : 1; t.part = nullptr;
-      t.vec = (aligned16(s.w) && aligned16(s.hist) && aligned16(s.grad)) ? 1 : 0;
+      t.mode = x.state_only ? CNB_NORM_NONE : s.norm_mode;
+      t.norm = s.norm_value; t.rows = t.mode ? s.rows : 1; t.part = nullptr;
+      t.s = x.rule == CNB_RULE_SGD ? nullptr : x.state;
+      t.rp = x.rule_param; t.scale = x.scale;
+      t.rule = x.state_only ? kRuleAdagradState
+                            : (x.rule == CNB_RULE_ADAGRAD ? kRuleAdagrad : (x.rule == CNB_RULE_RMSPROP ? kRuleRmsProp : kRuleSgd));
+      t.vec = (aligned16(s.w) && aligned16(s.hist) && aligned16(s.grad) && (!t.s || aligned16(t.s))) ? 1 : 0;
       if (t.mode) t.vec = t.vec && t.rows % 4 == 0 && norm_tile_rows(t.rows) == 128;
-      // the weights change: a staged bf16 copy of exactly this tensor is refreshed in the same pass, any other overlap dropped
-      const bool had_copy = bf16_staged(s.w, s.n) != nullptr;      // only a copy somebody keeps valid is worth refreshing
-      bf16_note_write(s.w, s.n);                    // every derived copy (bf16 twin, dgrad banks) goes stale ...
-      t.w16 = had_copy ? bf16_refresh_slot(s.w, s.n) : nullptr;    // ... and the bf16 twin is rewritten by this kernel
+      if (t.s) bf16_note_write(t.s, s.n);
+      if (t.rule == kRuleAdagradState) {                            // the weights stay as they are
+        t.w16 = nullptr;
+      } else {
+        // the weights change: a staged bf16 copy of exactly this tensor is refreshed in the same pass, any other overlap dropped
+        const bool had_copy = bf16_staged(s.w, s.n) != nullptr;    // only a copy somebody keeps valid is worth refreshing
+        bf16_note_write(s.w, s.n);                  // every derived copy (bf16 twin, dgrad banks) goes stale ...
+        t.w16 = had_copy ? bf16_refresh_slot(s.w, s.n) : nullptr;  // ... and the bf16 twin is rewritten by this kernel
+      }
       b.first_block[b.count] = blocks;
       if (t.mode) {
         const long long slabs = norm_slabs(t);
@@ -737,12 +791,17 @@ void cnb_sgd_update_multi(const CnbOptTensor* tensors, int count) {
     if (b.count == 0) continue;
     b.first_block[b.count] = blocks;
     sgd_multi_kernel<<<blocks, 256, 0, state().stream>>>(b);
-    count_launch(); CNB_LAUNCH_CHECK("sgd_update_multi");
+    count_launch(); CNB_LAUNCH_CHECK("opt_update_multi");
     if (nb.count == 0) continue;
     nb.first_block[nb.count] = nblocks;
     norm_rescale_kernel<<<nblocks, 256, 0, state().stream>>>(nb);
     count_launch(); CNB_LAUNCH_CHECK("sgd_norm_rescale");
   }
+}
+void cnb_sgd_update_multi(const CnbOptTensor* tensors, int count) {
+  std::vector<CnbOptTensorEx> t(count > 0 ? count : 0);
+  for (int i = 0; i < count; i++) t[i] = CnbOptTensorEx{tensors[i], CNB_RULE_SGD, 0, nullptr, 0.f, 1.f};
+  cnb_opt_update_multi(t.data(), count);
 }
 void cnb_sgd_momentum_multi(const CnbSgdTensor* tensors, int count) {
   std::vector<CnbOptTensor> t(count > 0 ? count : 0);

@@ -80,9 +80,12 @@ API int cnb_net_set_optimizer(void* p, int edge, int which, const OptimizerConfi
   EdgeWithWeight* e = WeightedEdge(p, edge);
   if (!e || which < 0 || which > 1) return -1;
   if (const char* err = OptimizerConfigError(*c)) { fprintf(stderr, "convnet_b200 host: %s\n", err); return -2; }
-  e->Optimizer(which) = *c;
+  ((NetHandle*)p)->net->SetOptimizer(e, which, *c);
   return 0;
 }
+// the adaptive optimizer state (cnb_net_num_params floats, carved like the parameters); NULL while no optimizer of the
+// net is ADAGRAD_SGD or RMSPROP_SGD
+API float* cnb_net_adaptive_state(void* p) { return ((NetHandle*)p)->net->AdaptiveState(); }
 // the step count of one optimizer and the (epsilon, momentum) its next update uses.  0 ok, -1 no such weighted edge
 API int cnb_net_get_optimizer_state(void* p, int edge, int which, long long* step, float* epsilon, float* momentum) {
   EdgeWithWeight* e = WeightedEdge(p, edge);
@@ -119,7 +122,7 @@ API int cnb_net_set_bn_optimizer(void* p, int layer, int which, const OptimizerC
   Layer* l = BnLayer(p, layer);
   if (!l || which < 0 || which > 1) return -1;
   if (const char* err = BnOptimizerConfigError(*c)) { fprintf(stderr, "convnet_b200 host: %s\n", err); return -2; }
-  l->BnOptimizer(which) = *c;
+  ((NetHandle*)p)->net->SetBnOptimizer(l, which, *c);
   return 0;
 }
 API int cnb_net_get_bn_optimizer_state(void* p, int layer, int which, long long* step, float* epsilon, float* momentum) {

@@ -82,10 +82,12 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   Matrix& GetPreBN() { return pre_bn_; }
   // gamma | beta: 2 * channels floats of the flat parameter, gradient and history buffers (ConvNet::PlanParameters)
   void SetBnMemory(Matrix& params, Matrix& grads, Matrix& hist);
+  void SetBnStateMemory(Matrix& state);                         // [gamma | beta] of the adaptive optimizer state
+  void InitBnState(int which);                                  // gamma's (0) or beta's (1) state back to its optimizer's start
   void InitializeBn();                                          // gamma = 1, beta = 0, mu = 0, sigma = 1 (layer.cc:271-278)
   void ApplyBatchNormalization(bool train, bool emit_bf16);     // activation included (its own pass is switched off)
   void ApplyDerivativeofBatchNormalization(bool emit_bf16);     // of the transform the last ApplyBatchNormalization applied
-  void AppendBnSgdTensors(std::vector<CnbOptTensor>& out);      // gamma and beta; advances both step counts
+  void AppendBnSgdTensors(std::vector<CnbOptTensorEx>& out);    // gamma and beta; advances both step counts
   OptimizerConfig& BnOptimizer(int which) { return which ? config_.beta_optimizer : config_.gamma_optimizer; }   // 0 gamma, 1 beta
   long long BnOptimizerStep(int which) const { return which ? beta_step_ : gamma_step_; }
   // device vectors of `channels` floats: 0 running mean, 1 running sigma, 2 batch mean, 3 batch sigma
@@ -96,7 +98,7 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   LayerConfig config_;
   int image_size_y_, image_size_x_, image_size_t_;
   Matrix state_, deriv_, loss_per_image_, dropout_mask_;
-  Matrix pre_bn_, bn_stats_, gamma_, beta_, grad_gamma_, grad_beta_, hist_gamma_, hist_beta_;
+  Matrix pre_bn_, bn_stats_, gamma_, beta_, grad_gamma_, grad_beta_, hist_gamma_, hist_beta_, state_gamma_, state_beta_;
   bool bn_train_ = false;                       // the last ApplyBatchNormalization used the batch statistics
   long long gamma_step_ = 0, beta_step_ = 0;
   int* labels_ = nullptr;
@@ -146,6 +148,15 @@ class ConvNet {
   virtual void Bprop();                                         // convnet.cc:390-405
   virtual void UpdateWeights();                                 // convnet.cc:440-450
   void ReduceLearningRate(float factor);                        // base epsilon of every weight and bias optimizer *= factor
+  // replace the settings of an edge's weight (which = 0) / bias (1) optimizer, or of a batch-normalised layer's gamma (0) /
+  // beta (1) optimizer; the step count and momentum history stay.  An adaptive optimizer allocates the net's state buffer
+  // if it has none, and the tensor's state restarts (adagrad_delta or 1) when optimizer_type or adagrad_delta changes.
+  // The caller has validated `c` (OptimizerConfigError / BnOptimizerConfigError) and the indices
+  void SetOptimizer(EdgeWithWeight* e, int which, const OptimizerConfig& c);
+  void SetBnOptimizer(Layer* l, int which, const OptimizerConfig& c);
+  // the adaptive optimizer state: one float per parameter, carved like the history (edge slices, then [gamma | beta]);
+  // nullptr until some optimizer of the net is ADAGRAD_SGD or RMSPROP_SGD
+  float* AdaptiveState() { return state_.GetDevData(); }
   void ComputeDeriv();
   void TrainOneBatch(float* loss_out);                          // convnet.cc:475-485
   float GetLoss();                                              // sum of per-image CE (synchronises)
@@ -178,7 +189,8 @@ class ConvNet {
   int batch_size_;
   std::vector<Layer*> layers_;
   std::vector<Edge*> edges_;                    // edges_[i]: layers_[i] -> layers_[i+1]
-  Matrix parameters_, grad_parameters_, history_, loss_sum_;
+  Matrix parameters_, grad_parameters_, history_, loss_sum_, state_;
+  void AllocateAdaptiveState();                 // state_ and its slices, each initialised for its optimizer
   std::vector<size_t> edge_offset_, edge_size_;
   std::vector<size_t> edge_span_;               // edge slice + the [gamma | beta] slice of its destination, both padded
   std::vector<long long> bn_offset_;

@@ -94,6 +94,7 @@ SIGNATURES = {
     "cnb_sgd_momentum": [FP, FP, FP, ct.c_longlong, F, F, F],
     "cnb_sgd_momentum_multi": [ct.c_void_p, I],
     "cnb_sgd_update_multi": [ct.c_void_p, I],
+    "cnb_opt_update_multi": [ct.c_void_p, I],
     "cnb_dropout": [FP, FP, ct.c_longlong, F, F, ct.c_ulonglong],
     "cnb_mult": [FP, FP, ct.c_longlong],
     "cnb_softmax": [FP, I, I],

@@ -8,20 +8,23 @@ from . import lib as _lib
 
 
 class OptimizerConfig(ct.Structure):
-    """host/edge.h OptimizerConfig: the SGD fields of the reference's proto Optimizer (proto/convnet_config.proto:64-113),
-    same names, same defaults, same order as the C struct."""
+    """host/edge.h OptimizerConfig: the SGD, Adagrad and RMSProp fields of the reference's proto Optimizer
+    (proto/convnet_config.proto:64-113), same names, same defaults, same order as the C struct."""
     _fields_ = [("epsilon", ct.c_float), ("epsilon_decay", ct.c_int), ("epsilon_decay_timescale", ct.c_int),
                 ("minimum_epsilon", ct.c_float), ("decay_factor", ct.c_float), ("initial_momentum", ct.c_float),
                 ("final_momentum", ct.c_float), ("momentum_transition_timescale", ct.c_int), ("l2_decay", ct.c_float),
                 ("gradient_clip", ct.c_float), ("start_optimization_after", ct.c_int), ("weight_norm_limit", ct.c_float),
-                ("weight_norm_constraint", ct.c_float)]
-    DEFAULTS = {"decay_factor": 1.0, "gradient_clip": -1.0}
+                ("weight_norm_constraint", ct.c_float), ("optimizer_type", ct.c_int), ("adagrad_delta", ct.c_float),
+                ("rms_prop_factor", ct.c_float)]
+    DEFAULTS = {"decay_factor": 1.0, "gradient_clip": -1.0, "adagrad_delta": 1.0}
     DECAY = {"NONE": 0, "INVERSE_T": 1, "EXPONENTIAL": 2, "LINEAR": 3, "EXPONENTIAL_STEP": 4}
+    TYPE = {"STOCHASTIC_GRADIENT_DESCENT": 0, "LBFGS": 1, "ADAGRAD_SGD": 2, "RMSPROP_SGD": 3}
 
     @classmethod
     def from_dict(cls, d):
-        """an optimizer block as a dict of proto field names (epsilon_decay also by name); unset fields take the proto's
-        defaults.  Fields outside the SGD path (Nesterov, Adagrad, RMSProp, LBFGS, shared prior) are not supported."""
+        """an optimizer block as a dict of proto field names (epsilon_decay and optimizer_type also by name); unset fields
+        take the proto's defaults.  Fields outside these paths (Nesterov, LBFGS's memory, shared prior) are not supported,
+        and the host refuses optimizer_type LBFGS."""
         c = cls(**cls.DEFAULTS)
         names = [f[0] for f in cls._fields_]
         for k, v in d.items():
@@ -29,6 +32,8 @@ class OptimizerConfig(ct.Structure):
                 raise KeyError("unsupported optimizer field %r (known: %s)" % (k, ", ".join(names)))
             if k == "epsilon_decay" and isinstance(v, str):
                 v = cls.DECAY[v]
+            if k == "optimizer_type" and isinstance(v, str):
+                v = cls.TYPE[v]
             setattr(c, k, v)
         return c
 
@@ -69,6 +74,7 @@ def load_host():
             "cnb_model_edge_params": ([ct.c_char_p, i, i, ct.POINTER(ll)], i),
             "cnb_net_reduce_learning_rate": ([vp, f], None),
             "cnb_net_set_optimizer": ([vp, i, i, ct.POINTER(OptimizerConfig)], i),
+            "cnb_net_adaptive_state": ([vp], vp),
             "cnb_net_get_optimizer_state": ([vp, i, i, ct.POINTER(ll), ct.POINTER(f), ct.POINTER(f)], i),
             "cnb_optimizer_schedule": ([ct.POINTER(OptimizerConfig), ll, ct.POINTER(f), ct.POINTER(f)], i),
             "cnb_model_edge_optimizer": ([ct.c_char_p, i, i, ct.POINTER(OptimizerConfig)], i),
@@ -95,6 +101,9 @@ class Net:
     "+bn": batch normalisation on every hidden layer written by a conv, 1x1 or FC edge; gamma / beta train with that
     edge's weight / bias optimizer, without L2 decay and norm rules ("tiny+bn", "lenet+bn", "alexnet+bn", "gradcheck+bn",
     "alexnet+ref-optimizer+bn"; not "c3d+bn": 3-D layers are not supported).
+    "+adagrad" / "+rmsprop": every weight, bias, gamma and beta optimizer on ADAGRAD_SGD (adagrad_delta 1, epsilon x 0.1) /
+    RMSPROP_SGD (rms_prop_factor 0.9, epsilon x 0.01); they compose with the others ("alexnet+ref-optimizer+rmsprop",
+    "tiny+bn+adagrad").
     "+gradcheck": run_grad_check's edge flags (e.g. "tiny+bn+gradcheck")."""
 
     def __init__(self, model, batch_size, seed=42, grad_checker=False):
@@ -148,6 +157,12 @@ class Net:
 
     def grads_tensor(self):
         return self._view(self.H.cnb_net_grads(self.h), self.num_params, "f")
+
+    def adaptive_state_tensor(self):
+        """the per-parameter state of the ADAGRAD_SGD / RMSPROP_SGD optimizers, laid out like params_tensor(); None while
+        no optimizer of the net is adaptive (the buffer is allocated by the first one)"""
+        ptr = self.H.cnb_net_adaptive_state(self.h)
+        return self._view(ptr, self.num_params, "f") if ptr else None
 
     def layer_state(self, i):
         return self._view(self.H.cnb_net_layer_state(self.h, i), self.H.cnb_net_layer_floats(self.h, i), "f")

@@ -187,6 +187,28 @@ typedef struct CnbOptTensor {
 } CnbOptTensor;
 void cnb_sgd_update_multi(const CnbOptTensor* tensors, int count);
 
+/* cnb_sgd_update_multi with a rule per tensor: the SGD step above, or the adaptive steps of AdagradSGDOptimizer and
+ * RMSPropSGDOptimizer::Optimize (src/optimizer.cc:202-279), which keep one more float per element, `state` (n floats;
+ * the caller initialises it to adagrad_delta resp. 1).  Per element, every operation rounded to nearest, fma the one
+ * fused operation (safe_div(x, s) = x / s, and 0 where x == 0: the reference's 0 / 0 gives NaN there):
+ *   CNB_RULE_ADAGRAD  e = s - delta;  s = delta + sqrt(e*e + g*g);  g = safe_div(g, s) * scale   (before the SGD step;
+ *                     rule_param = delta, scale = sqrt(step + 1) rounded to float; state_only != 0: only s is updated —
+ *                     the reference accumulates it also before start_optimization_after)
+ *   SGD step          d = fma(l2, w, g);  clip;  [RMSProp]  h = fma(momentum, h, lr*d);  w = w - h;  then the row-norm rule
+ *   CNB_RULE_RMSPROP  at [RMSProp]:  s = sqrt((f*s)*s + ((1-f)*d)*d);  d = safe_div(d, s)   (rule_param = f, the factor)
+ * A CNB_RULE_SGD tensor gets exactly the bits of cnb_sgd_update_multi.  Every rule goes into the same launches: one for
+ * the update and one for the rescale of rows when any tensor has a norm rule.  The gradient is only read. */
+enum { CNB_RULE_SGD = 0, CNB_RULE_ADAGRAD = 1, CNB_RULE_RMSPROP = 2 };
+typedef struct CnbOptTensorEx {
+  CnbOptTensor t;
+  int rule;            /* CNB_RULE_* */
+  int state_only;      /* CNB_RULE_ADAGRAD: update the state alone, leave w and hist as they are */
+  float* state;        /* adaptive rules: n floats */
+  float rule_param;    /* ADAGRAD: adagrad_delta; RMSPROP: rms_prop_factor */
+  float scale;         /* ADAGRAD: sqrt(step + 1) */
+} CnbOptTensorEx;
+void cnb_opt_update_multi(const CnbOptTensorEx* tensors, int count);
+
 /* ---- batch normalisation over the channels of a 2-D layer (Layer::ApplyBatchNormalization and
  * ApplyDerivativeofBatchNormalization, src/layer.cc:452-510).  x, y and deriv hold `channels` contiguous blocks of n
  * floats: channel c is [c*n, (c+1)*n), n = images * pixels (the layout of a layer state, DESIGN.md §3).  Per-channel

@@ -46,7 +46,6 @@ void finish_bias_grad(const Fuse& fuse, const float* part, int slices, const flo
 
 void conv_up(const ConvGeom& g, const float* images, const float* filters, float* targets, float st, float so) {
   Fuse fuse = take_fuse();
-  if (!g.conv && fuse.any()) { fprintf(stderr, "convnet_b200: epilogue fusion is not available for untied filters\n"); abort(); }
   CNB_REQUIRE(!fuse.bias_grad, "convUp: a fused bias gradient belongs to a backward call");
   Emit emit(targets, g.out_total, fuse.emit_bf16 != 0);
   emit.attach(fuse);
@@ -104,6 +103,7 @@ void simt_outp_auto(const ConvGeom& g, const float* images, const float* derivs,
 void conv_outp(const ConvGeom& g, const float* images, const float* derivs, float* targets, float st, float so) {
   take_fuse();                                 // a wgrad call has no epilogue to fuse: a pending request must not leak to a later call
   if (!g.conv) {                               // untied: one [Cout x K] block per module
+    if (state().precision != kPrecFP32 && tc_conv_outp(g, images, derivs, targets, st, so)) return;
     simt_conv_outp(g, images, derivs, targets, 1, 1, true, st, so);
     state().last_conv_path = kPathSimt;
     return;

@@ -27,7 +27,7 @@ struct FpropProblem {
   long long flt_z, img_z, out_z;  // per-blockIdx.z strides (untied module / 3-D frame)
   int z_is_module;              // untied: z = module and M = N
   float st, so;
-  const float* bias; int relu;  // fused epilogue (convnet_b200_fuse_next)
+  const float* bias; int relu;  // fused epilogue (convnet_b200_fuse_next); untied: one bias per output feature
   __device__ __forceinline__ long long rows() const { return M; }
   __device__ __forceinline__ int cols() const { return Cout; }
   __device__ __forceinline__ int depth() const { return K; }
@@ -49,7 +49,7 @@ struct FpropProblem {
   __device__ __forceinline__ void store(long long m, int o, float acc, int z) const {
     float* t = out + (z_is_module ? (long long)z * N : z * out_z) + m + (long long)N * modules * o;
     float r = (st == 0.f) ? so * acc : st * (*t) + so * acc;
-    if (bias) r += __ldg(bias + o);
+    if (bias) r += __ldg(bias + (z_is_module ? z + (long long)modules * o : o));
     if (relu) r = fmaxf(r, 0.f);
     *t = r;
   }
@@ -313,7 +313,7 @@ void reduce_partials(const float* part, float* out, long long elems, int groups,
 void simt_conv_up(const ConvGeom& g, const float* images, const float* filters, float* targets,
                   float scaleTargets, float scaleOutput, const Fuse& fuse) {
   FpropProblem p;
-  p.bias = fuse.bias ? fuse.bias + g.cout0 : nullptr; p.relu = fuse.relu;
+  p.bias = fuse.bias ? fuse.bias + (long long)g.cout0 * (g.conv ? 1 : g.modules) : nullptr; p.relu = fuse.relu;
   p.img = images + (long long)g.cin0 * g.H * g.W * g.N;
   p.flt = filters;
   p.out = targets + (long long)g.cout0 * g.modules * g.N;

@@ -64,7 +64,11 @@ struct TcParams {
   // merged requests: when N % 128 == 0 (2-D) the chunks of an m-tile are one box over a (chunk, ..., N/chunk, ...) view
   // of the tensor; when Cout % chunk == 0 the BN/chunk filter chunks are one box likewise.
   int a_merged, b_merged;
-  int total_chunks;                 // fprop: nbc*modules*frames ; dgrad: nbc*W*H   (< 2^31, checked on the host)
+  // untied filters (localUp / localDown / localOutp): one [K x Cout] bank per module, banks consecutive, and the B tensor
+  // map has a module dimension.  Only with N % 128 == 0 (2-D), so that every fprop / dgrad m-tile lies in ONE module /
+  // input pixel.  wgrad: `split` is the module, the reduction runs over the images alone.
+  int untied;
+  int total_chunks;                // fprop: nbc*modules*frames ; dgrad: nbc*W*H   (< 2^31, checked on the host)
   int splits, units_per_split;      // wgrad: (frame, module-row) units per reduction split;
                                     // fprop/dgrad of 1x1 / FC shapes with few tiles: K blocks per split (split-K)
   long long part_stride;            // fprop/dgrad split-K: floats between the partial outputs of consecutive splits
@@ -199,6 +203,8 @@ __device__ __forceinline__ int tile_kblocks(const TcParams& p, const Tile& tile)
     const DgradTaps own = dgrad_taps(p, decode_chunks(p, tile.m_tile, p.W * p.H));
     const int kcb = p.splits > 1 ? min(p.units_per_split, p.kc_blocks - tile.split * p.units_per_split) : p.kc_blocks;
     return max(dgrad_live_taps(p, own), 1) * kcb;
+  } else if (p.untied) {
+    return p.nbc;
   } else if (p.x_mode) {
     const int r0 = tile.split * p.units_per_split, r1 = min(r0 + p.units_per_split, p.modY * p.frames);
     return (r1 - r0) * p.modX * p.nb;
@@ -295,6 +301,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
           // split-K (host: only when taps == 1): this tile reduces K blocks [cb0, cb1)
           const int cb0 = p.splits > 1 ? tile.split * p.units_per_split : 0;
           const int cb1 = p.splits > 1 ? min(cb0 + p.units_per_split, p.kc_blocks) : p.kc_blocks;
+          const int mod = ch.pos[0];                  // untied: the module of the whole tile
           for (int ty = 0; ty < p.ky; ty++)
             for (int tx = 0; tx < p.kx; tx++) {
               const int tap = tx + p.kx * ty;
@@ -309,11 +316,14 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     if (c < p.cpt) lda5(&mapA, a + c * (p.bk * 128), ch.n[c], cb * p.bk, cX[c] + tx, cY[c] + ty, ch.f[c]);
                 }
                 const int o0 = tile.n_tile * p.BN;
-                if (p.b_merged) {                // dims (o_lo, c, o_hi, tap)
-                  lda4(&mapB, b, 0, cb * p.bk, o0 >> p.chunk_shift, tap);
+                if (p.b_merged) {                // dims (o_lo, c, o_hi, tap[, module])
+                  if (p.untied) lda5(&mapB, b, 0, cb * p.bk, o0 >> p.chunk_shift, tap, mod);
+                  else lda4(&mapB, b, 0, cb * p.bk, o0 >> p.chunk_shift, tap);
                 } else {
-                  for (int j = 0; j < ((p.BN + p.chunk - 1) >> p.chunk_shift); j++)
-                    lda3(&mapB, b + j * (p.bk * 128), o0 + j * p.chunk, tap, cb * p.bk);
+                  for (int j = 0; j < ((p.BN + p.chunk - 1) >> p.chunk_shift); j++) {
+                    if (p.untied) lda4(&mapB, b + j * (p.bk * 128), o0 + j * p.chunk, tap, cb * p.bk, mod);
+                    else lda3(&mapB, b + j * (p.bk * 128), o0 + j * p.chunk, tap, cb * p.bk);
+                  }
                 }
                 end_stage();
               }
@@ -339,6 +349,8 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
               my[c] = lv ? (cY[c] - p.py - ty) / p.sy : -1;
             }
             const int tap = tx + p.kx * ty;
+            // untied: the tile's pixel reaches this tap through one module, whose bank B reads (-1: none -> zeros)
+            const int mod = mx[0] >= 0 ? mx[0] + p.modX * my[0] : -1;
             for (int ob = ob0; ob < ob1; ob++) {
               uint8_t* a = begin_stage();
               uint8_t* b = smemB + (size_t)stage * kBStageBytes;
@@ -349,10 +361,22 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 for (int c = 0; c < 4; c++)
                   if (c < p.cpt) lda5(&mapA, a + c * (p.bk * 128), ch.n[c], ob * p.bk, mx[c], my[c], p.frame0);
               }
-              lda3(&mapB, b, ob * p.bk, tap, tile.n_tile * p.BN);
+              if (p.untied) lda4(&mapB, b, ob * p.bk, tap, tile.n_tile * p.BN, mod);
+              else lda3(&mapB, b, ob * p.bk, tap, tile.n_tile * p.BN);
               end_stage();
             }
           }
+      } else if (p.untied) {
+        // dW_module[o, tap, c]: the reduction runs over the images alone; a tap outside the image is zero-filled by TMA
+        const int mx = tile.split % p.modX, my = tile.split / p.modX;
+        const int X = mx * p.sx + p.px + tile.tap % p.kx, Y = my * p.sy + p.py + tile.tap / p.kx;
+        for (int ib = 0; ib < p.nbc; ib++) {
+          uint8_t* a = begin_stage();
+          uint8_t* b = smemB + (size_t)stage * kBStageBytes;
+          lda5(&mapA, a, ib * p.chunk, mx, my, tile.o_tile * BM, 0);
+          lda5(&mapB, b, ib * p.chunk, X, Y, tile.c_tile * p.BN, 0);
+          end_stage();
+        }
       } else if (p.x_mode) {
         // reduction over every module of this split's rows; B holds x_ct channels x ky rows x 8 taps
         const int r0 = tile.split * p.units_per_split, r1 = min(r0 + p.units_per_split, p.modY * p.frames);
@@ -508,10 +532,15 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     if (OP == kFprop || OP == kDgrad) ncols_valid = min(p.BN, (OP == kFprop ? p.Cout : p.Cin) - tile.n_tile * p.BN);
     else if (p.x_mode) ncols_valid = min(p.BN, p.x_ct * p.ky * 8);
     else ncols_valid = min(p.BN, p.Cin - tile.c_tile * p.BN);
-    const bool direct_scale = (p.splits == 1);
+    const bool direct_scale = (p.splits == 1) || (OP == kWgrad && p.untied);   // untied wgrad: one dW block per module
     const float so_eff = direct_scale ? p.so : 1.f;
     const bool rmw = direct_scale && p.st != 0.f;
     const float* bias = (OP == kFprop && p.bias) ? p.bias + tile.n_tile * p.BN : nullptr;
+    int bias_step = 1;
+    if (OP == kFprop && p.bias && p.untied) {         // one bias per output feature: bias[module + modules * o]
+      bias = p.bias + (tile.m_tile * p.cpt / p.nbc) + (long long)p.modules * tile.n_tile * p.BN;
+      bias_step = p.modules;
+    }
 #pragma unroll
     for (int h = 0; h < 2; h++) {
       float* const rp = rowp[h];
@@ -535,7 +564,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
           float r = so_eff * v;
           if (rmw) r += p.st * (*dst);
           if (OP == kFprop) {
-            if (bias) r += __ldg(bias + col);
+            if (bias) r += __ldg(bias + col * bias_step);
             if (p.relu) r = fmaxf(r, 0.f);
             if (p.drop_scale != 0.f) r *= dropout_keep(p.drop_seed + (unsigned long long)(dst - p.out), p.drop_prob, p.drop_scale);
           }
@@ -644,6 +673,7 @@ void fill_common(TcParams& p, const ConvGeom& g, const Elem& e) {
   p.splits = 1; p.units_per_split = 0; p.part_stride = 0;
   p.x_mode = 0; p.x_yblocks = 0; p.x_ct = 0; p.b_tx_bytes = 0;
   p.a_merged = 0; p.b_merged = 0;
+  p.untied = g.conv ? 0 : 1;
   p.bias = nullptr; p.relu = 0; p.mask = nullptr; p.out16 = nullptr;
   p.drop_prob = 0.f; p.drop_scale = 0.f; p.drop_seed = 0;
   p.o_sx = p.o_sy = 1; p.o_x0 = p.o_y0 = 0; p.o_W = g.modX; p.out_plane = g.modules;
@@ -685,19 +715,24 @@ bool merged_image_map(CUtensorMap* m, const void* base, const Elem& e, const Con
 
 // MN-major filter operand [K = (tap, c)] x [columns], columns contiguous: dims (col, tap, c), or (col_lo, c, col_hi, tap)
 // when `merged` (one request per stage).  `cols` = the column count of the whole tensor, `bn` = columns per tile.
+// `modules` > 0: untied, that many consecutive banks, and a trailing module dimension.
 bool filter_map(CUtensorMap* m, const void* base, const Elem& e, long long cols, long long taps, long long K_c, int bn,
-                bool merged) {
+                bool merged, long long modules = 0) {
+  const long long bank = cols * taps * K_c;
+  const int extra = modules > 0 ? 1 : 0;
   if (merged) {
-    const long long dims[4] = {e.chunk, K_c, cols / e.chunk, taps};
-    const long long str[3] = {cols * taps, e.chunk, cols};
-    const int box[4] = {e.chunk, e.bk, bn / e.chunk, 1};
-    return make_map(m, base, e, 4, dims, str, box);
+    const long long dims[5] = {e.chunk, K_c, cols / e.chunk, taps, modules};
+    const long long str[4] = {cols * taps, e.chunk, cols, bank};
+    const int box[5] = {e.chunk, e.bk, bn / e.chunk, 1, 1};
+    return make_map(m, base, e, 4 + extra, dims, str, box);
   }
-  const long long dims[3] = {cols, taps, K_c};
-  const long long str[2] = {cols, cols * taps};
-  const int box[3] = {e.chunk, 1, e.bk};
-  return make_map(m, base, e, 3, dims, str, box);
+  const long long dims[4] = {cols, taps, K_c, modules};
+  const long long str[3] = {cols, cols * taps, bank};
+  const int box[4] = {e.chunk, 1, e.bk, 1};
+  return make_map(m, base, e, 3 + extra, dims, str, box);
 }
+// floats in the filter tensor of a call: Cout x K, times the modules for untied filters
+inline long long filter_elems(const ConvGeom& g) { return (long long)g.Cout * g.K * (g.conv ? 1 : g.modules); }
 
 inline size_t align_up(size_t v) { return (v + 1023) & ~size_t(1023); }
 
@@ -759,11 +794,13 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
   const bool x_mode = g.Cin < 8;                                            // tiny channel counts: taps take the K block
   if (x_mode && (g.kx > 8 || g.ky > 8)) return false;
   if (bf && (x_mode || g.N % 8 != 0 || g.Cout % 8 != 0 || !aligned16(images) || !aligned16(filters))) return false;
+  if (!g.conv && (g.N % 128 != 0 || g.frames != 1 || x_mode)) return false;   // untied: each m-tile in one module
+  const long long flt_n = filter_elems(g);
   // few GEMM rows (FC layers at training batch sizes): the call streams the weights once and is HBM-bound on them; a bf16
   // conversion pass inside the call would read them a second time, so such shapes take bf16 only when the caller keeps a
   // staged bf16 copy of the weights (the training host does: cnb_sgd_momentum refreshes it in the same pass that updates
   // them) — then the call streams HALF the bytes
-  if (bf && (long long)g.N * g.modules * g.frames < 1024 && !bf16_staged(filters, (long long)g.Cout * g.K)) return false;
+  if (bf && (long long)g.N * g.modules * g.frames < 1024 && !bf16_staged(filters, flt_n)) return false;
   TcParams p; fill_common(p, g, e);
   p.BN = pick_bn(g.Cout, e.chunk);
   p.kc_blocks = ceil_div(g.Cin, e.bk);
@@ -778,9 +815,9 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
   // MN-major B is staged in whole chunks (BN is a multiple of the chunk)
   p.b_tx_bytes = (uint32_t)p.BN * 128;
   float* const out = targets + (long long)g.cout0 * g.modules * g.N;
-  const float* const bias = fuse.bias ? fuse.bias + g.cout0 : nullptr;
+  const float* const bias = fuse.bias ? fuse.bias + (long long)g.cout0 * (g.conv ? 1 : g.modules) : nullptr;
   const long long out_elems = (long long)g.Cout * g.modules * g.N;
-  const int ks = pick_ksplit(p, g, out_elems);
+  const int ks = g.conv ? pick_ksplit(p, g, out_elems) : 1;
   if (ks > 1) {
     p.units_per_split = ceil_div(p.kc_blocks, ks);
     p.splits = ceil_div(p.kc_blocks, p.units_per_split);
@@ -799,11 +836,11 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
   uint8_t* ws = nullptr;
   if (bf) {
     const __nv_bfloat16* si = bf16_staged(images, g.img_total);
-    const __nv_bfloat16* sf = bf16_staged(filters, (long long)g.Cout * g.K);
-    const size_t ib = si ? 0 : align_up((size_t)g.img_total * 2), fb = sf ? 0 : align_up((size_t)g.Cout * g.K * 2);
+    const __nv_bfloat16* sf = bf16_staged(filters, flt_n);
+    const size_t ib = si ? 0 : align_up((size_t)g.img_total * 2), fb = sf ? 0 : align_up((size_t)flt_n * 2);
     if (part_bytes + ib + fb) ws = (uint8_t*)workspace(part_bytes + ib + fb);
     if (!si) { to_bf16(images, (__nv_bfloat16*)(ws + part_bytes), g.img_total); si = (const __nv_bfloat16*)(ws + part_bytes); }
-    if (!sf) { to_bf16(filters, (__nv_bfloat16*)(ws + part_bytes + ib), (long long)g.Cout * g.K); sf = (const __nv_bfloat16*)(ws + part_bytes + ib); }
+    if (!sf) { to_bf16(filters, (__nv_bfloat16*)(ws + part_bytes + ib), flt_n); sf = (const __nv_bfloat16*)(ws + part_bytes + ib); }
     img = si + img_off;
     flt = sf;
   } else if (part_bytes) {
@@ -844,7 +881,7 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
     if (p.a_merged) {
       if (!merged_image_map(&ma, img, e, g, g.W, g.H, g.Cin, false)) return false;
     } else if (!image_map(&ma, img, e, g, g.W, g.H, g.Cin, g.in_frame_step, true, e.bk)) return false;
-    if (!filter_map(&mb, flt, e, g.Cout, taps, g.Cin, p.BN, p.b_merged)) return false;
+    if (!filter_map(&mb, flt, e, g.Cout, taps, g.Cin, p.BN, p.b_merged, g.conv ? 0 : g.modules)) return false;
   }
   launch<kFprop>(ma, mb, p);
   if (emit && fuse.emitted) *fuse.emitted = true;
@@ -855,7 +892,6 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
 }
 bool tc_conv_up(const ConvGeom& g, const float* images, const float* filters, float* targets, float st, float so,
                 const Fuse& fuse) {
-  if (!g.conv) return false;
   if (want_bf16() && tc_conv_up_impl(g, images, filters, targets, st, so, fuse, true)) return true;
   return tc_conv_up_impl(g, images, filters, targets, st, so, fuse, false);
 }
@@ -935,7 +971,9 @@ static bool tc_conv_down_impl(const ConvGeom& g, const float* derivs, const floa
   const Elem e = elem_for(bf);
   if (g.N % 4 != 0 || g.Cout % 4 != 0 || g.Cout < 8 || g.Cin < 8) return false;
   if (bf && (g.N % 8 != 0 || g.Cout % 8 != 0 || !aligned16(derivs) || !aligned16(filters))) return false;
-  if (bf && (long long)g.N * g.W * g.H < 1024 && !bf16_staged(filters, (long long)g.Cout * g.K)) return false;   // see tc_conv_up_impl
+  if (!g.conv && (g.N % 128 != 0 || g.frames != 1)) return false;          // untied: each m-tile on one input pixel
+  const long long flt_n = filter_elems(g);
+  if (bf && (long long)g.N * g.W * g.H < 1024 && !bf16_staged(filters, flt_n)) return false;   // see tc_conv_up_impl
   TcParams p; fill_common(p, g, e);
   p.BN = pick_bn(g.Cin, 16);
   p.kc_blocks = ceil_div(g.Cout, e.bk);
@@ -949,7 +987,7 @@ static bool tc_conv_down_impl(const ConvGeom& g, const float* derivs, const floa
   p.b_tx_bytes = (uint32_t)p.BN * 128;
   const bool whole = (g.frames == 1 && g.cin0 == 0 && g.Cin == g.CinT);
   const long long out_elems = (long long)g.Cin * g.W * g.H * g.N;
-  const int ks = whole ? pick_ksplit(p, g, out_elems) : 1;
+  const int ks = whole && g.conv ? pick_ksplit(p, g, out_elems) : 1;
   if (ks > 1) {
     p.units_per_split = ceil_div(p.kc_blocks, ks);
     p.splits = ceil_div(p.kc_blocks, p.units_per_split);
@@ -964,11 +1002,11 @@ static bool tc_conv_down_impl(const ConvGeom& g, const float* derivs, const floa
   uint8_t* ws = nullptr;
   if (bf) {
     const __nv_bfloat16* sd = bf16_staged(derivs, g.out_total);
-    const __nv_bfloat16* sf = bf16_staged(filters, (long long)g.Cout * g.K);
-    const size_t db = sd ? 0 : align_up((size_t)g.out_total * 2), fb = sf ? 0 : align_up((size_t)g.Cout * g.K * 2);
+    const __nv_bfloat16* sf = bf16_staged(filters, flt_n);
+    const size_t db = sd ? 0 : align_up((size_t)g.out_total * 2), fb = sf ? 0 : align_up((size_t)flt_n * 2);
     if (part_bytes + db + fb) ws = (uint8_t*)workspace(part_bytes + db + fb);
     if (!sd) { to_bf16(derivs, (__nv_bfloat16*)(ws + part_bytes), g.out_total); sd = (const __nv_bfloat16*)(ws + part_bytes); }
-    if (!sf) { to_bf16(filters, (__nv_bfloat16*)(ws + part_bytes + db), (long long)g.Cout * g.K); sf = (const __nv_bfloat16*)(ws + part_bytes + db); }
+    if (!sf) { to_bf16(filters, (__nv_bfloat16*)(ws + part_bytes + db), flt_n); sf = (const __nv_bfloat16*)(ws + part_bytes + db); }
     der = sd + der_off;
     flt = sf;
   } else if (part_bytes) {
@@ -978,11 +1016,11 @@ static bool tc_conv_down_impl(const ConvGeom& g, const float* derivs, const floa
   if (p.a_merged) {
     if (!merged_image_map(&ma, der, e, g, g.modX, g.modY, g.Cout, false)) return false;
   } else if (!image_map(&ma, der, e, g, g.modX, g.modY, g.Cout, g.out_frame_step, true, e.bk)) return false;
-  {
-    const long long dims[3] = {g.Cout, (long long)g.kx * g.ky, g.Cin};
-    const long long str[2] = {g.Cout, (long long)g.Cout * g.kx * g.ky};
-    const int box[3] = {e.chunk, 1, p.BN};
-    if (!make_map(&mb, flt, e, 3, dims, str, box)) return false;
+  {                                                    // (o, tap, c[, module])
+    const long long dims[4] = {g.Cout, (long long)g.kx * g.ky, g.Cin, g.modules};
+    const long long str[3] = {g.Cout, (long long)g.Cout * g.kx * g.ky, (long long)g.Cout * g.K};
+    const int box[4] = {e.chunk, 1, p.BN, 1};
+    if (!make_map(&mb, flt, e, g.conv ? 3 : 4, dims, str, box)) return false;
   }
   float* out = targets + (long long)g.cin0 * g.H * g.W * g.N;
   if (whole && p.splits > 1) {
@@ -1009,7 +1047,6 @@ static bool tc_conv_down_impl(const ConvGeom& g, const float* derivs, const floa
 }
 bool tc_conv_down(const ConvGeom& g, const float* derivs, const float* filters, float* targets, float st, float so,
                   const Fuse& fuse) {
-  if (!g.conv) return false;
   if (want_bf16() && st == 0.f && tc_conv_down_as_fprop(g, derivs, filters, targets, so, fuse)) return true;
   if (want_bf16() && tc_conv_down_impl(g, derivs, filters, targets, st, so, fuse, true)) return true;
   return tc_conv_down_impl(g, derivs, filters, targets, st, so, fuse, false);
@@ -1023,6 +1060,7 @@ static bool tc_conv_outp_impl(const ConvGeom& g, const float* images, const floa
   const bool x_mode = g.Cin < 8;
   if (x_mode && (g.kx > 8 || g.ky > 8)) return false;
   if (bf && (x_mode || g.N % 8 != 0 || !aligned16(images) || !aligned16(derivs))) return false;
+  if (!g.conv && (g.N % 128 != 0 || g.frames != 1 || x_mode)) return false;
   // few reduction rows (FC layers: K = batch): the call is bound by WRITING dW, and the operands a bf16 pass would convert
   // are tiny — such shapes take bf16 only in the whole-batch-tile layout the training step uses
   if (bf && (long long)g.N * g.modules * g.frames < 1024 && !(g.frames == 1 && g.N % 128 == 0 && g.Cin % 32 == 0)) return false;
@@ -1063,13 +1101,18 @@ static bool tc_conv_outp_impl(const ConvGeom& g, const float* images, const floa
   while (splits > 1 && elems * splits * 4 > (1LL << 30)) splits--;
   p.units_per_split = ceil_div(units, splits);
   p.splits = ceil_div(units, p.units_per_split);
+  if (!g.conv) {                 // untied: one tile per (module, tap, o-tile, c-tile), stored straight into its module's block
+    if (base_tiles * g.modules >= (1LL << 31)) return false;
+    p.splits = g.modules; p.units_per_split = 1;
+  }
   p.num_tiles = (int)(base_tiles * p.splits);
   p.st = st; p.so = so;
   CUtensorMap ma, mb;
   const long long img_off = (long long)g.cin0 * g.H * g.W * g.N, der_off = (long long)g.cout0 * g.modules * g.N;
   const void* img = images + img_off;
   const void* der = derivs + der_off;
-  const size_t part_bytes = p.splits > 1 ? align_up(sizeof(float) * elems * p.splits) : 0;
+  const bool partials = p.splits > 1 && g.conv;
+  const size_t part_bytes = partials ? align_up(sizeof(float) * elems * p.splits) : 0;
   uint8_t* ws = nullptr;
   if (bf) {
     const __nv_bfloat16* si = bf16_staged(images, g.img_total);
@@ -1091,14 +1134,13 @@ static bool tc_conv_outp_impl(const ConvGeom& g, const float* images, const floa
     const int box[5] = {32, 8, g.ky, 1, 1};                   // 8 x-taps x ky rows of one channel: ky*8 GEMM columns
     if (!make_map(&mb, img, e, 5, dims, str, box)) return false;
   } else if (!image_map(&mb, img, e, g, g.W, g.H, g.Cin, g.in_frame_step, false, p.BN)) return false;
-  p.out = p.splits == 1 ? targets : (float*)ws;
+  p.out = partials ? (float*)ws : targets;
   launch<kWgrad>(ma, mb, p);
-  if (p.splits > 1) reduce_partials((const float*)ws, targets, elems, 1, p.splits, st, so);
+  if (partials) reduce_partials((const float*)ws, targets, elems, 1, p.splits, st, so);
   state().last_conv_path = bf ? kPathTcBf16 : kPathTcTf32;
   return true;
 }
 bool tc_conv_outp(const ConvGeom& g, const float* images, const float* derivs, float* targets, float st, float so) {
-  if (!g.conv) return false;
   if (want_bf16() && tc_conv_outp_impl(g, images, derivs, targets, st, so, true)) return true;
   return tc_conv_outp_impl(g, images, derivs, targets, st, so, false);
 }

@@ -280,6 +280,13 @@ ConvNet::ConvNet(const ModelConfig& model, int batch_size) : model_(model), batc
     edges_[i]->SetImageSize(layers_[i]->GetSizeY(), layers_[i]->GetSizeX(), layers_[i]->GetSizeT());
     layers_[i + 1]->SetSize(edges_[i]->GetNumModulesY(), edges_[i]->GetNumModulesX(), edges_[i]->GetNumModulesT());
   }
+  for (size_t i = 0; i < edges_.size(); i++) {       // the untied conv kernels are 2-D only
+    if (model.edge[i].edge_type != LOCAL || layers_[i]->GetSizeT() == 1) continue;
+    const std::string msg = "edge '" + edges_[i]->GetName() + "': LOCAL is not supported on 3-D layers (image_size_t > 1)";
+    for (Edge* e : edges_) delete e;
+    for (Layer* x : layers_) delete x;
+    throw std::invalid_argument(msg);
+  }
   for (Layer* l : layers_) {                          // what the batch-norm passes cannot run is refused here
     if (!l->BatchNormalize()) continue;
     std::string why;

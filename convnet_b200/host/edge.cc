@@ -27,6 +27,7 @@ Edge* Edge::ChooseEdgeClass(const EdgeConfig& c) {          // src/edge.cc:17-60
     case AVGPOOL: return new AvgPoolEdge(c);
     case RESPONSE_NORM: return new ResponseNormEdge(c);
     case CONV_ONETOONE: return new ConvOneToOneEdge(c);
+    case LOCAL: return new LocalEdge(c);
   }
   fprintf(stderr, "Error: Undefined edge type.\n");
   exit(1);
@@ -339,6 +340,75 @@ void ConvEdge::ComputeOuter(Matrix& input, Matrix& deriv_output) {   // :183-245
 double ConvEdge::FlopsUp() const {
   return 2.0 * batch_size_ * num_modules_y_ * num_modules_x_ * num_modules_t_ * conv_desc_.num_output_channels * FanIn();
 }
+
+// ---------------------------------------------------------------- LocalEdge (src/local_edge.cc)
+void LocalEdge::SetImageSize(int y, int x, int t) {          // :20-33
+  Edge::SetImageSize(y, x, t);
+  conv_desc_.num_input_channels = num_input_channels_;
+  conv_desc_.num_output_channels = num_output_channels_;
+  conv_desc_.input_channel_end = num_input_channels_;
+  conv_desc_.output_channel_end = num_output_channels_;
+  Edge::GetNumModules(conv_desc_, y, x, t, num_modules_y_, num_modules_x_, num_modules_t_);
+}
+size_t LocalEdge::GetParameterMemoryRequirement() {           // :53-57
+  return (size_t)num_output_channels_ * ((size_t)KernelSize() * Modules() + (has_no_bias_ ? 0 : Modules()));
+}
+void LocalEdge::SetMemory(Matrix& p) {                        // :59-72
+  const int cols = KernelSize() * Modules();
+  p.Reshape(num_output_channels_, -1);
+  p.GetSlice(weights_, 0, cols);
+  weights_.SetShape4D(num_output_channels_, conv_desc_.kernel_size_x, conv_desc_.kernel_size_y,
+                      conv_desc_.num_input_channels * Modules());
+  if (!has_no_bias_) {
+    p.GetSlice(bias_, cols, cols + Modules());
+    bias_.Reshape(1, -1);
+  }
+}
+void LocalEdge::SetGradMemory(Matrix& p) {                    // :74-101
+  const int cols = KernelSize() * Modules();
+  p.Reshape(num_output_channels_, -1);
+  p.GetSlice(grad_weights_, 0, cols);
+  grad_weights_.SetShape4D_like(weights_);
+  if (!has_no_bias_) {
+    p.GetSlice(grad_bias_, cols, cols + Modules());
+    grad_bias_.Reshape(1, -1);
+  }
+}
+void LocalEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) {   // :103-119
+  const bool fused = fuse_relu_ && CanFuseReLU();        // per-feature bias (+ReLU of the destination layer) in the epilogue
+  StageForUp(input);
+  const bool bias_pass = !has_no_bias_ && !fused;
+  if (emit_up_ && !bias_pass) convnet_b200_emit_bf16_next();
+  if (fused) convnet_b200_fuse_next(bias_.GetDevData(), 1, nullptr);
+  ApplyDropoutRequest(fused);
+  Matrix::LocalUp(input, weights_, output, conv_desc_, overwrite ? 0 : 1);
+  NoteUp();
+  if (bias_pass) {                                       // output.AddRowVec(bias_): bias[j] to column j
+    if (emit_up_) convnet_b200_emit_bf16_next();
+    output.AddRowVec(bias_);
+  }
+}
+void LocalEdge::ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input,
+                            bool overwrite) {                 // :121-126
+  StageForBprop(deriv_output);
+  if (fuse_mask_) convnet_b200_fuse_next(nullptr, 0, input.GetDevData());
+  if (emit_down_) convnet_b200_emit_bf16_next();
+  ApplyBiasGradRequest();
+  Matrix::LocalDown(deriv_output, weights_, deriv_input, conv_desc_, overwrite ? 0 : 1);
+  NoteDown();
+}
+void LocalEdge::ComputeOuter(Matrix& input, Matrix& deriv_output) {   // :128-139
+  const int batch_size = input.GetRows();
+  const int scale_targets = GetNumGradsReceived() > 0 ? 1 : 0;
+  const float scale = scale_gradients_ / batch_size;
+  StageForBprop(deriv_output);
+  Matrix::LocalOutp(input, deriv_output, grad_weights_, conv_desc_, scale_targets, scale);
+  NoteOuter();
+  bias_grad_fused_ = false;                              // (BiasIsPerChannel2D is false: never offered)
+  if (!has_no_bias_) SumBiasRows(deriv_output, scale_targets, scale);   // one sum per output feature
+  IncrementNumGradsReceived();
+}
+double LocalEdge::FlopsUp() const { return 2.0 * batch_size_ * Modules() * (double)num_output_channels_ * KernelSize(); }
 
 // ---------------------------------------------------------------- FCEdge (src/fc_edge.cc) as a 1x1 conv on a 1x1 image
 static ConvDesc one_by_one(int cin, int cout) {

@@ -7,6 +7,7 @@
 //   ResponseNormEdge    src/response_norm_edge.{h,cc}
 //   FCEdge              src/fc_edge.{h,cc}              (reference: Matrix::Dot / cublasSgemm)
 //   ConvOneToOneEdge    src/conv_onetoone_edge.{h,cc}   (reference: Matrix::Dot / cublasSgemm)
+//   LocalEdge           src/local_edge.{h,cc}           untied conv -> per-feature bias ; wgrad -> bias grad
 // FC and 1x1 edges run on the same implicit-GEMM conv kernels (a 1x1 convolution IS that GEMM),
 // SURVEY.md §8(f) rank 1.  The protobuf `config::Edge` is replaced by the plain EdgeConfig struct
 // (protobuf is not in the image); field names follow proto/convnet_config.proto:120-221.
@@ -20,7 +21,7 @@ namespace cnbhost {
 
 class Layer;
 
-enum EdgeType { FC, CONVOLUTIONAL, MAXPOOL, AVGPOOL, RESPONSE_NORM, CONV_ONETOONE };
+enum EdgeType { FC, CONVOLUTIONAL, MAXPOOL, AVGPOOL, RESPONSE_NORM, CONV_ONETOONE, LOCAL };
 
 // proto/convnet_config.proto:64-113 Optimizer, the fields of the SGD, Adagrad and RMSProp paths (src/optimizer.cc:174-279),
 // with the proto's names, numbers and defaults.  Plain C layout: the C API (capi.cc) and net.py's ctypes mirror pass it as is.
@@ -266,6 +267,33 @@ class ConvEdge : public EdgeWithWeight {
   ConvDesc conv_desc_;
   int partial_sum_y_, partial_sum_x_;
   bool shared_bias_;
+};
+
+// Locally connected ("untied") layer, src/local_edge.{h,cc}: a conv whose filter bank differs per output position.
+// Parameters [Cout x (K*modules + modules)]: the banks of all modules (Shape4D (Cout, kx, ky, Cin*modules)), then one
+// bias per output feature (column m + modules*o of the output).  2-D only (ConvNet refuses it on 3-D layers).
+class LocalEdge : public EdgeWithWeight {
+ public:
+  explicit LocalEdge(const EdgeConfig& c) : EdgeWithWeight(c), conv_desc_(Edge::GetConvDesc(c)) {}
+  void SetImageSize(int y, int x, int t) override;
+  size_t GetParameterMemoryRequirement() override;
+  void SetMemory(Matrix& p) override;
+  void SetGradMemory(Matrix& p) override;
+  void ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) override;
+  void ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) override;
+  void ComputeOuter(Matrix& input, Matrix& deriv_output) override;
+  double FlopsUp() const override;
+  // the reference's initialisation scale: weights_.GetCols() = K * modules (edge_with_weight.cc:126)
+  int FanIn() const override { return KernelSize() * Modules(); }
+  bool CanFuseReLU() const override { return !has_no_bias_; }                  // per-feature bias in the epilogue
+  bool CanFuseDropout() const override { return fuse_relu_ && CanFuseReLU(); }
+  bool CanFuseMask() const override { return true; }
+  bool BiasIsPerChannel2D() const override { return false; }
+
+ private:
+  int KernelSize() const { return conv_desc_.kernel_size_y * conv_desc_.kernel_size_x * conv_desc_.num_input_channels; }
+  int Modules() const { return num_modules_y_ * num_modules_x_; }
+  ConvDesc conv_desc_;
 };
 
 class FCEdge : public EdgeWithWeight {          // weights [Cout x K] column-major, like a conv filter bank

@@ -115,6 +115,19 @@ void Matrix::ConvOutp(Matrix& input, Matrix& deriv_output, Matrix& dw, ConvDesc 
   convOutpGemm(input.GetMat(), deriv_output.GetMat(), dw.GetMat(), &input.GetShape4D(), &deriv_output.GetShape4D(),
                &dw.GetShape4D(), conv_desc, scale_targets, scale_outputs);
 }
+void Matrix::LocalUp(Matrix& input, Matrix& w, Matrix& output, ConvDesc conv_desc, float scale_targets) {   // :859-870
+  localUpGemm(input.GetMat(), w.GetMat(), output.GetMat(), &input.GetShape4D(), &w.GetShape4D(), &output.GetShape4D(),
+              conv_desc, scale_targets);
+}
+void Matrix::LocalDown(Matrix& deriv_output, Matrix& w, Matrix& deriv_input, ConvDesc conv_desc, float scale_targets) {
+  localDownGemm(deriv_output.GetMat(), w.GetMat(), deriv_input.GetMat(), &deriv_output.GetShape4D(), &w.GetShape4D(),
+                &deriv_input.GetShape4D(), conv_desc, scale_targets);
+}
+void Matrix::LocalOutp(Matrix& input, Matrix& deriv_output, Matrix& dw, ConvDesc conv_desc, float scale_targets,
+                       float scale_outputs) {                                                                  // :883-893
+  localOutpGemm(input.GetMat(), deriv_output.GetMat(), dw.GetMat(), &input.GetShape4D(), &deriv_output.GetShape4D(),
+                &dw.GetShape4D(), conv_desc, scale_targets, scale_outputs);
+}
 void Matrix::Conv3DUp(Matrix& input, Matrix& w, Matrix& output, ConvDesc conv_desc, float scale_targets) {
   convUp3DGemm(input.GetMat(), w.GetMat(), output.GetMat(), &input.GetShape4D(), &w.GetShape4D(),
                &output.GetShape4D(), conv_desc, scale_targets);

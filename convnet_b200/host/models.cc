@@ -115,6 +115,59 @@ ModelConfig BuildGradCheckNet() {
   return m;
 }
 
+// conv + locally connected classifier (cuda-convnet's conv+local nets, scaled to 96 x 96 inputs): the two LOCAL edges
+// carry a filter bank per output position (42 and 29 MB in bf16) and sit near the HBM / tensor-core balance point at
+// batch 128.  init_wt = sqrt(modules): the reference scales a local edge's initial weights by 1/sqrt(K*modules/3)
+// (weights_.GetCols(), edge_with_weight.cc:126); this undoes the modules factor, giving a conv-like initial scale.
+ModelConfig BuildLcNet() {
+  ModelConfig m; m.name = "lcnet";
+  LayerConfig in = L("input", 3); in.is_input = true; in.image_size_y = in.image_size_x = 96;
+  m.layer = {in, L("conv1", 64, RECTIFIED_LINEAR), L("pool1", 64), L("conv2", 128, RECTIFIED_LINEAR), L("pool2", 128),
+             L("local3", 128, RECTIFIED_LINEAR), L("local4", 128, RECTIFIED_LINEAR), L("fc5", 1024, RECTIFIED_LINEAR, 0.5f),
+             L("output", 1000, SOFTMAX)};
+  m.layer.back().is_output = true;
+  EdgeConfig l3 = E(LOCAL, 3, 1, 1), l4 = E(LOCAL, 3, 1, 0);
+  l3.init_wt = 12.f;                                        // sqrt(12 x 12 modules)
+  l4.init_wt = 10.f;                                        // sqrt(10 x 10 modules)
+  m.edge = {Conv(5, 2, 2), Pool(3, 2, 1), Conv(3, 1, 1), Pool(3, 2, 1), l3, l4, E(FC), E(FC)};
+  finish(m);
+  return m;
+}
+
+// run_grad_check net for the LOCAL edge, smooth like BuildGradCheckNet (linear units, average pooling): one local edge
+// with padding, one with stride 2 and no padding, then an FC.  init_wt = sqrt(modules) as in lcnet: with the reference's
+// 1/sqrt(K*modules/3) scale the derivative reaching local1 is so small that its per-feature bias gradients sit at the
+// float32 noise floor of the finite differences.  The check reads the FIRST parameters of a tensor, which for a local edge
+// are the taps of module 0 (the top-left corner).  With padding 1, 5 of local1's 9 taps there only ever read padding, so
+// local1 checks 72 parameters: all 8 outputs x 9 taps of input channel 0 of module 0, 32 of them live (the pairs whose
+// analytic and numeric gradients are both exactly 0 do not enter the mean).
+ModelConfig BuildLocalCheckNet() {
+  ModelConfig m; m.name = "localcheck";
+  LayerConfig in = L("input", 4); in.is_input = true; in.image_size_y = in.image_size_x = 8;
+  m.layer = {in, L("local1", 8), L("pool1", 8), L("local2", 8), L("output", 5, SOFTMAX)};
+  m.layer.back().is_output = true;
+  EdgeConfig l1 = E(LOCAL, 3, 1, 1), l2 = E(LOCAL, 3, 2, 0);
+  l1.init_wt = 8.f;                                         // sqrt(8 x 8 modules)
+  l2.init_wt = 3.f;                                         // sqrt(3 x 3 modules)
+  m.edge = {l1, E(AVGPOOL, 2, 1, 0), l2, E(FC)};
+  for (EdgeConfig& e : m.edge) { e.grad_check = true; e.grad_check_num_params = 10; e.grad_check_epsilon = {1e-2f, 3e-3f, 1e-3f}; }
+  m.edge[0].grad_check_num_params = 8 * 9;
+  finish(m);
+  return m;
+}
+
+// NOT a model: a deliberately invalid config (a 3-D clip net with a LOCAL edge) that the tests of the host's refusals
+// build by the name "invalid:local3d" — ConvNet refuses it, the untied kernels being 2-D
+ModelConfig BuildLocal3DNet() {
+  ModelConfig m; m.name = "invalid:local3d";
+  LayerConfig in = L("input", 3); in.is_input = true; in.image_size_y = in.image_size_x = 16; in.image_size_t = 4;
+  m.layer = {in, L("conv1", 16, RECTIFIED_LINEAR), L("local2", 16, RECTIFIED_LINEAR), L("output", 10, SOFTMAX)};
+  m.layer.back().is_output = true;
+  m.edge = {Conv(3, 2, 1), E(LOCAL, 3, 1, 1), E(FC)};
+  finish(m);
+  return m;
+}
+
 // "<model>+ref-optimizer": the optimizer blocks of the model's pbtxt exactly (BuildAlexNet / BuildLeNet keep the constant
 // momentum and leave out the norm rules and the FC l2_decay)
 static void UseReferenceOptimizers(const std::string& base, ModelConfig& m) {
@@ -149,7 +202,8 @@ static void UseBatchNorm(const std::string& name, ModelConfig& m) {
   for (size_t i = 0; i < m.edge.size(); i++) {
     const EdgeConfig& e = m.edge[i];
     LayerConfig& l = m.layer[i + 1];
-    if (l.is_output || (e.edge_type != CONVOLUTIONAL && e.edge_type != CONV_ONETOONE && e.edge_type != FC)) continue;
+    if (l.is_output || (e.edge_type != CONVOLUTIONAL && e.edge_type != CONV_ONETOONE && e.edge_type != FC && e.edge_type != LOCAL))
+      continue;
     if (l.batch_normalize) throw std::invalid_argument("model '" + name + "': +bn is given twice");
     l.batch_normalize = true;
     l.gamma_optimizer = e.weight_optimizer;
@@ -218,6 +272,9 @@ ModelConfig BuildModel(const std::string& name) {
   if (name == "lenet") return BuildLeNet();
   if (name == "c3d") return BuildC3D();
   if (name == "tiny") return BuildTinyNet();
+  if (name == "lcnet") return BuildLcNet();
+  if (name == "localcheck") return BuildLocalCheckNet();
+  if (name == "invalid:local3d") return BuildLocal3DNet();     // test-only, refused by ConvNet (see above)
   throw std::invalid_argument("unknown model '" + name + "'");
 }
 

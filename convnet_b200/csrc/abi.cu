@@ -72,7 +72,8 @@ void conv_down(const ConvGeom& g, const float* derivs, const float* filters, flo
   // the mask can ride in the epilogue only when one launch produces the final value of every target element
   const bool whole = g.conv && g.frames == 1 && g.cin0 == 0 && g.Cin == g.CinT;
   const float* late_mask = nullptr;
-  if (fuse.relu_mask && !whole) { late_mask = fuse.relu_mask; fuse.relu_mask = nullptr; }
+  const int late_act = fuse.state_act;
+  if (fuse.act_state && !whole) { late_mask = fuse.act_state; fuse.act_state = nullptr; fuse.state_act = kActNone; }
   Emit emit(targets, g.img_total, fuse.emit_bf16 != 0);
   if (!late_mask) emit.attach(fuse);               // a late mask changes the values after the kernel: convert afterwards
   if (!(state().precision != kPrecFP32 && tc_conv_down(g, derivs, filters, targets, st, so, fuse))) {
@@ -80,8 +81,9 @@ void conv_down(const ConvGeom& g, const float* derivs, const float* filters, flo
     state().last_conv_path = kPathSimt;
   }
   if (late_mask) {
-    const long long n4 = g.img_total;             // (cnb_relu_deriv would consume a pending fuse request; none is pending here)
-    cnb_relu_deriv(targets, late_mask, n4);
+    const long long n4 = g.img_total;             // (these passes would consume a pending fuse request; none is pending here)
+    if (late_act == kActLogistic) cnb_logistic_deriv(targets, late_mask, n4);
+    else cnb_relu_deriv(targets, late_mask, n4);
   }
   CNB_REQUIRE(!fuse.bias_grad || g.frames == 1, "convDown: fused bias gradient is 2-D only");
   finish_bias_grad(fuse, nullptr, 0, targets, (long long)g.N * g.W * g.H, g.CinT);
@@ -148,11 +150,14 @@ void do_max_undo(const char* what, cudamat* images, cudamat* maxGrads, cudamat* 
   CNB_REQUIRE(targets->size[0] == g.N && targets->size[1] == images->size[1], what);
   CNB_REQUIRE(maxActs->size[0] == g.N && maxActs->size[1] == maxGrads->size[1], what);
   const Fuse fuse = take_fuse();
-  Emit emit(targets->data_device, (long long)targets->size[0] * targets->size[1], fuse.emit_bf16 != 0);
+  const long long n = (long long)targets->size[0] * targets->size[1];
+  Emit emit(targets->data_device, n, fuse.emit_bf16 != 0);
+  const bool late = fuse.state_act == kActLogistic;   // the undo kernels fuse ReLU' only: sigma' is a pass after them
   int slices = 0;
   float* part = fuse.bias_grad ? (float*)workspace(sizeof(float) * (size_t)(g.H + 2) * g.C * g.T) : nullptr;
   emit.done = max_pool_undo(g, images->data_device, maxGrads->data_device, maxActs->data_device, targets->data_device, st,
-                            1.f, fuse.relu_mask, emit.buf, g.T == 1 ? part : nullptr, &slices);
+                            1.f, fuse.relu_mask(), late ? nullptr : emit.buf, g.T == 1 && !late ? part : nullptr, &slices);
+  if (late) cnb_logistic_deriv(targets->data_device, fuse.act_state, n);
   finish_bias_grad(fuse, part, slices, targets->data_device, (long long)g.N * g.W * g.H * g.T, g.C);
   emit.finish();
 }
@@ -161,11 +166,14 @@ void do_avg_undo(const char* what, cudamat* avgGrads, cudamat* targets, Shape4D*
   Range nvtx_range(what);
   PoolGeom g = pool_geom(*ts, *gs, targets, avgGrads, d, what);
   const Fuse fuse = take_fuse();
-  Emit emit(targets->data_device, (long long)targets->size[0] * targets->size[1], fuse.emit_bf16 != 0);
+  const long long n = (long long)targets->size[0] * targets->size[1];
+  Emit emit(targets->data_device, n, fuse.emit_bf16 != 0);
+  const bool late = fuse.state_act == kActLogistic;
   int slices = 0;
   float* part = fuse.bias_grad ? (float*)workspace(sizeof(float) * (size_t)(g.H + 2) * g.C * g.T) : nullptr;
-  emit.done = avg_pool_undo(g, avgGrads->data_device, targets->data_device, st, so, fuse.relu_mask, emit.buf,
-                            g.T == 1 ? part : nullptr, &slices);
+  emit.done = avg_pool_undo(g, avgGrads->data_device, targets->data_device, st, so, fuse.relu_mask(), late ? nullptr : emit.buf,
+                            g.T == 1 && !late ? part : nullptr, &slices);
+  if (late) cnb_logistic_deriv(targets->data_device, fuse.act_state, n);
   finish_bias_grad(fuse, part, slices, targets->data_device, (long long)g.N * g.W * g.H * g.T, g.C);
   emit.finish();
 }
@@ -191,14 +199,16 @@ void do_rnorm(const char* what, cudamat* images, cudamat* targets, int F, int si
   CNB_REQUIRE(targets->size[0] == images->size[0] && targets->size[1] == images->size[1], what);
   const long long L = els / F / frames;          // locations per frame
   // fused epilogue (convnet_b200_fuse_next relu / convnet_b200_emit_bf16_next): in the tile kernel when it applies, else
-  // as trailing passes
+  // as trailing passes; the logistic activation is always a trailing pass
   const Fuse fuse = take_fuse();
-  const bool fusable = rnorm_can_fuse(F);
+  const bool fusable = rnorm_can_fuse(F) && fuse.act != kActLogistic;
+  const bool relu = fuse.act == kActRelu;
   Emit emit(targets->data_device, els, fuse.emit_bf16 != 0);
   for (int t = 0; t < frames; t++)               // conv3d_gemm.cu:167-189: independent per frame
     rnorm_forward(images->data_device + (long long)t * L * F, targets->data_device + (long long)t * L * F, L, F, sizeF,
-                  a, b, blocked, fusable && fuse.relu, fusable && emit.buf ? emit.buf + (long long)t * L * F : nullptr);
-  if (fuse.relu && !fusable) cnb_relu(targets->data_device, els);
+                  a, b, blocked, fusable && relu, fusable && emit.buf ? emit.buf + (long long)t * L * F : nullptr);
+  if (relu && !fusable) cnb_relu(targets->data_device, els);
+  if (fuse.act == kActLogistic) cnb_logistic(targets->data_device, els);
   emit.done = fusable;
   emit.finish();
 }

@@ -80,11 +80,27 @@ inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
 enum Precision { kPrecFP32 = 0, kPrecTF32 = 1, kPrecBF16 = 2 };
 enum ConvPath { kPathNone = -1, kPathSimt = 0, kPathTcTf32 = 1, kPathTcBf16 = 2 };
 
-// one-shot epilogue fusion requested for the next conv / pool-undo call (convnet_b200_fuse_next)
+// ---- activations of a layer, as the fused epilogues and the stand-alone passes apply them (convnet_b200_fuse_next_act)
+enum Act { kActNone = 0, kActRelu = 1, kActLogistic = 2 };
+// the logistic unit: 1 / (1 + expf(-x)), each operation rounded to nearest (expf: <= 2 ulp, CUDA Programming Guide);
+// |result - sigma(x)| <= 3 * 2^-23 * sigma(x) + 2^-126 (DESIGN.md §5)
+__device__ __forceinline__ float logistic_f(float x) { return __fdiv_rn(1.f, __fadd_rn(1.f, expf(-x))); }
+// its derivative applied to d, from the stored state s = sigma(x):  (d * s) * (1 - s), three roundings
+__device__ __forceinline__ float logistic_deriv_f(float d, float s) { return __fmul_rn(__fmul_rn(d, s), __fsub_rn(1.f, s)); }
+__device__ __forceinline__ float act_apply(float x, int act) {
+  return act == kActRelu ? fmaxf(x, 0.f) : (act == kActLogistic ? logistic_f(x) : x);
+}
+// d times the activation's derivative at the state s: ReLU' zeroes d where s <= 0 (and where s is NaN)
+__device__ __forceinline__ float act_deriv(float d, float s, int act) {
+  return act == kActRelu ? (s > 0.f ? d : 0.f) : (act == kActLogistic ? logistic_deriv_f(d, s) : d);
+}
+
+// one-shot epilogue fusion requested for the next conv / pool-undo call (convnet_b200_fuse_next_act)
 struct Fuse {
   const float* bias = nullptr;       // fprop: + bias[output channel]
-  int relu = 0;                      // fprop: max(., 0) after the bias
-  const float* relu_mask = nullptr;  // dgrad / pool undo: result zeroed where relu_mask <= 0 (same shape as the target)
+  int act = 0;                       // fprop: Act applied after the bias
+  const float* act_state = nullptr;  // dgrad / pool undo: result times state_act'(act_state) (same shape as the target)
+  int state_act = 0;                 // the Act whose derivative act_state selects (0: none)
   // fprop: dropout after bias / ReLU (convnet_b200_fuse_next_dropout): element i (its index in the target tensor) is kept
   // iff dropout_uniform(seed + i) >= drop_prob, kept values are multiplied by drop_scale; drop_scale == 0: no dropout
   float drop_prob = 0.f, drop_scale = 0.f; unsigned long long drop_seed = 0;
@@ -99,7 +115,9 @@ struct Fuse {
   // internal (filled by the ABI wrapper): where the bf16 twin of the target goes; a kernel that writes it sets *emitted
   __nv_bfloat16* out16 = nullptr;
   bool* emitted = nullptr;
-  bool any() const { return bias || relu || relu_mask || drop_scale != 0.f; }
+  bool any() const { return bias || act || act_state || drop_scale != 0.f; }
+  // the ReLU' mask, for the kernels that fuse only that derivative (pool undo); nullptr otherwise
+  const float* relu_mask() const { return state_act == kActRelu ? act_state : nullptr; }
 };
 
 struct State {

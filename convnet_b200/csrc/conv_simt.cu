@@ -27,7 +27,7 @@ struct FpropProblem {
   long long flt_z, img_z, out_z;  // per-blockIdx.z strides (untied module / 3-D frame)
   int z_is_module;              // untied: z = module and M = N
   float st, so;
-  const float* bias; int relu;  // fused epilogue (convnet_b200_fuse_next); untied: one bias per output feature
+  const float* bias; int act;   // fused epilogue (convnet_b200_fuse_next_act); untied: one bias per output feature
   __device__ __forceinline__ long long rows() const { return M; }
   __device__ __forceinline__ int cols() const { return Cout; }
   __device__ __forceinline__ int depth() const { return K; }
@@ -50,7 +50,7 @@ struct FpropProblem {
     float* t = out + (z_is_module ? (long long)z * N : z * out_z) + m + (long long)N * modules * o;
     float r = (st == 0.f) ? so * acc : st * (*t) + so * acc;
     if (bias) r += __ldg(bias + (z_is_module ? z + (long long)modules * o : o));
-    if (relu) r = fmaxf(r, 0.f);
+    if (act) r = act_apply(r, act);
     *t = r;
   }
 };
@@ -63,7 +63,7 @@ struct DgradProblem {
   long long der_z, out_z;       // 3-D frame strides (sequential launches use z = 0)
   int untied;
   float st, so;
-  const float* mask;            // fused ReLU derivative: same layout as out
+  const float* mask; int mask_act;   // fused activation derivative act_deriv(., mask, mask_act): same layout as out
   __device__ __forceinline__ long long rows() const { return M; }
   __device__ __forceinline__ int cols() const { return Cin; }
   __device__ __forceinline__ int depth() const { return K; }
@@ -92,7 +92,7 @@ struct DgradProblem {
   __device__ __forceinline__ void store(long long m, int c, float acc, int z) const {
     float* t = out + z * out_z + m + M * c;
     float r = (st == 0.f) ? so * acc : st * (*t) + so * acc;
-    if (mask && !(__ldg(mask + z * out_z + m + M * c) > 0.f)) r = 0.f;
+    if (mask) r = act_deriv(r, __ldg(mask + z * out_z + m + M * c), mask_act);
     *t = r;
   }
 };
@@ -313,7 +313,7 @@ void reduce_partials(const float* part, float* out, long long elems, int groups,
 void simt_conv_up(const ConvGeom& g, const float* images, const float* filters, float* targets,
                   float scaleTargets, float scaleOutput, const Fuse& fuse) {
   FpropProblem p;
-  p.bias = fuse.bias ? fuse.bias + (long long)g.cout0 * (g.conv ? 1 : g.modules) : nullptr; p.relu = fuse.relu;
+  p.bias = fuse.bias ? fuse.bias + (long long)g.cout0 * (g.conv ? 1 : g.modules) : nullptr; p.act = fuse.act;
   p.img = images + (long long)g.cin0 * g.H * g.W * g.N;
   p.flt = filters;
   p.out = targets + (long long)g.cout0 * g.modules * g.N;
@@ -350,7 +350,7 @@ void simt_conv_down(const ConvGeom& g, const float* derivs, const float* filters
                     float scaleTargets, float scaleOutput, const Fuse& fuse) {
   if (!g.conv) { simt_local_down(g, derivs, filters, targets, scaleTargets, scaleOutput); return; }
   DgradProblem p;
-  p.mask = nullptr;
+  p.mask = nullptr; p.mask_act = 0;
   p.der = derivs + (long long)g.cout0 * g.modules * g.N;
   p.flt = filters;
   p.out = targets + (long long)g.cin0 * g.H * g.W * g.N;
@@ -362,7 +362,7 @@ void simt_conv_down(const ConvGeom& g, const float* derivs, const float* filters
   // The reference scales the WHOLE target (all channels, all frames) first (gemm.cu:760, conv3d:98).
   if (g.frames == 1 && g.cin0 == 0 && g.Cin == g.CinT) {
     p.st = scaleTargets;
-    p.mask = fuse.relu_mask;
+    p.mask = fuse.act_state; p.mask_act = fuse.state_act;
     launch(p, p.M, g.Cin, 1);
     return;
   }

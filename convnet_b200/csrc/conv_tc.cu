@@ -75,8 +75,8 @@ struct TcParams {
   float* out;
   __nv_bfloat16* out16;             // optional bf16 twin of `out` (same indexing): convnet_b200_emit_bf16_next
   float st, so;
-  const float* bias; int relu;      // fused fprop epilogue: + bias[o], then max(., 0)
-  const float* mask;                // fused epilogue: zero where mask <= 0 (same layout as out)
+  const float* bias; int act;       // fused fprop epilogue: + bias[o], then act_apply(., act)
+  const float* mask; int mask_act;  // fused epilogue: act_deriv(., mask, mask_act) (mask: same layout as out)
   // fprop: dropout of the (bias + ReLU'd) result, element index = offset from `out` (Fuse::drop_*); drop_scale 0 = none
   float drop_prob, drop_scale;
   unsigned long long drop_seed;
@@ -224,7 +224,9 @@ __device__ __forceinline__ uint32_t off_mnmajor(int row, int k) {
 }
 
 // ------------------------------------------------------------------------------------------------
-template <int OP, bool BF16>
+// SIG: the epilogue applies the activation code (logistic included); the other instances know only ReLU / ReLU', so the
+// logistic arithmetic costs the ReLU and linear layers nothing
+template <int OP, bool BF16, bool SIG>
 __global__ void __launch_bounds__(kThreads, 1)
 tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const __grid_constant__ TcParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -565,10 +567,12 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
           if (rmw) r += p.st * (*dst);
           if (OP == kFprop) {
             if (bias) r += __ldg(bias + col * bias_step);
-            if (p.relu) r = fmaxf(r, 0.f);
+            if (SIG) { if (p.act) r = act_apply(r, p.act); }
+            else if (p.act) r = fmaxf(r, 0.f);
             if (p.drop_scale != 0.f) r *= dropout_keep(p.drop_seed + (unsigned long long)(dst - p.out), p.drop_prob, p.drop_scale);
           }
-          if (p.mask && !(__ldg(p.mask + (dst - p.out)) > 0.f)) r = 0.f;
+          if (SIG) { if (p.mask) r = act_deriv(r, __ldg(p.mask + (dst - p.out)), p.mask_act); }
+          else if (p.mask && !(__ldg(p.mask + (dst - p.out)) > 0.f)) r = 0.f;
           *dst = r;
           if (p.out16) p.out16[dst - p.out] = __float2bfloat16_rn(r);
         }
@@ -640,25 +644,36 @@ int pick_stages() {
   return s;
 }
 
-template <int OP, bool BF16>
+template <int OP, bool BF16, bool SIG>
 void launch_one(const CUtensorMap& a, const CUtensorMap& b, const TcParams& p, size_t smem) {
   // the attribute belongs to the (function, device) pair: set it once per device this process launches on
   static unsigned long long attr_devices = 0;
   const int dev = current_device();
   if (dev >= 64 || !((attr_devices >> dev) & 1ULL)) {
-    CNB_CUDA_CHECK(cudaFuncSetAttribute(tc_conv_kernel<OP, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    CNB_CUDA_CHECK(cudaFuncSetAttribute(tc_conv_kernel<OP, BF16, SIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     if (dev < 64) attr_devices |= 1ULL << dev;
   }
   const int grid = std::min(p.num_tiles, num_sms());
-  launch_pdl(tc_conv_kernel<OP, BF16>, dim3((unsigned)grid), dim3(kThreads), smem, state().stream, a, b, p);
+  launch_pdl(tc_conv_kernel<OP, BF16, SIG>, dim3((unsigned)grid), dim3(kThreads), smem, state().stream, a, b, p);
 }
 
 template <int OP>
 void launch(const CUtensorMap& a, const CUtensorMap& b, TcParams& p) {
   p.stages = pick_stages();
   const size_t smem = smem_bytes_for(p.stages);
-  if (p.bf16) launch_one<OP, true>(a, b, p, smem);
-  else launch_one<OP, false>(a, b, p, smem);
+  const bool sig = p.act == kActLogistic || (p.mask && p.mask_act == kActLogistic);
+  if constexpr (OP != kWgrad) {                       // (a wgrad has no activation to apply)
+    if (sig) {
+      if (p.bf16) launch_one<OP, true, true>(a, b, p, smem);
+      else launch_one<OP, false, true>(a, b, p, smem);
+      count_launch();
+      CNB_LAUNCH_CHECK("tc_conv");
+      return;
+    }
+  }
+  CNB_REQUIRE(!sig, "tc_conv: wgrad has no activation epilogue");
+  if (p.bf16) launch_one<OP, true, false>(a, b, p, smem);
+  else launch_one<OP, false, false>(a, b, p, smem);
   count_launch();
   CNB_LAUNCH_CHECK("tc_conv");
 }
@@ -674,7 +689,7 @@ void fill_common(TcParams& p, const ConvGeom& g, const Elem& e) {
   p.x_mode = 0; p.x_yblocks = 0; p.x_ct = 0; p.b_tx_bytes = 0;
   p.a_merged = 0; p.b_merged = 0;
   p.untied = g.conv ? 0 : 1;
-  p.bias = nullptr; p.relu = 0; p.mask = nullptr; p.out16 = nullptr;
+  p.bias = nullptr; p.act = 0; p.mask = nullptr; p.mask_act = 0; p.out16 = nullptr;
   p.drop_prob = 0.f; p.drop_scale = 0.f; p.drop_seed = 0;
   p.o_sx = p.o_sy = 1; p.o_x0 = p.o_y0 = 0; p.o_W = g.modX; p.out_plane = g.modules;
   p.out_frame_step = g.out_frame_step;
@@ -737,11 +752,11 @@ inline long long filter_elems(const ConvGeom& g) { return (long long)g.Cout * g.
 inline size_t align_up(size_t v) { return (v + 1023) & ~size_t(1023); }
 
 // ---- split-K for 1x1 / FC shapes: too few output tiles to fill the GPU, long K ------------------------
-// out = st*out + so * sum_s part[s]  (+ bias[channel], ReLU | zero where mask <= 0): the fused epilogue moves here
+// out = st*out + so * sum_s part[s]  (+ bias[channel], act | times mask_act'(mask)): the fused epilogue moves here
 __global__ void __launch_bounds__(256) reduce_split_kernel(const float4* __restrict__ part, float4* out, long long elems4,
                                                            long long stride4, int splits, float st, float so,
-                                                           const float* __restrict__ bias, long long per_channel4, int relu,
-                                                           const float4* __restrict__ mask) {
+                                                           const float* __restrict__ bias, long long per_channel4, int act,
+                                                           const float4* __restrict__ mask, int mask_act) {
   pdl_wait();
   pdl_trigger();
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < elems4; i += (long long)gridDim.x * blockDim.x) {
@@ -753,23 +768,21 @@ __global__ void __launch_bounds__(256) reduce_split_kernel(const float4* __restr
     s.x *= so; s.y *= so; s.z *= so; s.w *= so;
     if (st != 0.f) { const float4 o = out[i]; s.x += st * o.x; s.y += st * o.y; s.z += st * o.z; s.w += st * o.w; }
     if (bias) { const float b = __ldg(bias + i / per_channel4); s.x += b; s.y += b; s.z += b; s.w += b; }
-    if (relu) { s.x = fmaxf(s.x, 0.f); s.y = fmaxf(s.y, 0.f); s.z = fmaxf(s.z, 0.f); s.w = fmaxf(s.w, 0.f); }
+    if (act) { s.x = act_apply(s.x, act); s.y = act_apply(s.y, act); s.z = act_apply(s.z, act); s.w = act_apply(s.w, act); }
     if (mask) {
       const float4 m = mask[i];
-      if (!(m.x > 0.f)) s.x = 0.f;
-      if (!(m.y > 0.f)) s.y = 0.f;
-      if (!(m.z > 0.f)) s.z = 0.f;
-      if (!(m.w > 0.f)) s.w = 0.f;
+      s.x = act_deriv(s.x, m.x, mask_act); s.y = act_deriv(s.y, m.y, mask_act);
+      s.z = act_deriv(s.z, m.z, mask_act); s.w = act_deriv(s.w, m.w, mask_act);
     }
     out[i] = s;
   }
 }
 void reduce_split(const float* part, float* out, long long elems, int splits, float st, float so, const float* bias,
-                  long long per_channel, int relu, const float* mask) {
+                  long long per_channel, int act, const float* mask, int mask_act) {
   const long long e4 = elems / 4;
   const int grid = (int)std::min<long long>(std::max<long long>(ceil_div<long long>(e4, 256), 1), 8LL * num_sms());
   launch_pdl(reduce_split_kernel, dim3((unsigned)grid), dim3(256), 0, state().stream, (const float4*)part, (float4*)out, e4, e4, splits,
-             st, so, bias, per_channel / 4, relu, (const float4*)mask);
+             st, so, bias, per_channel / 4, act, (const float4*)mask, mask_act);
   count_launch();
   CNB_LAUNCH_CHECK("reduce_split");
 }
@@ -827,7 +840,7 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
   const size_t part_bytes = p.splits > 1 ? align_up(sizeof(float) * out_elems * p.splits) : 0;
   p.out = out;
   p.st = st; p.so = so;
-  p.bias = bias; p.relu = fuse.relu;
+  p.bias = bias; p.act = fuse.act;
   CUtensorMap ma, mb;
   const long long img_off = (long long)g.cin0 * g.H * g.W * g.N;
   const void* img = images + img_off;
@@ -846,7 +859,7 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
   } else if (part_bytes) {
     ws = (uint8_t*)workspace(part_bytes);
   }
-  if (p.splits > 1) { p.out = (float*)ws; p.bias = nullptr; p.relu = 0; }   // partial sums; the epilogue moves to reduce_split
+  if (p.splits > 1) { p.out = (float*)ws; p.bias = nullptr; p.act = 0; }    // partial sums; the epilogue moves to reduce_split
   // bf16 twin of the output from the same registers: only when this launch writes the final value of EVERY element
   const bool emit = fuse.out16 != nullptr && p.splits == 1 && g.cout0 == 0 && g.Cout == g.CoutT;
   if (emit) p.out16 = fuse.out16;
@@ -886,7 +899,8 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
   launch<kFprop>(ma, mb, p);
   if (emit && fuse.emitted) *fuse.emitted = true;
   if (drop && fuse.dropped) *fuse.dropped = true;
-  if (p.splits > 1) reduce_split((const float*)ws, out, out_elems, p.splits, st, so, bias, (long long)g.modules * g.N, fuse.relu, nullptr);
+  if (p.splits > 1)
+    reduce_split((const float*)ws, out, out_elems, p.splits, st, so, bias, (long long)g.modules * g.N, fuse.act, nullptr, 0);
   state().last_conv_path = bf ? kPathTcBf16 : kPathTcTf32;
   return true;
 }
@@ -948,7 +962,7 @@ static bool tc_conv_down_as_fprop(const ConvGeom& g, const float* derivs, const 
     p.num_tiles = p.m_tiles * p.n_tiles;
     p.b_tx_bytes = (uint32_t)p.BN * 128;
     p.out = targets; p.st = 0.f; p.so = so;
-    p.mask = fuse.relu_mask; p.out16 = fuse.out16;
+    p.mask = fuse.act_state; p.mask_act = fuse.state_act; p.out16 = fuse.out16;
     p.o_sx = g.sx; p.o_sy = g.sy; p.o_x0 = P.a; p.o_y0 = P.b; p.o_W = g.W; p.out_plane = (long long)g.W * g.H;
     p.a_merged = 1;
     p.b_merged = (g.Cin % 64 == 0) ? 1 : 0;
@@ -1026,9 +1040,10 @@ static bool tc_conv_down_impl(const ConvGeom& g, const float* derivs, const floa
   if (whole && p.splits > 1) {
     p.st = 0.f; p.out = (float*)ws; p.mask = nullptr;
     launch<kDgrad>(ma, mb, p);
-    reduce_split((const float*)ws, out, out_elems, p.splits, st, so, nullptr, 1, 0, fuse.relu_mask);
+    reduce_split((const float*)ws, out, out_elems, p.splits, st, so, nullptr, 1, 0, fuse.act_state, fuse.state_act);
   } else if (whole) {
-    p.st = st; p.out = out; p.mask = fuse.relu_mask ? fuse.relu_mask + (long long)g.cin0 * g.H * g.W * g.N : nullptr;
+    p.st = st; p.out = out; p.mask = fuse.act_state ? fuse.act_state + (long long)g.cin0 * g.H * g.W * g.N : nullptr;
+    p.mask_act = fuse.state_act;
     p.out16 = fuse.out16;                              // `whole`: every element gets its final value here
     launch<kDgrad>(ma, mb, p);
     if (fuse.out16 && fuse.emitted) *fuse.emitted = true;

@@ -170,6 +170,112 @@ __global__ void relu_deriv_kernel(float* dx, const float* __restrict__ y, long l
   }
   for (long long i = 4 * n4 + tid; i < n; i += nt) dx[i] = y[i] > 0.f ? dx[i] : 0.f;
 }
+// the logistic unit and its derivative (LogisticLayer, src/layer.cc:586-602), laid out like relu_kernel / relu_deriv_kernel
+__global__ void logistic_kernel(float* x, long long n, long long n4, __nv_bfloat16* out16) {
+  const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
+  for (long long i = tid; i < n4; i += nt) {
+    float4 v = reinterpret_cast<float4*>(x)[i];
+    v.x = logistic_f(v.x); v.y = logistic_f(v.y); v.z = logistic_f(v.z); v.w = logistic_f(v.w);
+    reinterpret_cast<float4*>(x)[i] = v;
+    emit4(out16, i, v);
+  }
+  for (long long i = 4 * n4 + tid; i < n; i += nt) { const float v = logistic_f(x[i]); x[i] = v; if (out16) out16[i] = __float2bfloat16_rn(v); }
+}
+__global__ void logistic_deriv_kernel(float* dx, const float* __restrict__ y, long long n, long long n4, __nv_bfloat16* out16) {
+  const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
+  for (long long i = tid; i < n4; i += nt) {
+    float4 d = reinterpret_cast<float4*>(dx)[i];
+    const float4 s = __ldg(reinterpret_cast<const float4*>(y) + i);
+    d.x = logistic_deriv_f(d.x, s.x); d.y = logistic_deriv_f(d.y, s.y); d.z = logistic_deriv_f(d.z, s.z); d.w = logistic_deriv_f(d.w, s.w);
+    reinterpret_cast<float4*>(dx)[i] = d;
+    emit4(out16, i, d);
+  }
+  for (long long i = 4 * n4 + tid; i < n; i += nt) {
+    const float v = logistic_deriv_f(dx[i], y[i]);
+    dx[i] = v;
+    if (out16) out16[i] = __float2bfloat16_rn(v);
+  }
+}
+
+// ---- output layers (src/loss_functions.cc).  y, t, deriv: column-major [rows = images x cols], images fastest.  One
+// thread per image walks its columns in order, so each per-image value is a fixed-order float sum; ConvNet adds the images
+// up with sum_kernel.  Per column, with w = loss_function_weight (deriv may be NULL: the value alone, the performance
+// metric of a loss):
+//   SQUARED_ERROR                          deriv (y - t) * w          value 0.5 * sum (y - t)^2        (:39-53)
+//   LINEAR_ERROR                           deriv w                    value sum (y - t)                (:55-68)
+//   CROSS_ENTROPY_MULTINOMIAL (labels)     deriv (y - [c == l]) * w   value -log max(y[l], 1e-30)      (:70-83)
+//   CROSS_ENTROPY_BINARY (t < 0: ignored)  deriv (y - t) * w, 0       value sum -t log(y + 1e-10) - (1 - t) log(1 - y + 1e-10)
+//   CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED  deriv (y - t) * w          value sum -t log(y + 1e-10)      (:97-109)
+// Every operation is rounded to nearest (logf: <= 1 ulp); sums accumulate left to right over the columns.
+constexpr float kTiny = 1e-10f;
+__global__ void loss_kernel(int loss, const float* __restrict__ y, const float* __restrict__ t, const int* __restrict__ labels,
+                            float* deriv, float* value, int rows, int cols, float w) {
+  const int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= rows) return;
+  const int lab = loss == CNB_LOSS_CROSS_ENTROPY_MULTINOMIAL ? labels[n] : -1;
+  float s = 0.f;
+  for (int c = 0; c < cols; c++) {
+    const long long i = n + (long long)rows * c;
+    const float yv = __ldg(y + i);
+    const float tv = loss == CNB_LOSS_CROSS_ENTROPY_MULTINOMIAL ? (c == lab ? 1.f : 0.f) : __ldg(t + i);
+    const float d = __fsub_rn(yv, tv);
+    float g = d;
+    switch (loss) {
+      case CNB_LOSS_SQUARED_ERROR: s = __fmaf_rn(d, d, s); break;
+      case CNB_LOSS_LINEAR_ERROR: s = __fadd_rn(s, d); g = 1.f; break;
+      case CNB_LOSS_CROSS_ENTROPY_BINARY:
+        if (tv < 0.f) { g = 0.f; break; }
+        s = __fsub_rn(__fsub_rn(s, __fmul_rn(tv, logf(__fadd_rn(yv, kTiny)))),
+                      __fmul_rn(__fsub_rn(1.f, tv), logf(__fadd_rn(__fsub_rn(1.f, yv), kTiny))));
+        break;
+      case CNB_LOSS_CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED: s = __fsub_rn(s, __fmul_rn(tv, logf(__fadd_rn(yv, kTiny)))); break;
+      default: break;                                   // CROSS_ENTROPY_MULTINOMIAL: the value is the label's alone
+    }
+    if (deriv) deriv[i] = __fmul_rn(g, w);
+  }
+  if (loss == CNB_LOSS_SQUARED_ERROR) s = __fmul_rn(0.5f, s);
+  if (loss == CNB_LOSS_CROSS_ENTROPY_MULTINOMIAL) s = -logf(fmaxf(__ldg(y + n + (long long)rows * lab), 1e-30f));
+  value[n] = s;
+}
+// CLASSIFICATION_MULTINOMIAL: one warp per image decides the argmax as kSoftMaxCorrectRowMajor (cudamat_kernels.cu:1139,
+// launched with 32 threads) does: lane j keeps the first strict maximum of columns j, j + 32, ... (from -FLT_MAX), then the
+// lanes are compared in lane order, again strictly.  value = 1 when that column is the label.
+__global__ void __launch_bounds__(256) classification_multinomial_kernel(const float* __restrict__ y, const int* __restrict__ labels,
+                                                                         float* value, int rows, int cols) {
+  const int lane = threadIdx.x & 31, n = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (n >= rows) return;
+  float m = -3.402823466e38f;
+  int arg = 0;
+  for (int c = lane; c < cols; c += 32) {
+    const float v = __ldg(y + n + (long long)rows * c);
+    if (v > m) { m = v; arg = c; }
+  }
+  float bm = -3.402823466e38f;
+  int barg = 0;
+  for (int j = 0; j < 32; j++) {
+    const float mj = __shfl_sync(0xffffffffu, m, j);
+    const int aj = __shfl_sync(0xffffffffu, arg, j);
+    if (mj > bm) { bm = mj; barg = aj; }
+  }
+  if (lane == 0) value[n] = barg == labels[n] ? 1.f : 0.f;
+}
+// CLASSIFICATION_BINARY (kLogisticCorrectNormalized, cudamat_kernels.cu:827): the share of the features with t >= 0 whose
+// (t >= 0.5) == (y >= 0.5); 0 for an image without such features
+__global__ void classification_binary_kernel(const float* __restrict__ y, const float* __restrict__ t, float* value, int rows,
+                                             int cols) {
+  const int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= rows) return;
+  float correct = 0.f, total = 0.f;
+  for (int c = 0; c < cols; c++) {
+    const long long i = n + (long long)rows * c;
+    const float p = __ldg(y + i), tv = __ldg(t + i);
+    if (tv < 0.f) continue;
+    correct += ((tv >= 0.5f && p >= 0.5f) || (tv < 0.5f && p < 0.5f)) ? 1.f : 0.f;
+    total += 1.f;
+  }
+  value[n] = total > 0.f ? correct / total : 0.f;
+}
+
 // Multi-tensor SGD (SGDOptimizer::Optimize, src/optimizer.cc:174-200): ONE launch updates every tensor of a batch (an
 // all-reduce bucket, or the whole net).  The block -> tensor map is a prefix table that travels in the kernel parameters
 // (no device-side descriptor to keep coherent).  Tensors whose staged bf16 copy exists (conv weights in bf16 mode) get it
@@ -692,6 +798,49 @@ void cnb_relu_deriv(float* dx, const float* y, long long n) {
   relu_deriv_kernel<<<blocks_for(std::max(n4, n - 4 * n4), 256), 256, 0, state().stream>>>(dx, y, n, n4);
   count_launch(); CNB_LAUNCH_CHECK("relu_deriv");
   end_write(dx, n, emit, nullptr);
+}
+void cnb_logistic(float* x, long long n) {
+  const bool emit = take_fuse().emit_bf16 != 0;
+  if (n <= 0) return;
+  const long long n4 = aligned16(x) ? n / 4 : 0;
+  __nv_bfloat16* o16 = begin_write(x, n, emit, true);
+  logistic_kernel<<<blocks_for(std::max(n4, n - 4 * n4), 256), 256, 0, state().stream>>>(x, n, n4, o16);
+  count_launch(); CNB_LAUNCH_CHECK("logistic");
+  end_write(x, n, emit, o16);
+}
+void cnb_logistic_deriv(float* dx, const float* y, long long n) {
+  const bool emit = take_fuse().emit_bf16 != 0;
+  if (n <= 0) return;
+  const long long n4 = (aligned16(dx) && aligned16(y)) ? n / 4 : 0;
+  __nv_bfloat16* o16 = begin_write(dx, n, emit, true);
+  logistic_deriv_kernel<<<blocks_for(std::max(n4, n - 4 * n4), 256), 256, 0, state().stream>>>(dx, y, n, n4, o16);
+  count_launch(); CNB_LAUNCH_CHECK("logistic_deriv");
+  end_write(dx, n, emit, o16);
+}
+static bool is_loss(int f) { return f >= CNB_LOSS_SQUARED_ERROR && f <= CNB_LOSS_CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED; }
+void cnb_loss_deriv(int loss, const float* y, const float* targets, const int* labels, float* deriv, float* loss_per_image,
+                    int rows, int cols, float weight) {
+  CNB_REQUIRE(is_loss(loss), "cnb_loss_deriv");
+  if (rows <= 0) return;
+  if (loss == CNB_LOSS_CROSS_ENTROPY_MULTINOMIAL && weight == 1.f) {     // the kernel every softmax net has always run
+    cnb_softmax_ce_deriv(y, labels, deriv, loss_per_image, rows, cols);
+    return;
+  }
+  bf16_note_write(deriv, (long long)rows * cols);
+  loss_kernel<<<ceil_div(rows, 128), 128, 0, state().stream>>>(loss, y, targets, labels, deriv, loss_per_image, rows, cols, weight);
+  count_launch(); CNB_LAUNCH_CHECK("loss_deriv");
+}
+void cnb_metric(int metric, const float* y, const float* targets, const int* labels, float* metric_per_image, int rows, int cols) {
+  CNB_REQUIRE(is_loss(metric) || metric == CNB_LOSS_CLASSIFICATION_MULTINOMIAL || metric == CNB_LOSS_CLASSIFICATION_BINARY,
+              "cnb_metric");
+  if (rows <= 0) return;
+  if (metric == CNB_LOSS_CLASSIFICATION_MULTINOMIAL)
+    classification_multinomial_kernel<<<ceil_div(rows, 8), 256, 0, state().stream>>>(y, labels, metric_per_image, rows, cols);
+  else if (metric == CNB_LOSS_CLASSIFICATION_BINARY)
+    classification_binary_kernel<<<ceil_div(rows, 128), 128, 0, state().stream>>>(y, targets, metric_per_image, rows, cols);
+  else
+    loss_kernel<<<ceil_div(rows, 128), 128, 0, state().stream>>>(metric, y, targets, labels, nullptr, metric_per_image, rows, cols, 1.f);
+  count_launch(); CNB_LAUNCH_CHECK("metric");
 }
 void cnb_dropout(float* x, float* mask, long long n, float dropprob, float scale, unsigned long long seed) {
   const bool emit = take_fuse().emit_bf16 != 0;

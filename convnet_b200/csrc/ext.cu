@@ -76,7 +76,15 @@ void convnet_b200_set_conv_precision(int mode) {
 }
 int convnet_b200_get_conv_precision(void) { return state().precision; }
 void convnet_b200_fuse_next(const float* bias, int relu, const float* relu_mask) {
-  state().fuse.bias = bias; state().fuse.relu = relu; state().fuse.relu_mask = relu_mask;
+  Fuse& f = state().fuse;
+  f.bias = bias; f.act = relu ? kActRelu : kActNone;
+  f.act_state = relu_mask; f.state_act = relu_mask ? kActRelu : kActNone;
+}
+void convnet_b200_fuse_next_act(const float* bias, int act, const float* act_state) {
+  CNB_REQUIRE(act >= kActNone && act <= kActLogistic, "convnet_b200_fuse_next_act");
+  Fuse& f = state().fuse;
+  f.bias = bias; f.act = act;
+  f.act_state = act != kActNone ? act_state : nullptr; f.state_act = f.act_state ? act : kActNone;
 }
 void convnet_b200_emit_bf16_next(void) { state().fuse.emit_bf16 = 1; }
 void convnet_b200_fuse_next_bias_grad(float* grad_bias, float scaleTargets, float scaleOutput) {

@@ -138,8 +138,24 @@ API int cnb_bn_optimizer_check(const OptimizerConfig* c) {
   return 0;
 }
 
+// the output layer's float targets ([batch x state columns], column-major, written by the caller); NULL / 0 for an output
+// layer trained on labels (cnb_net_labels)
+API float* cnb_net_targets(void* p) { return ((NetHandle*)p)->net->OutputLayer().GetTargets().GetDevData(); }
+API long long cnb_net_targets_floats(void* p) { return (long long)((NetHandle*)p)->net->OutputLayer().GetTargets().GetNumEls(); }
+// loss_function_weight * the batch's loss (ConvNet::GetLoss) and the summed performance metric (GetPerformanceMetric)
 API float cnb_net_loss(void* p) { return ((NetHandle*)p)->net->GetLoss(); }
-// one training step; *loss (may be NULL) receives the summed cross-entropy of the batch (one scalar D2H, like GetLoss)
+API float cnb_net_metric(void* p) { return ((NetHandle*)p)->net->GetPerformanceMetric(); }
+// static description of a model's output layer (no device memory): 0 ok, -1 unknown model.  *activation: the Activation
+// enum of convnet.h; *loss / *metric: proto LossFunction numbers; *labels: 1 trained on integer labels, 0 on float targets
+API int cnb_model_output_layer(const char* model, int* activation, int* loss, int* metric, float* weight, int* labels) {
+  ModelConfig m;
+  if (!TryBuildModel(model, &m)) return -1;
+  const LayerConfig& l = m.layer.back();
+  *activation = l.activation; *loss = l.loss_function; *metric = l.performance_metric; *weight = l.loss_function_weight;
+  *labels = TakesLabels(l.activation) ? 1 : 0;
+  return 0;
+}
+// one training step; *loss (may be NULL) receives the batch's loss as cnb_net_loss gives it (one scalar D2H)
 API void cnb_net_train_step(void* p, float* loss) { ((NetHandle*)p)->net->TrainOneBatch(loss); }
 // one traced training step (ConvNet::TraceStep); returns the number of floats the full record has, writes min(cap, that)
 API int cnb_net_trace_step(void* p, float* out, int cap) {

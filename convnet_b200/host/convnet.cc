@@ -55,7 +55,38 @@ void Layer::AllocateMemory(int batch_size) {               // layer.cc:228-262 (
     HOST_CUDA_CHECK(cudaMalloc((void**)&labels_, sizeof(int) * batch_size));
     HOST_CUDA_CHECK(cudaMemset(labels_, 0, sizeof(int) * batch_size));
     loss_per_image_.AllocateGPUMemory(batch_size, 1);
+    metric_per_image_.AllocateGPUMemory(batch_size, 1);
+    if (!TakesLabels(config_.activation)) {                // layer.cc:530-602: data_ shaped like the state
+      targets_.AllocateGPUMemory(batch_size, cols);
+      targets_.Set(0);
+    }
   }
+}
+
+std::string LayerConfigError(const LayerConfig& c) {
+  const bool softmax = c.activation == SOFTMAX || c.activation == SOFTMAX_DIST;
+  if (!c.is_output) {
+    if (softmax) return "SOFTMAX / SOFTMAX_DIST is an output activation (back-propagation through a softmax is not implemented)";
+    return "";
+  }
+  auto name = [](int f) -> std::string {
+    static const char* n[] = {"SQUARED_ERROR", "LINEAR_ERROR", "CROSS_ENTROPY_MULTINOMIAL", "CROSS_ENTROPY_BINARY",
+                              "CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED", "CLASSIFICATION_MULTINOMIAL", "CLASSIFICATION_BINARY",
+                              "HINGE_LINEAR", "HINGE_QUADRATIC"};
+    return f >= 0 && f <= HINGE_QUADRATIC ? n[f] : "LossFunction " + std::to_string(f);
+  };
+  const std::string target = TakesLabels(c.activation) ? "integer labels" : "a float target per feature";
+  for (int which = 0; which < 2; which++) {
+    const int f = which ? c.performance_metric : c.loss_function;
+    const std::string field = which ? "performance_metric " : "loss_function ";
+    if (f < SQUARED_ERROR || f > CLASSIFICATION_BINARY) return field + name(f) + " is not supported";
+    if (!which && (f == CLASSIFICATION_MULTINOMIAL || f == CLASSIFICATION_BINARY))
+      return field + name(f) + " has no derivative to train with";
+    if (ReadsLabels(f) != TakesLabels(c.activation))
+      return field + name(f) + " reads " + (ReadsLabels(f) ? "integer labels" : "a float target per feature") +
+             ", but this output layer's activation has " + target;
+  }
+  return "";
 }
 
 // `emit`: this call is the last writer of the tensor and the next conv edge reads it as bf16 (see Edge::SetEmitUp)
@@ -67,14 +98,22 @@ void Layer::ApplyActivation(bool emit) {
       if (emit) convnet_b200_emit_bf16_next();
       state_.ApplyReLU();                                  // LowerBound(0), layer.cc:550
       break;
-    case SOFTMAX: state_.ApplySoftmax(); break;
+    case LOGISTIC:                                         // ApplyLogistic, layer.cc:598
+      if (emit) convnet_b200_emit_bf16_next();
+      cnb_logistic(state_.GetDevData(), (long long)state_.GetNumEls());
+      break;
+    case SOFTMAX: case SOFTMAX_DIST: state_.ApplySoftmax(); break;
   }
 }
+// (of the state as stored: for a layer with dropout that is act(x) * mask, the reference's order, DESIGN.md §5)
 void Layer::ApplyDerivativeOfActivation(bool emit) {
   if (deriv_fused_) return;
   if (config_.activation == RECTIFIED_LINEAR) {
     if (emit) convnet_b200_emit_bf16_next();
     deriv_.ApplyDerivOfReLU(state_);
+  } else if (config_.activation == LOGISTIC) {            // ApplyDerivativeOfLogistic, layer.cc:601
+    if (emit) convnet_b200_emit_bf16_next();
+    cnb_logistic_deriv(deriv_.GetDevData(), state_.GetDevData(), (long long)deriv_.GetNumEls());
   }
 }
 void Layer::ApplyDropout(bool train, unsigned long long step, unsigned long long salt, bool emit) {      // layer.cc:367-395, scale-up at train time
@@ -123,9 +162,14 @@ void Layer::ApplyBatchNormalization(bool train, bool emit) {
     mu = BnStat(2); sigma = BnStat(3);
   }
   bn_train_ = train;
-  if (emit) convnet_b200_emit_bf16_next();
+  const bool logistic = config_.activation == LOGISTIC;   // the BN kernel fuses max(., 0) only: sigma is a pass after it
+  if (emit && !logistic) convnet_b200_emit_bf16_next();
   cnb_bn_apply(pre_bn_.GetDevData(), state_.GetDevData(), n, C, gamma_.GetDevData(), beta_.GetDevData(), mu, sigma,
                config_.activation == RECTIFIED_LINEAR);
+  if (logistic) {
+    if (emit) convnet_b200_emit_bf16_next();
+    cnb_logistic(state_.GetDevData(), (long long)state_.GetNumEls());
+  }
 }
 // layer.cc:480-510, with xhat from the saved input (DESIGN.md §5: the state holds relu / dropout of the output)
 void Layer::ApplyDerivativeofBatchNormalization(bool emit) {
@@ -145,8 +189,12 @@ void Layer::AppendBnSgdTensors(std::vector<CnbOptTensorEx>& out) {
 }
 
 void Layer::ComputeDeriv() {
-  cnb_softmax_ce_deriv(state_.GetDevData(), labels_, deriv_.GetDevData(), loss_per_image_.GetDevData(),
-                       state_.GetRows(), state_.GetCols());
+  cnb_loss_deriv(config_.loss_function, state_.GetDevData(), targets_.GetDevData(), labels_, deriv_.GetDevData(),
+                 loss_per_image_.GetDevData(), state_.GetRows(), state_.GetCols(), config_.loss_function_weight);
+}
+void Layer::ComputePerformanceMetric() {
+  cnb_metric(config_.performance_metric, state_.GetDevData(), targets_.GetDevData(), labels_, metric_per_image_.GetDevData(),
+             state_.GetRows(), state_.GetCols());
 }
 
 // =================================================================== DataParallelSync (NCCL, loaded lazily)
@@ -265,13 +313,22 @@ ConvNet::ConvNet(const ModelConfig& model, int batch_size) : model_(model), batc
     e->SetBatchSize(batch_size);
     edges_.push_back(e);
   }
-  // epilogue fusion of the Layer-side ReLU / ReLU' into the neighbouring edges (SURVEY.md 8(f) rank 2)
+  for (const LayerConfig& lc : model.layer) {        // activations, loss functions and metrics this class cannot run
+    const std::string why = LayerConfigError(lc);
+    if (why.empty()) continue;
+    for (Edge* e : edges_) delete e;
+    for (Layer* x : layers_) delete x;
+    throw std::invalid_argument("layer '" + lc.name + "': " + why);
+  }
+  // epilogue fusion of the Layer-side activation (ReLU, logistic) and its derivative into the neighbouring edges
+  // (SURVEY.md 8(f) rank 2)
   for (size_t i = 0; i < edges_.size(); i++) {
     Layer *src = layers_[i], *dst = layers_[i + 1];
-    if (dst->GetActivation() == RECTIFIED_LINEAR) {
-      edges_[i]->SetFuseReLU(true);                // honoured only where CanFuseReLU() (checked after SetImageSize below)
-    }
-    if (!src->IsInput() && src->GetActivation() == RECTIFIED_LINEAR) edges_[i]->SetFuseMask(true);
+    const int up = ActCode(dst->GetActivation()), down = src->IsInput() ? CNB_ACT_LINEAR : ActCode(src->GetActivation());
+    edges_[i]->SetFuseActs(up, down);
+    // honoured only where CanFuseReLU() / CanFuseLogistic() (checked after SetImageSize below)
+    if (up != CNB_ACT_LINEAR) edges_[i]->SetFuseReLU(true);
+    if (down != CNB_ACT_LINEAR) edges_[i]->SetFuseMask(true);
   }
   // SetImageSize propagation (convnet.cc:226-268)
   const LayerConfig& in = model.layer.front();
@@ -306,10 +363,12 @@ ConvNet::ConvNet(const ModelConfig& model, int batch_size) : model_(model), batc
     Edge* e = edges_[i];
     // a batch-normalised layer: the edge writes the pre-normalisation input, the BN pass applies the activation
     const bool bn = layers_[i + 1]->BatchNormalize();
-    const bool relu = !bn && layers_[i + 1]->GetActivation() == RECTIFIED_LINEAR && e->CanFuseReLU() && e->WantsFuseReLU();
-    e->SetFuseReLU(relu);
-    layers_[i + 1]->SetActivationFused(relu || bn);
-    const bool mask = e->CanFuseMask() && e->WantsFuseMask();
+    const int up = ActCode(layers_[i + 1]->GetActivation()), down = ActCode(layers_[i]->GetActivation());
+    const bool act = !bn && up != CNB_ACT_LINEAR && e->CanFuseReLU() && e->WantsFuseReLU() &&
+                     (up == CNB_ACT_RELU || e->CanFuseLogistic());
+    e->SetFuseReLU(act);
+    layers_[i + 1]->SetActivationFused(act || bn);
+    const bool mask = e->CanFuseMask() && e->WantsFuseMask() && (down == CNB_ACT_RELU || e->CanFuseLogistic());
     e->SetFuseMask(mask);
     layers_[i]->SetDerivFused(mask);
   }
@@ -366,7 +425,7 @@ void ConvNet::AllocateMemory() {
   parameters_.AllocateGPUMemory(1, (int)total);
   grad_parameters_.AllocateGPUMemory(1, (int)total);
   history_.AllocateGPUMemory(1, (int)total);
-  loss_sum_.AllocateGPUMemory(1, 1);
+  loss_sum_.AllocateGPUMemory(1, 2);                           // the loss, the performance metric
   for (size_t i = 0; i < edges_.size(); i++) {
     if (edge_size_[i] == 0) continue;
     Matrix p, g, h;
@@ -474,17 +533,24 @@ bool ConvNet::DropoutFolds(size_t i) const {
   static const bool no_fold = getenv("CONVNET_B200_NO_DROPOUT_FOLD") && getenv("CONVNET_B200_NO_DROPOUT_FOLD")[0] == '1';
   if (no_fold || i == 0 || i >= edges_.size()) return false;        // edges_[i]: the edge whose ComputeDown writes layers_[i]'s derivative
   const Layer* l = layers_[i];
-  return l->HasDropout() && l->GetActivation() == RECTIFIED_LINEAR && !l->HasSeparateDerivPass() && edges_[i]->CanScaleDeriv();
+  // a ReLU or logistic layer: where the mask drops a unit its state is 0, and so is the derivative of the activation there
+  return l->HasDropout() && ActCode(l->GetActivation()) != CNB_ACT_LINEAR && !l->HasSeparateDerivPass() &&
+         edges_[i]->CanScaleDeriv();
 }
 
 void ConvNet::ComputeDeriv() { OutputLayer().ComputeDeriv(); }
 
-float ConvNet::GetLoss() {                                   // CrossEntropyMultinomial::GetLoss: sum over the batch
+float ConvNet::GetLoss() {                                   // Layer::GetLoss: the weighted sum over the batch (layer.cc:435-437)
   Layer& out = OutputLayer();
-  cnb_softmax_ce_deriv(out.GetState().GetDevData(), out.GetLabels(), out.GetDeriv().GetDevData(),
-                       out.GetLossPerImage(), batch_size_, out.GetState().GetCols());
+  out.ComputeDeriv();
   cnb_sum(out.GetLossPerImage(), loss_sum_.GetDevData(), batch_size_);
-  return loss_sum_.ReadValue(0);
+  return out.LossWeight() * loss_sum_.ReadValue(0);
+}
+float ConvNet::GetPerformanceMetric() {
+  Layer& out = OutputLayer();
+  out.ComputePerformanceMetric();
+  cnb_sum(out.GetMetricPerImage(), loss_sum_.GetDevData() + 1, batch_size_);
+  return loss_sum_.ReadValue(1);
 }
 
 void ConvNet::Bprop() {                                      // convnet.cc:390-405 + 362-375
@@ -629,7 +695,7 @@ void ConvNet::TrainOneBatch(float* loss_out) {               // convnet.cc:475-4
   eager_update_ = false;
   UpdateWeights();
   if (trace_.on) HOST_CUDA_CHECK(cudaEventRecord(trace_.end, Matrix::Stream()));
-  if (loss_out) *loss_out = loss_sum_.ReadValue(0);
+  if (loss_out) *loss_out = OutputLayer().LossWeight() * loss_sum_.ReadValue(0);
   step_++;
 }
 
@@ -720,14 +786,13 @@ double GradChecker::LossAtD(Matrix& w, size_t index, float value) {
   // per-image cross-entropy on the device, summed in double on the host: the finite difference of two ~O(batch)
   // losses must not lose the 1e-3-sized signal to fp32 summation noise
   Layer& out = OutputLayer();
-  cnb_softmax_ce_deriv(out.GetState().GetDevData(), out.GetLabels(), out.GetDeriv().GetDevData(), out.GetLossPerImage(),
-                       batch_size_, out.GetState().GetCols());
+  out.ComputeDeriv();
   std::vector<float> h(batch_size_);
   HOST_CUDA_CHECK(cudaMemcpyAsync(h.data(), out.GetLossPerImage(), sizeof(float) * batch_size_, cudaMemcpyDeviceToHost, Matrix::Stream()));
   HOST_CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
   double s = 0;
   for (float v : h) s += v;
-  return s;
+  return (double)out.LossWeight() * s;
 }
 
 std::vector<GradCheckResult> GradChecker::Run(unsigned seed) {
@@ -742,6 +807,25 @@ std::vector<GradCheckResult> GradChecker::Run(unsigned seed) {
   const int classes = OutputLayer().GetState().GetCols();
   for (int& v : hl) v = (int)(gen() % classes);
   HOST_CUDA_CHECK(cudaMemcpy(OutputLayer().GetLabels(), hl.data(), sizeof(int) * batch_size_, cudaMemcpyHostToDevice));
+  Matrix& t = OutputLayer().GetTargets();                     // a per-feature target: one the loss function accepts
+  if (t.GetNumEls()) {
+    const int rows = t.GetRows(), cols = t.GetCols();
+    std::vector<float> ht(t.GetNumEls());
+    std::uniform_real_distribution<float> ud(0.f, 1.f);
+    for (int n = 0; n < rows; n++) {
+      float total = 0.f;
+      for (int c = 0; c < cols; c++) {
+        float& v = ht[n + (size_t)rows * c];
+        switch (model_.layer.back().loss_function) {
+          case CROSS_ENTROPY_BINARY: v = c % 4 == 3 ? -1.f : (float)(gen() % 2); break;       // every 4th: don't care
+          case CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED: v = ud(gen) + 0.05f; total += v; break;  // normalised below
+          default: v = nd(gen); break;
+        }
+      }
+      if (total > 0.f) for (int c = 0; c < cols; c++) ht[n + (size_t)rows * c] /= total;
+    }
+    t.CopyFromHost(ht.data(), ht.size());
+  }
 
   Fprop(false);
   ComputeDeriv();

@@ -16,13 +16,29 @@
 
 namespace cnbhost {
 
-enum Activation { LINEAR, RECTIFIED_LINEAR, SOFTMAX };
+enum Activation { LINEAR, RECTIFIED_LINEAR, SOFTMAX, LOGISTIC, SOFTMAX_DIST };
+// proto/convnet_config.proto:34-44 LossFunction, same numbers (the CNB_LOSS_* codes of the kernels)
+enum LossFunction {
+  SQUARED_ERROR = 0, LINEAR_ERROR = 1, CROSS_ENTROPY_MULTINOMIAL = 2, CROSS_ENTROPY_BINARY = 3,
+  CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED = 4, CLASSIFICATION_MULTINOMIAL = 5, CLASSIFICATION_BINARY = 6,
+  HINGE_LINEAR = 7, HINGE_QUADRATIC = 8
+};
+// the kernel code of a fused or stand-alone activation (CNB_ACT_*): 0 for LINEAR and the softmaxes
+inline int ActCode(Activation a) { return a == RECTIFIED_LINEAR ? CNB_ACT_RELU : (a == LOGISTIC ? CNB_ACT_LOGISTIC : CNB_ACT_LINEAR); }
+// an output layer of this activation is trained on integer labels (SOFTMAX); every other one on a float target per feature
+inline bool TakesLabels(Activation a) { return a == SOFTMAX; }
+// a loss function or performance metric that reads labels (the others read per-feature targets)
+inline bool ReadsLabels(int f) { return f == CROSS_ENTROPY_MULTINOMIAL || f == CLASSIFICATION_MULTINOMIAL; }
 
 struct LayerConfig {
   std::string name;
   int num_channels = 0;
   bool is_input = false, is_output = false;
   Activation activation = LINEAR;
+  // output layers (proto/convnet_config.proto:46-48)
+  int loss_function = CROSS_ENTROPY_MULTINOMIAL;
+  int performance_metric = CLASSIFICATION_MULTINOMIAL;
+  float loss_function_weight = 1.f;
   int image_size_y = 0, image_size_x = 0, image_size_t = 1;   // input layer only
   float dropprob = 0.f;
   // batch normalisation between the incoming edge and the activation (proto/convnet_config.proto:56-61)
@@ -34,6 +50,8 @@ struct LayerConfig {
 
 // nullptr if `c` can train gamma or beta, else why not: OptimizerConfigError, or a norm rule (refused, DESIGN.md §5)
 const char* BnOptimizerConfigError(const OptimizerConfig& c);
+// "" if the activation, loss function and performance metric of `c` can run, else why not
+std::string LayerConfigError(const LayerConfig& c);
 
 struct ModelConfig {
   std::string name;
@@ -56,13 +74,19 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   float DropoutProb() const { return config_.dropprob; }
   unsigned long long DropoutSeed(unsigned long long step, unsigned long long salt) const;
   void SetDropoutDerivFolded(bool v) { dropout_deriv_folded_ = v; }   // this step: the edge above scaled the derivative instead
-  bool HasSeparateActivationPass() const { return config_.activation == RECTIFIED_LINEAR && !activation_fused_; }
-  bool HasSeparateDerivPass() const { return config_.activation == RECTIFIED_LINEAR && !deriv_fused_; }
-  void ComputeDeriv();                          // softmax + cross-entropy: deriv = p - onehot   (loss_functions.cc)
+  bool HasSeparateActivationPass() const { return ActCode(config_.activation) != CNB_ACT_LINEAR && !activation_fused_; }
+  bool HasSeparateDerivPass() const { return ActCode(config_.activation) != CNB_ACT_LINEAR && !deriv_fused_; }
+  // output layer: deriv = loss_function_weight * dLoss/dstate and the per-image loss (unweighted), layer.cc:426-437
+  void ComputeDeriv();
+  void ComputePerformanceMetric();              // the per-image performance metric (GetPerformanceMetric, layer.cc:422)
   Matrix& GetState() { return state_; }
   Matrix& GetDeriv() { return deriv_; }
   int* GetLabels() { return labels_; }
+  // the float targets of an output layer that does not take labels ([images x state columns]); empty otherwise
+  Matrix& GetTargets() { return targets_; }
   float* GetLossPerImage() { return loss_per_image_.GetDevData(); }
+  float* GetMetricPerImage() { return metric_per_image_.GetDevData(); }
+  float LossWeight() const { return config_.loss_function_weight; }
   bool IsInput() const { return config_.is_input; }
   bool IsOutput() const { return config_.is_output; }
   int GetNumChannels() const { return config_.num_channels; }
@@ -97,7 +121,7 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
  private:
   LayerConfig config_;
   int image_size_y_, image_size_x_, image_size_t_;
-  Matrix state_, deriv_, loss_per_image_, dropout_mask_;
+  Matrix state_, deriv_, loss_per_image_, metric_per_image_, targets_, dropout_mask_;
   Matrix pre_bn_, bn_stats_, gamma_, beta_, grad_gamma_, grad_beta_, hist_gamma_, hist_beta_, state_gamma_, state_beta_;
   bool bn_train_ = false;                       // the last ApplyBatchNormalization used the batch statistics
   long long gamma_step_ = 0, beta_step_ = 0;
@@ -159,7 +183,8 @@ class ConvNet {
   float* AdaptiveState() { return state_.GetDevData(); }
   void ComputeDeriv();
   void TrainOneBatch(float* loss_out);                          // convnet.cc:475-485
-  float GetLoss();                                              // sum of per-image CE (synchronises)
+  float GetLoss();                                              // loss_function_weight * the batch's loss (synchronises)
+  float GetPerformanceMetric();                                 // sum of the per-image performance metric (synchronises)
   void SetDataParallel(DataParallelSync* dp, size_t bucket_floats);
   void SetBucketFloats(size_t bucket_floats);                   // re-plan the buckets (also used without data parallelism)
   void BroadcastParameters();
@@ -245,6 +270,7 @@ ModelConfig BuildAlexNet();     // examples/imagenet/CLS_net_20140801232522.pbtx
 ModelConfig BuildLeNet();       // examples/mnist-conv/net.pbtxt
 ModelConfig BuildC3D();         // SURVEY.md §8(d) cfg4
 ModelConfig BuildTinyNet();     // small conv+pool+rnorm+1x1+fc net for tests / grad check
+ModelConfig BuildLogCheckNet(); // the gradcheck net with logistic hidden units
 ModelConfig BuildModel(const std::string& name);
 
 }  // namespace cnbhost

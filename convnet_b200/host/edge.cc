@@ -251,12 +251,12 @@ void ConvEdge::SetGradMemory(Matrix& p) {                    // :108-136
 void ConvEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) {   // :138-170
   const float scale_targets = overwrite ? 0 : 1;
   const int mods = num_modules_y_ * num_modules_x_ * num_modules_t_;
-  const bool fused = fuse_relu_ && CanFuseReLU();        // bias (+ReLU of the destination layer) in the conv epilogue
+  const bool fused = fuse_relu_ && CanFuseReLU();        // bias (+activation of the destination layer) in the conv epilogue
   StageForUp(input);
   const bool bias_pass = !has_no_bias_ && !fused;          // then the bias kernel, not the conv, writes the output last
   if (emit_up_ && !bias_pass) convnet_b200_emit_bf16_next();
   if (image_size_t_ == 1) {
-    if (fused) convnet_b200_fuse_next(bias_.GetDevData(), 1, nullptr);
+    if (fused) convnet_b200_fuse_next_act(bias_.GetDevData(), up_act_, nullptr);
     ApplyDropoutRequest(fused);
     Matrix::ConvUp(input, weights_, output, conv_desc_, scale_targets);
   } else {
@@ -287,7 +287,7 @@ void ConvEdge::ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, 
                            bool overwrite) {                 // :172-181
   const float scale_targets = overwrite ? 0 : 1;
   StageForBprop(deriv_output);
-  if (fuse_mask_) convnet_b200_fuse_next(nullptr, 0, input.GetDevData());      // ReLU' of the source layer
+  if (fuse_mask_) convnet_b200_fuse_next_act(nullptr, down_act_, input.GetDevData());      // activation' of the source layer
   if (emit_down_) convnet_b200_emit_bf16_next();
   ApplyBiasGradRequest();
   if (image_size_t_ == 1) Matrix::ConvDown(deriv_output, weights_, deriv_input, conv_desc_, scale_targets);
@@ -375,11 +375,11 @@ void LocalEdge::SetGradMemory(Matrix& p) {                    // :74-101
   }
 }
 void LocalEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) {   // :103-119
-  const bool fused = fuse_relu_ && CanFuseReLU();        // per-feature bias (+ReLU of the destination layer) in the epilogue
+  const bool fused = fuse_relu_ && CanFuseReLU();        // per-feature bias (+activation of the destination layer) in the epilogue
   StageForUp(input);
   const bool bias_pass = !has_no_bias_ && !fused;
   if (emit_up_ && !bias_pass) convnet_b200_emit_bf16_next();
-  if (fused) convnet_b200_fuse_next(bias_.GetDevData(), 1, nullptr);
+  if (fused) convnet_b200_fuse_next_act(bias_.GetDevData(), up_act_, nullptr);
   ApplyDropoutRequest(fused);
   Matrix::LocalUp(input, weights_, output, conv_desc_, overwrite ? 0 : 1);
   NoteUp();
@@ -391,7 +391,7 @@ void LocalEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool tr
 void LocalEdge::ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input,
                             bool overwrite) {                 // :121-126
   StageForBprop(deriv_output);
-  if (fuse_mask_) convnet_b200_fuse_next(nullptr, 0, input.GetDevData());
+  if (fuse_mask_) convnet_b200_fuse_next_act(nullptr, down_act_, input.GetDevData());
   if (emit_down_) convnet_b200_emit_bf16_next();
   ApplyBiasGradRequest();
   Matrix::LocalDown(deriv_output, weights_, deriv_input, conv_desc_, overwrite ? 0 : 1);
@@ -450,7 +450,7 @@ void FCEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train
   View(input, output);
   const bool fused = fuse_relu_ && !has_no_bias_;
   StageForUp(input);
-  if (fused) convnet_b200_fuse_next(bias_.GetDevData(), 1, nullptr);
+  if (fused) convnet_b200_fuse_next_act(bias_.GetDevData(), up_act_, nullptr);
   const bool bias_pass = !has_no_bias_ && !fused;
   if (emit_up_ && !bias_pass) convnet_b200_emit_bf16_next();
   ApplyDropoutRequest(fused);
@@ -463,7 +463,7 @@ void FCEdge::ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Ma
   Shape4D si = deriv_input.GetShape4D(), so = deriv_output.GetShape4D();
   View(deriv_input, deriv_output);
   StageForBprop(deriv_output);
-  if (fuse_mask_) convnet_b200_fuse_next(nullptr, 0, input.GetDevData());
+  if (fuse_mask_) convnet_b200_fuse_next_act(nullptr, down_act_, input.GetDevData());
   if (emit_down_) convnet_b200_emit_bf16_next();
   ApplyBiasGradRequest();
   Matrix::ConvDown(deriv_output, weights_, deriv_input, desc_, overwrite ? 0 : 1);
@@ -510,7 +510,7 @@ void ConvOneToOneEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, 
   const int batch_size = input.GetRows();
   const bool fused = fuse_relu_ && !has_no_bias_;
   StageForUp(input);
-  if (fused) convnet_b200_fuse_next(bias_.GetDevData(), 1, nullptr);
+  if (fused) convnet_b200_fuse_next_act(bias_.GetDevData(), up_act_, nullptr);
   const bool bias_pass = !has_no_bias_ && !fused;
   if (emit_up_ && !bias_pass) convnet_b200_emit_bf16_next();
   ApplyDropoutRequest(fused);
@@ -526,7 +526,7 @@ void ConvOneToOneEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, 
 void ConvOneToOneEdge::ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input,
                                    bool overwrite) {
   StageForBprop(deriv_output);
-  if (fuse_mask_) convnet_b200_fuse_next(nullptr, 0, input.GetDevData());
+  if (fuse_mask_) convnet_b200_fuse_next_act(nullptr, down_act_, input.GetDevData());
   if (emit_down_) convnet_b200_emit_bf16_next();
   ApplyBiasGradRequest();
   Matrix::ConvDown(deriv_output, weights_, deriv_input, desc_, overwrite ? 0 : 1);
@@ -582,7 +582,7 @@ void MaxPoolEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool 
   Matrix::ConvMaxPool(input, output, conv_desc_);
 }
 void MaxPoolEdge::ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) {
-  if (fuse_mask_) convnet_b200_fuse_next(nullptr, 0, input.GetDevData());
+  if (fuse_mask_) convnet_b200_fuse_next_act(nullptr, down_act_, input.GetDevData());
   if (emit_down_) convnet_b200_emit_bf16_next();
   ApplyBiasGradRequest();
   Matrix::ConvMaxPoolUndo(input, deriv_output, output, deriv_input, conv_desc_, overwrite ? 0 : 1);
@@ -593,7 +593,7 @@ void AvgPoolEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool 
   Matrix::ConvAvgPool(input, output, conv_desc_);
 }
 void AvgPoolEdge::ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) {
-  if (fuse_mask_) convnet_b200_fuse_next(nullptr, 0, input.GetDevData());
+  if (fuse_mask_) convnet_b200_fuse_next_act(nullptr, down_act_, input.GetDevData());
   if (emit_down_) convnet_b200_emit_bf16_next();
   ApplyBiasGradRequest();
   Matrix::ConvAvgPoolUndo(deriv_output, deriv_input, conv_desc_, overwrite ? 0 : 1);

@@ -114,8 +114,12 @@ class Edge {
   void SetBatchSize(int n) { batch_size_ = n; }
   // Epilogue fusion (convnet_b200_fuse_next): the ReLU of the destination layer rides in ComputeUp's conv epilogue
   // (together with the shared bias), the ReLU derivative of the source layer in ComputeDown's. ConvNet decides.
+  // The activation is that of the layer (CNB_ACT_*: ReLU or logistic): `up` the destination's, `down` the source's.  Where
+  // CanFuseReLU / CanFuseMask hold, the ReLU rides in the epilogue; the logistic unit only where CanFuseLogistic holds too
   virtual bool CanFuseReLU() const { return false; }
   virtual bool CanFuseMask() const { return false; }
+  virtual bool CanFuseLogistic() const { return false; }
+  void SetFuseActs(int up, int down) { up_act_ = up; down_act_ = down; }
   void SetFuseReLU(bool v) { fuse_relu_ = v; }
   void SetFuseMask(bool v) { fuse_mask_ = v; }
   bool WantsFuseReLU() const { return fuse_relu_; }
@@ -153,7 +157,8 @@ class Edge {
   int image_size_y_, image_size_x_, image_size_t_;
   int num_modules_y_, num_modules_x_, num_modules_t_;
   int batch_size_;
-  bool fuse_relu_ = false, fuse_mask_ = false;
+  bool fuse_relu_ = false, fuse_mask_ = false;      // the activation / its derivative is fused (whichever it is)
+  int up_act_ = CNB_ACT_RELU, down_act_ = CNB_ACT_RELU;
   bool emit_up_ = false, emit_down_ = false;
   BiasGradTarget bg_request_;
   float deriv_scale_ = 1.f;
@@ -218,6 +223,8 @@ class EdgeWithWeight : public Edge {
   // (a conv dgrad would only run the column-sum pass inside the library call, on the main stream; leaving it to the edge
   //  below puts it on the side lane instead — so only the pooling edges, whose kernels really fuse it, take the request)
   bool CanScaleDeriv() const override { return fuse_mask_; }               // (3-D ConvEdge: fuse_mask_ is off, CanFuseMask)
+  // sigma and sigma' ride in the conv epilogues exactly where max(., 0) and the ReLU' mask do
+  bool CanFuseLogistic() const override { return true; }
 
  protected:
   void StageForUp(Matrix& input);

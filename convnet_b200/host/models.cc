@@ -115,6 +115,20 @@ ModelConfig BuildGradCheckNet() {
   return m;
 }
 
+// the gradcheck net with logistic units in every hidden layer: the grad check of a smooth nonlinearity through the conv,
+// average-pooling, response-norm, 1x1 and FC edges (sigma after the pooling and sigma' into its undo run as passes).
+// init_wt 3: each sigma' scales the derivative by at most 1/4, and at the default scale the derivative reaching conv1
+// through four logistic layers sits at the float32 noise floor of the finite differences
+ModelConfig BuildLogCheckNet() {
+  ModelConfig m = BuildGradCheckNet();
+  m.name = "logcheck";
+  for (LayerConfig& l : m.layer)
+    if (!l.is_input && !l.is_output) l.activation = LOGISTIC;
+  for (EdgeConfig& e : m.edge)
+    if (e.edge_type == CONVOLUTIONAL || e.edge_type == CONV_ONETOONE || e.edge_type == FC) e.init_wt = 3.f;
+  return m;
+}
+
 // conv + locally connected classifier (cuda-convnet's conv+local nets, scaled to 96 x 96 inputs): the two LOCAL edges
 // carry a filter bank per output position (42 and 29 MB in bf16) and sit near the HBM / tensor-core balance point at
 // batch 128.  init_wt = sqrt(modules): the reference scales a local edge's initial weights by 1/sqrt(K*modules/3)
@@ -166,6 +180,22 @@ ModelConfig BuildLocal3DNet() {
   m.edge = {Conv(3, 2, 1), E(LOCAL, 3, 1, 1), E(FC)};
   finish(m);
   return m;
+}
+
+// NOT models: deliberately invalid output configs on the tiny net ("invalid:<what>") that the tests of ConvNet's refusals
+// build (LayerConfigError); false for an unknown <what>
+static bool BuildInvalidOutputNet(const std::string& what, ModelConfig* m) {
+  *m = BuildTinyNet();
+  LayerConfig& out = m->layer.back();
+  if (what == "hidden-softmax") m->layer[4].activation = SOFTMAX;                           // nin1
+  else if (what == "hinge-loss") out.loss_function = HINGE_LINEAR;
+  else if (what == "hinge-metric") out.performance_metric = HINGE_QUADRATIC;
+  else if (what == "loss-target") out.loss_function = SQUARED_ERROR;                        // labels output, per-feature loss
+  else if (what == "metric-target") { out.activation = LOGISTIC; out.loss_function = CROSS_ENTROPY_BINARY; }  // default metric
+  else if (what == "classification-loss") { out.activation = LOGISTIC; out.loss_function = CLASSIFICATION_BINARY; }
+  else return false;
+  m->name = "invalid:" + what;
+  return true;
 }
 
 // "<model>+ref-optimizer": the optimizer blocks of the model's pbtxt exactly (BuildAlexNet / BuildLeNet keep the constant
@@ -233,7 +263,43 @@ static void UseAdaptiveOptimizers(int type, ModelConfig& m) {
     if (l.batch_normalize) { use(l.gamma_optimizer); use(l.beta_optimizer); }
 }
 
+// "<model>+logistic": every hidden RECTIFIED_LINEAR layer becomes LOGISTIC (the parameter layout does not change)
+static void UseLogisticUnits(const std::string& name, ModelConfig& m) {
+  bool any = false;
+  for (LayerConfig& l : m.layer)
+    if (!l.is_output && l.activation == RECTIFIED_LINEAR) { l.activation = LOGISTIC; any = true; }
+  if (!any) throw std::invalid_argument("model '" + name + "': +logistic finds no RECTIFIED_LINEAR hidden layer");
+}
+
+// the output suffixes: the output layer's activation, loss function and performance metric (at most one per model)
+//   +squared-error  LINEAR, SQUARED_ERROR, metric SQUARED_ERROR (regression on a float target per output unit)
+//   +binary-ce      LOGISTIC, CROSS_ENTROPY_BINARY, metric CLASSIFICATION_BINARY (independent binary labels; t < 0: don't care)
+//   +soft-targets   SOFTMAX_DIST, CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED, metric the same (a distribution over the classes)
+struct OutputSuffix { const char* suffix; Activation act; int loss, metric; };
+static const OutputSuffix kOutputSuffixes[] = {
+    {"+squared-error", LINEAR, SQUARED_ERROR, SQUARED_ERROR},
+    {"+binary-ce", LOGISTIC, CROSS_ENTROPY_BINARY, CLASSIFICATION_BINARY},
+    {"+soft-targets", SOFTMAX_DIST, CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED, CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED}};
+
+static bool EndsWith(const std::string& s, const std::string& suffix) {
+  return s.size() > suffix.size() && s.compare(s.size() - suffix.size(), suffix.size(), suffix) == 0;
+}
+
 ModelConfig BuildModel(const std::string& name) {
+  for (const OutputSuffix& o : kOutputSuffixes) {
+    if (!EndsWith(name, o.suffix)) continue;
+    ModelConfig m = BuildModel(name.substr(0, name.size() - std::string(o.suffix).size()));
+    LayerConfig& out = m.layer.back();
+    if (out.activation != SOFTMAX || out.loss_function != CROSS_ENTROPY_MULTINOMIAL)
+      throw std::invalid_argument("model '" + name + "': one output suffix only (+squared-error, +binary-ce, +soft-targets)");
+    out.activation = o.act; out.loss_function = o.loss; out.performance_metric = o.metric;
+    return m;
+  }
+  if (EndsWith(name, "+logistic")) {
+    ModelConfig m = BuildModel(name.substr(0, name.size() - 9));
+    UseLogisticUnits(name, m);
+    return m;
+  }
   for (const auto& [suffix, type] : {std::make_pair(std::string("+adagrad"), (int)ADAGRAD_SGD),
                                      std::make_pair(std::string("+rmsprop"), (int)RMSPROP_SGD)}) {
     if (name.size() > suffix.size() && name.compare(name.size() - suffix.size(), suffix.size(), suffix) == 0) {
@@ -268,6 +334,7 @@ ModelConfig BuildModel(const std::string& name) {
     return m;
   }
   if (name == "gradcheck") return BuildGradCheckNet();
+  if (name == "logcheck") return BuildLogCheckNet();
   if (name == "alexnet") return BuildAlexNet();
   if (name == "lenet") return BuildLeNet();
   if (name == "c3d") return BuildC3D();
@@ -275,6 +342,8 @@ ModelConfig BuildModel(const std::string& name) {
   if (name == "lcnet") return BuildLcNet();
   if (name == "localcheck") return BuildLocalCheckNet();
   if (name == "invalid:local3d") return BuildLocal3DNet();     // test-only, refused by ConvNet (see above)
+  ModelConfig invalid;
+  if (name.rfind("invalid:", 0) == 0 && BuildInvalidOutputNet(name.substr(8), &invalid)) return invalid;
   throw std::invalid_argument("unknown model '" + name + "'");
 }
 

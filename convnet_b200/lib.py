@@ -72,6 +72,7 @@ SIGNATURES = {
     "convnet_b200_last_conv_path": [],
     "convnet_b200_launch_count": [],
     "convnet_b200_fuse_next": [FP, I, FP],
+    "convnet_b200_fuse_next_act": [FP, I, FP],
     "convnet_b200_bf16_stage": [FP, ct.c_longlong],
     "convnet_b200_bf16_ensure": [FP, ct.c_longlong],
     "convnet_b200_bf16_is_staged": [FP, ct.c_longlong],
@@ -100,6 +101,10 @@ SIGNATURES = {
     "cnb_softmax": [FP, I, I],
     "cnb_softmax_ce_deriv": [FP, FP, FP, FP, I, I],
     "cnb_sum": [FP, FP, I],
+    "cnb_logistic": [FP, ct.c_longlong],
+    "cnb_logistic_deriv": [FP, FP, ct.c_longlong],
+    "cnb_loss_deriv": [I, FP, FP, FP, FP, FP, I, I, F],
+    "cnb_metric": [I, FP, FP, FP, FP, I, I],
     "cnb_bn_stats": [FP, ct.c_longlong, I, F, F, FP, FP, FP, FP],
     "cnb_bn_apply": [FP, FP, ct.c_longlong, I, FP, FP, FP, FP, I],
     "cnb_bn_backward": [FP, FP, ct.c_longlong, I, FP, FP, FP, I, FP, FP],

@@ -87,6 +87,9 @@ def load_host():
             "cnb_model_param_layout": ([ct.c_char_p, i, i, ct.POINTER(ll), ct.POINTER(ll), ct.POINTER(ll)], i),
             "cnb_model_bn_layer": ([ct.c_char_p, i, ct.c_char_p, ct.POINTER(i), ct.POINTER(f), ct.POINTER(f),
                                     ct.POINTER(OptimizerConfig), ct.POINTER(OptimizerConfig)], i),
+            "cnb_net_targets": ([vp], vp), "cnb_net_targets_floats": ([vp], ll), "cnb_net_metric": ([vp], f),
+            "cnb_model_output_layer": ([ct.c_char_p, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(f),
+                                        ct.POINTER(i)], i),
         }
         for name, (args, res) in sig.items():
             fn = getattr(H, name)
@@ -104,7 +107,11 @@ class Net:
     "+adagrad" / "+rmsprop": every weight, bias, gamma and beta optimizer on ADAGRAD_SGD (adagrad_delta 1, epsilon x 0.1) /
     RMSPROP_SGD (rms_prop_factor 0.9, epsilon x 0.01); they compose with the others ("alexnet+ref-optimizer+rmsprop",
     "tiny+bn+adagrad").
-    "+gradcheck": run_grad_check's edge flags (e.g. "tiny+bn+gradcheck")."""
+    "+gradcheck": run_grad_check's edge flags (e.g. "tiny+bn+gradcheck").
+    "+logistic": every hidden RECTIFIED_LINEAR layer becomes LOGISTIC (same parameters; "alexnet+logistic", "tiny+bn+logistic").
+    One output suffix at most: "+squared-error" (LINEAR output, SQUARED_ERROR), "+binary-ce" (LOGISTIC output,
+    CROSS_ENTROPY_BINARY, metric CLASSIFICATION_BINARY), "+soft-targets" (SOFTMAX_DIST, CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED);
+    such outputs train on targets_tensor() instead of labels_tensor().  "logcheck": the gradcheck net with logistic units."""
 
     def __init__(self, model, batch_size, seed=42, grad_checker=False):
         self.H = load_host()
@@ -152,6 +159,12 @@ class Net:
     def output_tensor(self):
         return self._view(self.H.cnb_net_output(self.h), self.batch_size * self.num_classes, "f")
 
+    def targets_tensor(self):
+        """the output layer's float targets, column-major (element n + batch * j is feature j of image n), written by the
+        caller; None for an output layer trained on labels (labels_tensor())"""
+        n = self.H.cnb_net_targets_floats(self.h)
+        return self._view(self.H.cnb_net_targets(self.h), n, "f") if n else None
+
     def params_tensor(self):
         return self._view(self.H.cnb_net_params(self.h), self.num_params, "f")
 
@@ -178,7 +191,13 @@ class Net:
         self.H.cnb_net_update(self.h)
 
     def loss(self):
+        """loss_function_weight times the batch's loss under the output layer's loss function (after fprop)"""
         return self.H.cnb_net_loss(self.h)
+
+    def metric(self):
+        """the output layer's performance metric summed over the batch (after fprop): correct images for
+        CLASSIFICATION_MULTINOMIAL, the per-image share of correct features for CLASSIFICATION_BINARY, or a loss"""
+        return self.H.cnb_net_metric(self.h)
 
     # --- optimizer (SGDOptimizer, src/optimizer.cc): one for the weights and one for the bias of every weighted edge
     def _edge_index(self, edge):
@@ -336,6 +355,22 @@ def model_bn_layers(model):
         i += 1
 
 
+ACTIVATIONS = ("LINEAR", "RECTIFIED_LINEAR", "SOFTMAX", "LOGISTIC", "SOFTMAX_DIST")
+LOSS_FUNCTIONS = ("SQUARED_ERROR", "LINEAR_ERROR", "CROSS_ENTROPY_MULTINOMIAL", "CROSS_ENTROPY_BINARY",
+                  "CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED", "CLASSIFICATION_MULTINOMIAL", "CLASSIFICATION_BINARY",
+                  "HINGE_LINEAR", "HINGE_QUADRATIC")
+
+
+def model_output_layer(model):
+    """the output layer a model configures (host-only): {"activation", "loss_function", "performance_metric" (names),
+    "loss_function_weight", "labels" (True: trained on integer labels, False: on float targets)}"""
+    a, lf, pm, lab, w = ct.c_int(0), ct.c_int(0), ct.c_int(0), ct.c_int(0), ct.c_float(0)
+    if load_host().cnb_model_output_layer(model.encode(), ct.byref(a), ct.byref(lf), ct.byref(pm), ct.byref(w), ct.byref(lab)):
+        raise ValueError("unknown model %r (see stderr)" % model)
+    return {"activation": ACTIVATIONS[a.value], "loss_function": LOSS_FUNCTIONS[lf.value],
+            "performance_metric": LOSS_FUNCTIONS[pm.value], "loss_function_weight": w.value, "labels": bool(lab.value)}
+
+
 def model_param_layout(model, batch=1):
     """the flat parameter buffer of a model (host-only): {"edge_offsets": [...], "bn_offsets": per layer (None: not
     batch-normalised), "total": floats with padding}"""
@@ -425,3 +460,6 @@ def view_offset(multiplicity_id, max_offset_x, max_offset_y):
     w, h = ct.c_int(0), ct.c_int(0)
     H.cnb_data_view_offset(multiplicity_id, max_offset_x, max_offset_y, ct.byref(w), ct.byref(h))
     return w.value, h.value
+
+
+Net.model_output_layer = staticmethod(model_output_layer)

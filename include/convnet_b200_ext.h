@@ -101,6 +101,17 @@ void convnet_b200_release_workspace(void);
  *             on localDown* always as a pass at the end of the call.
  * Pass NULL / 0 for the parts not wanted.  Calls that cannot fuse (3-D dgrad) apply the same maths in a second pass. */
 void convnet_b200_fuse_next(const float* bias, int relu, const float* relu_mask);
+/* The same request with an activation code (CNB_ACT_*) in place of the ReLU flag:
+ *   act, fprop      (convUp*, localUp*): the activation after the bias — max(., 0), or the logistic sigma(.) of cnb_logistic
+ *                   (LogisticLayer::ApplyActivation, src/layer.cc:598); any fused dropout comes after it;
+ *   act_state, dgrad (convDown*, localDown*, MaxPoolUndo*, AvgPoolUndo*): the result times the derivative of `act` at the
+ *                   state act_state — the ReLU' mask as above, or (r * s) * (1 - s) as cnb_logistic_deriv computes it.  The
+ *                   pool-undo kernels and localDown* apply sigma' as a pass at the end of the call.
+ * Results are bit-identical to the unfused call followed by cnb_relu / cnb_logistic (fprop) or cnb_relu_deriv /
+ * cnb_logistic_deriv (dgrad).  convnet_b200_fuse_next(bias, relu, relu_mask) is fuse_next_act(bias, relu ? 1 : 0, ...) for
+ * fprop and fuse_next_act(NULL, 1, relu_mask) for the derivative. */
+enum { CNB_ACT_LINEAR = 0, CNB_ACT_RELU = 1, CNB_ACT_LOGISTIC = 2 };
+void convnet_b200_fuse_next_act(const float* bias, int act, const float* act_state);
 
 /* bf16 operand staging (precision mode 2 only; no-ops in the other modes).  In bf16 mode every conv call first rounds
  * its two fp32 operands to bf16 copies.  A caller that knows a tensor stays unchanged across several conv calls
@@ -154,6 +165,36 @@ void cnb_softmax(float* x, int rows, int cols);
  * (CrossEntropyMultinomial, src/loss_functions.cc:70-95) */
 void cnb_softmax_ce_deriv(const float* probs, const int* labels, float* deriv, float* loss_per_image,
                           int rows, int cols);
+/* the logistic unit (LogisticLayer, src/layer.cc:586-602):  x = 1 / (1 + expf(-x));  dx = (dx * y) * (1 - y).
+ * Arithmetic: every operation rounded to nearest, expf within 2 ulp (CUDA Programming Guide), so
+ *   |cnb_logistic(x) - sigma(x)| <= 3 * 2^-23 * sigma(x) + 2^-126            (sigma(x) = 0 below x = -88.7: expf overflows)
+ *   |cnb_logistic_deriv - dx * y * (1 - y)| <= 3 * 2^-24 * |dx * y * (1 - y)| + 2^-148
+ * The reference's CUDA uses __expf (cudamat_kernels.cu:146-148) and its derivative a * b * (1.0 - b) in double after
+ * the first product (:810-816); the fused conv epilogues (convnet_b200_fuse_next_act) use exactly these functions.
+ * Both honour convnet_b200_emit_bf16_next. */
+void cnb_logistic(float* x, long long n);
+void cnb_logistic_deriv(float* dx, const float* y, long long n);
+/* loss functions and performance metrics of an output layer (proto/convnet_config.proto LossFunction numbers;
+ * src/loss_functions.cc).  y, targets, deriv: column-major [rows = images x cols], images fastest (any number of pixels
+ * per image).  labels: `rows` ints (CROSS_ENTROPY_MULTINOMIAL, CLASSIFICATION_MULTINOMIAL); targets: per-feature floats
+ * (the others).  Per image, summed over its columns in order (DESIGN.md §5 has every rule):
+ *   SQUARED_ERROR 0.5 * sum (y - t)^2;  LINEAR_ERROR sum (y - t);  CROSS_ENTROPY_MULTINOMIAL -log y[label];
+ *   CROSS_ENTROPY_BINARY sum over t >= 0 of -t log(y + 1e-10) - (1 - t) log(1 - y + 1e-10);
+ *   CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED sum -t log(y + 1e-10);
+ *   CLASSIFICATION_MULTINOMIAL 1 if the argmax (kSoftMaxCorrectRowMajor's) is the label, else 0;
+ *   CLASSIFICATION_BINARY the share of features with t >= 0 where (t >= .5) == (y >= .5).
+ * cnb_loss_deriv writes deriv = weight * dLoss/dy ((y - t) | 1 | y - onehot; 0 where a binary target is < 0) and the
+ * per-image loss (NOT weighted: the caller scales the sum, as Layer::GetLoss does); CROSS_ENTROPY_MULTINOMIAL with weight 1
+ * is exactly cnb_softmax_ce_deriv.  cnb_metric writes the per-image value of a metric or a loss. */
+enum {
+  CNB_LOSS_SQUARED_ERROR = 0, CNB_LOSS_LINEAR_ERROR = 1, CNB_LOSS_CROSS_ENTROPY_MULTINOMIAL = 2,
+  CNB_LOSS_CROSS_ENTROPY_BINARY = 3, CNB_LOSS_CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED = 4,
+  CNB_LOSS_CLASSIFICATION_MULTINOMIAL = 5, CNB_LOSS_CLASSIFICATION_BINARY = 6
+};
+void cnb_loss_deriv(int loss, const float* y, const float* targets, const int* labels, float* deriv, float* loss_per_image,
+                    int rows, int cols, float weight);
+void cnb_metric(int metric, const float* y, const float* targets, const int* labels, float* metric_per_image, int rows,
+                int cols);
 /* *out = sum(a[0..n)) on the device (no host sync) */
 void cnb_sum(const float* a, float* out, int n);
 /* SGD with momentum and L2 decay, one fused pass (src/optimizer.cc:174-200):

@@ -260,11 +260,20 @@ def hash_u32(x):
         return ((x ^ (x >> np.uint64(31))) >> np.uint64(32)).astype(np.uint32)
 
 
-def dropout_kept(n, prob, seed):
-    """bool[n]: element i of the target is kept (hash(seed + i) * 2^-32 >= prob, in float32 as the kernel computes it)"""
-    idx = np.arange(n, dtype=np.uint64) + np.uint64(seed)
-    u = hash_u32(idx).astype(np.float32) * np.float32(2.0 ** -32)
-    return u >= np.float32(prob)
+def dropout_u(seed, idx):
+    """float32 u of the elements idx: float32(hash(seed + i)) * 2^-32, the conversion rounded to nearest (so u can be
+    1.0), the seed wrapping modulo 2^64"""
+    with np.errstate(over="ignore"):
+        x = np.asarray(idx, dtype=np.uint64) + np.uint64(seed)
+    return hash_u32(x).astype(np.float32) * np.float32(2.0 ** -32)
+
+
+def dropout_kept(n, prob, seed, return_u=False):
+    """bool[n]: element i of the target is kept (hash(seed + i) * 2^-32 >= prob, in float32 as the kernel computes it);
+    with return_u also the u of every element"""
+    u = dropout_u(seed, np.arange(n, dtype=np.uint64))
+    kept = u >= np.float32(prob)
+    return (kept, u) if return_u else kept
 
 
 # ---------------------------------------------------------------------------------------------------------------------

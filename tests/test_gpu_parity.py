@@ -461,27 +461,6 @@ def test_full_size_pool_rnorm_properties(gpu):
     assert abs(fd - an) < 2e-3 * np.sqrt(v.numel()), (fd, an)
 
 
-def test_elementwise_helpers(gpu):
-    torch = gpu.torch
-    L = gpu.lib.load()
-    rows, cols = 4 * 1000 + 0, 37
-    a = torch.randn(cols, rows, device="cuda")           # column-major [rows x cols]
-    b = torch.randn(cols, device="cuda")
-    x = a.clone(); L.cnb_add_channel_bias(x.data_ptr(), b.data_ptr(), rows, cols)
-    assert torch.allclose(x, a + b[:, None])
-    x = a.clone(); L.cnb_add_channel_bias_relu(x.data_ptr(), b.data_ptr(), rows, cols)
-    assert torch.allclose(x, torch.relu(a + b[:, None]))
-    gb = torch.full((cols,), float("nan"), device="cuda")
-    L.cnb_channel_bias_grad(a.data_ptr(), gb.data_ptr(), rows, cols, 0.0, 0.5)
-    assert torch.allclose(gb, 0.5 * a.sum(1), rtol=1e-4, atol=1e-3)
-    y = torch.relu(a); dx = torch.randn_like(a); ref = dx * (y > 0)
-    L.cnb_relu_deriv(dx.data_ptr(), y.data_ptr(), a.numel()); assert torch.equal(dx, ref)
-    w, h, g_ = torch.randn(1001, device="cuda"), torch.randn(1001, device="cuda"), torch.randn(1001, device="cuda")
-    h2 = 0.9 * h + 0.01 * (g_ + 5e-4 * w); w2 = w - h2
-    L.cnb_sgd_momentum(w.data_ptr(), h.data_ptr(), g_.data_ptr(), 1001, 0.01, 0.9, 5e-4)
-    assert torch.allclose(w, w2, atol=1e-6) and torch.allclose(h, h2, atol=1e-6)
-
-
 @pytest.mark.parametrize("mode", ["fp32", "tf32", "bf16"])
 def test_fused_epilogues(gpu, oracle, mode):
     """convnet_b200_fuse_next: bias + ReLU in the fprop epilogue, ReLU' mask in dgrad / pool-undo epilogues must equal the

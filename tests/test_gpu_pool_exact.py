@@ -16,12 +16,11 @@ import pytest
 import torch
 
 import pool_exact as px
+from gpu_buffers import check_twin as _check_twin, guards_ok as _guards_ok, launched as _launched, matrix as _matrix
 from pool_exact import PG
 
 pytestmark = pytest.mark.gpu
 
-SENTINEL = 0x7FC0DEAD
-GUARD = 64
 WORST = {}                 # (op, branch) -> largest |err|/bar
 
 
@@ -234,22 +233,9 @@ def hygiene(env):
         env.L.cnb_relu_deriv(None, None, 0)           # consumes any fuse request a failed call left pending
 
 
-def _matrix(rows, cols, s4, offset=0, guard=GUARD):
-    from convnet_b200.matrix import CUDAMatrix
-    n = rows * cols
-    buf = torch.empty(offset + n + guard, dtype=torch.float32, device="cuda")
-    buf.view(torch.int32).fill_(SENTINEL)
-    return CUDAMatrix(rows, cols, s4, storage=buf[offset:offset + n]), buf
-
-
 def _fill(m, values):
     m.storage.copy_(values)
     return m
-
-
-def _guards_ok(buf, offset, n):
-    s = buf.view(torch.int32)
-    return bool((s[:offset] == SENTINEL).all()) and bool((s[offset + n:] == SENTINEL).all())
 
 
 def _dyadic(n, gen, lo=-8, hi=9):
@@ -258,36 +244,6 @@ def _dyadic(n, gen, lo=-8, hi=9):
 
 def _note(op, branch, v):
     WORST[(op, branch)] = max(WORST.get((op, branch), 0.0), v.worst)
-
-
-def _launched(env, fn):
-    env.L.convnet_b200_reset_launch_count()
-    fn()
-    n = int(env.L.convnet_b200_launch_count())
-    torch.cuda.synchronize()
-    return n
-
-
-def _check_twin(env, m, shape):
-    """the staged bf16 copy of m, read exactly by a bf16 1x1 conv with identity filters (no conversion launch), must be
-    the round-to-nearest-even bf16 of m's fp32 values"""
-    from conv_exact import Geo
-    L = env.L
-    N, W, H, C = shape
-    n = N * W * H * C
-    assert L.convnet_b200_bf16_is_staged(m.ptr, n) == 1, "no staged twin"
-    g2 = Geo(N, W, H, C, C, 1, 1)
-    flt, _ = _matrix(*g2.flt_dims(), g2.flt_shape(), guard=0)
-    flt.storage.copy_(torch.eye(C, device="cuda").reshape(-1))
-    L.convnet_b200_bf16_stage(flt.ptr, C * C)
-    res, _ = _matrix(*g2.out_dims(), g2.out_shape(), guard=0)
-    launches = _launched(env, lambda: env.cg.convUp(m, flt, res, g2.desc()))
-    assert env.lib.last_conv_path() == "tc-bf16", env.lib.last_conv_path()
-    want = px.bf16_rne(m.storage[:n])
-    assert torch.equal(res.storage[:n].view(torch.int32), want.view(torch.int32)), "bf16 twin is not RNE of the output"
-    # the same conv on an explicitly staged copy launches as many kernels: the twin saved the conversion
-    L.convnet_b200_bf16_stage(m.ptr, n)
-    assert _launched(env, lambda: env.cg.convUp(m, flt, res, g2.desc())) == launches
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -71,8 +71,8 @@ API void cnb_net_reduce_learning_rate(void* p, float factor) { ((NetHandle*)p)->
 
 // ---- optimizer settings (edge.h OptimizerConfig: proto Optimizer, SGD fields).  which: 0 the weights, 1 the bias.
 static EdgeWithWeight* WeightedEdge(void* p, int edge) {
-  std::vector<Edge*>& e = ((NetHandle*)p)->net->Edges();
-  return edge >= 0 && edge < (int)e.size() ? dynamic_cast<EdgeWithWeight*>(e[edge]) : nullptr;
+  auto& e = ((NetHandle*)p)->net->Edges();
+  return edge >= 0 && edge < (int)e.size() ? dynamic_cast<EdgeWithWeight*>(e[edge].get()) : nullptr;
 }
 // replaces the settings of one optimizer (its step count and momentum history stay).  0 ok, -1 no such weighted edge,
 // -2 a config the SGD path cannot run (see OptimizerConfigError, printed on stderr)
@@ -103,8 +103,8 @@ API int cnb_optimizer_schedule(const OptimizerConfig* c, long long step, float* 
 
 // ---- batch normalisation (convnet.h Layer).  layer: index into the chain (0 = input).  which: 0 gamma, 1 beta.
 static Layer* BnLayer(void* p, int layer) {
-  std::vector<Layer*>& l = ((NetHandle*)p)->net->Layers();
-  return layer >= 0 && layer < (int)l.size() && l[layer]->BatchNormalize() ? l[layer] : nullptr;
+  auto& l = ((NetHandle*)p)->net->Layers();
+  return layer >= 0 && layer < (int)l.size() && l[layer]->BatchNormalize() ? l[layer].get() : nullptr;
 }
 API const char* cnb_net_layer_name(void* p, int i) { return ((NetHandle*)p)->net->Layers()[i]->GetName().c_str(); }
 API int cnb_net_layer_channels(void* p, int i) { return ((NetHandle*)p)->net->Layers()[i]->GetNumChannels(); }
@@ -211,7 +211,7 @@ API int cnb_model_edge_params(const char* model, int batch, int cap, long long* 
   ConvNet* net = TryBuildNet(model, batch);
   if (!net) return -1;
   int n = 0;
-  for (Edge* e : net->Edges()) { if (n >= cap) break; sizes[n++] = (long long)e->GetParameterMemoryRequirement(); }
+  for (auto& e : net->Edges()) { if (n >= cap) break; sizes[n++] = (long long)e->GetParameterMemoryRequirement(); }
   delete net;
   return n;
 }
@@ -227,6 +227,25 @@ API int cnb_model_param_layout(const char* model, int batch, int cap, long long*
   for (int i = 0; i < n && i < cap; i++) edge_offsets[i] = (long long)net->EdgeOffsets()[i];
   for (int i = 0; i <= n && i < cap; i++) bn_offsets[i] = net->BnOffsets()[i];
   *total = (long long)net->NumParameters();
+  delete net;
+  return n;
+}
+// static description of a model: the epilogue fusion ConvNet::PlanFusion decides.  Returns the number of edges E (-1:
+// unknown model); fills, up to `cap` entries each, per edge up_act / down_act[0, E) (the CNB_ACT_* code ComputeUp applies,
+// and the one whose derivative ComputeDown applies) and flags[0, E) (Edge::FusionPlan: bit 0 dropout_up, 1 scale_down,
+// 2 sums_bias_below, 3 offers_bias_grad), and per layer passes[0, E] (bit 0: a separate activation pass remains, bit 1:
+// a separate derivative pass remains)
+API int cnb_model_fusion(const char* model, int batch, int cap, int* up_act, int* down_act, int* flags, int* passes) {
+  ConvNet* net = TryBuildNet(model, batch);
+  if (!net) return -1;
+  const int n = (int)net->Edges().size();
+  for (int i = 0; i < n && i < cap; i++) {
+    const Edge::FusionPlan& p = net->Edges()[i]->Plan();
+    up_act[i] = p.up_act; down_act[i] = p.down_act;
+    flags[i] = p.dropout_up | p.scale_down << 1 | p.sums_bias_below << 2 | p.offers_bias_grad << 3;
+  }
+  for (int i = 0; i <= n && i < cap; i++)
+    passes[i] = net->Layers()[i]->HasSeparateActivationPass() | net->Layers()[i]->HasSeparateDerivPass() << 1;
   delete net;
   return n;
 }

@@ -89,7 +89,7 @@ std::string LayerConfigError(const LayerConfig& c) {
   return "";
 }
 
-// `emit`: this call is the last writer of the tensor and the next conv edge reads it as bf16 (see Edge::SetEmitUp)
+// `emit`: this call is the last writer of the tensor and the next conv edge reads it as bf16 (see LastStateWriter)
 void Layer::ApplyActivation(bool emit) {
   if (activation_fused_) return;
   switch (config_.activation) {
@@ -130,7 +130,6 @@ unsigned long long Layer::DropoutSeed(unsigned long long step, unsigned long lon
 }
 void Layer::ApplyDerivativeofDropout(bool emit) {
   if (config_.dropprob <= 0 || config_.is_input) return;
-  if (dropout_deriv_folded_) { dropout_deriv_folded_ = false; return; }    // the dgrad above already applied 1/(1-p) * [state > 0]
   if (emit) convnet_b200_emit_bf16_next();
   cnb_mult(deriv_.GetDevData(), dropout_mask_.GetDevData(), (long long)deriv_.GetNumEls());
 }
@@ -304,31 +303,14 @@ void DataParallelSync::AllReduceAverageAsync(float* buf, size_t offset, size_t c
 ConvNet::ConvNet(const ModelConfig& model, int batch_size) : model_(model), batch_size_(batch_size) {
   // BuildNet (convnet.cc:150-270), restricted to chains: edge i connects layer i to layer i+1
   if (model.layer.size() != model.edge.size() + 1) { fprintf(stderr, "ConvNet: model must be a chain\n"); exit(1); }
-  for (const LayerConfig& lc : model.layer) layers_.push_back(new Layer(lc));
+  for (const LayerConfig& lc : model.layer) layers_.emplace_back(new Layer(lc));
   for (size_t i = 0; i < model.edge.size(); i++) {
-    Edge* e = Edge::ChooseEdgeClass(model.edge[i]);
-    e->SetSource(layers_[i]); e->SetDest(layers_[i + 1]);
+    edges_.emplace_back(Edge::ChooseEdgeClass(model.edge[i]));
+    Edge* e = edges_.back().get();
+    e->SetSource(layers_[i].get()); e->SetDest(layers_[i + 1].get());
     e->SetInputChannels(layers_[i]->GetNumChannels());
     e->SetOutputChannels(layers_[i + 1]->GetNumChannels());
     e->SetBatchSize(batch_size);
-    edges_.push_back(e);
-  }
-  for (const LayerConfig& lc : model.layer) {        // activations, loss functions and metrics this class cannot run
-    const std::string why = LayerConfigError(lc);
-    if (why.empty()) continue;
-    for (Edge* e : edges_) delete e;
-    for (Layer* x : layers_) delete x;
-    throw std::invalid_argument("layer '" + lc.name + "': " + why);
-  }
-  // epilogue fusion of the Layer-side activation (ReLU, logistic) and its derivative into the neighbouring edges
-  // (SURVEY.md 8(f) rank 2)
-  for (size_t i = 0; i < edges_.size(); i++) {
-    Layer *src = layers_[i], *dst = layers_[i + 1];
-    const int up = ActCode(dst->GetActivation()), down = src->IsInput() ? CNB_ACT_LINEAR : ActCode(src->GetActivation());
-    edges_[i]->SetFuseActs(up, down);
-    // honoured only where CanFuseReLU() / CanFuseLogistic() (checked after SetImageSize below)
-    if (up != CNB_ACT_LINEAR) edges_[i]->SetFuseReLU(true);
-    if (down != CNB_ACT_LINEAR) edges_[i]->SetFuseMask(true);
   }
   // SetImageSize propagation (convnet.cc:226-268)
   const LayerConfig& in = model.layer.front();
@@ -337,14 +319,20 @@ ConvNet::ConvNet(const ModelConfig& model, int batch_size) : model_(model), batc
     edges_[i]->SetImageSize(layers_[i]->GetSizeY(), layers_[i]->GetSizeX(), layers_[i]->GetSizeT());
     layers_[i + 1]->SetSize(edges_[i]->GetNumModulesY(), edges_[i]->GetNumModulesX(), edges_[i]->GetNumModulesT());
   }
-  for (size_t i = 0; i < edges_.size(); i++) {       // the untied conv kernels are 2-D only
-    if (model.edge[i].edge_type != LOCAL || layers_[i]->GetSizeT() == 1) continue;
-    const std::string msg = "edge '" + edges_[i]->GetName() + "': LOCAL is not supported on 3-D layers (image_size_t > 1)";
-    for (Edge* e : edges_) delete e;
-    for (Layer* x : layers_) delete x;
-    throw std::invalid_argument(msg);
+  const std::string why = Refusal();
+  if (!why.empty()) throw std::invalid_argument(why);
+  PlanFusion();
+}
+
+std::string ConvNet::Refusal() const {
+  for (const LayerConfig& lc : model_.layer) {       // activations, loss functions and metrics this class cannot run
+    const std::string why = LayerConfigError(lc);
+    if (!why.empty()) return "layer '" + lc.name + "': " + why;
   }
-  for (Layer* l : layers_) {                          // what the batch-norm passes cannot run is refused here
+  for (size_t i = 0; i < edges_.size(); i++)         // the untied conv kernels are 2-D only
+    if (model_.edge[i].edge_type == LOCAL && layers_[i]->GetSizeT() != 1)
+      return "edge '" + edges_[i]->GetName() + "': LOCAL is not supported on 3-D layers (image_size_t > 1)";
+  for (const auto& l : layers_) {                    // what the batch-norm passes cannot run
     if (!l->BatchNormalize()) continue;
     std::string why;
     if (l->IsInput() || l->IsOutput()) why = "is not supported on the input or output layer";
@@ -352,25 +340,38 @@ ConvNet::ConvNet(const ModelConfig& model, int batch_size) : model_(model), batc
     for (int which = 0; which < 2 && why.empty(); which++)
       if (const char* err = BnOptimizerConfigError(l->BnOptimizer(which)))
         why = std::string(which ? "beta" : "gamma") + "_optimizer: " + err;
-    if (!why.empty()) {
-      const std::string msg = "layer '" + l->GetName() + "': batch_normalize " + why;
-      for (Edge* e : edges_) delete e;
-      for (Layer* x : layers_) delete x;
-      throw std::invalid_argument(msg);
-    }
+    if (!why.empty()) return "layer '" + l->GetName() + "': batch_normalize " + why;
   }
-  for (size_t i = 0; i < edges_.size(); i++) {       // settle the fusion flags now that shapes are known
-    Edge* e = edges_[i];
+  return "";
+}
+
+// Epilogue fusion of the layers' activation (ReLU, logistic), its derivative and the dropout into the neighbouring
+// edges (SURVEY.md 8(f) rank 2)
+void ConvNet::PlanFusion() {
+  // CONVNET_B200_NO_FUSED_DROPOUT=1, _NO_DROPOUT_FOLD=1, _NO_PRESTAGE=1: the separate passes these fusions replace (the
+  // reference run of tests/test_gpu_staging.py).  Read once per process
+  auto on = [](const char* name) { const char* v = getenv(name); return !(v && v[0] == '1'); };
+  static const bool fused_dropout = on("CONVNET_B200_NO_FUSED_DROPOUT"), dropout_fold = on("CONVNET_B200_NO_DROPOUT_FOLD"),
+                    prestage = on("CONVNET_B200_NO_PRESTAGE");
+  prestage_ = prestage;
+  for (size_t i = 0; i < edges_.size(); i++) {
+    Edge* e = edges_[i].get();
+    Layer *src = layers_[i].get(), *dst = layers_[i + 1].get();
+    const Edge::Absorbs a = e->CanAbsorb();
+    // the activation of a layer rides where the kernel applies ReLU, and sigma only where it can apply sigma too
+    auto fused = [&a](int act, bool can) { return act != CNB_ACT_LINEAR && can && (act == CNB_ACT_RELU || a.logistic); };
+    const int up = ActCode(dst->GetActivation()), down = src->IsInput() ? CNB_ACT_LINEAR : ActCode(src->GetActivation());
+    Edge::FusionPlan p;
     // a batch-normalised layer: the edge writes the pre-normalisation input, the BN pass applies the activation
-    const bool bn = layers_[i + 1]->BatchNormalize();
-    const int up = ActCode(layers_[i + 1]->GetActivation()), down = ActCode(layers_[i]->GetActivation());
-    const bool act = !bn && up != CNB_ACT_LINEAR && e->CanFuseReLU() && e->WantsFuseReLU() &&
-                     (up == CNB_ACT_RELU || e->CanFuseLogistic());
-    e->SetFuseReLU(act);
-    layers_[i + 1]->SetActivationFused(act || bn);
-    const bool mask = e->CanFuseMask() && e->WantsFuseMask() && (down == CNB_ACT_RELU || e->CanFuseLogistic());
-    e->SetFuseMask(mask);
-    layers_[i]->SetDerivFused(mask);
+    if (!dst->BatchNormalize() && fused(up, a.act_up)) p.up_act = up;
+    if (fused(down, a.act_down)) p.down_act = down;
+    p.dropout_up = a.dropout && p.up_act != CNB_ACT_LINEAR && fused_dropout;
+    p.scale_down = a.dropout && p.down_act != CNB_ACT_LINEAR && dropout_fold;
+    p.sums_bias_below = a.sums_bias_below;
+    p.offers_bias_grad = a.per_channel_bias;
+    e->SetFusionPlan(p);
+    dst->SetActivationFused(p.up_act != CNB_ACT_LINEAR || dst->BatchNormalize());
+    src->SetDerivFused(p.down_act != CNB_ACT_LINEAR);
   }
 }
 
@@ -392,8 +393,6 @@ ConvNet::~ConvNet() {
   for (std::vector<cudaEvent_t>* v : {&trace_.c0, &trace_.c1, &trace_.s1}) for (cudaEvent_t e : *v) cudaEventDestroy(e);
   convnet_b200_reserve_sms(0);
   convnet_b200_bf16_invalidate(nullptr);                     // the buffers go away; a later net may get the same addresses
-  for (Edge* e : edges_) delete e;
-  for (Layer* l : layers_) delete l;
 }
 
 // AllocateEdgeMemory (convnet.cc:272-298): one flat buffer, each edge's slice padded to 128 floats.  The [gamma | beta]
@@ -418,7 +417,7 @@ void ConvNet::PlanParameters() {
 }
 
 void ConvNet::AllocateMemory() {
-  for (Layer* l : layers_) l->AllocateMemory(batch_size_);
+  for (auto& l : layers_) l->AllocateMemory(batch_size_);
   PlanParameters();
   size_t total = num_params_;
   if (total == 0) total = 128;
@@ -448,8 +447,8 @@ void ConvNet::AllocateMemory() {
     layers_[i]->InitializeBn();
   }
   bool adaptive = false;
-  for (Edge* e : edges_)
-    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(e)) adaptive |= IsAdaptive(w->Optimizer(0)) || IsAdaptive(w->Optimizer(1));
+  for (auto& e : edges_)
+    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(e.get())) adaptive |= IsAdaptive(w->Optimizer(0)) || IsAdaptive(w->Optimizer(1));
   for (size_t i = 0; i < layers_.size(); i++)
     if (bn_offset_[i] >= 0) adaptive |= IsAdaptive(layers_[i]->BnOptimizer(0)) || IsAdaptive(layers_[i]->BnOptimizer(1));
   if (adaptive) AllocateAdaptiveState();
@@ -465,14 +464,14 @@ void ConvNet::AllocateMemory() {
   SetBucketFloats((size_t)8 << 20);
   lane_.stream = side_;
   HOST_CUDA_CHECK(cudaEventCreateWithFlags(&lane_.ready, cudaEventDisableTiming));
-  for (Edge* e : edges_)
-    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(e)) w->SetSideLane(&lane_);
+  for (auto& e : edges_)
+    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(e.get())) w->SetSideLane(&lane_);
 }
 
 void ConvNet::AllocateAdaptiveState() {
   state_.AllocateGPUMemory(1, parameters_.GetCols());
   for (size_t i = 0; i < edges_.size(); i++) {
-    EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i]);
+    EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i].get());
     if (!w || edge_size_[i] == 0) continue;
     Matrix s;
     state_.GetSlice(s, (int)edge_offset_[i], (int)(edge_offset_[i] + edge_size_[i]));
@@ -504,38 +503,52 @@ void ConvNet::SetBnOptimizer(Layer* l, int which, const OptimizerConfig& c) {
   else if (restart) l->InitBnState(which);
 }
 
+// The pass that writes a layer's state last in Fprop, or its derivative last in Bprop.  In bf16 mode it also writes the bf16
+// copy the next conv edge multiplies with (emit); a dgrad that writes a derivative last can also sum its channels, which
+// is the bias gradient of the edge below.
+enum class Writer { EDGE, BN, ACTIVATION, DROPOUT };
+// Fprop runs the edge (into the pre-normalisation input of a batch-normalised layer), BN apply (with the activation), the
+// activation pass, the dropout pass
+static Writer LastStateWriter(const Layer& l, bool dropout_pass) {
+  if (dropout_pass) return Writer::DROPOUT;
+  if (l.HasSeparateActivationPass()) return Writer::ACTIVATION;
+  if (l.BatchNormalize()) return Writer::BN;
+  return Writer::EDGE;
+}
+// Bprop runs the edge above, the dropout pass, the activation' pass, BN backward
+static Writer LastDerivWriter(const Layer& l, bool dropout_pass) {
+  if (l.BatchNormalize()) return Writer::BN;
+  if (l.HasSeparateDerivPass()) return Writer::ACTIVATION;
+  if (dropout_pass) return Writer::DROPOUT;
+  return Writer::EDGE;
+}
+
 void ConvNet::Fprop(bool train) {                            // convnet.cc:377-388
   const bool bf16 = convnet_b200_get_conv_precision() == 2;
   dropout_active_ = train;
   for (size_t i = 1; i < layers_.size(); i++) {
-    Layer* l = layers_[i];
-    Edge* e = edges_[i - 1];
-    // bf16 mode: whoever writes this layer's state LAST (dropout, else a separate activation pass, else the edge's own
-    // kernel) also writes the bf16 copy the next conv edge multiplies with
+    Layer* l = layers_[i].get();
+    Edge* e = edges_[i - 1].get();
     const bool want = bf16 && i < edges_.size() && edges_[i]->WantsBf16Input();
-    const bool act_pass = l->HasSeparateActivationPass();
-    // batch normalisation: the edge writes the layer's pre-normalisation input, the BN pass (with the activation) the state
-    const bool bn = l->BatchNormalize();
     // dropout inside the edge's epilogue (no mask tensor) when the backward pass will not need the mask either
-    static const bool no_fuse_drop = getenv("CONVNET_B200_NO_FUSED_DROPOUT") && getenv("CONVNET_B200_NO_FUSED_DROPOUT")[0] == '1';
-    const bool fuse_drop = train && l->HasDropout() && !no_fuse_drop && !act_pass && !bn && e->CanFuseDropout() && DropoutFolds(i);
-    if (fuse_drop) e->SetDropoutRequest(l->DropoutProb(), l->DropoutScale(), l->DropoutSeed(step_, dropout_salt_));
+    const bool fuse_drop = train && DropoutFolds(i) && e->Plan().dropout_up;
     const bool drop = train && l->HasDropout() && !fuse_drop;
-    e->SetEmitUp(want && !drop && !act_pass && !bn);
-    e->ComputeUp(layers_[i - 1]->GetState(), bn ? l->GetPreBN() : l->GetState(), /*overwrite=*/true, train);
-    if (bn) l->ApplyBatchNormalization(train, want && !drop);
-    l->ApplyActivation(want && !drop && act_pass);
-    if (!fuse_drop) l->ApplyDropout(train, step_, dropout_salt_, want && drop);
+    const Writer last = LastStateWriter(*l, drop);
+    Edge::UpRequest r;
+    r.emit = want && last == Writer::EDGE;
+    if (fuse_drop) { r.drop_prob = l->DropoutProb(); r.drop_scale = l->DropoutScale(); r.drop_seed = l->DropoutSeed(step_, dropout_salt_); }
+    e->Request(r);
+    e->ComputeUp(layers_[i - 1]->GetState(), l->BatchNormalize() ? l->GetPreBN() : l->GetState(), /*overwrite=*/true, train);
+    if (l->BatchNormalize()) l->ApplyBatchNormalization(train, want && last == Writer::BN);
+    l->ApplyActivation(want && last == Writer::ACTIVATION);
+    if (drop) l->ApplyDropout(train, step_, dropout_salt_, want && last == Writer::DROPOUT);
   }
 }
 
 bool ConvNet::DropoutFolds(size_t i) const {
-  static const bool no_fold = getenv("CONVNET_B200_NO_DROPOUT_FOLD") && getenv("CONVNET_B200_NO_DROPOUT_FOLD")[0] == '1';
-  if (no_fold || i == 0 || i >= edges_.size()) return false;        // edges_[i]: the edge whose ComputeDown writes layers_[i]'s derivative
-  const Layer* l = layers_[i];
-  // a ReLU or logistic layer: where the mask drops a unit its state is 0, and so is the derivative of the activation there
-  return l->HasDropout() && ActCode(l->GetActivation()) != CNB_ACT_LINEAR && !l->HasSeparateDerivPass() &&
-         edges_[i]->CanScaleDeriv();
+  // edges_[i]: the edge whose ComputeDown writes layers_[i]'s derivative.  Where the mask drops a unit of a ReLU or logistic
+  // layer its state is 0, and so is the derivative of the activation there
+  return i >= 1 && i < edges_.size() && layers_[i]->HasDropout() && edges_[i]->Plan().scale_down;
 }
 
 void ConvNet::ComputeDeriv() { OutputLayer().ComputeDeriv(); }
@@ -555,22 +568,24 @@ float ConvNet::GetPerformanceMetric() {
 
 void ConvNet::Bprop() {                                      // convnet.cc:390-405 + 362-375
   const bool bf16 = convnet_b200_get_conv_precision() == 2;
+  // a layer's dropout derivative is one factor on the kept units, which the fused act' of the dgrad above already selects:
+  // that dgrad scales by it when the last Fprop applied dropout; otherwise a pass multiplies by the mask
+  auto folds = [this](int k) { return dropout_active_ && DropoutFolds((size_t)k); };
+  auto dropout_pass = [&](int k) { return layers_[k]->HasDropout() && !folds(k); };
   for (int i = (int)layers_.size() - 1; i >= 1; i--) {
-    Layer* out = layers_[i];
-    Layer* in = layers_[i - 1];
-    Edge* e = edges_[i - 1];
-    // bf16 mode: the last writer of a derivative tensor (ReLU' pass, else dropout mask, else the ComputeDown of the edge
-    // above) leaves the bf16 copy the edge below reads in its wgrad and dgrad
-    // (the reference runs these two at the top of the NEXT loop iteration, i.e. before this layer's edges)
-    // batch normalisation: its backward pass follows and writes the derivative last; it produces the gamma / beta gradients
-    // before the ComputeOuter below, which makes this edge's bucket final
+    Layer* out = layers_[i].get();
+    Layer* in = layers_[i - 1].get();
+    Edge* e = edges_[i - 1].get();
+    // the derivative of `out` is final once its passes have run (the reference runs them at the top of the NEXT loop
+    // iteration, i.e. before this layer's edges); batch normalisation also produces the gamma / beta gradients before the
+    // ComputeOuter below, which makes this edge's bucket final
     if (!out->IsOutput()) {
-      const bool want_out = bf16 && e->WantsBf16Deriv();
-      const bool act_pass = out->HasSeparateDerivPass();
-      const bool bn = out->BatchNormalize();
-      out->ApplyDerivativeofDropout(want_out && !act_pass && !bn);
-      out->ApplyDerivativeOfActivation(want_out && act_pass && !bn);
-      if (bn) out->ApplyDerivativeofBatchNormalization(want_out);
+      const bool want = bf16 && e->WantsBf16Deriv();
+      const bool drop = dropout_pass(i);
+      const Writer last = LastDerivWriter(*out, drop);
+      if (drop) out->ApplyDerivativeofDropout(want && last == Writer::DROPOUT);
+      out->ApplyDerivativeOfActivation(want && last == Writer::ACTIVATION);
+      if (out->BatchNormalize()) out->ApplyDerivativeofBatchNormalization(want && last == Writer::BN);
     }
     e->ComputeOuter(in->GetState(), out->GetDeriv());
     // data parallel: ship every bucket whose last gradient just became final (side stream, overlaps the rest of bprop)
@@ -591,18 +606,13 @@ void ConvNet::Bprop() {                                      // convnet.cc:390-4
         comm_pending_ = true;
       }
     if (!in->IsInput()) {
-      const bool want_in = bf16 && i >= 2 && edges_[i - 2]->WantsBf16Deriv();
-      // dropout derivative of a ReLU layer = one factor on the kept units, which the fused mask already selects
-      const bool fold = dropout_active_ && in->HasDropout() && DropoutFolds((size_t)i - 1);
-      if (fold) { e->SetDerivScale(in->DropoutScale()); in->SetDropoutDerivFolded(true); }
-      const bool drop_pass = in->HasDropout() && !fold;
-      const bool last = !drop_pass && !in->HasSeparateDerivPass() && !in->BatchNormalize();   // this dgrad writes in's derivative last
-      e->SetEmitDown(want_in && last);
-      // the kernel that writes in's derivative LAST can also sum its channels: that is the bias gradient of the edge below
-      if (i >= 2 && e->CanProduceBiasGrad() && last) {
-        Edge::BiasGradTarget t;
-        if (edges_[i - 2]->OfferFusedBiasGrad(&t)) e->SetBiasGradRequest(t);
-      }
+      const bool last = LastDerivWriter(*in, dropout_pass(i - 1)) == Writer::EDGE;
+      EdgeWithWeight* below = i >= 2 ? dynamic_cast<EdgeWithWeight*>(edges_[i - 2].get()) : nullptr;
+      Edge::DownRequest r;
+      r.emit = bf16 && i >= 2 && edges_[i - 2]->WantsBf16Deriv() && last;
+      if (folds(i - 1)) r.scale = in->DropoutScale();
+      if (last && below && e->Plan().sums_bias_below && below->Plan().offers_bias_grad) r.bias_grad = below->HandOffBiasGrad();
+      e->Request(r);
       e->ComputeDown(out->GetDeriv(), in->GetState(), out->GetState(), in->GetDeriv(), /*overwrite=*/true);
     }
     // the optimizer step of a bucket follows its all-reduce on the side stream once its edges are done with the weights
@@ -623,7 +633,7 @@ void ConvNet::Bprop() {                                      // convnet.cc:390-4
 void ConvNet::IssueBucketUpdate(const Bucket& b) {
   std::vector<CnbOptTensorEx> tensors;
   for (int i = b.trigger; i <= b.last; i++) {
-    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i])) w->AppendSgdTensors(tensors);
+    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i].get())) w->AppendSgdTensors(tensors);
     layers_[i + 1]->AppendBnSgdTensors(tensors);               // gamma / beta of the layer edge i writes
   }
   if (tensors.empty()) return;
@@ -637,10 +647,9 @@ void ConvNet::IssueBucketUpdate(const Bucket& b) {
   // (PlanBuckets splits at edge boundaries, so every row of a tensor is updated in this one call)
   cnb_opt_update_multi(tensors.data(), (int)tensors.size());
   // what the next step's dgrad derives from these weights alone (bf16 filter banks): rebuilt here, behind the update
-  static const bool no_prestage = getenv("CONVNET_B200_NO_PRESTAGE") && getenv("CONVNET_B200_NO_PRESTAGE")[0] == '1';
-  if (!no_prestage)
+  if (prestage_)
     for (int i = b.trigger; i <= b.last; i++)
-      if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i])) w->PrestageDown();
+      if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i].get())) w->PrestageDown();
   convnet_b200_set_stream(main_stream);
   opt_pending_ = true;
 }
@@ -669,15 +678,15 @@ void ConvNet::UpdateWeights() {                              // convnet.cc:440-4
   // one multi-tensor launch for every weight and bias matrix of the net (the reference loops edges: optimizer.cc:174-279)
   std::vector<CnbOptTensorEx> tensors;
   for (size_t i = 0; i < edges_.size(); i++) {
-    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i])) w->AppendSgdTensors(tensors);
+    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i].get())) w->AppendSgdTensors(tensors);
     layers_[i + 1]->AppendBnSgdTensors(tensors);
   }
   cnb_opt_update_multi(tensors.data(), (int)tensors.size());
 }
 
 void ConvNet::ReduceLearningRate(float factor) {             // convnet.cc:820-825 (edges only: gamma / beta keep theirs)
-  for (Edge* e : edges_)
-    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(e)) w->ReduceLearningRate(factor);
+  for (auto& e : edges_)
+    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(e.get())) w->ReduceLearningRate(factor);
 }
 
 void ConvNet::TrainOneBatch(float* loss_out) {               // convnet.cc:475-485 (GetBatch is the caller's H2D copy)
@@ -767,7 +776,7 @@ void ConvNet::BroadcastParameters() {
 
 double ConvNet::FlopsFprop() const {
   double f = 0;
-  for (Edge* e : edges_) f += e->FlopsUp();
+  for (const auto& e : edges_) f += e->FlopsUp();
   return f;
 }
 double ConvNet::FlopsTrainStep() const {                     // BASELINE.md §2c: 3x fprop minus the dgrad into the input layer
@@ -777,8 +786,6 @@ double ConvNet::FlopsTrainStep() const {                     // BASELINE.md §2c
 }
 
 // =================================================================== GradChecker (src/grad_check.cc)
-float GradChecker::LossAt(Matrix& w, size_t index, float value) { return (float)LossAtD(w, index, value); }
-
 double GradChecker::LossAtD(Matrix& w, size_t index, float value) {
   w.WriteValue(index, value);
   InvalidateStaging();
@@ -832,9 +839,9 @@ std::vector<GradCheckResult> GradChecker::Run(unsigned seed) {
   Bprop();                                                    // analytical gradients now in grad_weights of each edge
 
   std::vector<GradCheckResult> results;
-  for (Edge* ed : edges_) {
+  for (auto& ed : edges_) {
     if (!ed->Config().grad_check) continue;
-    EdgeWithWeight* e = dynamic_cast<EdgeWithWeight*>(ed);
+    EdgeWithWeight* e = dynamic_cast<EdgeWithWeight*>(ed.get());
     if (!e) continue;
     std::vector<float> eps = ed->Config().grad_check_epsilon;
     if (eps.empty()) eps = {1e-2f, 1e-3f, 1e-4f};

@@ -68,12 +68,11 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   void ApplyActivation(bool emit_bf16 = false);               // layer.cc:545-560
   void ApplyDerivativeOfActivation(bool emit_bf16 = false);   // layer.cc:562-580
   void ApplyDropout(bool train, unsigned long long step, unsigned long long salt, bool emit_bf16 = false);   // layer.cc:  mask = rand > dropprob ; state *= mask
-  void ApplyDerivativeofDropout(bool emit_bf16 = false);
+  void ApplyDerivativeofDropout(bool emit_bf16 = false);        // unless ConvNet::DropoutFolds: the dgrad above scales instead
   bool HasDropout() const { return config_.dropprob > 0 && !config_.is_input; }
   float DropoutScale() const { return 1.0f / (1.0f - config_.dropprob); }
   float DropoutProb() const { return config_.dropprob; }
   unsigned long long DropoutSeed(unsigned long long step, unsigned long long salt) const;
-  void SetDropoutDerivFolded(bool v) { dropout_deriv_folded_ = v; }   // this step: the edge above scaled the derivative instead
   bool HasSeparateActivationPass() const { return ActCode(config_.activation) != CNB_ACT_LINEAR && !activation_fused_; }
   bool HasSeparateDerivPass() const { return ActCode(config_.activation) != CNB_ACT_LINEAR && !deriv_fused_; }
   // output layer: deriv = loss_function_weight * dLoss/dstate and the per-image loss (unweighted), layer.cc:426-437
@@ -126,7 +125,7 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   bool bn_train_ = false;                       // the last ApplyBatchNormalization used the batch statistics
   long long gamma_step_ = 0, beta_step_ = 0;
   int* labels_ = nullptr;
-  bool activation_fused_ = false, deriv_fused_ = false, dropout_deriv_folded_ = false;
+  bool activation_fused_ = false, deriv_fused_ = false;
 };
 
 // NCCL all-reduce of the flat gradient buffer, bucketed along edge boundaries and launched on a side
@@ -192,8 +191,8 @@ class ConvNet {
 
   Layer& InputLayer() { return *layers_.front(); }
   Layer& OutputLayer() { return *layers_.back(); }
-  std::vector<Edge*>& Edges() { return edges_; }
-  std::vector<Layer*>& Layers() { return layers_; }
+  std::vector<std::unique_ptr<Edge>>& Edges() { return edges_; }
+  std::vector<std::unique_ptr<Layer>>& Layers() { return layers_; }
   Matrix& Parameters() { return parameters_; }
   Matrix& GradParameters() { return grad_parameters_; }
   size_t NumParameters() const { return num_params_; }
@@ -212,8 +211,13 @@ class ConvNet {
  protected:
   ModelConfig model_;
   int batch_size_;
-  std::vector<Layer*> layers_;
-  std::vector<Edge*> edges_;                    // edges_[i]: layers_[i] -> layers_[i+1]
+  std::vector<std::unique_ptr<Layer>> layers_;
+  std::vector<std::unique_ptr<Edge>> edges_;    // edges_[i]: layers_[i] -> layers_[i+1]
+  std::string Refusal() const;                  // "" if this class can run the model, else why not
+  // which passes of the neighbouring layers ride in each edge's kernels (Edge::FusionPlan), once the shapes are known;
+  // also tells each layer whether its activation / derivative pass is left to do (Layer::SetActivationFused / SetDerivFused)
+  void PlanFusion();
+  bool prestage_ = true;                        // rebuild the dgrad banks behind each optimizer step (PrestageDown)
   Matrix parameters_, grad_parameters_, history_, loss_sum_, state_;
   void AllocateAdaptiveState();                 // state_ and its slices, each initialised for its optimizer
   std::vector<size_t> edge_offset_, edge_size_;
@@ -224,8 +228,9 @@ class ConvNet {
   // enqueued on side_, and once the bucket's edges have finished their dgrad the multi-tensor SGD step of that bucket
   // follows on the same stream — the exchange and the update of the FC layers hide under the conv back-propagation.
   void IssueBucketUpdate(const Bucket& b);
-  // layers_[i] is a ReLU layer with dropout whose derivative is written by a dgrad that can apply relu'(state) * 1/(1-p)
-  // itself: the backward pass needs no mask tensor, and the forward pass may fuse the dropout into the edge below
+  // layers_[i] is a ReLU or logistic layer with dropout whose derivative is written by a dgrad that applies
+  // act'(state) * 1/(1-p) itself: the backward pass needs no mask tensor, and the forward pass may fuse the dropout into
+  // the edge below
   bool DropoutFolds(size_t i) const;
   void WaitSide();
   DataParallelSync* dp_ = nullptr;
@@ -261,7 +266,6 @@ class GradChecker : public ConvNet {
   GradChecker(const ModelConfig& model, int batch_size) : ConvNet(model, batch_size) {}
   std::vector<GradCheckResult> Run(unsigned seed);
  private:
-  float LossAt(Matrix& w, size_t index, float value);
   double LossAtD(Matrix& w, size_t index, float value);
 };
 

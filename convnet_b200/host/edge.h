@@ -112,40 +112,41 @@ class Edge {
   void SetSource(Layer* l) { source_ = l; }
   void SetDest(Layer* l) { dest_ = l; }
   void SetBatchSize(int n) { batch_size_ = n; }
-  // Epilogue fusion (convnet_b200_fuse_next): the ReLU of the destination layer rides in ComputeUp's conv epilogue
-  // (together with the shared bias), the ReLU derivative of the source layer in ComputeDown's. ConvNet decides.
-  // The activation is that of the layer (CNB_ACT_*: ReLU or logistic): `up` the destination's, `down` the source's.  Where
-  // CanFuseReLU / CanFuseMask hold, the ReLU rides in the epilogue; the logistic unit only where CanFuseLogistic holds too
-  virtual bool CanFuseReLU() const { return false; }
-  virtual bool CanFuseMask() const { return false; }
-  virtual bool CanFuseLogistic() const { return false; }
-  void SetFuseActs(int up, int down) { up_act_ = up; down_act_ = down; }
-  void SetFuseReLU(bool v) { fuse_relu_ = v; }
-  void SetFuseMask(bool v) { fuse_mask_ = v; }
-  bool WantsFuseReLU() const { return fuse_relu_; }
-  bool WantsFuseMask() const { return fuse_mask_; }
-  // bf16 mode: the kernel that writes a tensor LAST also leaves its bf16 copy for the conv edge that reads it next
-  // (convnet_b200_emit_bf16_next) instead of that edge running a conversion pass.  ConvNet sets these before each call:
-  // emit_up: ComputeUp is the last writer of the destination state and the next edge multiplies in bf16;
-  // emit_down: ComputeDown is the last writer of the source layer's derivative and the edge below multiplies in bf16.
-  void SetEmitUp(bool v) { emit_up_ = v; }
-  void SetEmitDown(bool v) { emit_down_ = v; }
-  // Fused bias gradient: the edge ABOVE writes this edge's output derivative last, and its kernel can sum the channels
-  // while it stores them (convnet_b200_fuse_next_bias_grad).  ConvNet asks the lower edge for its target (which makes that
-  // edge skip its own SumRows in ComputeOuter) and hands it to the upper edge's ComputeDown.
+
+  // Epilogue fusion: passes of the neighbouring layers that ride in this edge's kernels (SURVEY.md 8(f) rank 2).
+  // What the kernels of this edge can absorb, once SetImageSize has fixed its shapes:
+  struct Absorbs {
+    bool act_up = false;           // ComputeUp: the destination's ReLU (after the bias, where there is one)
+    bool act_down = false;         // ComputeDown: the source's ReLU' mask
+    bool logistic = false;         // sigma / sigma' too, wherever the two above hold
+    bool dropout = false;          // behind a fused activation: the destination's dropout (ComputeUp), the source's
+                                   // dropout derivative as a scale (ComputeDown)
+    bool sums_bias_below = false;  // ComputeDown can sum the channels of the derivative it writes
+    bool per_channel_bias = false; // the bias gradient is that channel sum of this edge's output derivative
+  };
+  virtual Absorbs CanAbsorb() const { return Absorbs(); }
+  // What ConvNet::PlanFusion decided for this edge, fixed for the life of the net
+  struct FusionPlan {
+    int up_act = CNB_ACT_LINEAR;    // CNB_ACT_* that ComputeUp applies in its epilogue
+    int down_act = CNB_ACT_LINEAR;  // CNB_ACT_* whose derivative ComputeDown applies
+    bool dropout_up = false;        // the destination's dropout may ride in ComputeUp (UpRequest)
+    bool scale_down = false;        // the source's dropout derivative may fold into ComputeDown (DownRequest::scale)
+    bool sums_bias_below = false;   // ComputeDown may take the bias gradient of the edge below (DownRequest::bias_grad)
+    bool offers_bias_grad = false;  // the edge above may sum this edge's bias gradient
+  };
+  void SetFusionPlan(const FusionPlan& p) { plan_ = p; }
+  const FusionPlan& Plan() const { return plan_; }
+  // One-shot requests ConvNet makes before each ComputeUp / ComputeDown; the call consumes them.
+  // emit (bf16 mode): the call writes the tensor LAST and the next conv edge multiplies it in bf16, so the kernel leaves
+  // the bf16 copy too (convnet_b200_emit_bf16_next) instead of that edge running a conversion pass.
+  // Dropout (scale != 0): convnet_b200_fuse_next_dropout, no mask tensor (only where ConvNet::DropoutFolds).
+  // scale: the dropout derivative of the source layer folded into the dgrad (convnet_b200_fuse_next_scale).
+  // bias_grad: the edge below's bias gradient, summed while the derivative is stored (convnet_b200_fuse_next_bias_grad).
+  struct UpRequest { bool emit = false; float drop_prob = 0.f, drop_scale = 0.f; unsigned long long drop_seed = 0; };
   struct BiasGradTarget { float* grad_bias = nullptr; float st = 0.f, so = 1.f; };
-  virtual bool OfferFusedBiasGrad(BiasGradTarget*) { return false; }
-  void SetBiasGradRequest(const BiasGradTarget& t) { bg_request_ = t; }
-  // ComputeDown multiplies the derivative it writes by this factor (1 = none): the dropout derivative of a ReLU layer folded
-  // into the dgrad epilogue (convnet_b200_fuse_next_scale); only edges whose ComputeDown is a conv dgrad with the mask fused
-  void SetDerivScale(float s) { deriv_scale_ = s; }
-  virtual bool CanScaleDeriv() const { return false; }
-  // The dropout of the destination layer rides in ComputeUp's conv epilogue behind the fused bias + ReLU
-  // (convnet_b200_fuse_next_dropout: no mask tensor — ConvNet asks only when the backward pass folds the dropout derivative
-  // into the dgrad above, see ConvNet::DropoutFolds).  One-shot: the next ComputeUp consumes it.
-  virtual bool CanFuseDropout() const { return false; }
-  void SetDropoutRequest(float prob, float scale, unsigned long long seed) { drop_prob_ = prob; drop_scale_ = scale; drop_seed_ = seed; }
-  virtual bool CanProduceBiasGrad() const { return false; }   // ComputeDown kernels that take the request
+  struct DownRequest { bool emit = false; float scale = 1.f; BiasGradTarget bias_grad; };
+  void Request(const UpRequest& r) { up_req_ = r; }
+  void Request(const DownRequest& r) { down_req_ = r; }
   virtual bool WantsBf16Input() const { return false; }      // this edge reads its input (fprop / wgrad) as bf16
   virtual bool WantsBf16Deriv() const { return false; }      // this edge reads its output derivative (wgrad / dgrad) as bf16
 
@@ -157,23 +158,15 @@ class Edge {
   int image_size_y_, image_size_x_, image_size_t_;
   int num_modules_y_, num_modules_x_, num_modules_t_;
   int batch_size_;
-  bool fuse_relu_ = false, fuse_mask_ = false;      // the activation / its derivative is fused (whichever it is)
-  int up_act_ = CNB_ACT_RELU, down_act_ = CNB_ACT_RELU;
-  bool emit_up_ = false, emit_down_ = false;
-  BiasGradTarget bg_request_;
-  float deriv_scale_ = 1.f;
-  float drop_prob_ = 0.f, drop_scale_ = 0.f;
-  unsigned long long drop_seed_ = 0;
-  void ApplyDropoutRequest(bool fused_epilogue) {   // call right before the ComputeUp kernel (after convnet_b200_fuse_next)
-    if (drop_scale_ != 0.f && fused_epilogue) convnet_b200_fuse_next_dropout(drop_prob_, drop_scale_, drop_seed_);
-    drop_scale_ = 0.f;
-  }
-  void ApplyBiasGradRequest() {            // call right before the ComputeDown kernel
-    if (bg_request_.grad_bias) convnet_b200_fuse_next_bias_grad(bg_request_.grad_bias, bg_request_.st, bg_request_.so);
-    bg_request_ = BiasGradTarget();
-    if (deriv_scale_ != 1.f) convnet_b200_fuse_next_scale(deriv_scale_);
-    deriv_scale_ = 1.f;
-  }
+  // SetImageSize of an edge with a conv descriptor: its channels, then its output size (src/edge.cc:108-114)
+  void SetImageSize(int y, int x, int t, ConvDesc& d);
+  FusionPlan plan_;
+  UpRequest up_req_;
+  DownRequest down_req_;
+  // right before the ComputeUp / ComputeDown kernel: the plan's fused activation and the pending request as ABI calls.
+  // `emit`: this kernel is the one that writes the output last
+  void ArmUp(const float* bias, bool emit);
+  void ArmDown(const float* act_state);
 };
 
 // The side stream of ConvNet::TrainOneBatch (all-reduce + optimizer, see convnet.h): bias-gradient column sums are
@@ -181,19 +174,30 @@ class Edge {
 // kernels of the main stream.  ConvNet::AllocateMemory gives every weighted edge the lane together with its gradient memory.
 struct SideLane { cudaStream_t stream = nullptr; cudaEvent_t ready = nullptr; bool used = false; };
 
+// The call sequence of every edge with weights: ComputeUp / ComputeDown / ComputeOuter stage the bf16 operands, arm the
+// requests, run the edge type's GEMM, note the path it took and add the bias (or sum its gradient).  A subclass supplies
+// its three GEMM calls, its parameter sizes and whether it prestages dgrad banks.
 class EdgeWithWeight : public Edge {
  public:
   void SetSideLane(SideLane* s) { side_ = s; }
   // after this edge's optimizer step, on the optimizer's stream: rebuild what the next ComputeDown derives from the
-  // weights alone (convnet_b200_prestage_next), off the next step's critical path.  Default: nothing to prepare.
-  virtual void PrestageDown() {}
+  // weights alone (convnet_b200_prestage_next), off the next step's critical path (edges where PrestagesDown holds)
+  void PrestageDown();
   explicit EdgeWithWeight(const EdgeConfig& c)
       : Edge(c), has_no_bias_(c.has_no_bias), scale_gradients_(c.scale_gradients), num_grads_received_(0),
         weight_opt_(c.weight_optimizer), bias_opt_(c.bias_optimizer) {}
   bool HasNoParameters() const override { return false; }
+  void ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) override;
+  void ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) override;
+  void ComputeOuter(Matrix& input, Matrix& deriv_output) override;
+  // parameters [Cout x (WeightCols + BiasCols)]: the weights (Shape4D WeightShape), then the bias columns; the gradient,
+  // the history and the adaptive optimizer state are carved the same way
+  size_t GetParameterMemoryRequirement() override;
+  void SetMemory(Matrix& p) override { Carve(p, weights_, bias_); }
+  void SetGradMemory(Matrix& p) override { Carve(p, grad_weights_, grad_bias_); }
+  void SetHistoryMemory(Matrix& p) override { Carve(p, hist_weights_, hist_bias_); }
+  void SetStateMemory(Matrix& p) { Carve(p, state_weights_, state_bias_); }
   void UpdateWeights() override;                                         // src/edge_with_weight.cc:96-118
-  void SetHistoryMemory(Matrix& p) override;
-  void SetStateMemory(Matrix& p);          // the adaptive optimizer state, carved like the history
   void InitState(int which);               // the state of the weights (0) or the bias (1) back to its optimizer's start
   void Initialize(unsigned seed) override;
   Matrix& GetWeight() { return weights_; }
@@ -203,10 +207,9 @@ class EdgeWithWeight : public Edge {
   int GetNumGradsReceived() const { return num_grads_received_; }
   void IncrementNumGradsReceived() { num_grads_received_++; }
   void NotifyStart() { num_grads_received_ = 0; }
-  virtual int FanIn() const = 0;
   // bf16 mode (convnet_b200_set_conv_precision(2)): each tensor this edge feeds to two conv calls of a step has ONE bf16
   // copy — the input (fprop + wgrad), the output derivative (wgrad + dgrad) and the weights (fprop + dgrad).  The copy is
-  // normally written by the kernel that produced the tensor (emit_up / emit_down of the neighbouring edges, the dropout
+  // normally written by the kernel that produced the tensor (the emit requests of the neighbouring edges, the dropout
   // and SGD kernels); convnet_b200_bf16_ensure converts only when no valid copy exists.  Which calls really run in bf16 is
   // learnt from convnet_b200_last_conv_path() during the first step (FC-shaped calls stay on tf32 and are not staged).
   bool WantsBf16Input() const override { return bf_up_ == 1 || bf_outer_ == 1; }
@@ -218,18 +221,33 @@ class EdgeWithWeight : public Edge {
   OptimizerConfig& Optimizer(int which) { return which ? bias_opt_ : weight_opt_; }
   long long OptimizerStep(int which) const { return which ? bias_step_ : weight_step_; }
   void ReduceLearningRate(float factor) { weight_opt_.epsilon *= factor; bias_opt_.epsilon *= factor; }   // edge_with_weight.cc:90-93
-  bool OfferFusedBiasGrad(BiasGradTarget* t) override;
-  virtual bool BiasIsPerChannel2D() const { return !has_no_bias_; }       // one bias per output channel, 2-D layer
-  // (a conv dgrad would only run the column-sum pass inside the library call, on the main stream; leaving it to the edge
-  //  below puts it on the side lane instead — so only the pooling edges, whose kernels really fuse it, take the request)
-  bool CanScaleDeriv() const override { return fuse_mask_; }               // (3-D ConvEdge: fuse_mask_ is off, CanFuseMask)
-  // sigma and sigma' ride in the conv epilogues exactly where max(., 0) and the ReLU' mask do
-  bool CanFuseLogistic() const override { return true; }
+  // the target of this step's bias gradient for the edge above (Plan().offers_bias_grad): ComputeOuter then skips its sum
+  BiasGradTarget HandOffBiasGrad();
+  // sigma and sigma' ride in the conv epilogues exactly where max(., 0) and the ReLU' mask do; so does the dropout.
+  // (A conv dgrad would only run the bias-gradient column sum inside the library call, on the main stream; leaving it to
+  // the edge below puts it on the side lane instead — so only the pooling edges, whose kernels really fuse it, take it.)
+  Absorbs CanAbsorb() const override {
+    Absorbs a;
+    a.act_up = a.per_channel_bias = !has_no_bias_;
+    a.act_down = a.logistic = a.dropout = true;
+    return a;
+  }
 
  protected:
+  virtual void GemmUp(Matrix& input, Matrix& output, float scale_targets) = 0;
+  virtual void GemmDown(Matrix& deriv_output, Matrix& deriv_input, float scale_targets) = 0;
+  virtual void GemmOuter(Matrix& input, Matrix& deriv_output, float scale_targets, float scale) = 0;
+  virtual int WeightCols() const = 0;      // per output channel; also the fan-in of the initialisation (edge_with_weight.cc:126)
+  virtual int BiasCols() const { return 1; }
+  virtual Shape4D WeightShape() const = 0;
+  virtual bool PrestagesDown() const { return false; }
+  void Carve(Matrix& p, Matrix& w, Matrix& b);
+  // bias_ (1 x B) added to every B columns of the output, reshaped to [rows x B] (cnb_add_channel_bias); its gradient the
+  // column sum of the output derivative in that shape, on the side lane
+  virtual void AddBias(Matrix& output, bool emit);
+  virtual void SumBias(Matrix& deriv_output, float scale_targets, float scale);
   void StageForUp(Matrix& input);
   void StageForBprop(Matrix& deriv_output);
-  void SumBiasRows(Matrix& deriv_output, float scale_targets, float scale);      // SumRows on the side lane
   SideLane* side_ = nullptr;
   void NoteUp();
   void NoteDown();
@@ -244,10 +262,6 @@ class EdgeWithWeight : public Edge {
   // the tensors of the last ComputeDown that took the bf16 path (layer-owned, stable): PrestageDown re-describes that call
   Matrix* down_out_ = nullptr;
   Matrix* down_in_ = nullptr;
-  void RememberDown(Matrix& deriv_output, Matrix& deriv_input) {
-    down_out_ = bf_down_ == 1 ? &deriv_output : nullptr;
-    down_in_ = bf_down_ == 1 ? &deriv_input : nullptr;
-  }
   bool bias_grad_fused_ = false;                         // this step's bias gradient comes from the edge above (ComputeOuter skips SumRows)
 };
 
@@ -255,20 +269,25 @@ class ConvEdge : public EdgeWithWeight {
  public:
   explicit ConvEdge(const EdgeConfig& c);
   void SetImageSize(int y, int x, int t) override;
-  size_t GetParameterMemoryRequirement() override;
-  void SetMemory(Matrix& p) override;
-  void SetGradMemory(Matrix& p) override;
-  void ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) override;
-  void ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) override;
-  void PrestageDown() override;
-  void ComputeOuter(Matrix& input, Matrix& deriv_output) override;
   double FlopsUp() const override;
-  int FanIn() const override;
   ConvDesc GetConvDesc() const { return conv_desc_; }
-  bool CanFuseReLU() const override { return !has_no_bias_ && shared_bias_ && image_size_t_ == 1; }
-  bool CanFuseDropout() const override { return fuse_relu_ && CanFuseReLU(); }
-  bool CanFuseMask() const override { return image_size_t_ == 1; }
-  bool BiasIsPerChannel2D() const override { return !has_no_bias_ && shared_bias_ && image_size_t_ == 1; }
+  Absorbs CanAbsorb() const override {                   // the 3-D kernels fuse nothing; only a shared bias rides along
+    Absorbs a = EdgeWithWeight::CanAbsorb();
+    a.act_up = a.per_channel_bias = !has_no_bias_ && shared_bias_ && image_size_t_ == 1;
+    a.act_down = image_size_t_ == 1;
+    return a;
+  }
+
+ protected:
+  void GemmUp(Matrix& input, Matrix& output, float scale_targets) override;
+  void GemmDown(Matrix& deriv_output, Matrix& deriv_input, float scale_targets) override;
+  void GemmOuter(Matrix& input, Matrix& deriv_output, float scale_targets, float scale) override;
+  int WeightCols() const override;
+  int BiasCols() const override { return shared_bias_ ? 1 : num_modules_y_ * num_modules_x_ * num_modules_t_; }
+  Shape4D WeightShape() const override;
+  bool PrestagesDown() const override { return image_size_t_ == 1; }
+  void AddBias(Matrix& output, bool emit) override;
+  void SumBias(Matrix& deriv_output, float scale_targets, float scale) override;
 
  private:
   ConvDesc conv_desc_;
@@ -283,19 +302,21 @@ class LocalEdge : public EdgeWithWeight {
  public:
   explicit LocalEdge(const EdgeConfig& c) : EdgeWithWeight(c), conv_desc_(Edge::GetConvDesc(c)) {}
   void SetImageSize(int y, int x, int t) override;
-  size_t GetParameterMemoryRequirement() override;
-  void SetMemory(Matrix& p) override;
-  void SetGradMemory(Matrix& p) override;
-  void ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) override;
-  void ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) override;
-  void ComputeOuter(Matrix& input, Matrix& deriv_output) override;
   double FlopsUp() const override;
+  Absorbs CanAbsorb() const override {                   // the bias is per output feature, not per channel
+    Absorbs a = EdgeWithWeight::CanAbsorb();
+    a.per_channel_bias = false;
+    return a;
+  }
+
+ protected:
+  void GemmUp(Matrix& input, Matrix& output, float scale_targets) override;
+  void GemmDown(Matrix& deriv_output, Matrix& deriv_input, float scale_targets) override;
+  void GemmOuter(Matrix& input, Matrix& deriv_output, float scale_targets, float scale) override;
   // the reference's initialisation scale: weights_.GetCols() = K * modules (edge_with_weight.cc:126)
-  int FanIn() const override { return KernelSize() * Modules(); }
-  bool CanFuseReLU() const override { return !has_no_bias_; }                  // per-feature bias in the epilogue
-  bool CanFuseDropout() const override { return fuse_relu_ && CanFuseReLU(); }
-  bool CanFuseMask() const override { return true; }
-  bool BiasIsPerChannel2D() const override { return false; }
+  int WeightCols() const override { return KernelSize() * Modules(); }
+  int BiasCols() const override { return Modules(); }
+  Shape4D WeightShape() const override;
 
  private:
   int KernelSize() const { return conv_desc_.kernel_size_y * conv_desc_.kernel_size_x * conv_desc_.num_input_channels; }
@@ -307,21 +328,16 @@ class FCEdge : public EdgeWithWeight {          // weights [Cout x K] column-maj
  public:
   explicit FCEdge(const EdgeConfig& c) : EdgeWithWeight(c) {}
   void SetImageSize(int y, int x, int t) override;
-  size_t GetParameterMemoryRequirement() override;
-  void SetMemory(Matrix& p) override;
-  void SetGradMemory(Matrix& p) override;
-  void ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) override;
-  void ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) override;
-  void ComputeOuter(Matrix& input, Matrix& deriv_output) override;
   double FlopsUp() const override;
-  int FanIn() const override { return num_inputs_; }
-  bool CanFuseReLU() const override { return !has_no_bias_; }
-  bool CanFuseDropout() const override { return fuse_relu_ && CanFuseReLU(); }
-  bool CanFuseMask() const override { return true; }
 
+ protected:
+  void GemmUp(Matrix& input, Matrix& output, float scale_targets) override;
+  void GemmDown(Matrix& deriv_output, Matrix& deriv_input, float scale_targets) override;
+  void GemmOuter(Matrix& input, Matrix& deriv_output, float scale_targets, float scale) override;
+  int WeightCols() const override { return num_inputs_; }
+  Shape4D WeightShape() const override { return Shape4D{{num_output_channels_, 1, 1, num_inputs_}}; }
 
  private:
-  void View(Matrix& in, Matrix& out);
   int num_inputs_ = 0;
   ConvDesc desc_;
 };
@@ -330,18 +346,15 @@ class ConvOneToOneEdge : public EdgeWithWeight {
  public:
   explicit ConvOneToOneEdge(const EdgeConfig& c) : EdgeWithWeight(c) {}
   void SetImageSize(int y, int x, int t) override;
-  size_t GetParameterMemoryRequirement() override;
-  void SetMemory(Matrix& p) override;
-  void SetGradMemory(Matrix& p) override;
-  void ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) override;
-  void ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) override;
-  void PrestageDown() override;
-  void ComputeOuter(Matrix& input, Matrix& deriv_output) override;
   double FlopsUp() const override;
-  int FanIn() const override { return num_input_channels_; }
-  bool CanFuseReLU() const override { return !has_no_bias_; }
-  bool CanFuseDropout() const override { return fuse_relu_ && CanFuseReLU(); }
-  bool CanFuseMask() const override { return true; }
+
+ protected:
+  void GemmUp(Matrix& input, Matrix& output, float scale_targets) override;
+  void GemmDown(Matrix& deriv_output, Matrix& deriv_input, float scale_targets) override;
+  void GemmOuter(Matrix& input, Matrix& deriv_output, float scale_targets, float scale) override;
+  int WeightCols() const override { return num_input_channels_; }
+  Shape4D WeightShape() const override { return Shape4D{{num_output_channels_, 1, 1, num_input_channels_}}; }
+  bool PrestagesDown() const override { return true; }
 
  private:
   ConvDesc desc_;
@@ -353,8 +366,12 @@ class MaxPoolEdge : public Edge {
   void SetImageSize(int y, int x, int t) override;
   void ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) override;
   void ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) override;
-  bool CanFuseMask() const override { return true; }
-  bool CanProduceBiasGrad() const override { return image_size_t_ == 1; }
+  Absorbs CanAbsorb() const override {
+    Absorbs a;
+    a.act_down = true;
+    a.sums_bias_below = image_size_t_ == 1;
+    return a;
+  }
 
  protected:
   ConvDesc conv_desc_;
@@ -369,7 +386,11 @@ class AvgPoolEdge : public MaxPoolEdge {
 
 class ResponseNormEdge : public Edge {
  public:
-  bool CanFuseReLU() const override { return image_size_t_ == 1; }      // max(., 0) rides in the rnorm kernel's store
+  Absorbs CanAbsorb() const override {                  // max(., 0) rides in the rnorm kernel's store
+    Absorbs a;
+    a.act_up = image_size_t_ == 1;
+    return a;
+  }
   explicit ResponseNormEdge(const EdgeConfig& c)
       : Edge(c), num_filters_response_norm_(0), blocked_(c.response_norm_in_blocks), add_scale_(c.add_scale),
         pow_scale_(c.pow_scale), frac_of_filters_response_norm_(c.frac_of_filters_response_norm) {}

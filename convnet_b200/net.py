@@ -85,6 +85,7 @@ def load_host():
             "cnb_net_get_bn_optimizer_state": ([vp, i, i, ct.POINTER(ll), ct.POINTER(f), ct.POINTER(f)], i),
             "cnb_bn_optimizer_check": ([ct.POINTER(OptimizerConfig)], i),
             "cnb_model_param_layout": ([ct.c_char_p, i, i, ct.POINTER(ll), ct.POINTER(ll), ct.POINTER(ll)], i),
+            "cnb_model_fusion": ([ct.c_char_p, i, i, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i)], i),
             "cnb_model_bn_layer": ([ct.c_char_p, i, ct.c_char_p, ct.POINTER(i), ct.POINTER(f), ct.POINTER(f),
                                     ct.POINTER(OptimizerConfig), ct.POINTER(OptimizerConfig)], i),
             "cnb_net_targets": ([vp], vp), "cnb_net_targets_floats": ([vp], ll), "cnb_net_metric": ([vp], f),
@@ -381,6 +382,24 @@ def model_param_layout(model, batch=1):
         raise ValueError("cannot build model %r (see stderr)" % model)
     return {"edge_offsets": [eo[k] for k in range(n)], "bn_offsets": [bo[k] if bo[k] >= 0 else None for k in range(n + 1)],
             "total": total.value}
+
+
+FUSION_FLAGS = ("dropout_up", "scale_down", "sums_bias_below", "offers_bias_grad")
+
+
+def model_fusion(model, batch=1):
+    """the epilogue fusion plan of a model (host-only): {"edges": per edge {"up_act", "down_act" (CNB_ACT_* codes: 0 none,
+    1 ReLU, 2 logistic), "dropout_up", "scale_down", "sums_bias_below", "offers_bias_grad"}, "layers": per layer
+    {"activation_pass", "deriv_pass"} (True: a separate pass remains)}"""
+    cap = 256
+    up, down, flags, passes = [(ct.c_int * cap)() for _ in range(4)]
+    n = load_host().cnb_model_fusion(model.encode(), batch, cap, up, down, flags, passes)
+    if n < 0:
+        raise ValueError("cannot build model %r (see stderr)" % model)
+    edges = [dict(up_act=up[k], down_act=down[k], **{f: bool(flags[k] >> b & 1) for b, f in enumerate(FUSION_FLAGS)})
+             for k in range(n)]
+    layers = [{"activation_pass": bool(passes[k] & 1), "deriv_pass": bool(passes[k] & 2)} for k in range(n + 1)]
+    return {"edges": edges, "layers": layers}
 
 
 def check_bn_optimizer(config):

@@ -14,8 +14,11 @@
 // One persistent CTA per SM, 9 warps: warps 0..7 are two consumer warpgroups (GEMM rows 0-63 and 64-127 of the 128 x 128
 // tile), warp 8 is the TMA producer filling a ring of shared-memory stages guarded by mbarriers.
 //   bf16 operands: wgmma.mma_async m64n128k16 reads both operands from the swizzled tiles (either major);
-//   tf32 operands: mma.sync m16n8k8 with fragments loaded from the same tiles — wgmma takes 32-bit operands from shared
-//                  memory only K-major, and the image / filter operands of fprop and dgrad are MN-major.
+//   tf32 operands: wgmma takes 32-bit operands from shared memory only K-major, so
+//     wgrad (both operands K-major): wgmma m64n128k8 on the tiles, as bf16;
+//     x-mode fprop (Cin < 8): wgmma m64nNk8 with A (the MN-major image tile) loaded into registers and B the n-tile's
+//                  filter bank, written K-major into shared memory once per CTA and kept there;
+//     other fprop / dgrad (MN-major operands): mma.sync m16n8k8 with fragments loaded from the tiles.
 // Accumulators live in registers; the consumers store a finished tile straight from them (every group of 8 lanes writes
 // 8 consecutive images of one channel = one 32-byte sector) while the producer already fills the ring for the next tile.
 #include <cuda.h>
@@ -60,6 +63,10 @@ struct TcParams {
   // take the place of the channel block.  fprop: one K block = (channel c, 4 filter rows) = 4x8 K rows;
   // wgrad: the N tile is (x_ct channels) x (ky rows) x 8 taps, reduced over ALL modules at once.
   int x_mode, x_yblocks, x_ct;
+  // x-mode fprop: B is no ring but the filter bank of the tile's n-tile, resident in shared memory after the A ring
+  // (bank_bytes = Cin * x_yblocks * BN * 128), filled from the caller's filters `xw` ([c][ty][tx][o], o contiguous)
+  const float* xw;
+  uint32_t bank_bytes;              // 0: the B half of the ring follows the A ring
   uint32_t b_tx_bytes;              // bytes the B-operand TMA(s) of one stage actually deliver
   // merged requests: when N % 128 == 0 (2-D) the chunks of an m-tile are one box over a (chunk, ..., N/chunk, ...) view
   // of the tensor; when Cout % chunk == 0 the BN/chunk filter chunks are one box likewise.
@@ -223,6 +230,65 @@ __device__ __forceinline__ uint32_t off_mnmajor(int row, int k) {
   return (uint32_t)((row >> 5) * (BK * 128) + k * 128 + (((((row & 31) >> 2) ^ k) & 7) << 4) + ((row & 3) << 2));
 }
 
+// ---- x-mode fprop on tf32 wgmma -------------------------------------------------------------------------------------
+// The k-block of stage rows 8s .. 8s+7 is k-step s.  Inside a k-step, logical k j of the wgmma sits in stage K row
+// 2(j&3) + (j>>2): the A fragment of lane (g, q) is then K rows 2q and 2q+1, and the 16-byte units (row>>2 ^ K row) & 7
+// that one load instruction of a warp touches are all distinct — no bank conflicts.  The filter bank follows the same
+// permutation.
+__device__ __forceinline__ int xmode_k_row(int k) { return (k & ~7) | ((k & 3) << 1) | ((k >> 2) & 1); }
+
+// The n-tile's filter bank, K-major [k-block (c, yb)][BN columns][32 K] with the 128-byte swizzle, written by the 256
+// consumer threads: stage K row r of k-block (c, yb) is tap tx = r & 7 of filter row ty = 4 yb + (r >> 3).  The raw fp32
+// bits (the tensor core reads their tf32 part, as it does the images), and exact zeros at taps tx >= kx, rows ty >= ky
+// and columns beyond Cout: the A box covers 8 x 4 real pixels whatever the kernel size.
+__device__ __forceinline__ void xmode_fill_bank(const TcParams& p, uint8_t* bank, int n_tile) {
+  const int total = p.Cin * p.x_yblocks * 32 * p.BN;
+#pragma unroll 8
+  for (int i = threadIdx.x; i < total; i += 32 * kConsumerWarps) {
+    const int n = i % p.BN, rest = i / p.BN, k = rest & 31, kb = rest >> 5;
+    const int r = xmode_k_row(k), c = kb / p.x_yblocks, ty = 4 * (kb % p.x_yblocks) + (r >> 3), tx = r & 7;
+    const int o = n_tile * p.BN + n;
+    float v = 0.f;
+    if (tx < p.kx && ty < p.ky && o < p.Cout) v = __ldg(p.xw + o + (long long)p.Cout * (tx + p.kx * (ty + p.ky * c)));
+    *reinterpret_cast<float*>(bank + (size_t)kb * p.BN * 128 + off_kmajor(n, k)) = v;
+  }
+}
+
+// The k-blocks of one x-mode fprop tile: per stage, this warp's 16 rows of A into registers, then four wgmma m64nNk8
+// against the resident bank, and wgmma.wait_group 0 before the next stage's fragment loads.  (Loading the next fragment
+// into a second register buffer while the group is in flight makes ptxas serialize every wgmma — C7513, "non wgmma
+// instructions defining input registers ... between start and end of the pipeline stage" — so the overlap comes from
+// the other warpgroup instead.)  The slot is released once its MMAs retired.
+template <int N>
+__device__ __forceinline__ void xmode_fprop_mma(float (&acc)[16][4], const TcParams& p, SmemCtl* ctl, uint32_t sA,
+                                                uint32_t bank, int nkb, int& stage, uint32_t& phase, int row0, int tq,
+                                                int lane) {
+  const uint64_t db0 = ptx::gmma_desc(bank, 16u, 1024u);
+  ptx::wgmma_fence_operands(acc);
+  for (int kb = 0; kb < nkb; kb++) {
+    ptx::mbar_wait(&ctl->full[stage], phase);
+    const uint32_t A = sA + (uint32_t)stage * kAStageBytes;
+    uint32_t a[4][4];
+#pragma unroll
+    for (int ks = 0; ks < 4; ks++) {
+      const int k0 = ks * 8 + 2 * tq;
+      a[ks][0] = ptx::lds32(A + off_mnmajor(row0, k0));
+      a[ks][1] = ptx::lds32(A + off_mnmajor(row0 + 8, k0));
+      a[ks][2] = ptx::lds32(A + off_mnmajor(row0, k0 + 1));
+      a[ks][3] = ptx::lds32(A + off_mnmajor(row0 + 8, k0 + 1));
+    }
+    ptx::wgmma_fence();                            // orders the fragment writes before the wgmma reads them
+    const uint64_t db = db0 + ((uint32_t)kb * (N * 128) >> 4);
+#pragma unroll
+    for (int ks = 0; ks < 4; ks++) ptx::wgmma_m64nNk8_tf32_rs<N>(acc, a[ks], db + (ks * 32 >> 4));
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();                          // the fragment registers are free again, and so is the slot
+    if (lane == 0) ptx::mbar_arrive(&ctl->empty[stage]);
+    if (++stage == p.stages) { stage = 0; phase ^= 1; }
+  }
+  ptx::wgmma_fence_operands(acc);
+}
+
 // ------------------------------------------------------------------------------------------------
 // SIG: the epilogue applies the activation code (logistic included); the other instances know only ReLU / ReLU', so the
 // logistic arithmetic costs the ReLU and linear layers nothing
@@ -232,8 +298,8 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smemA = smem;
-  uint8_t* smemB = smem + (size_t)p.stages * kAStageBytes;
-  SmemCtl* ctl = reinterpret_cast<SmemCtl*>(smemB + (size_t)p.stages * kBStageBytes);
+  uint8_t* smemB = smem + (size_t)p.stages * kAStageBytes;      // the B ring, or the x-mode fprop filter bank
+  SmemCtl* ctl = reinterpret_cast<SmemCtl*>(smemB + (p.bank_bytes ? (size_t)p.bank_bytes : (size_t)p.stages * kBStageBytes));
 
   // warp index through a shuffle: provably warp-uniform, which keeps the role branches and their loops on the uniform path
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
@@ -279,23 +345,16 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
           cX[c] = (ch.pos[c] % p.modX) * p.sx + p.px;
           cY[c] = (ch.pos[c] / p.modX) * p.sy + p.py;
         }
-        if (p.x_mode) {
+        if (p.x_mode) {                        // A only: B is the consumers' resident filter bank
           for (int c = 0; c < p.Cin; c++)
             for (int yb = 0; yb < p.x_yblocks; yb++) {
               uint8_t* a = begin_stage();
-              uint8_t* b = smemB + (size_t)stage * kBStageBytes;
               if (p.a_merged) {                // dims (n_lo, x, y, n_hi, c): one 16 KiB request
                 lda5(&mapA, a, 0, cX[0], cY[0] + 4 * yb, ch.n[0] >> 5, c);
               } else {
 #pragma unroll
                 for (int q = 0; q < 4; q++)    // 8 consecutive x pixels x 4 filter rows of channel c = 32 K rows
                   lda5(&mapA, a + q * (BK * 128), ch.n[q], c, cX[q], cY[q] + 4 * yb, ch.f[q]);
-              }
-              if (p.b_merged) {                // dims (o_lo, tx, ty, o_hi, c)
-                lda5(&mapB, b, 0, 0, 4 * yb, tile.n_tile * (p.BN >> 5), c);
-              } else {
-                for (int j = 0; j < p.BN / 32; j++)   // taps >= kx and rows >= ky are out of range -> zero weights
-                  lda4(&mapB, b + j * (BK * 128), tile.n_tile * p.BN + j * 32, 0, 4 * yb, c);
               }
               end_stage();
             }
@@ -432,6 +491,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   const int g = lane >> 2, tq = lane & 3;
   const int row0 = warp * 16 + g;                  // this thread's GEMM rows in the tile: row0 and row0 + 8
   int stage = 0; uint32_t phase = 0;
+  int bank_tile = -1;                              // x-mode fprop: the n-tile whose filter bank is in shared memory
   for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
     const Tile tile = decode_tile<OP>(p, t);
     const int nkb = tile_kblocks<OP>(p, tile);
@@ -441,9 +501,9 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
 #pragma unroll
       for (int e = 0; e < 4; e++) acc[j][e] = 0.f;
 
-    if constexpr (BF16) {
+    if constexpr (BF16 || OP == kWgrad) {
       // warpgroup w multiplies GEMM rows 64w..64w+63: the second 64-image chunk (MN-major A) or rows 64.. (K-major A),
-      // 8 KiB into the stage either way
+      // 8 KiB into the stage either way.  tf32 (wgrad only): both operands K-major, the k8 step is +32 B like bf16's k16.
       constexpr bool a_mn = (OP != kWgrad), b_mn = (OP == kFprop);
       constexpr uint32_t a_step = a_mn ? 2048u : 32u, b_step = b_mn ? 2048u : 32u;
       const uint64_t da0 = ptx::gmma_desc(ptx::smem_u32(smemA) + (uint32_t)(warp >> 2) * 8192u, a_mn ? 8192u : 16u, 1024u);
@@ -455,8 +515,12 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         ptx::wgmma_fence();
         const uint64_t da = da0 + ((uint32_t)stage * kAStageBytes >> 4), db = db0 + ((uint32_t)stage * kBStageBytes >> 4);
 #pragma unroll
-        for (int ks = 0; ks < 4; ks++)
-          ptx::wgmma_m64n128k16_bf16<a_mn ? 1 : 0, b_mn ? 1 : 0>(acc, da + (ks * a_step >> 4), db + (ks * b_step >> 4));
+        for (int ks = 0; ks < 4; ks++) {
+          if constexpr (BF16)
+            ptx::wgmma_m64n128k16_bf16<a_mn ? 1 : 0, b_mn ? 1 : 0>(acc, da + (ks * a_step >> 4), db + (ks * b_step >> 4));
+          else
+            ptx::wgmma_m64n128k8_tf32(acc, da + (ks * a_step >> 4), db + (ks * b_step >> 4));
+        }
         ptx::wgmma_commit();
         ptx::wgmma_wait<1>();                        // the previous stage's MMAs have retired: its slot can be refilled
         if (prev >= 0 && lane == 0) ptx::mbar_arrive(&ctl->empty[prev]);
@@ -466,19 +530,35 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
       ptx::wgmma_wait<0>();
       ptx::wgmma_fence_operands(acc);
       if (prev >= 0 && lane == 0) ptx::mbar_arrive(&ctl->empty[prev]);
+    } else if (OP == kFprop && p.x_mode) {
+      if (tile.n_tile != bank_tile) {              // uniform over the CTA: every consumer thread sees the same tile
+        ptx::bar_sync(1, 32 * kConsumerWarps);     // both warpgroups are past the MMAs that read the previous bank
+        xmode_fill_bank(p, smemB, tile.n_tile);
+        ptx::fence_proxy_async_smem();             // the generic-proxy stores become visible to wgmma
+        ptx::bar_sync(1, 32 * kConsumerWarps);
+        bank_tile = tile.n_tile;
+      }
+      const uint32_t sA = ptx::smem_u32(smemA), bank = ptx::smem_u32(smemB);
+      switch (p.BN) {                              // the N sizes x-mode picks (host: tc_conv_up_impl)
+        case 32: xmode_fprop_mma<32>(acc, p, ctl, sA, bank, nkb, stage, phase, row0, tq, lane); break;
+        case 64: xmode_fprop_mma<64>(acc, p, ctl, sA, bank, nkb, stage, phase, row0, tq, lane); break;
+        case 96: xmode_fprop_mma<96>(acc, p, ctl, sA, bank, nkb, stage, phase, row0, tq, lane); break;
+        default: xmode_fprop_mma<128>(acc, p, ctl, sA, bank, nkb, stage, phase, row0, tq, lane); break;
+      }
     } else {
+      // tf32 fprop / dgrad: A MN-major; B MN-major (fprop: the caller's filters) or K-major (dgrad)
       const uint32_t sA = ptx::smem_u32(smemA), sB = ptx::smem_u32(smemB);
-      constexpr bool a_mn = (OP != kWgrad), b_mn = (OP == kFprop);
+      constexpr bool b_mn = (OP == kFprop);
       for (int kb = 0; kb < nkb; kb++) {
         ptx::mbar_wait(&ctl->full[stage], phase);
         const uint32_t A = sA + (uint32_t)stage * kAStageBytes, B = sB + (uint32_t)stage * kBStageBytes;
 #pragma unroll
         for (int ks = 0; ks < 4; ks++) {
           const int k0 = ks * 8 + tq, k1 = k0 + 4;
-          const uint32_t a0 = ptx::lds32(A + (a_mn ? off_mnmajor(row0, k0) : off_kmajor(row0, k0)));
-          const uint32_t a1 = ptx::lds32(A + (a_mn ? off_mnmajor(row0 + 8, k0) : off_kmajor(row0 + 8, k0)));
-          const uint32_t a2 = ptx::lds32(A + (a_mn ? off_mnmajor(row0, k1) : off_kmajor(row0, k1)));
-          const uint32_t a3 = ptx::lds32(A + (a_mn ? off_mnmajor(row0 + 8, k1) : off_kmajor(row0 + 8, k1)));
+          const uint32_t a0 = ptx::lds32(A + off_mnmajor(row0, k0));
+          const uint32_t a1 = ptx::lds32(A + off_mnmajor(row0 + 8, k0));
+          const uint32_t a2 = ptx::lds32(A + off_mnmajor(row0, k1));
+          const uint32_t a3 = ptx::lds32(A + off_mnmajor(row0 + 8, k1));
 #pragma unroll
           for (int j = 0; j < BN_MAX / 8; j++) {
             if (j * 8 >= p.BN) break;
@@ -634,13 +714,16 @@ int pick_bn(int cols, int granule) {              // N-tile: as wide as possible
   return std::min(BN_MAX, std::max(granule, bn));
 }
 
-size_t smem_bytes_for(int stages) {
-  return 1024 + (size_t)stages * (kAStageBytes + kBStageBytes) + sizeof(SmemCtl) + 16;
+// dynamic shared memory of a launch with `stages` ring stages: A stages, then B stages or (x-mode fprop) the filter bank
+size_t smem_bytes_for(int stages, uint32_t bank_bytes) {
+  const size_t b = bank_bytes ? (size_t)bank_bytes : (size_t)stages * kBStageBytes;
+  return 1024 + (size_t)stages * kAStageBytes + b + sizeof(SmemCtl) + 16;
 }
+constexpr size_t kSmemBudget = 225 * 1024;
 
-int pick_stages() {
+int pick_stages(uint32_t bank_bytes) {
   int s = kMaxStages;
-  while (s > 2 && smem_bytes_for(s) > 225 * 1024) s--;
+  while (s > 2 && smem_bytes_for(s, bank_bytes) > kSmemBudget) s--;
   return s;
 }
 
@@ -659,8 +742,8 @@ void launch_one(const CUtensorMap& a, const CUtensorMap& b, const TcParams& p, s
 
 template <int OP>
 void launch(const CUtensorMap& a, const CUtensorMap& b, TcParams& p) {
-  p.stages = pick_stages();
-  const size_t smem = smem_bytes_for(p.stages);
+  p.stages = pick_stages(p.bank_bytes);
+  const size_t smem = smem_bytes_for(p.stages, p.bank_bytes);
   const bool sig = p.act == kActLogistic || (p.mask && p.mask_act == kActLogistic);
   if constexpr (OP != kWgrad) {                       // (a wgrad has no activation to apply)
     if (sig) {
@@ -687,6 +770,7 @@ void fill_common(TcParams& p, const ConvGeom& g, const Elem& e) {
   p.frames = g.frames; p.frame0 = 0;
   p.splits = 1; p.units_per_split = 0; p.part_stride = 0;
   p.x_mode = 0; p.x_yblocks = 0; p.x_ct = 0; p.b_tx_bytes = 0;
+  p.xw = nullptr; p.bank_bytes = 0;
   p.a_merged = 0; p.b_merged = 0;
   p.untied = g.conv ? 0 : 1;
   p.bias = nullptr; p.act = 0; p.mask = nullptr; p.mask_act = 0; p.out16 = nullptr;
@@ -819,14 +903,22 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
   p.kc_blocks = ceil_div(g.Cin, e.bk);
   p.x_mode = x_mode ? 1 : 0;
   p.x_yblocks = ceil_div(g.ky, 4);
+  if (x_mode) {
+    // B is the n-tile's filter bank, resident beside the A ring: it must leave room for >= 3 A stages, else the tile
+    // narrows (Cin 7, ky 8 at BN 128) — more n-tiles, the same single launch
+    auto bank_bytes = [&](int bn) { return (uint32_t)g.Cin * p.x_yblocks * bn * 128; };
+    while (p.BN > 32 && smem_bytes_for(3, bank_bytes(p.BN)) > kSmemBudget) p.BN = ceil_div(p.BN / 2, 32) * 32;
+    p.bank_bytes = bank_bytes(p.BN);
+    p.xw = filters;
+  }
   const long long chunks = (long long)p.nb * g.modules * g.frames;
   if (chunks * 4 >= (1LL << 31)) return false;
   p.total_chunks = p.nbc * g.modules * g.frames;
   p.m_tiles = ceil_div(p.total_chunks, p.cpt);
   p.n_tiles = ceil_div(g.Cout, p.BN);
   p.num_tiles = p.m_tiles * p.n_tiles;
-  // MN-major B is staged in whole chunks (BN is a multiple of the chunk)
-  p.b_tx_bytes = (uint32_t)p.BN * 128;
+  // MN-major B is staged in whole chunks (BN is a multiple of the chunk); x-mode streams A alone
+  p.b_tx_bytes = x_mode ? 0u : (uint32_t)p.BN * 128;
   float* const out = targets + (long long)g.cout0 * g.modules * g.N;
   const float* const bias = fuse.bias ? fuse.bias + (long long)g.cout0 * (g.conv ? 1 : g.modules) : nullptr;
   const long long out_elems = (long long)g.Cout * g.modules * g.N;
@@ -879,17 +971,7 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
       const int abox[5] = {32, 1, 8, 4, 1};                     // 8 x-taps x 4 filter rows of one channel
       if (!make_map(&ma, img, e, 5, adims, astr, abox)) return false;
     }
-    if (p.b_merged) {
-      const long long bdims[5] = {32, g.kx, g.ky, g.Cout / 32, g.Cin};
-      const long long bstr[4] = {g.Cout, (long long)g.Cout * g.kx, 32, (long long)g.Cout * taps};
-      const int bbox[5] = {32, 8, 4, p.BN / 32, 1};
-      if (!make_map(&mb, flt, e, 5, bdims, bstr, bbox)) return false;
-    } else {
-      const long long bdims[4] = {g.Cout, g.kx, g.ky, g.Cin};
-      const long long bstr[3] = {g.Cout, (long long)g.Cout * g.kx, (long long)g.Cout * taps};
-      const int bbox[4] = {32, 8, 4, 1};
-      if (!make_map(&mb, flt, e, 4, bdims, bstr, bbox)) return false;
-    }
+    mb = ma;                                                    // no B map: the kernel reads the filters into its bank
   } else {
     if (p.a_merged) {
       if (!merged_image_map(&ma, img, e, g, g.W, g.H, g.Cin, false)) return false;

@@ -1,5 +1,5 @@
 // sm90_ptx.cuh — thin inline-PTX wrappers for the Hopper (sm_90a) features the conv kernels use: mbarrier, TMA tiled
-// loads, wgmma (bf16, operands in shared memory, accumulators in registers) and mma.sync (tf32).
+// loads, wgmma (bf16 and tf32, accumulators in registers) and mma.sync (tf32).
 // Hand-written from the PTX ISA; descriptor fields as in the PTX "matrix descriptor" section.
 #pragma once
 #include <cuda_runtime.h>
@@ -146,7 +146,79 @@ __device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[16][4], uint64_
         CNB_ACC4(8), CNB_ACC4(9), CNB_ACC4(10), CNB_ACC4(11), CNB_ACC4(12), CNB_ACC4(13), CNB_ACC4(14), CNB_ACC4(15)
       : "l"(desc_a), "l"(desc_b), "n"(TA), "n"(TB), "r"(1));
 }
+
+// D[64 x 128] += A[64 x 8] * B[8 x 128], tf32 (fp32 bit patterns; the tensor core reads their tf32 part), both operands
+// K-major in shared memory (32-bit operands have no transposed form).  The K step of 8 is +32 B inside the swizzle atom.
+__device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[16][4], uint64_t desc_a, uint64_t desc_b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t}"
+      : CNB_ACC4(0), CNB_ACC4(1), CNB_ACC4(2), CNB_ACC4(3), CNB_ACC4(4), CNB_ACC4(5), CNB_ACC4(6), CNB_ACC4(7),
+        CNB_ACC4(8), CNB_ACC4(9), CNB_ACC4(10), CNB_ACC4(11), CNB_ACC4(12), CNB_ACC4(13), CNB_ACC4(14), CNB_ACC4(15)
+      : "l"(desc_a), "l"(desc_b), "r"(1));
+}
+
+// D[64 x N] += A[64 x 8] * B[8 x N], tf32, A from registers, B K-major in shared memory.  A fragment of a thread (lane
+// l of warp w of the warpgroup, g = l / 4, q = l % 4): a[0] = (row 16w+g, k q), a[1] = (16w+g+8, q), a[2] = (16w+g,
+// q+4), a[3] = (16w+g+8, q+4) — the mma.sync m16n8k8 layout per warp.  N in {32, 64, 96, 128}: accumulators d[0 .. N/8).
+template <int N>
+__device__ __forceinline__ void wgmma_m64nNk8_tf32_rs(float (&d)[16][4], const uint32_t (&a)[4], uint64_t desc_b) {
+  static_assert(N == 32 || N == 64 || N == 96 || N == 128, "tf32 RS wgmma: N in {32, 64, 96, 128}");
+  if constexpr (N == 32) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+        : CNB_ACC4(0), CNB_ACC4(1), CNB_ACC4(2), CNB_ACC4(3)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+  } else if constexpr (N == 64) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+        : CNB_ACC4(0), CNB_ACC4(1), CNB_ACC4(2), CNB_ACC4(3), CNB_ACC4(4), CNB_ACC4(5), CNB_ACC4(6), CNB_ACC4(7)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+  } else if constexpr (N == 96) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %53, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+        "{%48, %49, %50, %51}, %52, p, 1, 1;\n\t}"
+        : CNB_ACC4(0), CNB_ACC4(1), CNB_ACC4(2), CNB_ACC4(3), CNB_ACC4(4), CNB_ACC4(5), CNB_ACC4(6), CNB_ACC4(7),
+          CNB_ACC4(8), CNB_ACC4(9), CNB_ACC4(10), CNB_ACC4(11)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+        : CNB_ACC4(0), CNB_ACC4(1), CNB_ACC4(2), CNB_ACC4(3), CNB_ACC4(4), CNB_ACC4(5), CNB_ACC4(6), CNB_ACC4(7),
+          CNB_ACC4(8), CNB_ACC4(9), CNB_ACC4(10), CNB_ACC4(11), CNB_ACC4(12), CNB_ACC4(13), CNB_ACC4(14), CNB_ACC4(15)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+  }
+}
 #undef CNB_ACC4
+
+// generic-proxy writes to shared memory become visible to the async proxy (wgmma operand reads, TMA)
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// named barrier `id` over the first `threads` threads of the block
+__device__ __forceinline__ void bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 }  // namespace ptx
 }  // namespace cnb

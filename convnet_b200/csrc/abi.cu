@@ -23,18 +23,8 @@ struct Range {
   ~Range() { nvtxRangePop(); }
 };
 
-// ---- dispatch: tensor-core path when the mode and the shape allow, else fp32 CUDA cores
-// Writer protocol (stage.cu): drop staged bf16 copies overlapping the target; when the caller asked for a fresh copy
-// (convnet_b200_emit_bf16_next) hand the kernel the buffer, and convert in a trailing pass if the kernel did not fill it.
-struct Emit {
-  float* target; long long n; __nv_bfloat16* buf = nullptr; bool done = false;
-  Emit(float* t, long long n_, bool want) : target(t), n(n_) {
-    bf16_note_write(t, n_);
-    if (want) buf = bf16_emit_slot(t, n_);          // nullptr outside bf16 mode; marked valid: the kernel below fills it
-  }
-  void attach(Fuse& f) { f.out16 = buf; f.emitted = &done; }
-  void finish() { if (buf && !done) bf16_stage(target, n); }     // nobody filled it: one conversion pass (re-validates the slot)
-};
+// ---- dispatch: tensor-core path when the mode and the shape allow, else fp32 CUDA cores; every write follows the writer
+// protocol (Emit, stage.cu)
 
 // bias gradient requested with the write (convnet_b200_fuse_next_bias_grad): finish from the kernel's per-slice sums, or
 // run the column-sum pass when the kernel did not produce them.  rows = images x positions, cols = channels.
@@ -45,19 +35,20 @@ void finish_bias_grad(const Fuse& fuse, const float* part, int slices, const flo
 }
 
 void conv_up(const ConvGeom& g, const float* images, const float* filters, float* targets, float st, float so) {
-  Fuse fuse = take_fuse();
+  const Fuse fuse = take_fuse();
   CNB_REQUIRE(!fuse.bias_grad, "convUp: a fused bias gradient belongs to a backward call");
   Emit emit(targets, g.out_total, fuse.emit_bf16 != 0);
-  emit.attach(fuse);
-  bool dropped = false;
-  fuse.dropped = &dropped;
-  if (!(state().precision != kPrecFP32 && tc_conv_up(g, images, filters, targets, st, so, fuse))) {
+  ConvOutcome r;
+  if (state().precision != kPrecFP32) r = tc_conv_up(g, images, filters, targets, st, so, fuse, emit.buf);
+  if (r.path == kPathNone) {
     simt_conv_up(g, images, filters, targets, st, so, fuse);
-    state().last_conv_path = kPathSimt;
+    r.path = kPathSimt;
   }
-  if (fuse.drop_scale != 0.f && !dropped) {        // the kernel could not apply the dropout: one pass, which also (re)writes the bf16 twin
+  state().last_conv_path = r.path;
+  emit.done = r.emitted;
+  if (fuse.drop_scale != 0.f && !r.dropped) {      // the kernel could not apply the dropout: one pass, which also (re)writes the bf16 twin
     dropout_apply(targets, g.out_total, fuse.drop_prob, fuse.drop_scale, fuse.drop_seed, emit.buf);
-    if (emit.buf) emit.done = true;
+    emit.done = true;
   }
   emit.finish();
 }
@@ -74,12 +65,16 @@ void conv_down(const ConvGeom& g, const float* derivs, const float* filters, flo
   const float* late_mask = nullptr;
   const int late_act = fuse.state_act;
   if (fuse.act_state && !whole) { late_mask = fuse.act_state; fuse.act_state = nullptr; fuse.state_act = kActNone; }
-  Emit emit(targets, g.img_total, fuse.emit_bf16 != 0);
-  if (!late_mask) emit.attach(fuse);               // a late mask changes the values after the kernel: convert afterwards
-  if (!(state().precision != kPrecFP32 && tc_conv_down(g, derivs, filters, targets, st, so, fuse))) {
+  // a late mask changes the values after the kernel: convert afterwards
+  Emit emit(targets, g.img_total, fuse.emit_bf16 != 0, !late_mask);
+  ConvOutcome r;
+  if (state().precision != kPrecFP32) r = tc_conv_down(g, derivs, filters, targets, st, so, fuse, emit.buf);
+  if (r.path == kPathNone) {
     simt_conv_down(g, derivs, filters, targets, st, so, fuse);
-    state().last_conv_path = kPathSimt;
+    r.path = kPathSimt;
   }
+  state().last_conv_path = r.path;
+  emit.done = r.emitted;
   if (late_mask) {
     const long long n4 = g.img_total;             // (these passes would consume a pending fuse request; none is pending here)
     if (late_act == kActLogistic) cnb_logistic_deriv(targets, late_mask, n4);
@@ -104,15 +99,14 @@ void simt_outp_auto(const ConvGeom& g, const float* images, const float* derivs,
 
 void conv_outp(const ConvGeom& g, const float* images, const float* derivs, float* targets, float st, float so) {
   take_fuse();                                 // a wgrad call has no epilogue to fuse: a pending request must not leak to a later call
-  if (!g.conv) {                               // untied: one [Cout x K] block per module
-    if (state().precision != kPrecFP32 && tc_conv_outp(g, images, derivs, targets, st, so)) return;
-    simt_conv_outp(g, images, derivs, targets, 1, 1, true, st, so);
-    state().last_conv_path = kPathSimt;
-    return;
+  ConvPath path = kPathNone;
+  if (state().precision != kPrecFP32) path = tc_conv_outp(g, images, derivs, targets, st, so);
+  if (path == kPathNone) {
+    if (!g.conv) simt_conv_outp(g, images, derivs, targets, 1, 1, true, st, so);   // untied: one [Cout x K] block per module
+    else simt_outp_auto(g, images, derivs, targets, st, so);
+    path = kPathSimt;
   }
-  if (state().precision != kPrecFP32 && tc_conv_outp(g, images, derivs, targets, st, so)) return;
-  simt_outp_auto(g, images, derivs, targets, st, so);
-  state().last_conv_path = kPathSimt;
+  state().last_conv_path = path;
 }
 
 void do_conv_up(const char* what, cudamat* images, cudamat* filters, cudamat* targets, Shape4D* is, Shape4D* fs,
@@ -223,7 +217,7 @@ void do_rnorm_undo(const char* what, cudamat* outGrads, cudamat* inputs, cudamat
   const long long L = els / F / frames;
   const Fuse fuse = take_fuse();
   CNB_REQUIRE(!fuse.bias_grad, "ResponseNormCrossMapUndo: no fused bias gradient here");
-  Emit emit(targets->data_device, els, fuse.emit_bf16 != 0);
+  Emit emit(targets->data_device, els, fuse.emit_bf16 != 0, false);
   for (int t = 0; t < frames; t++)
     rnorm_undo(outGrads->data_device + (long long)t * L * F, inputs->data_device + (long long)t * L * F,
                targets->data_device + (long long)t * L * F, L, F, sizeF, a, b, blocked);

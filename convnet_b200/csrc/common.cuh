@@ -104,7 +104,6 @@ struct Fuse {
   // fprop: dropout after bias / ReLU (convnet_b200_fuse_next_dropout): element i (its index in the target tensor) is kept
   // iff dropout_uniform(seed + i) >= drop_prob, kept values are multiplied by drop_scale; drop_scale == 0: no dropout
   float drop_prob = 0.f, drop_scale = 0.f; unsigned long long drop_seed = 0;
-  bool* dropped = nullptr;           // internal: the kernel sets it when it applied the dropout itself
   int prestage = 0;                  // convDown*: only build what the call can prepare from the FILTERS (convnet_b200_prestage_next)
   int pool_cache = 0;                // MaxPool*: also record the tie masks for the matching MaxPoolUndo* (convnet_b200_pool_cache_next)
   float out_scale = 1.f;             // dgrad: result multiplied by this (the kept-unit scale of a dropout layer, see ext.h)
@@ -112,9 +111,6 @@ struct Fuse {
   // the writer also produces the bias gradient of the edge that consumes the target as its output derivative
   // (convnet_b200_fuse_next_bias_grad): grad_bias[c] = bg_st*grad_bias[c] + bg_so * sum over images and positions
   float* bias_grad = nullptr; float bg_st = 0.f, bg_so = 1.f;
-  // internal (filled by the ABI wrapper): where the bf16 twin of the target goes; a kernel that writes it sets *emitted
-  __nv_bfloat16* out16 = nullptr;
-  bool* emitted = nullptr;
   bool any() const { return bias || act || act_state || drop_scale != 0.f; }
   // the ReLU' mask, for the kernels that fuse only that derivative (pool undo); nullptr otherwise
   const float* relu_mask() const { return state_act == kActRelu ? act_state : nullptr; }
@@ -146,5 +142,9 @@ inline Fuse take_fuse() { Fuse f = state().fuse; state().fuse = Fuse(); return f
 
 template <typename T>
 __host__ __device__ inline T ceil_div(T a, T b) { return (a + b - 1) / b; }
+// float4 / TMA access needs 16-byte aligned addresses
+inline bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
+// sub-buffers carved out of one allocation start on 1 KiB boundaries
+inline size_t align_up(size_t v) { return (v + 1023) & ~size_t(1023); }
 
 }  // namespace cnb

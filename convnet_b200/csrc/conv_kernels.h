@@ -19,16 +19,19 @@ void scale_buffer(float* a, long long n, float s);
 void reduce_partials(const float* part, float* out, long long elems, int groups, int per, float st, float so);
 
 // conv_tc.cu — TMA-fed implicit GEMM on the sm_90a tensor cores (wgmma bf16, mma.sync tf32)
-bool tc_conv_up(const ConvGeom& g, const float* images, const float* filters, float* targets,
-                float scaleTargets, float scaleOutput, const Fuse& fuse);
+// What a tensor-core call did: the path it took (kPathNone: it declined the call), whether its kernel wrote the bf16 twin
+// `targets_bf16` it was handed, and whether it applied the requested dropout itself.
+struct ConvOutcome { int path = kPathNone; bool emitted = false, dropped = false; };
+ConvOutcome tc_conv_up(const ConvGeom& g, const float* images, const float* filters, float* targets,
+                       float scaleTargets, float scaleOutput, const Fuse& fuse, __nv_bfloat16* targets_bf16);
 int extract_patches(const float* images, float* patches, const float* width_offset, const float* height_offset, const float* flip,
                     int N, int W, int H, int pw, int ph, int C);                                          // elementwise.cu
 void dropout_apply(float* x, long long n, float dropprob, float scale, unsigned long long seed, __nv_bfloat16* out16);   // elementwise.cu
 void tc_conv_down_prestage(const ConvGeom& g, const float* derivs, const float* filters);   // builds the dgrad filter banks, if that path will run
-bool tc_conv_down(const ConvGeom& g, const float* derivs, const float* filters, float* targets,
-                  float scaleTargets, float scaleOutput, const Fuse& fuse);
-bool tc_conv_outp(const ConvGeom& g, const float* images, const float* derivs, float* targets,
-                  float scaleTargets, float scaleOutput);
+ConvOutcome tc_conv_down(const ConvGeom& g, const float* derivs, const float* filters, float* targets,
+                         float scaleTargets, float scaleOutput, const Fuse& fuse, __nv_bfloat16* targets_bf16);
+ConvPath tc_conv_outp(const ConvGeom& g, const float* images, const float* derivs, float* targets,
+                      float scaleTargets, float scaleOutput);                  // kPathNone: declined
 
 // stage.cu — bf16 operand copies and their coherence (convnet_b200_bf16_stage / _ensure / _invalidate / emit)
 bool want_bf16();
@@ -57,10 +60,15 @@ const __nv_bfloat16* dgrad_weights(const float* filters, const ConvGeom& g, cons
 // max-pool tie masks (stage.cu), see pool.cu
 uint16_t* pool_masks_slot(const float* acts, long long n_out, const float* images, long long n_in, unsigned long long sig);
 const uint16_t* pool_masks_find(const float* acts, long long n_out, const float* images, unsigned long long sig);
-// writer protocol: begin_write drops stale copies and returns the buffer the kernel must fill when it can emit; end_write
-// falls back to a conversion pass when emission was wanted but the kernel could not do it
-__nv_bfloat16* begin_write(float* target, long long n, bool want_emit, bool kernel_can_emit);
-void end_write(float* target, long long n, bool want_emit, const __nv_bfloat16* emitted);
+// Writer protocol of every entry point that writes a tensor: construction drops the staged bf16 copies overlapping the
+// target.  When the caller asked for a fresh copy (`want`, convnet_b200_emit_bf16_next) and the kernel can write it, `buf`
+// is the twin it fills (nullptr outside bf16 mode), and the caller sets `done` once a kernel has filled it; finish()
+// converts in a trailing pass when nobody did.
+struct Emit {
+  float* target; long long n; bool want; __nv_bfloat16* buf = nullptr; bool done = false;
+  Emit(float* target, long long n, bool want, bool kernel_can_emit = true);
+  void finish();
+};
 
 // pool.cu
 // targets_bf16 (may be null): also write the bf16 twin of the target; the return value says whether the kernel did

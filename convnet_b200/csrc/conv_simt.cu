@@ -294,7 +294,7 @@ __global__ void __launch_bounds__(256) reduce_partials_v4_kernel(const float4* _
 }
 
 void reduce_partials(const float* part, float* out, long long elems, int groups, int per, float st, float so) {
-  if (groups == 1 && elems % 4 == 0 && ((reinterpret_cast<uintptr_t>(part) | reinterpret_cast<uintptr_t>(out)) & 15) == 0) {
+  if (groups == 1 && elems % 4 == 0 && aligned16(part) && aligned16(out)) {
     const long long e4 = elems / 4;
     const int blocks = (int)std::min<long long>(std::max<long long>(ceil_div<long long>(e4, 256), 1), 8LL * num_sms());
     reduce_partials_v4_kernel<<<blocks, 256, 0, state().stream>>>((const float4*)part, (float4*)out, e4, per, st, so);

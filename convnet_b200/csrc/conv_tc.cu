@@ -745,18 +745,13 @@ void launch(const CUtensorMap& a, const CUtensorMap& b, TcParams& p) {
   p.stages = pick_stages(p.bank_bytes);
   const size_t smem = smem_bytes_for(p.stages, p.bank_bytes);
   const bool sig = p.act == kActLogistic || (p.mask && p.mask_act == kActLogistic);
-  if constexpr (OP != kWgrad) {                       // (a wgrad has no activation to apply)
-    if (sig) {
-      if (p.bf16) launch_one<OP, true, true>(a, b, p, smem);
-      else launch_one<OP, false, true>(a, b, p, smem);
-      count_launch();
-      CNB_LAUNCH_CHECK("tc_conv");
-      return;
-    }
+  CNB_REQUIRE(OP != kWgrad || !sig, "tc_conv: wgrad has no activation epilogue");
+  void (*run)(const CUtensorMap&, const CUtensorMap&, const TcParams&, size_t) = nullptr;
+  if constexpr (OP != kWgrad) {                       // (no SIG instance of the wgrad kernel exists)
+    if (sig) run = p.bf16 ? launch_one<OP, true, true> : launch_one<OP, false, true>;
   }
-  CNB_REQUIRE(!sig, "tc_conv: wgrad has no activation epilogue");
-  if (p.bf16) launch_one<OP, true, false>(a, b, p, smem);
-  else launch_one<OP, false, false>(a, b, p, smem);
+  if (!run) run = p.bf16 ? launch_one<OP, true, false> : launch_one<OP, false, false>;
+  run(a, b, p, smem);
   count_launch();
   CNB_LAUNCH_CHECK("tc_conv");
 }
@@ -833,7 +828,22 @@ bool filter_map(CUtensorMap* m, const void* base, const Elem& e, long long cols,
 // floats in the filter tensor of a call: Cout x K, times the modules for untied filters
 inline long long filter_elems(const ConvGeom& g) { return (long long)g.Cout * g.K * (g.conv ? 1 : g.modules); }
 
-inline size_t align_up(size_t v) { return (v + 1023) & ~size_t(1023); }
+// fp32 operand of a call: the caller's tensor, its length in floats, and the element the kernel starts reading at
+struct Operand { const float* src; long long n; long long off; };
+// What the kernels of one call read: operands x and y, and `part_bytes` of partial sums at the start of the workspace.
+// bf16: each operand's staged copy, or a copy converted into the workspace behind the partial sums (x first, then y);
+// tf32: the fp32 buffers as they are.
+struct CallBuffers { const void* x; const void* y; float* part; };
+CallBuffers call_buffers(bool bf, size_t part_bytes, const Operand& x, const Operand& y) {
+  if (!bf) return {x.src + x.off, y.src + y.off, part_bytes ? (float*)workspace(part_bytes) : nullptr};
+  const __nv_bfloat16* sx = bf16_staged(x.src, x.n);
+  const __nv_bfloat16* sy = bf16_staged(y.src, y.n);
+  const size_t xb = sx ? 0 : align_up((size_t)x.n * 2), yb = sy ? 0 : align_up((size_t)y.n * 2);
+  uint8_t* ws = part_bytes + xb + yb ? (uint8_t*)workspace(part_bytes + xb + yb) : nullptr;
+  if (!sx) { to_bf16(x.src, (__nv_bfloat16*)(ws + part_bytes), x.n); sx = (const __nv_bfloat16*)(ws + part_bytes); }
+  if (!sy) { to_bf16(y.src, (__nv_bfloat16*)(ws + part_bytes + xb), y.n); sy = (const __nv_bfloat16*)(ws + part_bytes + xb); }
+  return {sx + x.off, sy + y.off, (float*)ws};
+}
 
 // ---- split-K for 1x1 / FC shapes: too few output tiles to fill the GPU, long K ------------------------
 // out = st*out + so * sum_s part[s]  (+ bias[channel], act | times mask_act'(mask)): the fused epilogue moves here
@@ -870,37 +880,53 @@ void reduce_split(const float* part, float* out, long long elems, int splits, fl
   count_launch();
   CNB_LAUNCH_CHECK("reduce_split");
 }
-// how many K splits a fprop/dgrad launch should use (1 = none): only 1x1 / FC shapes that leave most SMs idle
-int pick_ksplit(const TcParams& p, const ConvGeom& g, long long out_elems) {
-  if (p.x_mode || p.taps != 1 || g.frames != 1 || out_elems % 4 != 0) return 1;
-  if (p.num_tiles * 2 > num_sms() || p.kc_blocks < 8) return 1;
-  const int want = std::min(num_sms() / p.num_tiles, p.kc_blocks / 4);
-  return std::max(want, 1);
+// The fprop-form GEMM of a launch (fprop, dgrad, dgrad in fprop form): `total_chunks` image chunks of rows, `cols`
+// columns in n-tiles of p.BN, K in blocks of p.bk over `k_channels` channels.
+void set_tiles(TcParams& p, int total_chunks, int cols, int k_channels) {
+  p.kc_blocks = ceil_div(k_channels, p.bk);
+  p.total_chunks = total_chunks;
+  p.m_tiles = ceil_div(p.total_chunks, p.cpt);
+  p.n_tiles = ceil_div(cols, p.BN);
+  p.num_tiles = p.m_tiles * p.n_tiles;
+  // MN-major B is staged in whole chunks (BN is a multiple of the chunk); x-mode streams A alone
+  p.b_tx_bytes = p.x_mode ? 0u : (uint32_t)p.BN * 128;
 }
-inline bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
+// Split-K of a fprop/dgrad launch writing out_elems floats, where the caller's layout `allows` it: only 1x1 / FC shapes
+// that leave most SMs idle split.  Returns the bytes of partial sums the launch needs (0: no split).
+size_t split_k(TcParams& p, const ConvGeom& g, long long out_elems, bool allowed) {
+  if (!allowed || p.x_mode || p.taps != 1 || g.frames != 1 || out_elems % 4 != 0) return 0;
+  if (p.num_tiles * 2 > num_sms() || p.kc_blocks < 8) return 0;
+  const int ks = std::max(std::min(num_sms() / p.num_tiles, p.kc_blocks / 4), 1);
+  if (ks > 1) {
+    p.units_per_split = ceil_div(p.kc_blocks, ks);
+    p.splits = ceil_div(p.kc_blocks, p.units_per_split);
+    p.part_stride = out_elems;
+    p.num_tiles *= p.splits;
+  }
+  return p.splits > 1 ? align_up(sizeof(float) * out_elems * p.splits) : 0;
+}
 
 }  // namespace
 
 // ---- fprop ---------------------------------------------------------------------------------------
 // `bf` selects bf16 operands (CONVNET_B200_PRECISION=bf16): images and filters are first rounded to bf16 copies in
 // library scratch (unless the caller keeps staged copies), then the bf16 flavour of the kernel runs wgmma on them.
-static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float* filters, float* targets, float st, float so,
-                            const Fuse& fuse, bool bf) {
+static ConvOutcome tc_conv_up_impl(const ConvGeom& g, const float* images, const float* filters, float* targets, float st,
+                                   float so, const Fuse& fuse, __nv_bfloat16* out16, bool bf) {
   const Elem e = elem_for(bf);
-  if (g.N % 4 != 0 || g.Cout % 4 != 0) return false;                        // TMA stride alignment
+  if (g.N % 4 != 0 || g.Cout % 4 != 0) return {};                           // TMA stride alignment
   const bool x_mode = g.Cin < 8;                                            // tiny channel counts: taps take the K block
-  if (x_mode && (g.kx > 8 || g.ky > 8)) return false;
-  if (bf && (x_mode || g.N % 8 != 0 || g.Cout % 8 != 0 || !aligned16(images) || !aligned16(filters))) return false;
-  if (!g.conv && (g.N % 128 != 0 || g.frames != 1 || x_mode)) return false;   // untied: each m-tile in one module
+  if (x_mode && (g.kx > 8 || g.ky > 8)) return {};
+  if (bf && (x_mode || g.N % 8 != 0 || g.Cout % 8 != 0 || !aligned16(images) || !aligned16(filters))) return {};
+  if (!g.conv && (g.N % 128 != 0 || g.frames != 1 || x_mode)) return {};     // untied: each m-tile in one module
   const long long flt_n = filter_elems(g);
   // few GEMM rows (FC layers at training batch sizes): the call streams the weights once and is HBM-bound on them; a bf16
   // conversion pass inside the call would read them a second time, so such shapes take bf16 only when the caller keeps a
   // staged bf16 copy of the weights (the training host does: cnb_sgd_momentum refreshes it in the same pass that updates
   // them) — then the call streams HALF the bytes
-  if (bf && (long long)g.N * g.modules * g.frames < 1024 && !bf16_staged(filters, flt_n)) return false;
+  if (bf && (long long)g.N * g.modules * g.frames < 1024 && !bf16_staged(filters, flt_n)) return {};
   TcParams p; fill_common(p, g, e);
   p.BN = pick_bn(g.Cout, e.chunk);
-  p.kc_blocks = ceil_div(g.Cin, e.bk);
   p.x_mode = x_mode ? 1 : 0;
   p.x_yblocks = ceil_div(g.ky, 4);
   if (x_mode) {
@@ -912,49 +938,23 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
     p.xw = filters;
   }
   const long long chunks = (long long)p.nb * g.modules * g.frames;
-  if (chunks * 4 >= (1LL << 31)) return false;
-  p.total_chunks = p.nbc * g.modules * g.frames;
-  p.m_tiles = ceil_div(p.total_chunks, p.cpt);
-  p.n_tiles = ceil_div(g.Cout, p.BN);
-  p.num_tiles = p.m_tiles * p.n_tiles;
-  // MN-major B is staged in whole chunks (BN is a multiple of the chunk); x-mode streams A alone
-  p.b_tx_bytes = x_mode ? 0u : (uint32_t)p.BN * 128;
+  if (chunks * 4 >= (1LL << 31)) return {};
+  set_tiles(p, p.nbc * g.modules * g.frames, g.Cout, g.Cin);
   float* const out = targets + (long long)g.cout0 * g.modules * g.N;
   const float* const bias = fuse.bias ? fuse.bias + (long long)g.cout0 * (g.conv ? 1 : g.modules) : nullptr;
   const long long out_elems = (long long)g.Cout * g.modules * g.N;
-  const int ks = g.conv ? pick_ksplit(p, g, out_elems) : 1;
-  if (ks > 1) {
-    p.units_per_split = ceil_div(p.kc_blocks, ks);
-    p.splits = ceil_div(p.kc_blocks, p.units_per_split);
-    p.part_stride = out_elems;
-    p.num_tiles *= p.splits;
-  }
-  const size_t part_bytes = p.splits > 1 ? align_up(sizeof(float) * out_elems * p.splits) : 0;
+  const size_t part_bytes = split_k(p, g, out_elems, g.conv);
   p.out = out;
   p.st = st; p.so = so;
   p.bias = bias; p.act = fuse.act;
   CUtensorMap ma, mb;
-  const long long img_off = (long long)g.cin0 * g.H * g.W * g.N;
-  const void* img = images + img_off;
-  const void* flt = filters;
+  const CallBuffers buf = call_buffers(bf, part_bytes, {images, g.img_total, (long long)g.cin0 * g.H * g.W * g.N},
+                                       {filters, flt_n, 0});
   const long long taps = (long long)g.kx * g.ky;
-  uint8_t* ws = nullptr;
-  if (bf) {
-    const __nv_bfloat16* si = bf16_staged(images, g.img_total);
-    const __nv_bfloat16* sf = bf16_staged(filters, flt_n);
-    const size_t ib = si ? 0 : align_up((size_t)g.img_total * 2), fb = sf ? 0 : align_up((size_t)flt_n * 2);
-    if (part_bytes + ib + fb) ws = (uint8_t*)workspace(part_bytes + ib + fb);
-    if (!si) { to_bf16(images, (__nv_bfloat16*)(ws + part_bytes), g.img_total); si = (const __nv_bfloat16*)(ws + part_bytes); }
-    if (!sf) { to_bf16(filters, (__nv_bfloat16*)(ws + part_bytes + ib), flt_n); sf = (const __nv_bfloat16*)(ws + part_bytes + ib); }
-    img = si + img_off;
-    flt = sf;
-  } else if (part_bytes) {
-    ws = (uint8_t*)workspace(part_bytes);
-  }
-  if (p.splits > 1) { p.out = (float*)ws; p.bias = nullptr; p.act = 0; }    // partial sums; the epilogue moves to reduce_split
+  if (p.splits > 1) { p.out = buf.part; p.bias = nullptr; p.act = 0; }    // partial sums; the epilogue moves to reduce_split
   // bf16 twin of the output from the same registers: only when this launch writes the final value of EVERY element
-  const bool emit = fuse.out16 != nullptr && p.splits == 1 && g.cout0 == 0 && g.Cout == g.CoutT;
-  if (emit) p.out16 = fuse.out16;
+  const bool emit = out16 != nullptr && p.splits == 1 && g.cout0 == 0 && g.Cout == g.CoutT;
+  if (emit) p.out16 = out16;
   // dropout in the epilogue: the element index is the offset from the start of the WHOLE target tensor
   const bool drop = fuse.drop_scale != 0.f && p.splits == 1 && g.frames == 1 && g.cout0 == 0 && g.Cout == g.CoutT;
   if (drop) { p.drop_prob = fuse.drop_prob; p.drop_scale = fuse.drop_scale; p.drop_seed = fuse.drop_seed; }
@@ -964,32 +964,32 @@ static bool tc_conv_up_impl(const ConvGeom& g, const float* images, const float*
   if (x_mode) {
     const long long N = g.N;
     if (p.a_merged) {
-      if (!merged_image_map(&ma, img, e, g, g.W, g.H, g.Cin, true)) return false;
+      if (!merged_image_map(&ma, buf.x, e, g, g.W, g.H, g.Cin, true)) return {};
     } else {
       const long long adims[5] = {N, g.Cin, g.W, g.H, g.frames};
       const long long astr[4] = {N * g.W * g.H, N, N * g.W, g.in_frame_step};
       const int abox[5] = {32, 1, 8, 4, 1};                     // 8 x-taps x 4 filter rows of one channel
-      if (!make_map(&ma, img, e, 5, adims, astr, abox)) return false;
+      if (!make_map(&ma, buf.x, e, 5, adims, astr, abox)) return {};
     }
     mb = ma;                                                    // no B map: the kernel reads the filters into its bank
   } else {
     if (p.a_merged) {
-      if (!merged_image_map(&ma, img, e, g, g.W, g.H, g.Cin, false)) return false;
-    } else if (!image_map(&ma, img, e, g, g.W, g.H, g.Cin, g.in_frame_step, true, e.bk)) return false;
-    if (!filter_map(&mb, flt, e, g.Cout, taps, g.Cin, p.BN, p.b_merged, g.conv ? 0 : g.modules)) return false;
+      if (!merged_image_map(&ma, buf.x, e, g, g.W, g.H, g.Cin, false)) return {};
+    } else if (!image_map(&ma, buf.x, e, g, g.W, g.H, g.Cin, g.in_frame_step, true, e.bk)) return {};
+    if (!filter_map(&mb, buf.y, e, g.Cout, taps, g.Cin, p.BN, p.b_merged, g.conv ? 0 : g.modules)) return {};
   }
   launch<kFprop>(ma, mb, p);
-  if (emit && fuse.emitted) *fuse.emitted = true;
-  if (drop && fuse.dropped) *fuse.dropped = true;
   if (p.splits > 1)
-    reduce_split((const float*)ws, out, out_elems, p.splits, st, so, bias, (long long)g.modules * g.N, fuse.act, nullptr, 0);
-  state().last_conv_path = bf ? kPathTcBf16 : kPathTcTf32;
-  return true;
+    reduce_split(buf.part, out, out_elems, p.splits, st, so, bias, (long long)g.modules * g.N, fuse.act, nullptr, 0);
+  return {bf ? kPathTcBf16 : kPathTcTf32, emit, drop};
 }
-bool tc_conv_up(const ConvGeom& g, const float* images, const float* filters, float* targets, float st, float so,
-                const Fuse& fuse) {
-  if (want_bf16() && tc_conv_up_impl(g, images, filters, targets, st, so, fuse, true)) return true;
-  return tc_conv_up_impl(g, images, filters, targets, st, so, fuse, false);
+ConvOutcome tc_conv_up(const ConvGeom& g, const float* images, const float* filters, float* targets, float st, float so,
+                       const Fuse& fuse, __nv_bfloat16* out16) {
+  if (want_bf16()) {
+    const ConvOutcome r = tc_conv_up_impl(g, images, filters, targets, st, so, fuse, out16, true);
+    if (r.path != kPathNone) return r;
+  }
+  return tc_conv_up_impl(g, images, filters, targets, st, so, fuse, out16, false);
 }
 
 
@@ -1015,10 +1015,10 @@ void tc_conv_down_prestage(const ConvGeom& g, const float* derivs, const float* 
   dgrad_weights(filters, g, banks);
 }
 
-static bool tc_conv_down_as_fprop(const ConvGeom& g, const float* derivs, const float* filters, float* targets, float so,
-                                  const Fuse& fuse) {
+static ConvOutcome tc_conv_down_as_fprop(const ConvGeom& g, const float* derivs, const float* filters, float* targets,
+                                         float so, const Fuse& fuse, __nv_bfloat16* out16) {
   DgradBanks banks;
-  if (!dgrad_as_fprop_eligible(g, derivs, filters, &banks)) return false;
+  if (!dgrad_as_fprop_eligible(g, derivs, filters, &banks)) return {};
   const Elem e = elem_for(true);
   // the derivative as bf16 (staged by the producer, or converted here)
   const __nv_bfloat16* sd = bf16_staged(derivs, g.out_total);
@@ -1037,14 +1037,9 @@ static bool tc_conv_down_as_fprop(const ConvGeom& g, const float* derivs, const 
     p.kx = P.ku; p.ky = P.kv; p.taps = P.ku * P.kv; p.sx = p.sy = 1; p.px = P.px; p.py = P.py;
     p.Cin = g.Cout; p.Cout = g.Cin;
     p.BN = pick_bn(g.Cin, 64);
-    p.kc_blocks = ceil_div(g.Cout, e.bk);
-    p.total_chunks = p.nbc * p.modules;
-    p.m_tiles = ceil_div(p.total_chunks, p.cpt);
-    p.n_tiles = ceil_div(g.Cin, p.BN);
-    p.num_tiles = p.m_tiles * p.n_tiles;
-    p.b_tx_bytes = (uint32_t)p.BN * 128;
+    set_tiles(p, p.nbc * p.modules, g.Cin, g.Cout);
     p.out = targets; p.st = 0.f; p.so = so;
-    p.mask = fuse.act_state; p.mask_act = fuse.state_act; p.out16 = fuse.out16;
+    p.mask = fuse.act_state; p.mask_act = fuse.state_act; p.out16 = out16;
     p.o_sx = g.sx; p.o_sy = g.sy; p.o_x0 = P.a; p.o_y0 = P.b; p.o_W = g.W; p.out_plane = (long long)g.W * g.H;
     p.a_merged = 1;
     p.b_merged = (g.Cin % 64 == 0) ? 1 : 0;
@@ -1052,83 +1047,56 @@ static bool tc_conv_down_as_fprop(const ConvGeom& g, const float* derivs, const 
     if (!merged_image_map(&fa, sd, e, g, g.modX, g.modY, g.Cout, false) ||
         !filter_map(&fb, bank + P.offset, e, g.Cin, p.taps, g.Cout, p.BN, p.b_merged)) {
       CNB_REQUIRE(i == 0, "dgrad-as-fprop: tensor map failed after the first phase");
-      return false;
+      return {};
     }
     launch<kFprop>(fa, fb, p);
   }
-  if (fuse.out16 && fuse.emitted) *fuse.emitted = true;
-  state().last_conv_path = kPathTcBf16;
-  return true;
+  return {kPathTcBf16, out16 != nullptr, false};
 }
 
 // ---- dgrad ---------------------------------------------------------------------------------------
-static bool tc_conv_down_impl(const ConvGeom& g, const float* derivs, const float* filters, float* targets, float st, float so,
-                              const Fuse& fuse, bool bf) {
+static ConvOutcome tc_conv_down_impl(const ConvGeom& g, const float* derivs, const float* filters, float* targets, float st,
+                                     float so, const Fuse& fuse, __nv_bfloat16* out16, bool bf) {
   const Elem e = elem_for(bf);
-  if (g.N % 4 != 0 || g.Cout % 4 != 0 || g.Cout < 8 || g.Cin < 8) return false;
-  if (bf && (g.N % 8 != 0 || g.Cout % 8 != 0 || !aligned16(derivs) || !aligned16(filters))) return false;
-  if (!g.conv && (g.N % 128 != 0 || g.frames != 1)) return false;          // untied: each m-tile on one input pixel
+  if (g.N % 4 != 0 || g.Cout % 4 != 0 || g.Cout < 8 || g.Cin < 8) return {};
+  if (bf && (g.N % 8 != 0 || g.Cout % 8 != 0 || !aligned16(derivs) || !aligned16(filters))) return {};
+  if (!g.conv && (g.N % 128 != 0 || g.frames != 1)) return {};             // untied: each m-tile on one input pixel
   const long long flt_n = filter_elems(g);
-  if (bf && (long long)g.N * g.W * g.H < 1024 && !bf16_staged(filters, flt_n)) return false;   // see tc_conv_up_impl
+  if (bf && (long long)g.N * g.W * g.H < 1024 && !bf16_staged(filters, flt_n)) return {};   // see tc_conv_up_impl
   TcParams p; fill_common(p, g, e);
   p.BN = pick_bn(g.Cin, 16);
-  p.kc_blocks = ceil_div(g.Cout, e.bk);
   const long long chunks = (long long)p.nb * g.W * g.H;
-  if (chunks * 4 >= (1LL << 31) || g.kx > 32 || g.ky > 32) return false;
-  p.total_chunks = p.nbc * g.W * g.H;
-  p.m_tiles = ceil_div(p.total_chunks, p.cpt);
-  p.n_tiles = ceil_div(g.Cin, p.BN);
-  p.num_tiles = p.m_tiles * p.n_tiles;
+  if (chunks * 4 >= (1LL << 31) || g.kx > 32 || g.ky > 32) return {};
+  set_tiles(p, p.nbc * g.W * g.H, g.Cin, g.Cout);
   p.so = so;
-  p.b_tx_bytes = (uint32_t)p.BN * 128;
   const bool whole = (g.frames == 1 && g.cin0 == 0 && g.Cin == g.CinT);
   const long long out_elems = (long long)g.Cin * g.W * g.H * g.N;
-  const int ks = whole && g.conv ? pick_ksplit(p, g, out_elems) : 1;
-  if (ks > 1) {
-    p.units_per_split = ceil_div(p.kc_blocks, ks);
-    p.splits = ceil_div(p.kc_blocks, p.units_per_split);
-    p.part_stride = out_elems;
-    p.num_tiles *= p.splits;
-  }
-  const size_t part_bytes = p.splits > 1 ? align_up(sizeof(float) * out_elems * p.splits) : 0;
+  const size_t part_bytes = split_k(p, g, out_elems, whole && g.conv);
   CUtensorMap ma, mb;
-  const long long der_off = (long long)g.cout0 * g.modules * g.N;
-  const void* der = derivs + der_off;
-  const void* flt = filters;
-  uint8_t* ws = nullptr;
-  if (bf) {
-    const __nv_bfloat16* sd = bf16_staged(derivs, g.out_total);
-    const __nv_bfloat16* sf = bf16_staged(filters, flt_n);
-    const size_t db = sd ? 0 : align_up((size_t)g.out_total * 2), fb = sf ? 0 : align_up((size_t)flt_n * 2);
-    if (part_bytes + db + fb) ws = (uint8_t*)workspace(part_bytes + db + fb);
-    if (!sd) { to_bf16(derivs, (__nv_bfloat16*)(ws + part_bytes), g.out_total); sd = (const __nv_bfloat16*)(ws + part_bytes); }
-    if (!sf) { to_bf16(filters, (__nv_bfloat16*)(ws + part_bytes + db), flt_n); sf = (const __nv_bfloat16*)(ws + part_bytes + db); }
-    der = sd + der_off;
-    flt = sf;
-  } else if (part_bytes) {
-    ws = (uint8_t*)workspace(part_bytes);
-  }
+  const CallBuffers buf = call_buffers(bf, part_bytes, {derivs, g.out_total, (long long)g.cout0 * g.modules * g.N},
+                                       {filters, flt_n, 0});
   p.a_merged = (g.frames == 1 && g.N % 128 == 0) ? 1 : 0;
   if (p.a_merged) {
-    if (!merged_image_map(&ma, der, e, g, g.modX, g.modY, g.Cout, false)) return false;
-  } else if (!image_map(&ma, der, e, g, g.modX, g.modY, g.Cout, g.out_frame_step, true, e.bk)) return false;
+    if (!merged_image_map(&ma, buf.x, e, g, g.modX, g.modY, g.Cout, false)) return {};
+  } else if (!image_map(&ma, buf.x, e, g, g.modX, g.modY, g.Cout, g.out_frame_step, true, e.bk)) return {};
   {                                                    // (o, tap, c[, module])
     const long long dims[4] = {g.Cout, (long long)g.kx * g.ky, g.Cin, g.modules};
     const long long str[3] = {g.Cout, (long long)g.Cout * g.kx * g.ky, (long long)g.Cout * g.K};
     const int box[4] = {e.chunk, 1, p.BN, 1};
-    if (!make_map(&mb, flt, e, g.conv ? 3 : 4, dims, str, box)) return false;
+    if (!make_map(&mb, buf.y, e, g.conv ? 3 : 4, dims, str, box)) return {};
   }
   float* out = targets + (long long)g.cin0 * g.H * g.W * g.N;
+  bool emit = false;
   if (whole && p.splits > 1) {
-    p.st = 0.f; p.out = (float*)ws; p.mask = nullptr;
+    p.st = 0.f; p.out = buf.part; p.mask = nullptr;
     launch<kDgrad>(ma, mb, p);
-    reduce_split((const float*)ws, out, out_elems, p.splits, st, so, nullptr, 1, 0, fuse.act_state, fuse.state_act);
+    reduce_split(buf.part, out, out_elems, p.splits, st, so, nullptr, 1, 0, fuse.act_state, fuse.state_act);
   } else if (whole) {
     p.st = st; p.out = out; p.mask = fuse.act_state ? fuse.act_state + (long long)g.cin0 * g.H * g.W * g.N : nullptr;
     p.mask_act = fuse.state_act;
-    p.out16 = fuse.out16;                              // `whole`: every element gets its final value here
+    p.out16 = out16;                                   // `whole`: every element gets its final value here
+    emit = out16 != nullptr;
     launch<kDgrad>(ma, mb, p);
-    if (fuse.out16 && fuse.emitted) *fuse.emitted = true;
   } else {
     // the reference scales the WHOLE target first (gemm.cu:760, conv3d_gemm.cu:98); frame windows overlap,
     // so frames are accumulated by stream-ordered launches
@@ -1139,28 +1107,31 @@ static bool tc_conv_down_impl(const ConvGeom& g, const float* derivs, const floa
       launch<kDgrad>(ma, mb, p);
     }
   }
-  state().last_conv_path = bf ? kPathTcBf16 : kPathTcTf32;
-  return true;
+  return {bf ? kPathTcBf16 : kPathTcTf32, emit, false};
 }
-bool tc_conv_down(const ConvGeom& g, const float* derivs, const float* filters, float* targets, float st, float so,
-                  const Fuse& fuse) {
-  if (want_bf16() && st == 0.f && tc_conv_down_as_fprop(g, derivs, filters, targets, so, fuse)) return true;
-  if (want_bf16() && tc_conv_down_impl(g, derivs, filters, targets, st, so, fuse, true)) return true;
-  return tc_conv_down_impl(g, derivs, filters, targets, st, so, fuse, false);
+ConvOutcome tc_conv_down(const ConvGeom& g, const float* derivs, const float* filters, float* targets, float st, float so,
+                         const Fuse& fuse, __nv_bfloat16* out16) {
+  if (want_bf16()) {
+    ConvOutcome r;
+    if (st == 0.f) r = tc_conv_down_as_fprop(g, derivs, filters, targets, so, fuse, out16);
+    if (r.path == kPathNone) r = tc_conv_down_impl(g, derivs, filters, targets, st, so, fuse, out16, true);
+    if (r.path != kPathNone) return r;
+  }
+  return tc_conv_down_impl(g, derivs, filters, targets, st, so, fuse, out16, false);
 }
 
 // ---- wgrad ---------------------------------------------------------------------------------------
-static bool tc_conv_outp_impl(const ConvGeom& g, const float* images, const float* derivs, float* targets, float st, float so,
-                              bool bf) {
+static ConvPath tc_conv_outp_impl(const ConvGeom& g, const float* images, const float* derivs, float* targets, float st,
+                                  float so, bool bf) {
   const Elem e = elem_for(bf);
-  if (g.N % 4 != 0 || g.Cout < 8) return false;
+  if (g.N % 4 != 0 || g.Cout < 8) return kPathNone;
   const bool x_mode = g.Cin < 8;
-  if (x_mode && (g.kx > 8 || g.ky > 8)) return false;
-  if (bf && (x_mode || g.N % 8 != 0 || !aligned16(images) || !aligned16(derivs))) return false;
-  if (!g.conv && (g.N % 128 != 0 || g.frames != 1 || x_mode)) return false;
+  if (x_mode && (g.kx > 8 || g.ky > 8)) return kPathNone;
+  if (bf && (x_mode || g.N % 8 != 0 || !aligned16(images) || !aligned16(derivs))) return kPathNone;
+  if (!g.conv && (g.N % 128 != 0 || g.frames != 1 || x_mode)) return kPathNone;
   // few reduction rows (FC layers: K = batch): the call is bound by WRITING dW, and the operands a bf16 pass would convert
   // are tiny — such shapes take bf16 only in the whole-batch-tile layout the training step uses
-  if (bf && (long long)g.N * g.modules * g.frames < 1024 && !(g.frames == 1 && g.N % 128 == 0 && g.Cin % 32 == 0)) return false;
+  if (bf && (long long)g.N * g.modules * g.frames < 1024 && !(g.frames == 1 && g.N % 128 == 0 && g.Cin % 32 == 0)) return kPathNone;
   TcParams p; fill_common(p, g, e);
   p.kc_blocks = 0;
   p.m_tiles = ceil_div(g.Cout, BM);
@@ -1199,46 +1170,34 @@ static bool tc_conv_outp_impl(const ConvGeom& g, const float* images, const floa
   p.units_per_split = ceil_div(units, splits);
   p.splits = ceil_div(units, p.units_per_split);
   if (!g.conv) {                 // untied: one tile per (module, tap, o-tile, c-tile), stored straight into its module's block
-    if (base_tiles * g.modules >= (1LL << 31)) return false;
+    if (base_tiles * g.modules >= (1LL << 31)) return kPathNone;
     p.splits = g.modules; p.units_per_split = 1;
   }
   p.num_tiles = (int)(base_tiles * p.splits);
   p.st = st; p.so = so;
   CUtensorMap ma, mb;
-  const long long img_off = (long long)g.cin0 * g.H * g.W * g.N, der_off = (long long)g.cout0 * g.modules * g.N;
-  const void* img = images + img_off;
-  const void* der = derivs + der_off;
   const bool partials = p.splits > 1 && g.conv;
   const size_t part_bytes = partials ? align_up(sizeof(float) * elems * p.splits) : 0;
-  uint8_t* ws = nullptr;
-  if (bf) {
-    const __nv_bfloat16* si = bf16_staged(images, g.img_total);
-    const __nv_bfloat16* sd = bf16_staged(derivs, g.out_total);
-    const size_t ib = si ? 0 : align_up((size_t)g.img_total * 2), db = sd ? 0 : align_up((size_t)g.out_total * 2);
-    if (part_bytes + ib + db) ws = (uint8_t*)workspace(part_bytes + ib + db);
-    if (!si) { to_bf16(images, (__nv_bfloat16*)(ws + part_bytes), g.img_total); si = (const __nv_bfloat16*)(ws + part_bytes); }
-    if (!sd) { to_bf16(derivs, (__nv_bfloat16*)(ws + part_bytes + ib), g.out_total); sd = (const __nv_bfloat16*)(ws + part_bytes + ib); }
-    img = si + img_off;
-    der = sd + der_off;
-  } else if (part_bytes) {
-    ws = (uint8_t*)workspace(part_bytes);
-  }
-  if (!image_map(&ma, der, e, g, g.modX, g.modY, g.Cout, g.out_frame_step, false, BM)) return false;
+  const CallBuffers buf = call_buffers(bf, part_bytes, {images, g.img_total, (long long)g.cin0 * g.H * g.W * g.N},
+                                       {derivs, g.out_total, (long long)g.cout0 * g.modules * g.N});
+  if (!image_map(&ma, buf.y, e, g, g.modX, g.modY, g.Cout, g.out_frame_step, false, BM)) return kPathNone;
   if (x_mode) {
     const long long N = g.N;
     const long long dims[5] = {N, g.W, g.H, g.Cin, g.frames};
     const long long str[4] = {N, N * g.W, N * g.W * g.H, g.in_frame_step};
     const int box[5] = {32, 8, g.ky, 1, 1};                   // 8 x-taps x ky rows of one channel: ky*8 GEMM columns
-    if (!make_map(&mb, img, e, 5, dims, str, box)) return false;
-  } else if (!image_map(&mb, img, e, g, g.W, g.H, g.Cin, g.in_frame_step, false, p.BN)) return false;
-  p.out = partials ? (float*)ws : targets;
+    if (!make_map(&mb, buf.x, e, 5, dims, str, box)) return kPathNone;
+  } else if (!image_map(&mb, buf.x, e, g, g.W, g.H, g.Cin, g.in_frame_step, false, p.BN)) return kPathNone;
+  p.out = partials ? buf.part : targets;
   launch<kWgrad>(ma, mb, p);
-  if (partials) reduce_partials((const float*)ws, targets, elems, 1, p.splits, st, so);
-  state().last_conv_path = bf ? kPathTcBf16 : kPathTcTf32;
-  return true;
+  if (partials) reduce_partials(buf.part, targets, elems, 1, p.splits, st, so);
+  return bf ? kPathTcBf16 : kPathTcTf32;
 }
-bool tc_conv_outp(const ConvGeom& g, const float* images, const float* derivs, float* targets, float st, float so) {
-  if (want_bf16() && tc_conv_outp_impl(g, images, derivs, targets, st, so, true)) return true;
+ConvPath tc_conv_outp(const ConvGeom& g, const float* images, const float* derivs, float* targets, float st, float so) {
+  if (want_bf16()) {
+    const ConvPath path = tc_conv_outp_impl(g, images, derivs, targets, st, so, true);
+    if (path != kPathNone) return path;
+  }
   return tc_conv_outp_impl(g, images, derivs, targets, st, so, false);
 }
 

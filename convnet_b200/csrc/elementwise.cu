@@ -19,7 +19,6 @@ __device__ __forceinline__ void emit4(__nv_bfloat16* out16, long long i4, const 
   reinterpret_cast<uint2*>(out16)[i4] = o;
 }
 
-static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 static int blocks_for(long long work, int threads) {
   return (int)std::max<long long>(1, std::min<long long>(ceil_div<long long>(work, threads), (long long)num_sms() * 16));
 }
@@ -45,16 +44,36 @@ __global__ void bias_kernel_scalar(float* acts, const float* __restrict__ bias, 
   }
 }
 
+// One pass writing the n floats of x, on the pending emit request (consumed even when there is nothing to write): the
+// writer protocol around launch(out16), where out16 is the twin the kernel fills (nullptr unless can_emit).
+template <class Launch>
+static void write_pass(const char* what, float* x, long long n, bool can_emit, const Launch& launch) {
+  const bool want = take_fuse().emit_bf16 != 0;
+  if (n <= 0) return;
+  Emit emit(x, n, want, can_emit);
+  launch(emit.buf);
+  count_launch(); CNB_LAUNCH_CHECK(what);
+  emit.done = can_emit;
+  emit.finish();
+}
+// ... for the kernels below that take n4 float4 groups (x and y, if given, 16-byte aligned) and a scalar tail in one launch
+template <class Launch>
+static void vec4_pass(const char* what, float* x, const float* y, long long n, bool can_emit, const Launch& launch) {
+  write_pass(what, x, n, can_emit, [&](__nv_bfloat16* out16) {
+    const long long n4 = (aligned16(x) && aligned16(y)) ? n / 4 : 0;
+    launch(blocks_for(std::max(n4, n - 4 * n4), 256), n4, out16);
+  });
+}
+
 template <bool RELU>
 static void bias_launch(float* acts, const float* bias, long long rows, int cols) {
-  if (rows <= 0 || cols <= 0) return;
-  if (rows % 4 == 0 && aligned16(acts)) {
-    bias_kernel<RELU><<<blocks_for(rows / 4 * cols, 256), 256, 0, state().stream>>>(acts, bias, rows, cols);
-  } else {
-    bias_kernel_scalar<RELU><<<blocks_for(rows * cols, 256), 256, 0, state().stream>>>(acts, bias, rows, cols);
-  }
-  count_launch();
-  CNB_LAUNCH_CHECK("add_channel_bias");
+  write_pass("add_channel_bias", acts, rows > 0 && cols > 0 ? rows * cols : 0, false, [&](__nv_bfloat16*) {
+    if (rows % 4 == 0 && aligned16(acts)) {
+      bias_kernel<RELU><<<blocks_for(rows / 4 * cols, 256), 256, 0, state().stream>>>(acts, bias, rows, cols);
+    } else {
+      bias_kernel_scalar<RELU><<<blocks_for(rows * cols, 256), 256, 0, state().stream>>>(acts, bias, rows, cols);
+    }
+  });
 }
 
 // Column reductions of a column-major [rows x cols] matrix (a column = one channel of a 2-D layer, DESIGN.md §3): one
@@ -735,16 +754,10 @@ using namespace cnb;
 extern "C" {
 
 void cnb_add_channel_bias(float* acts, const float* bias, long long rows, int cols) {
-  const bool emit = take_fuse().emit_bf16 != 0;
-  begin_write(acts, rows * cols, emit, false);
   bias_launch<false>(acts, bias, rows, cols);
-  end_write(acts, rows * cols, emit, nullptr);
 }
 void cnb_add_channel_bias_relu(float* acts, const float* bias, long long rows, int cols) {
-  const bool emit = take_fuse().emit_bf16 != 0;
-  begin_write(acts, rows * cols, emit, false);
   bias_launch<true>(acts, bias, rows, cols);
-  end_write(acts, rows * cols, emit, nullptr);
 }
 // A device buffer that grows on demand.  The partial sums of the bias gradient and those of the SGD row norms each have
 // their OWN, not the shared workspace: a host may run those passes on side streams beside conv kernels that are using the
@@ -782,40 +795,24 @@ void cnb_channel_bias_grad(const float* derivs, float* grad_bias, long long rows
   CNB_LAUNCH_CHECK("channel_bias_grad");
 }
 void cnb_relu(float* x, long long n) {
-  const bool emit = take_fuse().emit_bf16 != 0;
-  if (n <= 0) return;
-  const long long n4 = aligned16(x) ? n / 4 : 0;
-  __nv_bfloat16* o16 = begin_write(x, n, emit, true);
-  relu_kernel<<<blocks_for(std::max(n4, n - 4 * n4), 256), 256, 0, state().stream>>>(x, n, n4, o16);
-  count_launch(); CNB_LAUNCH_CHECK("relu");
-  end_write(x, n, emit, o16);
+  vec4_pass("relu", x, nullptr, n, true, [&](int grid, long long n4, __nv_bfloat16* o16) {
+    relu_kernel<<<grid, 256, 0, state().stream>>>(x, n, n4, o16);
+  });
 }
 void cnb_relu_deriv(float* dx, const float* y, long long n) {
-  const bool emit = take_fuse().emit_bf16 != 0;
-  if (n <= 0) return;
-  begin_write(dx, n, emit, false);
-  const long long n4 = (aligned16(dx) && aligned16(y)) ? n / 4 : 0;
-  relu_deriv_kernel<<<blocks_for(std::max(n4, n - 4 * n4), 256), 256, 0, state().stream>>>(dx, y, n, n4);
-  count_launch(); CNB_LAUNCH_CHECK("relu_deriv");
-  end_write(dx, n, emit, nullptr);
+  vec4_pass("relu_deriv", dx, y, n, false, [&](int grid, long long n4, __nv_bfloat16*) {
+    relu_deriv_kernel<<<grid, 256, 0, state().stream>>>(dx, y, n, n4);
+  });
 }
 void cnb_logistic(float* x, long long n) {
-  const bool emit = take_fuse().emit_bf16 != 0;
-  if (n <= 0) return;
-  const long long n4 = aligned16(x) ? n / 4 : 0;
-  __nv_bfloat16* o16 = begin_write(x, n, emit, true);
-  logistic_kernel<<<blocks_for(std::max(n4, n - 4 * n4), 256), 256, 0, state().stream>>>(x, n, n4, o16);
-  count_launch(); CNB_LAUNCH_CHECK("logistic");
-  end_write(x, n, emit, o16);
+  vec4_pass("logistic", x, nullptr, n, true, [&](int grid, long long n4, __nv_bfloat16* o16) {
+    logistic_kernel<<<grid, 256, 0, state().stream>>>(x, n, n4, o16);
+  });
 }
 void cnb_logistic_deriv(float* dx, const float* y, long long n) {
-  const bool emit = take_fuse().emit_bf16 != 0;
-  if (n <= 0) return;
-  const long long n4 = (aligned16(dx) && aligned16(y)) ? n / 4 : 0;
-  __nv_bfloat16* o16 = begin_write(dx, n, emit, true);
-  logistic_deriv_kernel<<<blocks_for(std::max(n4, n - 4 * n4), 256), 256, 0, state().stream>>>(dx, y, n, n4, o16);
-  count_launch(); CNB_LAUNCH_CHECK("logistic_deriv");
-  end_write(dx, n, emit, o16);
+  vec4_pass("logistic_deriv", dx, y, n, true, [&](int grid, long long n4, __nv_bfloat16* o16) {
+    logistic_deriv_kernel<<<grid, 256, 0, state().stream>>>(dx, y, n, n4, o16);
+  });
 }
 static bool is_loss(int f) { return f >= CNB_LOSS_SQUARED_ERROR && f <= CNB_LOSS_CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED; }
 void cnb_loss_deriv(int loss, const float* y, const float* targets, const int* labels, float* deriv, float* loss_per_image,
@@ -843,23 +840,15 @@ void cnb_metric(int metric, const float* y, const float* targets, const int* lab
   count_launch(); CNB_LAUNCH_CHECK("metric");
 }
 void cnb_dropout(float* x, float* mask, long long n, float dropprob, float scale, unsigned long long seed) {
-  const bool emit = take_fuse().emit_bf16 != 0;
-  if (n <= 0) return;
-  const long long n4 = (aligned16(x) && aligned16(mask)) ? n / 4 : 0;
-  __nv_bfloat16* o16 = begin_write(x, n, emit, true);
-  bf16_note_write(mask, n);
-  dropout_kernel<<<blocks_for(std::max(n4, n - 4 * n4), 256), 256, 0, state().stream>>>(x, mask, n, n4, dropprob, scale, seed, o16);
-  count_launch(); CNB_LAUNCH_CHECK("dropout");
-  end_write(x, n, emit, o16);
+  vec4_pass("dropout", x, mask, n, true, [&](int grid, long long n4, __nv_bfloat16* o16) {
+    bf16_note_write(mask, n);
+    dropout_kernel<<<grid, 256, 0, state().stream>>>(x, mask, n, n4, dropprob, scale, seed, o16);
+  });
 }
 void cnb_mult(float* a, const float* b, long long n) {
-  const bool emit = take_fuse().emit_bf16 != 0;
-  if (n <= 0) return;
-  const long long n4 = (aligned16(a) && aligned16(b)) ? n / 4 : 0;
-  __nv_bfloat16* o16 = begin_write(a, n, emit, true);
-  mult_kernel<<<blocks_for(std::max(n4, n - 4 * n4), 256), 256, 0, state().stream>>>(a, b, n, n4, o16);
-  count_launch(); CNB_LAUNCH_CHECK("mult");
-  end_write(a, n, emit, o16);
+  vec4_pass("mult", a, b, n, true, [&](int grid, long long n4, __nv_bfloat16* o16) {
+    mult_kernel<<<grid, 256, 0, state().stream>>>(a, b, n, n4, o16);
+  });
 }
 void cnb_softmax(float* x, int rows, int cols) {
   if (rows <= 0) return;
@@ -987,24 +976,23 @@ void cnb_bn_stats(const float* x, long long n, int channels, float eps, float bn
 }
 void cnb_bn_apply(const float* x, float* y, long long n, int channels, const float* gamma, const float* beta, const float* mu,
                   const float* sigma, int relu) {
-  const bool emit = take_fuse().emit_bf16 != 0;
+  const bool want = take_fuse().emit_bf16 != 0;
   if (n <= 0 || channels <= 0) return;
   CNB_REQUIRE(channels <= 65535, "cnb_bn_apply");
-  const long long total = n * channels;
   const bool vec = bn_vec(n, x, y);
-  __nv_bfloat16* o16 = begin_write(y, total, emit, true);
+  Emit emit(y, n * channels, want);
   const dim3 grid = bn_grid(n, channels, vec);
-  if (relu) bn_apply_kernel<true><<<grid, 256, 0, state().stream>>>(x, y, n, vec, gamma, beta, mu, sigma, o16);
-  else bn_apply_kernel<false><<<grid, 256, 0, state().stream>>>(x, y, n, vec, gamma, beta, mu, sigma, o16);
+  if (relu) bn_apply_kernel<true><<<grid, 256, 0, state().stream>>>(x, y, n, vec, gamma, beta, mu, sigma, emit.buf);
+  else bn_apply_kernel<false><<<grid, 256, 0, state().stream>>>(x, y, n, vec, gamma, beta, mu, sigma, emit.buf);
   count_launch(); CNB_LAUNCH_CHECK("bn_apply");
-  end_write(y, total, emit, o16);
+  emit.done = true;
+  emit.finish();
 }
 void cnb_bn_backward(float* deriv, const float* x, long long n, int channels, const float* gamma, const float* mu,
                      const float* sigma, int train, float* grad_gamma, float* grad_beta) {
-  const bool emit = take_fuse().emit_bf16 != 0;
+  const bool want = take_fuse().emit_bf16 != 0;
   if (n <= 0 || channels <= 0) return;
   CNB_REQUIRE(channels <= 65535, "cnb_bn_backward");
-  const long long total = n * channels;
   const bool vec = bn_vec(n, x, deriv);
   bf16_note_write(grad_gamma, channels);
   bf16_note_write(grad_beta, channels);
@@ -1014,11 +1002,12 @@ void cnb_bn_backward(float* deriv, const float* x, long long n, int channels, co
   bn_grad_final_kernel<<<ceil_div(channels, 128), 128, 0, state().stream>>>(part, grad_gamma, grad_beta, channels, slices,
                                                                              1.f / (float)n);
   count_launch(); CNB_LAUNCH_CHECK("bn_grad");
-  __nv_bfloat16* o16 = begin_write(deriv, total, emit, true);
+  Emit emit(deriv, n * channels, want);
   bn_backward_kernel<<<bn_grid(n, channels, vec), 256, 0, state().stream>>>(deriv, x, n, vec, gamma, mu, sigma, grad_gamma,
-                                                                            grad_beta, train, o16);
+                                                                            grad_beta, train, emit.buf);
   count_launch(); CNB_LAUNCH_CHECK("bn_backward");
-  end_write(deriv, total, emit, o16);
+  emit.done = true;
+  emit.finish();
 }
 
 }  // extern "C"

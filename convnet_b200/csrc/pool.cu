@@ -587,8 +587,6 @@ __global__ void __launch_bounds__(256) pool_undo_patch_kernel(PoolGeom g, const 
 
 static int pow2_shift(unsigned v) { int s = 0; while ((1u << s) < v) s++; return (1u << s) == v ? s : -1; }
 
-static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 static unsigned long long pool_sig(const PoolGeom& g) {
   unsigned long long sig = 1469598103934665603ULL;
   for (int v : {g.N, g.W, g.H, g.C, g.modX, g.modY, g.kx, g.ky, g.sx, g.sy, g.px, g.py}) sig = (sig ^ (unsigned)v) * 1099511628211ULL;

@@ -415,8 +415,6 @@ static int pick_segments(long long L, int F, int k) {
   return segs;
 }
 
-static inline bool rn_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 template <int VEC>
 static void launch_fwd(const float* images, float* targets, long long L, int F, int k, float alpha, float beta, bool blocked) {
   const long long owners = L / VEC;                      // threads needed
@@ -466,7 +464,7 @@ void rnorm_forward(const float* images, float* targets, long long L, int F, int 
   size_t tsmem = 0;
   const int tl = L < (1LL << 31) * 32 ? pick_tile(F, 2, &tsmem) : 0;
   if (tl) {
-    const bool vec = L % 4 == 0 && rn_aligned16(images) && rn_aligned16(targets) &&
+    const bool vec = L % 4 == 0 && aligned16(images) && aligned16(targets) &&
                      (!targets_bf16 || (reinterpret_cast<uintptr_t>(targets_bf16) & 7) == 0);
     if (tl == 64) launch_fwd_tile<64>(images, targets, targets_bf16, L, F, k, alpha, beta, blocked, relu, tsmem, vec);
     else launch_fwd_tile<32>(images, targets, targets_bf16, L, F, k, alpha, beta, blocked, relu, tsmem, vec);
@@ -478,7 +476,7 @@ void rnorm_forward(const float* images, float* targets, long long L, int F, int 
   // four locations per thread only when that still leaves >= 4 blocks per SM: the channel walk is a serial dependency
   // chain, so small problems need the thread count more than the shorter instruction stream (measured: 105 -> 75 us on
   // 96 x 55 x 55 x 128, but 39 -> 47 us on 256 x 14 x 14 x 128)
-  const bool wide = L % 4 == 0 && rn_aligned16(images) && rn_aligned16(targets) && L / 4 / RN_THREADS >= 4LL * num_sms();
+  const bool wide = L % 4 == 0 && aligned16(images) && aligned16(targets) && L / 4 / RN_THREADS >= 4LL * num_sms();
   if (wide) launch_fwd<4>(images, targets, L, F, k, alpha, beta, blocked);
   else launch_fwd<1>(images, targets, L, F, k, alpha, beta, blocked);
   count_launch();
@@ -511,7 +509,7 @@ void rnorm_undo(const float* outGrads, const float* inputs, float* targets, long
   size_t tsmem = 0;
   const int tl = pick_tile(F, 4, &tsmem);
   if (tl) {
-    const bool vec = L % 4 == 0 && rn_aligned16(outGrads) && rn_aligned16(inputs) && rn_aligned16(targets);
+    const bool vec = L % 4 == 0 && aligned16(outGrads) && aligned16(inputs) && aligned16(targets);
     if (tl == 64) launch_undo_tile<64>(outGrads, inputs, targets, L, F, k, alpha, beta, blocked, tsmem, vec);
     else launch_undo_tile<32>(outGrads, inputs, targets, L, F, k, alpha, beta, blocked, tsmem, vec);
     count_launch();

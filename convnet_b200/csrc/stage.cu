@@ -28,8 +28,6 @@ struct Staged {
 std::vector<Staged>& table() { static std::vector<Staged> t; return t; }
 unsigned long long g_tick = 0;
 constexpr size_t kMaxStaged = 128;
-inline size_t align_up(size_t v) { return (v + 1023) & ~size_t(1023); }
-inline bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
 
 __global__ void __launch_bounds__(256) cvt_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long n) {
   const long long n8 = n >> 3;
@@ -284,13 +282,11 @@ const uint16_t* pool_masks_find(const float* acts, long long n_out, const float*
   return reinterpret_cast<const uint16_t*>(e->buf);
 }
 
-__nv_bfloat16* begin_write(float* target, long long n, bool want_emit, bool kernel_can_emit) {
+Emit::Emit(float* target_, long long n_, bool want_, bool kernel_can_emit) : target(target_), n(n_), want(want_) {
   bf16_note_write(target, n);
-  if (want_emit && kernel_can_emit) return bf16_emit_slot(target, n);
-  return nullptr;
+  if (want && kernel_can_emit) buf = bf16_emit_slot(target, n);    // marked valid: the kernel that follows fills it
 }
-void end_write(float* target, long long n, bool want_emit, const __nv_bfloat16* emitted) {
-  if (want_emit && !emitted) bf16_stage(target, n);
-}
+// bf16_stage converts only where bf16_emit_slot would have handed out a buffer, so an unfilled `want` needs no other test
+void Emit::finish() { if (want && !done) bf16_stage(target, n); }
 
 }  // namespace cnb

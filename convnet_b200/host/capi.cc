@@ -1,4 +1,5 @@
 // capi.cc — plain C doors onto the host C++ (ConvNet / GradChecker / DataParallelSync) for ctypes.
+#include <algorithm>
 #include <cstdio>
 #include <cstring>
 #include <stdexcept>
@@ -273,6 +274,37 @@ API int cnb_model_edge_optimizer(const char* model, int edge, int which, Optimiz
   if (e.edge_type == MAXPOOL || e.edge_type == AVGPOOL || e.edge_type == RESPONSE_NORM || (which == 1 && e.has_no_bias)) return -2;
   *out = which ? e.bias_optimizer : e.weight_optimizer;
   return 0;
+}
+
+// a model's resolved ModelConfig as a config::Model text proto (ModelText).  Returns its length in bytes (-1: unknown
+// model or unreadable file, the reason on stderr) and writes up to cap - 1 of them and a terminating NUL into buf
+API long long cnb_model_text(const char* model, char* buf, long long cap) {
+  ModelConfig m;
+  if (!TryBuildModel(model, &m)) return -1;
+  const std::string t = ModelText(m);
+  if (cap > 0) {
+    const size_t n = std::min((size_t)(cap - 1), t.size());
+    memcpy(buf, t.data(), n);
+    buf[n] = 0;
+  }
+  return (long long)t.size();
+}
+
+// static description of a model: the initial weights of edge `edge` under RNG seed `seed` (EdgeWithWeight::InitialWeights;
+// the net seeds edge i with its seed + 17 i).  Returns their number (writes up to `cap`); -1 unknown model, -2 edge out of
+// range or without parameters
+API long long cnb_model_initial_weights(const char* model, int edge, unsigned seed, float* out, long long cap) {
+  ConvNet* net = TryBuildNet(model, 1);
+  if (!net) return -1;
+  EdgeWithWeight* e = edge >= 0 && edge < (int)net->Edges().size() ? dynamic_cast<EdgeWithWeight*>(net->Edges()[edge].get()) : nullptr;
+  long long n = -2;
+  if (e) {
+    const std::vector<float> w = e->InitialWeights(seed);
+    n = (long long)w.size();
+    if (cap > 0) memcpy(out, w.data(), sizeof(float) * (size_t)std::min(n, cap));
+  }
+  delete net;
+  return n;
 }
 
 // ---- the device side of the input pipeline (data.h): a GPU-resident chunk + per-minibatch crop / mirror into the net's input

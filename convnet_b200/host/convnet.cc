@@ -63,6 +63,21 @@ void Layer::AllocateMemory(int batch_size) {               // layer.cc:228-262 (
   }
 }
 
+std::string EdgeShapeError(const Edge& e, int source_channels, int dest_channels) {
+  const int my = e.GetNumModulesY(), mx = e.GetNumModulesX(), mt = e.GetNumModulesT();
+  if (my < 1 || mx < 1 || mt < 1)
+    return "its kernel, stride and padding leave no output (" + std::to_string(my) + " x " + std::to_string(mx) + " x " +
+           std::to_string(mt) + " modules in y, x, t)";
+  const EdgeType t = e.Config().edge_type;
+  if ((t == MAXPOOL || t == AVGPOOL || t == RESPONSE_NORM) && source_channels != dest_channels)
+    return "pooling and response normalisation keep the channel count, but the source layer has " +
+           std::to_string(source_channels) + " channels and the destination " + std::to_string(dest_channels);
+  if ((t == CONVOLUTIONAL || t == LOCAL) && e.Config().padding_t != 0)
+    return "padding_t " + std::to_string(e.Config().padding_t) + " is not supported on a convolution (the 3-D kernels "
+           "fold the frames into channels)";
+  return "";
+}
+
 std::string LayerConfigError(const LayerConfig& c) {
   const bool softmax = c.activation == SOFTMAX || c.activation == SOFTMAX_DIST;
   if (!c.is_output) {
@@ -329,9 +344,16 @@ std::string ConvNet::Refusal() const {
     const std::string why = LayerConfigError(lc);
     if (!why.empty()) return "layer '" + lc.name + "': " + why;
   }
-  for (size_t i = 0; i < edges_.size(); i++)         // the untied conv kernels are 2-D only
-    if (model_.edge[i].edge_type == LOCAL && layers_[i]->GetSizeT() != 1)
+  for (size_t i = 0; i < edges_.size(); i++) {
+    const std::string shape = EdgeShapeError(*edges_[i], layers_[i]->GetNumChannels(), layers_[i + 1]->GetNumChannels());
+    if (!shape.empty()) return "edge '" + edges_[i]->GetName() + "': " + shape;
+    if (model_.edge[i].edge_type == LOCAL && layers_[i]->GetSizeT() != 1)     // the untied conv kernels are 2-D only
       return "edge '" + edges_[i]->GetName() + "': LOCAL is not supported on 3-D layers (image_size_t > 1)";
+    const int init = model_.edge[i].initialization;
+    if (!edges_[i]->HasNoParameters() && init != DENSE_GAUSSIAN && init != DENSE_GAUSSIAN_SQRT_FAN_IN &&
+        init != DENSE_UNIFORM && init != DENSE_UNIFORM_SQRT_FAN_IN && init != CONSTANT)
+      return "edge '" + edges_[i]->GetName() + "': initialization " + std::to_string(init) + " is not implemented";
+  }
   for (const auto& l : layers_) {                    // what the batch-norm passes cannot run
     if (!l->BatchNormalize()) continue;
     std::string why;

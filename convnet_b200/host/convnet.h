@@ -5,8 +5,8 @@
 // Accumulate + Broadcast (src/convnet.cc:407-438) with in-place NCCL all-reduce over NVLink.
 //
 // Layers form a chain (every BASELINE net is one: Appendix B of SURVEY.md).  The model comes
-// from a ModelConfig struct (protobuf / pbtxt parsing is out of scope, SURVEY.md §2.1);
-// builders for the BASELINE configs live in models.cc.
+// from a ModelConfig struct: built by name in models.cc, or read from the reference's config::Model
+// text proto (a net.pbtxt file) in model_file.cc.
 #pragma once
 #include <memory>
 #include <string>
@@ -52,6 +52,10 @@ struct LayerConfig {
 const char* BnOptimizerConfigError(const OptimizerConfig& c);
 // "" if the activation, loss function and performance metric of `c` can run, else why not
 std::string LayerConfigError(const LayerConfig& c);
+// "" if edge `e`, once SetImageSize has run, can run between layers of `source_channels` and `dest_channels`: it gives
+// its destination at least one module in y, x and t, a pooling or response-norm edge keeps the channel count, and a
+// convolution has no temporal padding (the 3-D kernels fold the frames into channels); else why not
+std::string EdgeShapeError(const Edge& e, int source_channels, int dest_channels);
 
 struct ModelConfig {
   std::string name;
@@ -275,6 +279,16 @@ ModelConfig BuildLeNet();       // examples/mnist-conv/net.pbtxt
 ModelConfig BuildC3D();         // SURVEY.md §8(d) cfg4
 ModelConfig BuildTinyNet();     // small conv+pool+rnorm+1x1+fc net for tests / grad check
 ModelConfig BuildLogCheckNet(); // the gradcheck net with logistic hidden units
+// a built-in name, a path ending in ".pbtxt" (ReadModelFile), either with suffixes ("+bn", "+rmsprop", ...).
+// std::invalid_argument: unknown name, unreadable or refused file
 ModelConfig BuildModel(const std::string& name);
+
+// model_file.cc: the reference's config::Model text proto (src/util.cc ReadPbtxt, proto/convnet_config.proto).
+// ReadModelFile applies the proto's defaults and presence rules, the default optimizers (src/convnet.cc:41-62) and the
+// chain order of the graph; std::invalid_argument names the file, the line and the field of what it cannot read or run.
+ModelConfig ReadModelFile(const std::string& path);
+// `m` as a config::Model text proto that ReadModelFile reads back to the same model: every field the host reads for a
+// layer or edge of that kind explicit, floats printed so that they read back bit-exactly
+std::string ModelText(const ModelConfig& m);
 
 }  // namespace cnbhost

@@ -286,6 +286,7 @@ static bool EndsWith(const std::string& s, const std::string& suffix) {
 }
 
 ModelConfig BuildModel(const std::string& name) {
+  if (EndsWith(name, ".pbtxt")) return ReadModelFile(name);          // no suffix ends in ".pbtxt"
   for (const OutputSuffix& o : kOutputSuffixes) {
     if (!EndsWith(name, o.suffix)) continue;
     ModelConfig m = BuildModel(name.substr(0, name.size() - std::string(o.suffix).size()));

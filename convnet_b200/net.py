@@ -91,6 +91,8 @@ def load_host():
             "cnb_net_targets": ([vp], vp), "cnb_net_targets_floats": ([vp], ll), "cnb_net_metric": ([vp], f),
             "cnb_model_output_layer": ([ct.c_char_p, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(f),
                                         ct.POINTER(i)], i),
+            "cnb_model_text": ([ct.c_char_p, ct.c_char_p, ll], ll),
+            "cnb_model_initial_weights": ([ct.c_char_p, i, ct.c_uint, ct.POINTER(f), ll], ll),
         }
         for name, (args, res) in sig.items():
             fn = getattr(H, name)
@@ -100,7 +102,11 @@ def load_host():
 
 
 class Net:
-    """A chain ConvNet built natively ("alexnet" | "lenet" | "c3d" | "tiny" | "gradcheck").  Suffixes:
+    """A chain ConvNet built natively, from a built-in name ("alexnet" | "lenet" | "c3d" | "tiny" | "lcnet" | "gradcheck" |
+    "logcheck" | "localcheck") or from a model file: any name ending in ".pbtxt" is the path of a config::Model text proto
+    as the reference writes them (examples/*/net.pbtxt), read with the proto's defaults (model_text() prints any model
+    as one).  The file's seed is printed but not used: `seed` decides, for files as for built-ins.  Suffixes compose with
+    both ("net.pbtxt+rmsprop"):
     "+ref-optimizer" (alexnet and lenet): train with the optimizer blocks of the reference's pbtxt files.
     "+bn": batch normalisation on every hidden layer written by a conv, 1x1 or FC edge; gamma / beta train with that
     edge's weight / bias optimizer, without L2 decay and norm rules ("tiny+bn", "lenet+bn", "alexnet+bn", "gradcheck+bn",
@@ -112,7 +118,8 @@ class Net:
     "+logistic": every hidden RECTIFIED_LINEAR layer becomes LOGISTIC (same parameters; "alexnet+logistic", "tiny+bn+logistic").
     One output suffix at most: "+squared-error" (LINEAR output, SQUARED_ERROR), "+binary-ce" (LOGISTIC output,
     CROSS_ENTROPY_BINARY, metric CLASSIFICATION_BINARY), "+soft-targets" (SOFTMAX_DIST, CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED);
-    such outputs train on targets_tensor() instead of labels_tensor().  "logcheck": the gradcheck net with logistic units."""
+    such outputs train on targets_tensor() instead of labels_tensor().  "logcheck": the gradcheck net with logistic units.
+    A model that cannot be read or run raises ValueError; the reason (for a file: its line and field) is on stderr."""
 
     def __init__(self, model, batch_size, seed=42, grad_checker=False):
         self.H = load_host()
@@ -370,6 +377,35 @@ def model_output_layer(model):
         raise ValueError("unknown model %r (see stderr)" % model)
     return {"activation": ACTIVATIONS[a.value], "loss_function": LOSS_FUNCTIONS[lf.value],
             "performance_metric": LOSS_FUNCTIONS[pm.value], "loss_function_weight": w.value, "labels": bool(lab.value)}
+
+
+def model_text(model):
+    """the resolved configuration of a model (built-in, suffixed or file) as a config::Model text proto: every field the
+    host reads for each layer and edge explicit, floats printed so that they read back bit-exactly.  Written to a file
+    ending in ".pbtxt", it builds the same model."""
+    H, cap = load_host(), 1 << 16
+    while True:
+        buf = ct.create_string_buffer(cap)
+        n = H.cnb_model_text(model.encode(), buf, cap)
+        if n < 0:
+            raise ValueError("cannot read model %r (see stderr)" % model)
+        if n < cap:
+            return buf.value.decode()
+        cap = n + 1
+
+
+def model_initial_weights(model, edge, seed=42):
+    """the initial weights (a list of floats, without the bias) of edge `edge` of a model under RNG seed `seed`
+    (host-only; the net seeds edge i with its seed + 17 i); None for an edge without parameters"""
+    H = load_host()
+    n = H.cnb_model_initial_weights(model.encode(), edge, seed, None, 0)
+    if n == -1:
+        raise ValueError("cannot build model %r (see stderr)" % model)
+    if n < 0:
+        return None
+    buf = (ct.c_float * n)()
+    H.cnb_model_initial_weights(model.encode(), edge, seed, buf, n)
+    return list(buf)
 
 
 def model_param_layout(model, batch=1):

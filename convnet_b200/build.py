@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libconvnet_b200.so")
-SOURCES = ["abi.cu", "ext.cu", "stage.cu", "conv_simt.cu", "conv_tc.cu", "pool.cu", "rnorm.cu", "elementwise.cu"]
+SOURCES = ["abi.cu", "ext.cu", "stage.cu", "conv_simt.cu", "conv_tc.cu", "pool.cu", "rnorm.cu", "mapnorm.cu", "elementwise.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",

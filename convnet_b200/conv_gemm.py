@@ -45,6 +45,12 @@ class Binding:
         self._get().convOutp(images.p_mat, hidSums.p_mat, targets.p_mat, images.p_shape4d, hidSums.p_shape4d,
                              targets.p_shape4d, conv_desc, partialSumY, partialSumX, scaleTargets, scaleGradients)
 
+    def convInnerp(self, images, hidSums, targets, conv_desc, scaleTargets=0, scaleGradients=1):
+        """ABI-1 only (cudamat_conv_gemm.py convInnerp): targets, shape (1, kx, ky, 1), gets per filter tap the sum over
+        images, modules and channels of the image patch value times the derivative of the same channel"""
+        self._get().convInnerpGemm(images.p_mat, hidSums.p_mat, targets.p_mat, images.p_shape4d, hidSums.p_shape4d,
+                                   targets.p_shape4d, conv_desc, scaleTargets, scaleGradients)
+
     def localUp(self, images, filters, targets, conv_desc, scaleTargets=0):
         self._f("localUp")(images.p_mat, filters.p_mat, targets.p_mat, images.p_shape4d, filters.p_shape4d,
                            targets.p_shape4d, conv_desc, scaleTargets)
@@ -61,6 +67,11 @@ class Binding:
     def MaxPool(self, images, targets, conv_desc):
         extra = (0.0, 1.0) if self.abi == "gemm" else ()
         self._f("MaxPool")(images.p_mat, targets.p_mat, images.p_shape4d, targets.p_shape4d, conv_desc, *extra)
+
+    def MaxPoolRprop(self, images, R_images, maxes, targets, conv_desc, scaleTargets=0):
+        """ABI-1 only (cudamat_conv_gemm.py MaxPoolRprop): the R-operator of max pooling"""
+        self._get().MaxPoolRpropGemm(images.p_mat, R_images.p_mat, maxes.p_mat, targets.p_mat, images.p_shape4d,
+                                     maxes.p_shape4d, conv_desc, scaleTargets)
 
     def AvgPool(self, images, targets, conv_desc):
         extra = (0.0, 1.0) if self.abi == "gemm" else ()
@@ -94,6 +105,32 @@ class Binding:
         else:
             self._f("ResponseNormCrossMapUndo")(derivs.p_mat, images.p_mat, targets.p_mat, num_filters, sizeF,
                                                 addScale, powScale, blocked)
+
+    def ResponseNormCrossMapRprop(self, images, R_images, targets, sizeF, addScale, powScale, blocked):
+        """ABI-1 only (cudamat_conv_gemm.py ResponseNormCrossMapRprop): the R-operator of cross-map normalisation"""
+        num_filters = images.shape4d[3]
+        self._get().ResponseNormCrossMapRpropGemm(images.p_mat, R_images.p_mat, targets.p_mat, num_filters, sizeF,
+                                                  addScale, powScale, blocked)
+
+    # ---- within-map normalisation and colour (ABI-2 only: cudamat_conv.cuh:44-78) -------------------------------------
+    def ResponseNorm(self, images, denoms, targets, numChannels, sizeX, addScale, powScale):
+        self._get().ResponseNorm(images.p_mat, denoms.p_mat, targets.p_mat, numChannels, sizeX, addScale, powScale)
+
+    def ResponseNormUndo(self, outGrad, denoms, inGrad, acts, targets, numChannels, sizeX, addScale, powScale):
+        self._get().ResponseNormUndo(outGrad.p_mat, denoms.p_mat, inGrad.p_mat, acts.p_mat, targets.p_mat, numChannels,
+                                     sizeX, addScale, powScale)
+
+    def ContrastNorm(self, images, meanDiffs, denoms, targets, numChannels, sizeX, addScale, powScale):
+        self._get().ContrastNorm(images.p_mat, meanDiffs.p_mat, denoms.p_mat, targets.p_mat, numChannels, sizeX,
+                                 addScale, powScale)
+
+    def ContrastNormUndo(self, outGrad, denoms, meanDiffs, acts, targets, numChannels, sizeX, addScale, powScale):
+        self._get().ContrastNormUndo(outGrad.p_mat, denoms.p_mat, meanDiffs.p_mat, acts.p_mat, targets.p_mat,
+                                     numChannels, sizeX, addScale, powScale)
+
+    def RGBToYUV(self, images, targets):
+        """images: (numImages, 3 * pixels), the R, G and B planes; targets: the Y, U and V planes, same shape"""
+        self._get().RGBToYUV(images.p_mat, targets.p_mat)
 
     # ---- 3-D (ABI-1 only: cudamat_conv3d_gemm.cu) -----------------------------------------------------
     def ResponseNormCrossMap3D(self, images, targets, sizeF, addScale, powScale, blocked, image_size_t):
@@ -142,3 +179,6 @@ ResponseNormCrossMap3D, ResponseNormCrossMap3DUndo = gemm.ResponseNormCrossMap3D
 convUp3D, convDown3D, convOutp3D = gemm.convUp3D, gemm.convDown3D, gemm.convOutp3D
 MaxPool3D, MaxPool3DUndo, AvgPool3D, AvgPool3DUndo = MaxPool, MaxPoolUndo, AvgPool, AvgPoolUndo
 convOutpPartial = gemm.convOutpPartial
+convInnerp, MaxPoolRprop, ResponseNormCrossMapRprop = gemm.convInnerp, gemm.MaxPoolRprop, gemm.ResponseNormCrossMapRprop
+ResponseNorm, ResponseNormUndo, ContrastNorm, ContrastNormUndo = cc2.ResponseNorm, cc2.ResponseNormUndo, cc2.ContrastNorm, cc2.ContrastNormUndo
+RGBToYUV = cc2.RGBToYUV

@@ -224,6 +224,101 @@ void do_rnorm_undo(const char* what, cudamat* outGrads, cudamat* inputs, cudamat
   emit.finish();
 }
 
+// ---- the R-operators, within-map normalisation, the colour transform and the tap inner products: kernels that cannot
+// write a bf16 twin, so a requested copy is converted after them (Emit::finish) and every other tensor they write has its
+// staged copies dropped (bf16_note_write)
+
+// both matrices hold `n` floats as (rows, cols) and are not transposed
+bool same_shape(const cudamat* a, const cudamat* b) {
+  return a->size[0] == b->size[0] && a->size[1] == b->size[1] && !a->is_trans && !b->is_trans;
+}
+
+void do_max_rprop(const char* what, cudamat* images, cudamat* R_images, cudamat* maxes, cudamat* targets, Shape4D* is,
+                  Shape4D* ms, ConvDesc d, float st) {
+  Range nvtx_range(what);
+  PoolGeom g = pool_geom(*is, *ms, images, maxes, as_2d(d), what);
+  CNB_REQUIRE(same_shape(R_images, images), what);
+  CNB_REQUIRE(same_shape(targets, maxes), what);
+  const Fuse fuse = take_fuse();
+  Emit emit(targets->data_device, (long long)targets->size[0] * targets->size[1], fuse.emit_bf16 != 0, false);
+  max_pool_rprop(g, images->data_device, R_images->data_device, maxes->data_device, targets->data_device, st);
+  emit.finish();
+}
+
+void do_rnorm_rprop(const char* what, cudamat* images, cudamat* R_images, cudamat* targets, int F, int sizeF, float a,
+                    float b, bool blocked) {
+  Range nvtx_range(what);
+  CNB_REQUIRE(F > 0 && sizeF >= 1, what);
+  const long long els = (long long)images->size[0] * images->size[1];
+  CNB_REQUIRE(els % F == 0, what);
+  CNB_REQUIRE(same_shape(R_images, images) && same_shape(targets, images), what);
+  const Fuse fuse = take_fuse();
+  Emit emit(targets->data_device, els, fuse.emit_bf16 != 0, false);
+  rnorm_rprop(images->data_device, R_images->data_device, targets->data_device, els / F, F, sizeF, a, b, blocked);
+  emit.finish();
+}
+
+// the (numFilters, S, S, numImages) geometry of the cudamat_conv.cuh norms: square maps (convContrastNorm's assert)
+int map_side(const char* what, const cudamat* m, int F) {
+  CNB_REQUIRE(F > 0 && m->size[1] % F == 0, what);
+  const int pixels = m->size[1] / F;
+  int S = 0;
+  while ((long long)(S + 1) * (S + 1) <= pixels) S++;
+  CNB_REQUIRE((long long)S * S == pixels, what);          // square images only
+  CNB_REQUIRE(!m->is_trans, what);
+  return S;
+}
+
+void do_mapnorm(const char* what, cudamat* images, cudamat* meanDiffs, cudamat* denoms, cudamat* targets, int F, int sizeX,
+                float a, float b) {
+  Range nvtx_range(what);
+  const int S = map_side(what, images, F);
+  CNB_REQUIRE(sizeX >= 1, what);
+  CNB_REQUIRE(same_shape(meanDiffs, images) && same_shape(denoms, images) && same_shape(targets, images), what);
+  const Fuse fuse = take_fuse();
+  const long long n = (long long)images->size[0] * images->size[1];
+  bf16_note_write(denoms->data_device, n);
+  Emit emit(targets->data_device, n, fuse.emit_bf16 != 0, false);
+  mapnorm_forward(images->data_device, meanDiffs->data_device, denoms->data_device, targets->data_device, images->size[0], S,
+                  F, sizeX, a, b);
+  emit.finish();
+}
+
+void do_mapnorm_undo(const char* what, cudamat* outGrads, cudamat* denoms, cudamat* inputs, cudamat* acts, cudamat* targets,
+                     int F, int sizeX, float a, float b) {
+  Range nvtx_range(what);
+  const int S = map_side(what, outGrads, F);
+  CNB_REQUIRE(sizeX >= 1, what);
+  CNB_REQUIRE(same_shape(denoms, outGrads) && same_shape(inputs, outGrads) && same_shape(acts, outGrads) &&
+              same_shape(targets, outGrads), what);
+  const Fuse fuse = take_fuse();
+  CNB_REQUIRE(!fuse.bias_grad, what);
+  Emit emit(targets->data_device, (long long)outGrads->size[0] * outGrads->size[1], fuse.emit_bf16 != 0, false);
+  mapnorm_undo(outGrads->data_device, denoms->data_device, inputs->data_device, acts->data_device, targets->data_device,
+               outGrads->size[0], S, F, sizeX, a, b);
+  emit.finish();
+}
+
+void do_innerp(const char* what, cudamat* images, cudamat* derivs, cudamat* targets, Shape4D* is, Shape4D* ds, Shape4D* ts,
+               ConvDesc d, float st, float so) {
+  Range nvtx_range(what);
+  d = as_2d(d);
+  // the target is one value per filter tap, shape [1][kx][ky][1] (gemm.cu:993-996)
+  CNB_REQUIRE(ts->shape[0] == 1 && ts->shape[3] == 1, what);
+  CNB_REQUIRE(ts->shape[1] == d.kernel_size_x && ts->shape[2] == d.kernel_size_y, what);
+  CNB_REQUIRE((long long)targets->size[0] * targets->size[1] == (long long)d.kernel_size_x * d.kernel_size_y, what);
+  CNB_REQUIRE(is->shape[3] == d.num_input_channels && ds->shape[3] == d.num_output_channels, what);   // 2-D only
+  Shape4D fs;                                   // the filter bank of the matching convolution, for the shared checks
+  fs.shape[0] = (d.output_channel_end == 0 ? d.num_output_channels : d.output_channel_end) - d.output_channel_begin;
+  fs.shape[1] = d.kernel_size_x; fs.shape[2] = d.kernel_size_y;
+  fs.shape[3] = (d.input_channel_end == 0 ? d.num_input_channels : d.input_channel_end) - d.input_channel_begin;
+  ConvGeom g = conv_geom(*is, fs, *ds, images, nullptr, derivs, d, true, what);
+  CNB_REQUIRE(g.Cin == g.Cout, what);           // each channel of the images meets the derivative of the same channel
+  take_fuse();
+  bf16_note_write(targets->data_device, (long long)g.kx * g.ky);
+  conv_innerp(g, images->data_device, derivs->data_device, targets->data_device, st, so);
+}
+
 }  // namespace
 
 extern "C" {
@@ -241,8 +336,9 @@ void convOutpGemm(cudamat* images, cudamat* derivs, cudamat* targets, Shape4D* i
                   ConvDesc d, float scaleTargets, float scaleOutput) {
   do_conv_outp("convOutpGemm", images, derivs, targets, is, ds, ts, as_2d(d), scaleTargets, scaleOutput, true);
 }
-void convInnerpGemm(cudamat*, cudamat*, cudamat*, Shape4D*, Shape4D*, Shape4D*, ConvDesc, float, float) {
-  not_implemented("convInnerpGemm", "no caller in the reference's C++ (SURVEY.md 2.3); out of scope");
+void convInnerpGemm(cudamat* images, cudamat* derivs, cudamat* targets, Shape4D* is, Shape4D* ds, Shape4D* ts,
+                    ConvDesc d, float scaleTargets, float scaleOutput) {
+  do_innerp("convInnerpGemm", images, derivs, targets, is, ds, ts, d, scaleTargets, scaleOutput);
 }
 void localUpGemm(cudamat* images, cudamat* filters, cudamat* targets, Shape4D* is, Shape4D* fs, Shape4D* ts,
                  ConvDesc d, float scaleTargets) {
@@ -269,8 +365,9 @@ void MaxPoolUndoGemm(cudamat* images, cudamat* maxGrads, cudamat* maxActs, cudam
                      Shape4D* gs, ConvDesc d, float scaleTargets) {
   do_max_undo("MaxPoolUndoGemm", images, maxGrads, maxActs, targets, is, gs, d, scaleTargets);
 }
-void MaxPoolRpropGemm(cudamat*, cudamat*, cudamat*, cudamat*, Shape4D*, Shape4D*, ConvDesc, float) {
-  not_implemented("MaxPoolRpropGemm", "R-operator has no caller in the reference's C++; out of scope");
+void MaxPoolRpropGemm(cudamat* images, cudamat* R_images, cudamat* maxActs, cudamat* targets, Shape4D* is,
+                      Shape4D* ms, ConvDesc d, float scaleTargets) {
+  do_max_rprop("MaxPoolRpropGemm", images, R_images, maxActs, targets, is, ms, d, scaleTargets);
 }
 void AvgPoolUndoGemm(cudamat* avgGrads, cudamat* targets, Shape4D* gs, Shape4D* ts, ConvDesc d, float scaleTargets) {
   do_avg_undo("AvgPoolUndoGemm", avgGrads, targets, gs, ts, d, scaleTargets, 1.f);
@@ -295,8 +392,9 @@ void ResponseNormCrossMapUndoGemm(cudamat* outGrads, cudamat* inputs, cudamat* t
   do_rnorm_undo("ResponseNormCrossMapUndoGemm", outGrads, inputs, targets, numFilters, sizeF, addScale, powScale,
                 blocked, 1);
 }
-void ResponseNormCrossMapRpropGemm(cudamat*, cudamat*, cudamat*, int, int, float, float, bool) {
-  not_implemented("ResponseNormCrossMapRpropGemm", "R-operator has no caller in the reference's C++; out of scope");
+void ResponseNormCrossMapRpropGemm(cudamat* images, cudamat* R_images, cudamat* targets, int numFilters, int sizeF,
+                                   float addScale, float powScale, bool blocked) {
+  do_rnorm_rprop("ResponseNormCrossMapRpropGemm", images, R_images, targets, numFilters, sizeF, addScale, powScale, blocked);
 }
 void Scale(cudamat* mat, float scale) {
   bf16_note_write(mat->data_device, (long long)mat->size[0] * mat->size[1]);
@@ -377,17 +475,24 @@ void ResponseNormCrossMapUndo(cudamat* outGrads, cudamat* inputs, cudamat* /*act
                               int sizeF, float addScale, float powScale, bool blocked) {
   do_rnorm_undo("ResponseNormCrossMapUndo", outGrads, inputs, targets, numFilters, sizeF, addScale, powScale, blocked, 1);
 }
-void ResponseNorm(cudamat*, cudamat*, cudamat*, int, int, float, float) {
-  not_implemented("ResponseNorm", "within-map response norm: no Edge type reaches it (src/edge.cc:17-60)");
+// within-map normalisation (cudamat_conv_others.cu:3669-3683): ResponseNorm is ContrastNorm with meanDiffs = images, and
+// both undos are one kernel with `inputs` = the images or the meanDiffs.  `acts` is read, not overwritten (the reference
+// leaves its scratch product in it).
+void ResponseNorm(cudamat* images, cudamat* denoms, cudamat* targets, int numFilters, int sizeX, float addScale,
+                  float powScale) {
+  do_mapnorm("ResponseNorm", images, images, denoms, targets, numFilters, sizeX, addScale, powScale);
 }
-void ResponseNormUndo(cudamat*, cudamat*, cudamat*, cudamat*, cudamat*, int, int, float, float) {
-  not_implemented("ResponseNormUndo", "within-map response norm: no Edge type reaches it (src/edge.cc:17-60)");
+void ResponseNormUndo(cudamat* outGrads, cudamat* denoms, cudamat* inputs, cudamat* acts, cudamat* targets, int numFilters,
+                      int sizeX, float addScale, float powScale) {
+  do_mapnorm_undo("ResponseNormUndo", outGrads, denoms, inputs, acts, targets, numFilters, sizeX, addScale, powScale);
 }
-void ContrastNorm(cudamat*, cudamat*, cudamat*, cudamat*, int, int, float, float) {
-  not_implemented("ContrastNorm", "contrast norm: no Edge type reaches it (src/edge.cc:17-60)");
+void ContrastNorm(cudamat* images, cudamat* meanDiffs, cudamat* denoms, cudamat* targets, int numFilters, int sizeX,
+                  float addScale, float powScale) {
+  do_mapnorm("ContrastNorm", images, meanDiffs, denoms, targets, numFilters, sizeX, addScale, powScale);
 }
-void ContrastNormUndo(cudamat*, cudamat*, cudamat*, cudamat*, cudamat*, int, int, float, float) {
-  not_implemented("ContrastNormUndo", "contrast norm: no Edge type reaches it (src/edge.cc:17-60)");
+void ContrastNormUndo(cudamat* outGrads, cudamat* denoms, cudamat* meanDiffs, cudamat* acts, cudamat* targets,
+                      int numFilters, int sizeX, float addScale, float powScale) {
+  do_mapnorm_undo("ContrastNormUndo", outGrads, denoms, meanDiffs, acts, targets, numFilters, sizeX, addScale, powScale);
 }
 
 void MaxPool(cudamat* images, cudamat* targets, Shape4D* is, Shape4D* ts, ConvDesc d) {
@@ -409,8 +514,16 @@ void UpSample(cudamat* images, cudamat* targets, Shape4D* is, Shape4D* ts, int f
 void DownSample(cudamat* images, cudamat* targets, Shape4D* is, Shape4D* ts, int factor) {
   DownSampleGemm(images, targets, is, ts, factor);
 }
-void RGBToYUV(cudamat*, cudamat*) {
-  not_implemented("RGBToYUV", "colour-space edge is a 3x3 dot in the reference (rgb_to_yuv_edge.cc); out of scope");
+// images (3, pixels, numImages) -> targets of the same shape (convRGBToYUV, cudamat_conv_others.cu:2715-2755)
+void RGBToYUV(cudamat* images, cudamat* targets) {
+  Range nvtx_range("RGBToYUV");
+  CNB_REQUIRE(images->size[1] % 3 == 0, "RGBToYUV: three colour planes");
+  CNB_REQUIRE(same_shape(images, targets), "RGBToYUV");
+  const Fuse fuse = take_fuse();
+  const long long n = (long long)images->size[0] * images->size[1];
+  Emit emit(targets->data_device, n, fuse.emit_bf16 != 0, false);
+  rgb_to_yuv(images->data_device, targets->data_device, n / 3);
+  emit.finish();
 }
 
 }  // extern "C"

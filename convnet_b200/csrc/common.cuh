@@ -41,11 +41,6 @@ namespace cnb {
     }                                                                                     \
   } while (0)
 
-[[noreturn]] inline void not_implemented(const char* sym, const char* why) {
-  fprintf(stderr, "convnet_b200: %s is not implemented: %s\n", sym, why);
-  abort();
-}
-
 // programmatic dependent launch: this CTA does not mind the NEXT kernel of the stream being placed on the machine already
 // (only kernels launched with the PDL attribute use it, and those wait for this grid's completion before their first
 // global access — conv_tc.cu: launch); a no-op for every other successor

@@ -82,6 +82,8 @@ bool max_pool_undo(const PoolGeom& g, const float* images, const float* maxGrads
 bool avg_pool_undo(const PoolGeom& g, const float* avgGrads, float* targets, float scaleTargets,
                    float scaleOutput, const float* relu_mask, __nv_bfloat16* targets_bf16 = nullptr,
                    float* colsum = nullptr, int* colsum_slices = nullptr);
+// max-pool R-operator: targets = st * targets + sum of R_images over the window elements equal to the stored maximum
+void max_pool_rprop(const PoolGeom& g, const float* images, const float* R_images, const float* maxes, float* targets, float st);
 // grad_bias[c] = st*grad_bias[c] + so * sum_slices part[slice*cols + c]   (elementwise.cu)
 void colsum_finish(const float* part, float* grad_bias, int cols, int slices, float st, float so);
 
@@ -92,5 +94,19 @@ void rnorm_forward(const float* images, float* targets, long long num_locs, int 
 bool rnorm_can_fuse(int numFilters);
 void rnorm_undo(const float* outGrads, const float* inputs, float* targets, long long num_locs,
                 int numFilters, int sizeF, float addScale, float powScale, bool blocked);
+// R-operator: t_j = R_j d_j^-b - 2ab x_j d_j^(-b-1) sum_{i in window(j)} x_i R_i,  d_j = 1 + a sum_{i in window(j)} x_i^2
+void rnorm_rprop(const float* images, const float* R_images, float* targets, long long num_locs, int numFilters, int sizeF,
+                 float addScale, float powScale, bool blocked);
+
+// mapnorm.cu — within-map normalisation over sizeX x sizeX windows of square S x S maps, and the colour transform
+void mapnorm_forward(const float* images, const float* meanDiffs, float* denoms, float* targets, int N, int S, int F,
+                     int sizeX, float addScale, float powScale);
+void mapnorm_undo(const float* outGrads, const float* denoms, const float* inputs, const float* acts, float* targets, int N,
+                  int S, int F, int sizeX, float addScale, float powScale);
+void rgb_to_yuv(const float* images, float* targets, long long plane);   // plane = pixels x images per colour
+
+// conv_simt.cu — filter-tap inner products of convInnerpGemm: targets[tap] = st * targets[tap] + so * sum over images,
+// modules and channels c of image(tap at the module, c) * derivs(module, c); `splits` partial sums (0: chosen here)
+int conv_innerp(const ConvGeom& g, const float* images, const float* derivs, float* targets, float st, float so, int splits = 0);
 
 }  // namespace cnb

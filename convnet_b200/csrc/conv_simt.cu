@@ -405,4 +405,104 @@ void simt_conv_outp(const ConvGeom& g, const float* images, const float* derivs,
   reduce_partials(p.part, targets, elems, 1, Z, scaleTargets, scaleOutput);
 }
 
+// ---- convInnerpGemm: per filter tap, the inner product of the image patches with the derivative of the same channel ------
+// targets[tx + kx*ty] = st * targets[.] + so * sum over images n, modules m and channels c of
+//                       image(n, X(m) + tx, Y(m) + ty, c) * derivs(n, m, c)          (zero outside the image)
+// which is what the reference computes by expanding the patches (kExpand), multiplying by the derivative
+// (kOutpTraceMultiplyImages) and summing with two cuBLAS gemv passes (gemm.cu:963-1115).  Here no patch matrix exists: CTA
+// `split` owns a contiguous range of (channel, module) pairs with all their images, every thread keeps the sums of up to
+// INNERP_TAPS taps in registers (the derivative is read once per pass over the taps), and a fixed-shape block reduction
+// leaves one partial sum per tap: the target itself when there is one CTA, else a partial-sum row that reduce_partials
+// adds in split order.  Deterministic, no atomics.
+constexpr int INNERP_TAPS = 16;
+constexpr int INNERP_THREADS = 256;
+
+struct InnerpArgs {
+  const float* img; const float* der; float* out;   // out: the target (splits == 1) or the partial sums [split][taps]
+  int N, W, H, modX, modules, kx, ky, sx, sy, px, py, taps;
+  long long pairs, per_split;                        // (channel, module) pairs, pairs per CTA
+  float st, so;
+};
+
+template <int VEC> __device__ __forceinline__ void ip_load(const float* p, float (&v)[VEC]);
+template <> __device__ __forceinline__ void ip_load<4>(const float* p, float (&v)[4]) {
+  const float4 t = __ldg(reinterpret_cast<const float4*>(p)); v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+}
+template <> __device__ __forceinline__ void ip_load<1>(const float* p, float (&v)[1]) { v[0] = __ldg(p); }
+
+template <int VEC>
+__global__ void __launch_bounds__(INNERP_THREADS) innerp_kernel(InnerpArgs a, int final_pass) {
+  __shared__ float red[INNERP_THREADS / 32][INNERP_TAPS];
+  const int NV = a.N / VEC;
+  const long long p0 = (long long)blockIdx.x * a.per_split, p1 = min(a.pairs, p0 + a.per_split);
+  const long long units = (p1 - p0) * NV;
+  for (int t0 = 0; t0 < a.taps; t0 += INNERP_TAPS) {
+    float acc[INNERP_TAPS];
+#pragma unroll
+    for (int t = 0; t < INNERP_TAPS; t++) acc[t] = 0.f;
+    for (int u = threadIdx.x; u < (int)units; u += INNERP_THREADS) {
+      const long long pair = p0 + u / NV;
+      const int nv = u % NV;
+      const int c = (int)(pair / a.modules), m = (int)(pair % a.modules);
+      const int X0 = (m % a.modX) * a.sx + a.px, Y0 = (m / a.modX) * a.sy + a.py;
+      float d[VEC];
+      ip_load<VEC>(a.der + (long long)a.N * pair + nv * VEC, d);     // derivs(n, m, c) at n + N*(m + modules*c)
+      const float* img = a.img + (long long)a.N * a.W * a.H * c + nv * VEC;
+#pragma unroll
+      for (int t = 0; t < INNERP_TAPS; t++) {
+        const int tap = t0 + t;
+        if (tap >= a.taps) break;
+        const int ty = tap / a.kx, tx = tap - ty * a.kx;
+        const int X = X0 + tx, Y = Y0 + ty;
+        if ((unsigned)X >= (unsigned)a.W || (unsigned)Y >= (unsigned)a.H) continue;
+        float v[VEC];
+        ip_load<VEC>(img + (long long)a.N * (X + (long long)a.W * Y), v);
+#pragma unroll
+        for (int e = 0; e < VEC; e++) acc[t] += v[e] * d[e];
+      }
+    }
+#pragma unroll
+    for (int t = 0; t < INNERP_TAPS; t++)
+      for (int o = 16; o > 0; o >>= 1) acc[t] += __shfl_xor_sync(0xffffffffu, acc[t], o);
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+      for (int t = 0; t < INNERP_TAPS; t++) red[threadIdx.x >> 5][t] = acc[t];
+    }
+    __syncthreads();
+    const int tap = t0 + threadIdx.x;
+    if (threadIdx.x < INNERP_TAPS && tap < a.taps) {
+      float s = 0.f;
+      for (int w = 0; w < INNERP_THREADS / 32; w++) s += red[w][threadIdx.x];
+      if (final_pass) a.out[tap] = (a.st == 0.f) ? a.so * s : a.st * a.out[tap] + a.so * s;
+      else a.out[(long long)blockIdx.x * a.taps + tap] = s;
+    }
+    __syncthreads();
+  }
+}
+
+int conv_innerp(const ConvGeom& g, const float* images, const float* derivs, float* targets, float st, float so, int splits) {
+  InnerpArgs a;
+  a.img = images + (long long)g.cin0 * g.H * g.W * g.N;
+  a.der = derivs + (long long)g.cout0 * g.modules * g.N;
+  a.N = g.N; a.W = g.W; a.H = g.H; a.modX = g.modX; a.modules = g.modules;
+  a.kx = g.kx; a.ky = g.ky; a.sx = g.sx; a.sy = g.sy; a.px = g.px; a.py = g.py; a.taps = g.kx * g.ky;
+  a.pairs = (long long)g.Cin * g.modules;
+  a.st = st; a.so = so;
+  // about 16K image values per CTA, at most two waves of CTAs
+  if (splits <= 0)
+    splits = (int)std::min<long long>(std::max<long long>(1, ceil_div<long long>(a.pairs * g.N, 16384)), 2LL * num_sms());
+  a.per_split = ceil_div<long long>(a.pairs, splits);
+  splits = (int)ceil_div<long long>(a.pairs, a.per_split);
+  CNB_REQUIRE(a.per_split * g.N < (1LL << 31), "convInnerpGemm: too many images x modules per channel");
+  const bool v4 = g.N % 4 == 0 && aligned16(images) && aligned16(derivs) && aligned16(a.img) && aligned16(a.der);
+  float* part = splits > 1 ? (float*)workspace(sizeof(float) * (size_t)splits * a.taps) : nullptr;
+  a.out = part ? part : targets;
+  if (v4) innerp_kernel<4><<<splits, INNERP_THREADS, 0, state().stream>>>(a, part ? 0 : 1);
+  else innerp_kernel<1><<<splits, INNERP_THREADS, 0, state().stream>>>(a, part ? 0 : 1);
+  count_launch();
+  CNB_LAUNCH_CHECK("conv_innerp");
+  if (part) reduce_partials(part, targets, a.taps, 1, splits, st, so);
+  return splits;
+}
+
 }  // namespace cnb

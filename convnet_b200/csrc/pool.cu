@@ -648,6 +648,63 @@ bool pool_forward(const PoolGeom& g, bool is_max, const float* images, float* ta
   return emitted;
 }
 
+// ---- max-pool R-operator (kMaxPoolRprop) ---------------------------------------------------------------------------------
+// targets[window] = st * targets[window] + the sum of R_images over every element of the clipped window whose image value
+// equals the stored maximum, ties counted once each, in the reference's (Y, X) order: the reference adds these terms with
+// atomicAdd, but one thread adds all terms of one output in that order, so the sum is the same.  One thread per VEC images
+// of one window: a gather with no atomics.
+template <int VEC>
+__global__ void __launch_bounds__(256) pool_rprop_kernel(PoolGeom g, const float* __restrict__ images,
+                                                          const float* __restrict__ R_images, const float* __restrict__ maxes,
+                                                          float* targets, float st) {
+  pdl_wait();
+  pdl_trigger();
+  const unsigned NV = g.N / VEC;
+  const unsigned plane = NV * g.modX * g.modY;
+  const float* img = images + (long long)g.N * g.W * g.H * blockIdx.y;
+  const float* rim = R_images + (long long)g.N * g.W * g.H * blockIdx.y;
+  for (unsigned pidx = blockIdx.x * blockDim.x + threadIdx.x; pidx < plane; pidx += gridDim.x * blockDim.x) {
+    const unsigned nv = pidx % NV, r = pidx / NV;
+    const int mx = r % g.modX, my = r / g.modX;
+    const long long idx = ((long long)blockIdx.y * plane + pidx) * VEC;
+    float m[VEC], acc[VEC];
+    vload<VEC>(maxes + idx, m);
+    if (st != 0.f) {
+      vload<VEC>(targets + idx, acc);
+#pragma unroll
+      for (int v = 0; v < VEC; v++) acc[v] *= st;
+    } else {
+#pragma unroll
+      for (int v = 0; v < VEC; v++) acc[v] = 0.f;
+    }
+    const int sX = max(mx * g.sx + g.px, 0), sY = max(my * g.sy + g.py, 0);
+    const int eX = min(mx * g.sx + g.px + g.kx, g.W), eY = min(my * g.sy + g.py + g.ky, g.H);
+    for (int Y = sY; Y < eY; Y++)
+      for (int X = sX; X < eX; X++) {
+        const long long off = (long long)g.N * (X + (long long)g.W * Y) + nv * VEC;
+        float a[VEC], ra[VEC];
+        vload<VEC>(img + off, a);
+        vload<VEC>(rim + off, ra);
+#pragma unroll
+        for (int v = 0; v < VEC; v++)
+          if (a[v] == m[v]) acc[v] += ra[v];           // (not `+= tie ? r : 0`: adding +0 would turn a -0 sum into +0)
+      }
+    vstore<VEC>(targets + idx, acc);
+  }
+}
+
+void max_pool_rprop(const PoolGeom& g, const float* images, const float* R_images, const float* maxes, float* targets, float st) {
+  CNB_REQUIRE(g.T == 1 && g.modT == 1 && g.kt == 1, "MaxPoolRpropGemm: 2-D pooling only");
+  const bool v4 = (g.N % 4 == 0) && aligned16(images) && aligned16(R_images) && aligned16(maxes) && aligned16(targets);
+  const long long per_plane = (long long)g.modX * g.modY * (v4 ? g.N / 4 : g.N);
+  CNB_REQUIRE(per_plane < (1LL << 30) && g.C <= 65535, "MaxPoolRpropGemm: plane too large");
+  const dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(ceil_div<long long>(per_plane, 256), 64)), g.C);
+  if (v4) launch_pdl(pool_rprop_kernel<4>, grid, dim3(256), 0, state().stream, g, images, R_images, maxes, targets, st);
+  else launch_pdl(pool_rprop_kernel<1>, grid, dim3(256), 0, state().stream, g, images, R_images, maxes, targets, st);
+  count_launch();
+  CNB_LAUNCH_CHECK("max_pool_rprop");
+}
+
 template <int VEC, bool MAX>
 // colsum (may be null): on return *colsum_slices > 0 iff the kernel wrote per-(row, plane) sums of its output to `colsum`
 static bool launch_undo(const PoolGeom& g, const float* images, const float* grads, const float* acts, float* targets,

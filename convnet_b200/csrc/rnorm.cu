@@ -391,6 +391,98 @@ __global__ void __launch_bounds__(RN_THREADS) rnorm_undo_tile_kernel(const float
   }
 }
 
+// R-operator (kCrossMapRNormRprop, gemm.cu:491-514): the directional derivative of the forward pass along R,
+//   t_j = R_j base_j^-beta - 2 alpha beta x_j base_j^(-beta-1) sum_{i in window(j)} x_i R_i,  base_j = 1 + alpha S_j,
+// with the FORWARD window of j for both sums.  Same phases as the forward tile: x and R tiles, exclusive prefixes of x^2
+// (Q) and of x R (P) along the channels, then every (channel, location) from two prefix differences and one __powf.
+template <int TL>
+__global__ void __launch_bounds__(RN_THREADS) rnorm_rprop_tile_kernel(const float* __restrict__ x, const float* __restrict__ rx,
+                                                                       float* __restrict__ out, long long L, int F, int k,
+                                                                       float alpha, float beta, int blocked, int vec) {
+  pdl_wait();
+  pdl_trigger();
+  extern __shared__ __align__(16) float sm[];
+  float* X = sm;                               // [F][TL]
+  float* Rv = X + (size_t)F * TL;              // [F][TL]
+  float* Q = Rv + (size_t)F * TL;              // [F+1][TL] exclusive prefix of x^2
+  float* P = Q + (size_t)(F + 1) * TL;         // [F+1][TL] x R, then its exclusive prefix
+  float* segtot = P + (size_t)(F + 1) * TL;
+  const long long l0 = (long long)blockIdx.x * TL;
+  const int valid = (int)min((long long)TL, L - l0);
+  rn_load_tile<TL>(X, x, L, l0, F, valid, vec != 0);
+  rn_load_tile<TL>(Rv, rx, L, l0, F, valid, vec != 0);
+  rn_cp_wait_all();
+  __syncthreads();
+  for (int idx = threadIdx.x; idx < F * TL; idx += RN_THREADS) P[idx] = X[idx] * Rv[idx];
+  __syncthreads();
+  rn_prefix<TL, true>(X, Q, segtot, F);
+  rn_prefix<TL, false>(P, P, segtot, F);
+  const int a = k / 2, b = k - a - 1;
+  const float c2 = 2.f * alpha * beta;
+  constexpr int Q4 = TL / 4;
+  for (int idx = threadIdx.x; idx < F * Q4; idx += RN_THREADS) {
+    const int f = idx / Q4, l = 4 * (idx - f * Q4);
+    if (l >= valid) continue;
+    int lo, hi; rn_window(f, F, k, a, b, blocked != 0, lo, hi);
+    const float4 qh = *reinterpret_cast<const float4*>(Q + hi * TL + l), ql = *reinterpret_cast<const float4*>(Q + lo * TL + l);
+    const float4 ph = *reinterpret_cast<const float4*>(P + hi * TL + l), pl = *reinterpret_cast<const float4*>(P + lo * TL + l);
+    const float4 xv = *reinterpret_cast<const float4*>(X + f * TL + l), rv = *reinterpret_cast<const float4*>(Rv + f * TL + l);
+    float4 r;
+    { const float base = 1.f + alpha * (qh.x - ql.x), den = __powf(base, -beta - 1.f); r.x = rv.x * (den * base) - c2 * xv.x * den * (ph.x - pl.x); }
+    { const float base = 1.f + alpha * (qh.y - ql.y), den = __powf(base, -beta - 1.f); r.y = rv.y * (den * base) - c2 * xv.y * den * (ph.y - pl.y); }
+    { const float base = 1.f + alpha * (qh.z - ql.z), den = __powf(base, -beta - 1.f); r.z = rv.z * (den * base) - c2 * xv.z * den * (ph.z - pl.z); }
+    { const float base = 1.f + alpha * (qh.w - ql.w), den = __powf(base, -beta - 1.f); r.w = rv.w * (den * base) - c2 * xv.w * den * (ph.w - pl.w); }
+    rn_store4(out, nullptr, (long long)f * L + l0 + l, r, l, valid, vec != 0);
+  }
+}
+
+// the R-operator when no tile fits (numFilters beyond ~440): one location per thread walks the channels with running
+// sums of x^2 and x R over the window, the last k values of x and R in a per-thread ring (shared memory, or workspace)
+template <bool BLOCKED>
+__global__ void __launch_bounds__(RN_THREADS) rnorm_rprop_kernel(const float* __restrict__ x, const float* __restrict__ rx,
+                                                                  float* __restrict__ out, long long L, int F, int k, float alpha,
+                                                                  float beta, float* gring, long long gstride) {
+  extern __shared__ __align__(16) float sring[];
+  const long long loc = blockIdx.x * (long long)RN_THREADS + threadIdx.x;
+  if (loc >= L) return;
+  const long long rs = gring ? gstride : RN_THREADS;
+  float* ring_x = gring ? gring + loc : sring + threadIdx.x;
+  float* ring_r = ring_x + (long long)k * rs;
+  x += loc; rx += loc; out += loc;
+  const float c2 = 2.f * alpha * beta;
+  auto emit = [&](long long j, float xj, float rj, float sq, float sxr) {
+    const float base = 1.f + alpha * sq, den = __powf(base, -beta - 1.f);
+    out[j * L] = rj * (den * base) - c2 * xj * den * sxr;
+  };
+  if (BLOCKED) {
+    for (int s = 0; s < F; s += k) {
+      const int e = min(F, s + k);
+      float sq = 0.f, sxr = 0.f;
+      for (int i = s; i < e; i++) {
+        const float xi = __ldg(x + (long long)i * L), ri = __ldg(rx + (long long)i * L);
+        ring_x[(i - s) * rs] = xi; ring_r[(i - s) * rs] = ri;
+        sq += xi * xi; sxr += xi * ri;
+      }
+      for (int i = s; i < e; i++) emit(i, ring_x[(i - s) * rs], ring_r[(i - s) * rs], sq, sxr);
+    }
+    return;
+  }
+  const int a = k / 2, b = k - a - 1;
+  float sq = 0.f, sxr = 0.f;
+  // q = entering channel; output channel j = q - b; window [j-a, j+b] = [q-k+1, q]; channels >= F enter as zeros
+  for (int q = 0; q < F + b; q++) {
+    const int slot = q % k;
+    float xo = 0.f, ro = 0.f, xq = 0.f, rq = 0.f;
+    if (q >= k) { xo = ring_x[slot * rs]; ro = ring_r[slot * rs]; }
+    if (q < F) { xq = __ldg(x + (long long)q * L); rq = __ldg(rx + (long long)q * L); }
+    ring_x[slot * rs] = xq; ring_r[slot * rs] = rq;
+    sq += xq * xq - xo * xo;
+    sxr += xq * rq - xo * ro;
+    const int j = q - b;
+    if (j >= 0) { const int sj = j % k; emit(j, ring_x[sj * rs], ring_r[sj * rs], sq, sxr); }
+  }
+}
+
 // tile width for `arrays` F-row arrays (+2 spare rows and the segment totals): the widest of 64 / 32 that lets two CTAs
 // share an SM, else the widest that fits at all; 0 = no tile kernel (window walk with the ring instead)
 static int pick_tile(int F, int arrays, size_t* smem_out) {
@@ -519,6 +611,34 @@ void rnorm_undo(const float* outGrads, const float* inputs, float* targets, long
   launch_undo(outGrads, inputs, targets, L, F, k, alpha, beta, blocked);
   count_launch();
   CNB_LAUNCH_CHECK("rnorm_undo");
+}
+
+void rnorm_rprop(const float* images, const float* R_images, float* targets, long long L, int F, int k, float alpha,
+                 float beta, bool blocked) {
+  CNB_REQUIRE(k >= 1 && F >= 1, "ResponseNormCrossMapRpropGemm");
+  cudaStream_t s = state().stream;
+  size_t tsmem = 0;
+  const int tl = L < (1LL << 31) * 32 ? pick_tile(F, 4, &tsmem) : 0;
+  if (tl) {
+    const bool vec = L % 4 == 0 && aligned16(images) && aligned16(R_images) && aligned16(targets);
+    const long long tiles = ceil_div<long long>(L, tl);
+    auto kern = tl == 64 ? rnorm_rprop_tile_kernel<64> : rnorm_rprop_tile_kernel<32>;
+    if (tsmem > 48 * 1024) CNB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tsmem));
+    launch_pdl(kern, dim3((unsigned)tiles), dim3(RN_THREADS), tsmem, s, images, R_images, targets, L, F, k, alpha, beta,
+               blocked ? 1 : 0, vec ? 1 : 0);
+    count_launch();
+    CNB_LAUNCH_CHECK("rnorm_rprop(tile)");
+    return;
+  }
+  size_t smem = sizeof(float) * 2 * (size_t)k * RN_THREADS;
+  float* gring = nullptr;
+  if (smem > kMaxRingSmem) { gring = (float*)workspace(sizeof(float) * 2 * (size_t)k * L); smem = 0; }
+  auto kern = blocked ? rnorm_rprop_kernel<true> : rnorm_rprop_kernel<false>;
+  if (smem > 48 * 1024) CNB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kern<<<(unsigned)ceil_div<long long>(L, RN_THREADS), RN_THREADS, smem, s>>>(images, R_images, targets, L, F, k, alpha, beta,
+                                                                             gring, L);
+  count_launch();
+  CNB_LAUNCH_CHECK("rnorm_rprop");
 }
 
 }  // namespace cnb

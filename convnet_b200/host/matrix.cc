@@ -1,6 +1,8 @@
 // matrix.cc — see matrix.h.  Thin dispatch to the C ABI, like src/matrix.cc:785-1011.
 #include "matrix.h"
 
+#include "../../include/convnet_b200_conv.h"
+
 #include <cstdio>
 #include <cstdlib>
 
@@ -104,6 +106,8 @@ void Matrix::ConvDown(Matrix& deriv_output, Matrix& w, Matrix& deriv_input, Conv
   convDownGemm(deriv_output.GetMat(), w.GetMat(), deriv_input.GetMat(), &deriv_output.GetShape4D(), &w.GetShape4D(),
                &deriv_input.GetShape4D(), conv_desc, scale_targets);
 }
+void Matrix::ConvRGBToYUV(Matrix& input, Matrix& output) { RGBToYUV(input.GetMat(), output.GetMat()); }
+
 void Matrix::ExtractPatches(Matrix& source, Matrix& dest, Matrix& width_offset, Matrix& height_offset, Matrix& flip_bit,
                             int image_size_y, int image_size_x, int patch_size_y, int patch_size_x) {   // src/matrix.cc:1030-1042
   const int err_code = convnet_b200_extract_patches(source.GetMat(), dest.GetMat(), width_offset.GetMat(), height_offset.GetMat(),

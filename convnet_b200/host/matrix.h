@@ -80,6 +80,8 @@ class Matrix {
                                              int image_size_t);
 
   // minibatch crop / mirror / transpose out of an image-major chunk (src/matrix.cc:1030-1042 -> extract_patches)
+  // RGB -> YUV of a batch: input (images, 3 * pixels) holds the R, G and B planes, output gets Y, U and V (src/matrix.cc:1013)
+  static void ConvRGBToYUV(Matrix& input, Matrix& output);
   static void ExtractPatches(Matrix& source, Matrix& dest, Matrix& width_offset, Matrix& height_offset, Matrix& flip_bit,
                              int image_size_y, int image_size_x, int patch_size_y, int patch_size_x);
 

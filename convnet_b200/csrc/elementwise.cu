@@ -189,6 +189,42 @@ __global__ void relu_deriv_kernel(float* dx, const float* __restrict__ y, long l
   }
   for (long long i = 4 * n4 + tid; i < n; i += nt) dx[i] = y[i] > 0.f ? dx[i] : 0.f;
 }
+// Polyak average of k queue slots, laid out like relu_kernel (slot_stride % 4 == 0 on the vector body).  K > 0: k known
+// at compile time, so the k loads of a float4 group are all issued before the first add; K == 0: any k
+template <int K>
+__global__ void __launch_bounds__(256) polyak_kernel(float* out, const float* __restrict__ queue, long long n, long long n4,
+                                                     long long stride, int k, __nv_bfloat16* out16) {
+  const int kk = K > 0 ? K : k;
+  const float kf = (float)kk;
+  const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
+  for (long long i = tid; i < n4; i += nt) {
+    float4 s[K > 0 ? K : 1];
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (K > 0) {
+#pragma unroll
+      for (int j = 0; j < (K > 0 ? K : 1); j++) s[j] = __ldcs(reinterpret_cast<const float4*>(queue + j * stride) + i);
+#pragma unroll
+      for (int j = 0; j < (K > 0 ? K : 1); j++) { a.x += s[j].x; a.y += s[j].y; a.z += s[j].z; a.w += s[j].w; }
+    } else {
+#pragma unroll 4
+      for (int j = 0; j < kk; j++) {
+        const float4 v = __ldcs(reinterpret_cast<const float4*>(queue + j * stride) + i);
+        a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
+      }
+    }
+    a.x = __fdiv_rn(a.x, kf); a.y = __fdiv_rn(a.y, kf); a.z = __fdiv_rn(a.z, kf); a.w = __fdiv_rn(a.w, kf);
+    reinterpret_cast<float4*>(out)[i] = a;
+    emit4(out16, i, a);
+  }
+  for (long long i = 4 * n4 + tid; i < n; i += nt) {
+    float a = 0.f;
+    for (int j = 0; j < kk; j++) a += queue[j * stride + i];
+    a = __fdiv_rn(a, kf);
+    out[i] = a;
+    if (out16) out16[i] = __float2bfloat16_rn(a);
+  }
+}
+
 // the logistic unit and its derivative (LogisticLayer, src/layer.cc:586-602), laid out like relu_kernel / relu_deriv_kernel
 __global__ void logistic_kernel(float* x, long long n, long long n4, __nv_bfloat16* out16) {
   const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
@@ -935,6 +971,21 @@ void cnb_opt_update_multi(const CnbOptTensorEx* tensors, int count) {
     norm_rescale_kernel<<<nblocks, 256, 0, state().stream>>>(nb);
     count_launch(); CNB_LAUNCH_CHECK("sgd_norm_rescale");
   }
+}
+void cnb_polyak_average(float* out, const float* queue, long long n, long long slot_stride, int k) {
+  CNB_REQUIRE(k >= 1 && slot_stride >= n && (n <= 0 || queue + (k - 1) * slot_stride + n <= out ||
+                                             out + n <= queue), "cnb_polyak_average");
+  write_pass("polyak_average", out, n, true, [&](__nv_bfloat16* o16) {
+    const long long n4 = aligned16(out) && aligned16(queue) && slot_stride % 4 == 0 ? n / 4 : 0;
+    const int grid = blocks_for(std::max(n4, n - 4 * n4), 256);
+    switch (k) {
+#define CNB_POLYAK_K(K) case K: polyak_kernel<K><<<grid, 256, 0, state().stream>>>(out, queue, n, n4, slot_stride, k, o16); break;
+      CNB_POLYAK_K(1) CNB_POLYAK_K(2) CNB_POLYAK_K(3) CNB_POLYAK_K(4) CNB_POLYAK_K(5) CNB_POLYAK_K(6) CNB_POLYAK_K(7)
+      CNB_POLYAK_K(8)
+#undef CNB_POLYAK_K
+      default: polyak_kernel<0><<<grid, 256, 0, state().stream>>>(out, queue, n, n4, slot_stride, k, o16);
+    }
+  });
 }
 void cnb_sgd_update_multi(const CnbOptTensor* tensors, int count) {
   std::vector<CnbOptTensorEx> t(count > 0 ? count : 0);

@@ -3,6 +3,7 @@
 #include <cstdio>
 #include <cstring>
 #include <stdexcept>
+#include <string>
 
 #include "convnet.h"
 #include "data.h"
@@ -37,7 +38,14 @@ API void* cnb_net_create(const char* model, int batch_size, unsigned seed, int g
     delete h;
     return nullptr;
   }
-  h->net->AllocateMemory();
+  try {
+    h->net->AllocateMemory();                                  // (reads the checkpoints of PRETRAINED edges)
+  } catch (const std::exception& e) {
+    fprintf(stderr, "convnet_b200 host: %s\n", e.what());
+    delete h->net;
+    delete h;
+    return nullptr;
+  }
   return h;
 }
 API void cnb_net_destroy(void* p) {
@@ -60,6 +68,8 @@ API int cnb_net_num_classes(void* p) { return ((NetHandle*)p)->net->OutputLayer(
 // the caller may write through this pointer: staged bf16 copies of the weights are dropped
 API float* cnb_net_params(void* p) { ((NetHandle*)p)->net->InvalidateStaging(); return ((NetHandle*)p)->net->Parameters().GetDevData(); }
 API float* cnb_net_grads(void* p) { return ((NetHandle*)p)->net->GradParameters().GetDevData(); }
+// the momentum history (laid out like the parameters); a write through it is the caller's
+API float* cnb_net_history(void* p) { return ((NetHandle*)p)->net->History().GetDevData(); }
 API float* cnb_net_layer_state(void* p, int i) { return ((NetHandle*)p)->net->Layers()[i]->GetState().GetDevData(); }
 API long long cnb_net_layer_floats(void* p, int i) { return (long long)((NetHandle*)p)->net->Layers()[i]->GetState().GetNumEls(); }
 API int cnb_net_num_layers(void* p) { return (int)((NetHandle*)p)->net->Layers().size(); }
@@ -291,20 +301,64 @@ API long long cnb_model_text(const char* model, char* buf, long long cap) {
 }
 
 // static description of a model: the initial weights of edge `edge` under RNG seed `seed` (EdgeWithWeight::InitialWeights;
-// the net seeds edge i with its seed + 17 i).  Returns their number (writes up to `cap`); -1 unknown model, -2 edge out of
-// range or without parameters
+// the net seeds edge i with its seed + 17 i), or a PRETRAINED edge's weights from its checkpoint.  Returns their number
+// (writes up to `cap`); -1 unknown model or unreadable checkpoint, -2 edge out of range or without parameters
 API long long cnb_model_initial_weights(const char* model, int edge, unsigned seed, float* out, long long cap) {
   ConvNet* net = TryBuildNet(model, 1);
   if (!net) return -1;
   EdgeWithWeight* e = edge >= 0 && edge < (int)net->Edges().size() ? dynamic_cast<EdgeWithWeight*>(net->Edges()[edge].get()) : nullptr;
   long long n = -2;
   if (e) {
-    const std::vector<float> w = e->InitialWeights(seed);
+    std::vector<float> w;
+    try {
+      w = e->Config().initialization == PRETRAINED ? PretrainedWeights(e->Config(), e->WeightCount()) : e->InitialWeights(seed);
+    } catch (const std::exception& x) {
+      fprintf(stderr, "convnet_b200 host: %s\n", x.what());
+      delete net;
+      return -1;
+    }
     n = (long long)w.size();
     if (cap > 0) memcpy(out, w.data(), sizeof(float) * (size_t)std::min(n, cap));
   }
   delete net;
   return n;
+}
+
+// ---- checkpoints and Polyak averaging (checkpoint.cc).  Each returns 0, or -1 with the message on stderr and in
+// cnb_last_error()
+static std::string g_last_error;
+API const char* cnb_last_error() { return g_last_error.c_str(); }
+template <class F>
+static int Guard(F f) {
+  try {
+    f();
+    return 0;
+  } catch (const std::exception& e) {
+    g_last_error = e.what();
+    fprintf(stderr, "convnet_b200 host: %s\n", e.what());
+    return -1;
+  }
+}
+API int cnb_net_save(void* p, const char* path) { return Guard([&] { ((NetHandle*)p)->net->Save(path); }); }
+API int cnb_net_load(void* p, const char* path) { return Guard([&] { ((NetHandle*)p)->net->Load(path); }); }
+API long long cnb_net_iteration(void* p) { return (long long)((NetHandle*)p)->net->Iteration(); }
+API int cnb_net_polyak_insert(void* p) { return Guard([&] { ((NetHandle*)p)->net->InsertPolyak(); }); }
+API int cnb_net_load_polyak_weights(void* p) { return Guard([&] { ((NetHandle*)p)->net->LoadPolyakWeights(); }); }
+API int cnb_net_load_current_weights(void* p) { return Guard([&] { ((NetHandle*)p)->net->LoadCurrentWeights(); }); }
+API int cnb_net_polyak_count(void* p) { return ((NetHandle*)p)->net->PolyakCount(); }
+// static description of a model: its Polyak settings.  1 Polyak on, 0 off, -1 unknown model
+API int cnb_model_polyak(const char* model, int* after, int* queue_size, int* validate_after, int* save_after) {
+  ModelConfig m;
+  if (!TryBuildModel(model, &m)) return -1;
+  *after = m.polyak_after; *queue_size = m.polyak_queue_size; *validate_after = m.validate_after; *save_after = m.save_after;
+  return PolyakOn(m) ? 1 : 0;
+}
+// pure host logic: 1 if the reference's loop inserts into the Polyak queue after TrainOneBatch call `iteration` (PolyakDue),
+// 0 if not, -1 unknown model
+API int cnb_polyak_due(const char* model, long long iteration) {
+  ModelConfig m;
+  if (!TryBuildModel(model, &m)) return -1;
+  return PolyakDue(m, iteration) ? 1 : 0;
 }
 
 // ---- the device side of the input pipeline (data.h): a GPU-resident chunk + per-minibatch crop / mirror into the net's input

@@ -351,8 +351,10 @@ std::string ConvNet::Refusal() const {
       return "edge '" + edges_[i]->GetName() + "': LOCAL is not supported on 3-D layers (image_size_t > 1)";
     const int init = model_.edge[i].initialization;
     if (!edges_[i]->HasNoParameters() && init != DENSE_GAUSSIAN && init != DENSE_GAUSSIAN_SQRT_FAN_IN &&
-        init != DENSE_UNIFORM && init != DENSE_UNIFORM_SQRT_FAN_IN && init != CONSTANT)
+        init != DENSE_UNIFORM && init != DENSE_UNIFORM_SQRT_FAN_IN && init != CONSTANT && init != PRETRAINED)
       return "edge '" + edges_[i]->GetName() + "': initialization " + std::to_string(init) + " is not implemented";
+    if (!edges_[i]->HasNoParameters() && init == PRETRAINED && model_.edge[i].pretrained_model.empty())
+      return "edge '" + edges_[i]->GetName() + "': initialization PRETRAINED without pretrained_model";
   }
   for (const auto& l : layers_) {                    // what the batch-norm passes cannot run
     if (!l->BatchNormalize()) continue;
@@ -413,6 +415,7 @@ ConvNet::~ConvNet() {
   if (lane_.ready) cudaEventDestroy(lane_.ready);
   for (cudaEvent_t e : {trace_.t0, trace_.fwd, trace_.bwd, trace_.end}) if (e) cudaEventDestroy(e);
   for (std::vector<cudaEvent_t>* v : {&trace_.c0, &trace_.c1, &trace_.s1}) for (cudaEvent_t e : *v) cudaEventDestroy(e);
+  if (polyak_) cudaFree(polyak_);
   convnet_b200_reserve_sms(0);
   convnet_b200_bf16_invalidate(nullptr);                     // the buffers go away; a later net may get the same addresses
 }
@@ -474,6 +477,10 @@ void ConvNet::AllocateMemory() {
   for (size_t i = 0; i < layers_.size(); i++)
     if (bn_offset_[i] >= 0) adaptive |= IsAdaptive(layers_[i]->BnOptimizer(0)) || IsAdaptive(layers_[i]->BnOptimizer(1));
   if (adaptive) AllocateAdaptiveState();
+  // the reference allocates the optimizers before Initialize reads a PRETRAINED edge (fc_edge.cc:42, convnet.cc:286-303),
+  // so the edge takes the history, the step and the adaptive state from the file too
+  for (size_t i = 0; i < edges_.size(); i++)
+    if (!edges_[i]->HasNoParameters() && model_.edge[i].initialization == PRETRAINED) LoadPretrained(i);
   HOST_CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
   InvalidateStaging();
   HOST_CUDA_CHECK(cudaStreamCreateWithFlags(&side_, cudaStreamNonBlocking));
@@ -779,9 +786,13 @@ std::vector<Bucket> PlanBuckets(const std::vector<size_t>& edge_offset, const st
 
 void ConvNet::SetDataParallel(DataParallelSync* dp, size_t bucket_floats) {
   dp_ = dp;
-  dropout_salt_ = ((unsigned long long)model_.seed * 0xA24BAED4963EE407ULL) ^
-                  ((unsigned long long)((dp ? dp->rank() : 0) + 1) * 0xD1B54A32D192ED03ULL);
+  SaltDropout();
   SetBucketFloats(bucket_floats);
+}
+void ConvNet::SaltDropout() {
+  salted_ = true;
+  dropout_salt_ = ((unsigned long long)model_.seed * 0xA24BAED4963EE407ULL) ^
+                  ((unsigned long long)((dp_ ? dp_->rank() : 0) + 1) * 0xD1B54A32D192ED03ULL);
 }
 void ConvNet::SetBucketFloats(size_t bucket_floats) {
   buckets_ = PlanBuckets(edge_offset_, edge_span_, bucket_floats);

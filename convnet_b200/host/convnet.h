@@ -8,6 +8,7 @@
 // from a ModelConfig struct: built by name in models.cc, or read from the reference's config::Model
 // text proto (a net.pbtxt file) in model_file.cc.
 #pragma once
+#include <map>
 #include <memory>
 #include <string>
 #include <vector>
@@ -62,6 +63,49 @@ struct ModelConfig {
   std::vector<LayerConfig> layer;
   std::vector<EdgeConfig> edge;
   unsigned seed = 42;
+  // Polyak averaging (proto Model fields, same defaults): on when polyak_after and polyak_queue_size are both > 0; its
+  // insertion rule (PolyakDue) also reads validate_after and save_after
+  int polyak_after = 0, polyak_queue_size = 0, validate_after = -1, save_after = -1;
+};
+inline bool PolyakOn(const ModelConfig& m) { return m.polyak_after > 0 && m.polyak_queue_size > 0; }
+// checkpoint.cc: whether the reference's training loop inserts the parameters into the Polyak queue after TrainOneBatch call
+// number `iteration` (src/convnet.cc:881-883, 965-967 with i + 1 = iteration; C++'s truncating %).  False with Polyak off
+bool PolyakDue(const ModelConfig& m, long long iteration);
+
+// checkpoint.cc: a checkpoint file (DESIGN.md §5 "Checkpoints"): an 8-byte magic, a u32 version, then records until EOF,
+// each a u32 name length, the name, a u8 type, a u64 element count and the payload, little-endian.  The constructor reads
+// the record headers and checks that every payload is there; std::invalid_argument names the file and what is wrong
+class CheckpointFile {
+ public:
+  enum Type { FLOAT32 = 0, INT64 = 1, TEXT = 2 };
+  explicit CheckpointFile(const std::string& path);
+  const std::string& Path() const { return path_; }
+  const std::vector<std::string>& Names() const { return names_; }        // in file order
+  bool Has(const std::string& name) const { return records_.count(name) != 0; }
+  // "" if record `name` exists with this type and element count (count < 0: any), else why not (the file, the record and
+  // both sizes where they apply)
+  std::string Check(const std::string& name, int type, long long count) const;
+  std::vector<char> Read(const std::string& name) const;                   // the payload bytes (std::runtime_error: I/O)
+ private:
+  struct Record { int type; long long count, offset; };
+  std::string path_;
+  std::vector<std::string> names_;
+  std::map<std::string, Record> records_;
+};
+// the weights a PRETRAINED edge `c` of `n` weights takes from its checkpoint (record <pretrained_edge_name>:weight)
+std::vector<float> PretrainedWeights(const EdgeConfig& c, long long n);
+
+// one record of a net's checkpoint: a float32 tensor at `offset` of the parameters, the momentum history, the adaptive
+// state or (RUNNING) the layer's running statistic `which`, or (STEP) the step count of optimizer `which` of `edge` / `layer`
+struct CheckpointEntry {
+  enum Buffer { PARAMS, HISTORY, STATE, RUNNING, STEP };
+  std::string name;
+  Buffer buffer;
+  size_t offset;
+  long long n;
+  EdgeWithWeight* edge;
+  Layer* layer;
+  int which;
 };
 
 class Layer {                                   // src/layer.{h,cc}, reduced to state/deriv + activation
@@ -117,6 +161,7 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   void AppendBnSgdTensors(std::vector<CnbOptTensorEx>& out);    // gamma and beta; advances both step counts
   OptimizerConfig& BnOptimizer(int which) { return which ? config_.beta_optimizer : config_.gamma_optimizer; }   // 0 gamma, 1 beta
   long long BnOptimizerStep(int which) const { return which ? beta_step_ : gamma_step_; }
+  void SetBnOptimizerStep(int which, long long step) { (which ? beta_step_ : gamma_step_) = step; }
   // device vectors of `channels` floats: 0 running mean, 1 running sigma, 2 batch mean, 3 batch sigma
   float* BnStat(int which) { return bn_stats_.GetDevData() + (size_t)which * config_.num_channels; }
   long long BnPixels() const { return (long long)image_size_y_ * image_size_x_; }
@@ -193,12 +238,29 @@ class ConvNet {
   void BroadcastParameters();
   void InvalidateStaging();                                     // after any write to the parameters from outside UpdateWeights
 
+  // ---- checkpoints and Polyak averaging (checkpoint.cc; src/convnet.cc:659-751)
+  // Save: waits for every stream, writes path + "temp", flushes and fsyncs it and renames it to `path`.  Load: reads and
+  // validates the whole file before it changes anything (std::invalid_argument names the record; the net is then
+  // unchanged), applies the file's optimizer blocks, copies every record, takes the file's seed and iteration, and leaves
+  // the staged bf16 copies and dgrad banks coherent.  std::runtime_error: an I/O failure
+  void Save(const std::string& path);
+  void Load(const std::string& path);
+  ModelConfig CurrentModel() const;                             // the model with the optimizer settings now in force
+  unsigned long long Iteration() const { return step_; }        // TrainOneBatch calls so far (the dropout step)
+  // Polyak queue on the device, allocated at the first insert: polyak_queue_size slots and a backup of the parameters.
+  // std::invalid_argument: Polyak is off, nothing inserted, no backup; std::runtime_error: the allocation failed
+  void InsertPolyak();                                          // parameters -> next slot (device copy, no host wait)
+  void LoadPolyakWeights();                                     // backup <- parameters; parameters <- the average
+  void LoadCurrentWeights();                                    // parameters <- backup
+  int PolyakCount() const { return polyak_full_ ? model_.polyak_queue_size : polyak_index_; }
+
   Layer& InputLayer() { return *layers_.front(); }
   Layer& OutputLayer() { return *layers_.back(); }
   std::vector<std::unique_ptr<Edge>>& Edges() { return edges_; }
   std::vector<std::unique_ptr<Layer>>& Layers() { return layers_; }
   Matrix& Parameters() { return parameters_; }
   Matrix& GradParameters() { return grad_parameters_; }
+  Matrix& History() { return history_; }
   size_t NumParameters() const { return num_params_; }
   int BatchSize() const { return batch_size_; }
   double FlopsFprop() const;
@@ -256,6 +318,17 @@ class ConvNet {
   } trace_;
   unsigned long long step_ = 0;
   unsigned long long dropout_salt_ = 0xD1B54A32D192ED03ULL;      // model seed and data-parallel rank, see SetDataParallel
+  bool salted_ = false;                                          // SetDataParallel has set dropout_salt_ (SaltDropout)
+  void SaltDropout();
+  // checkpoint.cc
+  std::vector<CheckpointEntry> CheckpointEntries(const ModelConfig& optimizers);   // in params order
+  float* EntryData(const CheckpointEntry& e);
+  void LoadPretrained(size_t edge);                             // a PRETRAINED edge's records, after AllocateAdaptiveState
+  void WaitAllStreams();                                        // host waits for the main, side, comm and optimizer streams
+  void PrestageAll();                                           // every prestaging edge rebuilds its dgrad banks (main stream)
+  float* polyak_ = nullptr;                                     // polyak_queue_size slots, then the backup
+  int polyak_index_ = 0;
+  bool polyak_full_ = false, polyak_backup_ = false;
 };
 
 // src/grad_check.{h,cc}: finite-difference check of dLoss/dparam for the first k weights and biases
@@ -287,6 +360,9 @@ ModelConfig BuildModel(const std::string& name);
 // ReadModelFile applies the proto's defaults and presence rules, the default optimizers (src/convnet.cc:41-62) and the
 // chain order of the graph; std::invalid_argument names the file, the line and the field of what it cannot read or run.
 ModelConfig ReadModelFile(const std::string& path);
+// the same for model text that `where` names in messages; check_pretrained = false skips opening the checkpoints of
+// PRETRAINED edges (ConvNet::Load reading a checkpoint's own __model__)
+ModelConfig ReadModelText(const std::string& text, const std::string& where, bool check_pretrained);
 // `m` as a config::Model text proto that ReadModelFile reads back to the same model: every field the host reads for a
 // layer or edge of that kind explicit, floats printed so that they read back bit-exactly
 std::string ModelText(const ModelConfig& m);

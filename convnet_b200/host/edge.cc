@@ -269,6 +269,7 @@ std::vector<float> EdgeWithWeight::InitialWeights(unsigned seed) const {
   return h;
 }
 void EdgeWithWeight::Initialize(unsigned seed) {
+  if (config_.initialization == PRETRAINED) return;          // ConvNet::AllocateMemory reads it from its checkpoint
   const std::vector<float> h = InitialWeights(seed);
   const size_t n = weights_.GetNumEls();
   weights_.CopyFromHost(h.data(), n);

@@ -59,8 +59,8 @@ void OptimizerSchedule(const OptimizerConfig& c, long long step, float* epsilon,
 void AppendOptTensor(const OptimizerConfig& o, long long& step, float* w, float* hist, const float* grad, float* state,
                      long long n, int rows, std::vector<CnbOptTensorEx>& out);
 
-// proto/convnet_config.proto:142-150 Initialization, same numbers.  SPARSE_GAUSSIAN and PRETRAINED are not implemented
-// (a model file that asks for them is refused)
+// proto/convnet_config.proto:142-150 Initialization, same numbers.  SPARSE_GAUSSIAN is not implemented (a model file that
+// asks for it is refused); PRETRAINED reads the edge from a checkpoint file (ConvNet::AllocateMemory, checkpoint.cc)
 enum Initialization {
   DENSE_GAUSSIAN = 0, SPARSE_GAUSSIAN = 1, CONSTANT = 2, DENSE_GAUSSIAN_SQRT_FAN_IN = 3, PRETRAINED = 4, DENSE_UNIFORM = 5,
   DENSE_UNIFORM_SQRT_FAN_IN = 6
@@ -85,6 +85,9 @@ struct EdgeConfig {
   int initialization = DENSE_UNIFORM_SQRT_FAN_IN;
   float init_wt = 1.f;
   float init_bias = 0.f;
+  // PRETRAINED: the checkpoint file, used as given, and the edge whose records it takes ("" = this edge's source:dest,
+  // edge_with_weight.cc:18-19)
+  std::string pretrained_model, pretrained_edge_name;
   OptimizerConfig weight_optimizer, bias_optimizer;
   bool grad_check = false;
   int grad_check_num_params = 10;
@@ -238,6 +241,10 @@ class EdgeWithWeight : public Edge {
   // the optimizer of the weights (which = 0) or of the bias (1): its settings, and how many updates it has counted
   OptimizerConfig& Optimizer(int which) { return which ? bias_opt_ : weight_opt_; }
   long long OptimizerStep(int which) const { return which ? bias_step_ : weight_step_; }
+  void SetOptimizerStep(int which, long long step) { (which ? bias_step_ : weight_step_) = step; }
+  // floats of the weights and of the bias (0 under has_no_bias) in the edge's parameter slice, weights first
+  long long WeightCount() const { return (long long)num_output_channels_ * WeightCols(); }
+  long long BiasCount() const { return has_no_bias_ ? 0 : (long long)num_output_channels_ * BiasCols(); }
   void ReduceLearningRate(float factor) { weight_opt_.epsilon *= factor; bias_opt_.epsilon *= factor; }   // edge_with_weight.cc:90-93
   // the target of this step's bias gradient for the edge above (Plan().offers_bias_grad): ComputeOuter then skips its sum
   BiasGradTarget HandOffBiasGrad();

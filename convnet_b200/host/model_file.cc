@@ -16,6 +16,7 @@
 #include <set>
 #include <sstream>
 #include <stdexcept>
+#include <tuple>
 
 #include "convnet.h"
 
@@ -437,15 +438,28 @@ bool HasConvGeometry(EdgeType t) { return t == CONVOLUTIONAL || t == LOCAL || t 
 // ---------------------------------------------------------------- Msg -> ModelConfig
 class Mapper {
  public:
-  explicit Mapper(const std::string& path) : path_(path) {}
+  Mapper(const std::string& path, bool check_pretrained) : path_(path), check_pretrained_(check_pretrained) {}
 
   ModelConfig Map(const Msg& model) {
     ModelConfig m;
     m.name = model.Get("name")->s;
     m.seed = (unsigned)model.Int("seed", 0);
     RefuseMessage(model, "subnet", "subnets are not supported");
-    for (const char* f : {"polyak_after", "polyak_queue_size"})
-      if (model.Int(f, 0) > 0) Fail(*model.Get(f), "", std::string("field '") + f + "': Polyak averaging is not supported");
+    // Polyak averaging: a queue without an insertion period, or a period without a queue, averages nothing
+    m.polyak_after = (int)model.Int("polyak_after", 0);
+    m.polyak_queue_size = (int)model.Int("polyak_queue_size", 0);
+    for (int k = 0; k < 2; k++) {
+      const char *f = k ? "polyak_queue_size" : "polyak_after", *other = k ? "polyak_after" : "polyak_queue_size";
+      if (model.Int(f, 0) > 0 && model.Int(other, 0) <= 0)
+        Fail(*model.Get(f), "", std::string("field '") + f + "': Polyak averaging needs both polyak_after and "
+             "polyak_queue_size > 0, and " + other + " is not");
+    }
+    m.validate_after = (int)model.Int("validate_after", -1);
+    m.save_after = (int)model.Int("save_after", -1);
+    if (PolyakOn(m))                                       // the insertion rule (PolyakDue) divides by both
+      for (const char* f : {"validate_after", "save_after"})
+        if (model.Int(f, -1) == 0) Fail(*model.Get(f), "", std::string("field '") + f + "': 0 with Polyak averaging on "
+                                        "(its insertion rule takes the iteration modulo " + f + ")");
     def_w_ = model.Get("default_weight_optimizer");
     def_b_ = model.Get("default_bias_optimizer");
     for (const Entry* d : {def_w_, def_b_}) if (d) CheckOptimizer(*d, "");
@@ -510,6 +524,8 @@ class Mapper {
       e->SetImageSize(y, x, t);
       const std::string why = EdgeShapeError(*e, m.layer[k].num_channels, m.layer[k + 1].num_channels);
       if (!why.empty()) Fail(at, EdgeName(*at.msg), why);
+      if (check_pretrained_ && m.edge[k].initialization == PRETRAINED && !e->HasNoParameters())
+        CheckPretrained(*at.msg, *dynamic_cast<EdgeWithWeight*>(e.get()), m.edge[k]);
       y = e->GetNumModulesY(); x = e->GetNumModulesX(); t = e->GetNumModulesT();
     }
     return m;
@@ -517,7 +533,34 @@ class Mapper {
 
  private:
   const std::string path_;
+  const bool check_pretrained_;
   const Entry *def_w_ = nullptr, *def_b_ = nullptr;
+
+  // a PRETRAINED edge (shapes known): its checkpoint has the weight and bias records, with their optimizers' history and
+  // step, at this edge's sizes (EdgeWithWeight::LoadParameters, edge_with_weight.cc:41-58)
+  void CheckPretrained(const Msg& e, const EdgeWithWeight& w, const EdgeConfig& c) const {
+    const std::string where = EdgeName(e);
+    const Entry& file = *e.Get("pretrained_model");
+    std::unique_ptr<CheckpointFile> f;
+    try {
+      f.reset(new CheckpointFile(c.pretrained_model));
+    } catch (const std::invalid_argument& x) {
+      Fail(file, where, std::string("field 'pretrained_model': ") + x.what());
+    }
+    const Entry& field = e.Has("pretrained_edge_name") ? *e.Get("pretrained_edge_name") : file;
+    const std::string from = c.pretrained_edge_name.empty() ? c.name : c.pretrained_edge_name;
+    for (int which = 0; which < 2; which++) {
+      const long long n = which ? w.BiasCount() : w.WeightCount();
+      if (n == 0) continue;
+      const std::string prefix = from + (which ? ":bias" : ":weight");
+      for (const auto& [name, type, count] : {std::make_tuple(prefix, (int)CheckpointFile::FLOAT32, n),
+                                              std::make_tuple(prefix + "_gradient_history", (int)CheckpointFile::FLOAT32, n),
+                                              std::make_tuple(prefix + "_step", (int)CheckpointFile::INT64, 1LL)}) {
+        const std::string why = f->Check(name, type, count);
+        if (!why.empty()) Fail(field, where, "field '" + field.name + "': " + why);
+      }
+    }
+  }
 
   [[noreturn]] void Fail(int line, const std::string& what) const {
     throw std::invalid_argument(path_ + ":" + std::to_string(line) + ": " + what);
@@ -674,10 +717,16 @@ class Mapper {
                std::to_string(source.num_channels) + " channels is below one channel");
 
     const std::string init = e.Enum("initialization", "DENSE_GAUSSIAN_SQRT_FAN_IN");
-    if (init == "SPARSE_GAUSSIAN" || init == "PRETRAINED")
+    if (init == "SPARSE_GAUSSIAN")
       Fail(*e.Get("initialization"), where, "field 'initialization': " + init + " is not supported");
+    if (init == "PRETRAINED" && !e.Has("pretrained_model"))
+      Fail(*e.Get("initialization"), where, "field 'initialization': PRETRAINED needs pretrained_model (a checkpoint file)");
     const std::vector<std::string> inits = EnumValues("Initialization");
     c.initialization = (int)(std::find(inits.begin(), inits.end(), init) - inits.begin());
+    if (init == "PRETRAINED" && HasParameters(c.edge_type)) {   // the path as given, as in the reference
+      c.pretrained_model = e.Get("pretrained_model")->s;
+      if (e.Has("pretrained_edge_name")) c.pretrained_edge_name = e.Get("pretrained_edge_name")->s;
+    }
     c.init_wt = e.Float("init_wt", 1.f);
     c.init_bias = e.Float("init_bias", 0.f);
     c.grad_check = e.Bool("grad_check", false);
@@ -748,19 +797,28 @@ class Writer {
 
 }  // namespace
 
+ModelConfig ReadModelText(const std::string& text, const std::string& where, bool check_pretrained) {
+  const std::shared_ptr<Msg> model = Parser(where, text).ParseFile();
+  return Mapper(where, check_pretrained).Map(*model);
+}
 ModelConfig ReadModelFile(const std::string& path) {
   std::ifstream f(path, std::ios::binary);
   if (!f) throw std::invalid_argument("cannot open model file '" + path + "'");
   std::stringstream ss;
   ss << f.rdbuf();
-  const std::shared_ptr<Msg> model = Parser(path, ss.str()).ParseFile();
-  return Mapper(path).Map(*model);
+  return ReadModelText(ss.str(), path, true);
 }
 
 std::string ModelText(const ModelConfig& m) {
   Writer w;
   w.Line("name", Quote(m.name));
   w.Int("seed", m.seed);
+  if (PolyakOn(m)) {                                       // (without Polyak the two periods configure nothing here)
+    w.Int("polyak_after", m.polyak_after);
+    w.Int("polyak_queue_size", m.polyak_queue_size);
+    w.Int("validate_after", m.validate_after);
+    w.Int("save_after", m.save_after);
+  }
   for (const LayerConfig& l : m.layer) {
     w.Open("layer");
     w.Line("name", Quote(l.name));
@@ -816,6 +874,10 @@ std::string ModelText(const ModelConfig& m) {
       if (e.edge_type == CONVOLUTIONAL) w.Bool("shared_bias", e.shared_bias);
       w.Bool("has_no_bias", e.has_no_bias);
       w.Line("initialization", Writer::EnumName("Initialization", e.initialization));
+      if (e.initialization == PRETRAINED) {
+        w.Line("pretrained_model", Quote(e.pretrained_model));
+        w.Line("pretrained_edge_name", Quote(e.pretrained_edge_name.empty() ? e.source + ":" + e.dest : e.pretrained_edge_name));
+      }
       w.Flt("init_wt", e.init_wt);
       w.Flt("init_bias", e.init_bias);
       w.Flt("scale_gradients", e.scale_gradients);

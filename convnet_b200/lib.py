@@ -108,6 +108,7 @@ SIGNATURES = {
     "cnb_bn_stats": [FP, ct.c_longlong, I, F, F, FP, FP, FP, FP],
     "cnb_bn_apply": [FP, FP, ct.c_longlong, I, FP, FP, FP, FP, I],
     "cnb_bn_backward": [FP, FP, ct.c_longlong, I, FP, FP, FP, I, FP, FP],
+    "cnb_polyak_average": [FP, FP, ct.c_longlong, ct.c_longlong, I],
 }
 RESTYPES = {
     "convnet_b200_version": I, "convnet_b200_get_stream": ct.c_void_p,

@@ -93,6 +93,12 @@ def load_host():
                                         ct.POINTER(i)], i),
             "cnb_model_text": ([ct.c_char_p, ct.c_char_p, ll], ll),
             "cnb_model_initial_weights": ([ct.c_char_p, i, ct.c_uint, ct.POINTER(f), ll], ll),
+            "cnb_net_history": ([vp], vp), "cnb_last_error": ([], ct.c_char_p), "cnb_net_save": ([vp, ct.c_char_p], i),
+            "cnb_net_load": ([vp, ct.c_char_p], i), "cnb_net_iteration": ([vp], ll),
+            "cnb_net_polyak_insert": ([vp], i), "cnb_net_load_polyak_weights": ([vp], i),
+            "cnb_net_load_current_weights": ([vp], i), "cnb_net_polyak_count": ([vp], i),
+            "cnb_model_polyak": ([ct.c_char_p, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i)], i),
+            "cnb_polyak_due": ([ct.c_char_p, ll], i),
         }
         for name, (args, res) in sig.items():
             fn = getattr(H, name)
@@ -119,7 +125,16 @@ class Net:
     One output suffix at most: "+squared-error" (LINEAR output, SQUARED_ERROR), "+binary-ce" (LOGISTIC output,
     CROSS_ENTROPY_BINARY, metric CLASSIFICATION_BINARY), "+soft-targets" (SOFTMAX_DIST, CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED);
     such outputs train on targets_tensor() instead of labels_tensor().  "logcheck": the gradcheck net with logistic units.
-    A model that cannot be read or run raises ValueError; the reason (for a file: its line and field) is on stderr."""
+    A model that cannot be read or run raises ValueError; the reason (for a file: its line and field) is on stderr.
+
+    Checkpoints (the reference's ConvNet::Save / Load): save(path) writes the parameters, the optimizers' histories, step
+    counts and adaptive state, the batch-norm running statistics, the iteration, the seed and the optimizer settings in
+    force; load(path) into a net of the same model resumes training bit for bit, whatever seed the Net was built with.
+    A model file with polyak_after and polyak_queue_size averages the parameters over a queue on the device, as the
+    reference's Save() does beside each checkpoint:
+        if polyak_due(model, net.iteration): net.polyak_insert()          # after each train_step
+        net.save(p)
+        net.load_polyak_weights(); net.save(p + "polyak"); net.load_current_weights()"""
 
     def __init__(self, model, batch_size, seed=42, grad_checker=False):
         self.H = load_host()
@@ -178,6 +193,10 @@ class Net:
 
     def grads_tensor(self):
         return self._view(self.H.cnb_net_grads(self.h), self.num_params, "f")
+
+    def history_tensor(self):
+        """the optimizers' momentum history (gradient_history), laid out like params_tensor()"""
+        return self._view(self.H.cnb_net_history(self.h), self.num_params, "f")
 
     def adaptive_state_tensor(self):
         """the per-parameter state of the ADAGRAD_SGD / RMSPROP_SGD optimizers, laid out like params_tensor(); None while
@@ -289,6 +308,35 @@ class Net:
             out[key] = {"step": step.value, "epsilon": eps.value, "momentum": mom.value}
         return out
 
+    # --- checkpoints and Polyak averaging (ConvNet::Save / Load / InsertPolyak / LoadPolyakWeights / LoadCurrentWeights)
+    def _check(self, rc):
+        if rc != 0:
+            raise ValueError(self.H.cnb_last_error().decode())
+
+    def save(self, path):
+        """write the net's state to `path` (through path + "temp", fsynced and renamed), after every pending step"""
+        self._check(self.H.cnb_net_save(self.h, os.fsencode(path)))
+
+    def load(self, path):
+        """restore the state `save` wrote from a net of the same model: ValueError (naming the record) if the file does not
+        fit this net, which is then unchanged"""
+        self._check(self.H.cnb_net_load(self.h, os.fsencode(path)))
+
+    iteration = property(lambda s: s.H.cnb_net_iteration(s.h), doc="train_step calls so far (restored by load)")
+    polyak_count = property(lambda s: s.H.cnb_net_polyak_count(s.h), doc="filled slots of the Polyak queue")
+
+    def polyak_insert(self):
+        """copy the parameters into the next slot of the Polyak queue (a ring of polyak_queue_size slots)"""
+        self._check(self.H.cnb_net_polyak_insert(self.h))
+
+    def load_polyak_weights(self):
+        """keep the parameters aside and replace them with the average of the filled queue slots"""
+        self._check(self.H.cnb_net_load_polyak_weights(self.h))
+
+    def load_current_weights(self):
+        """restore the parameters load_polyak_weights kept aside"""
+        self._check(self.H.cnb_net_load_current_weights(self.h))
+
     def train_step(self, want_loss=True):
         if want_loss:
             v = ct.c_float(0)
@@ -396,7 +444,8 @@ def model_text(model):
 
 def model_initial_weights(model, edge, seed=42):
     """the initial weights (a list of floats, without the bias) of edge `edge` of a model under RNG seed `seed`
-    (host-only; the net seeds edge i with its seed + 17 i); None for an edge without parameters"""
+    (host-only; the net seeds edge i with its seed + 17 i), or a PRETRAINED edge's weights from its checkpoint; None for
+    an edge without parameters"""
     H = load_host()
     n = H.cnb_model_initial_weights(model.encode(), edge, seed, None, 0)
     if n == -1:
@@ -406,6 +455,24 @@ def model_initial_weights(model, edge, seed=42):
     buf = (ct.c_float * n)()
     H.cnb_model_initial_weights(model.encode(), edge, seed, buf, n)
     return list(buf)
+
+
+def model_polyak(model):
+    """a model's Polyak averaging (host-only): None when it is off, else {"polyak_after", "polyak_queue_size",
+    "validate_after", "save_after"}"""
+    v = [ct.c_int(0) for _ in range(4)]
+    rc = load_host().cnb_model_polyak(model.encode(), *[ct.byref(x) for x in v])
+    if rc < 0:
+        raise ValueError("cannot build model %r (see stderr)" % model)
+    return dict(zip(("polyak_after", "polyak_queue_size", "validate_after", "save_after"), (x.value for x in v))) if rc else None
+
+
+def polyak_due(model, iteration):
+    """whether the reference's training loop inserts into the Polyak queue after train_step number `iteration`"""
+    rc = load_host().cnb_polyak_due(model.encode(), iteration)
+    if rc < 0:
+        raise ValueError("cannot build model %r (see stderr)" % model)
+    return bool(rc)
 
 
 def model_param_layout(model, batch=1):

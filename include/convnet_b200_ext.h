@@ -276,6 +276,14 @@ void cnb_bn_apply(const float* x, float* y, long long n, int channels, const flo
 void cnb_bn_backward(float* deriv, const float* x, long long n, int channels, const float* gamma, const float* mu,
                      const float* sigma, int train, float* grad_gamma, float* grad_beta);
 
+/* ---- Polyak averaging (ConvNet::LoadPolyakWeights, the reference's loop at src/convnet.cc:715-723).  `queue` holds k
+ * slots of n floats, slot s at queue + s*slot_stride:
+ *   out[j] = (((0 + s_0[j]) + s_1[j]) + ... + s_{k-1}[j]) / (float)k
+ * summed in slot order, each addition from +0.0f and rounded to nearest (so -0.0 averages to +0.0, as in the reference).
+ * `out` must not overlap the queue.  k >= 1.  Honours convnet_b200_emit_bf16_next for out; every other staged copy that
+ * overlaps out (the weights' bf16 twins, the dgrad filter banks) is dropped.  Runs on the library's stream. */
+void cnb_polyak_average(float* out, const float* queue, long long n, long long slot_stride, int k);
+
 /* ---- input pipeline, device side (SURVEY.md §8 f4) -------------------------------------------------------------------
  * The reference keeps a chunk of the data set on the GPU, one image per COLUMN (pixel index = col + W*(row + H*color)),
  * and cuts every minibatch out of it with a random crop and mirror per image while transposing it into the image-fastest

@@ -80,29 +80,31 @@ API void cnb_net_bprop(void* p) { ((NetHandle*)p)->net->ComputeDeriv(); ((NetHan
 API void cnb_net_update(void* p) { ((NetHandle*)p)->net->UpdateWeights(); }
 API void cnb_net_reduce_learning_rate(void* p, float factor) { ((NetHandle*)p)->net->ReduceLearningRate(factor); }
 
-// ---- optimizer settings (edge.h OptimizerConfig: proto Optimizer, SGD fields).  which: 0 the weights, 1 the bias.
-static EdgeWithWeight* WeightedEdge(void* p, int edge) {
-  auto& e = ((NetHandle*)p)->net->Edges();
-  return edge >= 0 && edge < (int)e.size() ? dynamic_cast<EdgeWithWeight*>(e[edge].get()) : nullptr;
+// ---- optimizer settings (edge.h OptimizerConfig: proto Optimizer, SGD fields) of one trained tensor, named as its
+// checkpoint records: "<edge>:weight", "<edge>:bias", "<layer>:gamma", "<layer>:beta" (ConvNet::Tensors)
+static TrainedTensor* Tensor(void* p, const char* name) {
+  for (TrainedTensor& t : ((NetHandle*)p)->net->Tensors())
+    if (t.name == name) return &t;
+  return nullptr;
 }
-// replaces the settings of one optimizer (its step count and momentum history stay).  0 ok, -1 no such weighted edge,
-// -2 a config the SGD path cannot run (see OptimizerConfigError, printed on stderr)
-API int cnb_net_set_optimizer(void* p, int edge, int which, const OptimizerConfig* c) {
-  EdgeWithWeight* e = WeightedEdge(p, edge);
-  if (!e || which < 0 || which > 1) return -1;
-  if (const char* err = OptimizerConfigError(*c)) { fprintf(stderr, "convnet_b200 host: %s\n", err); return -2; }
-  ((NetHandle*)p)->net->SetOptimizer(e, which, *c);
+// replaces the settings of one optimizer (its step count and momentum history stay).  0 ok, -1 no such tensor, -2 a
+// config this tensor cannot train with (OptimizerConfigError; BnOptimizerConfigError for gamma / beta; on stderr)
+API int cnb_net_set_optimizer(void* p, const char* tensor, const OptimizerConfig* c) {
+  TrainedTensor* t = Tensor(p, tensor);
+  if (!t) return -1;
+  if (const char* err = t->ConfigError(*c)) { fprintf(stderr, "convnet_b200 host: %s\n", err); return -2; }
+  ((NetHandle*)p)->net->SetOptimizer(*t, *c);
   return 0;
 }
 // the adaptive optimizer state (cnb_net_num_params floats, carved like the parameters); NULL while no optimizer of the
 // net is ADAGRAD_SGD or RMSPROP_SGD
 API float* cnb_net_adaptive_state(void* p) { return ((NetHandle*)p)->net->AdaptiveState(); }
-// the step count of one optimizer and the (epsilon, momentum) its next update uses.  0 ok, -1 no such weighted edge
-API int cnb_net_get_optimizer_state(void* p, int edge, int which, long long* step, float* epsilon, float* momentum) {
-  EdgeWithWeight* e = WeightedEdge(p, edge);
-  if (!e || which < 0 || which > 1) return -1;
-  *step = e->OptimizerStep(which);
-  OptimizerSchedule(e->Optimizer(which), *step, epsilon, momentum);
+// the step count of one optimizer and the (epsilon, momentum) its next update uses.  0 ok, -1 no such tensor
+API int cnb_net_get_optimizer_state(void* p, const char* tensor, long long* step, float* epsilon, float* momentum) {
+  const TrainedTensor* t = Tensor(p, tensor);
+  if (!t) return -1;
+  *step = t->step;
+  OptimizerSchedule(t->opt, *step, epsilon, momentum);
   return 0;
 }
 // pure host logic: (epsilon, momentum) of the update after `step` earlier ones.  0 ok, -2 invalid config
@@ -126,22 +128,6 @@ API long long cnb_net_bn_offset(void* p, int layer) { return BnLayer(p, layer) ?
 API float* cnb_net_bn_stat(void* p, int layer, int which) {
   Layer* l = BnLayer(p, layer);
   return l && which >= 0 && which < 4 ? l->BnStat(which) : nullptr;
-}
-// replaces the settings of the gamma or beta optimizer (its step count and momentum history stay).  0 ok, -1 not a
-// batch-normalised layer, -2 a config gamma / beta cannot train with (BnOptimizerConfigError, printed on stderr)
-API int cnb_net_set_bn_optimizer(void* p, int layer, int which, const OptimizerConfig* c) {
-  Layer* l = BnLayer(p, layer);
-  if (!l || which < 0 || which > 1) return -1;
-  if (const char* err = BnOptimizerConfigError(*c)) { fprintf(stderr, "convnet_b200 host: %s\n", err); return -2; }
-  ((NetHandle*)p)->net->SetBnOptimizer(l, which, *c);
-  return 0;
-}
-API int cnb_net_get_bn_optimizer_state(void* p, int layer, int which, long long* step, float* epsilon, float* momentum) {
-  Layer* l = BnLayer(p, layer);
-  if (!l || which < 0 || which > 1) return -1;
-  *step = l->BnOptimizerStep(which);
-  OptimizerSchedule(l->BnOptimizer(which), *step, epsilon, momentum);
-  return 0;
 }
 // pure host logic: 0 if `c` can train gamma / beta, -2 if not (the reason on stderr)
 API int cnb_bn_optimizer_check(const OptimizerConfig* c) {

@@ -139,31 +139,22 @@ std::vector<char> CheckpointFile::Read(const std::string& name) const {
 }
 
 // ---------------------------------------------------------------- what a net writes and reads
-std::vector<CheckpointEntry> ConvNet::CheckpointEntries(const ModelConfig& opt) {
+std::vector<CheckpointEntry> ConvNet::CheckpointEntries(const std::vector<OptimizerConfig>& opt) {
   std::vector<CheckpointEntry> out;
-  // a tensor and its optimizer's records (SGDOptimizer / AdagradSGDOptimizer / RMSPropSGDOptimizer ::SaveParameters)
-  auto tensor = [&](const std::string& prefix, size_t off, long long n, const OptimizerConfig& o, EdgeWithWeight* e, Layer* l,
-                    int which) {
-    out.push_back({prefix, CheckpointEntry::PARAMS, off, n, nullptr, nullptr, 0});
-    out.push_back({prefix + "_gradient_history", CheckpointEntry::HISTORY, off, n, nullptr, nullptr, 0});
-    out.push_back({prefix + "_step", CheckpointEntry::STEP, 0, 1, e, l, which});
-    if (const char* s = AdaptiveSuffix(o)) out.push_back({prefix + s, CheckpointEntry::STATE, off, n, nullptr, nullptr, 0});
-  };
-  for (size_t i = 0; i < edges_.size(); i++) {
-    EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i].get());
-    if (w && edge_size_[i] > 0) {
-      tensor(w->GetName() + ":weight", edge_offset_[i], w->WeightCount(), opt.edge[i].weight_optimizer, w, nullptr, 0);
-      if (w->BiasCount() > 0)
-        tensor(w->GetName() + ":bias", edge_offset_[i] + (size_t)w->WeightCount(), w->BiasCount(), opt.edge[i].bias_optimizer,
-               w, nullptr, 1);
+  for (size_t k = 0; k < tensors_.size(); k++) {
+    const TrainedTensor& t = tensors_[k];
+    // a tensor and its optimizer's records (SGDOptimizer / AdagradSGDOptimizer / RMSPropSGDOptimizer ::SaveParameters)
+    if (t.n > 0) {
+      out.push_back({t.name, CheckpointEntry::PARAMS, t.offset, t.n, k, nullptr});
+      out.push_back({t.name + "_gradient_history", CheckpointEntry::HISTORY, t.offset, t.n, k, nullptr});
+      out.push_back({t.name + "_step", CheckpointEntry::STEP, 0, 1, k, nullptr});
+      if (const char* s = AdaptiveSuffix(opt[k])) out.push_back({t.name + s, CheckpointEntry::STATE, t.offset, t.n, k, nullptr});
     }
-    Layer* l = layers_[i + 1].get();
-    if (bn_offset_[i + 1] < 0) continue;
-    const size_t off = (size_t)bn_offset_[i + 1], C = (size_t)l->GetNumChannels();
-    tensor(l->GetName() + ":gamma", off, (long long)C, opt.layer[i + 1].gamma_optimizer, nullptr, l, 0);
-    tensor(l->GetName() + ":beta", off + C, (long long)C, opt.layer[i + 1].beta_optimizer, nullptr, l, 1);
-    out.push_back({l->GetName() + ":running_mean", CheckpointEntry::RUNNING, 0, (long long)C, nullptr, l, 0});
-    out.push_back({l->GetName() + ":running_sigma", CheckpointEntry::RUNNING, 0, (long long)C, nullptr, l, 1});
+    if (t.kind == TrainedTensor::BETA) {               // the layer's running statistics follow its gamma and beta
+      Layer* l = layers_[t.edge + 1].get();
+      out.push_back({l->GetName() + ":running_mean", CheckpointEntry::RUNNING, 0, t.n, k, l->BnStat(0)});
+      out.push_back({l->GetName() + ":running_sigma", CheckpointEntry::RUNNING, 0, t.n, k, l->BnStat(1)});
+    }
   }
   return out;
 }
@@ -173,24 +164,14 @@ float* ConvNet::EntryData(const CheckpointEntry& e) {
     case CheckpointEntry::PARAMS: return parameters_.GetDevData() + e.offset;
     case CheckpointEntry::HISTORY: return history_.GetDevData() + e.offset;
     case CheckpointEntry::STATE: return AdaptiveState() + e.offset;
-    case CheckpointEntry::RUNNING: return e.layer->BnStat(e.which);
+    case CheckpointEntry::RUNNING: return e.running;
     default: return nullptr;
   }
 }
 
 ModelConfig ConvNet::CurrentModel() const {
   ModelConfig m = model_;
-  for (size_t i = 0; i < edges_.size(); i++) {
-    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i].get())) {
-      m.edge[i].weight_optimizer = w->Optimizer(0);
-      m.edge[i].bias_optimizer = w->Optimizer(1);
-    }
-  }
-  for (size_t i = 0; i < layers_.size(); i++)
-    if (layers_[i]->BatchNormalize()) {
-      m.layer[i].gamma_optimizer = layers_[i]->BnOptimizer(0);
-      m.layer[i].beta_optimizer = layers_[i]->BnOptimizer(1);
-    }
+  for (const TrainedTensor& t : tensors_) ModelOptimizer(m, t) = t.opt;
   return m;
 }
 
@@ -220,9 +201,11 @@ void ConvNet::Save(const std::string& path) {
     w.Text("__model__", ModelText(m));
     w.Int("__current_iter__", (long long)step_);
     w.Int("__seed__", (long long)model_.seed);
-    for (const CheckpointEntry& e : CheckpointEntries(m)) {
+    std::vector<OptimizerConfig> opt;
+    for (const TrainedTensor& t : tensors_) opt.push_back(t.opt);
+    for (const CheckpointEntry& e : CheckpointEntries(opt)) {
       if (e.buffer == CheckpointEntry::STEP)
-        w.Int(e.name, e.edge ? e.edge->OptimizerStep(e.which) : e.layer->BnOptimizerStep(e.which));
+        w.Int(e.name, tensors_[e.tensor].step);
       else
         w.Floats(e.name, EntryData(e), e.n);
     }
@@ -279,7 +262,9 @@ void ConvNet::Load(const std::string& path) {
       }
     if (!found && unmatched.empty()) unmatched = "has no batch-normalised layer '" + layers_[i]->GetName() + "'";
   }
-  const std::vector<CheckpointEntry> entries = CheckpointEntries(opt);
+  std::vector<OptimizerConfig> configs;
+  for (const TrainedTensor& t : tensors_) configs.push_back(ModelOptimizer(opt, t));
+  const std::vector<CheckpointEntry> entries = CheckpointEntries(configs);
   std::set<std::string> known = {"__model__", "__current_iter__", "__seed__"};
   for (const CheckpointEntry& e : entries) {
     const bool step = e.buffer == CheckpointEntry::STEP;
@@ -299,24 +284,12 @@ void ConvNet::Load(const std::string& path) {
   // 2. nothing runs on any stream any more
   WaitAllStreams();
   // 3. the optimizer settings (these allocate the adaptive state if the file's optimizers need it)
-  for (size_t i = 0; i < edges_.size(); i++)
-    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i].get())) {
-      SetOptimizer(w, 0, opt.edge[i].weight_optimizer);
-      SetOptimizer(w, 1, opt.edge[i].bias_optimizer);
-    }
-  for (size_t i = 0; i < layers_.size(); i++)
-    if (layers_[i]->BatchNormalize()) {
-      SetBnOptimizer(layers_[i].get(), 0, opt.layer[i].gamma_optimizer);
-      SetBnOptimizer(layers_[i].get(), 1, opt.layer[i].beta_optimizer);
-    }
+  for (size_t k = 0; k < tensors_.size(); k++) SetOptimizer(tensors_[k], configs[k]);
   // 4. every tensor, step count, the iteration and the seed
   for (size_t k = 0; k < entries.size(); k++) {
     const CheckpointEntry& e = entries[k];
     if (e.buffer == CheckpointEntry::STEP) {
-      long long s = 0;
-      memcpy(&s, data[k].data(), 8);
-      if (e.edge) e.edge->SetOptimizerStep(e.which, s);
-      else e.layer->SetBnOptimizerStep(e.which, s);
+      memcpy(&tensors_[e.tensor].step, data[k].data(), 8);
     } else if (e.n) {
       CKPT_CUDA_CHECK(cudaMemcpyAsync(EntryData(e), data[k].data(), sizeof(float) * (size_t)e.n, cudaMemcpyHostToDevice,
                                       Matrix::Stream()));
@@ -332,33 +305,29 @@ void ConvNet::Load(const std::string& path) {
 }
 
 void ConvNet::LoadPretrained(size_t i) {
-  EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i].get());
   const EdgeConfig& c = model_.edge[i];
-  const std::string from = c.pretrained_edge_name.empty() ? w->GetName() : c.pretrained_edge_name;
+  const std::string& edge = edges_[i]->GetName();
+  const std::string from = c.pretrained_edge_name.empty() ? edge : c.pretrained_edge_name;
   const CheckpointFile f(c.pretrained_model);
-  for (int which = 0; which < 2; which++) {
-    const long long n = which ? w->BiasCount() : w->WeightCount();
-    if (n == 0) continue;
-    const std::string prefix = from + (which ? ":bias" : ":weight");
-    const size_t off = edge_offset_[i] + (which ? (size_t)w->WeightCount() : 0);
-    const char* adaptive = AdaptiveSuffix(w->Optimizer(which));
-    std::vector<std::pair<std::string, float*>> tensors = {{prefix, parameters_.GetDevData() + off},
-                                                          {prefix + "_gradient_history", history_.GetDevData() + off}};
+  for (TrainedTensor& t : tensors_) {
+    if (t.edge != (int)i || !t.OnEdge() || t.n == 0) continue;
+    const std::string prefix = from + t.name.substr(edge.size());            // <from>:weight, <from>:bias
+    const char* adaptive = AdaptiveSuffix(t.opt);
+    std::vector<std::pair<std::string, float*>> tensors = {{prefix, parameters_.GetDevData() + t.offset},
+                                                          {prefix + "_gradient_history", history_.GetDevData() + t.offset}};
     // the adaptive state where the file has it for this edge's kind of optimizer; otherwise the fresh start stays
-    if (adaptive && f.Has(prefix + adaptive)) tensors.push_back({prefix + adaptive, AdaptiveState() + off});
+    if (adaptive && f.Has(prefix + adaptive)) tensors.push_back({prefix + adaptive, AdaptiveState() + t.offset});
     for (const auto& [name, dev] : tensors) {
-      const std::string why = f.Check(name, CheckpointFile::FLOAT32, n);
-      if (!why.empty()) throw std::invalid_argument("edge '" + w->GetName() + "' (PRETRAINED): " + why);
+      const std::string why = f.Check(name, CheckpointFile::FLOAT32, t.n);
+      if (!why.empty()) throw std::invalid_argument("edge '" + edge + "' (PRETRAINED): " + why);
     }
     const std::string why = f.Check(prefix + "_step", CheckpointFile::INT64, 1);
-    if (!why.empty()) throw std::invalid_argument("edge '" + w->GetName() + "' (PRETRAINED): " + why);
+    if (!why.empty()) throw std::invalid_argument("edge '" + edge + "' (PRETRAINED): " + why);
     for (const auto& [name, dev] : tensors) {
       const std::vector<char> h = f.Read(name);
       CKPT_CUDA_CHECK(cudaMemcpy(dev, h.data(), h.size(), cudaMemcpyHostToDevice));
     }
-    long long step = 0;
-    memcpy(&step, f.Read(prefix + "_step").data(), 8);
-    w->SetOptimizerStep(which, step);
+    memcpy(&t.step, f.Read(prefix + "_step").data(), 8);
   }
 }
 

@@ -95,17 +95,37 @@ class CheckpointFile {
 // the weights a PRETRAINED edge `c` of `n` weights takes from its checkpoint (record <pretrained_edge_name>:weight)
 std::vector<float> PretrainedWeights(const EdgeConfig& c, long long n);
 
-// one record of a net's checkpoint: a float32 tensor at `offset` of the parameters, the momentum history, the adaptive
-// state or (RUNNING) the layer's running statistic `which`, or (STEP) the step count of optimizer `which` of `edge` / `layer`
+// One trained tensor of a net, with its optimizer: an edge's weights or bias, or a batch-normalised layer's gamma or beta
+// (ConvNet::PlanParameters, in flat-buffer order).  The bias of a has_no_bias edge keeps a record of zero floats, so that
+// its optimizer can still be read and set; updates and checkpoints skip it.
+struct TrainedTensor {
+  enum Kind { WEIGHTS, BIAS, GAMMA, BETA };
+  Kind kind;
+  std::string name;        // the checkpoint record prefix: <edge>:weight, <edge>:bias, <layer>:gamma, <layer>:beta
+  int edge;                // the edge whose bucket carries it (for gamma / beta: the edge that writes the layer)
+  size_t offset;           // into the flat parameter, gradient, history and adaptive state buffers
+  long long n;             // floats
+  int rows;                // norm groups: the output units of the weights; one for the others
+  OptimizerConfig opt;     // the settings in force
+  long long step = 0;      // updates counted so far, the reference's per-optimizer step_ (optimizer.cc:199)
+  // ReduceLearningRate scales the edges' tensors only: gamma / beta keep their rate, as in the reference
+  bool OnEdge() const { return kind == WEIGHTS || kind == BIAS; }
+  // nullptr if `c` can train this tensor, else why not
+  const char* ConfigError(const OptimizerConfig& c) const { return OnEdge() ? OptimizerConfigError(c) : BnOptimizerConfigError(c); }
+};
+// the optimizer block of `m` that configures `t`
+OptimizerConfig& ModelOptimizer(ModelConfig& m, const TrainedTensor& t);
+
+// one record of a net's checkpoint: a float32 tensor at `offset` of the parameters, the momentum history or the adaptive
+// state, a layer's running statistic (RUNNING, at `running`), or (STEP) the step count of trained tensor `tensor`
 struct CheckpointEntry {
   enum Buffer { PARAMS, HISTORY, STATE, RUNNING, STEP };
   std::string name;
   Buffer buffer;
   size_t offset;
   long long n;
-  EdgeWithWeight* edge;
-  Layer* layer;
-  int which;
+  size_t tensor;
+  float* running;
 };
 
 class Layer {                                   // src/layer.{h,cc}, reduced to state/deriv + activation
@@ -151,17 +171,11 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   // backward pass reads x, not the state: the state has been through the ReLU and the dropout.
   bool BatchNormalize() const { return config_.batch_normalize; }
   Matrix& GetPreBN() { return pre_bn_; }
-  // gamma | beta: 2 * channels floats of the flat parameter, gradient and history buffers (ConvNet::PlanParameters)
-  void SetBnMemory(Matrix& params, Matrix& grads, Matrix& hist);
-  void SetBnStateMemory(Matrix& state);                         // [gamma | beta] of the adaptive optimizer state
-  void InitBnState(int which);                                  // gamma's (0) or beta's (1) state back to its optimizer's start
+  // gamma | beta: 2 * channels floats of the flat parameter and gradient buffers (ConvNet::PlanParameters)
+  void SetBnMemory(Matrix& params, Matrix& grads);
   void InitializeBn();                                          // gamma = 1, beta = 0, mu = 0, sigma = 1 (layer.cc:271-278)
   void ApplyBatchNormalization(bool train, bool emit_bf16);     // activation included (its own pass is switched off)
   void ApplyDerivativeofBatchNormalization(bool emit_bf16);     // of the transform the last ApplyBatchNormalization applied
-  void AppendBnSgdTensors(std::vector<CnbOptTensorEx>& out);    // gamma and beta; advances both step counts
-  OptimizerConfig& BnOptimizer(int which) { return which ? config_.beta_optimizer : config_.gamma_optimizer; }   // 0 gamma, 1 beta
-  long long BnOptimizerStep(int which) const { return which ? beta_step_ : gamma_step_; }
-  void SetBnOptimizerStep(int which, long long step) { (which ? beta_step_ : gamma_step_) = step; }
   // device vectors of `channels` floats: 0 running mean, 1 running sigma, 2 batch mean, 3 batch sigma
   float* BnStat(int which) { return bn_stats_.GetDevData() + (size_t)which * config_.num_channels; }
   long long BnPixels() const { return (long long)image_size_y_ * image_size_x_; }
@@ -170,9 +184,8 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   LayerConfig config_;
   int image_size_y_, image_size_x_, image_size_t_;
   Matrix state_, deriv_, loss_per_image_, metric_per_image_, targets_, dropout_mask_;
-  Matrix pre_bn_, bn_stats_, gamma_, beta_, grad_gamma_, grad_beta_, hist_gamma_, hist_beta_, state_gamma_, state_beta_;
+  Matrix pre_bn_, bn_stats_, gamma_, beta_, grad_gamma_, grad_beta_;
   bool bn_train_ = false;                       // the last ApplyBatchNormalization used the batch statistics
-  long long gamma_step_ = 0, beta_step_ = 0;
   int* labels_ = nullptr;
   bool activation_fused_ = false, deriv_fused_ = false;
 };
@@ -213,21 +226,21 @@ class ConvNet {
   ConvNet(const ModelConfig& model, int batch_size);            // std::invalid_argument: a model this class cannot run
   virtual ~ConvNet();
   // the layout of the flat parameter buffer (host only): each edge's slice padded to 128 floats, followed by the
-  // [gamma | beta] slice, also padded, of the layer the edge writes when that layer is batch-normalised
+  // [gamma | beta] slice, also padded, of the layer the edge writes when that layer is batch-normalised; and the table of
+  // trained tensors in that order, each with the optimizer the model gives it
   void PlanParameters();
   void AllocateMemory();                                        // convnet.cc:272-298: ONE flat parameter / gradient buffer
   virtual void Fprop(bool train);                               // convnet.cc:377-388
   virtual void Bprop();                                         // convnet.cc:390-405
   virtual void UpdateWeights();                                 // convnet.cc:440-450
   void ReduceLearningRate(float factor);                        // base epsilon of every weight and bias optimizer *= factor
-  // replace the settings of an edge's weight (which = 0) / bias (1) optimizer, or of a batch-normalised layer's gamma (0) /
-  // beta (1) optimizer; the step count and momentum history stay.  An adaptive optimizer allocates the net's state buffer
-  // if it has none, and the tensor's state restarts (adagrad_delta or 1) when optimizer_type or adagrad_delta changes.
-  // The caller has validated `c` (OptimizerConfigError / BnOptimizerConfigError) and the indices
-  void SetOptimizer(EdgeWithWeight* e, int which, const OptimizerConfig& c);
-  void SetBnOptimizer(Layer* l, int which, const OptimizerConfig& c);
-  // the adaptive optimizer state: one float per parameter, carved like the history (edge slices, then [gamma | beta]);
-  // nullptr until some optimizer of the net is ADAGRAD_SGD or RMSPROP_SGD
+  std::vector<TrainedTensor>& Tensors() { return tensors_; }
+  // replace the settings of one trained tensor's optimizer; the step count and momentum history stay.  An adaptive
+  // optimizer allocates the net's state buffer if it has none, and the tensor's state restarts (adagrad_delta or 1) when
+  // optimizer_type or adagrad_delta changes.  The caller has validated `c` (TrainedTensor::ConfigError)
+  void SetOptimizer(TrainedTensor& t, const OptimizerConfig& c);
+  // the adaptive optimizer state: one float per parameter, laid out like the parameters; nullptr until some optimizer of
+  // the net is ADAGRAD_SGD or RMSPROP_SGD
   float* AdaptiveState() { return state_.GetDevData(); }
   void ComputeDeriv();
   void TrainOneBatch(float* loss_out);                          // convnet.cc:475-485
@@ -285,7 +298,9 @@ class ConvNet {
   void PlanFusion();
   bool prestage_ = true;                        // rebuild the dgrad banks behind each optimizer step (PrestageDown)
   Matrix parameters_, grad_parameters_, history_, loss_sum_, state_;
-  void AllocateAdaptiveState();                 // state_ and its slices, each initialised for its optimizer
+  std::vector<TrainedTensor> tensors_;
+  void AllocateAdaptiveState();                 // state_, each tensor's slice initialised for its optimizer
+  void InitState(const TrainedTensor& t);       // t's slice of state_ back to its optimizer's start
   std::vector<size_t> edge_offset_, edge_size_;
   std::vector<size_t> edge_span_;               // edge slice + the [gamma | beta] slice of its destination, both padded
   std::vector<long long> bn_offset_;
@@ -294,6 +309,9 @@ class ConvNet {
   // enqueued on side_, and once the bucket's edges have finished their dgrad the multi-tensor SGD step of that bucket
   // follows on the same stream — the exchange and the update of the FC layers hide under the conv back-propagation.
   void IssueBucketUpdate(const Bucket& b);
+  // the update of every trained tensor that edges [first, last] carry, in table order (AppendOptTensor: advances the step
+  // counts); the weighted edges among them start counting gradients again
+  void AppendUpdates(int first, int last, std::vector<CnbOptTensorEx>& out);
   // layers_[i] is a ReLU or logistic layer with dropout whose derivative is written by a dgrad that applies
   // act'(state) * 1/(1-p) itself: the backward pass needs no mask tensor, and the forward pass may fuse the dropout into
   // the edge below
@@ -321,7 +339,8 @@ class ConvNet {
   bool salted_ = false;                                          // SetDataParallel has set dropout_salt_ (SaltDropout)
   void SaltDropout();
   // checkpoint.cc
-  std::vector<CheckpointEntry> CheckpointEntries(const ModelConfig& optimizers);   // in params order
+  // in params order; opt[k]: the optimizer of tensors_[k] (which adaptive record it has)
+  std::vector<CheckpointEntry> CheckpointEntries(const std::vector<OptimizerConfig>& opt);
   float* EntryData(const CheckpointEntry& e);
   void LoadPretrained(size_t edge);                             // a PRETRAINED edge's records, after AllocateAdaptiveState
   void WaitAllStreams();                                        // host waits for the main, side, comm and optimizer streams

@@ -73,16 +73,14 @@ def load_host():
             "cnb_plan_buckets": ([i, ct.POINTER(ll), ct.POINTER(ll), ll, i, ct.POINTER(ll), ct.POINTER(ll), ct.POINTER(i)], i),
             "cnb_model_edge_params": ([ct.c_char_p, i, i, ct.POINTER(ll)], i),
             "cnb_net_reduce_learning_rate": ([vp, f], None),
-            "cnb_net_set_optimizer": ([vp, i, i, ct.POINTER(OptimizerConfig)], i),
+            "cnb_net_set_optimizer": ([vp, ct.c_char_p, ct.POINTER(OptimizerConfig)], i),
             "cnb_net_adaptive_state": ([vp], vp),
-            "cnb_net_get_optimizer_state": ([vp, i, i, ct.POINTER(ll), ct.POINTER(f), ct.POINTER(f)], i),
+            "cnb_net_get_optimizer_state": ([vp, ct.c_char_p, ct.POINTER(ll), ct.POINTER(f), ct.POINTER(f)], i),
             "cnb_optimizer_schedule": ([ct.POINTER(OptimizerConfig), ll, ct.POINTER(f), ct.POINTER(f)], i),
             "cnb_model_edge_optimizer": ([ct.c_char_p, i, i, ct.POINTER(OptimizerConfig)], i),
             "cnb_net_grad_check": ([vp, ct.c_uint, i, ct.c_char_p, ct.POINTER(f), ct.POINTER(f), ct.POINTER(f)], i),
             "cnb_net_layer_name": ([vp, i], ct.c_char_p), "cnb_net_layer_channels": ([vp, i], i),
             "cnb_net_bn_offset": ([vp, i], ll), "cnb_net_bn_stat": ([vp, i, i], vp),
-            "cnb_net_set_bn_optimizer": ([vp, i, i, ct.POINTER(OptimizerConfig)], i),
-            "cnb_net_get_bn_optimizer_state": ([vp, i, i, ct.POINTER(ll), ct.POINTER(f), ct.POINTER(f)], i),
             "cnb_bn_optimizer_check": ([ct.POINTER(OptimizerConfig)], i),
             "cnb_model_param_layout": ([ct.c_char_p, i, i, ct.POINTER(ll), ct.POINTER(ll), ct.POINTER(ll)], i),
             "cnb_model_fusion": ([ct.c_char_p, i, i, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i)], i),
@@ -226,36 +224,45 @@ class Net:
         CLASSIFICATION_MULTINOMIAL, the per-image share of correct features for CLASSIFICATION_BINARY, or a loss"""
         return self.H.cnb_net_metric(self.h)
 
-    # --- optimizer (SGDOptimizer, src/optimizer.cc): one for the weights and one for the bias of every weighted edge
-    def _edge_index(self, edge):
+    # --- optimizer (SGDOptimizer, src/optimizer.cc): one per trained tensor, named "<edge>:weight", "<edge>:bias",
+    # "<layer>:gamma", "<layer>:beta" as in checkpoints
+    def _set_optimizer(self, tensor, d):
+        """0, -1 (no such tensor) or -2 (config refused, the reason on stderr)"""
+        return self.H.cnb_net_set_optimizer(self.h, tensor.encode(), ct.byref(OptimizerConfig.from_dict(d)))
+
+    def _optimizer_state(self, tensor):
+        step, eps, mom = ct.c_longlong(0), ct.c_float(0), ct.c_float(0)
+        rc = self.H.cnb_net_get_optimizer_state(self.h, tensor.encode(), ct.byref(step), ct.byref(eps), ct.byref(mom))
+        return {"step": step.value, "epsilon": eps.value, "momentum": mom.value} if rc == 0 else None
+
+    def _edge_name(self, edge):
+        """the name of `edge` (index or name); "" for an index out of range, whose tensors the host then does not find"""
+        names = [e[0] for e in self.edges()]
         if isinstance(edge, str):
-            names = [e[0] for e in self.edges()]
             if edge not in names:
                 raise KeyError("no edge %r (edges: %s)" % (edge, ", ".join(names)))
-            return names.index(edge)
-        return int(edge)
+            return edge
+        return names[int(edge)] if 0 <= int(edge) < len(names) else ""
 
     def set_optimizer(self, edge, weights=None, bias=None):
         """replace the settings of the weight and / or bias optimizer of `edge` (index or name) with the optimizer block
         `weights` / `bias` (dicts of proto field names, unset fields at the proto's defaults).  Step counts and momentum
         histories are kept."""
-        i = self._edge_index(edge)
-        for which, d in ((0, weights), (1, bias)):
+        name = self._edge_name(edge)
+        for key, kind, d in (("weights", ":weight", weights), ("bias", ":bias", bias)):
             if d is None:
                 continue
-            rc = self.H.cnb_net_set_optimizer(self.h, i, which, ct.byref(OptimizerConfig.from_dict(d)))
+            rc = self._set_optimizer(name + kind, d)
             if rc != 0:
-                raise ValueError("set_optimizer(%r, %s): %s" % (edge, ("weights", "bias")[which],
-                                 "no such weighted edge" if rc == -1 else "config not supported (see stderr)"))
+                raise ValueError("set_optimizer(%r, %s): %s" % (edge, key, "no such weighted edge" if rc == -1
+                                                                else "config not supported (see stderr)"))
 
     def optimizer_state(self, edge):
         """{"weights": {...}, "bias": {...}}: updates counted so far ("step") and the epsilon / momentum of the next one"""
-        i, out = self._edge_index(edge), {}
-        for which, key in ((0, "weights"), (1, "bias")):
-            step, eps, mom = ct.c_longlong(0), ct.c_float(0), ct.c_float(0)
-            if self.H.cnb_net_get_optimizer_state(self.h, i, which, ct.byref(step), ct.byref(eps), ct.byref(mom)) != 0:
-                raise ValueError("edge %r has no parameters" % (edge,))
-            out[key] = {"step": step.value, "epsilon": eps.value, "momentum": mom.value}
+        name = self._edge_name(edge)
+        out = {"weights": self._optimizer_state(name + ":weight"), "bias": self._optimizer_state(name + ":bias")}
+        if out["weights"] is None:
+            raise ValueError("edge %r has no parameters" % (edge,))
         return out
 
     def reduce_learning_rate(self, factor):
@@ -292,21 +299,15 @@ class Net:
     def set_bn_optimizer(self, layer, gamma=None, beta=None):
         """replace the settings of the gamma and / or beta optimizer of a batch-normalised layer (optimizer blocks as for
         set_optimizer; norm rules are refused).  Step counts and momentum histories are kept."""
-        i = self._bn_layer(layer)[0]
-        for which, d in ((0, gamma), (1, beta)):
-            if d is None:
-                continue
-            if self.H.cnb_net_set_bn_optimizer(self.h, i, which, ct.byref(OptimizerConfig.from_dict(d))) != 0:
-                raise ValueError("set_bn_optimizer(%r, %s): config not supported (see stderr)" % (layer, ("gamma", "beta")[which]))
+        name = self._bn_layer(layer)[1]
+        for key, d in (("gamma", gamma), ("beta", beta)):
+            if d is not None and self._set_optimizer(name + ":" + key, d) != 0:
+                raise ValueError("set_bn_optimizer(%r, %s): config not supported (see stderr)" % (layer, key))
 
     def bn_optimizer_state(self, layer):
         """{"gamma": {...}, "beta": {...}}: updates counted so far ("step") and the epsilon / momentum of the next one"""
-        i, out = self._bn_layer(layer)[0], {}
-        for which, key in ((0, "gamma"), (1, "beta")):
-            step, eps, mom = ct.c_longlong(0), ct.c_float(0), ct.c_float(0)
-            self.H.cnb_net_get_bn_optimizer_state(self.h, i, which, ct.byref(step), ct.byref(eps), ct.byref(mom))
-            out[key] = {"step": step.value, "epsilon": eps.value, "momentum": mom.value}
-        return out
+        name = self._bn_layer(layer)[1]
+        return {key: self._optimizer_state(name + ":" + key) for key in ("gamma", "beta")}
 
     # --- checkpoints and Polyak averaging (ConvNet::Save / Load / InsertPolyak / LoadPolyakWeights / LoadCurrentWeights)
     def _check(self, rc):

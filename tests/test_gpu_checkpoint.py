@@ -3,6 +3,8 @@
 - Resume bit for bit: train 3 steps, save, train 3 more and save (A); a fresh net built with another seed loads the first
   file, trains the same 3 steps and saves (B).  A and B are the same bytes and the last 3 losses are equal.
 - Contents: the records (read by tests/checkpoint_format.py) equal the net's tensors and step counts.
+- An edge with has_no_bias: its bias optimizer answers and takes settings but never steps, the file holds no bias
+  records, and a resumed net trains on bit for bit.
 - Refusals: another model's checkpoint and a truncated file raise ValueError naming a record; the net is unchanged.
 - Staging: train steps after load / load_polyak_weights / load_current_weights under CONVNET_B200_STAGE_VERIFY=1.
 - Polyak: the average of a wrapped ring equals a float32 restatement of the reference's loop in slot order, fprop follows
@@ -150,6 +152,36 @@ def test_contents(tmp_path):
             seen.add(lname + ":" + k)
     assert seen == set(rec)
     n.close()
+
+
+def test_edge_without_bias(tmp_path):
+    lib.set_precision("bf16")
+    path = str(tmp_path / "nobias.pbtxt")
+    text = model_text("tiny")
+    assert "has_no_bias: false" in text
+    open(path, "w").write(text.replace("has_no_bias: false", "has_no_bias: true", 1))
+    a = Net(path, 32, seed=5)
+    name = [e[0] for e in a.edges() if e[3] > 0][0]   # the first weighted edge carries the first has_no_bias line
+    data = batches(a, 4)
+    train(a, data[:2])
+    st = a.optimizer_state(name)
+    assert st["weights"]["step"] == 2 and st["bias"]["step"] == 0
+    a.set_optimizer(name, bias={"epsilon": 0.5})
+    assert a.optimizer_state(name)["bias"] == {"step": 0, "epsilon": 0.5, "momentum": 0.0}
+    first, pa, pb = str(tmp_path / "first.ckpt"), str(tmp_path / "a.ckpt"), str(tmp_path / "b.ckpt")
+    a.save(first)
+    rec = CF.read(first)
+    assert name + ":weight" in rec and not [r for r in rec if r.startswith(name + ":bias")]
+    la = train(a, data[2:])
+    a.save(pa)
+    a.close()
+    b = Net(path, 32, seed=77)
+    b.load(first)
+    lb = train(b, data[2:])
+    b.save(pb)
+    b.close()
+    assert la == lb
+    assert same_files(pa, pb)
 
 
 def test_refusals_leave_the_net_unchanged(tmp_path, capfd):

@@ -623,39 +623,67 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
       bias = p.bias + (tile.m_tile * p.cpt / p.nbc) + (long long)p.modules * tile.n_tile * p.BN;
       bias_step = p.modules;
     }
+    // where column `col` of a row starting at `rp` lands, or nullptr (x-mode wgrad: taps / channels beyond the filter)
+    auto dst_of = [&](float* rp, int col) -> float* {
+      if (OP == kWgrad && p.x_mode) {
+        // column = tap tx + 8*(row ty + ky*channel): scattered to dW[o, tx + kx*(ty + ky*c)]
+        const int tx = col & 7, rr = col >> 3, ty = rr % p.ky, c = tile.c_tile * p.x_ct + rr / p.ky;
+        if (tx >= p.kx || c >= p.Cin) return nullptr;
+        return rp + (long long)p.Cout * (tx + p.kx * (ty + p.ky * c));
+      }
+      return rp + col_stride * col;
+    };
+    // The loads an element's store depends on (old target, ReLU' mask, bias) are issued for a batch of kEpiBatch
+    // n8-tiles before any of the batch's stores: a store may alias a later element's load as far as the compiler knows,
+    // so loads interleaved with the stores would cost one memory round trip per element.  The batch is as large as the
+    // registers allow without spilling (the tf32 fprop instance holds the mma.sync fragments as well).  wgrad has no
+    // mask or bias: it keeps the single pass, whose smaller code matters to its store-bound epilogue.
+    constexpr bool kPreload = OP != kWgrad;
+    constexpr int kEpiBatch = (!BF16 && OP == kFprop) ? 2 : 4;
 #pragma unroll
     for (int h = 0; h < 2; h++) {
       float* const rp = rowp[h];
       if (rp == nullptr) continue;
 #pragma unroll
-      for (int j = 0; j < BN_MAX / 8; j++)
+      for (int j0 = 0; j0 < BN_MAX / 8; j0 += kEpiBatch) {
+        float old[kEpiBatch][2], msk[kEpiBatch][2], bv[kEpiBatch][2];
 #pragma unroll
-        for (int e = 0; e < 2; e++) {
-          const int col = j * 8 + 2 * tq + e;
-          if (col >= ncols_valid) continue;
-          const float v = acc[j][2 * h + e];
-          float* dst;
-          if (OP == kWgrad && p.x_mode) {
-            // column = tap tx + 8*(row ty + ky*channel): scattered to dW[o, tx + kx*(ty + ky*c)]
-            const int tx = col & 7, rr = col >> 3, ty = rr % p.ky, c = tile.c_tile * p.x_ct + rr / p.ky;
-            if (tx >= p.kx || c >= p.Cin) continue;
-            dst = rp + (long long)p.Cout * (tx + p.kx * (ty + p.ky * c));
-          } else {
-            dst = rp + col_stride * col;
+        for (int jj = 0; jj < kEpiBatch; jj++)
+#pragma unroll
+          for (int e = 0; e < 2; e++) {
+            const int col = (j0 + jj) * 8 + 2 * tq + e;
+            old[jj][e] = msk[jj][e] = bv[jj][e] = 0.f;
+            if (!kPreload || col >= ncols_valid) continue;
+            const float* dst = dst_of(rp, col);
+            if (dst == nullptr) continue;
+            if (rmw) old[jj][e] = *dst;
+            if (p.mask) msk[jj][e] = __ldg(p.mask + (dst - p.out));
+            if (OP == kFprop && bias) bv[jj][e] = __ldg(bias + col * bias_step);
           }
-          float r = so_eff * v;
-          if (rmw) r += p.st * (*dst);
-          if (OP == kFprop) {
-            if (bias) r += __ldg(bias + col * bias_step);
-            if (SIG) { if (p.act) r = act_apply(r, p.act); }
-            else if (p.act) r = fmaxf(r, 0.f);
-            if (p.drop_scale != 0.f) r *= dropout_keep(p.drop_seed + (unsigned long long)(dst - p.out), p.drop_prob, p.drop_scale);
+#pragma unroll
+        for (int jj = 0; jj < kEpiBatch; jj++)
+#pragma unroll
+          for (int e = 0; e < 2; e++) {
+            const int j = j0 + jj, col = j * 8 + 2 * tq + e;
+            if (col >= ncols_valid) continue;
+            float* const dst = dst_of(rp, col);
+            if (dst == nullptr) continue;
+            float r = so_eff * acc[j][2 * h + e];
+            if (rmw) r += p.st * (kPreload ? old[jj][e] : *dst);
+            if (OP == kFprop) {
+              if (bias) r += bv[jj][e];
+              if (SIG) { if (p.act) r = act_apply(r, p.act); }
+              else if (p.act) r = fmaxf(r, 0.f);
+              if (p.drop_scale != 0.f) r *= dropout_keep(p.drop_seed + (unsigned long long)(dst - p.out), p.drop_prob, p.drop_scale);
+            }
+            if (kPreload) {                          // (wgrad: no mask)
+              if (SIG) { if (p.mask) r = act_deriv(r, msk[jj][e], p.mask_act); }
+              else if (p.mask && !(msk[jj][e] > 0.f)) r = 0.f;
+            }
+            *dst = r;
+            if (p.out16) p.out16[dst - p.out] = __float2bfloat16_rn(r);
           }
-          if (SIG) { if (p.mask) r = act_deriv(r, __ldg(p.mask + (dst - p.out)), p.mask_act); }
-          else if (p.mask && !(__ldg(p.mask + (dst - p.out)) > 0.f)) r = 0.f;
-          *dst = r;
-          if (p.out16) p.out16[dst - p.out] = __float2bfloat16_rn(r);
-        }
+      }
     }
   }
 }

@@ -11,16 +11,18 @@
 //   dgrad : D[(n,pixel), c]  = sum_{tap,o}  der[n, module(pixel,tap), o] * w[o, tap, c]    A MN-major, B K-major
 //   wgrad : D[o, c] (per tap)= sum_{module,n} der[n, module, o] * img[n, x, y, c]          A K-major,  B K-major
 //
-// One persistent CTA per SM, 9 warps: warps 0..7 are two consumer warpgroups (GEMM rows 0-63 and 64-127 of the 128 x 128
-// tile), warp 8 is the TMA producer filling a ring of shared-memory stages guarded by mbarriers.
+// One persistent CTA per SM, 12 warps: warps 0..7 are two consumer warpgroups (GEMM rows 0-63 and 64-127 of the 128 x 128
+// tile), warp 8 is the TMA producer filling a ring of shared-memory stages guarded by mbarriers, warps 9..11 store the
+// fprop / dgrad output tiles.
 //   bf16 operands: wgmma.mma_async m64n128k16 reads both operands from the swizzled tiles (either major);
 //   tf32 operands: wgmma takes 32-bit operands from shared memory only K-major, so
 //     wgrad (both operands K-major): wgmma m64n128k8 on the tiles, as bf16;
 //     x-mode fprop (Cin < 8): wgmma m64nNk8 with A (the MN-major image tile) loaded into registers and B the n-tile's
 //                  filter bank, written K-major into shared memory once per CTA and kept there;
 //     other fprop / dgrad (MN-major operands): mma.sync m16n8k8 with fragments loaded from the tiles.
-// Accumulators live in registers; the consumers store a finished tile straight from them (every group of 8 lanes writes
-// 8 consecutive images of one channel = one 32-byte sector) while the producer already fills the ring for the next tile.
+// Accumulators live in registers.  fprop / dgrad: the consumers copy a finished tile into a shared-memory staging tile and
+// go on to the next tile's k-blocks; the store warps apply the epilogue and write it with 16-byte stores (one warp
+// instruction = 128 consecutive images of one channel).  wgrad: the consumers store their tile straight from registers.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cudaTypedefs.h>
@@ -36,7 +38,8 @@ namespace cnb {
 namespace {
 
 constexpr int kConsumerWarps = 8;
-constexpr int kThreads = 32 * kConsumerWarps + 32;
+constexpr int kStoreWarps = 3;
+constexpr int kThreads = 32 * (kConsumerWarps + 1 + kStoreWarps);   // 384: ptxas caps a thread at 168 registers
 constexpr int BM = 128;             // GEMM rows per tile
 constexpr int BN_MAX = 128;         // GEMM columns per tile (the wgmma N); narrower tiles leave the extra columns unstored
 constexpr int BK = 32;              // fp32 (tf32) elements of K per pipeline stage (4 MMA steps of 8); x-mode constant
@@ -67,6 +70,7 @@ struct TcParams {
   // (bank_bytes = Cin * x_yblocks * BN * 128), filled from the caller's filters `xw` ([c][ty][tx][o], o contiguous)
   const float* xw;
   uint32_t bank_bytes;              // 0: the B half of the ring follows the A ring
+  uint32_t epi_bytes;               // fprop / dgrad: the staging tile (BM x BN fp32) after the ring or bank; wgrad: 0
   uint32_t b_tx_bytes;              // bytes the B-operand TMA(s) of one stage actually deliver
   // merged requests: when N % 128 == 0 (2-D) the chunks of an m-tile are one box over a (chunk, ..., N/chunk, ...) view
   // of the tensor; when Cout % chunk == 0 the BN/chunk filter chunks are one box likewise.
@@ -81,6 +85,7 @@ struct TcParams {
   long long part_stride;            // fprop/dgrad split-K: floats between the partial outputs of consecutive splits
   float* out;
   __nv_bfloat16* out16;             // optional bf16 twin of `out` (same indexing): convnet_b200_emit_bf16_next
+  int vec;                          // out / mask 16-byte and out16 8-byte aligned: the store warps move 4 rows at once
   float st, so;
   const float* bias; int act;       // fused fprop epilogue: + bias[o], then act_apply(., act)
   const float* mask; int mask_act;  // fused epilogue: act_deriv(., mask, mask_act) (mask: same layout as out)
@@ -98,6 +103,8 @@ struct TcParams {
 struct __align__(8) SmemCtl {
   uint64_t full[kMaxStages];
   uint64_t empty[kMaxStages];
+  uint64_t epi_full;                // the 8 consumer warps have written the staging tile
+  uint64_t epi_empty;               // the store warps have read it
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -289,6 +296,141 @@ __device__ __forceinline__ void xmode_fprop_mma(float (&acc)[16][4], const TcPar
   ptx::wgmma_fence_operands(acc);
 }
 
+// ---- fprop / dgrad epilogue: the staging tile and the store warps ---------------------------------------------------
+// Byte offset of (row, col) in the staging tile: column-major, 512 bytes per column, the 16-byte unit row / 4 XORed with
+// col & 7.  A consumer st.shared of one accumulator (lanes g = 0..7 on 8 consecutive rows, tq = 0..3 on columns 2 tq + e)
+// then hits 32 distinct banks, and a store warp's ld.shared.v4 of one column reads 512 contiguous bytes.
+__device__ __forceinline__ uint32_t epi_off(int row, int col) {
+  return (uint32_t)(col * (BM * 4) + ((((row >> 2) ^ col) & 7) << 4) + (((row >> 2) & ~7) << 4) + ((row & 3) << 2));
+}
+
+__device__ __forceinline__ float4 ld4(const float* a, bool vec) {
+  if (vec) return *reinterpret_cast<const float4*>(a);
+  return make_float4(a[0], a[1], a[2], a[3]);
+}
+__device__ __forceinline__ float4 ldg4(const float* a, bool vec) {
+  if (vec) return __ldg(reinterpret_cast<const float4*>(a));
+  return make_float4(__ldg(a), __ldg(a + 1), __ldg(a + 2), __ldg(a + 3));
+}
+
+// Store warp `sw` (0..2) of the CTA: for each of the CTA's tiles, wait until the consumers have staged it, then write
+// columns sw, sw + 3, ... Lane l holds rows 4l .. 4l+3, four consecutive images of one chunk: with N % 4 == 0 they are
+// all valid or all not.  Each element gets exactly the arithmetic of the in-register epilogue it replaces.  The loads an
+// element's store depends on (old target, ReLU' mask, bias) are issued for a batch of kEpiCols columns before any of the
+// batch's stores, since a store may alias a later load as far as the compiler knows.
+template <int OP, bool SIG>
+__device__ __forceinline__ void store_tiles(const TcParams& p, SmemCtl* ctl, uint32_t stg, int sw, int lane) {
+  constexpr int kEpiCols = SIG ? 4 : 8;            // the logistic arithmetic needs the registers of half the batch
+  const bool vec = p.vec != 0;
+  const int lr = 4 * lane;                          // this lane's first row
+  const int per_frame = (OP == kFprop) ? p.modules : p.W * p.H;
+  const long long col_stride = (long long)p.N * (OP == kFprop ? p.out_plane : (long long)per_frame);
+  const bool direct_scale = p.splits == 1;
+  const float so_eff = direct_scale ? p.so : 1.f;
+  const bool rmw = direct_scale && p.st != 0.f;
+  uint32_t phase = 0;
+  for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
+    const Tile tile = decode_tile<OP>(p, t);
+    long long row = -1;                               // offset of this lane's first row from p.out, -1: no rows
+    const int q = tile.m_tile * p.cpt + (lr >> p.chunk_shift);
+    if (q < p.total_chunks) {
+      const int ib = q % p.nbc, rr = q / p.nbc, pos = rr % per_frame, f = rr / per_frame;
+      const int n = ib * p.chunk + (lr & (p.chunk - 1));
+      if (n < p.N) {
+        if (OP == kFprop) {
+          const int i = pos % p.modX, j = pos / p.modX;
+          const long long pix = (long long)(i * p.o_sx + p.o_x0) + (long long)p.o_W * (j * p.o_sy + p.o_y0);
+          row = f * p.out_frame_step + n + (long long)p.N * pix;
+        } else {
+          row = n + (long long)p.N * pos;
+        }
+        row += col_stride * ((long long)tile.n_tile * p.BN) + tile.split * p.part_stride;
+      }
+    }
+    const int ncols = min(p.BN, (OP == kFprop ? p.Cout : p.Cin) - tile.n_tile * p.BN);
+    const float* bias = (OP == kFprop && p.bias) ? p.bias + tile.n_tile * p.BN : nullptr;
+    int bias_step = 1;
+    if (OP == kFprop && p.bias && p.untied) {         // one bias per output feature: bias[module + modules * o]
+      bias = p.bias + (tile.m_tile * p.cpt / p.nbc) + (long long)p.modules * tile.n_tile * p.BN;
+      bias_step = p.modules;
+    }
+    const int mine = ncols > sw ? (ncols - sw + kStoreWarps - 1) / kStoreWarps : 0;
+    const int batches = (mine + kEpiCols - 1) / kEpiCols;
+    ptx::mbar_wait(&ctl->epi_full, phase);
+    if (batches == 0 && lane == 0) ptx::mbar_arrive(&ctl->epi_empty);
+    for (int b = 0; b < batches; b++) {
+      const int c0 = sw + kStoreWarps * kEpiCols * b;
+      float4 acc[kEpiCols], old[kEpiCols], msk[kEpiCols];
+      float bv[kEpiCols];
+#pragma unroll
+      for (int k = 0; k < kEpiCols; k++) {
+        const int col = c0 + kStoreWarps * k;
+        acc[k] = col < ncols ? ptx::lds128(stg + epi_off(lr, col)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      if (b == batches - 1) {                         // the last read of the staging tile: the consumers may refill it
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&ctl->epi_empty);
+      }
+      if (row < 0) continue;
+#pragma unroll
+      for (int k = 0; k < kEpiCols; k++) {
+        const int col = c0 + kStoreWarps * k;
+        old[k] = msk[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+        bv[k] = 0.f;
+        if (col >= ncols) continue;
+        const long long idx = row + col_stride * col;
+        if (rmw) old[k] = ld4(p.out + idx, vec);
+        if (p.mask) msk[k] = ldg4(p.mask + idx, vec);
+        if (OP == kFprop && bias) bv[k] = __ldg(bias + col * bias_step);
+      }
+#pragma unroll
+      for (int k = 0; k < kEpiCols; k++) {
+        const int col = c0 + kStoreWarps * k;
+        if (col >= ncols) continue;
+        const long long idx = row + col_stride * col;
+        const float a[4] = {acc[k].x, acc[k].y, acc[k].z, acc[k].w};
+        const float o[4] = {old[k].x, old[k].y, old[k].z, old[k].w};
+        const float m[4] = {msk[k].x, msk[k].y, msk[k].z, msk[k].w};
+        float v[4];
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+          float r = so_eff * a[e];
+          if (rmw) r += p.st * o[e];
+          if (OP == kFprop) {
+            if (bias) r += bv[k];
+            if (SIG) { if (p.act) r = act_apply(r, p.act); }
+            else if (p.act) r = fmaxf(r, 0.f);
+            if (p.drop_scale != 0.f) r *= dropout_keep(p.drop_seed + (unsigned long long)(idx + e), p.drop_prob, p.drop_scale);
+          }
+          if (SIG) { if (p.mask) r = act_deriv(r, m[e], p.mask_act); }
+          else if (p.mask && !(m[e] > 0.f)) r = 0.f;
+          v[e] = r;
+        }
+        float* const dst = p.out + idx;
+        if (vec) {
+          *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+        } else {
+#pragma unroll
+          for (int e = 0; e < 4; e++) dst[e] = v[e];
+        }
+        if (p.out16) {
+          __nv_bfloat16* const d16 = p.out16 + idx;
+          const __nv_bfloat162 lo = __floats2bfloat162_rn(v[0], v[1]), hi = __floats2bfloat162_rn(v[2], v[3]);
+          if (vec) {
+            uint2 w;
+            w.x = *reinterpret_cast<const uint32_t*>(&lo);
+            w.y = *reinterpret_cast<const uint32_t*>(&hi);
+            *reinterpret_cast<uint2*>(d16) = w;
+          } else {
+            d16[0] = lo.x; d16[1] = lo.y; d16[2] = hi.x; d16[3] = hi.y;
+          }
+        }
+      }
+    }
+    phase ^= 1;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // SIG: the epilogue applies the activation code (logistic included); the other instances know only ReLU / ReLU', so the
 // logistic arithmetic costs the ReLU and linear layers nothing
@@ -299,13 +441,16 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smemA = smem;
   uint8_t* smemB = smem + (size_t)p.stages * kAStageBytes;      // the B ring, or the x-mode fprop filter bank
-  SmemCtl* ctl = reinterpret_cast<SmemCtl*>(smemB + (p.bank_bytes ? (size_t)p.bank_bytes : (size_t)p.stages * kBStageBytes));
+  uint8_t* smemE = smemB + (p.bank_bytes ? (size_t)p.bank_bytes : (size_t)p.stages * kBStageBytes);   // staging tile
+  SmemCtl* ctl = reinterpret_cast<SmemCtl*>(smemE + p.epi_bytes);
 
   // warp index through a shuffle: provably warp-uniform, which keeps the role branches and their loops on the uniform path
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; s++) { ptx::mbar_init(&ctl->full[s], 1); ptx::mbar_init(&ctl->empty[s], kConsumerWarps); }
+    ptx::mbar_init(&ctl->epi_full, kConsumerWarps);
+    ptx::mbar_init(&ctl->epi_empty, kStoreWarps);
     ptx::fence_barrier_init();
     ptx::tma_prefetch_desc(&mapA);
     ptx::tma_prefetch_desc(&mapB);
@@ -314,6 +459,11 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   ptx::pdl_launch_dependents();       // the kernel queued behind this one may start its prologue (it waits for this grid's end)
   ptx::pdl_wait();                    // ... as this one's just overlapped its predecessor's tail; from here on: global memory
 
+  if (warp > kConsumerWarps) {
+    // =============================== store warps (fprop / dgrad) ===============================
+    if constexpr (OP != kWgrad) store_tiles<OP, SIG>(p, ctl, ptx::smem_u32(smemE), warp - kConsumerWarps - 1, lane);
+    return;
+  }
   if (warp == kConsumerWarps) {
     // =============================== TMA producer (one lane) ===============================
     if (lane != 0) return;
@@ -492,6 +642,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   const int row0 = warp * 16 + g;                  // this thread's GEMM rows in the tile: row0 and row0 + 8
   int stage = 0; uint32_t phase = 0;
   int bank_tile = -1;                              // x-mode fprop: the n-tile whose filter bank is in shared memory
+  uint32_t epi_phase = 0;                          // fprop / dgrad: parity of the staging tile's handoff
   for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
     const Tile tile = decode_tile<OP>(p, t);
     const int nkb = tile_kblocks<OP>(p, tile);
@@ -575,33 +726,33 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     }
 
     // =============================== epilogue ===================================
-    float* rowp[2] = {nullptr, nullptr};
-    long long col_stride = 0;
-    int ncols_valid = 0;
+    if constexpr (OP != kWgrad) {
+      // hand the tile to the store warps through the staging tile, then go on to the next tile's k-blocks
+      ptx::mbar_wait(&ctl->epi_empty, epi_phase ^ 1);
+      // column j*8 + c (c < 8) lies j*8 columns past column c with the same swizzle: four base addresses serve all 64
+      uint32_t base[2][2];
 #pragma unroll
-    for (int h = 0; h < 2; h++) {
-      const int r = row0 + 8 * h;
-      if (OP == kFprop || OP == kDgrad) {
-        const int q = tile.m_tile * p.cpt + (r >> p.chunk_shift);
-        const int per_frame = (OP == kFprop) ? p.modules : p.W * p.H;
-        if (q < p.total_chunks) {
-          const int ib = q % p.nbc, rr = q / p.nbc, pos = rr % per_frame, f = rr / per_frame;
-          const int n = ib * p.chunk + (r & (p.chunk - 1));
-          if (n < p.N) {
-            if (OP == kFprop) {
-              const int i = pos % p.modX, j = pos / p.modX;
-              const long long pix = (long long)(i * p.o_sx + p.o_x0) + (long long)p.o_W * (j * p.o_sy + p.o_y0);
-              col_stride = (long long)p.N * p.out_plane;
-              rowp[h] = p.out + f * p.out_frame_step + n + (long long)p.N * pix;
-            } else {
-              col_stride = (long long)p.N * per_frame;
-              rowp[h] = p.out + n + (long long)p.N * pos;
-            }
-            rowp[h] += col_stride * ((long long)tile.n_tile * p.BN) + tile.split * p.part_stride;
-          }
-        }
-      } else {
-        const int o = tile.o_tile * BM + r;
+      for (int h = 0; h < 2; h++)
+#pragma unroll
+        for (int e = 0; e < 2; e++) base[h][e] = ptx::smem_u32(smemE) + epi_off(row0 + 8 * h, 2 * tq + e);
+#pragma unroll
+      for (int j = 0; j < BN_MAX / 8; j++) {
+        if (j * 8 >= p.BN) break;
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+          for (int e = 0; e < 2; e++) ptx::sts32(base[h][e] + j * 8 * BM * 4, acc[j][2 * h + e]);
+      }
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(&ctl->epi_full);
+      epi_phase ^= 1;
+    } else {
+      // wgrad: dW[o, tap, c] straight from the registers
+      float* rowp[2] = {nullptr, nullptr};
+      long long col_stride = 0;
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int o = tile.o_tile * BM + row0 + 8 * h;
         if (o < p.Cout) {
           rowp[h] = p.out + (long long)tile.split * p.Cout * p.taps * p.Cin + o;
           if (!p.x_mode) {
@@ -610,78 +761,35 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
           }
         }
       }
-    }
-    if (OP == kFprop || OP == kDgrad) ncols_valid = min(p.BN, (OP == kFprop ? p.Cout : p.Cin) - tile.n_tile * p.BN);
-    else if (p.x_mode) ncols_valid = min(p.BN, p.x_ct * p.ky * 8);
-    else ncols_valid = min(p.BN, p.Cin - tile.c_tile * p.BN);
-    const bool direct_scale = (p.splits == 1) || (OP == kWgrad && p.untied);   // untied wgrad: one dW block per module
-    const float so_eff = direct_scale ? p.so : 1.f;
-    const bool rmw = direct_scale && p.st != 0.f;
-    const float* bias = (OP == kFprop && p.bias) ? p.bias + tile.n_tile * p.BN : nullptr;
-    int bias_step = 1;
-    if (OP == kFprop && p.bias && p.untied) {         // one bias per output feature: bias[module + modules * o]
-      bias = p.bias + (tile.m_tile * p.cpt / p.nbc) + (long long)p.modules * tile.n_tile * p.BN;
-      bias_step = p.modules;
-    }
-    // where column `col` of a row starting at `rp` lands, or nullptr (x-mode wgrad: taps / channels beyond the filter)
-    auto dst_of = [&](float* rp, int col) -> float* {
-      if (OP == kWgrad && p.x_mode) {
-        // column = tap tx + 8*(row ty + ky*channel): scattered to dW[o, tx + kx*(ty + ky*c)]
-        const int tx = col & 7, rr = col >> 3, ty = rr % p.ky, c = tile.c_tile * p.x_ct + rr / p.ky;
-        if (tx >= p.kx || c >= p.Cin) return nullptr;
-        return rp + (long long)p.Cout * (tx + p.kx * (ty + p.ky * c));
-      }
-      return rp + col_stride * col;
-    };
-    // The loads an element's store depends on (old target, ReLU' mask, bias) are issued for a batch of kEpiBatch
-    // n8-tiles before any of the batch's stores: a store may alias a later element's load as far as the compiler knows,
-    // so loads interleaved with the stores would cost one memory round trip per element.  The batch is as large as the
-    // registers allow without spilling (the tf32 fprop instance holds the mma.sync fragments as well).  wgrad has no
-    // mask or bias: it keeps the single pass, whose smaller code matters to its store-bound epilogue.
-    constexpr bool kPreload = OP != kWgrad;
-    constexpr int kEpiBatch = (!BF16 && OP == kFprop) ? 2 : 4;
+      const int ncols_valid = p.x_mode ? min(p.BN, p.x_ct * p.ky * 8) : min(p.BN, p.Cin - tile.c_tile * p.BN);
+      const bool direct_scale = (p.splits == 1) || p.untied;   // untied wgrad: one dW block per module
+      const float so_eff = direct_scale ? p.so : 1.f;
+      const bool rmw = direct_scale && p.st != 0.f;
+      // where column `col` of a row starting at `rp` lands, or nullptr (x-mode: taps / channels beyond the filter)
+      auto dst_of = [&](float* rp, int col) -> float* {
+        if (p.x_mode) {
+          // column = tap tx + 8*(row ty + ky*channel): scattered to dW[o, tx + kx*(ty + ky*c)]
+          const int tx = col & 7, rr = col >> 3, ty = rr % p.ky, c = tile.c_tile * p.x_ct + rr / p.ky;
+          if (tx >= p.kx || c >= p.Cin) return nullptr;
+          return rp + (long long)p.Cout * (tx + p.kx * (ty + p.ky * c));
+        }
+        return rp + col_stride * col;
+      };
 #pragma unroll
-    for (int h = 0; h < 2; h++) {
-      float* const rp = rowp[h];
-      if (rp == nullptr) continue;
+      for (int h = 0; h < 2; h++) {
+        float* const rp = rowp[h];
+        if (rp == nullptr) continue;
 #pragma unroll
-      for (int j0 = 0; j0 < BN_MAX / 8; j0 += kEpiBatch) {
-        float old[kEpiBatch][2], msk[kEpiBatch][2], bv[kEpiBatch][2];
-#pragma unroll
-        for (int jj = 0; jj < kEpiBatch; jj++)
+        for (int j = 0; j < BN_MAX / 8; j++)
 #pragma unroll
           for (int e = 0; e < 2; e++) {
-            const int col = (j0 + jj) * 8 + 2 * tq + e;
-            old[jj][e] = msk[jj][e] = bv[jj][e] = 0.f;
-            if (!kPreload || col >= ncols_valid) continue;
-            const float* dst = dst_of(rp, col);
-            if (dst == nullptr) continue;
-            if (rmw) old[jj][e] = *dst;
-            if (p.mask) msk[jj][e] = __ldg(p.mask + (dst - p.out));
-            if (OP == kFprop && bias) bv[jj][e] = __ldg(bias + col * bias_step);
-          }
-#pragma unroll
-        for (int jj = 0; jj < kEpiBatch; jj++)
-#pragma unroll
-          for (int e = 0; e < 2; e++) {
-            const int j = j0 + jj, col = j * 8 + 2 * tq + e;
+            const int col = j * 8 + 2 * tq + e;
             if (col >= ncols_valid) continue;
             float* const dst = dst_of(rp, col);
             if (dst == nullptr) continue;
             float r = so_eff * acc[j][2 * h + e];
-            if (rmw) r += p.st * (kPreload ? old[jj][e] : *dst);
-            if (OP == kFprop) {
-              if (bias) r += bv[jj][e];
-              if (SIG) { if (p.act) r = act_apply(r, p.act); }
-              else if (p.act) r = fmaxf(r, 0.f);
-              if (p.drop_scale != 0.f) r *= dropout_keep(p.drop_seed + (unsigned long long)(dst - p.out), p.drop_prob, p.drop_scale);
-            }
-            if (kPreload) {                          // (wgrad: no mask)
-              if (SIG) { if (p.mask) r = act_deriv(r, msk[jj][e], p.mask_act); }
-              else if (p.mask && !(msk[jj][e] > 0.f)) r = 0.f;
-            }
+            if (rmw) r += p.st * *dst;
             *dst = r;
-            if (p.out16) p.out16[dst - p.out] = __float2bfloat16_rn(r);
           }
       }
     }
@@ -742,16 +850,18 @@ int pick_bn(int cols, int granule) {              // N-tile: as wide as possible
   return std::min(BN_MAX, std::max(granule, bn));
 }
 
-// dynamic shared memory of a launch with `stages` ring stages: A stages, then B stages or (x-mode fprop) the filter bank
-size_t smem_bytes_for(int stages, uint32_t bank_bytes) {
+// dynamic shared memory of a launch with `stages` ring stages: A stages, then B stages or (x-mode fprop) the filter bank,
+// then (fprop / dgrad) the staging tile
+size_t smem_bytes_for(int stages, uint32_t bank_bytes, uint32_t epi_bytes) {
   const size_t b = bank_bytes ? (size_t)bank_bytes : (size_t)stages * kBStageBytes;
-  return 1024 + (size_t)stages * kAStageBytes + b + sizeof(SmemCtl) + 16;
+  return 1024 + (size_t)stages * kAStageBytes + b + epi_bytes + sizeof(SmemCtl) + 16;
 }
-constexpr size_t kSmemBudget = 225 * 1024;
+constexpr size_t kSmemBudget = 227 * 1024;        // the most a block may use; launch_one requests it
+inline uint32_t epi_bytes_for(int bn) { return (uint32_t)BM * bn * 4; }
 
-int pick_stages(uint32_t bank_bytes) {
+int pick_stages(uint32_t bank_bytes, uint32_t epi_bytes) {
   int s = kMaxStages;
-  while (s > 2 && smem_bytes_for(s, bank_bytes) > kSmemBudget) s--;
+  while (s > 2 && smem_bytes_for(s, bank_bytes, epi_bytes) > kSmemBudget) s--;
   return s;
 }
 
@@ -770,8 +880,12 @@ void launch_one(const CUtensorMap& a, const CUtensorMap& b, const TcParams& p, s
 
 template <int OP>
 void launch(const CUtensorMap& a, const CUtensorMap& b, TcParams& p) {
-  p.stages = pick_stages(p.bank_bytes);
-  const size_t smem = smem_bytes_for(p.stages, p.bank_bytes);
+  p.epi_bytes = OP == kWgrad ? 0u : epi_bytes_for(p.BN);
+  p.stages = pick_stages(p.bank_bytes, p.epi_bytes);
+  const size_t smem = smem_bytes_for(p.stages, p.bank_bytes, p.epi_bytes);
+  // the store warps move 4 rows (16 bytes of out / mask, 8 of out16) per access where the pointers allow it
+  auto aligned = [](const void* q, uintptr_t a) { return (reinterpret_cast<uintptr_t>(q) & (a - 1)) == 0; };
+  p.vec = aligned(p.out, 16) && aligned(p.mask, 16) && aligned(p.out16, 8) ? 1 : 0;
   const bool sig = p.act == kActLogistic || (p.mask && p.mask_act == kActLogistic);
   CNB_REQUIRE(OP != kWgrad || !sig, "tc_conv: wgrad has no activation epilogue");
   void (*run)(const CUtensorMap&, const CUtensorMap&, const TcParams&, size_t) = nullptr;
@@ -793,10 +907,10 @@ void fill_common(TcParams& p, const ConvGeom& g, const Elem& e) {
   p.frames = g.frames; p.frame0 = 0;
   p.splits = 1; p.units_per_split = 0; p.part_stride = 0;
   p.x_mode = 0; p.x_yblocks = 0; p.x_ct = 0; p.b_tx_bytes = 0;
-  p.xw = nullptr; p.bank_bytes = 0;
+  p.xw = nullptr; p.bank_bytes = 0; p.epi_bytes = 0;
   p.a_merged = 0; p.b_merged = 0;
   p.untied = g.conv ? 0 : 1;
-  p.bias = nullptr; p.act = 0; p.mask = nullptr; p.mask_act = 0; p.out16 = nullptr;
+  p.bias = nullptr; p.act = 0; p.mask = nullptr; p.mask_act = 0; p.out16 = nullptr; p.vec = 0;
   p.drop_prob = 0.f; p.drop_scale = 0.f; p.drop_seed = 0;
   p.o_sx = p.o_sy = 1; p.o_x0 = p.o_y0 = 0; p.o_W = g.modX; p.out_plane = g.modules;
   p.out_frame_step = g.out_frame_step;
@@ -958,10 +1072,10 @@ static ConvOutcome tc_conv_up_impl(const ConvGeom& g, const float* images, const
   p.x_mode = x_mode ? 1 : 0;
   p.x_yblocks = ceil_div(g.ky, 4);
   if (x_mode) {
-    // B is the n-tile's filter bank, resident beside the A ring: it must leave room for >= 3 A stages, else the tile
-    // narrows (Cin 7, ky 8 at BN 128) — more n-tiles, the same single launch
+    // B is the n-tile's filter bank, resident beside the A ring and the staging tile: it must leave room for >= 3 A
+    // stages, else the tile narrows (Cin 7, ky 8 at BN 128) — more n-tiles, the same single launch
     auto bank_bytes = [&](int bn) { return (uint32_t)g.Cin * p.x_yblocks * bn * 128; };
-    while (p.BN > 32 && smem_bytes_for(3, bank_bytes(p.BN)) > kSmemBudget) p.BN = ceil_div(p.BN / 2, 32) * 32;
+    while (p.BN > 32 && smem_bytes_for(3, bank_bytes(p.BN), epi_bytes_for(p.BN)) > kSmemBudget) p.BN = ceil_div(p.BN / 2, 32) * 32;
     p.bank_bytes = bank_bytes(p.BN);
     p.xw = filters;
   }

@@ -97,6 +97,14 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 __device__ __forceinline__ uint32_t lds32(uint32_t addr) {
   uint32_t v; asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory"); return v;
 }
+__device__ __forceinline__ float4 lds128(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void sts32(uint32_t addr, float v) {
+  asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+}
 
 // ---- mma.sync (tf32): D[16x8] += A[16x8] * B[8x8], fp32 bit patterns in, the tensor core reads their tf32 part ---------
 __device__ __forceinline__ void mma_tf32_16x8x8(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,

@@ -316,8 +316,9 @@ __device__ __forceinline__ float4 ldg4(const float* a, bool vec) {
 // Store warp `sw` (0..2) of the CTA: for each of the CTA's tiles, wait until the consumers have staged it, then write
 // columns sw, sw + 3, ... Lane l holds rows 4l .. 4l+3, four consecutive images of one chunk: with N % 4 == 0 they are
 // all valid or all not.  Each element gets exactly the arithmetic of the in-register epilogue it replaces.  The loads an
-// element's store depends on (old target, ReLU' mask, bias) are issued for a batch of kEpiCols columns before any of the
-// batch's stores, since a store may alias a later load as far as the compiler knows.
+// element's store depends on (old target, ReLU' mask, bias) are issued ahead of the stores they would otherwise wait
+// behind, since a store may alias a later load as far as the compiler knows: the bias once per tile, the old target and
+// the mask one batch of kEpiCols columns ahead.
 template <int OP, bool SIG>
 __device__ __forceinline__ void store_tiles(const TcParams& p, SmemCtl* ctl, uint32_t stg, int sw, int lane) {
   constexpr int kEpiCols = SIG ? 4 : 8;            // the logistic arithmetic needs the registers of half the batch
@@ -356,11 +357,38 @@ __device__ __forceinline__ void store_tiles(const TcParams& p, SmemCtl* ctl, uin
     }
     const int mine = ncols > sw ? (ncols - sw + kStoreWarps - 1) / kStoreWarps : 0;
     const int batches = (mine + kEpiCols - 1) / kEpiCols;
+    // the bias of this warp's (at most 43) columns, loaded once per tile before the wait: lane l holds that of its
+    // l-th and (l+32)-th column, and a batch takes them by shuffle.  A bias load inside a batch would wait a full
+    // memory round trip behind the previous batch's stores, which the compiler must assume may alias it.
+    static_assert(BN_MAX <= 64 * kStoreWarps, "two bias values per lane cover a store warp's columns");
+    float bias_lo = 0.f, bias_hi = 0.f;
+    if (OP == kFprop && bias) {
+      const int ca = sw + kStoreWarps * lane, cb = ca + kStoreWarps * 32;
+      if (ca < ncols) bias_lo = __ldg(bias + ca * bias_step);
+      if (cb < ncols) bias_hi = __ldg(bias + cb * bias_step);
+    }
+    // the loads a batch's arithmetic depends on (old target, ReLU' mask), software-pipelined: batch b+1's are issued
+    // after batch b's arithmetic and before its stores, and batch 0's before the wait for the tile.  Issued after the
+    // previous batch's stores instead, each batch would wait one full memory round trip.  Batches cover disjoint
+    // columns, so a load never reads an element that an earlier store in program order wrote.
+    float4 acc[kEpiCols], old[kEpiCols], msk[kEpiCols];
+    auto load_batch = [&](int b) {
+      const int c0 = sw + kStoreWarps * kEpiCols * b;
+#pragma unroll
+      for (int k = 0; k < kEpiCols; k++) {
+        const int col = c0 + kStoreWarps * k;
+        old[k] = msk[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (row < 0 || col >= ncols) continue;
+        const long long idx = row + col_stride * col;
+        if (rmw) old[k] = ld4(p.out + idx, vec);
+        if (p.mask) msk[k] = ldg4(p.mask + idx, vec);
+      }
+    };
+    if (batches > 0) load_batch(0);
     ptx::mbar_wait(&ctl->epi_full, phase);
     if (batches == 0 && lane == 0) ptx::mbar_arrive(&ctl->epi_empty);
     for (int b = 0; b < batches; b++) {
       const int c0 = sw + kStoreWarps * kEpiCols * b;
-      float4 acc[kEpiCols], old[kEpiCols], msk[kEpiCols];
       float bv[kEpiCols];
 #pragma unroll
       for (int k = 0; k < kEpiCols; k++) {
@@ -371,20 +399,16 @@ __device__ __forceinline__ void store_tiles(const TcParams& p, SmemCtl* ctl, uin
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(&ctl->epi_empty);
       }
+      if (OP == kFprop && bias) {
+#pragma unroll
+        for (int k = 0; k < kEpiCols; k++) {          // column c0 + 3k is this warp's (kEpiCols b + k)-th
+          const int j = kEpiCols * b + k;
+          bv[k] = __shfl_sync(0xffffffffu, j < 32 ? bias_lo : bias_hi, j & 31);
+        }
+      }
       if (row < 0) continue;
 #pragma unroll
-      for (int k = 0; k < kEpiCols; k++) {
-        const int col = c0 + kStoreWarps * k;
-        old[k] = msk[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-        bv[k] = 0.f;
-        if (col >= ncols) continue;
-        const long long idx = row + col_stride * col;
-        if (rmw) old[k] = ld4(p.out + idx, vec);
-        if (p.mask) msk[k] = ldg4(p.mask + idx, vec);
-        if (OP == kFprop && bias) bv[k] = __ldg(bias + col * bias_step);
-      }
-#pragma unroll
-      for (int k = 0; k < kEpiCols; k++) {
+      for (int k = 0; k < kEpiCols; k++) {            // the results replace the accumulators in acc
         const int col = c0 + kStoreWarps * k;
         if (col >= ncols) continue;
         const long long idx = row + col_stride * col;
@@ -406,9 +430,18 @@ __device__ __forceinline__ void store_tiles(const TcParams& p, SmemCtl* ctl, uin
           else if (p.mask && !(m[e] > 0.f)) r = 0.f;
           v[e] = r;
         }
+        acc[k] = make_float4(v[0], v[1], v[2], v[3]);
+      }
+      if ((rmw || p.mask) && b + 1 < batches) load_batch(b + 1);
+#pragma unroll
+      for (int k = 0; k < kEpiCols; k++) {
+        const int col = c0 + kStoreWarps * k;
+        if (col >= ncols) continue;
+        const long long idx = row + col_stride * col;
+        const float v[4] = {acc[k].x, acc[k].y, acc[k].z, acc[k].w};
         float* const dst = p.out + idx;
         if (vec) {
-          *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+          *reinterpret_cast<float4*>(dst) = acc[k];
         } else {
 #pragma unroll
           for (int e = 0; e < 4; e++) dst[e] = v[e];

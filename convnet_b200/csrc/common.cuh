@@ -116,6 +116,8 @@ struct State {
   int precision = kPrecFP32;      // the raw C ABI computes in fp32 (the reference's arithmetic) until a caller opts into tf32 / bf16
   int last_conv_path = kPathNone;
   unsigned long long launches = 0;  // kernels launched by this library
+  // dgrad filter banks built (convnet_b200_dgrad_bank_builds): [0] inside a convDown call, [1] in a prestage request
+  unsigned long long bank_builds[2] = {0, 0};
   // scratch (wgrad partial sums, rnorm-free) — grown on demand, never per-call malloc'd
   void* ws = nullptr;
   size_t ws_bytes = 0;

@@ -1187,7 +1187,7 @@ static bool dgrad_as_fprop_eligible(const ConvGeom& g, const float* derivs, cons
 void tc_conv_down_prestage(const ConvGeom& g, const float* derivs, const float* filters) {
   DgradBanks banks;
   if (!g.conv || !want_bf16() || !dgrad_as_fprop_eligible(g, derivs, filters, &banks)) return;
-  dgrad_weights(filters, g, banks);
+  dgrad_weights(filters, g, banks, true);
 }
 
 static ConvOutcome tc_conv_down_as_fprop(const ConvGeom& g, const float* derivs, const float* filters, float* targets,
@@ -1202,7 +1202,7 @@ static ConvOutcome tc_conv_down_as_fprop(const ConvGeom& g, const float* derivs,
     to_bf16(derivs, tmp, g.out_total);
     sd = tmp;
   }
-  const __nv_bfloat16* bank = dgrad_weights(filters, g, banks);
+  const __nv_bfloat16* bank = dgrad_weights(filters, g, banks, false);
   for (int i = 0; i < banks.count; i++) {
     const DgradPhase& P = banks.phase[i];
     TcParams p; fill_common(p, g, e);

@@ -119,6 +119,7 @@ void convnet_b200_bf16_invalidate(const float* ptr) { bf16_invalidate(ptr); }
 int convnet_b200_last_conv_path(void) { return state().last_conv_path; }
 unsigned long long convnet_b200_launch_count(void) { return state().launches; }
 void convnet_b200_reset_launch_count(void) { state().launches = 0; }
+unsigned long long convnet_b200_dgrad_bank_builds(int in_prestage) { return state().bank_builds[in_prestage ? 1 : 0]; }
 void convnet_b200_release_workspace(void) {
   State& s = state();
   bf16_release();

@@ -77,16 +77,18 @@ void verify(const Staged& e, long long n) {
   }
 }
 
-Staged* find_slot(const float* ptr, int dev, int kind = 0) {
-  for (Staged& e : table()) if (e.src == ptr && e.dev == dev && e.kind == kind) return &e;
+// kind 1 slots are keyed by the geometry too: one filter tensor used at several geometries (tied edges) keeps a set of
+// banks per geometry, and a write to the filters drops them all (bf16_note_write)
+Staged* find_slot(const float* ptr, int dev, int kind = 0, unsigned long long sig = 0) {
+  for (Staged& e : table()) if (e.src == ptr && e.dev == dev && e.kind == kind && (kind != 1 || e.sig == sig)) return &e;
   return nullptr;
 }
 
 // slot for [ptr, ptr+n) with a buffer of at least n bf16; contents undefined, valid == false
-Staged* acquire_slot(const float* ptr, long long n, int kind = 0) {
+Staged* acquire_slot(const float* ptr, long long n, int kind = 0, unsigned long long sig = 0) {
   std::vector<Staged>& t = table();
   const int dev = current_device();
-  Staged* slot = find_slot(ptr, dev, kind);
+  Staged* slot = find_slot(ptr, dev, kind, sig);
   if (!slot) {
     if (t.size() >= kMaxStaged) {                                       // recycle the least recently used entry
       slot = &t[0];
@@ -108,7 +110,7 @@ Staged* acquire_slot(const float* ptr, long long n, int kind = 0) {
     CNB_CUDA_CHECK(cudaMalloc((void**)&slot->buf, bytes));
     slot->cap = bytes;
   }
-  slot->src = ptr; slot->n = n; slot->dev = dev; slot->valid = false; slot->tick = ++g_tick; slot->kind = kind; slot->sig = 0;
+  slot->src = ptr; slot->n = n; slot->dev = dev; slot->valid = false; slot->tick = ++g_tick; slot->kind = kind; slot->sig = sig;
   slot->src2 = nullptr; slot->n2 = 0;
   return slot;
 }
@@ -168,19 +170,20 @@ int dgrad_phases(const ConvGeom& g, DgradBanks* b) {
   return b->count;
 }
 
-const __nv_bfloat16* dgrad_weights(const float* filters, const ConvGeom& g, const DgradBanks& b) {
+const __nv_bfloat16* dgrad_weights(const float* filters, const ConvGeom& g, const DgradBanks& b, bool prestage) {
   const long long n = (long long)g.Cout * g.K;
   unsigned long long sig = 1469598103934665603ULL;
   for (int v : {g.Cin, g.Cout, g.kx, g.ky, g.sx, g.sy, g.px, g.py, g.W, g.H}) sig = (sig ^ (unsigned)v) * 1099511628211ULL;
   const int dev = current_device();
-  Staged* e = find_slot(filters, dev, 1);
-  if (e && e->valid && e->n == n && e->sig == sig) { e->tick = ++g_tick; return e->buf; }
-  e = acquire_slot(filters, n, 1);
+  Staged* e = find_slot(filters, dev, 1, sig);
+  if (e && e->valid && e->n == n) { e->tick = ++g_tick; return e->buf; }
+  e = acquire_slot(filters, n, 1, sig);
   const dim3 grid((unsigned)ceil_div(g.Cout, 32), (unsigned)ceil_div(g.Cin, 32), (unsigned)(g.kx * g.ky));
   dgrad_bank_kernel<<<grid, 256, 0, state().stream>>>(filters, e->buf, b, g.Cin, g.Cout, g.kx, g.ky, g.sx, g.sy);
   count_launch();
+  state().bank_builds[prestage ? 1 : 0]++;
   CNB_LAUNCH_CHECK("dgrad_banks");
-  e->valid = true; e->sig = sig;
+  e->valid = true;
   return e->buf;
 }
 

@@ -56,8 +56,11 @@ API long long cnb_net_num_params(void* p) { return (long long)((NetHandle*)p)->n
 API int cnb_net_num_edges(void* p) { return (int)((NetHandle*)p)->net->Edges().size(); }
 API const char* cnb_net_edge_name(void* p, int i) { return ((NetHandle*)p)->net->Edges()[i]->GetName().c_str(); }
 API double cnb_net_edge_flops(void* p, int i) { return ((NetHandle*)p)->net->Edges()[i]->FlopsUp(); }
-API long long cnb_net_edge_offset(void* p, int i) { return (long long)((NetHandle*)p)->net->EdgeOffsets()[i]; }
-API long long cnb_net_edge_size(void* p, int i) { return (long long)((NetHandle*)p)->net->EdgeSizes()[i]; }
+// where edge i's parameters begin in the flat buffers (a tied edge: its owner's), and how many floats it owns (0 if tied)
+API long long cnb_net_edge_offset(void* p, int i) { return (long long)((NetHandle*)p)->net->ParamOffset(i); }
+API long long cnb_net_edge_size(void* p, int i) { return (long long)((NetHandle*)p)->net->Edges()[i]->GetParameterMemoryRequirement(); }
+// the edge whose parameters edge i runs with ("" when untied)
+API const char* cnb_net_edge_tied_to(void* p, int i) { return ((NetHandle*)p)->net->Edges()[i]->Config().tied_to.c_str(); }
 API double cnb_net_flops_fprop(void* p) { return ((NetHandle*)p)->net->FlopsFprop(); }
 API double cnb_net_flops_train(void* p) { return ((NetHandle*)p)->net->FlopsTrainStep(); }
 API float* cnb_net_input(void* p) { return ((NetHandle*)p)->net->InputLayer().GetState().GetDevData(); }
@@ -71,6 +74,8 @@ API float* cnb_net_grads(void* p) { return ((NetHandle*)p)->net->GradParameters(
 // the momentum history (laid out like the parameters); a write through it is the caller's
 API float* cnb_net_history(void* p) { return ((NetHandle*)p)->net->History().GetDevData(); }
 API float* cnb_net_layer_state(void* p, int i) { return ((NetHandle*)p)->net->Layers()[i]->GetState().GetDevData(); }
+// the derivative of layer i's state after bprop (laid out like its state); NULL for the input layer
+API float* cnb_net_layer_deriv(void* p, int i) { return ((NetHandle*)p)->net->Layers()[i]->GetDeriv().GetDevData(); }
 API long long cnb_net_layer_floats(void* p, int i) { return (long long)((NetHandle*)p)->net->Layers()[i]->GetState().GetNumEls(); }
 API int cnb_net_num_layers(void* p) { return (int)((NetHandle*)p)->net->Layers().size(); }
 API float* cnb_net_device_loss(void* p) { return ((NetHandle*)p)->net->DeviceLoss(); }
@@ -261,15 +266,29 @@ API int cnb_model_bn_layer(const char* model, int layer, char* name, int* channe
   return 1;
 }
 // static description of a model: the optimizer config of edge `edge` (which: 0 weights, 1 bias).  0 ok, -1 unknown model,
-// -2 edge out of range or without parameters
+// -2 edge out of range or without parameters of its own (a tied edge trains with its owner's optimizers)
 API int cnb_model_edge_optimizer(const char* model, int edge, int which, OptimizerConfig* out) {
   ModelConfig m;
   if (!TryBuildModel(model, &m)) return -1;
   if (edge < 0 || edge >= (int)m.edge.size() || which < 0 || which > 1) return -2;
   const EdgeConfig& e = m.edge[edge];
-  if (e.edge_type == MAXPOOL || e.edge_type == AVGPOOL || e.edge_type == RESPONSE_NORM || (which == 1 && e.has_no_bias)) return -2;
+  if (e.edge_type == MAXPOOL || e.edge_type == AVGPOOL || e.edge_type == RESPONSE_NORM || (which == 1 && e.has_no_bias) ||
+      !e.tied_to.empty())
+    return -2;
   *out = which ? e.bias_optimizer : e.weight_optimizer;
   return 0;
+}
+
+// static description of a model: the name of edge `edge` and, if it is tied, the edge whose parameters it uses (both
+// NUL-terminated, up to 256 bytes).  1 tied, 0 untied, -1 unknown model, -2 edge out of range
+API int cnb_model_tie(const char* model, int edge, char* name, char* owner) {
+  ModelConfig m;
+  if (!TryBuildModel(model, &m)) return -1;
+  if (edge < 0 || edge >= (int)m.edge.size()) return -2;
+  const EdgeConfig& e = m.edge[edge];
+  snprintf(name, 256, "%s", e.name.c_str());
+  snprintf(owner, 256, "%s", e.tied_to.c_str());
+  return e.tied_to.empty() ? 0 : 1;
 }
 
 // a model's resolved ModelConfig as a config::Model text proto (ModelText).  Returns its length in bytes (-1: unknown
@@ -288,13 +307,13 @@ API long long cnb_model_text(const char* model, char* buf, long long cap) {
 
 // static description of a model: the initial weights of edge `edge` under RNG seed `seed` (EdgeWithWeight::InitialWeights;
 // the net seeds edge i with its seed + 17 i), or a PRETRAINED edge's weights from its checkpoint.  Returns their number
-// (writes up to `cap`); -1 unknown model or unreadable checkpoint, -2 edge out of range or without parameters
+// (writes up to `cap`); -1 unknown model or unreadable checkpoint, -2 edge out of range or without parameters of its own
 API long long cnb_model_initial_weights(const char* model, int edge, unsigned seed, float* out, long long cap) {
   ConvNet* net = TryBuildNet(model, 1);
   if (!net) return -1;
   EdgeWithWeight* e = edge >= 0 && edge < (int)net->Edges().size() ? dynamic_cast<EdgeWithWeight*>(net->Edges()[edge].get()) : nullptr;
   long long n = -2;
-  if (e) {
+  if (e && !e->Tied()) {
     std::vector<float> w;
     try {
       w = e->Config().initialization == PRETRAINED ? PretrainedWeights(e->Config(), e->WeightCount()) : e->InitialWeights(seed);

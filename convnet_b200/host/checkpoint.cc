@@ -241,10 +241,10 @@ void ConvNet::Load(const std::string& path) {
   ModelConfig opt = CurrentModel();
   std::string unmatched;
   for (size_t i = 0; i < edges_.size(); i++) {
-    if (edges_[i]->HasNoParameters()) continue;
+    if (owner_[i] != (int)i) continue;                 // no parameters, or a tied edge's (its owner's records hold them)
     bool found = false;
     for (const EdgeConfig& e : saved.edge)
-      if (e.source + ":" + e.dest == edges_[i]->GetName() && e.edge_type == model_.edge[i].edge_type) {
+      if (e.source + ":" + e.dest == edges_[i]->GetName() && e.edge_type == model_.edge[i].edge_type && e.tied_to.empty()) {
         opt.edge[i].weight_optimizer = e.weight_optimizer;
         if (!e.has_no_bias) opt.edge[i].bias_optimizer = e.bias_optimizer;
         found = true;
@@ -310,7 +310,7 @@ void ConvNet::LoadPretrained(size_t i) {
   const std::string from = c.pretrained_edge_name.empty() ? edge : c.pretrained_edge_name;
   const CheckpointFile f(c.pretrained_model);
   for (TrainedTensor& t : tensors_) {
-    if (t.edge != (int)i || !t.OnEdge() || t.n == 0) continue;
+    if (t.owner != (int)i || !t.OnEdge() || t.n == 0) continue;
     const std::string prefix = from + t.name.substr(edge.size());            // <from>:weight, <from>:bias
     const char* adaptive = AdaptiveSuffix(t.opt);
     std::vector<std::pair<std::string, float*>> tensors = {{prefix, parameters_.GetDevData() + t.offset},

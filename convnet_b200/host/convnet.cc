@@ -78,6 +78,43 @@ std::string EdgeShapeError(const Edge& e, int source_channels, int dest_channels
   return "";
 }
 
+std::string TieError(const std::vector<const Edge*>& edges, size_t i) {
+  const EdgeConfig& c = edges[i]->Config();
+  if (c.tied_to.empty()) return "";
+  const std::string f = "field 'tied_to': ", owner = "edge '" + c.tied_to + "'";
+  size_t k = 0;
+  while (k < edges.size() && edges[k]->GetName() != c.tied_to) k++;
+  if (k == edges.size()) return f + "the net has no edge '" + c.tied_to + "'";
+  if (k == i) return f + "an edge cannot be tied to itself";
+  const EdgeConfig& o = edges[k]->Config();
+  if (!o.tied_to.empty()) return f + owner + " is itself tied (to '" + o.tied_to + "'): tie to '" + o.tied_to + "' instead";
+  if (edges[k]->HasNoParameters()) return f + owner + " has no parameters";
+  static const char* const types[] = {"FC", "CONVOLUTIONAL", "MAXPOOL", "AVERAGE_POOL", "RESPONSE_NORM", "CONV_ONETOONE", "LOCAL"};
+  if (o.edge_type != c.edge_type)
+    return f + owner + " is " + types[o.edge_type] + ", this edge " + types[c.edge_type] + " (a tie joins edges of one edge_type)";
+  const EdgeWithWeight *w = dynamic_cast<const EdgeWithWeight*>(edges[i]), *ow = dynamic_cast<const EdgeWithWeight*>(edges[k]);
+  auto shape = [](const Shape4D& s) {
+    return "(" + std::to_string(s.shape[0]) + ", " + std::to_string(s.shape[1]) + ", " + std::to_string(s.shape[2]) + ", " +
+           std::to_string(s.shape[3]) + ")";
+  };
+  const Shape4D a = w->GetWeightShape(), b = ow->GetWeightShape();
+  if (memcmp(&a, &b, sizeof(a)) != 0)
+    return f + "the weights of this edge have shape " + shape(a) + ", those of " + owner + " " + shape(b);
+  auto bias = [](const EdgeWithWeight* e) {
+    const EdgeConfig& x = e->Config();
+    if (x.has_no_bias) return std::string("none (has_no_bias)");
+    return std::to_string(e->GetNumOutputChannels()) + " x " + std::to_string(e->GetBiasCols()) +
+           (x.edge_type == CONVOLUTIONAL ? (x.shared_bias ? " (shared_bias)" : " (one per output position)") : "");
+  };
+  if (bias(w) != bias(ow)) return f + "the bias of this edge is " + bias(w) + ", that of " + owner + " " + bias(ow);
+  // every contribution to the shared bias gradient must come from one stream: a 3-D conv sums its bias on the main stream,
+  // a 2-D one on the side lane
+  if (c.edge_type == CONVOLUTIONAL && (edges[i]->GetImageSizeT() == 1) != (edges[k]->GetImageSizeT() == 1))
+    return f + "a tie joins a 3-D and a 2-D convolution";
+  if (c.grad_check) return f + "grad_check on a tied edge (set it on " + owner + ", which checks the shared tensors)";
+  return "";
+}
+
 std::string LayerConfigError(const LayerConfig& c) {
   const bool softmax = c.activation == SOFTMAX || c.activation == SOFTMAX_DIST;
   if (!c.is_output) {
@@ -321,7 +358,31 @@ ConvNet::ConvNet(const ModelConfig& model, int batch_size) : model_(model), batc
   }
   const std::string why = Refusal();
   if (!why.empty()) throw std::invalid_argument(why);
+  ResolveTies();
   PlanFusion();
+}
+
+void ConvNet::ResolveTies() {
+  const int n = (int)edges_.size();
+  owner_.assign(n, -1);
+  home_.assign(n, -1);
+  for (int i = 0; i < n; i++) {
+    if (edges_[i]->HasNoParameters()) continue;
+    owner_[i] = i;
+    for (int k = 0; k < n; k++)
+      if (edges_[k]->GetName() == model_.edge[i].tied_to) owner_[i] = k;
+  }
+  for (int i = n - 1; i >= 0; i--)                   // from the top down: the group's lowest edge is written last
+    if (owner_[i] >= 0) home_[owner_[i]] = i;
+  for (int i = 0; i < n; i++) {
+    if (owner_[i] < 0) continue;
+    home_[i] = home_[owner_[i]];
+    if (owner_[i] != i)
+      static_cast<EdgeWithWeight*>(edges_[i].get())->TieTo(static_cast<EdgeWithWeight*>(edges_[owner_[i]].get()));
+  }
+}
+bool ConvNet::Grouped(size_t i) const {
+  return owner_[i] >= 0 && std::count(owner_.begin(), owner_.end(), owner_[i]) > 1;
 }
 
 std::string ConvNet::Refusal() const {
@@ -329,12 +390,17 @@ std::string ConvNet::Refusal() const {
     const std::string why = LayerConfigError(lc);
     if (!why.empty()) return "layer '" + lc.name + "': " + why;
   }
+  std::vector<const Edge*> chain;
+  for (const auto& e : edges_) chain.push_back(e.get());
   for (size_t i = 0; i < edges_.size(); i++) {
     const std::string shape = EdgeShapeError(*edges_[i], layers_[i]->GetNumChannels(), layers_[i + 1]->GetNumChannels());
     if (!shape.empty()) return "edge '" + edges_[i]->GetName() + "': " + shape;
+    const std::string tie = TieError(chain, i);
+    if (!tie.empty()) return "edge '" + edges_[i]->GetName() + "': " + tie;
     if (model_.edge[i].edge_type == LOCAL && layers_[i]->GetSizeT() != 1)     // the untied conv kernels are 2-D only
       return "edge '" + edges_[i]->GetName() + "': LOCAL is not supported on 3-D layers (image_size_t > 1)";
     const int init = model_.edge[i].initialization;
+    if (!model_.edge[i].tied_to.empty()) continue;                          // (its initialisation is never used)
     if (!edges_[i]->HasNoParameters() && init != DENSE_GAUSSIAN && init != DENSE_GAUSSIAN_SQRT_FAN_IN &&
         init != DENSE_UNIFORM && init != DENSE_UNIFORM_SQRT_FAN_IN && init != CONSTANT && init != PRETRAINED)
       return "edge '" + edges_[i]->GetName() + "': initialization " + std::to_string(init) + " is not implemented";
@@ -378,7 +444,9 @@ void ConvNet::PlanFusion() {
     p.dropout_up = a.dropout && p.up_act != CNB_ACT_LINEAR && fused_dropout;
     p.scale_down = a.dropout && p.down_act != CNB_ACT_LINEAR && dropout_fold;
     p.sums_bias_below = a.sums_bias_below;
-    p.offers_bias_grad = a.per_channel_bias;
+    // a pool-undo sums the handed-off bias gradient on the main stream, the other edges of a tie group sum theirs into the
+    // same bias on the side lane: a tie group keeps every contribution on the side lane, in back-propagation order
+    p.offers_bias_grad = a.per_channel_bias && !Grouped(i);
     e->SetFusionPlan(p);
     dst->SetActivationFused(p.up_act != CNB_ACT_LINEAR || dst->BatchNormalize());
     src->SetDerivFused(p.down_act != CNB_ACT_LINEAR);
@@ -411,8 +479,8 @@ ConvNet::~ConvNet() {
 // has run ComputeOuter, so the bucket that carries the edge carries them too (edge_span_ is what PlanBuckets sees)
 OptimizerConfig& ModelOptimizer(ModelConfig& m, const TrainedTensor& t) {
   switch (t.kind) {
-    case TrainedTensor::WEIGHTS: return m.edge[t.edge].weight_optimizer;
-    case TrainedTensor::BIAS: return m.edge[t.edge].bias_optimizer;
+    case TrainedTensor::WEIGHTS: return m.edge[t.owner].weight_optimizer;
+    case TrainedTensor::BIAS: return m.edge[t.owner].bias_optimizer;
     case TrainedTensor::GAMMA: return m.layer[t.edge + 1].gamma_optimizer;
     default: return m.layer[t.edge + 1].beta_optimizer;
   }
@@ -422,28 +490,32 @@ void ConvNet::PlanParameters() {
   edge_offset_.clear(); edge_size_.clear(); edge_span_.clear(); tensors_.clear();
   bn_offset_.assign(layers_.size(), -1);
   size_t total = 0;
-  auto add = [&](TrainedTensor::Kind kind, const std::string& owner, int edge, size_t offset, long long n, int rows) {
+  auto add = [&](TrainedTensor::Kind kind, const std::string& owner, int edge, size_t offset, long long n, int rows, int of) {
     static const char* const suffix[] = {":weight", ":bias", ":gamma", ":beta"};
     TrainedTensor t{kind, owner + suffix[kind], edge, offset, n, rows};
+    t.owner = of;
     t.opt = ModelOptimizer(model_, t);
     tensors_.push_back(t);
   };
   for (size_t i = 0; i < edges_.size(); i++) {
-    const size_t req = edges_[i]->GetParameterMemoryRequirement();
+    // the slice at edge i: the parameters of the owner whose tie group starts here (edge i's own when untied), else none
+    const int o = owner_[i] >= 0 && home_[i] == (int)i ? owner_[i] : -1;
+    const size_t req = o >= 0 ? edges_[o]->GetParameterMemoryRequirement() : 0;
     edge_offset_.push_back(total);
     edge_size_.push_back(req);
     // the rows of the weights are the output units; the bias is ONE row (fc_edge.cc:29-32)
-    if (const EdgeWithWeight* w = dynamic_cast<const EdgeWithWeight*>(edges_[i].get())) {
-      add(TrainedTensor::WEIGHTS, w->GetName(), (int)i, total, w->WeightCount(), w->GetNumOutputChannels());
-      add(TrainedTensor::BIAS, w->GetName(), (int)i, total + (size_t)w->WeightCount(), w->BiasCount(), 1);
+    if (o >= 0) {
+      const EdgeWithWeight* w = static_cast<const EdgeWithWeight*>(edges_[o].get());
+      add(TrainedTensor::WEIGHTS, w->GetName(), (int)i, total, w->WeightCount(), w->GetNumOutputChannels(), o);
+      add(TrainedTensor::BIAS, w->GetName(), (int)i, total + (size_t)w->WeightCount(), w->BiasCount(), 1, o);
     }
     total += DIVUP(req, (size_t)128) * 128;
     Layer* l = layers_[i + 1].get();
     if (l->BatchNormalize()) {
       const int C = l->GetNumChannels();
       bn_offset_[i + 1] = (long long)total;
-      add(TrainedTensor::GAMMA, l->GetName(), (int)i, total, C, 1);
-      add(TrainedTensor::BETA, l->GetName(), (int)i, total + C, C, 1);
+      add(TrainedTensor::GAMMA, l->GetName(), (int)i, total, C, 1, (int)i);
+      add(TrainedTensor::BETA, l->GetName(), (int)i, total + C, C, 1, (int)i);
       total += DIVUP(2 * (size_t)C, (size_t)128) * 128;
     }
     edge_span_.push_back(total - edge_offset_.back());
@@ -461,13 +533,14 @@ void ConvNet::AllocateMemory() {
   history_.AllocateGPUMemory(1, (int)total);
   loss_sum_.AllocateGPUMemory(1, 2);                           // the loss, the performance metric
   for (size_t i = 0; i < edges_.size(); i++) {
-    if (edge_size_[i] == 0) continue;
+    if (owner_[i] < 0) continue;
+    const int h = home_[i];                                    // every edge of a tie group is carved from the one slice
     Matrix p, g;
-    parameters_.GetSlice(p, (int)edge_offset_[i], (int)(edge_offset_[i] + edge_size_[i]));
-    grad_parameters_.GetSlice(g, (int)edge_offset_[i], (int)(edge_offset_[i] + edge_size_[i]));
+    parameters_.GetSlice(p, (int)edge_offset_[h], (int)(edge_offset_[h] + edge_size_[h]));
+    grad_parameters_.GetSlice(g, (int)edge_offset_[h], (int)(edge_offset_[h] + edge_size_[h]));
     edges_[i]->SetMemory(p);
     edges_[i]->SetGradMemory(g);
-    edges_[i]->Initialize(model_.seed + 17 * (unsigned)i);
+    edges_[i]->Initialize(model_.seed + 17 * (unsigned)i);     // (a tied edge initialises nothing)
   }
   for (size_t i = 0; i < layers_.size(); i++) {
     if (bn_offset_[i] < 0) continue;
@@ -483,7 +556,7 @@ void ConvNet::AllocateMemory() {
   // the reference allocates the optimizers before Initialize reads a PRETRAINED edge (fc_edge.cc:42, convnet.cc:286-303),
   // so the edge takes the history, the step and the adaptive state from the file too
   for (size_t i = 0; i < edges_.size(); i++)
-    if (!edges_[i]->HasNoParameters() && model_.edge[i].initialization == PRETRAINED) LoadPretrained(i);
+    if (owner_[i] == (int)i && model_.edge[i].initialization == PRETRAINED) LoadPretrained(i);
   HOST_CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
   InvalidateStaging();
   HOST_CUDA_CHECK(cudaStreamCreateWithFlags(&side_, cudaStreamNonBlocking));
@@ -658,9 +731,12 @@ void ConvNet::IssueBucketUpdate(const Bucket& b) {
   // (PlanBuckets splits at edge boundaries, so every row of a tensor is updated in this one call)
   cnb_opt_update_multi(tensors.data(), (int)tensors.size());
   // what the next step's dgrad derives from these weights alone (bf16 filter banks): rebuilt here, behind the update
+  // (a tie group's weights are updated in the bucket of its lowest edge: every edge of the group rebuilds its banks here)
   if (prestage_)
     for (int i = b.trigger; i <= b.last; i++)
-      if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i].get())) w->PrestageDown();
+      if (owner_[i] >= 0 && home_[i] == i)
+        for (size_t k = 0; k < edges_.size(); k++)
+          if (owner_[k] == owner_[i]) static_cast<EdgeWithWeight*>(edges_[k].get())->PrestageDown();
   convnet_b200_set_stream(main_stream);
   opt_pending_ = true;
 }
@@ -693,8 +769,8 @@ void ConvNet::UpdateWeights() {                              // convnet.cc:440-4
 }
 
 void ConvNet::AppendUpdates(int first, int last, std::vector<CnbOptTensorEx>& out) {
-  for (int i = first; i <= last; i++)
-    if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(edges_[i].get())) w->NotifyStart();
+  for (int i = first; i <= last; i++)                          // one gradient counter per tie group, reset with its update
+    if (owner_[i] >= 0 && home_[i] == i) static_cast<EdgeWithWeight*>(edges_[owner_[i]].get())->NotifyStart();
   float *p = parameters_.GetDevData(), *h = history_.GetDevData(), *g = grad_parameters_.GetDevData(), *s = AdaptiveState();
   for (TrainedTensor& t : tensors_)
     if (t.edge >= first && t.edge <= last && t.n > 0)

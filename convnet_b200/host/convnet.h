@@ -57,6 +57,11 @@ std::string LayerConfigError(const LayerConfig& c);
 // its destination at least one module in y, x and t, a pooling or response-norm edge keeps the channel count, and a
 // convolution has no temporal padding (the 3-D kernels fold the frames into channels); else why not
 std::string EdgeShapeError(const Edge& e, int source_channels, int dest_channels);
+// "" if edge `i` of a chain (every edge's SetImageSize has run) is untied, or may run with and train the parameters of the
+// edge its tied_to names; else why not, starting with "field 'tied_to': ".  The owner must exist, be another edge, be
+// untied itself, have parameters of the same edge_type and the same weight and bias shapes, and sum its bias gradient on
+// the same stream; a tied edge may not ask for grad_check (its owner checks the shared tensors)
+std::string TieError(const std::vector<const Edge*>& edges, size_t i);
 
 struct ModelConfig {
   std::string name;
@@ -102,12 +107,14 @@ struct TrainedTensor {
   enum Kind { WEIGHTS, BIAS, GAMMA, BETA };
   Kind kind;
   std::string name;        // the checkpoint record prefix: <edge>:weight, <edge>:bias, <layer>:gamma, <layer>:beta
-  int edge;                // the edge whose bucket carries it (for gamma / beta: the edge that writes the layer)
+  int edge;                // the edge whose bucket carries it (for gamma / beta: the edge that writes the layer; for a tie
+                           // group's weights and bias: the group's lowest edge)
   size_t offset;           // into the flat parameter, gradient, history and adaptive state buffers
   long long n;             // floats
   int rows;                // norm groups: the output units of the weights; one for the others
   OptimizerConfig opt;     // the settings in force
   long long step = 0;      // updates counted so far, the reference's per-optimizer step_ (optimizer.cc:199)
+  int owner = -1;          // weights / bias: the edge whose tensors they are and whose config gives their optimizer
   // ReduceLearningRate scales the edges' tensors only: gamma / beta keep their rate, as in the reference
   bool OnEdge() const { return kind == WEIGHTS || kind == BIAS; }
   // nullptr if `c` can train this tensor, else why not
@@ -278,8 +285,12 @@ class ConvNet {
   int BatchSize() const { return batch_size_; }
   double FlopsFprop() const;
   double FlopsTrainStep() const;                                // fprop + wgrad for every weighted edge + dgrad except into the input
+  // per edge position: the slice of the flat buffer placed there (a tie group's slice sits at its lowest edge; the other
+  // edges of the group have an empty one)
   const std::vector<size_t>& EdgeOffsets() const { return edge_offset_; }
   const std::vector<size_t>& EdgeSizes() const { return edge_size_; }
+  // where the parameters edge `i` runs with begin (its owner's slice for a tied edge)
+  size_t ParamOffset(size_t i) const { return edge_offset_[owner_[i] >= 0 ? home_[i] : (int)i]; }
   const std::vector<long long>& BnOffsets() const { return bn_offset_; }     // per layer: offset of [gamma | beta], -1 none
   float* DeviceLoss() { return loss_sum_.GetDevData(); }
   // One traced TrainOneBatch: device times (ms since the step began) of the pipeline's milestones, for the scaling report:
@@ -296,7 +307,14 @@ class ConvNet {
   // which passes of the neighbouring layers ride in each edge's kernels (Edge::FusionPlan), once the shapes are known;
   // also tells each layer whether its activation / derivative pass is left to do (Layer::SetActivationFused / SetDerivFused)
   void PlanFusion();
-  bool prestage_ = true;                        // rebuild the dgrad banks behind each optimizer step (PrestageDown)
+  // tie groups (EdgeConfig::tied_to), resolved once Refusal has accepted them: per edge, owner_ is the edge whose parameters
+  // it runs with (itself when untied, -1 without parameters) and home_ the group's lowest edge, where the parameters sit in
+  // the flat buffer.  Back-propagation reaches that edge last, so its bucket becomes final after every contribution to
+  // the shared gradients and every read of the shared weights
+  std::vector<int> owner_, home_;
+  void ResolveTies();
+  bool Grouped(size_t i) const;                 // edge i shares its parameters with another edge
+  bool prestage_ = true;                       // rebuild the dgrad banks behind each optimizer step (PrestageDown)
   Matrix parameters_, grad_parameters_, history_, loss_sum_, state_;
   std::vector<TrainedTensor> tensors_;
   void AllocateAdaptiveState();                 // state_, each tensor's slice initialised for its optimizer

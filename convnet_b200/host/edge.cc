@@ -114,6 +114,7 @@ void EdgeWithWeight::SumBias(Matrix& deriv_output, float scale_targets, float sc
 }
 
 size_t EdgeWithWeight::GetParameterMemoryRequirement() {
+  if (Tied()) return 0;                                      // it runs on its owner's slice
   return (size_t)num_output_channels_ * (WeightCols() + (has_no_bias_ ? 0 : BiasCols()));
 }
 void EdgeWithWeight::Carve(Matrix& p, Matrix& w, Matrix& b) {    // e.g. conv_edge.cc:80-96, 108-136
@@ -167,7 +168,10 @@ void EdgeWithWeight::ComputeOuter(Matrix& input, Matrix& deriv_output) {   // e.
 void EdgeWithWeight::NoteUp() { bf_up_ = convnet_b200_last_conv_path() == 2 ? 1 : 0; }
 void EdgeWithWeight::NoteDown() {
   bf_down_ = convnet_b200_last_conv_path() == 2 ? 1 : 0;
-  if (bf_up_ == 0 && bf_down_ == 0) convnet_b200_bf16_invalidate(weights_.GetDevData());     // nobody reads the bf16 weights
+  // nobody reads the bf16 weights: no edge of the tie group (just this edge when untied) has taken or may take a bf16 path
+  for (const EdgeWithWeight* e : owner_->group_)
+    if (e->bf_up_ != 0 || e->bf_down_ != 0) return;
+  convnet_b200_bf16_invalidate(weights_.GetDevData());
 }
 void EdgeWithWeight::NoteOuter() { bf_outer_ = convnet_b200_last_conv_path() == 2 ? 1 : 0; }
 
@@ -252,7 +256,8 @@ std::vector<float> EdgeWithWeight::InitialWeights(unsigned seed) const {
   return h;
 }
 void EdgeWithWeight::Initialize(unsigned seed) {
-  if (config_.initialization == PRETRAINED) return;          // ConvNet::AllocateMemory reads it from its checkpoint
+  // PRETRAINED: ConvNet::AllocateMemory reads it from its checkpoint; a tied edge's parameters are its owner's
+  if (config_.initialization == PRETRAINED || Tied()) return;
   const std::vector<float> h = InitialWeights(seed);
   const size_t n = weights_.GetNumEls();
   weights_.CopyFromHost(h.data(), n);

@@ -92,6 +92,9 @@ struct EdgeConfig {
   bool grad_check = false;
   int grad_check_num_params = 10;
   std::vector<float> grad_check_epsilon;
+  // the name of the edge whose weights and bias this edge runs with and trains ("" = its own; src/edge.cc:131-180).  A tied
+  // edge has no parameters of its own: its optimizers, initialisation and pretrained_* fields are not used (TieError)
+  std::string tied_to;
 };
 
 class Edge {
@@ -118,6 +121,7 @@ class Edge {
   int GetNumModulesY() const { return num_modules_y_; }
   int GetNumModulesX() const { return num_modules_x_; }
   int GetNumModulesT() const { return num_modules_t_; }
+  int GetImageSizeT() const { return image_size_t_; }
   void SetInputChannels(int a) { num_input_channels_ = a; }
   void SetOutputChannels(int a) { num_output_channels_ = a; }
   int GetNumOutputChannels() const { return num_output_channels_; }
@@ -208,6 +212,13 @@ class EdgeWithWeight : public Edge {
   // parameters [Cout x (WeightCols + BiasCols)]: the weights (Shape4D WeightShape), then the bias columns; the gradient
   // is carved the same way
   size_t GetParameterMemoryRequirement() override;
+  // tied edges (EdgeConfig::tied_to): ConvNet hands this edge the owner's parameter and gradient slices, and the group
+  // shares the owner's gradient counter, so the first contribution of a step overwrites and the others accumulate
+  // (edge_with_weight.cc:150-188)
+  bool Tied() const { return !config_.tied_to.empty(); }
+  void TieTo(EdgeWithWeight* owner) { owner_ = owner; owner->group_.push_back(this); }
+  Shape4D GetWeightShape() const { return WeightShape(); }
+  int GetBiasCols() const { return has_no_bias_ ? 0 : BiasCols(); }
   void SetMemory(Matrix& p) override { Carve(p, weights_, bias_); }
   void SetGradMemory(Matrix& p) override { Carve(p, grad_weights_, grad_bias_); }
   void Initialize(unsigned seed) override;
@@ -218,9 +229,9 @@ class EdgeWithWeight : public Edge {
   Matrix& GetGradWeight() { return grad_weights_; }
   Matrix& GetBias() { return bias_; }
   Matrix& GetGradBias() { return grad_bias_; }
-  int GetNumGradsReceived() const { return num_grads_received_; }
-  void IncrementNumGradsReceived() { num_grads_received_++; }
-  void NotifyStart() { num_grads_received_ = 0; }             // the optimizer has taken this step's gradients
+  int GetNumGradsReceived() const { return owner_->num_grads_received_; }
+  void IncrementNumGradsReceived() { owner_->num_grads_received_++; }
+  void NotifyStart() { owner_->num_grads_received_ = 0; }     // the optimizer has taken this step's gradients
   // bf16 mode (convnet_b200_set_conv_precision(2)): each tensor this edge feeds to two conv calls of a step has ONE bf16
   // copy — the input (fprop + wgrad), the output derivative (wgrad + dgrad) and the weights (fprop + dgrad).  The copy is
   // normally written by the kernel that produced the tensor (the emit requests of the neighbouring edges, the dropout
@@ -266,6 +277,8 @@ class EdgeWithWeight : public Edge {
   bool has_no_bias_;
   float scale_gradients_;
   int num_grads_received_;
+  EdgeWithWeight* owner_ = this;                         // whose parameters and gradient counter this edge uses
+  std::vector<EdgeWithWeight*> group_{this};             // the owner's: every edge that uses its parameters, itself first
   int bf_up_ = -1, bf_down_ = -1, bf_outer_ = -1;        // -1 unknown, 0 tf32 / fp32 path, 1 bf16 path
   // the tensors of the last ComputeDown that took the bf16 path (layer-owned, stable): PrestageDown re-describes that call
   Matrix* down_out_ = nullptr;

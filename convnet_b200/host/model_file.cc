@@ -515,18 +515,28 @@ class Mapper {
     // the image sizes along the chain, as ConvNet propagates them: each edge type's own SetImageSize, so that an edge
     // ConvNet::Refusal would refuse (EdgeShapeError) is refused here with its line
     int y = m.layer[0].image_size_y, x = m.layer[0].image_size_x, t = m.layer[0].image_size_t;
+    std::vector<std::unique_ptr<Edge>> built;
     for (size_t k = 0; k + 1 < chain.size(); k++) {
       const Entry& at = *edges[out[chain[k]]];
       m.edge.push_back(MapEdge(at, m.layer[k]));
-      std::unique_ptr<Edge> e(Edge::ChooseEdgeClass(m.edge[k]));
+      built.emplace_back(Edge::ChooseEdgeClass(m.edge[k]));
+      Edge* e = built.back().get();
       e->SetInputChannels(m.layer[k].num_channels);
       e->SetOutputChannels(m.layer[k + 1].num_channels);
       e->SetImageSize(y, x, t);
       const std::string why = EdgeShapeError(*e, m.layer[k].num_channels, m.layer[k + 1].num_channels);
       if (!why.empty()) Fail(at, EdgeName(*at.msg), why);
-      if (check_pretrained_ && m.edge[k].initialization == PRETRAINED && !e->HasNoParameters())
-        CheckPretrained(*at.msg, *dynamic_cast<EdgeWithWeight*>(e.get()), m.edge[k]);
+      if (check_pretrained_ && m.edge[k].initialization == PRETRAINED && !e->HasNoParameters() && m.edge[k].tied_to.empty())
+        CheckPretrained(*at.msg, *dynamic_cast<EdgeWithWeight*>(e), m.edge[k]);
       y = e->GetNumModulesY(); x = e->GetNumModulesX(); t = e->GetNumModulesT();
+    }
+    // ties, once every edge knows its shapes (ConvNet::Refusal runs the same checks), at the line of tied_to
+    std::vector<const Edge*> chain_edges;
+    for (const auto& e : built) chain_edges.push_back(e.get());
+    for (size_t k = 0; k < built.size(); k++) {
+      const std::string why = TieError(chain_edges, k);
+      const Msg& e = *edges[out[chain[k]]]->msg;
+      if (!why.empty()) Fail(*e.Get("tied_to"), EdgeName(e), why);
     }
     return m;
   }
@@ -664,7 +674,7 @@ class Mapper {
     const int t = HostValue(kEdgeTypeNames, type);
     if (t < 0) Fail(*e.Get("edge_type"), where, "field 'edge_type': " + type + " is not supported");
     c.edge_type = (EdgeType)t;
-    RefuseMessage(e, "tied_to", "tied edges are not supported", where);
+    if (const Entry* tie = e.Get("tied_to")) c.tied_to = tie->s;      // checked with the whole chain (TieError)
     RefuseMessage(e, "source_slice", "layer slices are not supported", where);
     RefuseMessage(e, "dest_slice", "layer slices are not supported", where);
     if (e.Bool("block_backprop", false)) Fail(*e.Get("block_backprop"), where, "field 'block_backprop': not supported");
@@ -873,16 +883,20 @@ std::string ModelText(const ModelConfig& m) {
     if (HasParameters(e.edge_type)) {
       if (e.edge_type == CONVOLUTIONAL) w.Bool("shared_bias", e.shared_bias);
       w.Bool("has_no_bias", e.has_no_bias);
-      w.Line("initialization", Writer::EnumName("Initialization", e.initialization));
-      if (e.initialization == PRETRAINED) {
-        w.Line("pretrained_model", Quote(e.pretrained_model));
-        w.Line("pretrained_edge_name", Quote(e.pretrained_edge_name.empty() ? e.source + ":" + e.dest : e.pretrained_edge_name));
+      if (!e.tied_to.empty()) {                            // the owner's initialisation and optimizers apply
+        w.Line("tied_to", Quote(e.tied_to));
+      } else {
+        w.Line("initialization", Writer::EnumName("Initialization", e.initialization));
+        if (e.initialization == PRETRAINED) {
+          w.Line("pretrained_model", Quote(e.pretrained_model));
+          w.Line("pretrained_edge_name", Quote(e.pretrained_edge_name.empty() ? e.source + ":" + e.dest : e.pretrained_edge_name));
+        }
+        w.Flt("init_wt", e.init_wt);
+        w.Flt("init_bias", e.init_bias);
       }
-      w.Flt("init_wt", e.init_wt);
-      w.Flt("init_bias", e.init_bias);
       w.Flt("scale_gradients", e.scale_gradients);
-      w.Optimizer("weight_optimizer", e.weight_optimizer);
-      if (!e.has_no_bias) w.Optimizer("bias_optimizer", e.bias_optimizer);
+      if (e.tied_to.empty()) w.Optimizer("weight_optimizer", e.weight_optimizer);
+      if (e.tied_to.empty() && !e.has_no_bias) w.Optimizer("bias_optimizer", e.bias_optimizer);
       w.Bool("grad_check", e.grad_check);
       if (e.grad_check) {
         w.Int("grad_check_num_params", e.grad_check_num_params);

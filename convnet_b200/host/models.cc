@@ -170,6 +170,49 @@ ModelConfig BuildLocalCheckNet() {
   return m;
 }
 
+// weight sharing (EdgeConfig::tied_to) on the training path: one 64 -> 64 3x3 conv runs at three geometries — 32 x 32
+// with padding 1, 16 x 16 after a max-pool, and with stride 2 — so one filter tensor keeps three sets of dgrad banks; and
+// two 256 -> 256 FC edges share weights with the LOWER edge naming the higher one, so the shared slice sits at the tied
+// edge rather than at its owner.  Dropout on the owner's output layer, a softmax classifier
+ModelConfig BuildTiedNet() {
+  ModelConfig m; m.name = "tiednet";
+  LayerConfig in = L("input", 3); in.is_input = true; in.image_size_y = in.image_size_x = 32;
+  m.layer = {in, L("conv1", 64, RECTIFIED_LINEAR), L("conv2", 64, RECTIFIED_LINEAR), L("pool2", 64),
+             L("conv3", 64, RECTIFIED_LINEAR), L("conv4", 64, RECTIFIED_LINEAR), L("fc5", 256, RECTIFIED_LINEAR),
+             L("fc6", 256, RECTIFIED_LINEAR), L("fc7", 256, RECTIFIED_LINEAR, 0.5f), L("output", 10, SOFTMAX)};
+  m.layer.back().is_output = true;
+  m.edge = {Conv(3, 1, 1), Conv(3, 1, 1), Pool(2, 2, 0), Conv(3, 1, 1), Conv(3, 2, 1), E(FC), E(FC), E(FC), E(FC)};
+  finish(m);
+  m.edge[3].tied_to = m.edge[4].tied_to = m.edge[1].name;          // pool2:conv3 and conv3:conv4 run conv1:conv2's filters
+  m.edge[6].tied_to = m.edge[7].name;                                // fc5:fc6 runs with fc6:fc7's weights
+  return m;
+}
+
+// run_grad_check net for ties, smooth like BuildGradCheckNet (linear units, average pooling): a conv used at padding 1
+// and padding 0, a CONV_ONETOONE, a LOCAL and an FC tie (the FC one named by the lower edge).  grad_check is set on every
+// edge with parameters of its own; an owner's check perturbs the shared tensors, so it checks the summed gradient
+ModelConfig BuildTiedCheckNet() {
+  ModelConfig m; m.name = "tiedcheck";
+  LayerConfig in = L("input", 4); in.is_input = true; in.image_size_y = in.image_size_x = 8;
+  m.layer = {in, L("c0", 8), L("c1", 8), L("c2", 8), L("pool", 8), L("o1", 8), L("o2", 8), L("l1", 8), L("l2", 8),
+             L("f1", 16), L("f2", 16), L("f3", 16), L("output", 5, SOFTMAX)};
+  m.layer.back().is_output = true;
+  EdgeConfig l1 = E(LOCAL, 3, 1, 1);
+  l1.init_wt = 3.f;                                         // sqrt(3 x 3 modules), as in localcheck
+  m.edge = {Conv(3, 1, 1), Conv(3, 1, 1), Conv(3, 1, 0), E(AVGPOOL, 2, 2, 0), E(CONV_ONETOONE), E(CONV_ONETOONE), l1, l1,
+            E(FC), E(FC), E(FC), E(FC)};
+  finish(m);
+  m.edge[2].tied_to = m.edge[1].name;                                // 8 x 8 at padding 1, then at padding 0
+  m.edge[5].tied_to = m.edge[4].name;
+  m.edge[7].tied_to = m.edge[6].name;
+  m.edge[9].tied_to = m.edge[10].name;
+  for (EdgeConfig& e : m.edge) {
+    e.grad_check = e.tied_to.empty(); e.grad_check_num_params = 10; e.grad_check_epsilon = {1e-2f, 3e-3f, 1e-3f};
+  }
+  m.edge[6].grad_check_num_params = 8 * 9;                 // module 0's taps of input channel 0 (see localcheck)
+  return m;
+}
+
 // NOT a model: a deliberately invalid config (a 3-D clip net with a LOCAL edge) that the tests of the host's refusals
 // build by the name "invalid:local3d" — ConvNet refuses it, the untied kernels being 2-D
 ModelConfig BuildLocal3DNet() {
@@ -331,10 +374,14 @@ ModelConfig BuildModel(const std::string& name) {
   const std::string suffix = "+gradcheck";
   if (name.size() > suffix.size() && name.compare(name.size() - suffix.size(), suffix.size(), suffix) == 0) {
     ModelConfig m = BuildModel(name.substr(0, name.size() - suffix.size()));
-    for (EdgeConfig& e : m.edge) { e.grad_check = true; e.grad_check_num_params = 10; e.grad_check_epsilon = {1e-2f, 1e-3f, 1e-4f}; }
+    for (EdgeConfig& e : m.edge) {                          // (a tied edge is checked through its owner)
+      e.grad_check = e.tied_to.empty(); e.grad_check_num_params = 10; e.grad_check_epsilon = {1e-2f, 1e-3f, 1e-4f};
+    }
     return m;
   }
   if (name == "gradcheck") return BuildGradCheckNet();
+  if (name == "tiednet") return BuildTiedNet();
+  if (name == "tiedcheck") return BuildTiedCheckNet();
   if (name == "logcheck") return BuildLogCheckNet();
   if (name == "alexnet") return BuildAlexNet();
   if (name == "lenet") return BuildLeNet();

@@ -80,6 +80,7 @@ SIGNATURES = {
     "convnet_b200_reserve_sms": [I],
     "convnet_b200_pool_cache_next": [],
     "convnet_b200_prestage_next": [],
+    "convnet_b200_dgrad_bank_builds": [I],
     "convnet_b200_extract_patches": [MP, MP, MP, MP, MP, I, I, I, I],
     "convnet_b200_fuse_next_dropout": [ct.c_float, ct.c_float, ct.c_ulonglong],
     "convnet_b200_fuse_next_scale": [F],
@@ -114,6 +115,7 @@ RESTYPES = {
     "convnet_b200_version": I, "convnet_b200_get_stream": ct.c_void_p,
     "convnet_b200_get_conv_precision": I, "convnet_b200_last_conv_path": I, "convnet_b200_bf16_is_staged": I,
     "convnet_b200_launch_count": ct.c_ulonglong, "convnet_b200_extract_patches": I,
+    "convnet_b200_dgrad_bank_builds": ct.c_ulonglong,
 }
 
 _lib = None

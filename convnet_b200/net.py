@@ -97,6 +97,9 @@ def load_host():
             "cnb_net_load_current_weights": ([vp], i), "cnb_net_polyak_count": ([vp], i),
             "cnb_model_polyak": ([ct.c_char_p, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i)], i),
             "cnb_polyak_due": ([ct.c_char_p, ll], i),
+            "cnb_net_edge_tied_to": ([vp, i], ct.c_char_p),
+            "cnb_net_layer_deriv": ([vp, i], vp),
+            "cnb_model_tie": ([ct.c_char_p, i, ct.c_char_p, ct.c_char_p], i),
         }
         for name, (args, res) in sig.items():
             fn = getattr(H, name)
@@ -107,7 +110,7 @@ def load_host():
 
 class Net:
     """A chain ConvNet built natively, from a built-in name ("alexnet" | "lenet" | "c3d" | "tiny" | "lcnet" | "gradcheck" |
-    "logcheck" | "localcheck") or from a model file: any name ending in ".pbtxt" is the path of a config::Model text proto
+    "logcheck" | "localcheck" | "tiednet" | "tiedcheck") or from a model file: any name ending in ".pbtxt" is the path of a config::Model text proto
     as the reference writes them (examples/*/net.pbtxt), read with the proto's defaults (model_text() prints any model
     as one).  The file's seed is printed but not used: `seed` decides, for files as for built-ins.  Suffixes compose with
     both ("net.pbtxt+rmsprop"):
@@ -124,6 +127,10 @@ class Net:
     CROSS_ENTROPY_BINARY, metric CLASSIFICATION_BINARY), "+soft-targets" (SOFTMAX_DIST, CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED);
     such outputs train on targets_tensor() instead of labels_tensor().  "logcheck": the gradcheck net with logistic units.
     A model that cannot be read or run raises ValueError; the reason (for a file: its line and field) is on stderr.
+
+    Tied edges (the reference's Edge.tied_to, see model_ties()) run with their owner's weights and bias and add their
+    gradients to the owner's: they own no parameters (edges() reports size 0 and the owner's offset), and the owner's
+    optimizers, tensors ("<owner>:weight", "<owner>:bias") and checkpoint records serve the whole group.
 
     Checkpoints (the reference's ConvNet::Save / Load): save(path) writes the parameters, the optimizers' histories, step
     counts and adaptive state, the batch-norm running statistics, the iteration, the seed and the optimizer settings in
@@ -205,6 +212,12 @@ class Net:
     def layer_state(self, i):
         return self._view(self.H.cnb_net_layer_state(self.h, i), self.H.cnb_net_layer_floats(self.h, i), "f")
 
+    def layer_deriv(self, i):
+        """the derivative of the loss with respect to layer i's state after bprop, laid out like layer_state(i); None for
+        the input layer"""
+        ptr = self.H.cnb_net_layer_deriv(self.h, i)
+        return self._view(ptr, self.H.cnb_net_layer_floats(self.h, i), "f") if ptr else None
+
     # --- compute
     def fprop(self, train=False):
         self.H.cnb_net_fprop(self.h, int(train))
@@ -236,13 +249,21 @@ class Net:
         return {"step": step.value, "epsilon": eps.value, "momentum": mom.value} if rc == 0 else None
 
     def _edge_name(self, edge):
-        """the name of `edge` (index or name); "" for an index out of range, whose tensors the host then does not find"""
+        """the name of `edge` (index or name); "" for an index out of range, whose tensors the host then does not find.
+        ValueError for a tied edge, whose optimizers are its owner's"""
         names = [e[0] for e in self.edges()]
         if isinstance(edge, str):
             if edge not in names:
                 raise KeyError("no edge %r (edges: %s)" % (edge, ", ".join(names)))
-            return edge
-        return names[int(edge)] if 0 <= int(edge) < len(names) else ""
+            i = names.index(edge)
+        elif 0 <= int(edge) < len(names):
+            i = int(edge)
+        else:
+            return ""
+        owner = self.H.cnb_net_edge_tied_to(self.h, i).decode()
+        if owner:
+            raise ValueError("edge %r is tied to %r: its weights, bias and optimizers are those of %r" % (edge, owner, owner))
+        return names[i]
 
     def set_optimizer(self, edge, weights=None, bias=None):
         """replace the settings of the weight and / or bias optimizer of `edge` (index or name) with the optimizer block
@@ -446,7 +467,7 @@ def model_text(model):
 def model_initial_weights(model, edge, seed=42):
     """the initial weights (a list of floats, without the bias) of edge `edge` of a model under RNG seed `seed`
     (host-only; the net seeds edge i with its seed + 17 i), or a PRETRAINED edge's weights from its checkpoint; None for
-    an edge without parameters"""
+    an edge without parameters of its own (a tied edge starts from its owner's)"""
     H = load_host()
     n = H.cnb_model_initial_weights(model.encode(), edge, seed, None, 0)
     if n == -1:
@@ -456,6 +477,21 @@ def model_initial_weights(model, edge, seed=42):
     buf = (ct.c_float * n)()
     H.cnb_model_initial_weights(model.encode(), edge, seed, buf, n)
     return list(buf)
+
+
+def model_ties(model):
+    """the tied edges of a model (host-only): {tied edge name: the name of the edge whose parameters it uses}"""
+    H, out, i = load_host(), {}, 0
+    while True:
+        name, owner = ct.create_string_buffer(256), ct.create_string_buffer(256)
+        rc = H.cnb_model_tie(model.encode(), i, name, owner)
+        if rc == -1:
+            raise ValueError("cannot build model %r (see stderr)" % model)
+        if rc == -2:
+            return out
+        if rc == 1:
+            out[name.value.decode()] = owner.value.decode()
+        i += 1
 
 
 def model_polyak(model):

@@ -80,6 +80,12 @@ void convnet_b200_fuse_next_dropout(float dropprob, float scale, unsigned long l
  * convDown finds the banks ready instead of rebuilding them on the critical path. */
 void convnet_b200_prestage_next(void);
 
+/* How many times the bf16 dgrad filter banks have been built since the library was loaded: in_prestage 0 counts the
+ * builds inside a convDown* call (on its critical path), 1 those made for a convnet_b200_prestage_next request.  The
+ * banks are cached per filter tensor and call geometry, so a filter tensor that several calls use at different strides,
+ * paddings or image sizes keeps one set per geometry; any write to the filters drops them all. */
+unsigned long long convnet_b200_dgrad_bank_builds(int in_prestage);
+
 /* The conv kernels are persistent: one CTA per SM, each owning most of the SM's shared memory.  A kernel
  * of another library that must run CONCURRENTLY (an NCCL collective on a side stream) cannot co-reside with them and
  * would otherwise wait for — or push out — a whole wave.  convnet_b200_reserve_sms(n) makes the persistent grids leave

@@ -11,9 +11,9 @@
 //   dgrad : D[(n,pixel), c]  = sum_{tap,o}  der[n, module(pixel,tap), o] * w[o, tap, c]    A MN-major, B K-major
 //   wgrad : D[o, c] (per tap)= sum_{module,n} der[n, module, o] * img[n, x, y, c]          A K-major,  B K-major
 //
-// One persistent CTA per SM, 12 warps: warps 0..7 are two consumer warpgroups (GEMM rows 0-63 and 64-127 of the 128 x 128
-// tile), warp 8 is the TMA producer filling a ring of shared-memory stages guarded by mbarriers, warps 9..11 store the
-// fprop / dgrad output tiles.
+// One persistent CTA per SM, 12 or 16 warps: warps 0..7 are two consumer warpgroups (GEMM rows 0-63 and 64-127 of the
+// 128 x 128 tile), warp 8 is the TMA producer filling a ring of shared-memory stages guarded by mbarriers, the SW = 3
+// or 7 warps after it store the fprop / dgrad output tiles (the launch plan picks SW: pick_store_warps).
 //   bf16 operands: wgmma.mma_async m64n128k16 reads both operands from the swizzled tiles (either major);
 //   tf32 operands: wgmma takes 32-bit operands from shared memory only K-major, so
 //     wgrad (both operands K-major): wgmma m64n128k8 on the tiles, as bf16;
@@ -38,8 +38,8 @@ namespace cnb {
 namespace {
 
 constexpr int kConsumerWarps = 8;
-constexpr int kStoreWarps = 3;
-constexpr int kThreads = 32 * (kConsumerWarps + 1 + kStoreWarps);   // 384: ptxas caps a thread at 168 registers
+// Threads of a CTA with SW store warps: 384 (ptxas caps a thread at 168 registers) or 512 (128 registers)
+template <int SW> constexpr int kThreadsFor = 32 * (kConsumerWarps + 1 + SW);
 constexpr int BM = 128;             // GEMM rows per tile
 constexpr int BN_MAX = 128;         // GEMM columns per tile (the wgmma N); narrower tiles leave the extra columns unstored
 constexpr int BK = 32;              // fp32 (tf32) elements of K per pipeline stage (4 MMA steps of 8); x-mode constant
@@ -313,15 +313,19 @@ __device__ __forceinline__ float4 ldg4(const float* a, bool vec) {
   return make_float4(__ldg(a), __ldg(a + 1), __ldg(a + 2), __ldg(a + 3));
 }
 
-// Store warp `sw` (0..2) of the CTA: for each of the CTA's tiles, wait until the consumers have staged it, then write
-// columns sw, sw + 3, ... Lane l holds rows 4l .. 4l+3, four consecutive images of one chunk: with N % 4 == 0 they are
-// all valid or all not.  Each element gets exactly the arithmetic of the in-register epilogue it replaces.  The loads an
-// element's store depends on (old target, ReLU' mask, bias) are issued ahead of the stores they would otherwise wait
-// behind, since a store may alias a later load as far as the compiler knows: the bias once per tile, the old target and
-// the mask one batch of kEpiCols columns ahead.
-template <int OP, bool SIG>
+// Store warp `sw` (0..SW-1) of the CTA: for each of the CTA's tiles, wait until the consumers have staged it, then write
+// columns sw, sw + SW, ... (a warp with no column, when the tile has fewer than SW, only releases the tile).  Lane l
+// holds rows 4l .. 4l+3, four consecutive images of one chunk: with N % 4 == 0 they are all valid or all not.  Each
+// element gets exactly the arithmetic of the in-register epilogue it replaces.  The loads an element's store depends on
+// (old target, ReLU' mask, bias) are issued ahead of the stores they would otherwise wait behind, since a store may
+// alias a later load as far as the compiler knows: the bias once per tile, the old target and the mask one batch of
+// kEpiCols columns ahead.
+template <int OP, bool SIG, int SW>
 __device__ __forceinline__ void store_tiles(const TcParams& p, SmemCtl* ctl, uint32_t stg, int sw, int lane) {
-  constexpr int kEpiCols = SIG ? 4 : 8;            // the logistic arithmetic needs the registers of half the batch
+  constexpr int kStoreWarps = SW;
+  // columns per batch.  Three warps: 8 (4 in the logistic instances, whose arithmetic needs the registers of half the
+  // batch); seven: 4, which fits their 128 registers
+  constexpr int kEpiCols = (SW == 3 && !SIG) ? 8 : 4;
   const bool vec = p.vec != 0;
   const int lr = 4 * lane;                          // this lane's first row
   const int per_frame = (OP == kFprop) ? p.modules : p.W * p.H;
@@ -361,11 +365,12 @@ __device__ __forceinline__ void store_tiles(const TcParams& p, SmemCtl* ctl, uin
     // l-th and (l+32)-th column, and a batch takes them by shuffle.  A bias load inside a batch would wait a full
     // memory round trip behind the previous batch's stores, which the compiler must assume may alias it.
     static_assert(BN_MAX <= 64 * kStoreWarps, "two bias values per lane cover a store warp's columns");
+    constexpr bool kBiasHi = BN_MAX > 32 * kStoreWarps;   // seven warps: at most 19 columns, one value per lane
     float bias_lo = 0.f, bias_hi = 0.f;
     if (OP == kFprop && bias) {
       const int ca = sw + kStoreWarps * lane, cb = ca + kStoreWarps * 32;
       if (ca < ncols) bias_lo = __ldg(bias + ca * bias_step);
-      if (cb < ncols) bias_hi = __ldg(bias + cb * bias_step);
+      if (kBiasHi && cb < ncols) bias_hi = __ldg(bias + cb * bias_step);
     }
     // the loads a batch's arithmetic depends on (old target, ReLU' mask), software-pipelined: batch b+1's are issued
     // after batch b's arithmetic and before its stores, and batch 0's before the wait for the tile.  Issued after the
@@ -401,9 +406,9 @@ __device__ __forceinline__ void store_tiles(const TcParams& p, SmemCtl* ctl, uin
       }
       if (OP == kFprop && bias) {
 #pragma unroll
-        for (int k = 0; k < kEpiCols; k++) {          // column c0 + 3k is this warp's (kEpiCols b + k)-th
+        for (int k = 0; k < kEpiCols; k++) {          // column c0 + SW k is this warp's (kEpiCols b + k)-th
           const int j = kEpiCols * b + k;
-          bv[k] = __shfl_sync(0xffffffffu, j < 32 ? bias_lo : bias_hi, j & 31);
+          bv[k] = __shfl_sync(0xffffffffu, (kBiasHi && j >= 32) ? bias_hi : bias_lo, j & 31);
         }
       }
       if (row < 0) continue;
@@ -467,8 +472,8 @@ __device__ __forceinline__ void store_tiles(const TcParams& p, SmemCtl* ctl, uin
 // ------------------------------------------------------------------------------------------------
 // SIG: the epilogue applies the activation code (logistic included); the other instances know only ReLU / ReLU', so the
 // logistic arithmetic costs the ReLU and linear layers nothing
-template <int OP, bool BF16, bool SIG>
-__global__ void __launch_bounds__(kThreads, 1)
+template <int OP, bool BF16, bool SIG, int SW>
+__global__ void __launch_bounds__(kThreadsFor<SW>, 1)
 tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const __grid_constant__ TcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -483,7 +488,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; s++) { ptx::mbar_init(&ctl->full[s], 1); ptx::mbar_init(&ctl->empty[s], kConsumerWarps); }
     ptx::mbar_init(&ctl->epi_full, kConsumerWarps);
-    ptx::mbar_init(&ctl->epi_empty, kStoreWarps);
+    ptx::mbar_init(&ctl->epi_empty, SW);
     ptx::fence_barrier_init();
     ptx::tma_prefetch_desc(&mapA);
     ptx::tma_prefetch_desc(&mapB);
@@ -494,7 +499,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
 
   if (warp > kConsumerWarps) {
     // =============================== store warps (fprop / dgrad) ===============================
-    if constexpr (OP != kWgrad) store_tiles<OP, SIG>(p, ctl, ptx::smem_u32(smemE), warp - kConsumerWarps - 1, lane);
+    if constexpr (OP != kWgrad) store_tiles<OP, SIG, SW>(p, ctl, ptx::smem_u32(smemE), warp - kConsumerWarps - 1, lane);
     return;
   }
   if (warp == kConsumerWarps) {
@@ -898,17 +903,31 @@ int pick_stages(uint32_t bank_bytes, uint32_t epi_bytes) {
   return s;
 }
 
-template <int OP, bool BF16, bool SIG>
+// Store warps of an fprop / dgrad launch.  A CTA writes its tiles about as fast as it has warps storing them: on an
+// H100, conv1's fprop drains its 595 MB in 0.83 ms with 3 store warps and in 0.53 ms with 7, while sending the same
+// stores to a few L2-resident lines, or laying each tile out contiguously, gains far less (DESIGN.md §6).  But
+// MMA-bound tiles run 3-5 % slower beside 7 store warps (conv4 fprop; not because 512 threads cap a thread at 128
+// registers: the 3-warp kernel built at that cap is as fast as before).  So a plan takes 7 when its tiles are bound by
+// their epilogue, or nearly so: when writing a tile's `tile_bytes` takes at least half as long as its `kblocks`
+// k-blocks take to multiply.  Times in microseconds, coarse, as in the wgrad split model: one k-block ~0.3 us, the
+// tile's traffic at an H100 SM's share of ~3 TB/s (~23 KB/us).
+int pick_store_warps(int kblocks, double tile_bytes) {
+  const double mma_us = 0.3 * kblocks;
+  const double epi_us = tile_bytes / (3e6 / 132);
+  return 2.0 * epi_us >= mma_us ? 7 : 3;
+}
+
+template <int OP, bool BF16, bool SIG, int SW>
 void launch_one(const CUtensorMap& a, const CUtensorMap& b, const TcParams& p, size_t smem) {
   // the attribute belongs to the (function, device) pair: set it once per device this process launches on
   static unsigned long long attr_devices = 0;
   const int dev = current_device();
   if (dev >= 64 || !((attr_devices >> dev) & 1ULL)) {
-    CNB_CUDA_CHECK(cudaFuncSetAttribute(tc_conv_kernel<OP, BF16, SIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    CNB_CUDA_CHECK(cudaFuncSetAttribute(tc_conv_kernel<OP, BF16, SIG, SW>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     if (dev < 64) attr_devices |= 1ULL << dev;
   }
   const int grid = std::min(p.num_tiles, num_sms());
-  launch_pdl(tc_conv_kernel<OP, BF16, SIG>, dim3((unsigned)grid), dim3(kThreads), smem, state().stream, a, b, p);
+  launch_pdl(tc_conv_kernel<OP, BF16, SIG, SW>, dim3((unsigned)grid), dim3(kThreadsFor<SW>), smem, state().stream, a, b, p);
 }
 
 template <int OP>
@@ -922,10 +941,20 @@ void launch(const CUtensorMap& a, const CUtensorMap& b, TcParams& p) {
   const bool sig = p.act == kActLogistic || (p.mask && p.mask_act == kActLogistic);
   CNB_REQUIRE(OP != kWgrad || !sig, "tc_conv: wgrad has no activation epilogue");
   void (*run)(const CUtensorMap&, const CUtensorMap&, const TcParams&, size_t) = nullptr;
-  if constexpr (OP != kWgrad) {                       // (no SIG instance of the wgrad kernel exists)
-    if (sig) run = p.bf16 ? launch_one<OP, true, true> : launch_one<OP, false, true>;
+  // wgrad has no SIG instance, and stores from the MMA warps: its 3 store warps exit at once
+  if constexpr (OP != kWgrad) {
+    // k-blocks of a full tile (dgrad: every tap live), and the bytes its store warps move
+    const int kcb = p.splits > 1 ? p.units_per_split : p.kc_blocks;
+    const int kblocks = (OP == kFprop && p.x_mode) ? p.Cin * p.x_yblocks : p.taps * kcb;
+    const double bytes = BM * p.BN * (4.0 + (p.out16 ? 2 : 0) + (p.mask ? 4 : 0) + (p.st != 0.f && p.splits == 1 ? 4 : 0));
+    if (pick_store_warps(kblocks, bytes) == 7) {
+      if (sig) run = p.bf16 ? launch_one<OP, true, true, 7> : launch_one<OP, false, true, 7>;
+      else run = p.bf16 ? launch_one<OP, true, false, 7> : launch_one<OP, false, false, 7>;
+    } else if (sig) {
+      run = p.bf16 ? launch_one<OP, true, true, 3> : launch_one<OP, false, true, 3>;
+    }
   }
-  if (!run) run = p.bf16 ? launch_one<OP, true, false> : launch_one<OP, false, false>;
+  if (!run) run = p.bf16 ? launch_one<OP, true, false, 3> : launch_one<OP, false, false, 3>;
   run(a, b, p, smem);
   count_launch();
   CNB_LAUNCH_CHECK("tc_conv");

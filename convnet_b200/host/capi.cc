@@ -79,6 +79,8 @@ API float* cnb_net_layer_deriv(void* p, int i) { return ((NetHandle*)p)->net->La
 API long long cnb_net_layer_floats(void* p, int i) { return (long long)((NetHandle*)p)->net->Layers()[i]->GetState().GetNumEls(); }
 API int cnb_net_num_layers(void* p) { return (int)((NetHandle*)p)->net->Layers().size(); }
 API float* cnb_net_device_loss(void* p) { return ((NetHandle*)p)->net->DeviceLoss(); }
+// the seed of the dropout mask the next training-mode Fprop draws for layer i (0: the layer has no dropout)
+API unsigned long long cnb_net_dropout_seed(void* p, int i) { return ((NetHandle*)p)->net->NextDropoutSeed((size_t)i); }
 
 API void cnb_net_fprop(void* p, int train) { ((NetHandle*)p)->net->Fprop(train != 0); }
 API void cnb_net_bprop(void* p) { ((NetHandle*)p)->net->ComputeDeriv(); ((NetHandle*)p)->net->Bprop(); }

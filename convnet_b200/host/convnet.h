@@ -267,6 +267,10 @@ class ConvNet {
   void Load(const std::string& path);
   ModelConfig CurrentModel() const;                             // the model with the optimizer settings now in force
   unsigned long long Iteration() const { return step_; }        // TrainOneBatch calls so far (the dropout step)
+  // the keep-mask seed the next training Fprop gives layer i; 0 for a layer without dropout
+  unsigned long long NextDropoutSeed(size_t i) const {
+    return layers_[i]->HasDropout() ? layers_[i]->DropoutSeed(step_, dropout_salt_) : 0;
+  }
   // Polyak queue on the device, allocated at the first insert: polyak_queue_size slots and a backup of the parameters.
   // std::invalid_argument: Polyak is off, nothing inserted, no backup; std::runtime_error: the allocation failed
   void InsertPolyak();                                          // parameters -> next slot (device copy, no host wait)

@@ -100,6 +100,7 @@ def load_host():
             "cnb_net_edge_tied_to": ([vp, i], ct.c_char_p),
             "cnb_net_layer_deriv": ([vp, i], vp),
             "cnb_model_tie": ([ct.c_char_p, i, ct.c_char_p, ct.c_char_p], i),
+            "cnb_net_dropout_seed": ([vp, i], ct.c_ulonglong),
         }
         for name, (args, res) in sig.items():
             fn = getattr(H, name)
@@ -217,6 +218,11 @@ class Net:
         the input layer"""
         ptr = self.H.cnb_net_layer_deriv(self.h, i)
         return self._view(ptr, self.H.cnb_net_layer_floats(self.h, i), "f") if ptr else None
+
+    def dropout_seed(self, i):
+        """the seed of the keep mask the next training step draws for layer i (element k of the state is kept when
+        float32(hash(seed + k)) * 2^-32 >= dropprob, csrc/common.cuh); 0 for a layer without dropout"""
+        return self.H.cnb_net_dropout_seed(self.h, i)
 
     # --- compute
     def fprop(self, train=False):

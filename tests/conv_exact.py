@@ -74,6 +74,34 @@ def model(x, kind):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# dispatch mirror: the operand model of the path a call takes (conv_tc.cu tc_conv_*_impl and abi.cu), for whole,
+# 16-byte-aligned 2-D operands whose filters have a staged bf16 copy (the training host keeps one for every edge that may
+# take a bf16 path), which lets an FC-shaped fprop / dgrad take bf16.
+# ---------------------------------------------------------------------------------------------------------------------
+PATH_MODEL = {"cuda-core-fp32": "fp32", "tc-tf32": "tf32", "tc-bf16": "bf16"}
+
+
+def conv_path(op, g, mode):
+    """'cuda-core-fp32', 'tc-tf32' or 'tc-bf16': the path of a conv call in precision `mode`"""
+    x_mode = g.Cin * g.kt < 8
+    rows = g.N * g.modX * g.modY * g.modT
+    if mode == "fp32" or (x_mode and (g.kx > 8 or g.ky > 8)):
+        return "cuda-core-fp32"
+    if op == "fprop":
+        tc = g.N % 4 == 0 and g.Cout % 4 == 0
+        bf = not x_mode and g.N % 8 == 0 and g.Cout % 8 == 0
+    elif op == "dgrad":
+        tc = g.N % 4 == 0 and g.Cout % 4 == 0 and g.Cout >= 8 and g.Cin >= 8 and g.kx <= 32 and g.ky <= 32
+        bf = g.N % 8 == 0 and g.Cout % 8 == 0
+    else:
+        tc = g.N % 4 == 0 and g.Cout >= 8
+        bf = not x_mode and g.N % 8 == 0 and (rows >= 1024 or (g.T == 1 and g.N % 128 == 0 and g.Cin % 32 == 0))
+    if not tc:
+        return "cuda-core-fp32"
+    return "tc-bf16" if mode == "bf16" and bf else "tc-tf32"
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # geometry of one call
 # ---------------------------------------------------------------------------------------------------------------------
 @dataclasses.dataclass

@@ -506,6 +506,21 @@ def pool_undo_branch(g, is_max, aligned=True, mask=None, st=0.0, cached=False):
     return Branch("undo_generic<%d,%s,Q%d>" % (v, kind, Q), "pool_undo_kernel<%d, %s, %d>" % (v, mx, Q), False, 0)
 
 
+def bias_depth(branch, g):
+    """(values one thread adds, slices colsum_finish adds) of the bias-gradient sum of an undo branch"""
+    v = 4 if branch.name.split("<")[1].startswith("4") else 1
+    NV = g.N // v
+    if branch.slices and "patch" in branch.name:
+        PX = (g.W - 1 + g.px) // 2 + 1
+        return -(-NV * PX // 256) * 4 * v, branch.slices
+    if branch.slices:
+        return -(-NV * g.W // 256) * v, branch.slices
+    rows = g.N * g.W * g.H * g.T
+    slices = max(1, min(64, (4 * SMS) // g.C))
+    slices = min(slices, max(1, rows // 1024))
+    return -(-(-(-rows // slices)) // 256), slices
+
+
 def pick_tile(F, arrays):
     sm = 224 * 1024
     for per_sm in (3, 2, 1):

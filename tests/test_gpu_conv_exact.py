@@ -23,7 +23,6 @@ pytestmark = pytest.mark.gpu
 SENTINEL = 0x7FC0DEAD      # NaN bits of the guard zones and of targets the call must not read
 GUARD = 64                 # floats of guard zone after each target
 OFFSETS = (32, 36)         # target offsets in floats: 128-byte aligned, and 16-byte but not 128-byte aligned
-PATH_MODEL = {"cuda-core-fp32": "fp32", "tc-tf32": "tf32", "tc-bf16": "bf16"}
 WORST = {}                 # (op, path precision) -> largest |err|/S seen, printed at the end of the module
 
 
@@ -186,7 +185,7 @@ def run(env, c, mode, offset=OFFSETS[0], reserve=0, controls=True):
     tag = "%s[%s] %s" % (c.name, mode, c.branch)
     assert _sentinel_ok(buf[:offset]) and _sentinel_ok(buf[offset + n:]), tag + ": wrote outside its target"
     kw = dict(t0=t0, st=c.st, so=c.so, bias=bias, relu="relu" in fuse, mask=mask, drop=fuse.get("drop"))
-    kind = PATH_MODEL[path]
+    kind = cx.PATH_MODEL[path]
     v = cx.check(op, g, y, cx.expect(op, g, a.storage, b.storage, kind, **kw), t0=t0)
     key = (op, kind)
     WORST[key] = max(WORST.get(key, 0.0), v.worst_ratio)

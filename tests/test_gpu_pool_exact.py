@@ -277,21 +277,6 @@ def _pool_undo_call(env, c, u, x, gr, acts, tgt, mask, bias, bias_so):
         b.AvgPoolUndo(gr, tgt, c.g.desc(), u.st)
 
 
-def bias_depth(branch, g):
-    """(values one thread adds, slices colsum_finish adds) of the bias-gradient sum of an undo branch"""
-    v = 4 if branch.name.split("<")[1].startswith("4") else 1
-    NV = g.N // v
-    if branch.slices and "patch" in branch.name:
-        PX = (g.W - 1 + g.px) // 2 + 1
-        return -(-NV * PX // 256) * 4 * v, branch.slices
-    if branch.slices:
-        return -(-NV * g.W // 256) * v, branch.slices
-    rows = g.N * g.W * g.H * g.T
-    slices = max(1, min(64, (4 * px.SMS) // g.C))
-    slices = min(slices, max(1, rows // 1024))
-    return -(-(-(-rows // slices)) // 256), slices
-
-
 def run_pool(env, c, inputs=None, check=True):
     """forward + undos of case c; returns the launched-branch bookkeeping for the kernel-name test"""
     g = c.g
@@ -365,7 +350,7 @@ def run_pool(env, c, inputs=None, check=True):
             print("%-50s %s" % (tag, v))
             assert v.ok, "%s: %s" % (tag, v)
             if bias is not None:
-                per_thread, slices = bias_depth(ub, g)
+                per_thread, slices = px.bias_depth(ub, g)
                 eb = px.bias_grad(tgt.storage, g.N * g.W * g.H, g.C, 1, b0, u.bias_st, bias_so, per_thread, slices,
                                   exact_arm=exact_arm)
                 vb = px.check(bias, eb)

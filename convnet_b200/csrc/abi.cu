@@ -128,13 +128,63 @@ void do_conv_outp(const char* what, cudamat* images, cudamat* derivs, cudamat* t
   conv_outp(g, images->data_device, derivs->data_device, targets->data_device, st, so);
 }
 
+// What an average-pool call (AvgPool*, DownSample*) or average undo (AvgPoolUndo*, UpSample*) honours of a request, as the
+// PoolEpi its kernel applies: the forward activation and dropout, the dropout fold (scale) and the ReLU' mask.  sigma and
+// sigma' are passes after the kernel (`late_act`, `late_state`), as for the other pool calls: the scale still rides in the
+// kernel, the mask, the forward dropout and a fused bias gradient then follow as passes.
+struct AvgRequest {
+  PoolEpi epi;
+  bool late_act = false, late_state = false;
+  AvgRequest(const Fuse& f, const float* relu_mask) {
+    const int act = f.act_state ? kActNone : f.act;   // (a request with a state is the derivative's)
+    late_act = act == kActLogistic;
+    late_state = f.state_act == kActLogistic;
+    epi.relu = act == kActRelu;
+    if (!late_act) { epi.drop_prob = f.drop_prob; epi.drop_scale = f.drop_scale; epi.drop_seed = f.drop_seed; }
+    epi.scale = f.out_scale;
+    epi.mask = relu_mask;
+  }
+  bool late() const { return late_act || late_state; }
+};
+// the epilogue a kernel could not apply, as the stand-alone passes in the order the kernels apply it (bit-identical)
+void epi_passes(float* t, long long n, const PoolEpi& e) {
+  if (e.relu) cnb_relu(t, n);
+  if (e.drop_scale != 0.f) dropout_apply(t, n, e.drop_prob, e.drop_scale, e.drop_seed, nullptr);
+  if (e.scale != 1.f) scale_buffer(t, n, e.scale);
+  if (e.mask) cnb_relu_deriv(t, e.mask, n);
+}
+// sigma / sigma' and the dropout that follows sigma
+void late_passes(float* t, long long n, const Fuse& f, const AvgRequest& r) {
+  if (r.late_act) {
+    cnb_logistic(t, n);
+    if (f.drop_scale != 0.f) dropout_apply(t, n, f.drop_prob, f.drop_scale, f.drop_seed, nullptr);
+  }
+  if (r.late_state) cnb_logistic_deriv(t, f.act_state, n);
+}
+
 void do_pool(const char* what, bool is_max, cudamat* images, cudamat* targets, Shape4D* is, Shape4D* ts, ConvDesc d,
              float so) {
   Range nvtx_range(what);
   PoolGeom g = pool_geom(*is, *ts, images, targets, d, what);
   const Fuse fuse = take_fuse();
-  Emit emit(targets->data_device, (long long)targets->size[0] * targets->size[1], fuse.emit_bf16 != 0);
-  emit.done = pool_forward(g, is_max, images->data_device, targets->data_device, so, emit.buf, fuse.pool_cache != 0);
+  const long long n = (long long)targets->size[0] * targets->size[1];
+  Emit emit(targets->data_device, n, fuse.emit_bf16 != 0);
+  if (is_max) {
+    emit.done = pool_forward(g, is_max, images->data_device, targets->data_device, so, emit.buf, fuse.pool_cache != 0);
+    emit.finish();
+    return;
+  }
+  AvgRequest r(fuse, fuse.relu_mask());
+  const bool late = r.late();
+  float* part = fuse.bias_grad && !late && g.T == 1 ? (float*)workspace(sizeof(float) * (size_t)(g.modY + 2) * g.C * g.modT) : nullptr;
+  r.epi.rowsum = part;
+  bool epi_done = false;
+  int slices = 0;
+  emit.done = pool_forward(g, false, images->data_device, targets->data_device, so, late ? nullptr : emit.buf, false, r.epi,
+                           &epi_done, &slices);
+  if (r.epi.any() && !epi_done) { epi_passes(targets->data_device, n, r.epi); emit.done = false; slices = 0; }
+  late_passes(targets->data_device, n, fuse, r);
+  finish_bias_grad(fuse, part, slices, targets->data_device, (long long)g.N * g.modX * g.modY * g.modT, g.C);
   emit.finish();
 }
 void do_max_undo(const char* what, cudamat* images, cudamat* maxGrads, cudamat* maxActs, cudamat* targets,
@@ -162,12 +212,17 @@ void do_avg_undo(const char* what, cudamat* avgGrads, cudamat* targets, Shape4D*
   const Fuse fuse = take_fuse();
   const long long n = (long long)targets->size[0] * targets->size[1];
   Emit emit(targets->data_device, n, fuse.emit_bf16 != 0);
-  const bool late = fuse.state_act == kActLogistic;
+  AvgRequest r(fuse, fuse.relu_mask());
+  const bool late = r.late();
   int slices = 0;
   float* part = fuse.bias_grad ? (float*)workspace(sizeof(float) * (size_t)(g.H + 2) * g.C * g.T) : nullptr;
-  emit.done = avg_pool_undo(g, avgGrads->data_device, targets->data_device, st, so, fuse.relu_mask(), late ? nullptr : emit.buf,
-                            g.T == 1 && !late ? part : nullptr, &slices);
-  if (late) cnb_logistic_deriv(targets->data_device, fuse.act_state, n);
+  bool epi_done = false;
+  PoolEpi epi = r.epi;
+  epi.mask = nullptr;                                // (the kernels take the mask as relu_mask)
+  emit.done = avg_pool_undo(g, avgGrads->data_device, targets->data_device, st, so, r.epi.mask, late ? nullptr : emit.buf,
+                            g.T == 1 && !late ? part : nullptr, &slices, epi, &epi_done);
+  if (epi.any() && !epi_done) { epi_passes(targets->data_device, n, r.epi); emit.done = false; slices = 0; }
+  late_passes(targets->data_device, n, fuse, r);
   finish_bias_grad(fuse, part, slices, targets->data_device, (long long)g.N * g.W * g.H * g.T, g.C);
   emit.finish();
 }

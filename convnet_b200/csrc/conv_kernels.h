@@ -72,17 +72,35 @@ struct Emit {
 };
 
 // pool.cu
-// targets_bf16 (may be null): also write the bf16 twin of the target; the return value says whether the kernel did
+// The epilogue an average-pool kernel applies to each result (after scaleOutput, and after scaleTargets * old for an undo),
+// in this order: relu: max(., 0); dropout (drop_scale != 0): times the keep value of cnb_dropout at the element's index;
+// times `scale`; then zeroed where mask[i] <= 0 (forward kernel: `mask`; undo: its relu_mask argument).  rowsum (forward
+// kernel): per-(row, plane) sums of the stored values, as the undo's colsum.  The default is no epilogue.
+struct PoolEpi {
+  int relu = 0;
+  float drop_prob = 0.f, drop_scale = 0.f; unsigned long long drop_seed = 0;
+  float scale = 1.f;
+  const float* mask = nullptr;
+  float* rowsum = nullptr;
+  bool any() const { return relu || drop_scale != 0.f || scale != 1.f || mask || rowsum; }
+};
+// targets_bf16 (may be null): also write the bf16 twin of the target; the return value says whether the kernel did.
+// epi (average pooling only): *epi_done says whether the kernel applied it (else the caller runs it as passes); with a
+// rowsum, *colsum_slices is the number of row slices the kernel summed
 bool pool_forward(const PoolGeom& g, bool is_max, const float* images, float* targets, float scaleOutput,
-                  __nv_bfloat16* targets_bf16 = nullptr, bool cache_masks = false);
+                  __nv_bfloat16* targets_bf16 = nullptr, bool cache_masks = false, const PoolEpi& epi = PoolEpi(),
+                  bool* epi_done = nullptr, int* colsum_slices = nullptr);
 // colsum / colsum_slices (may be null): where a kernel that can do so leaves per-slice channel sums of the tensor it wrote,
 // colsum[slice * channels + c] (*colsum_slices = number of slices, 0 = not done) — the bias gradient of the edge below
 bool max_pool_undo(const PoolGeom& g, const float* images, const float* maxGrads, const float* maxActs,
                    float* targets, float scaleTargets, float scaleOutput, const float* relu_mask,
                    __nv_bfloat16* targets_bf16 = nullptr, float* colsum = nullptr, int* colsum_slices = nullptr);
+// epi: its relu / dropout / scale steps (mask and rowsum are relu_mask and colsum); *epi_done as for pool_forward.  When
+// the kernel cannot apply them it applies none of relu_mask, colsum and the bf16 twin either (the caller's passes do)
 bool avg_pool_undo(const PoolGeom& g, const float* avgGrads, float* targets, float scaleTargets,
                    float scaleOutput, const float* relu_mask, __nv_bfloat16* targets_bf16 = nullptr,
-                   float* colsum = nullptr, int* colsum_slices = nullptr);
+                   float* colsum = nullptr, int* colsum_slices = nullptr, const PoolEpi& epi = PoolEpi(),
+                   bool* epi_done = nullptr);
 // max-pool R-operator: targets = st * targets + sum of R_images over the window elements equal to the stored maximum
 void max_pool_rprop(const PoolGeom& g, const float* images, const float* R_images, const float* maxes, float* targets, float st);
 // grad_bias[c] = st*grad_bias[c] + so * sum_slices part[slice*cols + c]   (elementwise.cu)

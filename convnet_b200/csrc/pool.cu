@@ -209,6 +209,33 @@ __global__ void __launch_bounds__(256) pool_undo_kernel(PoolGeom g, const float*
 // once per block iteration from blockIdx (uniform), the stride is a template constant (S = 0: run time), the image
 // index is a shift when N/VEC is a power of two, and per-thread offsets are 32-bit.
 template <int S> __device__ __forceinline__ int div_s(int a, int s) { return S > 0 ? a / S : a / s; }
+
+// the epilogue of PoolEpi on VEC results whose first element has index `i` in the target tensor, in the order of the
+// stand-alone passes it replaces: cnb_relu, the dropout of cnb_dropout (mask-free, element index i), cnb_mult by a
+// constant.  Each step is the pass's own single rounding, so the results are bit-identical to those passes.
+template <int VEC>
+__device__ __forceinline__ void epilogue(const PoolEpi& e, float (&acc)[VEC], long long i) {
+#pragma unroll
+  for (int v = 0; v < VEC; v++) {
+    float x = acc[v];
+    if (e.relu) x = fmaxf(x, 0.f);
+    if (e.drop_scale != 0.f) x *= dropout_keep(e.drop_seed + (unsigned long long)(i + v), e.drop_prob, e.drop_scale);
+    if (e.scale != 1.f) x *= e.scale;
+    acc[v] = x;
+  }
+}
+// deterministic block sum of `total` -> rowsum[blockIdx.x][plane] (256 threads)
+__device__ __forceinline__ void block_rowsum(float total, float* rowsum) {
+  __shared__ float sh[8];
+  for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = total;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int w = 0; w < 8; w++) s += sh[w];
+    rowsum[(size_t)blockIdx.x * gridDim.y + blockIdx.y] = s;
+  }
+}
 template <int S>
 __device__ __forceinline__ void cover_s(int X, int s, int p, int k, int mods, int& lo, int& hi) {
   const int a = X - p - k + 1;
@@ -217,11 +244,11 @@ __device__ __forceinline__ void cover_s(int X, int s, int p, int k, int mods, in
   hi = b < 0 ? -1 : min(div_s<S>(b, s), mods - 1);
 }
 
-template <int VEC, bool MAX, int K, int S>
-__global__ void __launch_bounds__(256) pool_fwd_rows_kernel(PoolGeom g, const float* __restrict__ images,
-                                                             float* __restrict__ targets, float so, int nv_shift,
-                                                             __nv_bfloat16* __restrict__ targets16,
-                                                             uint16_t* __restrict__ tie_masks) {
+// EPI: the epilogue of PoolEpi after the scaled average (average pooling only; EPI == false is the plain kernel)
+template <int VEC, bool MAX, int K, int S, bool EPI>
+__device__ __forceinline__ void pool_fwd_rows(PoolGeom g, const float* __restrict__ images, float* __restrict__ targets,
+                                              float so, int nv_shift, __nv_bfloat16* __restrict__ targets16,
+                                              uint16_t* __restrict__ tie_masks, const PoolEpi& epi) {
   pdl_wait();
   pdl_trigger();
   const unsigned NV = g.N / VEC;
@@ -231,6 +258,9 @@ __global__ void __launch_bounds__(256) pool_fwd_rows_kernel(PoolGeom g, const fl
   float* out = targets + (long long)g.N * g.modX * g.modY * blockIdx.y;
   __nv_bfloat16* out16 = targets16 ? targets16 + (long long)g.N * g.modX * g.modY * blockIdx.y : nullptr;
   uint16_t* outm = (MAX && tie_masks) ? tie_masks + (long long)g.N * g.modX * g.modY * blockIdx.y : nullptr;
+  const long long out_plane = (long long)g.N * g.modX * g.modY * blockIdx.y;
+  const float* mk_p = EPI && epi.mask ? epi.mask + out_plane : nullptr;
+  float total = 0.f;
   for (int my = blockIdx.x; my < g.modY; my += gridDim.x) {
     const int Y0 = my * sy + g.py;
     for (unsigned t = threadIdx.x; t < rowlen; t += blockDim.x) {
@@ -277,19 +307,48 @@ __global__ void __launch_bounds__(256) pool_fwd_rows_kernel(PoolGeom g, const fl
       }
 #pragma unroll
       for (int v = 0; v < VEC; v++) acc[v] = so * acc[v];
-      vstore<VEC>(out + (unsigned)(my * rowlen + t) * VEC, acc);
-      if (out16) vemit<VEC>(out16 + (unsigned)(my * rowlen + t) * VEC, acc);
+      const unsigned o = (unsigned)(my * rowlen + t) * VEC;
+      if constexpr (EPI) {
+        epilogue<VEC>(epi, acc, out_plane + o);
+        if (mk_p) {
+          float mk[VEC];
+          vload<VEC>(mk_p + o, mk);
+#pragma unroll
+          for (int v = 0; v < VEC; v++) acc[v] = mk[v] > 0.f ? acc[v] : 0.f;
+        }
+        if (epi.rowsum) {
+#pragma unroll
+          for (int v = 0; v < VEC; v++) total += acc[v];
+        }
+      }
+      vstore<VEC>(out + o, acc);
+      if (out16) vemit<VEC>(out16 + o, acc);
     }
   }
+  if (EPI && epi.rowsum) block_rowsum(total, epi.rowsum);
+}
+template <int VEC, bool MAX, int K, int S>
+__global__ void __launch_bounds__(256) pool_fwd_rows_kernel(PoolGeom g, const float* __restrict__ images,
+                                                             float* __restrict__ targets, float so, int nv_shift,
+                                                             __nv_bfloat16* __restrict__ targets16,
+                                                             uint16_t* __restrict__ tie_masks) {
+  pool_fwd_rows<VEC, MAX, K, S, false>(g, images, targets, so, nv_shift, targets16, tie_masks, PoolEpi());
+}
+// average pooling with the epilogue of PoolEpi (the sampling calls' fused requests)
+template <int VEC, int K, int S>
+__global__ void __launch_bounds__(256) pool_fwd_rows_epi_kernel(PoolGeom g, const float* __restrict__ images,
+                                                                 float* __restrict__ targets, float so, int nv_shift,
+                                                                 __nv_bfloat16* __restrict__ targets16, PoolEpi epi) {
+  pool_fwd_rows<VEC, false, K, S, true>(g, images, targets, so, nv_shift, targets16, nullptr, epi);
 }
 
-template <int VEC, bool MAX, int Q, int S>
-__global__ void __launch_bounds__(256) pool_undo_rows_kernel(PoolGeom g, const float* __restrict__ images,
-                                                              const float* __restrict__ grads,
-                                                              const float* __restrict__ acts, float* targets,
-                                                              float st, float so, const float* __restrict__ relu_mask,
-                                                              int nv_shift, __nv_bfloat16* __restrict__ targets16,
-                                                              float* __restrict__ rowsum) {
+// EPI: the relu / dropout / scale steps of PoolEpi before the ReLU' mask (average undo only; EPI == false: the plain kernel)
+template <int VEC, bool MAX, int Q, int S, bool EPI>
+__device__ __forceinline__ void pool_undo_rows(PoolGeom g, const float* __restrict__ images, const float* __restrict__ grads,
+                                               const float* __restrict__ acts, float* targets, float st, float so,
+                                               const float* __restrict__ relu_mask, int nv_shift,
+                                               __nv_bfloat16* __restrict__ targets16, float* __restrict__ rowsum,
+                                               const PoolEpi& epi) {
   pdl_wait();
   pdl_trigger();
   const unsigned NV = g.N / VEC;
@@ -350,6 +409,7 @@ __global__ void __launch_bounds__(256) pool_undo_rows_kernel(PoolGeom g, const f
           }
 #pragma unroll
       for (int v = 0; v < VEC; v++) acc[v] += st * old[v];
+      if constexpr (EPI) epilogue<VEC>(epi, acc, in_plane + idx);
       if (relu_mask) {                         // fused ApplyDerivativeOfActivation of the layer receiving this derivative
         float mk[VEC];
         if (mask_is_input) {
@@ -378,6 +438,24 @@ __global__ void __launch_bounds__(256) pool_undo_rows_kernel(PoolGeom g, const f
       rowsum[(size_t)blockIdx.x * gridDim.y + blockIdx.y] = s;
     }
   }
+}
+
+template <int VEC, bool MAX, int Q, int S>
+__global__ void __launch_bounds__(256) pool_undo_rows_kernel(PoolGeom g, const float* __restrict__ images,
+                                                              const float* __restrict__ grads,
+                                                              const float* __restrict__ acts, float* targets,
+                                                              float st, float so, const float* __restrict__ relu_mask,
+                                                              int nv_shift, __nv_bfloat16* __restrict__ targets16,
+                                                              float* __restrict__ rowsum) {
+  pool_undo_rows<VEC, MAX, Q, S, false>(g, images, grads, acts, targets, st, so, relu_mask, nv_shift, targets16, rowsum, PoolEpi());
+}
+// average undo with the relu / dropout / scale steps of PoolEpi (the sampling calls' fused requests)
+template <int VEC, int Q, int S>
+__global__ void __launch_bounds__(256) pool_undo_rows_epi_kernel(PoolGeom g, const float* __restrict__ grads, float* targets,
+                                                                  float st, float so, const float* __restrict__ relu_mask,
+                                                                  int nv_shift, __nv_bfloat16* __restrict__ targets16,
+                                                                  float* __restrict__ rowsum, PoolEpi epi) {
+  pool_undo_rows<VEC, false, Q, S, true>(g, nullptr, grads, nullptr, targets, st, so, relu_mask, nv_shift, targets16, rowsum, epi);
 }
 
 // max-pool undo from the tie masks the forward kernel recorded (convnet_b200_pool_cache_next), stride 2, windows up to
@@ -602,7 +680,7 @@ static bool patch_geometry(const PoolGeom& g) {
 
 template <int VEC, bool MAX>
 static bool launch_fwd(const PoolGeom& g, const float* images, float* targets, float so, long long total, __nv_bfloat16* t16,
-                       uint16_t* masks) {
+                       uint16_t* masks, const PoolEpi& epi, bool* epi_done, int* colsum_slices) {
   cudaStream_t s = state().stream;
   const int planes = g.C * g.modT;
   const long long per_plane = total / planes;
@@ -614,7 +692,14 @@ static bool launch_fwd(const PoolGeom& g, const float* images, float* targets, f
     const dim3 rgrid((unsigned)g.modY, planes);
     const int sh = pow2_shift(g.N / VEC);
     const int S = (g.sx == g.sy && g.sx <= 2) ? g.sx : 0;
-#define CNB_POOL_FWD(KK, SS) launch_pdl(pool_fwd_rows_kernel<VEC, MAX, KK, SS>, rgrid, dim3(256), 0, s, g, images, targets, so, sh, t16, masks)
+    const bool e = !MAX && epi.any();
+    if (e && epi_done) *epi_done = true;
+    if (e && epi.rowsum && colsum_slices) *colsum_slices = g.modY;
+#define CNB_POOL_FWD(KK, SS)                                                                                                  \
+  do {                                                                                                                        \
+    if (e) launch_pdl(pool_fwd_rows_epi_kernel<VEC, KK, SS>, rgrid, dim3(256), 0, s, g, images, targets, so, sh, t16, epi); \
+    else launch_pdl(pool_fwd_rows_kernel<VEC, MAX, KK, SS>, rgrid, dim3(256), 0, s, g, images, targets, so, sh, t16, masks); \
+  } while (0)
     if (k <= 2) { if (S == 1) CNB_POOL_FWD(2, 1); else if (S == 2) CNB_POOL_FWD(2, 2); else CNB_POOL_FWD(2, 0); }
     else { if (S == 1) CNB_POOL_FWD(3, 1); else if (S == 2) CNB_POOL_FWD(3, 2); else CNB_POOL_FWD(3, 0); }
 #undef CNB_POOL_FWD
@@ -628,8 +713,10 @@ static bool launch_fwd(const PoolGeom& g, const float* images, float* targets, f
 }
 
 bool pool_forward(const PoolGeom& g, bool is_max, const float* images, float* targets, float so, __nv_bfloat16* targets_bf16,
-                  bool cache_masks) {
-  const bool v4 = (g.N % 4 == 0) && aligned16(images) && aligned16(targets);
+                  bool cache_masks, const PoolEpi& epi, bool* epi_done, int* colsum_slices) {
+  if (epi_done) *epi_done = false;
+  if (colsum_slices) *colsum_slices = 0;
+  const bool v4 = (g.N % 4 == 0) && aligned16(images) && aligned16(targets) && (!epi.mask || aligned16(epi.mask));
   const long long outs = (long long)g.modX * g.modY * g.C * g.modT;
   // tie masks for the matching undo: unscaled outputs only
   uint16_t* masks = nullptr;
@@ -637,11 +724,11 @@ bool pool_forward(const PoolGeom& g, bool is_max, const float* images, float* ta
     masks = pool_masks_slot(targets, outs * g.N, images, (long long)g.N * g.W * g.H * g.C, pool_sig(g));
   bool emitted;
   if (v4) {
-    if (is_max) emitted = launch_fwd<4, true>(g, images, targets, so, outs * (g.N / 4), targets_bf16, masks);
-    else emitted = launch_fwd<4, false>(g, images, targets, so, outs * (g.N / 4), targets_bf16, nullptr);
+    if (is_max) emitted = launch_fwd<4, true>(g, images, targets, so, outs * (g.N / 4), targets_bf16, masks, epi, epi_done, colsum_slices);
+    else emitted = launch_fwd<4, false>(g, images, targets, so, outs * (g.N / 4), targets_bf16, nullptr, epi, epi_done, colsum_slices);
   } else {
-    if (is_max) emitted = launch_fwd<1, true>(g, images, targets, so, outs * g.N, targets_bf16, masks);
-    else emitted = launch_fwd<1, false>(g, images, targets, so, outs * g.N, targets_bf16, nullptr);
+    if (is_max) emitted = launch_fwd<1, true>(g, images, targets, so, outs * g.N, targets_bf16, masks, epi, epi_done, colsum_slices);
+    else emitted = launch_fwd<1, false>(g, images, targets, so, outs * g.N, targets_bf16, nullptr, epi, epi_done, colsum_slices);
   }
   count_launch();
   CNB_LAUNCH_CHECK("pool_forward");
@@ -709,7 +796,7 @@ template <int VEC, bool MAX>
 // colsum (may be null): on return *colsum_slices > 0 iff the kernel wrote per-(row, plane) sums of its output to `colsum`
 static bool launch_undo(const PoolGeom& g, const float* images, const float* grads, const float* acts, float* targets,
                         float st, float so, long long total, const float* mask, __nv_bfloat16* t16, float* colsum,
-                        int* colsum_slices) {
+                        int* colsum_slices, const PoolEpi& epi, bool* epi_done) {
   cudaStream_t s = state().stream;
   const int planes = g.C * g.T;
   const long long per_plane = total / planes;
@@ -740,11 +827,21 @@ static bool launch_undo(const PoolGeom& g, const float* images, const float* gra
       return t16 != nullptr;
     }
     if (colsum && colsum_slices) *colsum_slices = g.H;
-#define CNB_POOL_UNDO(QQ, SS) pool_undo_rows_kernel<VEC, MAX, QQ, SS><<<rgrid, 256, 0, s>>>(g, images, grads, acts, targets, st, so, mask, sh, t16, colsum)
+    const bool e = !MAX && epi.any();
+    if (e && epi_done) *epi_done = true;
+#define CNB_POOL_UNDO(QQ, SS)                                                                                                 \
+  do {                                                                                                                        \
+    if (e) pool_undo_rows_epi_kernel<VEC, QQ, SS><<<rgrid, 256, 0, s>>>(g, grads, targets, st, so, mask, sh, t16, colsum, epi); \
+    else pool_undo_rows_kernel<VEC, MAX, QQ, SS><<<rgrid, 256, 0, s>>>(g, images, grads, acts, targets, st, so, mask, sh, t16, colsum); \
+  } while (0)
     if (q <= 1) { if (S == 1) CNB_POOL_UNDO(1, 1); else if (S == 2) CNB_POOL_UNDO(1, 2); else CNB_POOL_UNDO(1, 0); }
     else { if (S == 1) CNB_POOL_UNDO(2, 1); else if (S == 2) CNB_POOL_UNDO(2, 2); else CNB_POOL_UNDO(2, 0); }
 #undef CNB_POOL_UNDO
     return t16 != nullptr;
+  }
+  if (!MAX && epi.any()) {                         // the epilogue runs as passes after this kernel: so must the mask
+    mask = nullptr;
+    t16 = nullptr;
   }
   if (q <= 1) pool_undo_kernel<VEC, MAX, 1><<<grid, 256, 0, s>>>(g, images, grads, acts, targets, st, so, total, mask);
   else if (q == 2) pool_undo_kernel<VEC, MAX, 2><<<grid, 256, 0, s>>>(g, images, grads, acts, targets, st, so, total, mask);
@@ -753,17 +850,19 @@ static bool launch_undo(const PoolGeom& g, const float* images, const float* gra
 }
 
 static bool undo(const PoolGeom& g, bool is_max, const float* images, const float* grads, const float* acts,
-                 float* targets, float st, float so, const float* mask, __nv_bfloat16* t16, float* colsum, int* colsum_slices) {
+                 float* targets, float st, float so, const float* mask, __nv_bfloat16* t16, float* colsum, int* colsum_slices,
+                 const PoolEpi& epi = PoolEpi(), bool* epi_done = nullptr) {
+  if (epi_done) *epi_done = false;
   const bool v4 = (g.N % 4 == 0) && aligned16(grads) && aligned16(targets) && (!mask || aligned16(mask)) &&
                   (!is_max || (aligned16(images) && aligned16(acts)));
   const long long ins = (long long)g.W * g.H * g.C * g.T;
   bool emitted;
   if (v4) {
-    if (is_max) emitted = launch_undo<4, true>(g, images, grads, acts, targets, st, so, ins * (g.N / 4), mask, t16, colsum, colsum_slices);
-    else emitted = launch_undo<4, false>(g, images, grads, acts, targets, st, so, ins * (g.N / 4), mask, t16, colsum, colsum_slices);
+    if (is_max) emitted = launch_undo<4, true>(g, images, grads, acts, targets, st, so, ins * (g.N / 4), mask, t16, colsum, colsum_slices, epi, epi_done);
+    else emitted = launch_undo<4, false>(g, images, grads, acts, targets, st, so, ins * (g.N / 4), mask, t16, colsum, colsum_slices, epi, epi_done);
   } else {
-    if (is_max) emitted = launch_undo<1, true>(g, images, grads, acts, targets, st, so, ins * g.N, mask, t16, colsum, colsum_slices);
-    else emitted = launch_undo<1, false>(g, images, grads, acts, targets, st, so, ins * g.N, mask, t16, colsum, colsum_slices);
+    if (is_max) emitted = launch_undo<1, true>(g, images, grads, acts, targets, st, so, ins * g.N, mask, t16, colsum, colsum_slices, epi, epi_done);
+    else emitted = launch_undo<1, false>(g, images, grads, acts, targets, st, so, ins * g.N, mask, t16, colsum, colsum_slices, epi, epi_done);
   }
   count_launch();
   CNB_LAUNCH_CHECK("pool_undo");
@@ -777,8 +876,8 @@ bool max_pool_undo(const PoolGeom& g, const float* images, const float* maxGrads
 }
 
 bool avg_pool_undo(const PoolGeom& g, const float* avgGrads, float* targets, float st, float so, const float* relu_mask,
-                   __nv_bfloat16* targets_bf16, float* colsum, int* colsum_slices) {
-  return undo(g, false, nullptr, avgGrads, nullptr, targets, st, so, relu_mask, targets_bf16, colsum, colsum_slices);
+                   __nv_bfloat16* targets_bf16, float* colsum, int* colsum_slices, const PoolEpi& epi, bool* epi_done) {
+  return undo(g, false, nullptr, avgGrads, nullptr, targets, st, so, relu_mask, targets_bf16, colsum, colsum_slices, epi, epi_done);
 }
 
 }  // namespace cnb

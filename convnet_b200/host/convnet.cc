@@ -41,7 +41,7 @@ void Layer::AllocateMemory(int batch_size) {               // layer.cc:228-262 (
   const int cols = image_size_y_ * image_size_x_ * image_size_t_ * config_.num_channels;
   state_.AllocateGPUMemory(batch_size, cols);
   state_.SetShape4D(batch_size, image_size_x_, image_size_y_, config_.num_channels * image_size_t_);
-  if (!config_.is_input) {
+  if (ReceivesDeriv()) {
     deriv_.AllocateGPUMemory(batch_size, cols);
     deriv_.SetShape4D(batch_size, image_size_x_, image_size_y_, config_.num_channels * image_size_t_);
   }
@@ -78,6 +78,30 @@ std::string EdgeShapeError(const Edge& e, int source_channels, int dest_channels
   return "";
 }
 
+std::string SampleEdgeError(const Edge& e, int source_channels, int dest_channels, bool on_input, bool into_output) {
+  const EdgeType t = e.Config().edge_type;
+  if (t != UPSAMPLE && t != DOWNSAMPLE && t != RGBTOYUV) return "";
+  const std::string name = kEdgeTypeNames[t], f = std::to_string(e.Config().sample_factor);
+  if (t != RGBTOYUV && e.Config().sample_factor < 1) return "field 'sample_factor': " + f + " is below 1";
+  if (source_channels != dest_channels)
+    return "field 'edge_type': " + name + " keeps the channel count, but the source layer has " +
+           std::to_string(source_channels) + " channels and the destination " + std::to_string(dest_channels);
+  const int y = e.GetImageSizeY(), x = e.GetImageSizeX();
+  if (t == DOWNSAMPLE && (y % e.Config().sample_factor || x % e.Config().sample_factor))
+    return "field 'sample_factor': DOWNSAMPLE by " + f + " needs image sizes divisible by " + f + ", and the source layer is " +
+           std::to_string(y) + " x " + std::to_string(x);
+  if (t == RGBTOYUV) {
+    if (!on_input) return "field 'edge_type': RGBTOYUV runs only on the input layer's outgoing edge (it has no backward pass)";
+    if (source_channels != 3)
+      return "field 'edge_type': RGBTOYUV maps 3 colour channels to 3, and the layers have " + std::to_string(source_channels);
+    if (e.GetImageSizeT() != 1) return "field 'edge_type': RGBTOYUV is not supported on 3-D layers (image_size_t > 1)";
+    if (into_output)
+      return "field 'edge_type': RGBTOYUV cannot write the output layer (the layer it writes receives no derivative, and the "
+             "loss needs one)";
+  }
+  return "";
+}
+
 std::string TieError(const std::vector<const Edge*>& edges, size_t i) {
   const EdgeConfig& c = edges[i]->Config();
   if (c.tied_to.empty()) return "";
@@ -89,9 +113,9 @@ std::string TieError(const std::vector<const Edge*>& edges, size_t i) {
   const EdgeConfig& o = edges[k]->Config();
   if (!o.tied_to.empty()) return f + owner + " is itself tied (to '" + o.tied_to + "'): tie to '" + o.tied_to + "' instead";
   if (edges[k]->HasNoParameters()) return f + owner + " has no parameters";
-  static const char* const types[] = {"FC", "CONVOLUTIONAL", "MAXPOOL", "AVERAGE_POOL", "RESPONSE_NORM", "CONV_ONETOONE", "LOCAL"};
   if (o.edge_type != c.edge_type)
-    return f + owner + " is " + types[o.edge_type] + ", this edge " + types[c.edge_type] + " (a tie joins edges of one edge_type)";
+    return f + owner + " is " + kEdgeTypeNames[o.edge_type] + ", this edge " + kEdgeTypeNames[c.edge_type] +
+           " (a tie joins edges of one edge_type)";
   const EdgeWithWeight *w = dynamic_cast<const EdgeWithWeight*>(edges[i]), *ow = dynamic_cast<const EdgeWithWeight*>(edges[k]);
   auto shape = [](const Shape4D& s) {
     return "(" + std::to_string(s.shape[0]) + ", " + std::to_string(s.shape[1]) + ", " + std::to_string(s.shape[2]) + ", " +
@@ -358,6 +382,8 @@ ConvNet::ConvNet(const ModelConfig& model, int batch_size) : model_(model), batc
   }
   const std::string why = Refusal();
   if (!why.empty()) throw std::invalid_argument(why);
+  for (size_t i = 0; i < edges_.size(); i++)
+    if (model.edge[i].edge_type == RGBTOYUV) layers_[i + 1]->SetNoDeriv();
   ResolveTies();
   PlanFusion();
 }
@@ -393,6 +419,10 @@ std::string ConvNet::Refusal() const {
   std::vector<const Edge*> chain;
   for (const auto& e : edges_) chain.push_back(e.get());
   for (size_t i = 0; i < edges_.size(); i++) {
+    const std::string sample =
+        SampleEdgeError(*edges_[i], layers_[i]->GetNumChannels(), layers_[i + 1]->GetNumChannels(), layers_[i]->IsInput(),
+                        layers_[i + 1]->IsOutput());
+    if (!sample.empty()) return "edge '" + edges_[i]->GetName() + "': " + sample;
     const std::string shape = EdgeShapeError(*edges_[i], layers_[i]->GetNumChannels(), layers_[i + 1]->GetNumChannels());
     if (!shape.empty()) return "edge '" + edges_[i]->GetName() + "': " + shape;
     const std::string tie = TieError(chain, i);
@@ -412,6 +442,7 @@ std::string ConvNet::Refusal() const {
     if (!l->BatchNormalize()) continue;
     std::string why;
     if (l->IsInput() || l->IsOutput()) why = "is not supported on the input or output layer";
+    else if (model_.edge[i - 1].edge_type == RGBTOYUV) why = "is not supported on the layer RGBTOYUV writes (it receives no derivative)";
     else if (l->GetSizeT() > 1) why = "is not supported on 3-D layers (image_size_t > 1)";
     for (int which = 0; which < 2 && why.empty(); which++)
       if (const char* err = BnOptimizerConfigError(which ? model_.layer[i].beta_optimizer : model_.layer[i].gamma_optimizer))
@@ -436,7 +467,7 @@ void ConvNet::PlanFusion() {
     const Edge::Absorbs a = e->CanAbsorb();
     // the activation of a layer rides where the kernel applies ReLU, and sigma only where it can apply sigma too
     auto fused = [&a](int act, bool can) { return act != CNB_ACT_LINEAR && can && (act == CNB_ACT_RELU || a.logistic); };
-    const int up = ActCode(dst->GetActivation()), down = src->IsInput() ? CNB_ACT_LINEAR : ActCode(src->GetActivation());
+    const int up = ActCode(dst->GetActivation()), down = src->ReceivesDeriv() ? ActCode(src->GetActivation()) : CNB_ACT_LINEAR;
     Edge::FusionPlan p;
     // a batch-normalised layer: the edge writes the pre-normalisation input, the BN pass applies the activation
     if (!dst->BatchNormalize() && fused(up, a.act_up)) p.up_act = up;
@@ -666,7 +697,7 @@ void ConvNet::Bprop() {                                      // convnet.cc:390-4
     // the derivative of `out` is final once its passes have run (the reference runs them at the top of the NEXT loop
     // iteration, i.e. before this layer's edges); batch normalisation also produces the gamma / beta gradients before the
     // ComputeOuter below, which makes this edge's bucket final
-    if (!out->IsOutput()) {
+    if (!out->IsOutput() && out->ReceivesDeriv()) {
       const bool want = bf16 && e->WantsBf16Deriv();
       const bool drop = dropout_pass(i);
       const Writer last = LastDerivWriter(*out, drop);
@@ -692,7 +723,7 @@ void ConvNet::Bprop() {                                      // convnet.cc:390-4
         if (trace_.on) HOST_CUDA_CHECK(cudaEventRecord(trace_.c1[bi], comm_));
         comm_pending_ = true;
       }
-    if (!in->IsInput()) {
+    if (in->ReceivesDeriv()) {
       const bool last = LastDerivWriter(*in, dropout_pass(i - 1)) == Writer::EDGE;
       EdgeWithWeight* below = i >= 2 ? dynamic_cast<EdgeWithWeight*>(edges_[i - 2].get()) : nullptr;
       Edge::DownRequest r;

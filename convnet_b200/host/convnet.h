@@ -57,6 +57,13 @@ std::string LayerConfigError(const LayerConfig& c);
 // its destination at least one module in y, x and t, a pooling or response-norm edge keeps the channel count, and a
 // convolution has no temporal padding (the 3-D kernels fold the frames into channels); else why not
 std::string EdgeShapeError(const Edge& e, int source_channels, int dest_channels);
+// "" if `e` is not an UPSAMPLE, DOWNSAMPLE or RGBTOYUV edge, or (SetImageSize has run) can run between layers of
+// `source_channels` and `dest_channels`, its source being the input layer when `on_input` and its destination the output
+// layer when `into_output`; else why not, starting with the field it objects to ("field 'sample_factor': " or
+// "field 'edge_type': ").  A factor is at least 1, the three keep the channel count, a DOWNSAMPLE's image size is divisible
+// by its factor, and RGBTOYUV maps the 3 channels of a 2-D input layer to a hidden layer (the layer it writes receives no
+// derivative, and an output layer needs one for its loss)
+std::string SampleEdgeError(const Edge& e, int source_channels, int dest_channels, bool on_input, bool into_output);
 // "" if edge `i` of a chain (every edge's SetImageSize has run) is untied, or may run with and train the parameters of the
 // edge its tied_to names; else why not, starting with "field 'tied_to': ".  The owner must exist, be another edge, be
 // untied itself, have parameters of the same edge_type and the same weight and bias shapes, and sum its bias gradient on
@@ -162,6 +169,10 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   float* GetMetricPerImage() { return metric_per_image_.GetDevData(); }
   float LossWeight() const { return config_.loss_function_weight; }
   bool IsInput() const { return config_.is_input; }
+  // back-propagation writes a derivative for this layer: not the input layer, nor the layer an RGBTOYUV edge writes (it
+  // has no backward pass; ConvNet::SetNoDeriv).  A layer without one has no derivative buffer and runs no derivative pass
+  bool ReceivesDeriv() const { return !config_.is_input && !no_deriv_; }
+  void SetNoDeriv() { no_deriv_ = true; }
   bool IsOutput() const { return config_.is_output; }
   int GetNumChannels() const { return config_.num_channels; }
   int GetSizeY() const { return image_size_y_; }
@@ -195,6 +206,7 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   bool bn_train_ = false;                       // the last ApplyBatchNormalization used the batch statistics
   int* labels_ = nullptr;
   bool activation_fused_ = false, deriv_fused_ = false;
+  bool no_deriv_ = false;
 };
 
 // NCCL all-reduce of the flat gradient buffer, bucketed along edge boundaries and launched on a side
@@ -393,6 +405,8 @@ ModelConfig BuildLeNet();       // examples/mnist-conv/net.pbtxt
 ModelConfig BuildC3D();         // SURVEY.md §8(d) cfg4
 ModelConfig BuildTinyNet();     // small conv+pool+rnorm+1x1+fc net for tests / grad check
 ModelConfig BuildLogCheckNet(); // the gradcheck net with logistic hidden units
+ModelConfig BuildUpDownNet();   // encoder-decoder with RGBTOYUV, DOWNSAMPLE and UPSAMPLE edges (bench size)
+ModelConfig BuildUpDownCheckNet();  // run_grad_check net for the sampling edges
 // a built-in name, a path ending in ".pbtxt" (ReadModelFile), either with suffixes ("+bn", "+rmsprop", ...).
 // std::invalid_argument: unknown name, unreadable or refused file
 ModelConfig BuildModel(const std::string& name);

@@ -9,6 +9,9 @@
 
 namespace cnbhost {
 
+const char* const kEdgeTypeNames[RGBTOYUV + 1] = {"FC", "CONVOLUTIONAL", "MAXPOOL", "AVERAGE_POOL", "RESPONSE_NORM",
+                                                 "CONV_ONETOONE", "LOCAL", "UPSAMPLE", "DOWNSAMPLE", "RGBTOYUV"};
+
 // ---------------------------------------------------------------- Edge (src/edge.cc)
 Edge::Edge(const EdgeConfig& c)
     : config_(c), name_(c.name.empty() ? c.source + ":" + c.dest : c.name), source_(nullptr), dest_(nullptr),
@@ -24,6 +27,9 @@ Edge* Edge::ChooseEdgeClass(const EdgeConfig& c) {          // src/edge.cc:17-60
     case RESPONSE_NORM: return new ResponseNormEdge(c);
     case CONV_ONETOONE: return new ConvOneToOneEdge(c);
     case LOCAL: return new LocalEdge(c);
+    case UPSAMPLE: return new UpSampleEdge(c);
+    case DOWNSAMPLE: return new DownSampleEdge(c);
+    case RGBTOYUV: return new RgbToYuvEdge(c);
   }
   fprintf(stderr, "Error: Undefined edge type.\n");
   exit(1);
@@ -456,6 +462,63 @@ void ResponseNormEdge::ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& 
     Matrix::ConvResponseNormCrossMapUndo(deriv_output, input, output, deriv_input, num_input_channels_, num_filters_response_norm_, add_scale_, pow_scale_, blocked_);
   else
     Matrix::ConvResponseNormCrossMapUndo3D(deriv_output, input, output, deriv_input, num_input_channels_, num_filters_response_norm_, add_scale_, pow_scale_, blocked_, image_size_t_);
+}
+
+// ---------------------------------------------------------------- UpSampleEdge / DownSampleEdge / RgbToYuvEdge
+ConvDesc SampleEdge::Desc() const {
+  ConvDesc d = Edge::GetConvDesc(config_);
+  d.kernel_size_y = d.kernel_size_x = d.stride_y = d.stride_x = factor_;
+  d.kernel_size_t = d.stride_t = 1;
+  d.padding_y = d.padding_x = d.padding_t = 0;
+  d.num_input_channels = d.num_output_channels = d.input_channel_end = d.output_channel_end = num_input_channels_ * image_size_t_;
+  return d;
+}
+static void NotOverwrite(const char* what) {
+  fprintf(stderr, " In %s : some other layer is writing to this layer. Not implemented.\n", what);
+  exit(1);
+}
+
+void UpSampleEdge::SetImageSize(int y, int x, int t) {        // upsample_edge.cc:17-22
+  Edge::SetImageSize(y, x, t);
+  num_modules_y_ = y * factor_;
+  num_modules_x_ = x * factor_;
+}
+void UpSampleEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) {
+  ArmUp(nullptr, up_req_.emit);
+  UpSampleGemm(input.GetMat(), output.GetMat(), &input.GetShape4D(), &output.GetShape4D(), factor_, overwrite ? 0 : 1);
+}
+// the derivative of replication: the sum over each f x f block
+void UpSampleEdge::ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) {
+  if (!overwrite) NotOverwrite("UpSampleEdge::ComputeDown()");
+  ArmDown(input.GetDevData());
+  AvgPoolGemm(deriv_output.GetMat(), deriv_input.GetMat(), &deriv_output.GetShape4D(), &deriv_input.GetShape4D(), Desc(), 0,
+              (float)(factor_ * factor_));
+}
+
+void DownSampleEdge::SetImageSize(int y, int x, int t) {      // (the reference multiplies here, DESIGN.md §5)
+  Edge::SetImageSize(y, x, t);
+  num_modules_y_ = factor_ > 0 ? y / factor_ : 0;            // (a factor below 1 is refused: SampleEdgeError)
+  num_modules_x_ = factor_ > 0 ? x / factor_ : 0;
+}
+void DownSampleEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) {
+  if (!overwrite) NotOverwrite("DownSampleEdge::ComputeUp()");
+  ArmUp(nullptr, up_req_.emit);
+  DownSampleGemm(input.GetMat(), output.GetMat(), &input.GetShape4D(), &output.GetShape4D(), factor_);
+}
+// the derivative of the block mean: d / f^2 to every element of the block, AvgPoolEdge's call
+void DownSampleEdge::ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) {
+  ArmDown(input.GetDevData());
+  Matrix::ConvAvgPoolUndo(deriv_output, deriv_input, Desc(), overwrite ? 0 : 1);
+}
+
+void RgbToYuvEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) {   // rgbtoyuv_edge.cc
+  if (!overwrite) NotOverwrite("RgbToYuvEdge::ComputeUp()");
+  ArmUp(nullptr, up_req_.emit);
+  Matrix::ConvRGBToYUV(input, output);
+}
+void RgbToYuvEdge::ComputeDown(Matrix&, Matrix&, Matrix&, Matrix&, bool) {
+  fprintf(stderr, "RgbToYuvEdge::ComputeDown: RGBTOYUV has no backward pass\n");
+  exit(1);
 }
 
 }  // namespace cnbhost

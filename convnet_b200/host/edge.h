@@ -8,6 +8,9 @@
 //   FCEdge              src/fc_edge.{h,cc}              (reference: Matrix::Dot / cublasSgemm)
 //   ConvOneToOneEdge    src/conv_onetoone_edge.{h,cc}   (reference: Matrix::Dot / cublasSgemm)
 //   LocalEdge           src/local_edge.{h,cc}           untied conv -> per-feature bias ; wgrad -> bias grad
+//   UpSampleEdge        src/upsample_edge.{h,cc}        UpSampleGemm ; dgrad: the block sum (DESIGN.md §5)
+//   DownSampleEdge      src/downsample_edge.{h,cc}      DownSampleGemm ; dgrad: AvgPoolUndoGemm
+//   RgbToYuvEdge        src/rgbtoyuv_edge.{h,cc}        RGBToYUV ; no backward pass (input layer only)
 // FC and 1x1 edges run on the same implicit-GEMM conv kernels (a 1x1 convolution IS that GEMM),
 // SURVEY.md §8(f) rank 1.  The protobuf `config::Edge` is replaced by the plain EdgeConfig struct
 // (protobuf is not in the image); field names follow proto/convnet_config.proto:120-221.
@@ -21,7 +24,9 @@ namespace cnbhost {
 
 class Layer;
 
-enum EdgeType { FC, CONVOLUTIONAL, MAXPOOL, AVGPOOL, RESPONSE_NORM, CONV_ONETOONE, LOCAL };
+enum EdgeType { FC, CONVOLUTIONAL, MAXPOOL, AVGPOOL, RESPONSE_NORM, CONV_ONETOONE, LOCAL, UPSAMPLE, DOWNSAMPLE, RGBTOYUV };
+// the proto value name of each EdgeType (model files, messages)
+extern const char* const kEdgeTypeNames[RGBTOYUV + 1];
 
 // proto/convnet_config.proto:64-113 Optimizer, the fields of the SGD, Adagrad and RMSProp paths (src/optimizer.cc:174-279),
 // with the proto's names, numbers and defaults.  Plain C layout: the C API (capi.cc) and net.py's ctypes mirror pass it as is.
@@ -80,6 +85,7 @@ struct EdgeConfig {
   float add_scale = 0.0005f, pow_scale = 0.75f, frac_of_filters_response_norm = 0.25f;
   bool response_norm_in_blocks = false;
   float scale_gradients = 1.f;
+  int sample_factor = 1;                     // UPSAMPLE / DOWNSAMPLE: the factor per spatial axis
   // EdgeWithWeight::Initialize (edge_with_weight.cc:108-143).  The built-in models keep the host's defaults (uniform,
   // bias 0); a model file takes the proto's (DENSE_GAUSSIAN_SQRT_FAN_IN, init_wt 1, init_bias 0)
   int initialization = DENSE_UNIFORM_SQRT_FAN_IN;
@@ -121,6 +127,8 @@ class Edge {
   int GetNumModulesY() const { return num_modules_y_; }
   int GetNumModulesX() const { return num_modules_x_; }
   int GetNumModulesT() const { return num_modules_t_; }
+  int GetImageSizeY() const { return image_size_y_; }
+  int GetImageSizeX() const { return image_size_x_; }
   int GetImageSizeT() const { return image_size_t_; }
   void SetInputChannels(int a) { num_input_channels_ = a; }
   void SetOutputChannels(int a) { num_output_channels_ = a; }
@@ -423,6 +431,48 @@ class ResponseNormEdge : public Edge {
   int num_filters_response_norm_;
   bool blocked_;
   float add_scale_, pow_scale_, frac_of_filters_response_norm_;
+};
+
+// UPSAMPLE and DOWNSAMPLE: every pixel replicated into an f x f block, and the mean of each f x f block.  Channels and
+// frames are kept; on a 3-D layer the frames are folded into the Shape4D planes (C * T), so the 2-D calls apply as they
+// are.  The derivatives are the true ones (DESIGN.md §5): the block sum (AvgPoolGemm with scaleOutput f^2) and the mean's
+// derivative d / f^2 (AvgPoolUndoGemm) — the reference's calls are f^2 too small and f^2 too large.
+class SampleEdge : public Edge {
+ public:
+  explicit SampleEdge(const EdgeConfig& c) : Edge(c), factor_(c.sample_factor) {}
+  int Factor() const { return factor_; }
+  Absorbs CanAbsorb() const override {                   // ReLU / ReLU' in the kernels, sigma / sigma' as passes in the call
+    Absorbs a;
+    a.act_up = a.act_down = a.dropout = true;
+    a.sums_bias_below = image_size_t_ == 1;
+    return a;
+  }
+
+ protected:
+  int factor_;
+  ConvDesc Desc() const;                                  // the f x f window with stride f over the C * T planes
+};
+class UpSampleEdge : public SampleEdge {
+ public:
+  explicit UpSampleEdge(const EdgeConfig& c) : SampleEdge(c) {}
+  void SetImageSize(int y, int x, int t) override;
+  void ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) override;
+  void ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) override;
+};
+class DownSampleEdge : public SampleEdge {
+ public:
+  explicit DownSampleEdge(const EdgeConfig& c) : SampleEdge(c) {}
+  void SetImageSize(int y, int x, int t) override;
+  void ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) override;
+  void ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) override;
+};
+// RGB -> YUV of the input layer (3 -> 3 channels, 2-D).  The reference has no backward pass for it, so its destination
+// layer receives no derivative (ConvNet: Layer::ReceivesDeriv) and ComputeDown is never called
+class RgbToYuvEdge : public Edge {
+ public:
+  explicit RgbToYuvEdge(const EdgeConfig& c) : Edge(c) {}
+  void ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) override;
+  void ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& output, Matrix& deriv_input, bool overwrite) override;
 };
 
 }  // namespace cnbhost

@@ -403,8 +403,6 @@ class Parser {
 // ---------------------------------------------------------------- names shared by the reader and the writer
 // host enum -> proto value name
 const char* const kActivationNames[] = {"LINEAR", "RECTIFIED_LINEAR", "SOFTMAX", "LOGISTIC", "SOFTMAX_DIST"};
-const char* const kEdgeTypeNames[] = {"FC", "CONVOLUTIONAL", "MAXPOOL", "AVERAGE_POOL", "RESPONSE_NORM", "CONV_ONETOONE",
-                                      "LOCAL"};
 template <size_t N>
 int HostValue(const char* const (&names)[N], const std::string& name) {
   for (size_t k = 0; k < N; k++) if (name == names[k]) return (int)k;
@@ -434,6 +432,7 @@ const OptField kOptFields[] = {
 
 bool HasParameters(EdgeType t) { return t == FC || t == CONVOLUTIONAL || t == LOCAL || t == CONV_ONETOONE; }
 bool HasConvGeometry(EdgeType t) { return t == CONVOLUTIONAL || t == LOCAL || t == MAXPOOL || t == AVGPOOL; }
+bool IsSampling(EdgeType t) { return t == UPSAMPLE || t == DOWNSAMPLE; }
 
 // ---------------------------------------------------------------- Msg -> ModelConfig
 class Mapper {
@@ -524,11 +523,23 @@ class Mapper {
       e->SetInputChannels(m.layer[k].num_channels);
       e->SetOutputChannels(m.layer[k + 1].num_channels);
       e->SetImageSize(y, x, t);
+      // at the line of the field the message names (sample_factor, else edge_type)
+      const std::string sample = SampleEdgeError(*e, m.layer[k].num_channels, m.layer[k + 1].num_channels, k == 0,
+                                                 k + 2 == chain.size());
+      if (!sample.empty()) {
+        const Msg& em = *at.msg;
+        const char* field = sample.rfind("field 'sample_factor'", 0) == 0 ? "sample_factor" : "edge_type";
+        Fail(em.Has(field) ? *em.Get(field) : at, EdgeName(em), sample);
+      }
       const std::string why = EdgeShapeError(*e, m.layer[k].num_channels, m.layer[k + 1].num_channels);
       if (!why.empty()) Fail(at, EdgeName(*at.msg), why);
       if (check_pretrained_ && m.edge[k].initialization == PRETRAINED && !e->HasNoParameters() && m.edge[k].tied_to.empty())
         CheckPretrained(*at.msg, *dynamic_cast<EdgeWithWeight*>(e), m.edge[k]);
       y = e->GetNumModulesY(); x = e->GetNumModulesX(); t = e->GetNumModulesT();
+      const Msg& dest = *layers[chain[k + 1]]->msg;
+      if (m.edge[k].edge_type == RGBTOYUV && m.layer[k + 1].batch_normalize)
+        Fail(*dest.Get("batch_normalize"), "layer '" + m.layer[k + 1].name + "'",
+             "field 'batch_normalize': not supported on the layer RGBTOYUV writes (it receives no derivative)");
     }
     // ties, once every edge knows its shapes (ConvNet::Refusal runs the same checks), at the line of tied_to
     std::vector<const Edge*> chain_edges;
@@ -717,6 +728,9 @@ class Mapper {
     c.shared_bias = e.Bool("shared_bias", false);
     c.has_no_bias = e.Bool("has_no_bias", false);
     c.scale_gradients = e.Float("scale_gradients", 1.f);
+    c.sample_factor = (int)e.Int("sample_factor", 1);
+    if (IsSampling(c.edge_type) && c.sample_factor < 1)
+      Fail(*e.Get("sample_factor"), where, "field 'sample_factor': " + std::to_string(c.sample_factor) + " is below 1");
     c.response_norm_in_blocks = e.Bool("response_norm_in_blocks", false);
     c.add_scale = e.Float("add_scale", 0.f);
     c.pow_scale = e.Float("pow_scale", 0.f);
@@ -874,6 +888,7 @@ std::string ModelText(const ModelConfig& m) {
       w.Int("padding_x", -d.padding_x);
       w.Int("padding_t", -d.padding_t);
     }
+    if (IsSampling(e.edge_type)) w.Int("sample_factor", e.sample_factor);
     if (e.edge_type == RESPONSE_NORM) {
       w.Flt("add_scale", e.add_scale);
       w.Flt("pow_scale", e.pow_scale);

@@ -170,6 +170,42 @@ ModelConfig BuildLocalCheckNet() {
   return m;
 }
 
+EdgeConfig Sample(EdgeType t, int f) { EdgeConfig e = E(t); e.sample_factor = f; return e; }
+
+// encoder-decoder at bench size: a YUV front end, two 2x down-samplings and two 2x up-samplings between 3x3 convs, and a
+// LINEAR 3-channel output trained on a float target per pixel (SQUARED_ERROR).  128 x 128 inputs; the up-sampled 128-channel
+// layer is the largest tensor (8 MB per image)
+ModelConfig BuildUpDownNet() {
+  ModelConfig m; m.name = "updown";
+  LayerConfig in = L("input", 3); in.is_input = true; in.image_size_y = in.image_size_x = 128;
+  m.layer = {in, L("yuv", 3), L("conv1", 64, RECTIFIED_LINEAR), L("down1", 64), L("conv2", 128, RECTIFIED_LINEAR),
+             L("down2", 128), L("conv3", 256, RECTIFIED_LINEAR), L("up3", 256), L("conv4", 128, RECTIFIED_LINEAR),
+             L("up4", 128), L("conv5", 64, RECTIFIED_LINEAR), L("output", 3)};
+  LayerConfig& out = m.layer.back();
+  out.is_output = true; out.loss_function = SQUARED_ERROR; out.performance_metric = SQUARED_ERROR;
+  m.edge = {E(RGBTOYUV), Conv(3, 1, 1), Sample(DOWNSAMPLE, 2), Conv(3, 1, 1), Sample(DOWNSAMPLE, 2), Conv(3, 1, 1),
+            Sample(UPSAMPLE, 2), Conv(3, 1, 1), Sample(UPSAMPLE, 2), Conv(3, 1, 1), Conv(3, 1, 1)};
+  finish(m);
+  return m;
+}
+
+// run_grad_check net for the sampling edges, smooth like BuildGradCheckNet: down- and up-sampling by 3 and by 2, a conv
+// under every sampling edge, a logistic layer written by an UPSAMPLE (sigma after the up-sampling, sigma' into its block
+// sum as passes) and LINEAR units elsewhere, then an FC into a softmax as in gradcheck: the loss of a per-pixel regression
+// output (SQUARED_ERROR on random targets) is so large that its float32 rounding drowns the finite differences
+ModelConfig BuildUpDownCheckNet() {
+  ModelConfig m; m.name = "updowncheck";
+  LayerConfig in = L("input", 4); in.is_input = true; in.image_size_y = in.image_size_x = 6;
+  m.layer = {in, L("conv1", 8), L("down1", 8), L("conv2", 8), L("up2", 8, LOGISTIC), L("conv3", 6), L("down3", 6),
+             L("conv4", 6), L("up4", 6), L("output", 5, SOFTMAX)};
+  m.layer.back().is_output = true;
+  m.edge = {Conv(3, 1, 1), Sample(DOWNSAMPLE, 3), Conv(3, 1, 1), Sample(UPSAMPLE, 3), Conv(3, 1, 1), Sample(DOWNSAMPLE, 2),
+            Conv(3, 1, 1), Sample(UPSAMPLE, 2), E(FC)};
+  for (EdgeConfig& e : m.edge) { e.grad_check = true; e.grad_check_num_params = 10; e.grad_check_epsilon = {1e-2f, 3e-3f, 1e-3f}; }
+  finish(m);
+  return m;
+}
+
 // weight sharing (EdgeConfig::tied_to) on the training path: one 64 -> 64 3x3 conv runs at three geometries — 32 x 32
 // with padding 1, 16 x 16 after a max-pool, and with stride 2 — so one filter tensor keeps three sets of dgrad banks; and
 // two 256 -> 256 FC edges share weights with the LOWER edge naming the higher one, so the shared slice sits at the tied
@@ -389,6 +425,8 @@ ModelConfig BuildModel(const std::string& name) {
   if (name == "tiny") return BuildTinyNet();
   if (name == "lcnet") return BuildLcNet();
   if (name == "localcheck") return BuildLocalCheckNet();
+  if (name == "updown") return BuildUpDownNet();
+  if (name == "updowncheck") return BuildUpDownCheckNet();
   if (name == "invalid:local3d") return BuildLocal3DNet();     // test-only, refused by ConvNet (see above)
   ModelConfig invalid;
   if (name.rfind("invalid:", 0) == 0 && BuildInvalidOutputNet(name.substr(8), &invalid)) return invalid;

@@ -111,7 +111,7 @@ def load_host():
 
 class Net:
     """A chain ConvNet built natively, from a built-in name ("alexnet" | "lenet" | "c3d" | "tiny" | "lcnet" | "gradcheck" |
-    "logcheck" | "localcheck" | "tiednet" | "tiedcheck") or from a model file: any name ending in ".pbtxt" is the path of a config::Model text proto
+    "logcheck" | "localcheck" | "tiednet" | "tiedcheck" | "updown" | "updowncheck") or from a model file: any name ending in ".pbtxt" is the path of a config::Model text proto
     as the reference writes them (examples/*/net.pbtxt), read with the proto's defaults (model_text() prints any model
     as one).  The file's seed is printed but not used: `seed` decides, for files as for built-ins.  Suffixes compose with
     both ("net.pbtxt+rmsprop"):
@@ -215,7 +215,7 @@ class Net:
 
     def layer_deriv(self, i):
         """the derivative of the loss with respect to layer i's state after bprop, laid out like layer_state(i); None for
-        the input layer"""
+        a layer that receives no derivative: the input layer and the layer an RGBTOYUV edge writes"""
         ptr = self.H.cnb_net_layer_deriv(self.h, i)
         return self._view(ptr, self.H.cnb_net_layer_floats(self.h, i), "f") if ptr else None
 

@@ -49,7 +49,8 @@ void convnet_b200_reset_launch_count(void);
  * kernel), so the separate pass over the derivative disappears; calls that cannot do it run that pass themselves. */
 void convnet_b200_fuse_next_bias_grad(float* grad_bias, float scaleTargets, float scaleOutput);
 
-/* One-shot: the NEXT convDown* call multiplies its result by `scale` (before the relu_mask of convnet_b200_fuse_next).
+/* One-shot: the NEXT convDown* call multiplies its result by `scale` (before the relu_mask of convnet_b200_fuse_next);
+ * so do AvgPool* / DownSample* (after scaleOutput), AvgPoolUndo* and UpSample* (after scaleTargets * old).
  * This is how the derivative of inverted dropout disappears as a pass: for a ReLU layer with dropout the state holds
  * relu(x) * m with m in {0, 1/(1-p)}, so  deriv * m * [state > 0]  (Layer::ApplyDerivativeofDropout followed by
  * ApplyDerivativeOfActivation, src/layer.cc:367-395,562-580)  ==  deriv * 1/(1-p) * [state > 0]. */
@@ -118,6 +119,14 @@ void convnet_b200_fuse_next(const float* bias, int relu, const float* relu_mask)
  * fprop and fuse_next_act(NULL, 1, relu_mask) for the derivative. */
 enum { CNB_ACT_LINEAR = 0, CNB_ACT_RELU = 1, CNB_ACT_LOGISTIC = 2 };
 void convnet_b200_fuse_next_act(const float* bias, int act, const float* act_state);
+/* The average-pool calls (AvgPool*, DownSample*, AvgPoolUndo*, UpSample*) honour, besides convnet_b200_emit_bf16_next:
+ *   act with act_state NULL: the forward activation of the result (max(., 0) in the kernel, sigma a pass in the call),
+ *       then convnet_b200_fuse_next_dropout (mask-free, element i of the target kept iff cnb_dropout keeps it);
+ *   act_state: the derivative of act at act_state, after convnet_b200_fuse_next_scale;
+ *   convnet_b200_fuse_next_bias_grad: the per-channel sums of the stored values (AvgPool* / DownSample* here too).
+ * Every result is bit-identical to the unfused call followed by cnb_relu / cnb_logistic, cnb_dropout, cnb_mult (by a
+ * tensor of `scale`) and cnb_relu_deriv / cnb_logistic_deriv; the bias gradient equals cnb_channel_bias_grad's up to the
+ * order of the fp32 sum.  Shapes the row-structured kernels do not take run the same passes inside the call. */
 
 /* bf16 operand staging (precision mode 2 only; no-ops in the other modes).  In bf16 mode every conv call first rounds
  * its two fp32 operands to bf16 copies.  A caller that knows a tensor stays unchanged across several conv calls

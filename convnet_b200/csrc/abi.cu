@@ -128,38 +128,58 @@ void do_conv_outp(const char* what, cudamat* images, cudamat* derivs, cudamat* t
   conv_outp(g, images->data_device, derivs->data_device, targets->data_device, st, so);
 }
 
-// What an average-pool call (AvgPool*, DownSample*) or average undo (AvgPoolUndo*, UpSample*) honours of a request, as the
-// PoolEpi its kernel applies: the forward activation and dropout, the dropout fold (scale) and the ReLU' mask.  sigma and
-// sigma' are passes after the kernel (`late_act`, `late_state`), as for the other pool calls: the scale still rides in the
-// kernel, the mask, the forward dropout and a fused bias gradient then follow as passes.
-struct AvgRequest {
+// A pool call's request split into the PoolEpi its kernel is asked to fuse and the passes that follow the kernel whatever
+// it did: sigma with the dropout after it (late_act) and sigma' (late_state), which no pool kernel applies.  When a late
+// pass is to change the values, the bf16 twin and the bias-gradient sums wait for it too.  Max pooling honours no
+// activation, dropout or scale request, and its forward pass no derivative or bias-gradient request either.
+// colsum_floats: the workspace the kernel's per-slice channel sums need (0: the call is 3-D and a pass sums them).
+struct PoolRequest {
+  Fuse fuse;                                       // the request as the call honours it
   PoolEpi epi;
   bool late_act = false, late_state = false;
-  AvgRequest(const Fuse& f, const float* relu_mask) {
-    const int act = f.act_state ? kActNone : f.act;   // (a request with a state is the derivative's)
-    late_act = act == kActLogistic;
-    late_state = f.state_act == kActLogistic;
-    epi.relu = act == kActRelu;
-    if (!late_act) { epi.drop_prob = f.drop_prob; epi.drop_scale = f.drop_scale; epi.drop_seed = f.drop_seed; }
-    epi.scale = f.out_scale;
-    epi.mask = relu_mask;
-  }
-  bool late() const { return late_act || late_state; }
 };
-// the epilogue a kernel could not apply, as the stand-alone passes in the order the kernels apply it (bit-identical)
-void epi_passes(float* t, long long n, const PoolEpi& e) {
-  if (e.relu) cnb_relu(t, n);
-  if (e.drop_scale != 0.f) dropout_apply(t, n, e.drop_prob, e.drop_scale, e.drop_seed, nullptr);
-  if (e.scale != 1.f) scale_buffer(t, n, e.scale);
-  if (e.mask) cnb_relu_deriv(t, e.mask, n);
+PoolRequest pool_request(Fuse f, bool is_max, bool undo, __nv_bfloat16* twin, size_t colsum_floats) {
+  if (is_max) {
+    f.act = kActNone; f.drop_scale = 0.f; f.out_scale = 1.f;
+    if (!undo) { f.act_state = nullptr; f.state_act = kActNone; f.bias_grad = nullptr; }
+  }
+  PoolRequest r;
+  const int act = f.act_state ? kActNone : f.act;   // (a request with a state is the derivative's)
+  r.late_act = act == kActLogistic;
+  r.late_state = f.state_act == kActLogistic;
+  r.epi.relu = act == kActRelu;
+  if (!r.late_act) { r.epi.drop_prob = f.drop_prob; r.epi.drop_scale = f.drop_scale; r.epi.drop_seed = f.drop_seed; }
+  r.epi.scale = f.out_scale;
+  r.epi.mask = f.relu_mask();
+  r.epi.cache_masks = f.pool_cache != 0;
+  if (!r.late_act && !r.late_state) {
+    r.epi.twin = twin;
+    if (f.bias_grad && colsum_floats) r.epi.colsum = (float*)workspace(sizeof(float) * colsum_floats);
+  }
+  r.fuse = f;
+  return r;
 }
-// sigma / sigma' and the dropout that follows sigma
-void late_passes(float* t, long long n, const Fuse& f, const AvgRequest& r) {
+// the end of every pool call: the steps and the mask as passes when the kernel applied none of them (the order of
+// PoolEpi, bit-identical), the late passes, the bias gradient of `rows` x `channels` from the kernel's sums or a
+// column-sum pass, and the twin where no kernel wrote it
+void finish_pool(const PoolRequest& r, const PoolOutcome& o, Emit& emit, long long rows, int channels) {
+  float* t = emit.target;
+  const long long n = emit.n;
+  const PoolEpi& e = r.epi;
+  if (!o.fused) {
+    if (e.relu) cnb_relu(t, n);
+    if (e.drop_scale != 0.f) dropout_apply(t, n, e.drop_prob, e.drop_scale, e.drop_seed, nullptr);
+    if (e.scale != 1.f) scale_buffer(t, n, e.scale);
+    if (e.mask) cnb_relu_deriv(t, e.mask, n);
+  }
   if (r.late_act) {
     cnb_logistic(t, n);
-    if (f.drop_scale != 0.f) dropout_apply(t, n, f.drop_prob, f.drop_scale, f.drop_seed, nullptr);
+    if (r.fuse.drop_scale != 0.f) dropout_apply(t, n, r.fuse.drop_prob, r.fuse.drop_scale, r.fuse.drop_seed, nullptr);
   }
-  if (r.late_state) cnb_logistic_deriv(t, f.act_state, n);
+  if (r.late_state) cnb_logistic_deriv(t, r.fuse.act_state, n);
+  finish_bias_grad(r.fuse, e.colsum, o.colsum_slices, t, rows, channels);
+  emit.done = o.emitted;
+  emit.finish();
 }
 
 void do_pool(const char* what, bool is_max, cudamat* images, cudamat* targets, Shape4D* is, Shape4D* ts, ConvDesc d,
@@ -167,64 +187,26 @@ void do_pool(const char* what, bool is_max, cudamat* images, cudamat* targets, S
   Range nvtx_range(what);
   PoolGeom g = pool_geom(*is, *ts, images, targets, d, what);
   const Fuse fuse = take_fuse();
-  const long long n = (long long)targets->size[0] * targets->size[1];
-  Emit emit(targets->data_device, n, fuse.emit_bf16 != 0);
+  Emit emit(targets->data_device, (long long)targets->size[0] * targets->size[1], fuse.emit_bf16 != 0);
+  const PoolRequest r = pool_request(fuse, is_max, false, emit.buf, g.T == 1 ? (size_t)(g.modY + 2) * g.C * g.modT : 0);
+  const PoolOutcome o = pool_forward(g, is_max, images->data_device, targets->data_device, so, r.epi);
+  finish_pool(r, o, emit, (long long)g.N * g.modX * g.modY * g.modT, g.C);
+}
+// is: the shape of the pool input, which the undo writes; images and acts (the pool input and output): max pooling only
+void do_pool_undo(const char* what, bool is_max, cudamat* images, cudamat* grads, cudamat* acts, cudamat* targets,
+                  Shape4D* is, Shape4D* gs, ConvDesc d, float st, float so) {
+  Range nvtx_range(what);
+  PoolGeom g = pool_geom(*is, *gs, targets, grads, d, what);
   if (is_max) {
-    emit.done = pool_forward(g, is_max, images->data_device, targets->data_device, so, emit.buf, fuse.pool_cache != 0);
-    emit.finish();
-    return;
+    CNB_REQUIRE(images->size[0] == g.N && images->size[1] == targets->size[1], what);
+    CNB_REQUIRE(acts->size[0] == g.N && acts->size[1] == grads->size[1], what);
   }
-  AvgRequest r(fuse, fuse.relu_mask());
-  const bool late = r.late();
-  float* part = fuse.bias_grad && !late && g.T == 1 ? (float*)workspace(sizeof(float) * (size_t)(g.modY + 2) * g.C * g.modT) : nullptr;
-  r.epi.rowsum = part;
-  bool epi_done = false;
-  int slices = 0;
-  emit.done = pool_forward(g, false, images->data_device, targets->data_device, so, late ? nullptr : emit.buf, false, r.epi,
-                           &epi_done, &slices);
-  if (r.epi.any() && !epi_done) { epi_passes(targets->data_device, n, r.epi); emit.done = false; slices = 0; }
-  late_passes(targets->data_device, n, fuse, r);
-  finish_bias_grad(fuse, part, slices, targets->data_device, (long long)g.N * g.modX * g.modY * g.modT, g.C);
-  emit.finish();
-}
-void do_max_undo(const char* what, cudamat* images, cudamat* maxGrads, cudamat* maxActs, cudamat* targets,
-                 Shape4D* is, Shape4D* gs, ConvDesc d, float st) {
-  Range nvtx_range(what);
-  PoolGeom g = pool_geom(*is, *gs, images, maxGrads, d, what);
-  CNB_REQUIRE(targets->size[0] == g.N && targets->size[1] == images->size[1], what);
-  CNB_REQUIRE(maxActs->size[0] == g.N && maxActs->size[1] == maxGrads->size[1], what);
   const Fuse fuse = take_fuse();
-  const long long n = (long long)targets->size[0] * targets->size[1];
-  Emit emit(targets->data_device, n, fuse.emit_bf16 != 0);
-  const bool late = fuse.state_act == kActLogistic;   // the undo kernels fuse ReLU' only: sigma' is a pass after them
-  int slices = 0;
-  float* part = fuse.bias_grad ? (float*)workspace(sizeof(float) * (size_t)(g.H + 2) * g.C * g.T) : nullptr;
-  emit.done = max_pool_undo(g, images->data_device, maxGrads->data_device, maxActs->data_device, targets->data_device, st,
-                            1.f, fuse.relu_mask(), late ? nullptr : emit.buf, g.T == 1 && !late ? part : nullptr, &slices);
-  if (late) cnb_logistic_deriv(targets->data_device, fuse.act_state, n);
-  finish_bias_grad(fuse, part, slices, targets->data_device, (long long)g.N * g.W * g.H * g.T, g.C);
-  emit.finish();
-}
-void do_avg_undo(const char* what, cudamat* avgGrads, cudamat* targets, Shape4D* gs, Shape4D* ts, ConvDesc d, float st,
-                 float so) {
-  Range nvtx_range(what);
-  PoolGeom g = pool_geom(*ts, *gs, targets, avgGrads, d, what);
-  const Fuse fuse = take_fuse();
-  const long long n = (long long)targets->size[0] * targets->size[1];
-  Emit emit(targets->data_device, n, fuse.emit_bf16 != 0);
-  AvgRequest r(fuse, fuse.relu_mask());
-  const bool late = r.late();
-  int slices = 0;
-  float* part = fuse.bias_grad ? (float*)workspace(sizeof(float) * (size_t)(g.H + 2) * g.C * g.T) : nullptr;
-  bool epi_done = false;
-  PoolEpi epi = r.epi;
-  epi.mask = nullptr;                                // (the kernels take the mask as relu_mask)
-  emit.done = avg_pool_undo(g, avgGrads->data_device, targets->data_device, st, so, r.epi.mask, late ? nullptr : emit.buf,
-                            g.T == 1 && !late ? part : nullptr, &slices, epi, &epi_done);
-  if (epi.any() && !epi_done) { epi_passes(targets->data_device, n, r.epi); emit.done = false; slices = 0; }
-  late_passes(targets->data_device, n, fuse, r);
-  finish_bias_grad(fuse, part, slices, targets->data_device, (long long)g.N * g.W * g.H * g.T, g.C);
-  emit.finish();
+  Emit emit(targets->data_device, (long long)targets->size[0] * targets->size[1], fuse.emit_bf16 != 0);
+  const PoolRequest r = pool_request(fuse, is_max, true, emit.buf, g.T == 1 ? (size_t)(g.H + 2) * g.C * g.T : 0);
+  const PoolOutcome o = pool_undo(g, is_max, is_max ? images->data_device : nullptr, grads->data_device,
+                                  is_max ? acts->data_device : nullptr, targets->data_device, st, so, r.epi);
+  finish_pool(r, o, emit, (long long)g.N * g.W * g.H * g.T, g.C);
 }
 
 ConvDesc sample_desc(Shape4D* is, Shape4D* ts, int factor) {      // gemm.cu:1503-1541
@@ -418,20 +400,20 @@ void AvgPoolGemm(cudamat* images, cudamat* targets, Shape4D* is, Shape4D* ts, Co
 }
 void MaxPoolUndoGemm(cudamat* images, cudamat* maxGrads, cudamat* maxActs, cudamat* targets, Shape4D* is,
                      Shape4D* gs, ConvDesc d, float scaleTargets) {
-  do_max_undo("MaxPoolUndoGemm", images, maxGrads, maxActs, targets, is, gs, d, scaleTargets);
+  do_pool_undo("MaxPoolUndoGemm", true, images, maxGrads, maxActs, targets, is, gs, d, scaleTargets, 1.f);
 }
 void MaxPoolRpropGemm(cudamat* images, cudamat* R_images, cudamat* maxActs, cudamat* targets, Shape4D* is,
                       Shape4D* ms, ConvDesc d, float scaleTargets) {
   do_max_rprop("MaxPoolRpropGemm", images, R_images, maxActs, targets, is, ms, d, scaleTargets);
 }
 void AvgPoolUndoGemm(cudamat* avgGrads, cudamat* targets, Shape4D* gs, Shape4D* ts, ConvDesc d, float scaleTargets) {
-  do_avg_undo("AvgPoolUndoGemm", avgGrads, targets, gs, ts, d, scaleTargets, 1.f);
+  do_pool_undo("AvgPoolUndoGemm", false, nullptr, avgGrads, nullptr, targets, ts, gs, d, scaleTargets, 1.f);
 }
 void UpSampleGemm(cudamat* images, cudamat* targets, Shape4D* is, Shape4D* ts, int factor, float scaleTargets) {
   CNB_REQUIRE(factor >= 1, "UpSampleGemm");
   // up-sampling == avg-pool undo with output scale factor^2 (gemm.cu:1503-1521)
-  do_avg_undo("UpSampleGemm", images, targets, is, ts, sample_desc(ts, is, factor), scaleTargets,
-              (float)(factor * factor));
+  do_pool_undo("UpSampleGemm", false, nullptr, images, nullptr, targets, ts, is, sample_desc(ts, is, factor), scaleTargets,
+               (float)(factor * factor));
 }
 void DownSampleGemm(cudamat* images, cudamat* targets, Shape4D* is, Shape4D* ts, int factor) {
   CNB_REQUIRE(factor >= 1, "DownSampleGemm");
@@ -558,10 +540,10 @@ void AvgPool(cudamat* images, cudamat* targets, Shape4D* is, Shape4D* ts, ConvDe
 }
 void MaxPoolUndo(cudamat* images, cudamat* maxGrads, cudamat* maxActs, cudamat* targets, Shape4D* is, Shape4D* gs,
                  ConvDesc d, float scaleTargets) {
-  do_max_undo("MaxPoolUndo", images, maxGrads, maxActs, targets, is, gs, d, scaleTargets);
+  do_pool_undo("MaxPoolUndo", true, images, maxGrads, maxActs, targets, is, gs, d, scaleTargets, 1.f);
 }
 void AvgPoolUndo(cudamat* avgGrads, cudamat* targets, Shape4D* gs, Shape4D* ts, ConvDesc d, float scaleTargets) {
-  do_avg_undo("AvgPoolUndo", avgGrads, targets, gs, ts, d, scaleTargets, 1.f);
+  do_pool_undo("AvgPoolUndo", false, nullptr, avgGrads, nullptr, targets, ts, gs, d, scaleTargets, 1.f);
 }
 void UpSample(cudamat* images, cudamat* targets, Shape4D* is, Shape4D* ts, int factor, float scaleTargets) {
   UpSampleGemm(images, targets, is, ts, factor, scaleTargets);

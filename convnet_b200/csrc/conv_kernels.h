@@ -72,35 +72,34 @@ struct Emit {
 };
 
 // pool.cu
-// The epilogue an average-pool kernel applies to each result (after scaleOutput, and after scaleTargets * old for an undo),
-// in this order: relu: max(., 0); dropout (drop_scale != 0): times the keep value of cnb_dropout at the element's index;
-// times `scale`; then zeroed where mask[i] <= 0 (forward kernel: `mask`; undo: its relu_mask argument).  rowsum (forward
-// kernel): per-(row, plane) sums of the stored values, as the undo's colsum.  The default is no epilogue.
+// Everything a pool call may fuse into the tensor it writes; the default fuses nothing.  Each result, after scaleOutput
+// (and after scaleTargets * old for an undo), goes through the steps, in the order of the stand-alone passes they replace
+// and bit-identical to them: relu: max(., 0) (cnb_relu); dropout (drop_scale != 0): times the keep value of cnb_dropout at
+// the element's index; times `scale` (cnb_mult); then the ReLU' mask: zeroed where mask[i] <= 0 (cnb_relu_deriv).  The
+// stored values then give colsum[slice * planes + plane], per-(row slice, plane) sums — the bias gradient of the edge
+// below, finished by colsum_finish — and the bf16 twin.  cache_masks (max forward): record the tie masks its undo reads.
+//   - Max pooling takes no steps, and its forward no mask or colsum either (a request that does is refused).
+//   - The row and patch kernels (2-D, windows up to 3 wide, or covered by at most 2 x 2 windows for an undo) apply it all.
+//   - The flat-index kernels apply none of it, except that the undo applies a mask when there are no steps.
+// What the call did: `emitted`: its kernel wrote the twin; `colsum_slices`: the slices of colsum it wrote (0: none);
+// `fused`: it applied the steps and the mask.  When fused is false it applied none of them, nor the twin or colsum: the
+// caller runs the steps and the mask as passes, in the order above, then sums and converts the result.
 struct PoolEpi {
   int relu = 0;
   float drop_prob = 0.f, drop_scale = 0.f; unsigned long long drop_seed = 0;
   float scale = 1.f;
   const float* mask = nullptr;
-  float* rowsum = nullptr;
-  bool any() const { return relu || drop_scale != 0.f || scale != 1.f || mask || rowsum; }
+  float* colsum = nullptr;
+  __nv_bfloat16* twin = nullptr;
+  bool cache_masks = false;
+  bool steps() const { return relu || drop_scale != 0.f || scale != 1.f; }
 };
-// targets_bf16 (may be null): also write the bf16 twin of the target; the return value says whether the kernel did.
-// epi (average pooling only): *epi_done says whether the kernel applied it (else the caller runs it as passes); with a
-// rowsum, *colsum_slices is the number of row slices the kernel summed
-bool pool_forward(const PoolGeom& g, bool is_max, const float* images, float* targets, float scaleOutput,
-                  __nv_bfloat16* targets_bf16 = nullptr, bool cache_masks = false, const PoolEpi& epi = PoolEpi(),
-                  bool* epi_done = nullptr, int* colsum_slices = nullptr);
-// colsum / colsum_slices (may be null): where a kernel that can do so leaves per-slice channel sums of the tensor it wrote,
-// colsum[slice * channels + c] (*colsum_slices = number of slices, 0 = not done) — the bias gradient of the edge below
-bool max_pool_undo(const PoolGeom& g, const float* images, const float* maxGrads, const float* maxActs,
-                   float* targets, float scaleTargets, float scaleOutput, const float* relu_mask,
-                   __nv_bfloat16* targets_bf16 = nullptr, float* colsum = nullptr, int* colsum_slices = nullptr);
-// epi: its relu / dropout / scale steps (mask and rowsum are relu_mask and colsum); *epi_done as for pool_forward.  When
-// the kernel cannot apply them it applies none of relu_mask, colsum and the bf16 twin either (the caller's passes do)
-bool avg_pool_undo(const PoolGeom& g, const float* avgGrads, float* targets, float scaleTargets,
-                   float scaleOutput, const float* relu_mask, __nv_bfloat16* targets_bf16 = nullptr,
-                   float* colsum = nullptr, int* colsum_slices = nullptr, const PoolEpi& epi = PoolEpi(),
-                   bool* epi_done = nullptr);
+struct PoolOutcome { bool emitted = false; bool fused = true; int colsum_slices = 0; };
+PoolOutcome pool_forward(const PoolGeom& g, bool is_max, const float* images, float* targets, float scaleOutput,
+                         const PoolEpi& epi);
+// images and acts (the pool input and output) are read by max pooling only
+PoolOutcome pool_undo(const PoolGeom& g, bool is_max, const float* images, const float* grads, const float* acts,
+                      float* targets, float scaleTargets, float scaleOutput, const PoolEpi& epi);
 // max-pool R-operator: targets = st * targets + sum of R_images over the window elements equal to the stored maximum
 void max_pool_rprop(const PoolGeom& g, const float* images, const float* R_images, const float* maxes, float* targets, float st);
 // grad_bias[c] = st*grad_bias[c] + so * sum_slices part[slice*cols + c]   (elementwise.cu)

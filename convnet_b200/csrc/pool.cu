@@ -10,6 +10,7 @@
 #include <cuda_bf16.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "conv_kernels.h"
 
@@ -38,6 +39,31 @@ template <> __device__ __forceinline__ void vemit<4>(__nv_bfloat16* p16, const f
 }
 template <> __device__ __forceinline__ void vemit<1>(__nv_bfloat16* p16, const float (&v)[1]) { *p16 = __float2bfloat16_rn(v[0]); }
 
+// the fused ReLU' step of PoolEpi (cnb_relu_deriv): acc is zeroed where the mask is not > 0.  The mask is read at p[i], or,
+// where it is the pool input itself (a max pool right above its ReLU layer), taken from that input's values `in`
+template <int VEC, typename I>
+__device__ __forceinline__ void mask_step(float (&acc)[VEC], const float* p, I i, bool is_input, const float (&in)[VEC]) {
+  float mk[VEC];
+  if (is_input) {
+#pragma unroll
+    for (int v = 0; v < VEC; v++) mk[v] = in[v];
+  } else vload<VEC>(p + i, mk);
+#pragma unroll
+  for (int v = 0; v < VEC; v++) acc[v] = mk[v] > 0.f ? acc[v] : 0.f;
+}
+// the colsum of PoolEpi: deterministic block sum of `total` -> rowsum[blockIdx.x][plane] (256 threads)
+__device__ __forceinline__ void block_rowsum(float total, float* rowsum) {
+  __shared__ float sh[8];
+  for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = total;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int w = 0; w < 8; w++) s += sh[w];
+    rowsum[(size_t)blockIdx.x * gridDim.y + blockIdx.y] = s;
+  }
+}
+
 // ---- forward -------------------------------------------------------------------------
 // the divisor of a 2-D average: the product of the CLIPPED extents, as the reference computes it (gemm.cu:185).  A window
 // wholly in the padding has an extent <= 0 on some axis, so its average is 0 / region: NaN where an extent is 0, a signed
@@ -50,11 +76,11 @@ __device__ __forceinline__ int clipped_region(int X0, int Y0, const PoolGeom& g)
 // thread are in flight together (the generic K == 0 version walks the window with runtime loops, one load at a time).
 template <int VEC, bool MAX, int K>
 __global__ void __launch_bounds__(256) pool_fwd_kernel(PoolGeom g, const float* __restrict__ images,
-                                                        float* __restrict__ targets, float so, long long total) {
+                                                        float* __restrict__ targets, float so) {
   // blockIdx.y = (channel, output frame) plane; inside a plane all index arithmetic is 32-bit (the 64-bit
   // divisions of a flat index made these kernels instruction-bound, not HBM-bound)
   const unsigned NV = g.N / VEC;
-  const unsigned plane = NV * g.modX * g.modY;                   // `total` = elements per plane
+  const unsigned plane = NV * g.modX * g.modY;                   // elements per plane
   const int c = blockIdx.y % g.C, mt = blockIdx.y / g.C;
   for (unsigned pidx = blockIdx.x * blockDim.x + threadIdx.x; pidx < plane; pidx += gridDim.x * blockDim.x) {
     const unsigned nv = pidx % NV, r = pidx / NV;
@@ -125,8 +151,7 @@ template <int VEC, bool MAX, int Q>
 __global__ void __launch_bounds__(256) pool_undo_kernel(PoolGeom g, const float* __restrict__ images,
                                                          const float* __restrict__ grads,
                                                          const float* __restrict__ acts, float* targets,
-                                                         float st, float so, long long total,
-                                                         const float* __restrict__ relu_mask) {
+                                                         float st, float so, const float* __restrict__ relu_mask) {
   const unsigned NV = g.N / VEC;
   const unsigned plane = NV * g.W * g.H;
   const int c = blockIdx.y % g.C, T = blockIdx.y / g.C;
@@ -189,15 +214,7 @@ __global__ void __launch_bounds__(256) pool_undo_kernel(PoolGeom g, const float*
     }
 #pragma unroll
     for (int v = 0; v < VEC; v++) acc[v] += st * old[v];
-    if (relu_mask) {                           // fused ApplyDerivativeOfActivation of the layer receiving this derivative
-      float mk[VEC];
-      if (MAX && relu_mask == images) {        // max-pool right above the ReLU layer: the mask is the pool input itself
-#pragma unroll
-        for (int v = 0; v < VEC; v++) mk[v] = img[v];
-      } else vload<VEC>(relu_mask + idx * VEC, mk);
-#pragma unroll
-      for (int v = 0; v < VEC; v++) acc[v] = mk[v] > 0.f ? acc[v] : 0.f;
-    }
+    if (relu_mask) mask_step<VEC>(acc, relu_mask, idx * VEC, MAX && relu_mask == images, img);
     vstore<VEC>(targets + idx * VEC, acc);
   }
 }
@@ -210,8 +227,8 @@ __global__ void __launch_bounds__(256) pool_undo_kernel(PoolGeom g, const float*
 // index is a shift when N/VEC is a power of two, and per-thread offsets are 32-bit.
 template <int S> __device__ __forceinline__ int div_s(int a, int s) { return S > 0 ? a / S : a / s; }
 
-// the epilogue of PoolEpi on VEC results whose first element has index `i` in the target tensor, in the order of the
-// stand-alone passes it replaces: cnb_relu, the dropout of cnb_dropout (mask-free, element index i), cnb_mult by a
+// the steps of PoolEpi on VEC results whose first element has index `i` in the target tensor, in the order of the
+// stand-alone passes they replace: cnb_relu, the dropout of cnb_dropout (mask-free, element index i), cnb_mult by a
 // constant.  Each step is the pass's own single rounding, so the results are bit-identical to those passes.
 template <int VEC>
 __device__ __forceinline__ void epilogue(const PoolEpi& e, float (&acc)[VEC], long long i) {
@@ -224,18 +241,6 @@ __device__ __forceinline__ void epilogue(const PoolEpi& e, float (&acc)[VEC], lo
     acc[v] = x;
   }
 }
-// deterministic block sum of `total` -> rowsum[blockIdx.x][plane] (256 threads)
-__device__ __forceinline__ void block_rowsum(float total, float* rowsum) {
-  __shared__ float sh[8];
-  for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = total;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float s = 0.f;
-    for (int w = 0; w < 8; w++) s += sh[w];
-    rowsum[(size_t)blockIdx.x * gridDim.y + blockIdx.y] = s;
-  }
-}
 template <int S>
 __device__ __forceinline__ void cover_s(int X, int s, int p, int k, int mods, int& lo, int& hi) {
   const int a = X - p - k + 1;
@@ -244,11 +249,13 @@ __device__ __forceinline__ void cover_s(int X, int s, int p, int k, int mods, in
   hi = b < 0 ? -1 : min(div_s<S>(b, s), mods - 1);
 }
 
-// EPI: the epilogue of PoolEpi after the scaled average (average pooling only; EPI == false is the plain kernel)
+// EPI: the steps, the mask and the colsum of PoolEpi after the scaled average (average pooling only).  Every instance
+// writes the twin (epi.twin, passed as a __restrict__ parameter of its own); the max instances record the tie masks.
 template <int VEC, bool MAX, int K, int S, bool EPI>
-__device__ __forceinline__ void pool_fwd_rows(PoolGeom g, const float* __restrict__ images, float* __restrict__ targets,
-                                              float so, int nv_shift, __nv_bfloat16* __restrict__ targets16,
-                                              uint16_t* __restrict__ tie_masks, const PoolEpi& epi) {
+__global__ void __launch_bounds__(256) pool_fwd_rows_kernel(PoolGeom g, const float* __restrict__ images,
+                                                             float* __restrict__ targets, float so, int nv_shift,
+                                                             __nv_bfloat16* __restrict__ twin,
+                                                             uint16_t* __restrict__ tie_masks, PoolEpi epi) {
   pdl_wait();
   pdl_trigger();
   const unsigned NV = g.N / VEC;
@@ -256,7 +263,7 @@ __device__ __forceinline__ void pool_fwd_rows(PoolGeom g, const float* __restric
   const int sx = S > 0 ? S : g.sx, sy = S > 0 ? S : g.sy;
   const float* img = images + (long long)g.N * g.W * g.H * blockIdx.y;        // this channel's input plane
   float* out = targets + (long long)g.N * g.modX * g.modY * blockIdx.y;
-  __nv_bfloat16* out16 = targets16 ? targets16 + (long long)g.N * g.modX * g.modY * blockIdx.y : nullptr;
+  __nv_bfloat16* out16 = twin ? twin + (long long)g.N * g.modX * g.modY * blockIdx.y : nullptr;
   uint16_t* outm = (MAX && tie_masks) ? tie_masks + (long long)g.N * g.modX * g.modY * blockIdx.y : nullptr;
   const long long out_plane = (long long)g.N * g.modX * g.modY * blockIdx.y;
   const float* mk_p = EPI && epi.mask ? epi.mask + out_plane : nullptr;
@@ -310,13 +317,8 @@ __device__ __forceinline__ void pool_fwd_rows(PoolGeom g, const float* __restric
       const unsigned o = (unsigned)(my * rowlen + t) * VEC;
       if constexpr (EPI) {
         epilogue<VEC>(epi, acc, out_plane + o);
-        if (mk_p) {
-          float mk[VEC];
-          vload<VEC>(mk_p + o, mk);
-#pragma unroll
-          for (int v = 0; v < VEC; v++) acc[v] = mk[v] > 0.f ? acc[v] : 0.f;
-        }
-        if (epi.rowsum) {
+        if (mk_p) mask_step<VEC>(acc, mk_p, o, false, acc);
+        if (epi.colsum) {
 #pragma unroll
           for (int v = 0; v < VEC; v++) total += acc[v];
         }
@@ -325,30 +327,18 @@ __device__ __forceinline__ void pool_fwd_rows(PoolGeom g, const float* __restric
       if (out16) vemit<VEC>(out16 + o, acc);
     }
   }
-  if (EPI && epi.rowsum) block_rowsum(total, epi.rowsum);
-}
-template <int VEC, bool MAX, int K, int S>
-__global__ void __launch_bounds__(256) pool_fwd_rows_kernel(PoolGeom g, const float* __restrict__ images,
-                                                             float* __restrict__ targets, float so, int nv_shift,
-                                                             __nv_bfloat16* __restrict__ targets16,
-                                                             uint16_t* __restrict__ tie_masks) {
-  pool_fwd_rows<VEC, MAX, K, S, false>(g, images, targets, so, nv_shift, targets16, tie_masks, PoolEpi());
-}
-// average pooling with the epilogue of PoolEpi (the sampling calls' fused requests)
-template <int VEC, int K, int S>
-__global__ void __launch_bounds__(256) pool_fwd_rows_epi_kernel(PoolGeom g, const float* __restrict__ images,
-                                                                 float* __restrict__ targets, float so, int nv_shift,
-                                                                 __nv_bfloat16* __restrict__ targets16, PoolEpi epi) {
-  pool_fwd_rows<VEC, false, K, S, true>(g, images, targets, so, nv_shift, targets16, nullptr, epi);
+  if (EPI && epi.colsum) block_rowsum(total, epi.colsum);
 }
 
-// EPI: the relu / dropout / scale steps of PoolEpi before the ReLU' mask (average undo only; EPI == false: the plain kernel)
+// EPI: the steps of PoolEpi before its mask (average undo only).  Every instance applies the mask, the colsum and the
+// twin, which it takes as __restrict__ parameters of their own (the `epi` pointers are not read).
 template <int VEC, bool MAX, int Q, int S, bool EPI>
-__device__ __forceinline__ void pool_undo_rows(PoolGeom g, const float* __restrict__ images, const float* __restrict__ grads,
-                                               const float* __restrict__ acts, float* targets, float st, float so,
-                                               const float* __restrict__ relu_mask, int nv_shift,
-                                               __nv_bfloat16* __restrict__ targets16, float* __restrict__ rowsum,
-                                               const PoolEpi& epi) {
+__global__ void __launch_bounds__(256) pool_undo_rows_kernel(PoolGeom g, const float* __restrict__ images,
+                                                              const float* __restrict__ grads,
+                                                              const float* __restrict__ acts, float* targets,
+                                                              float st, float so, const float* __restrict__ relu_mask,
+                                                              int nv_shift, __nv_bfloat16* __restrict__ targets16,
+                                                              float* __restrict__ rowsum, PoolEpi epi) {
   pdl_wait();
   pdl_trigger();
   const unsigned NV = g.N / VEC;
@@ -410,15 +400,7 @@ __device__ __forceinline__ void pool_undo_rows(PoolGeom g, const float* __restri
 #pragma unroll
       for (int v = 0; v < VEC; v++) acc[v] += st * old[v];
       if constexpr (EPI) epilogue<VEC>(epi, acc, in_plane + idx);
-      if (relu_mask) {                         // fused ApplyDerivativeOfActivation of the layer receiving this derivative
-        float mk[VEC];
-        if (mask_is_input) {
-#pragma unroll
-          for (int v = 0; v < VEC; v++) mk[v] = im[v];
-        } else vload<VEC>(mk_p + idx, mk);
-#pragma unroll
-        for (int v = 0; v < VEC; v++) acc[v] = mk[v] > 0.f ? acc[v] : 0.f;
-      }
+      if (relu_mask) mask_step<VEC>(acc, mk_p, idx, mask_is_input, im);
       vstore<VEC>(out + idx, acc);
       if (out16) vemit<VEC>(out16 + idx, acc);
       if (rowsum) {
@@ -427,36 +409,9 @@ __device__ __forceinline__ void pool_undo_rows(PoolGeom g, const float* __restri
       }
     }
   }
-  if (rowsum) {                                 // deterministic block sum -> rowsum[blockIdx.x][plane]
-    __shared__ float sh[8];
-    for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = total;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      float s = 0.f;
-      for (int w = 0; w < 8; w++) s += sh[w];
-      rowsum[(size_t)blockIdx.x * gridDim.y + blockIdx.y] = s;
-    }
-  }
+  if (rowsum) block_rowsum(total, rowsum);
 }
 
-template <int VEC, bool MAX, int Q, int S>
-__global__ void __launch_bounds__(256) pool_undo_rows_kernel(PoolGeom g, const float* __restrict__ images,
-                                                              const float* __restrict__ grads,
-                                                              const float* __restrict__ acts, float* targets,
-                                                              float st, float so, const float* __restrict__ relu_mask,
-                                                              int nv_shift, __nv_bfloat16* __restrict__ targets16,
-                                                              float* __restrict__ rowsum) {
-  pool_undo_rows<VEC, MAX, Q, S, false>(g, images, grads, acts, targets, st, so, relu_mask, nv_shift, targets16, rowsum, PoolEpi());
-}
-// average undo with the relu / dropout / scale steps of PoolEpi (the sampling calls' fused requests)
-template <int VEC, int Q, int S>
-__global__ void __launch_bounds__(256) pool_undo_rows_epi_kernel(PoolGeom g, const float* __restrict__ grads, float* targets,
-                                                                  float st, float so, const float* __restrict__ relu_mask,
-                                                                  int nv_shift, __nv_bfloat16* __restrict__ targets16,
-                                                                  float* __restrict__ rowsum, PoolEpi epi) {
-  pool_undo_rows<VEC, false, Q, S, true>(g, nullptr, grads, nullptr, targets, st, so, relu_mask, nv_shift, targets16, rowsum, epi);
-}
 
 // max-pool undo from the tie masks the forward kernel recorded (convnet_b200_pool_cache_next), stride 2, windows up to
 // 3 x 3: every window covering an input element contributes its gradient iff the mask says this element equalled the
@@ -553,17 +508,7 @@ __global__ void __launch_bounds__(256, 4) pool_undo_masked_patch_kernel(PoolGeom
       }
     }
   }
-  if (rowsum) {
-    __shared__ float sh[8];
-    for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = total;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      float s = 0.f;
-      for (int w = 0; w < 8; w++) s += sh[w];
-      rowsum[(size_t)blockIdx.x * gridDim.y + blockIdx.y] = s;
-    }
-  }
+  if (rowsum) block_rowsum(total, rowsum);
 }
 
 // Compare-based max-pool undo (no cached masks) in the same patch organisation: per thread the 2 x 2 inputs of a patch and
@@ -632,15 +577,7 @@ __global__ void __launch_bounds__(256) pool_undo_patch_kernel(PoolGeom g, const 
           }
 #pragma unroll
           for (int v = 0; v < VEC; v++) acc[v] += st * old[v];
-          if (relu_mask) {
-            float mk[VEC];
-            if (mask_is_input) {
-#pragma unroll
-              for (int v = 0; v < VEC; v++) mk[v] = im[b * 2 + a][v];
-            } else vload<VEC>(mk_p + idx, mk);
-#pragma unroll
-            for (int v = 0; v < VEC; v++) acc[v] = mk[v] > 0.f ? acc[v] : 0.f;
-          }
+          if (relu_mask) mask_step<VEC>(acc, mk_p, idx, mask_is_input, im[b * 2 + a]);
           vstore<VEC>(out + idx, acc);
           if (out16) vemit<VEC>(out16 + idx, acc);
           if (rowsum) {
@@ -650,17 +587,7 @@ __global__ void __launch_bounds__(256) pool_undo_patch_kernel(PoolGeom g, const 
         }
     }
   }
-  if (rowsum) {
-    __shared__ float sh[8];
-    for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = total;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      float s = 0.f;
-      for (int w = 0; w < 8; w++) s += sh[w];
-      rowsum[(size_t)blockIdx.x * gridDim.y + blockIdx.y] = s;
-    }
-  }
+  if (rowsum) block_rowsum(total, rowsum);
 }
 
 static int pow2_shift(unsigned v) { int s = 0; while ((1u << s) < v) s++; return (1u << s) == v ? s : -1; }
@@ -678,61 +605,59 @@ static bool patch_geometry(const PoolGeom& g) {
          g.py <= 0 && g.px >= -2 && g.py >= -2 && (long long)g.N * g.W * g.H < (1LL << 31);
 }
 
+// f(std::integral_constant<T, v>()) for the run-time value v, which is one of Vs: the kernel instance of a run-time choice
+template <typename T, T... Vs, typename F>
+static void with_const(T v, F&& f) {
+  (void)((v == Vs && (f(std::integral_constant<T, Vs>()), true)) || ...);
+}
+// the S of the row kernels: the stride as a template constant (1 or 2), or 0 (read at run time)
+static int row_stride(const PoolGeom& g) { return (g.sx == g.sy && g.sx <= 2) ? g.sx : 0; }
+
 template <int VEC, bool MAX>
-static bool launch_fwd(const PoolGeom& g, const float* images, float* targets, float so, long long total, __nv_bfloat16* t16,
-                       uint16_t* masks, const PoolEpi& epi, bool* epi_done, int* colsum_slices) {
+static PoolOutcome launch_fwd(const PoolGeom& g, const float* images, float* targets, float so, uint16_t* masks,
+                              const PoolEpi& epi) {
   cudaStream_t s = state().stream;
   const int planes = g.C * g.modT;
-  const long long per_plane = total / planes;
+  const long long per_plane = (long long)g.modX * g.modY * (g.N / VEC);
   CNB_REQUIRE(per_plane < (1LL << 30) && planes <= 65535, "pool_forward: plane too large");
-  const dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(ceil_div<long long>(per_plane, 256), 64)), planes);
+  PoolOutcome o;
   const int k = (g.kt == 1 && g.T == 1 && g.modT == 1) ? std::max(g.kx, g.ky) : 99;
-  const long long in_plane = (long long)g.N * g.W * g.H;
-  if (k <= 3 && in_plane < (1LL << 31)) {          // 2-D, small window: the row-structured kernels
-    const dim3 rgrid((unsigned)g.modY, planes);
+  if (k <= 3 && (long long)g.N * g.W * g.H < (1LL << 31)) {          // 2-D, small window: the row-structured kernels
+    const bool e = epi.steps() || epi.mask || epi.colsum;    // (never with max pooling: the EPI instances are average's)
     const int sh = pow2_shift(g.N / VEC);
-    const int S = (g.sx == g.sy && g.sx <= 2) ? g.sx : 0;
-    const bool e = !MAX && epi.any();
-    if (e && epi_done) *epi_done = true;
-    if (e && epi.rowsum && colsum_slices) *colsum_slices = g.modY;
-#define CNB_POOL_FWD(KK, SS)                                                                                                  \
-  do {                                                                                                                        \
-    if (e) launch_pdl(pool_fwd_rows_epi_kernel<VEC, KK, SS>, rgrid, dim3(256), 0, s, g, images, targets, so, sh, t16, epi); \
-    else launch_pdl(pool_fwd_rows_kernel<VEC, MAX, KK, SS>, rgrid, dim3(256), 0, s, g, images, targets, so, sh, t16, masks); \
-  } while (0)
-    if (k <= 2) { if (S == 1) CNB_POOL_FWD(2, 1); else if (S == 2) CNB_POOL_FWD(2, 2); else CNB_POOL_FWD(2, 0); }
-    else { if (S == 1) CNB_POOL_FWD(3, 1); else if (S == 2) CNB_POOL_FWD(3, 2); else CNB_POOL_FWD(3, 0); }
-#undef CNB_POOL_FWD
-    return t16 != nullptr;
+    o.emitted = epi.twin != nullptr;
+    o.colsum_slices = epi.colsum ? g.modY : 0;
+    with_const<int, 2, 3>(k <= 2 ? 2 : 3, [&](auto K) {
+      with_const<int, 0, 1, 2>(row_stride(g), [&](auto S) {
+        launch_pdl(e ? pool_fwd_rows_kernel<VEC, false, K, S, true> : pool_fwd_rows_kernel<VEC, MAX, K, S, false>,
+                   dim3((unsigned)g.modY, planes), dim3(256), 0, s, g, images, targets, so, sh, epi.twin, masks, epi);
+      });
+    });
+    return o;
   }
-  if (k <= 2) pool_fwd_kernel<VEC, MAX, 2><<<grid, 256, 0, s>>>(g, images, targets, so, total);
-  else if (k == 3) pool_fwd_kernel<VEC, MAX, 3><<<grid, 256, 0, s>>>(g, images, targets, so, total);
-  else if (k == 4) pool_fwd_kernel<VEC, MAX, 4><<<grid, 256, 0, s>>>(g, images, targets, so, total);
-  else pool_fwd_kernel<VEC, MAX, 0><<<grid, 256, 0, s>>>(g, images, targets, so, total);
-  return false;
+  o.fused = false;
+  const dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(ceil_div<long long>(per_plane, 256), 64)), planes);
+  with_const<int, 2, 3, 4, 0>(k <= 2 ? 2 : k <= 4 ? k : 0, [&](auto K) {
+    pool_fwd_kernel<VEC, MAX, K><<<grid, 256, 0, s>>>(g, images, targets, so);
+  });
+  return o;
 }
 
-bool pool_forward(const PoolGeom& g, bool is_max, const float* images, float* targets, float so, __nv_bfloat16* targets_bf16,
-                  bool cache_masks, const PoolEpi& epi, bool* epi_done, int* colsum_slices) {
-  if (epi_done) *epi_done = false;
-  if (colsum_slices) *colsum_slices = 0;
+PoolOutcome pool_forward(const PoolGeom& g, bool is_max, const float* images, float* targets, float so, const PoolEpi& epi) {
+  CNB_REQUIRE(!is_max || !(epi.steps() || epi.mask || epi.colsum), "pool_forward: max pooling fuses only the twin and the tie masks");
   const bool v4 = (g.N % 4 == 0) && aligned16(images) && aligned16(targets) && (!epi.mask || aligned16(epi.mask));
-  const long long outs = (long long)g.modX * g.modY * g.C * g.modT;
   // tie masks for the matching undo: unscaled outputs only
   uint16_t* masks = nullptr;
-  if (cache_masks && is_max && so == 1.f && patch_geometry(g))
-    masks = pool_masks_slot(targets, outs * g.N, images, (long long)g.N * g.W * g.H * g.C, pool_sig(g));
-  bool emitted;
-  if (v4) {
-    if (is_max) emitted = launch_fwd<4, true>(g, images, targets, so, outs * (g.N / 4), targets_bf16, masks, epi, epi_done, colsum_slices);
-    else emitted = launch_fwd<4, false>(g, images, targets, so, outs * (g.N / 4), targets_bf16, nullptr, epi, epi_done, colsum_slices);
-  } else {
-    if (is_max) emitted = launch_fwd<1, true>(g, images, targets, so, outs * g.N, targets_bf16, masks, epi, epi_done, colsum_slices);
-    else emitted = launch_fwd<1, false>(g, images, targets, so, outs * g.N, targets_bf16, nullptr, epi, epi_done, colsum_slices);
-  }
+  if (epi.cache_masks && is_max && so == 1.f && patch_geometry(g))
+    masks = pool_masks_slot(targets, (long long)g.modX * g.modY * g.C * g.modT * g.N, images,
+                            (long long)g.N * g.W * g.H * g.C, pool_sig(g));
+  PoolOutcome o;
+  with_const<int, 1, 4>(v4 ? 4 : 1, [&](auto VEC) {
+    with_const<bool, false, true>(is_max, [&](auto MAX) { o = launch_fwd<VEC, MAX>(g, images, targets, so, masks, epi); });
+  });
   count_launch();
   CNB_LAUNCH_CHECK("pool_forward");
-  return emitted;
+  return o;
 }
 
 // ---- max-pool R-operator (kMaxPoolRprop) ---------------------------------------------------------------------------------
@@ -793,91 +718,69 @@ void max_pool_rprop(const PoolGeom& g, const float* images, const float* R_image
 }
 
 template <int VEC, bool MAX>
-// colsum (may be null): on return *colsum_slices > 0 iff the kernel wrote per-(row, plane) sums of its output to `colsum`
-static bool launch_undo(const PoolGeom& g, const float* images, const float* grads, const float* acts, float* targets,
-                        float st, float so, long long total, const float* mask, __nv_bfloat16* t16, float* colsum,
-                        int* colsum_slices, const PoolEpi& epi, bool* epi_done) {
+static PoolOutcome launch_undo(const PoolGeom& g, const float* images, const float* grads, const float* acts, float* targets,
+                               float st, float so, const PoolEpi& epi) {
   cudaStream_t s = state().stream;
   const int planes = g.C * g.T;
-  const long long per_plane = total / planes;
+  const long long per_plane = (long long)g.W * g.H * (g.N / VEC);
   CNB_REQUIRE(per_plane < (1LL << 30) && planes <= 65535, "pool_undo: plane too large");
-  const dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(ceil_div<long long>(per_plane, 256), 64)), planes);
+  PoolOutcome o;
   // windows covering one element per axis: ceil(k / stride)
   const int q = (g.kt == 1 && g.T == 1 && g.modT == 1) ? std::max(ceil_div(g.kx, g.sx), ceil_div(g.ky, g.sy)) : 99;
   if (q <= 2 && per_plane * VEC < (1LL << 31)) {   // 2-D, at most 2 x 2 covering windows: the row-structured kernels
-    const dim3 rgrid((unsigned)g.H, planes);
     const int sh = pow2_shift(g.N / VEC);
-    const int S = (g.sx == g.sy && g.sx <= 2) ? g.sx : 0;
+    o.emitted = epi.twin != nullptr;
     if (MAX && patch_geometry(g)) {
       // patches: element X belongs to patch (X - px) / 2; the first patch holds X = 0, the last X = W - 1
       const int PX = (g.W - 1 - g.px) / 2 + 1, PY = (g.H - 1 - g.py) / 2 + 1;
-      if (colsum && colsum_slices) *colsum_slices = PY;
+      o.colsum_slices = epi.colsum ? PY : 0;
       // the forward pass left tie masks for exactly this (input, output) pair and nothing wrote either since: no need to
       // reload and compare them.  A fused ReLU' mask is only expressible when it IS the pool input (bit 15 = maximum > 0).
       // (with scaleTargets != 0 the compare path also zeroes the OLD target where the mask fails; the tie masks cannot say
       // that for elements that are no window's maximum, so that combination stays on the compare path)
-      const uint16_t* tm = mask == nullptr || (mask == images && st == 0.f)
+      const uint16_t* tm = epi.mask == nullptr || (epi.mask == images && st == 0.f)
                                ? pool_masks_find(acts, (long long)g.N * g.modX * g.modY * g.C, images, pool_sig(g)) : nullptr;
       if (tm)
         launch_pdl(pool_undo_masked_patch_kernel<VEC>, dim3((unsigned)PY, planes), dim3(256), 0, s, g, grads, tm, targets, st, so,
-                   mask != nullptr ? 1 : 0, sh, t16, colsum, PX, PY);
+                   epi.mask != nullptr ? 1 : 0, sh, epi.twin, epi.colsum, PX, PY);
       else
         launch_pdl(pool_undo_patch_kernel<VEC>, dim3((unsigned)PY, planes), dim3(256), 0, s, g, images, grads, acts, targets, st,
-                   so, mask, sh, t16, colsum, PX, PY);
-      return t16 != nullptr;
+                   so, epi.mask, sh, epi.twin, epi.colsum, PX, PY);
+      return o;
     }
-    if (colsum && colsum_slices) *colsum_slices = g.H;
-    const bool e = !MAX && epi.any();
-    if (e && epi_done) *epi_done = true;
-#define CNB_POOL_UNDO(QQ, SS)                                                                                                 \
-  do {                                                                                                                        \
-    if (e) pool_undo_rows_epi_kernel<VEC, QQ, SS><<<rgrid, 256, 0, s>>>(g, grads, targets, st, so, mask, sh, t16, colsum, epi); \
-    else pool_undo_rows_kernel<VEC, MAX, QQ, SS><<<rgrid, 256, 0, s>>>(g, images, grads, acts, targets, st, so, mask, sh, t16, colsum); \
-  } while (0)
-    if (q <= 1) { if (S == 1) CNB_POOL_UNDO(1, 1); else if (S == 2) CNB_POOL_UNDO(1, 2); else CNB_POOL_UNDO(1, 0); }
-    else { if (S == 1) CNB_POOL_UNDO(2, 1); else if (S == 2) CNB_POOL_UNDO(2, 2); else CNB_POOL_UNDO(2, 0); }
-#undef CNB_POOL_UNDO
-    return t16 != nullptr;
+    o.colsum_slices = epi.colsum ? g.H : 0;
+    with_const<int, 1, 2>(q, [&](auto Q) {
+      with_const<int, 0, 1, 2>(row_stride(g), [&](auto S) {
+        auto* kernel = epi.steps() ? pool_undo_rows_kernel<VEC, false, Q, S, true> : pool_undo_rows_kernel<VEC, MAX, Q, S, false>;
+        kernel<<<dim3((unsigned)g.H, planes), 256, 0, s>>>(g, images, grads, acts, targets, st, so, epi.mask, sh, epi.twin,
+                                                           epi.colsum, epi);
+      });
+    });
+    return o;
   }
-  if (!MAX && epi.any()) {                         // the epilogue runs as passes after this kernel: so must the mask
-    mask = nullptr;
-    t16 = nullptr;
-  }
-  if (q <= 1) pool_undo_kernel<VEC, MAX, 1><<<grid, 256, 0, s>>>(g, images, grads, acts, targets, st, so, total, mask);
-  else if (q == 2) pool_undo_kernel<VEC, MAX, 2><<<grid, 256, 0, s>>>(g, images, grads, acts, targets, st, so, total, mask);
-  else pool_undo_kernel<VEC, MAX, 0><<<grid, 256, 0, s>>>(g, images, grads, acts, targets, st, so, total, mask);
-  return false;
+  // the flat-index kernels fuse a bare ReLU' mask: with steps to run, the caller's passes apply the mask after them
+  o.fused = !epi.steps();
+  const dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(ceil_div<long long>(per_plane, 256), 64)), planes);
+  with_const<int, 1, 2, 0>(q <= 2 ? q : 0, [&](auto Q) {
+    pool_undo_kernel<VEC, MAX, Q><<<grid, 256, 0, s>>>(g, images, grads, acts, targets, st, so, o.fused ? epi.mask : nullptr);
+  });
+  return o;
 }
 
-static bool undo(const PoolGeom& g, bool is_max, const float* images, const float* grads, const float* acts,
-                 float* targets, float st, float so, const float* mask, __nv_bfloat16* t16, float* colsum, int* colsum_slices,
-                 const PoolEpi& epi = PoolEpi(), bool* epi_done = nullptr) {
-  if (epi_done) *epi_done = false;
-  const bool v4 = (g.N % 4 == 0) && aligned16(grads) && aligned16(targets) && (!mask || aligned16(mask)) &&
+PoolOutcome pool_undo(const PoolGeom& g, bool is_max, const float* images, const float* grads, const float* acts,
+                      float* targets, float st, float so, const PoolEpi& epi) {
+  CNB_REQUIRE(!is_max || !epi.steps(), "pool_undo: max pooling fuses no activation, dropout or scale");
+  const bool v4 = (g.N % 4 == 0) && aligned16(grads) && aligned16(targets) && (!epi.mask || aligned16(epi.mask)) &&
                   (!is_max || (aligned16(images) && aligned16(acts)));
-  const long long ins = (long long)g.W * g.H * g.C * g.T;
-  bool emitted;
-  if (v4) {
-    if (is_max) emitted = launch_undo<4, true>(g, images, grads, acts, targets, st, so, ins * (g.N / 4), mask, t16, colsum, colsum_slices, epi, epi_done);
-    else emitted = launch_undo<4, false>(g, images, grads, acts, targets, st, so, ins * (g.N / 4), mask, t16, colsum, colsum_slices, epi, epi_done);
-  } else {
-    if (is_max) emitted = launch_undo<1, true>(g, images, grads, acts, targets, st, so, ins * g.N, mask, t16, colsum, colsum_slices, epi, epi_done);
-    else emitted = launch_undo<1, false>(g, images, grads, acts, targets, st, so, ins * g.N, mask, t16, colsum, colsum_slices, epi, epi_done);
-  }
+  PoolOutcome o;
+  with_const<int, 1, 4>(v4 ? 4 : 1, [&](auto VEC) {
+    with_const<bool, false, true>(is_max, [&](auto MAX) {
+      o = launch_undo<VEC, MAX>(g, images, grads, acts, targets, st, so, epi);
+    });
+  });
   count_launch();
   CNB_LAUNCH_CHECK("pool_undo");
-  return emitted;
-}
-
-bool max_pool_undo(const PoolGeom& g, const float* images, const float* maxGrads, const float* maxActs,
-                   float* targets, float st, float so, const float* relu_mask, __nv_bfloat16* targets_bf16,
-                   float* colsum, int* colsum_slices) {
-  return undo(g, true, images, maxGrads, maxActs, targets, st, so, relu_mask, targets_bf16, colsum, colsum_slices);
-}
-
-bool avg_pool_undo(const PoolGeom& g, const float* avgGrads, float* targets, float st, float so, const float* relu_mask,
-                   __nv_bfloat16* targets_bf16, float* colsum, int* colsum_slices, const PoolEpi& epi, bool* epi_done) {
-  return undo(g, false, nullptr, avgGrads, nullptr, targets, st, so, relu_mask, targets_bf16, colsum, colsum_slices, epi, epi_done);
+  return o;
 }
 
 }  // namespace cnb

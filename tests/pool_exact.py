@@ -459,6 +459,7 @@ class Branch:
     in_kernel_twin: bool = False
     slices: int = 0           # per-slice bias sums the kernel leaves for colsum_finish (0: a column-sum pass)
     masks: bool = False       # the forward pass records tie masks
+    fused: bool = True        # the kernel applies the request's steps and ReLU' mask (else: passes after it)
 
 
 def patch_geometry(g):
@@ -470,27 +471,36 @@ def _vec(g, aligned):
     return 4 if g.N % 4 == 0 and aligned else 1
 
 
-def pool_fwd_branch(g, is_max, aligned=True, cache=False, so=1.0):
+def _rows_kernel(name, v, is_max, A, S, epi):
+    """the row-kernel instance: EPI (a request's epilogue) is an average-pooling instance"""
+    return "%s<%d, %s, %d, %d, %s>" % (name, v, "true" if is_max else "false", A, S, "true" if epi else "false")
+
+
+def pool_fwd_branch(g, is_max, aligned=True, cache=False, so=1.0, epi=False):
+    """epi: the average call has a request to fuse (steps, ReLU' mask or bias gradient)"""
     v = _vec(g, aligned)
     mx = "true" if is_max else "false"
     k = max(g.kx, g.ky) if g.two_d else 99
     masks = bool(cache and is_max and so == 1.0 and patch_geometry(g))
+    epi = epi and not is_max
     if k <= 3 and g.N * g.W * g.H < 2 ** 31:
         K = 2 if k <= 2 else 3
         S = g.sx if g.sx == g.sy and g.sx <= 2 else 0
-        return Branch("rows<%d,%s,K%d,S%d>" % (v, "max" if is_max else "avg", K, S),
-                      "pool_fwd_rows_kernel<%d, %s, %d, %d>" % (v, mx, K, S), True, masks=masks)
+        return Branch("rows<%d,%s,K%d,S%d>%s" % (v, "max" if is_max else "avg", K, S, "+epi" if epi else ""),
+                      _rows_kernel("pool_fwd_rows_kernel", v, is_max, K, S, epi), True,
+                      g.modY if epi else 0, masks=masks)
     K = 2 if k <= 2 else 3 if k == 3 else 4 if k == 4 else 0
     return Branch("generic<%d,%s,K%d>" % (v, "max" if is_max else "avg", K),
-                  "pool_fwd_kernel<%d, %s, %d>" % (v, mx, K), False, masks=masks)
+                  "pool_fwd_kernel<%d, %s, %d>" % (v, mx, K), False, masks=masks, fused=not epi)
 
 
-def pool_undo_branch(g, is_max, aligned=True, mask=None, st=0.0, cached=False):
+def pool_undo_branch(g, is_max, aligned=True, mask=None, st=0.0, cached=False, epi=False):
     """mask: None, 'input' (the ReLU' mask is the pool input) or 'other'; cached: the forward pass recorded tie masks
-    for this (input, output) pair"""
+    for this (input, output) pair; epi: the average undo has steps to fuse (ReLU, dropout or scale)"""
     v = _vec(g, aligned)
     mx = "true" if is_max else "false"
     kind = "max" if is_max else "avg"
+    epi = epi and not is_max
     q = max(-(-g.kx // g.sx), -(-g.ky // g.sy)) if g.two_d else 99
     if q <= 2 and (g.N // v) * g.W * g.H * v < 2 ** 31:
         if is_max and patch_geometry(g):
@@ -500,22 +510,24 @@ def pool_undo_branch(g, is_max, aligned=True, mask=None, st=0.0, cached=False):
             return Branch("patch<%d>" % v, "pool_undo_patch_kernel<%d>" % v, True, PY)
         S = g.sx if g.sx == g.sy and g.sx <= 2 else 0
         Q = 1 if q <= 1 else 2
-        return Branch("undo_rows<%d,%s,Q%d,S%d>" % (v, kind, Q, S),
-                      "pool_undo_rows_kernel<%d, %s, %d, %d>" % (v, mx, Q, S), True, g.H)
+        return Branch("undo_rows<%d,%s,Q%d,S%d>%s" % (v, kind, Q, S, "+epi" if epi else ""),
+                      _rows_kernel("pool_undo_rows_kernel", v, is_max, Q, S, epi), True, g.H)
     Q = 1 if q <= 1 else 2 if q == 2 else 0
-    return Branch("undo_generic<%d,%s,Q%d>" % (v, kind, Q), "pool_undo_kernel<%d, %s, %d>" % (v, mx, Q), False, 0)
+    return Branch("undo_generic<%d,%s,Q%d>" % (v, kind, Q), "pool_undo_kernel<%d, %s, %d>" % (v, mx, Q), False, 0,
+                  fused=not epi)
 
 
 def bias_depth(branch, g):
-    """(values one thread adds, slices colsum_finish adds) of the bias-gradient sum of an undo branch"""
+    """(values one thread adds, slices colsum_finish adds) of the bias-gradient sum of a branch"""
     v = 4 if branch.name.split("<")[1].startswith("4") else 1
     NV = g.N // v
+    fwd = branch.kernel.startswith("pool_fwd")        # (the bias gradient of a forward call sums its output)
     if branch.slices and "patch" in branch.name:
         PX = (g.W - 1 + g.px) // 2 + 1
         return -(-NV * PX // 256) * 4 * v, branch.slices
     if branch.slices:
-        return -(-NV * g.W // 256) * v, branch.slices
-    rows = g.N * g.W * g.H * g.T
+        return -(-NV * (g.modX if fwd else g.W) // 256) * v, branch.slices
+    rows = g.N * (g.modX * g.modY * g.modT if fwd else g.W * g.H * g.T)
     slices = max(1, min(64, (4 * SMS) // g.C))
     slices = min(slices, max(1, rows // 1024))
     return -(-(-(-rows // slices)) // 256), slices

@@ -155,6 +155,8 @@ def _pool_cases():
 
 POOL_CASES = _pool_cases()
 POOL_BY_NAME = {c.name: c for c in POOL_CASES}
+# the average cases once more under the sampling edges' requests (run_pool_epi); empty windows' NaN averages left out
+EPI_CASES = [c for c in POOL_CASES if not c.is_max and c.g.px < c.g.kx and c.g.py < c.g.ky]
 
 
 def _rn(name, N, W, H, F, k, **kw):
@@ -374,6 +376,95 @@ def test_pool_branch(env, name):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# the fused epilogues of the average calls: the forward with ReLU, dropout, a scale, the bias gradient and the twin
+# requested, the undo with a scale, the ReLU' mask, the bias gradient and the twin, each bit for bit against the unfused
+# call followed by the stand-alone passes it replaces
+# ---------------------------------------------------------------------------------------------------------------------
+EPI_P, EPI_SCALE, EPI_SEED = 0.3, 1.0 / 0.7, 0x5EED1234
+
+
+def _epi_call(env, c, fwd, src, tgt, mask, bias, st, request=True):
+    L = env.L
+    if request:
+        if fwd:
+            L.convnet_b200_fuse_next_act(None, 1, None)
+            L.convnet_b200_fuse_next_dropout(EPI_P, EPI_SCALE, EPI_SEED)
+        else:
+            L.convnet_b200_fuse_next_act(None, 1, mask.data_ptr())
+        L.convnet_b200_fuse_next_scale(EPI_SCALE)
+        if bias is not None:
+            L.convnet_b200_fuse_next_bias_grad(bias.data_ptr(), 0.5, 0.25)
+        if c.emit:
+            L.convnet_b200_emit_bf16_next()
+    d = c.g.desc()
+    if fwd:
+        L.AvgPoolGemm(src.p_mat, tgt.p_mat, src.p_shape4d, tgt.p_shape4d, d, 0.0, c.so)
+    else:
+        env.cg.gemm.AvgPoolUndo(src, tgt, d, st)
+
+
+def _epi_passes(env, fwd, y, mask):
+    L, n = env.L, y.numel()
+    scale = torch.full_like(y, EPI_SCALE)
+    if fwd:
+        L.cnb_relu(y.data_ptr(), n)
+        L.cnb_dropout(y.data_ptr(), torch.empty_like(y).data_ptr(), n, EPI_P, EPI_SCALE, EPI_SEED)
+    L.cnb_mult(y.data_ptr(), scale.data_ptr(), n)
+    if not fwd:
+        L.cnb_relu_deriv(y.data_ptr(), mask.data_ptr(), n)
+
+
+def run_pool_epi(env, c, check=True):
+    """forward then undo of case c, each unfused and then fused; returns the branches in launch order"""
+    g = c.g
+    gen = torch.Generator(device="cuda").manual_seed(zlib.crc32(("epi" + c.name).encode()))
+    nin, nout = g.N * g.W * g.H * g.C * g.T, g.N * g.modX * g.modY * g.C * g.modT
+    calls = ((True, g.in_dims(), g.in_shape(), g.out_dims(), g.out_shape(), nout, g.N * g.modX * g.modY),
+             (False, g.out_dims(), g.out_shape(), g.in_dims(), g.in_shape(), nin, g.N * g.W * g.H))
+    branches = []
+    for fwd, sdims, sshape, tdims, tshape, n, rows in calls:
+        st = 0.0 if fwd else 1.0
+        src, _ = _matrix(*sdims, sshape, c.offset, guard=0)
+        src.storage.normal_(generator=gen)
+        t0 = torch.randn(n, generator=gen, device="cuda")
+        mask = torch.randn(n, generator=gen, device="cuda")
+        plain, _ = _matrix(*tdims, tshape, c.offset)
+        plain.storage.copy_(t0)
+        b0 = torch.randn(g.C, generator=gen, device="cuda")
+        bias = b0.clone() if g.T == 1 else None          # (the edges ask a bias gradient of 2-D calls only)
+        b = (px.pool_fwd_branch(g, False, c.aligned, so=c.so, epi=True) if fwd
+             else px.pool_undo_branch(g, False, c.aligned, st=st, epi=True))
+        branches += [(px.pool_fwd_branch(g, False, c.aligned, so=c.so) if fwd
+                      else px.pool_undo_branch(g, False, c.aligned, st=st)), b]
+        tag = "%s %s+epi %s" % (c.name, "fwd" if fwd else "undo", b.name)
+        assert _launched(env, lambda: _epi_call(env, c, fwd, src, plain, mask, None, st, False)) == 1, tag
+        _epi_passes(env, fwd, plain.storage, mask)
+        tgt, tbuf = _matrix(*tdims, tshape, c.offset)
+        tgt.storage.copy_(t0)
+        launches = _launched(env, lambda: _epi_call(env, c, fwd, src, tgt, mask, bias, st))
+        passes = 0 if b.fused else 3 if fwd else 2
+        want = 1 + passes + (bias is not None and (1 if b.slices else 2)) + (c.emit and not b.in_kernel_twin)
+        assert launches == want, (tag, launches, want)
+        assert _guards_ok(tbuf, c.offset, n), tag + ": wrote outside its target"
+        if not check:
+            continue
+        assert torch.equal(tgt.storage.view(torch.int32), plain.storage.view(torch.int32)), tag + ": not the passes' result"
+        if bias is not None:
+            per_thread, slices = px.bias_depth(b, g)
+            vb = px.check(bias, px.bias_grad(tgt.storage, rows, g.C, 1, b0, 0.5, 0.25, per_thread, slices))
+            _note("bias_grad", "%s/%d slices" % (b.name.split("<")[0], slices), vb)
+            assert vb.ok, "%s bias: %s" % (tag, vb)
+        if c.emit:
+            _check_twin(env, tgt, tshape)
+    return branches
+
+
+@pytest.mark.parametrize("name", [c.name for c in EPI_CASES])
+def test_pool_epilogue_branch(env, name):
+    run_pool_epi(env, POOL_BY_NAME[name])
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # UpSample / DownSample
 # ---------------------------------------------------------------------------------------------------------------------
 def test_up_down_sample(env):
@@ -510,7 +601,8 @@ def _hot_kernels(prof):
 
 def test_kernel_names(env):
     """every small branch case once more, unchecked, under torch.profiler: the pool / rnorm kernels CUPTI records must
-    be, in order, the ones the mirror names (two launches per call: each call runs twice)"""
+    be, in order, the ones the mirror names (two launches per call: each call runs twice; the epilogue cases run each
+    call unfused, then fused)"""
     from torch.profiler import ProfilerActivity, profile
     want = []
     small_rn = [c for c in RN_CASES if c.L * c.F < (1 << 22)]
@@ -522,6 +614,8 @@ def test_kernel_names(env):
             for i, u in enumerate(c.undos):
                 want += [px.pool_undo_branch(c.g, c.is_max, c.aligned, u.mask, u.st,
                                              cached=c.cache and c.so == 1.0).kernel] * 2
+        for c in EPI_CASES:
+            want += [b.kernel for b in run_pool_epi(env, c, check=False)]
         for c in small_rn:
             run_rnorm(env, c, check=False)
             a = c.offset % 4 == 0

@@ -308,10 +308,10 @@ def _pool_universe():
                 g = PG(N, 12, 11, 4, ky, kx, sy, sx, min(p, ky - 1 + 1), min(p, kx - 1 + 1))
                 if g.modX < 1 or g.modY < 1:
                     continue
-                for is_max in (True, False):
-                    fwd.add(px.pool_fwd_branch(g, is_max, al).name)
+                for is_max, epi in ((True, False), (False, False), (False, True)):
+                    fwd.add(px.pool_fwd_branch(g, is_max, al, epi=epi).name)
                     for mask, st, cached in itertools.product((None, "input", "other"), (0.0, 1.0), (False, True)):
-                        undo.add(px.pool_undo_branch(g, is_max, al, mask, st, cached).name)
+                        undo.add(px.pool_undo_branch(g, is_max, al, mask, st, cached, epi=epi).name)
     for is_max in (True, False):
         for N, al in ((32, True), (7, True)):
             g = PG(N, 6, 7, 2, 2, 2, 1, 1, 0, 0, T=5, kt=2, st_t=2)
@@ -340,6 +340,9 @@ def test_every_mirror_branch_has_a_case():
             b = px.pool_undo_branch(c.g, c.is_max, c.aligned, u.mask, u.st, c.cache and c.so == 1.0).name
             assert b == c.undo_branch(i), (c.name, i, b)
             undo.add(b)
+    for c in T.EPI_CASES:                            # the epilogue instances of the average row kernels
+        fwd.add(px.pool_fwd_branch(c.g, False, c.aligned, so=c.so, epi=True).name)
+        undo.add(px.pool_undo_branch(c.g, False, c.aligned, st=1.0, epi=True).name)
     want_f, want_u = _pool_universe()
     assert not want_f - fwd, ("pool forward branches without a case", sorted(want_f - fwd))
     assert not want_u - undo, ("pool undo branches without a case", sorted(want_u - undo))

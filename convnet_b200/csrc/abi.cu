@@ -221,40 +221,45 @@ ConvDesc sample_desc(Shape4D* is, Shape4D* ts, int factor) {      // gemm.cu:150
   return d;
 }
 
-void do_rnorm(const char* what, cudamat* images, cudamat* targets, int F, int sizeF, float a, float b, bool blocked,
-              int frames) {
-  Range nvtx_range(what);
+// the checks of a cross-map norm over `images` (F channels per frame, `frames` frames per row) writing `targets`, and of
+// its second input `other` when there is one; returns the locations per frame
+long long rnorm_locs(const char* what, const cudamat* images, const cudamat* other, const cudamat* targets, int F,
+                     int frames) {
   CNB_REQUIRE(F > 0 && frames > 0, what);
   const long long els = (long long)images->size[0] * images->size[1];
   CNB_REQUIRE(els % ((long long)F * frames) == 0, what);
   CNB_REQUIRE(targets->size[0] == images->size[0] && targets->size[1] == images->size[1], what);
-  const long long L = els / F / frames;          // locations per frame
-  // fused epilogue (convnet_b200_fuse_next relu / convnet_b200_emit_bf16_next): in the tile kernel when it applies, else
-  // as trailing passes; the logistic activation is always a trailing pass
+  if (other) CNB_REQUIRE(other->size[0] == images->size[0] && other->size[1] == images->size[1], what);
+  return els / F / frames;
+}
+
+void do_rnorm(const char* what, cudamat* images, cudamat* targets, int F, int sizeF, float a, float b, bool blocked,
+              int frames) {
+  Range nvtx_range(what);
+  const long long L = rnorm_locs(what, images, nullptr, targets, F, frames);
+  const long long els = L * F * frames;
+  // the ReLU and the twin (convnet_b200_fuse_next relu / convnet_b200_emit_bf16_next) in the kernel when it applies them,
+  // else as passes; the logistic activation is always a pass, so its twin is converted after it
   const Fuse fuse = take_fuse();
-  const bool fusable = rnorm_can_fuse(F) && fuse.act != kActLogistic;
-  const bool relu = fuse.act == kActRelu;
+  const bool relu = fuse.act == kActRelu, logistic = fuse.act == kActLogistic;
   Emit emit(targets->data_device, els, fuse.emit_bf16 != 0);
+  __nv_bfloat16* twin = logistic ? nullptr : emit.buf;
+  bool fused = false;
   for (int t = 0; t < frames; t++)               // conv3d_gemm.cu:167-189: independent per frame
-    rnorm_forward(images->data_device + (long long)t * L * F, targets->data_device + (long long)t * L * F, L, F, sizeF,
-                  a, b, blocked, fusable && relu, fusable && emit.buf ? emit.buf + (long long)t * L * F : nullptr);
-  if (relu && !fusable) cnb_relu(targets->data_device, els);
-  if (fuse.act == kActLogistic) cnb_logistic(targets->data_device, els);
-  emit.done = fusable;
+    fused = rnorm_forward(images->data_device + (long long)t * L * F, targets->data_device + (long long)t * L * F, L, F,
+                          sizeF, a, b, blocked, relu, twin ? twin + (long long)t * L * F : nullptr);
+  if (relu && !fused) cnb_relu(targets->data_device, els);
+  if (logistic) cnb_logistic(targets->data_device, els);
+  emit.done = fused && !logistic;
   emit.finish();
 }
 void do_rnorm_undo(const char* what, cudamat* outGrads, cudamat* inputs, cudamat* targets, int F, int sizeF, float a,
                    float b, bool blocked, int frames) {
   Range nvtx_range(what);
-  CNB_REQUIRE(F > 0 && frames > 0, what);
-  const long long els = (long long)inputs->size[0] * inputs->size[1];
-  CNB_REQUIRE(els % ((long long)F * frames) == 0, what);
-  CNB_REQUIRE(targets->size[0] == inputs->size[0] && targets->size[1] == inputs->size[1], what);
-  CNB_REQUIRE(outGrads->size[0] == inputs->size[0] && outGrads->size[1] == inputs->size[1], what);
-  const long long L = els / F / frames;
+  const long long L = rnorm_locs(what, inputs, outGrads, targets, F, frames);
   const Fuse fuse = take_fuse();
   CNB_REQUIRE(!fuse.bias_grad, "ResponseNormCrossMapUndo: no fused bias gradient here");
-  Emit emit(targets->data_device, els, fuse.emit_bf16 != 0, false);
+  Emit emit(targets->data_device, L * F * frames, fuse.emit_bf16 != 0, false);
   for (int t = 0; t < frames; t++)
     rnorm_undo(outGrads->data_device + (long long)t * L * F, inputs->data_device + (long long)t * L * F,
                targets->data_device + (long long)t * L * F, L, F, sizeF, a, b, blocked);

@@ -134,6 +134,12 @@ void* workspace(size_t bytes);       // device scratch of at least `bytes`, vali
 int num_sms();
 inline int current_device() { int d = 0; CNB_CUDA_CHECK(cudaGetDevice(&d)); return d; }
 
+// lets `kernel` launch with up to `bytes` of dynamic shared memory (beyond the default 48 KiB) on the current device.  The
+// limit belongs to the (kernel, device) pair, so it is set once per pair, keyed by the kernel's address.
+void smem_opt_in(const void* kernel, int bytes);
+template <typename... KArgs>
+inline void smem_opt_in(void (*kernel)(KArgs...), int bytes) { smem_opt_in(reinterpret_cast<const void*>(kernel), bytes); }
+
 inline void count_launch(int n = 1) { state().launches += n; }
 inline Fuse take_fuse() { Fuse f = state().fuse; state().fuse = Fuse(); return f; }
 

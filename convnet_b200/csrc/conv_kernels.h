@@ -105,11 +105,12 @@ void max_pool_rprop(const PoolGeom& g, const float* images, const float* R_image
 // grad_bias[c] = st*grad_bias[c] + so * sum_slices part[slice*cols + c]   (elementwise.cu)
 void colsum_finish(const float* part, float* grad_bias, int cols, int slices, float st, float so);
 
-// rnorm.cu
-// relu / targets_bf16: fused epilogue (max(., 0); a bf16 copy of the output) — only when rnorm_can_fuse(numFilters)
-void rnorm_forward(const float* images, float* targets, long long num_locs, int numFilters, int sizeF,
-                   float addScale, float powScale, bool blocked, bool relu = false, __nv_bfloat16* targets_bf16 = nullptr);
-bool rnorm_can_fuse(int numFilters);
+// rnorm.cu — each call runs the tile kernel when one tile of numFilters channels fits in shared memory, else the ring
+// kernel.  The forward may fuse max(., 0) (`relu`) and write the bf16 twin `targets_bf16` (nullptr: none).  It returns
+// whether it did: true from the tile kernel, which applies both; false from the ring kernel, which applies neither, and
+// the caller then runs the ReLU and converts the twin as passes.
+bool rnorm_forward(const float* images, float* targets, long long num_locs, int numFilters, int sizeF,
+                   float addScale, float powScale, bool blocked, bool relu, __nv_bfloat16* targets_bf16);
 void rnorm_undo(const float* outGrads, const float* inputs, float* targets, long long num_locs,
                 int numFilters, int sizeF, float addScale, float powScale, bool blocked);
 // R-operator: t_j = R_j d_j^-b - 2ab x_j d_j^(-b-1) sum_{i in window(j)} x_i R_i,  d_j = 1 + a sum_{i in window(j)} x_i^2

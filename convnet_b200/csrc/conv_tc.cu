@@ -919,13 +919,7 @@ int pick_store_warps(int kblocks, double tile_bytes) {
 
 template <int OP, bool BF16, bool SIG, int SW>
 void launch_one(const CUtensorMap& a, const CUtensorMap& b, const TcParams& p, size_t smem) {
-  // the attribute belongs to the (function, device) pair: set it once per device this process launches on
-  static unsigned long long attr_devices = 0;
-  const int dev = current_device();
-  if (dev >= 64 || !((attr_devices >> dev) & 1ULL)) {
-    CNB_CUDA_CHECK(cudaFuncSetAttribute(tc_conv_kernel<OP, BF16, SIG, SW>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    if (dev < 64) attr_devices |= 1ULL << dev;
-  }
+  smem_opt_in(tc_conv_kernel<OP, BF16, SIG, SW>, 227 * 1024);
   const int grid = std::min(p.num_tiles, num_sms());
   launch_pdl(tc_conv_kernel<OP, BF16, SIG, SW>, dim3((unsigned)grid), dim3(kThreadsFor<SW>), smem, state().stream, a, b, p);
 }

@@ -1,6 +1,9 @@
 // ext.cu — library state, scratch, and the extension C API (include/convnet_b200_ext.h).
 #include <string.h>
 
+#include <set>
+#include <utility>
+
 #include "../../include/convnet_b200_ext.h"
 #include "common.cuh"
 #include "conv_kernels.h"
@@ -58,6 +61,12 @@ int num_sms() {
   }
   const int usable = s.num_sms - s.sm_reserve;
   return usable >= 8 ? usable : (s.num_sms < 8 ? s.num_sms : 8);
+}
+
+void smem_opt_in(const void* kernel, int bytes) {
+  static std::set<std::pair<const void*, int>> done;
+  if (done.insert({kernel, current_device()}).second)
+    CNB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
 }
 
 }  // namespace cnb

@@ -147,12 +147,7 @@ static void launch_mapnorm(const float* a, const float* b, const float* c, const
   const int TI = mapnorm_width(S, R, VEC == 4);
   const size_t smem = mapnorm_smem(S, R, TI);
   CNB_REQUIRE(smem <= 200 * 1024, UNDO ? "ResponseNormUndo: image too large for the row ring" : "ResponseNorm: image too large for the row ring");
-  static int attr_dev_mask = 0;
-  const int dev = current_device();
-  if (smem > 48 * 1024 && (dev >= 31 || !((attr_dev_mask >> dev) & 1))) {
-    CNB_CUDA_CHECK(cudaFuncSetAttribute(mapnorm_kernel<UNDO, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    if (dev < 31) attr_dev_mask |= 1 << dev;
-  }
+  smem_opt_in(mapnorm_kernel<UNDO, VEC>, 200 * 1024);
   const int off = UNDO ? sizeX / 2 - sizeX + 1 : -(sizeX / 2);
   launch_pdl(mapnorm_kernel<UNDO, VEC>, dim3((unsigned)ceil_div(N, TI), (unsigned)F), dim3(MN_THREADS), smem, state().stream,
              a, b, c, d, o0, o1, N, S, sizeX, off, R, TI, alpha, beta);

@@ -227,12 +227,12 @@ __global__ void __launch_bounds__(RN_THREADS) rnorm_undo_kernel(const float* __r
 
 
 // ------------------------------------------------------------------------------------------------
-// Tile kernels (the default whenever one tile fits in shared memory).
+// The tile kernel (the default whenever one tile fits in shared memory).
 //
 // The channel walk above is a serial dependency chain per location with its loads inside the chain, which leaves the
 // backward pass issue/latency-bound well below the HBM bandwidth.  Here a CTA owns a tile of TL consecutive locations x ALL
 // channels and works in phases that are either fully parallel or touch shared memory only:
-//   1. the whole x (and dy) tile is fetched with 16-byte cp.async — every load of the tile is in flight at once;
+//   1. the whole x (and dy or R) tile is fetched with 16-byte cp.async — every load of the tile is in flight at once;
 //   2. an exclusive prefix sum of x^2 along the channels is built in shared memory (a thread per (location, channel
 //      segment); two short passes: segment totals, then the running prefix offset by the earlier segments);
 //   3. every (channel, location) in parallel: S = Q[hi] - Q[lo] (the window sum as a prefix difference), base, one
@@ -289,150 +289,98 @@ __device__ __forceinline__ void rn_window(int i, int F, int k, int a, int b, boo
   else { lo = max(0, i - a); hi = min(F, i + b + 1); }
 }
 
-__device__ __forceinline__ void rn_store4(float* __restrict__ out, __nv_bfloat16* __restrict__ out16, long long off, float4 r,
-                                          int l, int valid, bool vec) {
+__device__ __forceinline__ void rn_store4(float* __restrict__ out, __nv_bfloat16* __restrict__ out16, long long off,
+                                          const float (&r)[4], int l, int valid, bool vec) {
   if (vec && valid >= l + 4) {
-    *reinterpret_cast<float4*>(out + off) = r;
+    rput<4>(out + off, r);
     if (out16) {
-      const __nv_bfloat162 lo = __floats2bfloat162_rn(r.x, r.y), hi = __floats2bfloat162_rn(r.z, r.w);
+      const __nv_bfloat162 lo = __floats2bfloat162_rn(r[0], r[1]), hi = __floats2bfloat162_rn(r[2], r[3]);
       uint2 o; o.x = *reinterpret_cast<const uint32_t*>(&lo); o.y = *reinterpret_cast<const uint32_t*>(&hi);
       *reinterpret_cast<uint2*>(out16 + off) = o;
     }
   } else {
-    const float rv[4] = {r.x, r.y, r.z, r.w};
+    const float rv[4] = {r[0], r[1], r[2], r[3]};      // indexing the caller's array would keep it out of registers
     for (int v = 0; v < 4; v++)
       if (l + v < valid) { out[off + v] = rv[v]; if (out16) out16[off + v] = __float2bfloat16_rn(rv[v]); }
   }
 }
 
-template <int TL>
-__global__ void __launch_bounds__(RN_THREADS) rnorm_fwd_tile_kernel(const float* __restrict__ x, float* __restrict__ y,
-                                                                     __nv_bfloat16* __restrict__ y16, long long L, int F,
-                                                                     int k, float alpha, float beta, int blocked, int relu,
-                                                                     int vec) {
-  pdl_wait();
-  pdl_trigger();
-  extern __shared__ __align__(16) float sm[];
-  float* X = sm;                               // [F][TL]
-  float* Q = X + (size_t)F * TL;               // [F+1][TL] exclusive prefix of x^2
-  float* segtot = Q + (size_t)(F + 1) * TL;    // [128/TL][TL]
-  const long long l0 = (long long)blockIdx.x * TL;
-  const int valid = (int)min((long long)TL, L - l0);
-  rn_load_tile<TL>(X, x, L, l0, F, valid, vec != 0);
-  rn_cp_wait_all();
-  __syncthreads();
-  rn_prefix<TL, true>(X, Q, segtot, F);
-  const int a = k / 2, b = k - a - 1;
-  constexpr int Q4 = TL / 4;
-  for (int idx = threadIdx.x; idx < F * Q4; idx += RN_THREADS) {
-    const int f = idx / Q4, l = 4 * (idx - f * Q4);
-    if (l >= valid) continue;
-    int lo, hi; rn_window(f, F, k, a, b, blocked != 0, lo, hi);
-    const float4 qh = *reinterpret_cast<const float4*>(Q + hi * TL + l), ql = *reinterpret_cast<const float4*>(Q + lo * TL + l);
-    const float4 xv = *reinterpret_cast<const float4*>(X + f * TL + l);
-    float4 r;
-    r.x = xv.x * __powf(1.f + alpha * (qh.x - ql.x), -beta);
-    r.y = xv.y * __powf(1.f + alpha * (qh.y - ql.y), -beta);
-    r.z = xv.z * __powf(1.f + alpha * (qh.z - ql.z), -beta);
-    r.w = xv.w * __powf(1.f + alpha * (qh.w - ql.w), -beta);
-    if (relu) { r.x = fmaxf(r.x, 0.f); r.y = fmaxf(r.y, 0.f); r.z = fmaxf(r.z, 0.f); r.w = fmaxf(r.w, 0.f); }
-    rn_store4(y, y16, (long long)f * L + l0 + l, r, l, valid, vec != 0);
-  }
-}
+// fn(0) .. fn(3): the per-element arithmetic of the tile kernel, written once.  Not a `#pragma unroll` loop: that is
+// unrolled only after the compiler has decided whether to specialise the enclosing loop, and it then decides otherwise.
+template <class Fn> __device__ __forceinline__ void for4(Fn fn) { fn(0); fn(1); fn(2); fn(3); }
 
-template <int TL>
-__global__ void __launch_bounds__(RN_THREADS) rnorm_undo_tile_kernel(const float* __restrict__ dy, const float* __restrict__ x,
-                                                                      float* __restrict__ dx, long long L, int F, int k,
-                                                                      float alpha, float beta, int blocked, int vec) {
-  pdl_wait();
-  pdl_trigger();
-  extern __shared__ __align__(16) float sm[];
-  float* X = sm;                               // [F][TL]
-  float* G = X + (size_t)F * TL;               // [F][TL]   dy, then p = dy * base^(-beta)
-  float* Q = G + (size_t)F * TL;               // [F+1][TL] exclusive prefix of x^2
-  float* T = Q + (size_t)(F + 1) * TL;         // [F+1][TL] t = dy * x * base^(-beta-1), then its exclusive prefix
-  float* segtot = T + (size_t)(F + 1) * TL;
-  const long long l0 = (long long)blockIdx.x * TL;
-  const int valid = (int)min((long long)TL, L - l0);
-  rn_load_tile<TL>(X, x, L, l0, F, valid, vec != 0);
-  rn_load_tile<TL>(G, dy, L, l0, F, valid, vec != 0);
-  rn_cp_wait_all();
-  __syncthreads();
-  rn_prefix<TL, true>(X, Q, segtot, F);
-  const int a = k / 2, b = k - a - 1;
-  constexpr int Q4 = TL / 4;
-  for (int idx = threadIdx.x; idx < F * Q4; idx += RN_THREADS) {
-    const int f = idx / Q4, l = 4 * (idx - f * Q4);
-    int lo, hi; rn_window(f, F, k, a, b, blocked != 0, lo, hi);
-    const float4 qh = *reinterpret_cast<const float4*>(Q + hi * TL + l), ql = *reinterpret_cast<const float4*>(Q + lo * TL + l);
-    const float4 xv = *reinterpret_cast<const float4*>(X + f * TL + l), g = *reinterpret_cast<const float4*>(G + f * TL + l);
-    float4 t, p;
-    { const float base = 1.f + alpha * (qh.x - ql.x), den = __powf(base, -beta - 1.f); t.x = g.x * xv.x * den; p.x = g.x * den * base; }
-    { const float base = 1.f + alpha * (qh.y - ql.y), den = __powf(base, -beta - 1.f); t.y = g.y * xv.y * den; p.y = g.y * den * base; }
-    { const float base = 1.f + alpha * (qh.z - ql.z), den = __powf(base, -beta - 1.f); t.z = g.z * xv.z * den; p.z = g.z * den * base; }
-    { const float base = 1.f + alpha * (qh.w - ql.w), den = __powf(base, -beta - 1.f); t.w = g.w * xv.w * den; p.w = g.w * den * base; }
-    *reinterpret_cast<float4*>(T + f * TL + l) = t;
-    *reinterpret_cast<float4*>(G + f * TL + l) = p;
-  }
-  __syncthreads();
-  rn_prefix<TL, false>(T, T, segtot, F);
-  const float c2 = 2.f * alpha * beta;
-  for (int idx = threadIdx.x; idx < F * Q4; idx += RN_THREADS) {
-    const int j = idx / Q4, l = 4 * (idx - j * Q4);
-    if (l >= valid) continue;
-    int lo, hi;                                                       // inverse window: [j-b, j+a]
-    if (blocked) { lo = (j / k) * k; hi = min(F, lo + k); } else { lo = max(0, j - b); hi = min(F, j + a + 1); }
-    const float4 rh = *reinterpret_cast<const float4*>(T + hi * TL + l), rl = *reinterpret_cast<const float4*>(T + lo * TL + l);
-    const float4 xv = *reinterpret_cast<const float4*>(X + j * TL + l), p = *reinterpret_cast<const float4*>(G + j * TL + l);
-    float4 r;
-    r.x = p.x - c2 * xv.x * (rh.x - rl.x); r.y = p.y - c2 * xv.y * (rh.y - rl.y);
-    r.z = p.z - c2 * xv.z * (rh.z - rl.z); r.w = p.w - c2 * xv.w * (rh.w - rl.w);
-    rn_store4(dx, nullptr, (long long)j * L + l0 + l, r, l, valid, vec != 0);
-  }
-}
-
-// R-operator (kCrossMapRNormRprop, gemm.cu:491-514): the directional derivative of the forward pass along R,
+// One kernel for the three passes; `in2` is the second input (undo: dy, R-operator: R; unused by the forward).  The
+// R-operator (kCrossMapRNormRprop, gemm.cu:491-514) is the directional derivative of the forward pass along R,
 //   t_j = R_j base_j^-beta - 2 alpha beta x_j base_j^(-beta-1) sum_{i in window(j)} x_i R_i,  base_j = 1 + alpha S_j,
-// with the FORWARD window of j for both sums.  Same phases as the forward tile: x and R tiles, exclusive prefixes of x^2
-// (Q) and of x R (P) along the channels, then every (channel, location) from two prefix differences and one __powf.
-template <int TL>
-__global__ void __launch_bounds__(RN_THREADS) rnorm_rprop_tile_kernel(const float* __restrict__ x, const float* __restrict__ rx,
-                                                                       float* __restrict__ out, long long L, int F, int k,
-                                                                       float alpha, float beta, int blocked, int vec) {
+// with the FORWARD window of j for both sums: it builds the prefix of x R beside that of x^2 and takes both window sums
+// as prefix differences.
+enum RnPass { kRnForward, kRnUndo, kRnRprop };
+
+template <int TL, RnPass PASS>
+__global__ void __launch_bounds__(RN_THREADS) rnorm_tile_kernel(const float* __restrict__ x, const float* __restrict__ in2,
+                                                                 float* __restrict__ out, __nv_bfloat16* __restrict__ out16,
+                                                                 long long L, int F, int k, float alpha, float beta,
+                                                                 int blocked, int relu, int vec) {
+  constexpr int VEC = 4;                       // a thread takes four consecutive locations of one channel per step
   pdl_wait();
   pdl_trigger();
   extern __shared__ __align__(16) float sm[];
-  float* X = sm;                               // [F][TL]
-  float* Rv = X + (size_t)F * TL;              // [F][TL]
-  float* Q = Rv + (size_t)F * TL;              // [F+1][TL] exclusive prefix of x^2
-  float* P = Q + (size_t)(F + 1) * TL;         // [F+1][TL] x R, then its exclusive prefix
-  float* segtot = P + (size_t)(F + 1) * TL;
+  float* X = sm;                                                // [F][TL]
+  float* G = X + (size_t)F * TL;                                // [F][TL]   undo: dy, then p;  R-operator: R
+  float* Q = PASS == kRnForward ? G : G + (size_t)F * TL;       // [F+1][TL] exclusive prefix of x^2
+  float* T = Q + (size_t)(F + 1) * TL;         // [F+1][TL] undo: t, then its exclusive prefix;  R-operator: x R, then its prefix
+  float* segtot = PASS == kRnForward ? T : T + (size_t)(F + 1) * TL;
   const long long l0 = (long long)blockIdx.x * TL;
   const int valid = (int)min((long long)TL, L - l0);
   rn_load_tile<TL>(X, x, L, l0, F, valid, vec != 0);
-  rn_load_tile<TL>(Rv, rx, L, l0, F, valid, vec != 0);
+  if constexpr (PASS != kRnForward) rn_load_tile<TL>(G, in2, L, l0, F, valid, vec != 0);
   rn_cp_wait_all();
   __syncthreads();
-  for (int idx = threadIdx.x; idx < F * TL; idx += RN_THREADS) P[idx] = X[idx] * Rv[idx];
-  __syncthreads();
+  if constexpr (PASS == kRnRprop) {
+    for (int idx = threadIdx.x; idx < F * TL; idx += RN_THREADS) T[idx] = X[idx] * G[idx];
+    __syncthreads();
+  }
   rn_prefix<TL, true>(X, Q, segtot, F);
-  rn_prefix<TL, false>(P, P, segtot, F);
+  if constexpr (PASS == kRnRprop) rn_prefix<TL, false>(T, T, segtot, F);
   const int a = k / 2, b = k - a - 1;
   const float c2 = 2.f * alpha * beta;
   constexpr int Q4 = TL / 4;
   for (int idx = threadIdx.x; idx < F * Q4; idx += RN_THREADS) {
     const int f = idx / Q4, l = 4 * (idx - f * Q4);
-    if (l >= valid) continue;
+    if (PASS != kRnUndo && l >= valid) continue;       // the undo fills the padding lanes too: its prefix reads them
     int lo, hi; rn_window(f, F, k, a, b, blocked != 0, lo, hi);
-    const float4 qh = *reinterpret_cast<const float4*>(Q + hi * TL + l), ql = *reinterpret_cast<const float4*>(Q + lo * TL + l);
-    const float4 ph = *reinterpret_cast<const float4*>(P + hi * TL + l), pl = *reinterpret_cast<const float4*>(P + lo * TL + l);
-    const float4 xv = *reinterpret_cast<const float4*>(X + f * TL + l), rv = *reinterpret_cast<const float4*>(Rv + f * TL + l);
-    float4 r;
-    { const float base = 1.f + alpha * (qh.x - ql.x), den = __powf(base, -beta - 1.f); r.x = rv.x * (den * base) - c2 * xv.x * den * (ph.x - pl.x); }
-    { const float base = 1.f + alpha * (qh.y - ql.y), den = __powf(base, -beta - 1.f); r.y = rv.y * (den * base) - c2 * xv.y * den * (ph.y - pl.y); }
-    { const float base = 1.f + alpha * (qh.z - ql.z), den = __powf(base, -beta - 1.f); r.z = rv.z * (den * base) - c2 * xv.z * den * (ph.z - pl.z); }
-    { const float base = 1.f + alpha * (qh.w - ql.w), den = __powf(base, -beta - 1.f); r.w = rv.w * (den * base) - c2 * xv.w * den * (ph.w - pl.w); }
-    rn_store4(out, nullptr, (long long)f * L + l0 + l, r, l, valid, vec != 0);
+    float qh[VEC], ql[VEC], xv[VEC], g[VEC], th[VEC], tl[VEC], r[VEC], p[VEC];
+    rget<VEC>(Q + hi * TL + l, qh); rget<VEC>(Q + lo * TL + l, ql);
+    if constexpr (PASS == kRnRprop) { rget<VEC>(T + hi * TL + l, th); rget<VEC>(T + lo * TL + l, tl); }
+    rget<VEC>(X + f * TL + l, xv);
+    if constexpr (PASS != kRnForward) rget<VEC>(G + f * TL + l, g);
+    for4([&](int v) {
+      const float base = 1.f + alpha * (qh[v] - ql[v]);
+      if constexpr (PASS == kRnForward) {
+        r[v] = xv[v] * __powf(base, -beta);
+      } else {
+        const float den = __powf(base, -beta - 1.f);
+        if constexpr (PASS == kRnUndo) { r[v] = g[v] * xv[v] * den; p[v] = g[v] * den * base; }
+        else r[v] = g[v] * (den * base) - c2 * xv[v] * den * (th[v] - tl[v]);
+      }
+    });
+    if constexpr (PASS == kRnForward) { if (relu) for4([&](int v) { r[v] = fmaxf(r[v], 0.f); }); }
+    if constexpr (PASS == kRnUndo) { rput<VEC>(T + f * TL + l, r); rput<VEC>(G + f * TL + l, p); }
+    else rn_store4(out, PASS == kRnForward ? out16 : nullptr, (long long)f * L + l0 + l, r, l, valid, vec != 0);
+  }
+  if constexpr (PASS == kRnUndo) {
+    __syncthreads();
+    rn_prefix<TL, false>(T, T, segtot, F);
+    for (int idx = threadIdx.x; idx < F * Q4; idx += RN_THREADS) {
+      const int j = idx / Q4, l = 4 * (idx - j * Q4);
+      if (l >= valid) continue;
+      int lo, hi; rn_window(j, F, k, b, a, blocked != 0, lo, hi);       // the inverse window: [j-b, j+a]
+      float th[VEC], tl[VEC], xv[VEC], p[VEC];
+      rget<VEC>(T + hi * TL + l, th); rget<VEC>(T + lo * TL + l, tl);
+      rget<VEC>(X + j * TL + l, xv); rget<VEC>(G + j * TL + l, p);
+      for4([&](int v) { p[v] -= c2 * xv[v] * (th[v] - tl[v]); });
+      rn_store4(out, nullptr, (long long)j * L + l0 + l, p, l, valid, vec != 0);
+    }
   }
 }
 
@@ -483,132 +431,95 @@ __global__ void __launch_bounds__(RN_THREADS) rnorm_rprop_kernel(const float* __
   }
 }
 
+// the shared memory a tile CTA may use; pick_tile sizes the tiles against it
+static constexpr int kTileSmem = 224 * 1024;
+
 // tile width for `arrays` F-row arrays (+2 spare rows and the segment totals): the widest of 64 / 32 that lets two CTAs
 // share an SM, else the widest that fits at all; 0 = no tile kernel (window walk with the ring instead)
 static int pick_tile(int F, int arrays, size_t* smem_out) {
   auto bytes = [&](int tl) { return sizeof(float) * ((size_t)arrays * (F + 1) * tl + RN_THREADS); };
   // a CTA works in phases (load everything, scan, compute, store): the loads of one CTA only overlap the arithmetic of
   // ANOTHER one on the same SM, so prefer the width that leaves room for >= 3 resident CTAs, then 2, then whatever fits
-  const size_t sm = 224 * 1024;
   for (int per_sm : {3, 2, 1})
     for (int tl : {64, 32})
-      if (bytes(tl) + 1024 <= sm / per_sm) { *smem_out = bytes(tl); return tl; }
+      if (bytes(tl) + 1024 <= (size_t)kTileSmem / per_sm) { *smem_out = bytes(tl); return tl; }
   return 0;
+}
+
+// runs the tile kernel of PASS when one tile of F channels fits in shared memory (the forward keeps two arrays per tile,
+// the undo and the R-operator four); false: nothing was launched
+template <RnPass PASS>
+static bool launch_tile(const float* x, const float* in2, float* out, __nv_bfloat16* out16, long long L, int F, int k,
+                        float alpha, float beta, bool blocked, bool relu, const char* what) {
+  size_t smem = 0;
+  const int tl = pick_tile(F, PASS == kRnForward ? 2 : 4, &smem);
+  if (!tl) return false;
+  const bool vec = L % 4 == 0 && aligned16(x) && aligned16(in2) && aligned16(out) &&
+                   (reinterpret_cast<uintptr_t>(out16) & 7) == 0;
+  auto kern = tl == 64 ? rnorm_tile_kernel<64, PASS> : rnorm_tile_kernel<32, PASS>;
+  smem_opt_in(kern, kTileSmem);
+  launch_pdl(kern, dim3((unsigned)ceil_div<long long>(L, tl)), dim3(RN_THREADS), smem, state().stream, x, in2, out, out16,
+             L, F, k, alpha, beta, blocked ? 1 : 0, relu ? 1 : 0, vec ? 1 : 0);
+  count_launch();
+  CNB_LAUNCH_CHECK(what);
+  return true;
 }
 
 static constexpr size_t kMaxRingSmem = 160 * 1024;
 
-// channel segments per location: 1 unless the location count cannot fill the GPU
-static int pick_segments(long long L, int F, int k) {
-  const long long blocks = ceil_div<long long>(L, RN_THREADS);
+// The grid of a ring kernel that walks the channels with `rings` rings of k entries for each of `vec` locations per thread.
+// blockIdx.y is a channel segment: one segment unless the location count cannot fill the GPU.  The rings live in shared
+// memory when they fit in kMaxRingSmem, else in workspace, one set per segment.
+struct RingLaunch { dim3 grid; int seg; size_t smem; float* gring; };
+static RingLaunch ring_launch(long long L, int F, int k, bool blocked, int vec, int rings) {
+  const long long owners = L / vec;                      // threads needed
+  const long long blocks = ceil_div<long long>(owners, RN_THREADS);
   const long long want = ceil_div<long long>(2LL * num_sms(), blocks);
   int segs = (int)std::min<long long>(want, std::max(1, F / std::max(k, 1)));      // segment >= k: halo <= 2x / 3x reads
   if (segs < 1) segs = 1;
-  return segs;
+  RingLaunch r;
+  r.seg = ceil_div(F, segs);
+  if (blocked) r.seg = ceil_div(r.seg, k) * k;
+  segs = ceil_div(F, r.seg);
+  r.grid = dim3((unsigned)blocks, segs);
+  r.smem = sizeof(float) * rings * (size_t)k * RN_THREADS * vec;
+  r.gring = nullptr;
+  if (r.smem > kMaxRingSmem) { r.gring = (float*)workspace(sizeof(float) * rings * (size_t)k * L * segs); r.smem = 0; }
+  return r;
 }
 
-template <int VEC>
-static void launch_fwd(const float* images, float* targets, long long L, int F, int k, float alpha, float beta, bool blocked) {
-  const long long owners = L / VEC;                      // threads needed
-  const int blocks = (int)ceil_div<long long>(owners, RN_THREADS);
-  int segs = pick_segments(owners, F, k);
-  int seg = ceil_div(F, segs);
-  if (blocked) seg = ceil_div(seg, k) * k;
-  segs = ceil_div(F, seg);
-  size_t smem = sizeof(float) * (size_t)k * RN_THREADS * VEC;
-  float* gring = nullptr;
-  if (smem > kMaxRingSmem) { gring = (float*)workspace(sizeof(float) * (size_t)k * L * segs); smem = 0; }
-  auto kern = blocked ? rnorm_fwd_kernel<true, VEC> : rnorm_fwd_kernel<false, VEC>;
-  if (smem > 48 * 1024) CNB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<dim3(blocks, segs), RN_THREADS, smem, state().stream>>>(images, targets, L, F, k, alpha, beta, gring, L, seg);
-}
-
-template <int TL>
-static void launch_fwd_tile(const float* images, float* targets, __nv_bfloat16* t16, long long L, int F, int k, float alpha,
-                            float beta, bool blocked, bool relu, size_t smem, bool vec) {
-  static int attr_dev_mask = 0;
-  const int dev = current_device();
-  if (smem > 48 * 1024 && (dev >= 31 || !((attr_dev_mask >> dev) & 1))) {
-    CNB_CUDA_CHECK(cudaFuncSetAttribute(rnorm_fwd_tile_kernel<TL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-    if (dev < 31) attr_dev_mask |= 1 << dev;
-  }
-  const long long tiles = ceil_div<long long>(L, TL);
-  launch_pdl(rnorm_fwd_tile_kernel<TL>, dim3((unsigned)tiles), dim3(RN_THREADS), smem, state().stream, images, targets, t16, L, F, k,
-             alpha, beta, blocked ? 1 : 0, relu ? 1 : 0, vec ? 1 : 0);
-}
-template <int TL>
-static void launch_undo_tile(const float* outGrads, const float* inputs, float* targets, long long L, int F, int k, float alpha,
-                             float beta, bool blocked, size_t smem, bool vec) {
-  static int attr_dev_mask = 0;
-  const int dev = current_device();
-  if (smem > 48 * 1024 && (dev >= 31 || !((attr_dev_mask >> dev) & 1))) {
-    CNB_CUDA_CHECK(cudaFuncSetAttribute(rnorm_undo_tile_kernel<TL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-    if (dev < 31) attr_dev_mask |= 1 << dev;
-  }
-  const long long tiles = ceil_div<long long>(L, TL);
-  launch_pdl(rnorm_undo_tile_kernel<TL>, dim3((unsigned)tiles), dim3(RN_THREADS), smem, state().stream, outGrads, inputs, targets, L,
-             F, k, alpha, beta, blocked ? 1 : 0, vec ? 1 : 0);
-}
-
-void rnorm_forward(const float* images, float* targets, long long L, int F, int k, float alpha, float beta,
-                   bool blocked, bool relu, __nv_bfloat16* targets_bf16) {
+bool rnorm_forward(const float* images, float* targets, long long L, int F, int k, float alpha, float beta, bool blocked,
+                   bool relu, __nv_bfloat16* targets_bf16) {
   CNB_REQUIRE(k >= 1 && F >= 1, "ResponseNormCrossMap");
-  size_t tsmem = 0;
-  const int tl = L < (1LL << 31) * 32 ? pick_tile(F, 2, &tsmem) : 0;
-  if (tl) {
-    const bool vec = L % 4 == 0 && aligned16(images) && aligned16(targets) &&
-                     (!targets_bf16 || (reinterpret_cast<uintptr_t>(targets_bf16) & 7) == 0);
-    if (tl == 64) launch_fwd_tile<64>(images, targets, targets_bf16, L, F, k, alpha, beta, blocked, relu, tsmem, vec);
-    else launch_fwd_tile<32>(images, targets, targets_bf16, L, F, k, alpha, beta, blocked, relu, tsmem, vec);
-    count_launch();
-    CNB_LAUNCH_CHECK("rnorm_forward(tile)");
-    return;
-  }
-  CNB_REQUIRE(!relu && !targets_bf16, "rnorm_forward: the ring fallback has no fused epilogue (callers check rnorm_can_fuse)");
+  if (launch_tile<kRnForward>(images, nullptr, targets, targets_bf16, L, F, k, alpha, beta, blocked, relu,
+                              "rnorm_forward(tile)"))
+    return true;
   // four locations per thread only when that still leaves >= 4 blocks per SM: the channel walk is a serial dependency
   // chain, so small problems need the thread count more than the shorter instruction stream (measured: 105 -> 75 us on
   // 96 x 55 x 55 x 128, but 39 -> 47 us on 256 x 14 x 14 x 128)
   const bool wide = L % 4 == 0 && aligned16(images) && aligned16(targets) && L / 4 / RN_THREADS >= 4LL * num_sms();
-  if (wide) launch_fwd<4>(images, targets, L, F, k, alpha, beta, blocked);
-  else launch_fwd<1>(images, targets, L, F, k, alpha, beta, blocked);
+  const RingLaunch r = ring_launch(L, F, k, blocked, wide ? 4 : 1, 1);
+  auto kern = wide ? (blocked ? rnorm_fwd_kernel<true, 4> : rnorm_fwd_kernel<false, 4>)
+                   : (blocked ? rnorm_fwd_kernel<true, 1> : rnorm_fwd_kernel<false, 1>);
+  smem_opt_in(kern, kMaxRingSmem);
+  kern<<<r.grid, RN_THREADS, r.smem, state().stream>>>(images, targets, L, F, k, alpha, beta, r.gring, L, r.seg);
   count_launch();
   CNB_LAUNCH_CHECK("rnorm_forward");
+  return false;
 }
-
-// one location per thread: the backward walk carries three rings and two dependent stages per channel, so it is
-// latency-bound, and a version with four locations per thread (a quarter of the threads, 4x the shared memory per block)
-// was slower when measured before the port to the H100
-static void launch_undo(const float* outGrads, const float* inputs, float* targets, long long L, int F, int k, float alpha,
-                        float beta, bool blocked) {
-  const int blocks = (int)ceil_div<long long>(L, RN_THREADS);
-  int segs = pick_segments(L, F, k);
-  int seg = ceil_div(F, segs);
-  if (blocked) seg = ceil_div(seg, k) * k;
-  segs = ceil_div(F, seg);
-  size_t smem = sizeof(float) * 3 * (size_t)k * RN_THREADS;
-  float* gring = nullptr;
-  if (smem > kMaxRingSmem) { gring = (float*)workspace(sizeof(float) * 3 * (size_t)k * L * segs); smem = 0; }
-  auto kern = blocked ? rnorm_undo_kernel<true> : rnorm_undo_kernel<false>;
-  if (smem > 48 * 1024) CNB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<dim3(blocks, segs), RN_THREADS, smem, state().stream>>>(outGrads, inputs, targets, L, F, k, alpha, beta, gring, L, seg);
-}
-
-bool rnorm_can_fuse(int F) { size_t b; return pick_tile(F, 2, &b) != 0; }
 
 void rnorm_undo(const float* outGrads, const float* inputs, float* targets, long long L, int F, int k,
                 float alpha, float beta, bool blocked) {
   CNB_REQUIRE(k >= 1 && F >= 1, "ResponseNormCrossMapUndo");
-  size_t tsmem = 0;
-  const int tl = pick_tile(F, 4, &tsmem);
-  if (tl) {
-    const bool vec = L % 4 == 0 && aligned16(outGrads) && aligned16(inputs) && aligned16(targets);
-    if (tl == 64) launch_undo_tile<64>(outGrads, inputs, targets, L, F, k, alpha, beta, blocked, tsmem, vec);
-    else launch_undo_tile<32>(outGrads, inputs, targets, L, F, k, alpha, beta, blocked, tsmem, vec);
-    count_launch();
-    CNB_LAUNCH_CHECK("rnorm_undo(tile)");
+  if (launch_tile<kRnUndo>(inputs, outGrads, targets, nullptr, L, F, k, alpha, beta, blocked, false, "rnorm_undo(tile)"))
     return;
-  }
-  launch_undo(outGrads, inputs, targets, L, F, k, alpha, beta, blocked);
+  // one location per thread: the backward walk carries three rings and two dependent stages per channel, so it is
+  // latency-bound, and a version with four locations per thread (a quarter of the threads, 4x the shared memory per
+  // block) was slower when measured before the port to the H100
+  const RingLaunch r = ring_launch(L, F, k, blocked, 1, 3);
+  auto kern = blocked ? rnorm_undo_kernel<true> : rnorm_undo_kernel<false>;
+  smem_opt_in(kern, kMaxRingSmem);
+  kern<<<r.grid, RN_THREADS, r.smem, state().stream>>>(outGrads, inputs, targets, L, F, k, alpha, beta, r.gring, L, r.seg);
   count_launch();
   CNB_LAUNCH_CHECK("rnorm_undo");
 }
@@ -616,27 +527,15 @@ void rnorm_undo(const float* outGrads, const float* inputs, float* targets, long
 void rnorm_rprop(const float* images, const float* R_images, float* targets, long long L, int F, int k, float alpha,
                  float beta, bool blocked) {
   CNB_REQUIRE(k >= 1 && F >= 1, "ResponseNormCrossMapRpropGemm");
-  cudaStream_t s = state().stream;
-  size_t tsmem = 0;
-  const int tl = L < (1LL << 31) * 32 ? pick_tile(F, 4, &tsmem) : 0;
-  if (tl) {
-    const bool vec = L % 4 == 0 && aligned16(images) && aligned16(R_images) && aligned16(targets);
-    const long long tiles = ceil_div<long long>(L, tl);
-    auto kern = tl == 64 ? rnorm_rprop_tile_kernel<64> : rnorm_rprop_tile_kernel<32>;
-    if (tsmem > 48 * 1024) CNB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tsmem));
-    launch_pdl(kern, dim3((unsigned)tiles), dim3(RN_THREADS), tsmem, s, images, R_images, targets, L, F, k, alpha, beta,
-               blocked ? 1 : 0, vec ? 1 : 0);
-    count_launch();
-    CNB_LAUNCH_CHECK("rnorm_rprop(tile)");
+  if (launch_tile<kRnRprop>(images, R_images, targets, nullptr, L, F, k, alpha, beta, blocked, false, "rnorm_rprop(tile)"))
     return;
-  }
   size_t smem = sizeof(float) * 2 * (size_t)k * RN_THREADS;
   float* gring = nullptr;
   if (smem > kMaxRingSmem) { gring = (float*)workspace(sizeof(float) * 2 * (size_t)k * L); smem = 0; }
   auto kern = blocked ? rnorm_rprop_kernel<true> : rnorm_rprop_kernel<false>;
-  if (smem > 48 * 1024) CNB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<(unsigned)ceil_div<long long>(L, RN_THREADS), RN_THREADS, smem, s>>>(images, R_images, targets, L, F, k, alpha, beta,
-                                                                             gring, L);
+  smem_opt_in(kern, kMaxRingSmem);
+  kern<<<(unsigned)ceil_div<long long>(L, RN_THREADS), RN_THREADS, smem, state().stream>>>(images, R_images, targets, L, F,
+                                                                                          k, alpha, beta, gring, L);
   count_launch();
   CNB_LAUNCH_CHECK("rnorm_rprop");
 }

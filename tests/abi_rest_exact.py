@@ -184,9 +184,9 @@ def max_rprop_branch(N, aligned=True):
 
 
 def rnorm_rprop_branch(L, F, blocked, aligned=True):
-    tl = px.pick_tile(F, 4) if L < 2 ** 31 * 32 else 0
+    tl = px.pick_tile(F, 4)
     if tl:
-        return "rnorm_rprop_tile_kernel<%d>" % tl, ("vec" if L % 4 == 0 and aligned else "scalar")
+        return "rnorm_tile_kernel<%d, (cnb::RnPass)2>" % tl, ("vec" if L % 4 == 0 and aligned else "scalar")
     return "rnorm_rprop_kernel<%s>" % ("true" if blocked else "false"), "ring"
 
 

@@ -557,6 +557,7 @@ def _segments(owners, F, k, blocked, sms):
 
 
 def rnorm_can_fuse(F):
+    """rnorm_forward's result: its kernel applied the ReLU and wrote the twin (the tile kernel) or neither (the ring)"""
     return pick_tile(F, 2) != 0
 
 
@@ -565,11 +566,11 @@ def rnorm_fwd_branch(L, F, k, blocked, aligned=True, sms=SMS):
     shared-memory or global ring); after '|' the partial last tile / channel segments, which are not branches of their
     own but must each be reached by a case."""
     bl = "true" if blocked else "false"
-    tl = pick_tile(F, 2) if L < 2 ** 31 * 32 else 0
+    tl = pick_tile(F, 2)
     if tl:
         vec = L % 4 == 0 and aligned
         return Branch("tile_fwd<%d,%s>%s" % (tl, "vec" if vec else "scalar", "|partial" if L % tl else ""),
-                      "rnorm_fwd_tile_kernel<%d>" % tl, True)
+                      "rnorm_tile_kernel<%d, (cnb::RnPass)0>" % tl, True)
     wide = L % 4 == 0 and aligned and L // 4 // 128 >= 4 * sms
     v = 4 if wide else 1
     segs = _segments(L // v, F, k, blocked, sms)
@@ -583,7 +584,7 @@ def rnorm_undo_branch(L, F, k, blocked, aligned=True, sms=SMS):
     if tl:
         vec = L % 4 == 0 and aligned
         return Branch("tile_undo<%d,%s>%s" % (tl, "vec" if vec else "scalar", "|partial" if L % tl else ""),
-                      "rnorm_undo_tile_kernel<%d>" % tl, False)
+                      "rnorm_tile_kernel<%d, (cnb::RnPass)1>" % tl, False)
     segs = _segments(L, F, k, blocked, sms)
     ring = "gring" if 4 * 3 * k * 128 > 160 * 1024 else "smem"
     bl = "true" if blocked else "false"

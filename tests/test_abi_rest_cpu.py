@@ -236,6 +236,6 @@ def test_module_level_names():
 def test_dispatch_mirror():
     assert ax.innerp_splits(8, 12 * 5)[0] == 1
     assert ax.innerp_splits(128, 96 * 27 * 27)[0] > 1
-    assert ax.rnorm_rprop_branch(1000, 32, False)[0] == "rnorm_rprop_tile_kernel<64>"
+    assert ax.rnorm_rprop_branch(1000, 32, False)[0] == "rnorm_tile_kernel<64, (cnb::RnPass)2>"
     assert ax.rnorm_rprop_branch(1000, 512, True) == ("rnorm_rprop_kernel<true>", "ring")
     assert ax.mapnorm_width(55, 5, True) == 16

@@ -244,7 +244,7 @@ def test_control_twin_rounding():
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# 3. the window-sum bar: an fp32 emulation of the tile kernel's prefix sums (rn_prefix, rnorm_fwd_tile_kernel)
+# 3. the window-sum bar: an fp32 emulation of the tile kernel's prefix sums (rn_prefix, rnorm_tile_kernel)
 # ---------------------------------------------------------------------------------------------------------------------
 def _tile_fwd_emulated(x, F_, k, alpha, beta, TL):
     """x: (F, L) float32.  The kernel's exclusive fp32 prefix of x^2 in 128/TL channel segments (segment totals, then the

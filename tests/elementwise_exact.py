@@ -21,8 +21,8 @@ Three kinds of expectation.
     u >= p; the value is fl(x * scale) or x * 0, the mask scale or 0;
   - the mask multiply fl(a * b);
   - every bf16 twin: the round-to-nearest-even bf16 of the fp32 value the kernel stored.
-* BIT-EXACT GIVEN THE KERNEL'S OWN INPUTS.  The SASS of bn_apply_kernel is FADD (x - mu), an IEEE division for
-  gamma / sigma (MUFU.RCP and its FFMA fix-up), one FFMA, FMNMX; bn_backward_kernel is FADD (x - mu), the IEEE
+* BIT-EXACT GIVEN THE KERNEL'S OWN INPUTS.  The SASS of bn_channel_kernel<BnApplyOp> is FADD (x - mu), an IEEE division
+  for gamma / sigma (MUFU.RCP and its FFMA fix-up), one FFMA, FMNMX; <BnBackOp> is FADD (x - mu), the IEEE
   reciprocal of sigma, FMUL (gamma * inv), FMUL ((x - mu) * inv), FADD (d - E[d]), FFMA with the product negated,
   FMUL.  So, with mu and sigma the ones the call was given (or the kernel wrote) and the kernel's own grad_gamma /
   grad_beta:
@@ -428,15 +428,15 @@ def _gs(work, sms):
 
 def bias_branch(rows, cols, aligned, relu, sms=SMS):
     vec = rows % 4 == 0 and aligned
-    k = "bias_kernel<%s>" % ("true" if relu else "false") if vec else \
-        "bias_kernel_scalar<%s>" % ("true" if relu else "false")
+    k = "stream_kernel<cnb::BiasOp<%d>" % (1 if relu else 0)
     work = rows // 4 * cols if vec else rows * cols
     return Branch("bias%s<%s>%s" % ("_relu" if relu else "", "vec" if vec else "scalar", _gs(work, sms)), [k],
                   "pass" if aligned else "none")
 
 
-_N4_KERNEL = {"relu": "relu_kernel", "relu_deriv": "relu_deriv_kernel", "dropout": "dropout_kernel",
-              "mult": "mult_kernel"}
+# the act template argument is the library's Act: 1 = ReLU (demanglers differ in writing the closing "> >")
+_N4_KERNEL = {"relu": "stream_kernel<cnb::ActOp<1>", "relu_deriv": "stream_kernel<cnb::ActDerivOp<1>",
+              "dropout": "stream_kernel<cnb::DropOp>", "mult": "stream_kernel<cnb::MultOp>"}
 
 
 def n4_of(n, aligned_all):
@@ -458,7 +458,7 @@ def colsum_slices_name(slices, cap):
 def bias_grad_branch(rows, cols, st, sms=SMS):
     s = bias_grad_slices(rows, cols, sms)
     return Branch("bias_grad<%s slices>%s" % (colsum_slices_name(s, 64), "|st" if st != 0 else ""),
-                  ["colsum_partial_kernel<cnb::SumOp, false>", "colsum_final_kernel"])
+                  ["colsum_partial_kernel<cnb::SumOp, false>", "colsum_final_kernel<cnb::BiasGradFin>"])
 
 
 def bn_slices(n, C, sms=SMS):
@@ -477,15 +477,15 @@ def bn_stats_branch(n, C, aligned_x, run, sms=SMS):
     v = "true" if vec else "false"
     return Branch("bn_stats<%s,%s slices>%s" % ("vec" if vec else "scalar", colsum_slices_name(s, 1024),
                                                "|run" if run else ""),
-                  ["colsum_partial_kernel<cnb::SumOp, %s>" % v, "bn_mean_final_kernel",
-                   "colsum_partial_kernel<cnb::SqDevOp, %s>" % v, "bn_sigma_final_kernel"])
+                  ["colsum_partial_kernel<cnb::SumOp, %s>" % v, "colsum_final_kernel<cnb::MeanFin>",
+                   "colsum_partial_kernel<cnb::SqDevOp, %s>" % v, "colsum_final_kernel<cnb::SigmaFin>"])
 
 
 def bn_apply_branch(n, C, aligned_x, aligned_y, relu, sms=SMS):
     vec = n % 4 == 0 and aligned_x and aligned_y
     gs = "|gs" if bn_grid_x(n, C, vec, sms) < cdiv(n // 4 if vec else n, BLOCK) else ""
     return Branch("bn_apply<%s,%s>%s" % ("vec" if vec else "scalar", "relu" if relu else "linear", gs),
-                  ["bn_apply_kernel<%s>" % ("true" if relu else "false")], "kernel" if aligned_y else "none")
+                  ["bn_channel_kernel<cnb::BnApplyOp<%d>" % (1 if relu else 0)], "kernel" if aligned_y else "none")
 
 
 def bn_backward_branch(n, C, aligned_x, aligned_d, train, sms=SMS):
@@ -493,8 +493,8 @@ def bn_backward_branch(n, C, aligned_x, aligned_d, train, sms=SMS):
     s = bn_slices(n, C, sms)
     return Branch("bn_backward<%s,%s slices>%s" % ("vec" if vec else "scalar", colsum_slices_name(s, 1024),
                                                   "" if train else "|test"),
-                  ["colsum_partial_kernel<cnb::BnGradOp, %s>" % ("true" if vec else "false"), "bn_grad_final_kernel",
-                   "bn_backward_kernel"], "kernel" if aligned_d else "none")
+                  ["colsum_partial_kernel<cnb::BnGradOp, %s>" % ("true" if vec else "false"),
+                   "colsum_final_kernel<cnb::BnGradFin>", "bn_channel_kernel<cnb::BnBackOp>"], "kernel" if aligned_d else "none")
 
 
 def softmax_branch(rows, cols):
@@ -507,6 +507,5 @@ def sum_branch(n):
 
 
 # every library kernel the mirror can name (the profiler test filters on these)
-KERNEL_NAMES = ("bias_kernel", "bias_kernel_scalar", "colsum_partial_kernel", "colsum_final_kernel", "relu_kernel", "relu_deriv_kernel",
-                "dropout_kernel", "mult_kernel", "bn_mean_final_kernel", "bn_sigma_final_kernel", "bn_grad_final_kernel",
-                "bn_apply_kernel", "bn_backward_kernel", "softmax_kernel", "sum_kernel")
+KERNEL_NAMES = ("stream_kernel", "colsum_partial_kernel", "colsum_final_kernel", "bn_channel_kernel", "softmax_kernel",
+                "sum_kernel")

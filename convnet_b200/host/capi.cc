@@ -61,6 +61,11 @@ API long long cnb_net_edge_offset(void* p, int i) { return (long long)((NetHandl
 API long long cnb_net_edge_size(void* p, int i) { return (long long)((NetHandle*)p)->net->Edges()[i]->GetParameterMemoryRequirement(); }
 // the edge whose parameters edge i runs with ("" when untied)
 API const char* cnb_net_edge_tied_to(void* p, int i) { return ((NetHandle*)p)->net->Edges()[i]->Config().tied_to.c_str(); }
+// the frozen edges are [0, n) (ConvNet::NumFrozenEdges); their parameters the prefix [0, *trained_offset) of the buffers
+API int cnb_net_frozen_edges(void* p, long long* trained_offset) {
+  *trained_offset = (long long)((NetHandle*)p)->net->TrainedOffset();
+  return ((NetHandle*)p)->net->NumFrozenEdges();
+}
 API double cnb_net_flops_fprop(void* p) { return ((NetHandle*)p)->net->FlopsFprop(); }
 API double cnb_net_flops_train(void* p) { return ((NetHandle*)p)->net->FlopsTrainStep(); }
 API float* cnb_net_input(void* p) { return ((NetHandle*)p)->net->InputLayer().GetState().GetDevData(); }
@@ -219,6 +224,16 @@ API int cnb_model_edge_params(const char* model, int batch, int cap, long long* 
   delete net;
   return n;
 }
+// static description of a model: the FLOPs of one forward pass and of one training step at `batch` (FlopsFprop,
+// FlopsTrainStep).  0 ok, -1 unknown model
+API int cnb_model_flops(const char* model, int batch, double* fprop, double* train) {
+  ConvNet* net = TryBuildNet(model, batch);
+  if (!net) return -1;
+  *fprop = net->FlopsFprop();
+  *train = net->FlopsTrainStep();
+  delete net;
+  return 0;
+}
 // static description of a model: the flat parameter buffer (ConvNet::PlanParameters).  Returns the number of edges E
 // (-1: unknown model); fills edge_offsets[0, E) and, per layer, bn_offsets[0, E] (-1: not batch-normalised), each up to
 // `cap` entries, and *total (floats, padding included)
@@ -291,6 +306,23 @@ API int cnb_model_tie(const char* model, int edge, char* name, char* owner) {
   snprintf(name, 256, "%s", e.name.c_str());
   snprintf(owner, 256, "%s", e.tied_to.c_str());
   return e.tied_to.empty() ? 0 : 1;
+}
+
+// static description of a model: frozen edge `edge` (block_backprop, FrozenEdges) and the layer it writes, unless that is the
+// output layer (names NUL-terminated, up to 256 bytes; layer "" for the output).  1 frozen, 0 trained, -1 unknown model
+// or one the host cannot run, -2 edge out of range
+API int cnb_model_frozen(const char* model, int edge, char* name, char* layer) {
+  ConvNet* net = TryBuildNet(model, 1);
+  if (!net) return -1;
+  const int n = (int)net->Edges().size(), frozen = net->NumFrozenEdges();
+  int rc = edge < 0 || edge >= n ? -2 : edge < frozen ? 1 : 0;
+  if (rc == 1) {
+    Layer& l = *net->Layers()[edge + 1];
+    snprintf(name, 256, "%s", net->Edges()[edge]->GetName().c_str());
+    snprintf(layer, 256, "%s", l.IsOutput() ? "" : l.GetName().c_str());
+  }
+  delete net;
+  return rc;
 }
 
 // a model's resolved ModelConfig as a config::Model text proto (ModelText).  Returns its length in bytes (-1: unknown

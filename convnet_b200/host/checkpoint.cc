@@ -377,8 +377,10 @@ void ConvNet::LoadPolyakWeights() {
   CKPT_CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), ev_opt_, 0));
   float* backup = polyak_ + (size_t)model_.polyak_queue_size * n;
   CKPT_CUDA_CHECK(cudaMemcpyAsync(backup, parameters_.GetDevData(), sizeof(float) * n, cudaMemcpyDeviceToDevice, Matrix::Stream()));
-  // the kernel's write drops the staged copies of the old weights (bf16 twins and dgrad banks) itself
-  cnb_polyak_average(parameters_.GetDevData(), polyak_, (long long)n, (long long)n, PolyakCount());
+  // the kernel's write drops the staged copies of the old weights (bf16 twins and dgrad banks) itself.  Only the trained
+  // range: the frozen parameters are equal in every slot, and their average could still round (DESIGN.md §5)
+  const size_t lo = TrainedOffset();
+  if (lo < n) cnb_polyak_average(parameters_.GetDevData() + lo, polyak_ + lo, (long long)(n - lo), (long long)n, PolyakCount());
   polyak_backup_ = true;
   PrestageAll();
 }

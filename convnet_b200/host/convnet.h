@@ -69,6 +69,16 @@ std::string SampleEdgeError(const Edge& e, int source_channels, int dest_channel
 // untied itself, have parameters of the same edge_type and the same weight and bias shapes, and sum its bias gradient on
 // the same stream; a tied edge may not ask for grad_check (its owner checks the shared tensors)
 std::string TieError(const std::vector<const Edge*>& edges, size_t i);
+// Fine-tuning (EdgeConfig::block_backprop): an edge is frozen if it is blocked or lies below a blocked edge, so the frozen
+// edges of a chain are [0, FrozenEdges).  They run their forward pass only: no weight gradient, no derivative into their
+// source, no optimizer step.  The hidden layers they write receive no derivative (the output layer keeps the one its
+// loss writes)
+int FrozenEdges(const std::vector<EdgeConfig>& edges);
+// "" if edge `i` of a chain (shapes known, ties accepted by TieError) may be frozen or trained as its block_backprop says,
+// else why not, starting with "field 'block_backprop': ", and in *at the blocked edge whose field the message is about.
+// A weighted edge below a blocked one must be blocked itself, the edges of a tie group agree, and a frozen edge may not
+// ask for grad_check
+std::string FrozenError(const std::vector<const Edge*>& edges, size_t i, size_t* at);
 
 struct ModelConfig {
   std::string name;
@@ -156,7 +166,7 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   float DropoutProb() const { return config_.dropprob; }
   unsigned long long DropoutSeed(unsigned long long step, unsigned long long salt) const;
   bool HasSeparateActivationPass() const { return ActCode(config_.activation) != CNB_ACT_LINEAR && !activation_fused_; }
-  bool HasSeparateDerivPass() const { return ActCode(config_.activation) != CNB_ACT_LINEAR && !deriv_fused_; }
+  bool HasSeparateDerivPass() const { return ReceivesDeriv() && ActCode(config_.activation) != CNB_ACT_LINEAR && !deriv_fused_; }
   // output layer: deriv = loss_function_weight * dLoss/dstate and the per-image loss (unweighted), layer.cc:426-437
   void ComputeDeriv();
   void ComputePerformanceMetric();              // the per-image performance metric (GetPerformanceMetric, layer.cc:422)
@@ -170,7 +180,8 @@ class Layer {                                   // src/layer.{h,cc}, reduced to 
   float LossWeight() const { return config_.loss_function_weight; }
   bool IsInput() const { return config_.is_input; }
   // back-propagation writes a derivative for this layer: not the input layer, nor the layer an RGBTOYUV edge writes (it
-  // has no backward pass; ConvNet::SetNoDeriv).  A layer without one has no derivative buffer and runs no derivative pass
+  // has no backward pass), nor a hidden layer a frozen edge writes (SetNoDeriv).  A layer without one has no derivative
+  // buffer and runs no derivative pass
   bool ReceivesDeriv() const { return !config_.is_input && !no_deriv_; }
   void SetNoDeriv() { no_deriv_ = true; }
   bool IsOutput() const { return config_.is_output; }
@@ -235,7 +246,8 @@ class DataParallelSync {
 // bucket is the contiguous range [lo, hi) — the edges [trigger, last] — that becomes final when edge `trigger` has run
 // ComputeOuter.  Buckets are closed once they hold >= bucket_floats; the FIRST weighted edge of the net always gets a
 // bucket of its own (its gradient is the last to appear: only that small exchange stays exposed at the end of the step);
-// every parameter belongs to exactly one bucket.
+// every parameter belongs to exactly one bucket.  (ConvNet passes frozen edges as empty: the buckets cover the trained
+// edges only, and the first of them travels alone.)
 struct Bucket { size_t lo, hi; int trigger, last; };
 std::vector<Bucket> PlanBuckets(const std::vector<size_t>& edge_offset, const std::vector<size_t>& edge_size,
                                 size_t bucket_floats);
@@ -299,8 +311,14 @@ class ConvNet {
   Matrix& History() { return history_; }
   size_t NumParameters() const { return num_params_; }
   int BatchSize() const { return batch_size_; }
+  // the frozen edges are [0, NumFrozenEdges()) (FrozenEdges); their trained tensors are the prefix [0, TrainedOffset()) of
+  // the flat buffers, which no optimizer step, bucket or Polyak average touches
+  int NumFrozenEdges() const { return frozen_; }
+  size_t TrainedOffset() const { return frozen_ < (int)edges_.size() ? edge_offset_[frozen_] : num_params_; }
   double FlopsFprop() const;
-  double FlopsTrainStep() const;                                // fprop + wgrad for every weighted edge + dgrad except into the input
+  // fprop + wgrad + dgrad of every edge, less the dgrad into the input layer, the wgrad of each frozen edge and the dgrad
+  // into each layer a frozen edge writes
+  double FlopsTrainStep() const;
   // per edge position: the slice of the flat buffer placed there (a tie group's slice sits at its lowest edge; the other
   // edges of the group have an empty one)
   const std::vector<size_t>& EdgeOffsets() const { return edge_offset_; }
@@ -328,6 +346,7 @@ class ConvNet {
   // the flat buffer.  Back-propagation reaches that edge last, so its bucket becomes final after every contribution to
   // the shared gradients and every read of the shared weights
   std::vector<int> owner_, home_;
+  int frozen_ = 0;                              // FrozenEdges(model_.edge)
   void ResolveTies();
   bool Grouped(size_t i) const;                 // edge i shares its parameters with another edge
   bool prestage_ = true;                       // rebuild the dgrad banks behind each optimizer step (PrestageDown)

@@ -101,6 +101,8 @@ struct EdgeConfig {
   // the name of the edge whose weights and bias this edge runs with and trains ("" = its own; src/edge.cc:131-180).  A tied
   // edge has no parameters of its own: its optimizers, initialisation and pretrained_* fields are not used (TieError)
   std::string tied_to;
+  // no derivative passes through this edge (proto field 13): it and every edge below it are frozen (FrozenEdges)
+  bool block_backprop = false;
 };
 
 class Edge {
@@ -135,6 +137,7 @@ class Edge {
   int GetNumOutputChannels() const { return num_output_channels_; }
   const std::string& GetName() const { return name_; }
   const EdgeConfig& Config() const { return config_; }
+  bool IsBackPropBlocked() const { return config_.block_backprop; }
   Layer* GetSource() { return source_; }
   Layer* GetDest() { return dest_; }
   void SetSource(Layer* l) { source_ = l; }

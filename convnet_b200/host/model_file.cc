@@ -119,6 +119,7 @@ const std::map<std::string, FieldSpec>& Schema(const std::string& message) {
 struct Msg;
 struct Entry {
   std::string name;
+  std::string file;          // the file the line is in (a subnet's fields come from the subnet's model file)
   int line = 0;
   long long i = 0;           // INT, BOOL, ENUM (the value's number)
   float f = 0.f;             // FLOAT
@@ -308,7 +309,7 @@ class Parser {
     else if (TrySymbol('<')) close = '>';
     else Fail(tok_line_, "field '" + name + "': expected '{', found " + Describe());
     Entry e;
-    e.name = name; e.line = line;
+    e.name = name; e.file = path_; e.line = line;
     e.msg = std::make_shared<Msg>();
     e.msg->type = f.type; e.msg->line = line;
     ParseBody(*e.msg, close);
@@ -317,6 +318,7 @@ class Parser {
   Entry ParseScalar(const std::string& name, const FieldSpec& f) {
     Entry e;
     e.name = name;
+    e.file = path_;
     e.line = tok_line_;
     auto bad = [&](const std::string& want) { Fail(e.line, "field '" + name + "': expected " + want + ", found " + Describe()); };
     if (f.kind == STRING) {
@@ -439,11 +441,12 @@ class Mapper {
  public:
   Mapper(const std::string& path, bool check_pretrained) : path_(path), check_pretrained_(check_pretrained) {}
 
-  ModelConfig Map(const Msg& model) {
+  ModelConfig Map(Msg& model) {
+    std::vector<std::string> open = {path_};
+    ExpandSubnets(model, open);
     ModelConfig m;
     m.name = model.Get("name")->s;
     m.seed = (unsigned)model.Int("seed", 0);
-    RefuseMessage(model, "subnet", "subnets are not supported");
     // Polyak averaging: a queue without an insertion period, or a period without a queue, averages nothing
     m.polyak_after = (int)model.Int("polyak_after", 0);
     m.polyak_queue_size = (int)model.Int("polyak_queue_size", 0);
@@ -549,6 +552,12 @@ class Mapper {
       const Msg& e = *edges[out[chain[k]]]->msg;
       if (!why.empty()) Fail(*e.Get("tied_to"), EdgeName(e), why);
     }
+    // block_backprop (ConvNet::Refusal runs the same checks), at the line of the blocked edge's field
+    for (size_t k = 0; k < built.size(); k++) {
+      size_t at = k;
+      const std::string why = FrozenError(chain_edges, k, &at);
+      if (!why.empty()) Fail(*edges[out[chain[at]]]->msg->Get("block_backprop"), EdgeName(*edges[out[chain[k]]]->msg), why);
+    }
     return m;
   }
 
@@ -588,12 +597,137 @@ class Mapper {
   }
   // "<where>: field '<name>': <what>" at the field's line
   [[noreturn]] void Fail(const Entry& at, const std::string& where, const std::string& what) const {
-    Fail(at.line, (where.empty() ? "" : where + ": ") + what);
+    throw std::invalid_argument(at.file + ":" + std::to_string(at.line) + ": " + (where.empty() ? "" : where + ": ") + what);
   }
   void RefuseMessage(const Msg& m, const char* field, const std::string& why, const std::string& where = "") const {
     if (const Entry* e = m.Get(field)) Fail(*e, where, std::string("field '") + field + "': " + why);
   }
   static std::string EdgeName(const Msg& e) { return "edge '" + e.Get("source")->s + ":" + e.Get("dest")->s + "'"; }
+
+  // ---- subnets (ConvNet::AddSubnet, src/convnet.cc:94-148): the layers and edges of each subnet join `model` before its
+  // graph is mapped, and the subnet blocks go (convnet.cc:39).  `open`: the model files being expanded, outermost first
+  void ExpandSubnets(Msg& model, std::vector<std::string>& open) const {
+    std::vector<Entry> subnets;
+    for (const Entry& e : model.fields) if (e.name == "subnet") subnets.push_back(e);
+    model.fields.erase(std::remove_if(model.fields.begin(), model.fields.end(), [](const Entry& e) { return e.name == "subnet"; }),
+                       model.fields.end());
+    for (const Entry& s : subnets) AddSubnet(model, s, open);
+  }
+  // field v.name of `m` set to `v`
+  static void Set(Msg& m, const Entry& v) {
+    for (Entry& e : m.fields) if (e.name == v.name) { e = v; return; }
+    m.fields.push_back(v);
+  }
+  // a field that a subnet block sets, at the line of `at`
+  static Entry Value(const Entry& at, const std::string& name) {
+    Entry e;
+    e.name = name; e.file = at.file; e.line = at.line;
+    return e;
+  }
+  void AddSubnet(Msg& model, const Entry& at, std::vector<std::string>& open) const {
+    const Msg& s = *at.msg;
+    const std::string name = s.Get("name")->s, where = "subnet '" + name + "'";
+    const Entry& file = *s.Get("model_file");
+    if (s.Int("gpu_id_offset", 0) != 0)
+      Fail(*s.Get("gpu_id_offset"), where, "field 'gpu_id_offset': one GPU per model (data parallelism replicates it)");
+    const long long mult = s.Int("num_channels_multiplier", 1);
+    if (mult <= 0) Fail(*s.Get("num_channels_multiplier"), where, "field 'num_channels_multiplier' must be positive");
+    if (std::find(open.begin(), open.end(), file.s) != open.end())
+      Fail(file, where, "field 'model_file': '" + file.s + "' contains itself as a subnet");
+    std::ifstream in(file.s, std::ios::binary);
+    if (!in) Fail(file, where, "field 'model_file': cannot open model file '" + file.s + "'");
+    std::stringstream text;
+    text << in.rdbuf();
+    const std::shared_ptr<Msg> sub = Parser(file.s, text.str()).ParseFile();
+    open.push_back(file.s);
+    ExpandSubnets(*sub, open);                             // its own subnets first
+    open.pop_back();
+
+    std::set<std::string> sub_layers, net_layers;
+    for (const Entry* l : sub->All("layer")) sub_layers.insert(l->msg->Get("name")->s);
+    for (const Entry* l : model.All("layer")) net_layers.insert(l->msg->Get("name")->s);
+    // the reference ignores a merge_layer or remove_layer that names no layer of the subnet; here it is refused
+    std::map<std::string, std::string> merge;
+    for (const Entry* ml : s.All("merge_layer")) {
+      const Entry &from = *ml->msg->Get("subnet_layer"), &to = *ml->msg->Get("net_layer");
+      if (!sub_layers.count(from.s)) Fail(from, where, "field 'subnet_layer': " + file.s + " has no layer '" + from.s + "'");
+      if (!net_layers.count(to.s)) Fail(to, where, "field 'net_layer': the net has no layer '" + to.s + "'");
+      merge[from.s] = to.s;
+    }
+    std::set<std::string> removed;
+    for (const Entry* r : s.All("remove_layer")) {
+      if (!sub_layers.count(r->s)) Fail(*r, where, "field 'remove_layer': " + file.s + " has no layer '" + r->s + "'");
+      removed.insert(r->s);
+    }
+    auto renamed = [&](const std::string& l) { return merge.count(l) ? merge.at(l) : name + "_" + l; };
+
+    for (const Entry* l : sub->All("layer")) {              // a merged layer takes the net's config: the subnet's goes
+      const std::string& old = l->msg->Get("name")->s;
+      if (merge.count(old) || removed.count(old)) continue;
+      Entry layer = *l;
+      layer.msg = std::make_shared<Msg>(*l->msg);
+      Entry n = *layer.msg->Get("name");
+      n.s = renamed(old);
+      if (!net_layers.insert(n.s).second) Fail(*l, where, "layer '" + old + "' becomes '" + n.s + "', a layer the net already has");
+      Set(*layer.msg, n);
+      if (const Entry* c = layer.msg->Get("num_channels")) {
+        Entry v = *c;
+        v.i *= mult;
+        if (v.i > 2147483647LL) Fail(*c, where, "field 'num_channels': " + std::to_string(v.i) + " channels after the multiplier");
+        Set(*layer.msg, v);
+      }
+      model.fields.push_back(layer);
+    }
+
+    std::map<std::string, std::string> edge_names;          // subnet edge -> its name in the net (tied_to)
+    for (const Entry* e : sub->All("edge")) {
+      const std::string &src = e->msg->Get("source")->s, &dst = e->msg->Get("dest")->s;
+      if (!removed.count(src) && !removed.count(dst)) edge_names[src + ":" + dst] = renamed(src) + ":" + renamed(dst);
+    }
+    const Entry* params = s.Get("parameters_file");
+    const Entry* block = s.Bool("block_backprop", false) ? s.Get("block_backprop") : nullptr;
+    const Entry& soa = s.Has("start_optimization_after") ? *s.Get("start_optimization_after") : at;
+    for (const Entry* e : sub->All("edge")) {
+      const std::string src = e->msg->Get("source")->s, dst = e->msg->Get("dest")->s;
+      if (removed.count(src) || removed.count(dst)) continue;
+      Entry edge = *e;
+      edge.msg = std::make_shared<Msg>(*e->msg);
+      Msg& m = *edge.msg;
+      if (params && !params->s.empty()) {                  // PRETRAINED from the checkpoint, by the edge's subnet name
+        Entry v = Value(*params, "initialization");
+        v.i = PRETRAINED; v.s = "PRETRAINED";
+        Set(m, v);
+        v = Value(*params, "pretrained_model"); v.s = params->s; Set(m, v);
+        v = Value(*params, "pretrained_edge_name"); v.s = src + ":" + dst; Set(m, v);
+      }
+      for (const char* f : {"source", "dest"}) {
+        Entry v = *m.Get(f);
+        v.s = renamed(v.s);
+        Set(m, v);
+      }
+      // the reference leaves tied_to as the subnet wrote it, naming an edge the net does not have
+      if (const Entry* tie = m.Get("tied_to"); tie && edge_names.count(tie->s)) {
+        Entry v = *tie;
+        v.s = edge_names.at(tie->s);
+        Set(m, v);
+      }
+      if (block && !m.Bool("block_backprop", false)) {
+        Entry v = Value(*block, "block_backprop");
+        v.i = 1;
+        Set(m, v);
+      }
+      for (const char* f : {"weight_optimizer", "bias_optimizer"}) {
+        Entry o = m.Has(f) ? *m.Get(f) : Value(soa, f);
+        o.msg = o.msg ? std::make_shared<Msg>(*o.msg) : std::make_shared<Msg>();
+        if (!m.Has(f)) { o.msg->type = "Optimizer"; o.msg->line = soa.line; }
+        Entry v = Value(soa, "start_optimization_after");
+        v.i = s.Int("start_optimization_after", 0);
+        Set(*o.msg, v);
+        Set(m, o);
+      }
+      model.fields.push_back(edge);
+    }
+  }
 
   // Optimizer fields outside the SGD / Adagrad / RMSProp paths: refused wherever a block sets them
   void CheckOptimizer(const Entry& block, const std::string& where) const {
@@ -618,9 +752,10 @@ class Mapper {
         else c.*f.i = (int)e->i;
       }
     }
-    if (const char* err = OptimizerConfigError(c))
-      Fail(own ? own->line : def ? def->line : 1,
-           where + ": " + (own ? own->name : def ? def->name : std::string("optimizer")) + ": " + err);
+    if (const char* err = OptimizerConfigError(c)) {
+      if (const Entry* at = own ? own : def) Fail(*at, where, at->name + ": " + err);
+      Fail(1, where + ": optimizer: " + err);
+    }
     return c;
   }
 
@@ -688,7 +823,7 @@ class Mapper {
     if (const Entry* tie = e.Get("tied_to")) c.tied_to = tie->s;      // checked with the whole chain (TieError)
     RefuseMessage(e, "source_slice", "layer slices are not supported", where);
     RefuseMessage(e, "dest_slice", "layer slices are not supported", where);
-    if (e.Bool("block_backprop", false)) Fail(*e.Get("block_backprop"), where, "field 'block_backprop': not supported");
+    c.block_backprop = e.Bool("block_backprop", false);     // checked with the whole chain (FrozenError)
     if (e.Int("gpu_id", 0) != 0) Fail(*e.Get("gpu_id"), where, "field 'gpu_id': one GPU per model (data parallelism replicates it)");
 
     // geometry: the *_y / *_x fields fall back to kernel_size / stride / padding only when absent (src/edge.cc:87-106)
@@ -920,6 +1055,7 @@ std::string ModelText(const ModelConfig& m) {
         w.Line("grad_check_epsilon", eps + "]");
       }
     }
+    if (e.block_backprop) w.Bool("block_backprop", true);
     w.Close();
   }
   return w.str();

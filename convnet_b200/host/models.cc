@@ -410,9 +410,21 @@ ModelConfig BuildModel(const std::string& name) {
   const std::string suffix = "+gradcheck";
   if (name.size() > suffix.size() && name.compare(name.size() - suffix.size(), suffix.size(), suffix) == 0) {
     ModelConfig m = BuildModel(name.substr(0, name.size() - suffix.size()));
-    for (EdgeConfig& e : m.edge) {                          // (a tied edge is checked through its owner)
-      e.grad_check = e.tied_to.empty(); e.grad_check_num_params = 10; e.grad_check_epsilon = {1e-2f, 1e-3f, 1e-4f};
+    const int frozen = FrozenEdges(m.edge);
+    for (int i = 0; i < (int)m.edge.size(); i++) {        // (a tied edge is checked through its owner, a frozen one not at all)
+      EdgeConfig& e = m.edge[i];
+      e.grad_check = e.tied_to.empty() && i >= frozen; e.grad_check_num_params = 10; e.grad_check_epsilon = {1e-2f, 1e-3f, 1e-4f};
     }
+    return m;
+  }
+  // "<model>+finetune": block_backprop on every edge below the lowest FC edge, whose grad_check flags go (a frozen edge has
+  // no gradient to check): the trunk keeps its weights and the FC classifier trains on its features
+  if (EndsWith(name, "+finetune")) {
+    ModelConfig m = BuildModel(name.substr(0, name.size() - 9));
+    size_t fc = 0;
+    while (fc < m.edge.size() && m.edge[fc].edge_type != FC) fc++;
+    if (fc == m.edge.size()) throw std::invalid_argument("model '" + name + "': +finetune trains the FC edges, and it has none");
+    for (size_t i = 0; i < fc; i++) { m.edge[i].block_backprop = true; m.edge[i].grad_check = false; }
     return m;
   }
   if (name == "gradcheck") return BuildGradCheckNet();

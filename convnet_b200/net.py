@@ -101,6 +101,9 @@ def load_host():
             "cnb_net_layer_deriv": ([vp, i], vp),
             "cnb_model_tie": ([ct.c_char_p, i, ct.c_char_p, ct.c_char_p], i),
             "cnb_net_dropout_seed": ([vp, i], ct.c_ulonglong),
+            "cnb_net_frozen_edges": ([vp, ct.POINTER(ll)], i),
+            "cnb_model_frozen": ([ct.c_char_p, i, ct.c_char_p, ct.c_char_p], i),
+            "cnb_model_flops": ([ct.c_char_p, i, ct.POINTER(d), ct.POINTER(d)], i),
         }
         for name, (args, res) in sig.items():
             fn = getattr(H, name)
@@ -122,7 +125,9 @@ class Net:
     "+adagrad" / "+rmsprop": every weight, bias, gamma and beta optimizer on ADAGRAD_SGD (adagrad_delta 1, epsilon x 0.1) /
     RMSPROP_SGD (rms_prop_factor 0.9, epsilon x 0.01); they compose with the others ("alexnet+ref-optimizer+rmsprop",
     "tiny+bn+adagrad").
-    "+gradcheck": run_grad_check's edge flags (e.g. "tiny+bn+gradcheck").
+    "+gradcheck": run_grad_check's edge flags on the trained edges (e.g. "tiny+bn+gradcheck").
+    "+finetune": block_backprop on every edge below the lowest FC edge: the trunk keeps its weights and the FC classifier
+    trains ("alexnet+finetune", "alexnet+ref-optimizer+finetune", "tiny+bn+finetune"; refused without an FC edge).
     "+logistic": every hidden RECTIFIED_LINEAR layer becomes LOGISTIC (same parameters; "alexnet+logistic", "tiny+bn+logistic").
     One output suffix at most: "+squared-error" (LINEAR output, SQUARED_ERROR), "+binary-ce" (LOGISTIC output,
     CROSS_ENTROPY_BINARY, metric CLASSIFICATION_BINARY), "+soft-targets" (SOFTMAX_DIST, CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED);
@@ -140,7 +145,15 @@ class Net:
     reference's Save() does beside each checkpoint:
         if polyak_due(model, net.iteration): net.polyak_insert()          # after each train_step
         net.save(p)
-        net.load_polyak_weights(); net.save(p + "polyak"); net.load_current_weights()"""
+        net.load_polyak_weights(); net.save(p + "polyak"); net.load_current_weights()
+
+    Fine-tuning (the reference's Edge.block_backprop, see model_frozen()): a blocked edge and every edge below it are frozen.
+    They run their forward pass only (dropout and batch statistics as in training, running statistics updated); they get
+    no gradient and no optimizer step, and the hidden layers they write no derivative (layer_deriv() is None).  Their
+    parameters stay in the buffers, as the prefix [0, trained_offset) of params_tensor(), which no update, all-reduce or
+    Polyak average touches; checkpoints save them.  A model file's subnet blocks (the reference's Model.subnet) pull
+    another model file in, optionally PRETRAINED from a checkpoint and blocked: the usual way to train a new head on a
+    trained trunk."""
 
     def __init__(self, model, batch_size, seed=42, grad_checker=False):
         self.H = load_host()
@@ -161,6 +174,13 @@ class Net:
     input_floats = property(lambda s: s.H.cnb_net_input_floats(s.h))
     flops_fprop = property(lambda s: s.H.cnb_net_flops_fprop(s.h))
     flops_train = property(lambda s: s.H.cnb_net_flops_train(s.h))
+
+    def _frozen(self):
+        off = ct.c_longlong(0)
+        return self.H.cnb_net_frozen_edges(self.h, ct.byref(off)), off.value
+
+    trained_offset = property(lambda s: s._frozen()[1],
+                              doc="floats at the start of params_tensor() held by frozen edges and layers, which nothing trains")
 
     def edges(self):
         return [(self.H.cnb_net_edge_name(self.h, i).decode(), self.H.cnb_net_edge_flops(self.h, i),
@@ -215,7 +235,8 @@ class Net:
 
     def layer_deriv(self, i):
         """the derivative of the loss with respect to layer i's state after bprop, laid out like layer_state(i); None for
-        a layer that receives no derivative: the input layer and the layer an RGBTOYUV edge writes"""
+        a layer that receives no derivative: the input layer, the layer an RGBTOYUV edge writes and every hidden layer a
+        frozen edge writes (block_backprop)"""
         ptr = self.H.cnb_net_layer_deriv(self.h, i)
         return self._view(ptr, self.H.cnb_net_layer_floats(self.h, i), "f") if ptr else None
 
@@ -274,8 +295,10 @@ class Net:
     def set_optimizer(self, edge, weights=None, bias=None):
         """replace the settings of the weight and / or bias optimizer of `edge` (index or name) with the optimizer block
         `weights` / `bias` (dicts of proto field names, unset fields at the proto's defaults).  Step counts and momentum
-        histories are kept."""
+        histories are kept.  ValueError for a frozen edge (block_backprop), which nothing trains."""
         name = self._edge_name(edge)
+        if name and [e[0] for e in self.edges()].index(name) < self._frozen()[0]:
+            raise ValueError("edge %r is blocked (block_backprop): it is frozen, and no optimizer trains it" % (name,))
         for key, kind, d in (("weights", ":weight", weights), ("bias", ":bias", bias)):
             if d is None:
                 continue
@@ -497,6 +520,32 @@ def model_ties(model):
             return out
         if rc == 1:
             out[name.value.decode()] = owner.value.decode()
+        i += 1
+
+
+def model_flops(model, batch):
+    """{"fprop", "train"}: the FLOPs of one forward pass and of one training step of a model at `batch` (host-only; the
+    flops_fprop / flops_train of a Net)"""
+    fprop, train = ct.c_double(0), ct.c_double(0)
+    if load_host().cnb_model_flops(model.encode(), batch, ct.byref(fprop), ct.byref(train)):
+        raise ValueError("cannot build model %r (see stderr)" % model)
+    return {"fprop": fprop.value, "train": train.value}
+
+
+def model_frozen(model):
+    """the frozen part of a model (host-only): {"edges": the blocked edges and those below them, "layers": the hidden layers
+    they write}, in chain order"""
+    H, out, i = load_host(), {"edges": [], "layers": []}, 0
+    while True:
+        name, layer = ct.create_string_buffer(256), ct.create_string_buffer(256)
+        rc = H.cnb_model_frozen(model.encode(), i, name, layer)
+        if rc == -1:
+            raise ValueError("cannot build model %r (see stderr)" % model)
+        if rc != 1:
+            return out
+        out["edges"].append(name.value.decode())
+        if layer.value:
+            out["layers"].append(layer.value.decode())
         i += 1
 
 

@@ -10,7 +10,9 @@ So every output element y is held to
 
 with ref and sum|a*b| computed in float64 from the modelled operands; where S == 0 the output must equal ref exactly.
 ReLU is applied to ref (it is 1-Lipschitz); elements the ReLU' mask or the dropout drops must be exactly 0, and elements
-outside the call's output channel range must keep their bits.
+outside the call's output channel range must keep their bits.  A logistic unit's sigma (fprop) and sigma' (dgrad) move
+the bar with them: sigma' <= 1/4 scales S by 1/4, the logistic derivative mask s(1 - s) scales it by s(1 - s), and each
+adds the bar of its own float32 arithmetic (loss_ref.sigmoid_bar, loss_ref.logistic_deriv_bar) as (bar / BAR) to S.
 
 Layouts are the library's (DESIGN.md §3): activations a[n + N*(x + W*(y + H*c))], filters f[o + Cout*(x + kx*(y + ky*c))];
 3-D tensors stack frames as channel blocks (channel c + C*t).  Everything here is torch float64 on the device of the inputs,
@@ -25,6 +27,7 @@ import torch.nn.functional as tF
 from convnet_b200.abi import GetConvDesc, num_modules
 
 BAR = 2.0 ** -16
+U = 2.0 ** -24
 CHUNK_BYTES = 512 << 20
 
 
@@ -315,10 +318,12 @@ class Expect:
     keep: torch.Tensor        # bool: must keep the prefilled bits (outside the call's output channels)
 
 
-def expect(op, g, a, b, kind, t0=None, st=0.0, so=1.0, bias=None, relu=False, mask=None, drop=None):
+def expect(op, g, a, b, kind, t0=None, st=0.0, so=1.0, bias=None, relu=False, mask=None, drop=None, logistic=False,
+           lmask=None):
     """Expected result of one call.  a, b: the fp32 operands (flat tensors, see _raw); t0: the target's contents before
     the call; bias: fprop bias per output channel of the call; mask: dgrad ReLU' mask (flat, target-shaped);
-    drop: (prob, scale, seed) of the fused fprop dropout."""
+    drop: (prob, scale, seed) of the fused fprop dropout; logistic: fprop applies sigma; lmask: the dgrad logistic
+    derivative mask, the stored state s of the logistic layer below (flat, target-shaped): the result is times s(1 - s)."""
     A, B = model(a, kind), model(b, kind)
     ref = so * _raw(op, g, A, B)
     S = abs(so) * _raw(op, g, A.abs(), B.abs())
@@ -348,6 +353,15 @@ def expect(op, g, a, b, kind, t0=None, st=0.0, so=1.0, bias=None, relu=False, ma
         S = torch.where(written, S + fb.abs(), S)
     if relu:
         ref = torch.where(written, ref.clamp_min(0.0), ref)
+    if logistic:                     # sigma' <= 1/4; sigma itself: 6u sigma + 2^-126 (loss_ref.sigmoid_bar)
+        sig = torch.sigmoid(ref)
+        ref = torch.where(written, sig, ref)
+        S = torch.where(written, S / 4 + (6 * U * sig + 2.0 ** -126) / BAR, S)
+    if lmask is not None:            # d s (1 - s): three roundings, 3u |r| + 2^-148 (loss_ref.logistic_deriv_bar)
+        sl = lmask[:n].to(torch.float64)
+        ds = sl * (1 - sl)
+        ref = ref * ds
+        S = S * ds + (3 * U * ref.abs() + 2.0 ** -148) / BAR
     zero = torch.zeros(n, dtype=torch.bool, device=dev)
     if drop is not None:
         prob, scale, seed = drop

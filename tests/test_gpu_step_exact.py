@@ -6,7 +6,13 @@ eagerly during bprop), at the bench's second per-GPU batch, with the fusions swi
 Before the audited step every layer derivative and the whole gradient buffer hold a NaN sentinel: the step must
 overwrite every element of them.  The stale-weight control raises the learning rate of one conv and one FC edge so that
 the step changes many of their bf16 weight copies; their dgrad must then pass against the weights before the step and
-fail against the weights after it, or the audit could not tell a filter bank rebuilt too early from a correct one."""
+fail against the weights after it, or the audit could not tell a filter bank rebuilt too early from a correct one.
+
+Beyond AlexNet's kind of net the cases cover logistic units (tiny+logistic, logcheck), the LINEAR / squared-error,
+LOGISTIC / binary cross-entropy and SOFTMAX_DIST / soft-target output layers on float targets, Adagrad and RMSProp, tied
+edges (tiednet: one conv filter bank at three geometries, an FC pair whose slice sits at the lower edge), the sampling
+and colour edges (updown, updowncheck, and updowncheck with dropout around its sampling edges) and fine-tuning on a frozen trunk (whose parameters, history and adaptive state must keep their bits, whose gradients must
+keep the sentinel and whose hidden layers have no derivative)."""
 import os
 import subprocess
 import sys
@@ -55,6 +61,17 @@ def _record(tag, mode, rows, left, t0):
 
 CASES = [("alexnet", 128, m, w) for w in (0, 3) for m in ("fp32", "tf32", "bf16")] + [
     ("alexnet", 256, "bf16", 3), ("lenet", 100, "bf16", 3), ("tiny", 32, "fp32", 3)]
+# logistic units (sigma fused into the conv epilogue or run as a pass after pooling, sigma' likewise), the target-trained
+# output layers, the adaptive optimizers and frozen trunks
+CASES += [("tiny+logistic", 32, "bf16", 0), ("tiny+logistic", 32, "bf16", 3), ("logcheck", 32, "fp32", 3),
+          ("tiny+squared-error", 32, "tf32", 3), ("tiny+binary-ce", 32, "bf16", 3), ("tiny+soft-targets", 32, "fp32", 3),
+          ("tiny+adagrad", 32, "bf16", 3), ("lenet+rmsprop", 100, "bf16", 3),
+          ("lenet+ref-optimizer+rmsprop", 100, "tf32", 3), ("alexnet+finetune", 128, "bf16", 0),
+          ("alexnet+finetune", 128, "bf16", 3), ("tiny+logistic+adagrad+finetune", 32, "bf16", 3),
+          ("tiednet", 64, "bf16", 0), ("tiednet", 64, "bf16", 3), ("tiednet", 64, "fp32", 3),
+          ("updown", 128, "bf16", 0), ("updowncheck", 32, "fp32", 3), ("updowncheck", 32, "bf16", 3)]
+# (updown is audited on its first step: its loss sums the squared error of 49,152 outputs per image, and on N(0, 1)
+# targets at the model's learning rate the warm-up steps diverge; updowncheck audits the sampling edges warmed up)
 
 
 @pytest.mark.parametrize("name,batch,mode,warmup", CASES)
@@ -64,6 +81,18 @@ def test_step(name, batch, mode, warmup):
     rows, left, _ = se.audit_case(name, batch, mode, warmup)
     _record("%s/%d/%s/step%d" % (name, batch, mode, warmup), mode, rows, left, t0)
     torch.cuda.empty_cache()
+
+
+@pytest.mark.parametrize("mode", ["fp32", "bf16"])
+def test_sampling_dropout_step(tmp_path, mode):
+    """dropout on the layers a DOWNSAMPLE and an UPSAMPLE write (fused into the average-pool row kernels) and below a
+    DOWNSAMPLE (folded into its undo)"""
+    t0 = time.time()
+    path = str(tmp_path / "updowndrop.pbtxt")
+    with open(path, "w") as f:
+        f.write(se.sample_dropout_text())
+    rows, left, _ = se.audit_case(path, 32, mode, 3)
+    _record("updowncheck+dropout/32/%s/step3" % mode, mode, rows, left, t0)
 
 
 def test_step_without_fusions():

@@ -1,10 +1,13 @@
 """The step auditor (tests/step_exact.py) without a GPU: it passes a float32 torch step of `tiny` and `gradcheck` (and
-of `tiny` with dropout on its 1x1 layer), and it fails every single injected fault, naming the layer and quantity.
+of `tiny` with dropout on its 1x1 layer, with logistic units, with each target-trained output layer, with Adagrad or
+RMSProp, on a frozen trunk, and of `logcheck` and `tiednet`), and it fails every single injected fault, naming the layer
+and quantity.
 
 The snapshot is made the way the net makes one: torch float32 forward and autograd backward in the library's layouts,
-with the fusion plan's semantics (each layer's derivative is the loss gradient at its pre-activation, ReLU' and the
-dropout mask applied; weight and bias gradients scaled by 1 / batch; the output derivative p - onehot), then the SGD
-step of every weight and bias tensor."""
+with the fusion plan's semantics (each layer's derivative is the loss gradient at its pre-activation, ReLU' or sigma'
+and the dropout mask applied; weight and bias gradients scaled by 1 / batch, a tie group's summed over its members; the
+output derivative p - onehot or y - t, 0 at don't-care binary targets), then the optimizer step of every trained weight
+and bias tensor.  Frozen edges get no gradient (the sentinel stays), no step, and the layers they write no derivative."""
 import math
 
 import numpy as np
@@ -12,7 +15,9 @@ import pytest
 import torch
 import torch.nn.functional as tF
 
+import abi_rest_exact as ax
 import conv_exact as cx
+import loss_ref as lr
 import opt_rules as opt
 import step_exact as se
 from convnet_b200 import net
@@ -42,9 +47,11 @@ def _rnorm(x, k, alpha, beta, blocked):
     return x * (1.0 + alpha * S) ** -beta
 
 
-def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None):
+def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None, fault=None):
     """a Snapshot of one float32 step of `model` (a step_exact.Model).  seeds: per layer dropout seed (default: drawn);
-    fprop_operands: {edge index: operand-model kind} rounds that edge's fprop operands like a tensor-core path"""
+    fprop_operands: {edge index: operand-model kind} rounds that edge's fprop operands like a tensor-core path;
+    fault: 'relu_deriv' takes ReLU' instead of sigma' at every logistic layer, 'labels_deriv' makes a soft-target
+    output derivative against one-hot labels, 'adagrad_twice' adds the squared gradient to the Adagrad state twice"""
     g = torch.Generator().manual_seed(seed)
     m = model
     L = len(m.layers)
@@ -63,6 +70,9 @@ def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None):
         seeds = [int(s) for s in torch.randint(1, 2 ** 62, (L,), generator=g)]
         seeds = [s if m.layers[i].dropprob > 0 else 0 for i, s in enumerate(seeds)]
     labels = torch.randint(0, m.layers[-1].C, (N,), generator=g)
+    targets = None
+    if m.loss != lr.CE_MULTINOMIAL:
+        targets = se.make_targets(m.loss, N, m.layers[-1].floats(N) // N, g).reshape(-1)
     l0 = m.layers[0]
     x = torch.randn(l0.floats(N), generator=g)
 
@@ -85,6 +95,14 @@ def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None):
             else:
                 wt = W.view(gg.Cin, gg.ky, gg.kx, gg.Cout).permute(3, 0, 1, 2)
                 z = tF.conv2d(xin, wt, b, stride=(gg.sy, gg.sx), padding=(gg.py, gg.px))
+        elif e.kind == "RGBTOYUV":
+            z = torch.einsum("ij,njhw->nihw", torch.tensor(ax.YUV, dtype=torch.float32), h)
+        elif e.kind == "UPSAMPLE":
+            f = int(e.cfg["sample_factor"])
+            z = h.repeat_interleave(f, 2).repeat_interleave(f, 3)
+        elif e.kind == "DOWNSAMPLE":
+            f = int(e.cfg["sample_factor"])
+            z = tF.avg_pool2d(h, f, f)
         elif e.kind == "MAXPOOL":
             pg = m.pool_geo(e, N)
             z = tF.max_pool2d(h, (pg.ky, pg.kx), (pg.sy, pg.sx), (pg.py, pg.px))
@@ -95,12 +113,17 @@ def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None):
             c = e.cfg
             kk = int(np.float32(c["frac_of_filters_response_norm"]) * np.float32(s.C))
             z = _rnorm(h, kk, se.f32(c["add_scale"]), se.f32(c["pow_scale"]), bool(c["response_norm_in_blocks"]))
-        z.retain_grad()
+        if z.requires_grad:                 # (not the RGBTOYUV output: nothing below it is trained)
+            z.retain_grad()
         zs.append(z)
         if d.act == "RECTIFIED_LINEAR":
             h = torch.relu(z)
-        elif d.act == "SOFTMAX":
+        elif d.act in ("SOFTMAX", "SOFTMAX_DIST"):
             h = torch.softmax(z, 1)
+        elif d.act == "LOGISTIC" and fault == "relu_deriv" and e.dst < L - 1:
+            h = _LogisticReluDeriv.apply(z)
+        elif d.act == "LOGISTIC":
+            h = torch.sigmoid(z)
         else:
             h = z
         if d.dropprob > 0:
@@ -108,21 +131,37 @@ def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None):
             mask = torch.from_numpy(kept).float() * se.dropout_scale(d.dropprob)
             h = h * _nchw(mask, N, d.C, d.H, d.W)
         states.append(_flat(h.detach()))
-    p = h.detach().reshape(N, -1)
-    onehot = tF.one_hot(labels, p.shape[1]).float()
-    loss = float(-torch.log(p[torch.arange(N), labels]).sum())
-    zs[-1].backward((p - onehot).reshape(zs[-1].shape))
-    derivs = [None] + [_flat(z.grad) for z in zs[1:]]
-    grads = torch.zeros(m.total, dtype=torch.float32)
+    C = m.layers[-1].floats(N) // N           # output features (units x pixels), image fastest like the targets
+    p = _flat(h.detach()).view(C, N).t()
+    t = None if targets is None else targets.view(C, N).t()
+    if fault == "labels_deriv":
+        t = None
+    # the output derivative at the pre-activation: y - onehot, y - t (don't-care entries 0), times the loss weight
+    dz = p - (tF.one_hot(labels, C).float() if t is None else t)
+    if m.loss == lr.CE_BINARY:
+        dz = torch.where(targets.view(C, N).t() >= 0, dz, torch.zeros_like(dz))
+    dz = dz * m.loss_weight
+    _, _, v, _ = lr.loss_ref(m.loss, p.double().numpy(), t=None if targets is None else targets.view(C, N).t().numpy(),
+                             labels=labels.numpy(), weight=m.loss_weight)
+    loss = float(m.loss_weight * v.sum())
+    zs[-1].backward(_nchw(dz.t().reshape(-1), N, m.layers[-1].C, m.layers[-1].H, m.layers[-1].W))
+    derivs = [None] + [_flat(z.grad) if m.receives_deriv(i + 1) else None for i, z in enumerate(zs[1:])]
+    grads = torch.full((m.total,), float("nan"))
+    grads.view(torch.int32).fill_(se.SENTINEL)
     for k, e in enumerate(m.edges):
-        if e.kind in se.WEIGHTED:
+        if e.kind in se.WEIGHTED and k >= m.frozen:
             (w0, w1), bs = m.weight_slices(k, N)
             grads[w0:w1] = P.grad[w0:w1] / N
             grads[bs[0]:bs[1]] = P.grad[bs[0]:bs[1]] / N
     opt_state = {}
     p_after, h_after = params.clone(), hist.clone()
+    adaptive = any(se.RULES[m.edges[k].cfg[key][0].get("optimizer_type", "STOCHASTIC_GRADIENT_DESCENT")] != opt.SGD
+                   for k in range(len(m.edges)) if m.edges[k].kind in se.WEIGHTED and m.owner[k] == k
+                   for key in ("weight_optimizer", "bias_optimizer"))
+    s_before = (torch.rand(m.total, generator=g) + 0.5) if adaptive else None
+    s_after = None if s_before is None else s_before.clone()
     for k, e in enumerate(m.edges):
-        if e.kind not in se.WEIGHTED:
+        if e.kind not in se.WEIGHTED or k < m.frozen or m.owner[k] != k:      # (a tie group is updated once)
             continue
         opt_state[k] = {}
         (w0, w1), bs = m.weight_slices(k, N)
@@ -131,10 +170,41 @@ def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None):
             eps, mom = net.optimizer_schedule(cfg, 0)
             eps = se.f32(eps * lr_scale)
             opt_state[k][which] = {"step": 0, "epsilon": eps, "momentum": mom}
-            w, hh, _ = opt.opt_update(params[a:b].numpy(), hist[a:b].numpy(), None, grads[a:b].numpy(), lr=eps,
-                                      mom=mom, l2=max(cfg["l2_decay"], 0.0), clip=max(cfg["gradient_clip"], 0.0))
+            rule = {0: opt.SGD, 2: opt.ADAGRAD, 3: opt.RMSPROP}[cfg["optimizer_type"]]     # (proto OptimizerType)
+            param = cfg["adagrad_delta"] if rule == opt.ADAGRAD else cfg["rms_prop_factor"]
+            st = None if rule == opt.SGD else s_before[a:b].numpy()
+            if fault == "adagrad_twice" and rule == opt.ADAGRAD:
+                st = opt.adagrad_state(st, grads[a:b].numpy(), param)
+            w, hh, st = opt.opt_update(params[a:b].numpy(), hist[a:b].numpy(), st, grads[a:b].numpy(), rule, lr=eps,
+                                       mom=mom, l2=max(cfg["l2_decay"], 0.0), clip=max(cfg["gradient_clip"], 0.0),
+                                       param=param, scale=opt.adagrad_scale(0))
             p_after[a:b], h_after[a:b] = torch.from_numpy(w), torch.from_numpy(hh)
-    return se.Snapshot(N, labels, states, derivs, params, hist, grads, p_after, h_after, loss, seeds, opt_state)
+            if st is not None:
+                s_after[a:b] = torch.from_numpy(st)
+    return se.Snapshot(N, labels, states, derivs, params, hist, grads, p_after, h_after, loss, seeds, opt_state,
+                       targets, s_before, s_after)
+
+
+class _LogisticReluDeriv(torch.autograd.Function):
+    """sigma forward, ReLU' backward (a logistic layer whose derivative pass takes the ReLU rule)"""
+
+    @staticmethod
+    def forward(ctx, z):
+        y = torch.sigmoid(z)
+        ctx.save_for_backward(y)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        y, = ctx.saved_tensors
+        return dy * (y > 0).float()
+
+
+def _sample_dropout_model(tmp_path):
+    path = str(tmp_path / "updowndrop.pbtxt")
+    with open(path, "w") as f:
+        f.write(se.sample_dropout_text())
+    return path
 
 
 def _dropout_model(tmp_path):
@@ -288,7 +358,192 @@ def test_bf16_operand_truncated_instead_of_rounded():
     assert not r.ok and (r.layer, r.quantity) == ("conv2", "fprop"), str(r)
 
 
-@pytest.mark.parametrize("name", ["tiny+bn", "lcnet", "tiednet", "logcheck", "c3d"])
+# the kinds beyond SGD chains of ReLU / linear layers with a softmax output: logistic units, the target-trained output
+# layers, the adaptive optimizers and frozen trunks
+NEW_KINDS = [("tiny+logistic", 32), ("logcheck", 32), ("tiny+squared-error", 32), ("tiny+binary-ce", 32),
+             ("tiny+soft-targets", 32), ("tiny+adagrad", 32), ("tiny+rmsprop", 32), ("tiny+finetune", 32),
+             ("tiny+logistic+adagrad+finetune", 32), ("tiednet", 8), ("updowncheck", 32), ("updown", 2)]
+
+
+@pytest.mark.parametrize("name,N", NEW_KINDS)
+def test_auditor_passes_new_kinds(name, N):
+    m = se.load_model(name, N)
+    rows = _audit(m, simulate(m, N))
+    assert not se.failures(rows), "\n".join(map(str, se.failures(rows)))
+    kinds = {r.quantity for r in rows}
+    assert {"output_deriv", "loss"} <= kinds
+    if "adagrad" in name or "rmsprop" in name:
+        assert {"state_weights", "state_bias"} <= kinds
+    if "finetune" in name:
+        assert {"frozen_params", "frozen_history", "frozen_grads", "frozen_deriv"} <= kinds
+        assert not any(r.quantity in ("dgrad", "undo") and r.layer in ("conv1", "pool1", "rnorm1", "nin1", "conv2")
+                       for r in rows)
+
+
+def test_sigma_deriv_replaced_by_relu_deriv():
+    """logcheck with ReLU' (1 everywhere on a logistic layer) where sigma' belongs: the dgrad of the 1x1 edge into rnorm1
+    and the undos into the logistic pooling layers fail"""
+    m = se.load_model("logcheck", 32)
+    s = simulate(m, 32, fault="relu_deriv")
+    _caught(m, s, "rnorm1", "dgrad")
+    _caught(m, s, "pool1", "undo")
+
+
+def test_sigma_left_out_of_logistic_fprop():
+    m = se.load_model("tiny+logistic", 32)
+    s = simulate(m, 32)
+    i = _layer_index(m, "conv2")
+    k = _edge_index(m, "conv2")
+    e = cx.expect("fprop", m.conv_geo(m.edges[k], 32), s.states[i - 1], se.Auditor(m, "fp32").weights(
+        s.params_before, k, 32)[0], "fp32", bias=se.Auditor(m, "fp32").weights(s.params_before, k, 32)[1])
+    s.states[i] = e.ref.to(torch.float32)
+    _caught(m, s, "conv2", "fprop")
+
+
+@pytest.mark.parametrize("name", ["tiny+squared-error", "tiny+binary-ce", "tiny+soft-targets"])
+def test_output_derivative_against_labels(name):
+    """the output derivative taken against one-hot labels instead of the layer's float targets"""
+    m = se.load_model(name, 32)
+    _caught(m, simulate(m, 32, fault="labels_deriv"), "output", "output_deriv")
+
+
+def test_binary_dont_care_targets_get_a_derivative():
+    m = se.load_model("tiny+binary-ce", 32)
+    s = simulate(m, 32)
+    care = s.targets >= 0
+    assert 0 < int((~care).sum()) < care.numel() // 4
+    i = int(torch.nonzero(~care)[0])
+    s.derivs[-1][i] = s.states[-1][i] - 0.5
+    _caught(m, s, "output", "output_deriv")
+
+
+def test_adagrad_state_updated_twice():
+    m = se.load_model("tiny+adagrad", 32)
+    _caught(m, simulate(m, 32, fault="adagrad_twice"), m.edges[_edge_index(m, "conv2")].name, "state_weights")
+
+
+def test_frozen_weight_changed_by_one_ulp():
+    m = se.load_model("tiny+finetune", 32)
+    assert m.frozen == 6 and m.trained_offset == m.offsets[6]
+    s = simulate(m, 32)
+    k = _edge_index(m, "conv2")
+    (w0, _), _ = m.weight_slices(k, 32)
+    _flip_lsb(s.params_after, w0 + 5)
+    _caught(m, s, m.edges[k].name, "frozen_params")
+
+
+@pytest.mark.parametrize("name,which", [("tiny+adagrad", "weights"), ("tiny+adagrad", "bias"),
+                                        ("tiny+rmsprop", "weights"), ("tiny+rmsprop", "bias")])
+def test_adaptive_state_off_by_one_ulp(name, which):
+    m = se.load_model(name, 32)
+    s = simulate(m, 32)
+    k = _edge_index(m, "nin1")
+    (w0, _), bs = m.weight_slices(k, 32)
+    _flip_lsb(s.state_after, (w0 if which == "weights" else bs[0]) + 1)
+    _caught(m, s, m.edges[k].name, "state_" + which)
+
+
+@pytest.mark.parametrize("qty", ["frozen_history", "frozen_state"])
+def test_frozen_history_or_state_changed_by_one_ulp(qty):
+    m = se.load_model("tiny+logistic+adagrad+finetune", 32)
+    s = simulate(m, 32)
+    k = _edge_index(m, "nin1")
+    (w0, _), _ = m.weight_slices(k, 32)
+    _flip_lsb(s.hist_after if qty == "frozen_history" else s.state_after, w0 + 3)
+    _caught(m, s, m.edges[k].name, qty)
+
+
+def test_frozen_gradient_written():
+    m = se.load_model("tiny+finetune", 32)
+    s = simulate(m, 32)
+    k = _edge_index(m, "conv1")
+    (w0, _), _ = m.weight_slices(k, 32)
+    s.grads[w0 + 2] = 0.0
+    _caught(m, s, m.edges[k].name, "frozen_grads")
+    s = simulate(m, 32)
+    s.derivs[_layer_index(m, "nin1")] = torch.zeros_like(s.states[_layer_index(m, "nin1")])
+    _caught(m, s, "nin1", "frozen_deriv")
+
+
+def test_tie_group_missing_a_member():
+    """tiednet's conv group (conv1:conv2 with pool2:conv3 and conv3:conv4) trained on two of its three wgrads"""
+    m = se.load_model("tiednet", 8)
+    s = simulate(m, 8)
+    assert not se.failures(_audit(m, s))
+    o = _edge_index(m, "conv2")
+    assert m.group(o) == [1, 3, 4] and m.owner[4] == o
+    e = m.edges[4]
+    (w0, w1), _ = m.weight_slices(4, 8)
+    assert m.weight_slices(o, 8)[0] == (w0, w1)
+    miss = cx.expect("wgrad", m.conv_geo(e, 8), s.states[e.src], s.derivs[e.dst], "fp32", so=1.0 / 8)
+    s.grads[w0:w1] -= miss.ref.to(torch.float32)
+    _caught(m, s, m.edges[o].name, "wgrad")
+
+
+@pytest.fixture(scope="module")
+def sample_drop_model(tmp_path_factory):
+    path = _sample_dropout_model(tmp_path_factory.mktemp("model"))
+    return se.load_model(path, 32)
+
+
+def test_auditor_passes_sampling_dropout_step(sample_drop_model):
+    m = sample_drop_model
+    s = simulate(m, 32)
+    assert s.seeds[_layer_index(m, "down1")] and s.seeds[_layer_index(m, "up4")]
+    rows = _audit(m, s)
+    assert not se.failures(rows), "\n".join(map(str, se.failures(rows)))
+    assert {("down1", "fprop"), ("down1", "dgrad"), ("up4", "fprop"), ("up4", "dgrad"), ("conv3", "undo")} <= {
+        (r.layer, r.quantity) for r in rows}
+
+
+def test_sampling_dropout_faults(sample_drop_model):
+    """a dropout scale left out of the DOWNSAMPLE and UPSAMPLE fprops, and the dropout fold left out of the DOWNSAMPLE
+    undo into conv3"""
+    m = sample_drop_model
+    for name in ("down1", "up4"):
+        s = simulate(m, 32)
+        s.states[_layer_index(m, name)] /= se.dropout_scale(0.25)
+        _caught(m, s, name, "fprop")
+    s = simulate(m, 32)
+    s.derivs[_layer_index(m, "conv3")] /= se.dropout_scale(0.25)
+    _caught(m, s, "conv3", "undo")
+
+
+def test_upsample_backward_without_f2():
+    """the derivative into conv2 (below up2, f = 3) as the block mean instead of the block sum"""
+    m = se.load_model("updowncheck", 32)
+    s = simulate(m, 32)
+    s.derivs[_layer_index(m, "conv2")] /= 9
+    _caught(m, s, "conv2", "undo")
+
+
+def test_yuv_row_swapped():
+    """RGBTOYUV with its U and V rows exchanged"""
+    m = se.load_model("updown", 2)
+    s = simulate(m, 2)
+    y = s.states[_layer_index(m, "yuv")].view(3, -1)
+    s.states[_layer_index(m, "yuv")] = y[[0, 2, 1]].reshape(-1).clone()
+    _caught(m, s, "yuv", "fprop")
+    s = simulate(m, 2)
+    s.derivs[_layer_index(m, "yuv")] = torch.zeros_like(s.states[_layer_index(m, "yuv")])
+    _caught(m, s, "yuv", "no_deriv")
+
+
+def test_tie_group_bias_missing_a_member():
+    """tiednet's FC pair (fc5:fc6 tied to fc6:fc7): the bias gradient from the owner's column sum alone"""
+    m = se.load_model("tiednet", 8)
+    s = simulate(m, 8)
+    o = _edge_index(m, "fc7")
+    assert m.group(o) == [6, 7]
+    e = m.edges[6]
+    d = m.layers[e.dst]
+    _, bs = m.weight_slices(o, 8)
+    miss = s.derivs[e.dst].double().view(d.C, -1).sum(1) / 8
+    s.grads[bs[0]:bs[1]] -= miss.to(torch.float32)
+    _caught(m, s, m.edges[o].name, "bias_grad")
+
+
+@pytest.mark.parametrize("name", ["tiny+bn", "lcnet", "c3d", "tiedcheck", "localcheck"])
 def test_unsupported_models_raise(name):
     with pytest.raises(se.Unsupported):
         se.load_model(name, 32)

@@ -703,11 +703,11 @@ void dropout_apply(float* x, long long n, float dropprob, float scale, unsigned 
 // (image, patch column) for one (patch row, colour) goes through shared memory: the reads run along a source row (128
 // contiguous bytes per image, reversed when mirrored), the writes along the images (the fastest axis of the layer state).
 // The reference's kernel maps threads to patch columns and so stores with a stride of N floats (cudamat_kernels.cu:1655).
-__global__ void __launch_bounds__(256) extract_patches_kernel(const float* __restrict__ images, float* __restrict__ patches,
-                                                              const float* __restrict__ width_offset,
-                                                              const float* __restrict__ height_offset,
-                                                              const float* __restrict__ flip, int N, int W, int H, int pw, int ph,
-                                                              int C) {
+// Batch image n reads chunk column index[n], or column n when index is null.
+__device__ __forceinline__ void extract_patch_tile(const float* __restrict__ images, float* __restrict__ patches,
+                                                   const float* __restrict__ width_offset,
+                                                   const float* __restrict__ height_offset, const float* __restrict__ flip,
+                                                   const int* __restrict__ index, int N, int W, int H, int pw, int ph, int C) {
   __shared__ float tile[32][33];
   const int row = (int)(blockIdx.z % (unsigned)ph), color = (int)(blockIdx.z / (unsigned)ph);
   const int n0 = blockIdx.y * 32, c0 = blockIdx.x * 32;
@@ -717,7 +717,8 @@ __global__ void __launch_bounds__(256) extract_patches_kernel(const float* __res
       int sr = (int)height_offset[n] + row, sc = (int)width_offset[n] + dc;
       if (flip[n] > 0.5f) sc = W - sc - 1;
       sr = min(max(sr, 0), H - 1); sc = min(max(sc, 0), W - 1);
-      tile[k][threadIdx.x] = __ldg(images + sc + (size_t)W * (sr + (size_t)H * (color + (size_t)C * n)));
+      const size_t col = index ? (size_t)__ldg(index + n) : (size_t)n;
+      tile[k][threadIdx.x] = __ldg(images + sc + (size_t)W * (sr + (size_t)H * (color + (size_t)C * col)));
     }
   }
   __syncthreads();
@@ -725,6 +726,13 @@ __global__ void __launch_bounds__(256) extract_patches_kernel(const float* __res
     const int dc = c0 + k, n = n0 + (int)threadIdx.x;
     if (n < N && dc < pw) patches[n + (size_t)N * (dc + (size_t)pw * (row + (size_t)ph * color))] = tile[threadIdx.x][k];
   }
+}
+__global__ void __launch_bounds__(256) extract_patches_kernel(const float* __restrict__ images, float* __restrict__ patches,
+                                                              const float* __restrict__ width_offset,
+                                                              const float* __restrict__ height_offset,
+                                                              const float* __restrict__ flip, int N, int W, int H, int pw, int ph,
+                                                              int C) {
+  extract_patch_tile(images, patches, width_offset, height_offset, flip, nullptr, N, W, H, pw, ph, C);
 }
 int extract_patches(const float* images, float* patches, const float* width_offset, const float* height_offset,
                     const float* flip, int N, int W, int H, int pw, int ph, int C) {
@@ -736,12 +744,53 @@ int extract_patches(const float* images, float* patches, const float* width_offs
   count_launch();
   return cudaGetLastError() == cudaSuccess ? 0 : -3;
 }
+
+// cnb_extract_patches_indexed: the tile kernel above through a permutation of the chunk, plus one tail slice of blocks
+// (blockIdx.z == ph * C) that gathers the same 32 images' labels and targets.  Only the tail's blockIdx.x == 0 column
+// works, so each image's label and target row is written once.
+__global__ void __launch_bounds__(256) extract_patches_indexed_kernel(
+    const float* __restrict__ images, float* __restrict__ patches, const int* __restrict__ index,
+    const float* __restrict__ width_offset, const float* __restrict__ height_offset, const float* __restrict__ flip,
+    const int* __restrict__ labels_src, int* __restrict__ labels_dst, const float* __restrict__ targets_src,
+    float* __restrict__ targets_dst, int target_dims, int N, int W, int H, int pw, int ph, int C) {
+  if (blockIdx.z < (unsigned)(ph * C)) {
+    extract_patch_tile(images, patches, width_offset, height_offset, flip, index, N, W, H, pw, ph, C);
+    return;
+  }
+  if (blockIdx.x != 0) return;
+  const int n0 = blockIdx.y * 32, t = threadIdx.x + 32 * threadIdx.y;
+  const int rows = min(32, N - n0);
+  if (labels_dst && t < rows) labels_dst[n0 + t] = __ldg(labels_src + __ldg(index + n0 + t));
+  if (targets_dst)                                           // thread t: image t % 32, features t / 32, t / 32 + 8, ...
+    for (int j = t >> 5; j < target_dims; j += 8) {
+      const int n = n0 + (t & 31);
+      if ((t & 31) < rows) targets_dst[n + (size_t)N * j] = __ldg(targets_src + (size_t)target_dims * __ldg(index + n) + j);
+    }
+}
 }  // namespace cnb
 
 using namespace cnb;
 
 extern "C" {
 
+int cnb_extract_patches_indexed(const float* images, float* patches, const int* index, const float* width_offset,
+                                const float* height_offset, const float* flip, int N, int C, int W, int H, int pw,
+                                int ph, const int* labels_src, int* labels_dst, const float* targets_src,
+                                float* targets_dst, int target_dims) {
+  if (N < 0 || C <= 0 || W <= 0 || H <= 0 || pw <= 0 || ph <= 0 || pw > W || ph > H || target_dims < 0) return -1;
+  if (!images || !patches || !index || !width_offset || !height_offset || !flip) return -1;
+  if (!labels_src != !labels_dst || !targets_src != !targets_dst || (targets_dst && target_dims == 0)) return -1;
+  if (N == 0) return 0;
+  if ((long long)ph * C + 1 > 65535 || ceil_div(N, 32) > 65535) return -1;
+  bf16_note_write(patches, (long long)N * pw * ph * C);
+  if (targets_dst) bf16_note_write(targets_dst, (long long)N * target_dims);
+  const dim3 grid((unsigned)ceil_div(pw, 32), (unsigned)ceil_div(N, 32), (unsigned)(ph * C + 1));
+  extract_patches_indexed_kernel<<<grid, dim3(32, 8), 0, state().stream>>>(images, patches, index, width_offset, height_offset,
+                                                                flip, labels_src, labels_dst, targets_src,
+                                                                targets_dst, target_dims, N, W, H, pw, ph, C);
+  count_launch();
+  return cudaGetLastError() == cudaSuccess ? 0 : -3;
+}
 void cnb_add_channel_bias(float* acts, const float* bias, long long rows, int cols) {
   stream_pass("add_channel_bias", acts, rows > 0 && cols > 0 ? rows * cols : 0, rows % 4 == 0 && aligned16(acts), false,
               BiasOp<kActNone>{bias, rows});

@@ -429,3 +429,66 @@ API int cnb_data_last_noise(void* d, float* out, int cap) {
 API void cnb_data_view_offset(int multiplicity_id, int max_offset_x, int max_offset_y, int* w, int* h) {
   DataIterator::ViewOffset(multiplicity_id, max_offset_x, max_offset_y, w, h);
 }
+
+// ---- the data set feed (data.h): DataSchedule is the pure host state machine, DataHandler runs it on the GPU.  A refused
+// configuration gives NULL / -1 and the reason in cnb_last_error()
+API void* cnb_schedule_create(const DatasetOrder* c, int dataset_size, unsigned long long seed) {
+  try { return new DataSchedule(*c, dataset_size, seed); }
+  catch (const std::invalid_argument& e) { g_last_error = e.what(); return nullptr; }
+}
+API void cnb_schedule_destroy(void* s) { delete (DataSchedule*)s; }
+API int cnb_schedule_chunk_size(void* s) { return ((DataSchedule*)s)->ChunkSize(); }
+// the next minibatch: *start, *multiplicity_id; returns 1 if a chunk was loaded for it (its data set rows into rows[chunk]),
+// else 0; perm[chunk] receives the permutation in force
+API int cnb_schedule_next(void* p, int* start, int* multiplicity_id, int* rows, int* perm) {
+  DataSchedule* s = (DataSchedule*)p;
+  const DataSchedule::Batch b = s->Next();
+  *start = b.start; *multiplicity_id = b.multiplicity_id;
+  memcpy(perm, s->Permutation().data(), sizeof(int) * s->ChunkSize());
+  if (b.loaded) memcpy(rows, s->Rows().data(), sizeof(int) * s->ChunkSize());
+  return b.loaded ? 1 : 0;
+}
+API int cnb_schedule_seek(void* s, int row) {
+  try { ((DataSchedule*)s)->Seek(row); return 0; }
+  catch (const std::invalid_argument& e) { g_last_error = e.what(); return -1; }
+}
+// images: dataset_size x channels*y*x floats, labels: dataset_size ints (or NULL), targets: dataset_size x target_dims
+// floats (or NULL), all in host memory that outlives the handler
+API void* cnb_handler_create(const DatasetOrder* c, int dataset_size, int channels, int image_size_y, int image_size_x,
+                             int gpu_image_size_y, int gpu_image_size_x, int translate, int flip, const float* images,
+                             const int* labels, const float* targets, int target_dims, unsigned long long seed) {
+  try {
+    return new DataHandler(*c, dataset_size, channels, image_size_y, image_size_x, gpu_image_size_y, gpu_image_size_x,
+                           translate != 0, flip != 0, images, labels, targets, target_dims, seed);
+  } catch (const std::invalid_argument& e) { g_last_error = e.what(); return nullptr; }
+}
+API void cnb_handler_destroy(void* h) { delete (DataHandler*)h; }
+API int cnb_handler_get_batch(void* h, void* net) {
+  try { ((DataHandler*)h)->GetBatch(*((NetHandle*)net)->net); return 0; }
+  catch (const std::invalid_argument& e) { g_last_error = e.what(); return -1; }
+}
+API int cnb_handler_seek(void* h, int row) {
+  try { ((DataHandler*)h)->Seek(row); return 0; }
+  catch (const std::invalid_argument& e) { g_last_error = e.what(); return -1; }
+}
+// the last minibatch (host copies): *start, *multiplicity_id, the data set row of each image (rows[batch]) and its jitter
+// (noise[3 x batch]: width offsets, height offsets, mirror bits); returns the batch size
+API int cnb_handler_last(void* p, int* start, int* multiplicity_id, int* rows, float* noise) {
+  DataHandler* h = (DataHandler*)p;
+  const DataSchedule& s = h->Schedule();
+  const int n = (int)h->LastNoise().size() / 3;
+  *start = h->LastBatch().start; *multiplicity_id = h->LastBatch().multiplicity_id;
+  for (int i = 0; i < n; i++) rows[i] = s.Rows()[s.Permutation()[h->LastBatch().start + i]];
+  memcpy(noise, h->LastNoise().data(), sizeof(float) * 3 * n);
+  return n;
+}
+// a model's train_dataset (which 0) or valid_dataset (1): 1 and its fields, 0 when the model has none, -1 unknown model
+API int cnb_model_dataset(const char* model, int which, DatasetOrder* order, int* translate, int* flip, int* gpu_image_size_y,
+                          int* gpu_image_size_x) {
+  ModelConfig m;
+  if (!TryBuildModel(model, &m)) return -1;
+  const ModelConfig::Dataset& d = which ? m.valid_dataset : m.train_dataset;
+  *order = d.order; *translate = d.translate; *flip = d.flip;
+  *gpu_image_size_y = d.gpu_image_size_y; *gpu_image_size_x = d.gpu_image_size_x;
+  return d.present ? 1 : 0;
+}

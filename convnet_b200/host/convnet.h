@@ -13,6 +13,7 @@
 #include <string>
 #include <vector>
 
+#include "data.h"
 #include "edge.h"
 
 namespace cnbhost {
@@ -88,6 +89,14 @@ struct ModelConfig {
   // Polyak averaging (proto Model fields, same defaults): on when polyak_after and polyak_queue_size are both > 0; its
   // insertion rule (PolyakDue) also reads validate_after and save_after
   int polyak_after = 0, polyak_queue_size = 0, validate_after = -1, save_after = -1;
+  // train_dataset / valid_dataset: the batch order and, from the data stream of the input layer, its crop (gpu_image_size
+  // 0: the whole image) and jitter
+  struct Dataset {
+    bool present = false;
+    DatasetOrder order;
+    int translate = 0, flip = 0, gpu_image_size_y = 0, gpu_image_size_x = 0;
+  };
+  Dataset train_dataset, valid_dataset;
 };
 inline bool PolyakOn(const ModelConfig& m) { return m.polyak_after > 0 && m.polyak_queue_size > 0; }
 // checkpoint.cc: whether the reference's training loop inserts the parameters into the Polyak queue after TrainOneBatch call

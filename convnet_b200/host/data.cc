@@ -4,6 +4,10 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <stdexcept>
+#include <string>
+
+#include "convnet.h"
 
 namespace cnbhost {
 
@@ -99,6 +103,266 @@ void DataIterator::AddNoise(int start, Matrix& dest) {
   // (the reference copies with CopyTranspose when there is neither crop nor mirror; the same kernel covers that case)
   Matrix::ExtractPatches(data_slice, dest, width_offset_, height_offset_, flip_bit_, image_size_y_, image_size_x_,
                          gpu_image_size_y_, gpu_image_size_x_);
+}
+
+uint64_t SplitMix64(uint64_t& state) {
+  uint64_t z = (state += 0x9E3779B97F4A7C15ULL);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL; z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
+  return z ^ (z >> 31);
+}
+
+// ---------------------------------------------------------------- DataSchedule
+DataSchedule::DataSchedule(const DatasetOrder& c, int dataset_size, uint64_t seed)
+    : c_(c), dataset_size_(dataset_size), chunk_size_(c.chunk_size),
+      cpu_rng_(seed * 0x9E3779B97F4A7C15ULL + 0x632BE59BD9B4E019ULL), gpu_rng_(seed * 0x9E3779B97F4A7C15ULL + 0x8CB92BA72F3D8DD7ULL) {
+  auto refuse = [](const std::string& why) { throw std::invalid_argument("DataHandler: " + why); };
+  if (dataset_size <= 0) refuse("the data set is empty");
+  if (c.batch_size <= 0) refuse("batch_size must be positive");
+  if (c.multiplicity <= 0) refuse("multiplicity must be positive");
+  if (c.max_reuse_count < 0) refuse("max_reuse_count must not be negative");
+  if (c.random_access_chunk_size <= 0) refuse("random_access_chunk_size must be positive");
+  if (chunk_size_ <= 0 || chunk_size_ > dataset_size) {              // :45-48
+    chunk_size_ = dataset_size;
+    fits_on_gpu_ = true;
+  }
+  if (c.batch_size > chunk_size_)
+    refuse("batch_size " + std::to_string(c.batch_size) + " is larger than the chunk (" + std::to_string(chunk_size_) +
+           " images): every minibatch would reload it");
+  if (c.randomize_cpu && chunk_size_ % c.random_access_chunk_size != 0)
+    refuse("random_access_chunk_size " + std::to_string(c.random_access_chunk_size) + " does not divide the chunk (" +
+           std::to_string(chunk_size_) + " images); the reference's LoadChunk would write past the chunk's end");
+  perm_.resize(chunk_size_);                                        // SetupShuffler, :111-118 (identity when not shuffled)
+  for (int i = 0; i < chunk_size_; i++) perm_[i] = i;
+  if (c.randomize_cpu) {                                            // :54-60
+    random_indices_.resize(dataset_size);
+    for (int i = 0; i < dataset_size; i++) random_indices_[i] = i;
+    Shuffle(random_indices_, cpu_rng_);
+  }
+  Seek(0);
+}
+
+void DataSchedule::Shuffle(std::vector<int>& v, uint64_t& rng) {
+  for (size_t i = v.size(); i > 1; i--) std::swap(v[i - 1], v[SplitMix64(rng) % i]);
+}
+
+void DataSchedule::Seek(int row) {
+  if (row < 0 || row >= dataset_size_) throw std::invalid_argument("DataHandler::Seek: row " + std::to_string(row) + " is outside the data set");
+  preloading_ = false; preload_.clear();                            // Sync(): the preload finishes and is not used
+  start_ = row;
+  reuse_counter_ = 0;
+  multiplicity_counter_ = 0;
+  restart_ = true;
+  row_ = row;                                                       // the data iterators' Seek(row)
+}
+
+std::vector<int> DataSchedule::DiskAccess() {
+  std::vector<int> rows;
+  rows.reserve(chunk_size_);
+  if (c_.randomize_cpu) {
+    const size_t num_rand = (size_t)(chunk_size_ / c_.random_access_chunk_size);
+    if (random_indices_ind_ + num_rand > (size_t)dataset_size_) {
+      Shuffle(random_indices_, cpu_rng_);
+      random_indices_ind_ = 0;
+    }
+    for (size_t i = 0; i < num_rand; i++) {                         // LoadChunk(it, mat, random_rows), :290-307
+      const int row = random_indices_[random_indices_ind_++];
+      for (int k = 0; k < c_.random_access_chunk_size; k++) rows.push_back((row + k) % dataset_size_);
+    }
+  } else {
+    for (int i = 0; i < chunk_size_; i++) {                         // LoadChunk(it, mat): GetNext, wrapping at the end
+      rows.push_back(row_);
+      if (++row_ == dataset_size_) row_ = 0;
+    }
+  }
+  return rows;
+}
+
+DataSchedule::Batch DataSchedule::Next() {
+  Batch b;
+  int end = start_ + c_.batch_size;
+  if (end > chunk_size_ || restart_) {
+    if (reuse_counter_ < c_.max_reuse_count && !restart_) {
+      reuse_counter_++;
+    } else if (nothing_on_gpu_ || !fits_on_gpu_) {
+      if (restart_ && c_.pipeline_loads) { preload_ = DiskAccess(); preloading_ = true; }    // StartPreload
+      nothing_on_gpu_ = false;
+      reuse_counter_ = 0;
+      if (c_.pipeline_loads) { rows_ = preload_; preloading_ = false; }                   // PipelinedDiskAccess
+      else rows_ = DiskAccess();
+      b.loaded = true;
+      if (c_.pipeline_loads) { preload_ = DiskAccess(); preloading_ = true; }
+    }
+    restart_ = false;
+    if (c_.randomize_gpu) { Shuffle(perm_, gpu_rng_); b.reshuffled = true; }             // ShuffleIndices
+    start_ = 0;
+    end = c_.batch_size;
+  }
+  b.start = start_;
+  b.multiplicity_id = multiplicity_counter_;
+  if (++multiplicity_counter_ == c_.multiplicity) {
+    multiplicity_counter_ = 0;
+    start_ = end;
+  }
+  if (!preloading_) preload_.clear();
+  return b;
+}
+
+// ---------------------------------------------------------------- DataHandler
+DataHandler::DataHandler(const DatasetOrder& c, int dataset_size, int channels, int image_size_y, int image_size_x,
+                         int gpu_image_size_y, int gpu_image_size_x, bool translate, bool flip, const float* images,
+                         const int* labels, const float* targets, int target_dims, uint64_t seed)
+    : schedule_(c, dataset_size, seed), channels_(channels), isy_(image_size_y), isx_(image_size_x), gy_(gpu_image_size_y),
+      gx_(gpu_image_size_x), target_dims_(targets ? target_dims : 0), batch_(c.batch_size), translate_(translate),
+      flip_(flip), images_(images), labels_(labels), targets_(targets),
+      rng_(seed * 0x9E3779B97F4A7C15ULL + 0xD1B54A32D192ED03ULL) {
+  if (channels <= 0 || gy_ <= 0 || gx_ <= 0 || gy_ > isy_ || gx_ > isx_)
+    throw std::invalid_argument("DataHandler: the crop must fit the image");
+  if (!images || (targets && target_dims <= 0)) throw std::invalid_argument("DataHandler: no images, or targets without a width");
+  const size_t chunk = (size_t)schedule_.ChunkSize(), dims = (size_t)channels * isy_ * isx_;
+  const int nbuf = schedule_.Pipelined() && !schedule_.FitsOnGpu() ? 2 : 1;
+  for (int b = 0; b < nbuf; b++) {
+    DATA_CUDA_CHECK(cudaMalloc((void**)&d_images_[b], sizeof(float) * chunk * dims));
+    if (labels_) DATA_CUDA_CHECK(cudaMalloc((void**)&d_labels_[b], sizeof(int) * chunk));
+    if (targets_) DATA_CUDA_CHECK(cudaMalloc((void**)&d_targets_[b], sizeof(float) * chunk * target_dims_));
+  }
+  DATA_CUDA_CHECK(cudaMalloc((void**)&d_perm_, sizeof(int) * chunk));
+  DATA_CUDA_CHECK(cudaMalloc((void**)&d_noise_, sizeof(float) * 3 * batch_));
+  DATA_CUDA_CHECK(cudaMallocHost((void**)&pinned_noise_, sizeof(float) * 3 * batch_ * kRing));
+  DATA_CUDA_CHECK(cudaMallocHost((void**)&pinned_perm_, sizeof(int) * chunk * kRing));
+  for (int k = 0; k < kRing; k++) {
+    DATA_CUDA_CHECK(cudaEventCreateWithFlags(&noise_done_[k], cudaEventDisableTiming));
+    DATA_CUDA_CHECK(cudaEventCreateWithFlags(&perm_done_[k], cudaEventDisableTiming));
+  }
+  for (int b = 0; b < 2; b++) {
+    DATA_CUDA_CHECK(cudaEventCreateWithFlags(&loaded_[b], cudaEventDisableTiming));
+    DATA_CUDA_CHECK(cudaEventCreateWithFlags(&consumed_[b], cudaEventDisableTiming));
+  }
+  if (nbuf == 2) DATA_CUDA_CHECK(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
+  UploadPermutation();                                              // the identity, until a pass reshuffles it
+}
+
+DataHandler::~DataHandler() {
+  cudaStreamSynchronize(Matrix::Stream());                          // crops and uploads may still read these buffers
+  if (copy_stream_) { cudaStreamSynchronize(copy_stream_); cudaStreamDestroy(copy_stream_); }
+  for (int b = 0; b < 2; b++) {
+    cudaFree(d_images_[b]); cudaFree(d_labels_[b]); cudaFree(d_targets_[b]);
+    cudaEventDestroy(loaded_[b]); cudaEventDestroy(consumed_[b]);
+  }
+  for (int k = 0; k < kRing; k++) { cudaEventDestroy(noise_done_[k]); cudaEventDestroy(perm_done_[k]); }
+  cudaFree(d_perm_); cudaFree(d_noise_);
+  cudaFreeHost(pinned_noise_); cudaFreeHost(pinned_perm_);
+}
+
+// the data set rows `rows` into chunk buffer `buf`, one copy per run of consecutive rows
+void DataHandler::CopyRows(const std::vector<int>& rows, int buf, cudaStream_t s) {
+  const size_t dims = (size_t)channels_ * isy_ * isx_;
+  for (size_t i = 0; i < rows.size();) {
+    size_t run = 1;
+    while (i + run < rows.size() && rows[i + run] == rows[i] + (int)run) run++;
+    const size_t r = (size_t)rows[i];
+    DATA_CUDA_CHECK(cudaMemcpyAsync(d_images_[buf] + i * dims, images_ + r * dims, sizeof(float) * run * dims,
+                                    cudaMemcpyHostToDevice, s));
+    if (labels_) DATA_CUDA_CHECK(cudaMemcpyAsync(d_labels_[buf] + i, labels_ + r, sizeof(int) * run, cudaMemcpyHostToDevice, s));
+    if (targets_)
+      DATA_CUDA_CHECK(cudaMemcpyAsync(d_targets_[buf] + i * target_dims_, targets_ + r * target_dims_,
+                                      sizeof(float) * run * target_dims_, cudaMemcpyHostToDevice, s));
+    i += run;
+  }
+}
+
+void DataHandler::UploadPermutation() {
+  const int slot = perm_slot_;
+  perm_slot_ = (perm_slot_ + 1) % kRing;
+  const std::vector<int>& perm = schedule_.Permutation();
+  int* block = pinned_perm_ + (size_t)slot * perm.size();
+  DATA_CUDA_CHECK(cudaEventSynchronize(perm_done_[slot]));          // the block's last copy has left it
+  memcpy(block, perm.data(), sizeof(int) * perm.size());
+  DATA_CUDA_CHECK(cudaMemcpyAsync(d_perm_, block, sizeof(int) * perm.size(), cudaMemcpyHostToDevice, Matrix::Stream()));
+  DATA_CUDA_CHECK(cudaEventRecord(perm_done_[slot], Matrix::Stream()));
+}
+
+// the rules of DataIterator::SampleNoise (src/datahandler.cc:533-568), on this handler's generator, into a pinned block
+void DataHandler::SampleNoise(int multiplicity_id) {
+  const int max_offset_y = isy_ - gy_, max_offset_x = isx_ - gx_, n = batch_;
+  h_noise_.assign(3 * (size_t)n, 0.f);
+  float *wo = h_noise_.data(), *ho = wo + n, *fl = ho + n;
+  auto uniform = [this] { return (float)(SplitMix64(rng_) >> 40) * (1.0f / 16777216.0f); };
+  if (translate_) {
+    for (int i = 0; i < n; i++) {
+      const int oy = (int)(uniform() * (max_offset_y + 1)), ox = (int)(uniform() * (max_offset_x + 1));
+      ho[i] = (float)(oy > max_offset_y ? max_offset_y : oy);
+      wo[i] = (float)(ox > max_offset_x ? max_offset_x : ox);
+    }
+  } else {
+    int w, h;
+    DataIterator::ViewOffset(multiplicity_id, max_offset_x, max_offset_y, &w, &h);
+    for (int i = 0; i < n; i++) { wo[i] = (float)w; ho[i] = (float)h; }
+  }
+  for (int i = 0; i < n; i++) fl[i] = flip_ ? uniform() : (float)(multiplicity_id / 5);
+  const int slot = noise_slot_;
+  noise_slot_ = (noise_slot_ + 1) % kRing;
+  float* block = pinned_noise_ + (size_t)slot * 3 * n;
+  DATA_CUDA_CHECK(cudaEventSynchronize(noise_done_[slot]));         // kRing batches ago: long done
+  memcpy(block, h_noise_.data(), sizeof(float) * 3 * n);
+  DATA_CUDA_CHECK(cudaMemcpyAsync(d_noise_, block, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, Matrix::Stream()));
+  DATA_CUDA_CHECK(cudaEventRecord(noise_done_[slot], Matrix::Stream()));
+}
+
+void DataHandler::Seek(int row) {
+  schedule_.Seek(row);
+  staged_ = false;                                                  // a copy still in flight is overwritten in stream order
+}
+
+void DataHandler::GetBatch(Matrix& input, int* labels_out, float* targets_out) {
+  if (input.GetRows() != batch_ || input.GetCols() != channels_ * gy_ * gx_)
+    throw std::invalid_argument("DataHandler::GetBatch: the input layer is not batch_size x channels * crop");
+  if ((labels_out && !labels_) || (targets_out && !targets_))
+    throw std::invalid_argument(std::string("DataHandler::GetBatch: the net trains on ") + (labels_out ? "labels" : "targets") +
+                                " and the data set has none");
+  const cudaStream_t s = Matrix::Stream();
+  last_ = schedule_.Next();
+  if (last_.loaded) {
+    if (!copy_stream_) {
+      CopyRows(schedule_.Rows(), cur_, s);
+    } else {                                                        // WaitForPreload: swap in the staged chunk
+      const int next = 1 - cur_;
+      if (!staged_) {                                               // a preload begun within this GetBatch (a restart)
+        DATA_CUDA_CHECK(cudaStreamWaitEvent(copy_stream_, consumed_[next], 0));
+        CopyRows(schedule_.Rows(), next, copy_stream_);
+        DATA_CUDA_CHECK(cudaEventRecord(loaded_[next], copy_stream_));
+      }
+      DATA_CUDA_CHECK(cudaStreamWaitEvent(s, loaded_[next], 0));
+      DATA_CUDA_CHECK(cudaEventRecord(consumed_[cur_], s));         // behind the last crop that read the old chunk
+      cur_ = next;
+      staged_ = false;
+      if (!schedule_.PreloadRows().empty()) {                       // StartPreload: the next chunk into the free buffer
+        DATA_CUDA_CHECK(cudaStreamWaitEvent(copy_stream_, consumed_[1 - cur_], 0));
+        CopyRows(schedule_.PreloadRows(), 1 - cur_, copy_stream_);
+        DATA_CUDA_CHECK(cudaEventRecord(loaded_[1 - cur_], copy_stream_));
+        staged_ = true;
+      }
+    }
+  }
+  if (last_.reshuffled) UploadPermutation();
+  SampleNoise(last_.multiplicity_id);
+  const int rc = cnb_extract_patches_indexed(d_images_[cur_], input.GetDevData(), d_perm_ + last_.start, d_noise_,
+                                             d_noise_ + batch_, d_noise_ + 2 * batch_, batch_, channels_, isx_, isy_, gx_, gy_,
+                                             labels_out ? d_labels_[cur_] : nullptr, labels_out,
+                                             targets_out ? d_targets_[cur_] : nullptr, targets_out, target_dims_);
+  if (rc != 0) { fprintf(stderr, "DataHandler::GetBatch: cnb_extract_patches_indexed returned %d\n", rc); exit(1); }
+}
+
+void DataHandler::GetBatch(ConvNet& net) {
+  Layer& out = net.OutputLayer();
+  Matrix& targets = out.GetTargets();
+  if (targets.GetNumEls() > 0) {
+    if (targets.GetCols() != target_dims_)
+      throw std::invalid_argument("DataHandler::GetBatch: the output layer takes " + std::to_string(targets.GetCols()) +
+                                  " targets per image and the data set has " + std::to_string(target_dims_));
+    GetBatch(net.InputLayer().GetState(), nullptr, targets.GetDevData());
+  } else {
+    GetBatch(net.InputLayer().GetState(), out.GetLabels(), nullptr);
+  }
 }
 
 }  // namespace cnbhost

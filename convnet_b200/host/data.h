@@ -11,6 +11,11 @@
 
 namespace cnbhost {
 
+class ConvNet;
+
+// splitmix64: the generator behind the jitter of DataIterator and DataHandler and the shuffles of DataSchedule
+uint64_t SplitMix64(uint64_t& state);
+
 class DataIterator {
  public:
   // images of image_size_y x image_size_x x channels, `chunk_size` of them on the GPU; the net sees gpu_image_size_* crops
@@ -42,6 +47,106 @@ class DataIterator {
   int pinned_cap_ = 0;
   uint64_t NextRand();
   float Uniform();                                // [0, 1)
+};
+
+// The fields of the reference's DatasetConfig (proto/convnet_config.proto:371-382) that decide the batch order, with the
+// proto's defaults.  max_dataset_size and the data streams' file fields are the caller's business.
+struct DatasetOrder {
+  int batch_size = 1, chunk_size = 0, max_reuse_count = 0;
+  int pipeline_loads = 0, randomize_cpu = 0, randomize_gpu = 0;
+  int random_access_chunk_size = 1, multiplicity = 1;
+};
+
+// The reference's DataHandler state machine (src/datahandler.cc:124-315) without the data: which data set rows each chunk
+// holds, which slice of the chunk each minibatch takes, its multiplicity_id, and the permutation it is read through.
+// Rule for rule: GetBatch's start_ / restart_ / reuse_counter_ / multiplicity_counter_, DiskAccess's random_indices_ when
+// randomize_cpu (blocks of random_access_chunk_size rows from random starts, wrapping at the end of the data set, the
+// index reshuffled when too few are left) and consecutive rows with wrap-around otherwise (LoadChunk), the preload that
+// pipeline_loads runs one chunk ahead (and that Seek discards), and a reshuffle of the GPU permutation on every pass.
+// Shuffles are seeded Fisher-Yates (j = SplitMix64 % (i + 1) for i = n-1 .. 1), on one generator for the CPU side and one
+// for the GPU side, so that pipelining does not change the order.  Configurations the reference cannot run correctly are
+// refused with std::invalid_argument: a batch larger than the chunk, and a random_access_chunk_size that does not divide
+// the chunk (the reference's LoadChunk writes past its chunk).
+class DataSchedule {
+ public:
+  DataSchedule(const DatasetOrder& c, int dataset_size, uint64_t seed);
+  struct Batch {
+    bool loaded = false;           // a new chunk became resident before this batch: `rows` holds its data set rows
+    bool reshuffled = false;       // the permutation was redrawn before this batch
+    int start = 0, multiplicity_id = 0;
+  };
+  Batch Next();                    // DataHandler::GetBatch, :146-200
+  void Seek(int row);              // DataHandler::Seek, :124-133
+  int ChunkSize() const { return chunk_size_; }
+  bool FitsOnGpu() const { return fits_on_gpu_; }
+  bool Pipelined() const { return c_.pipeline_loads != 0; }
+  const std::vector<int>& Rows() const { return rows_; }            // the resident chunk's data set rows
+  const std::vector<int>& Permutation() const { return perm_; }     // batch image n is chunk column perm[start + n]
+  // with pipeline_loads: the rows of the chunk being preloaded (empty when none is); a new preload begins after each load
+  const std::vector<int>& PreloadRows() const { return preload_; }
+
+ private:
+  DatasetOrder c_;
+  int dataset_size_, chunk_size_;
+  bool fits_on_gpu_ = false, nothing_on_gpu_ = true, restart_ = true, preloading_ = false;
+  int start_ = 0, reuse_counter_ = 0, multiplicity_counter_ = 0, row_ = 0;
+  size_t random_indices_ind_ = 0;
+  uint64_t cpu_rng_, gpu_rng_;
+  std::vector<int> random_indices_, perm_, rows_, preload_;
+  void Shuffle(std::vector<int>& v, uint64_t& rng);
+  std::vector<int> DiskAccess();   // :232-264: the rows of the next chunk
+};
+
+// The reference's DataHandler over a data set the caller holds in host memory (pinned or not): images image-major, each
+// (colour, row, column); optional labels (one int per image) and targets (target_dims floats per image).  The resident
+// chunk lives on the GPU with its labels and targets; each minibatch is one cnb_extract_patches_indexed launch that crops
+// through the schedule's permutation into the input layer and gathers the labels or targets the output layer takes.
+// Streams: chunk copies without pipeline_loads, the jitter and permutation uploads, and the crop run on the library
+// stream.  With pipeline_loads (and a data set larger than a chunk) the next chunk is copied into a second buffer on a
+// copy stream of its own; that copy waits for an event recorded after the last crop that read the buffer, and the crop
+// after the swap waits for the copy's event.  Jitter and permutations reach the device through rings of pinned blocks,
+// each reused only after the event recorded behind its last copy: no stream is synchronised per batch.
+class DataHandler {
+ public:
+  DataHandler(const DatasetOrder& c, int dataset_size, int channels, int image_size_y, int image_size_x,
+              int gpu_image_size_y, int gpu_image_size_x, bool translate, bool flip, const float* images, const int* labels,
+              const float* targets, int target_dims, uint64_t seed);
+  ~DataHandler();
+  // the next minibatch into `input` (batch x C*gy*gx, image fastest) and `labels_out` / `targets_out` (batch x
+  // target_dims, column-major) when not null
+  void GetBatch(Matrix& input, int* labels_out, float* targets_out);
+  void GetBatch(ConvNet& net);     // into the net's input layer and its labels or targets, whichever its output takes
+  void Seek(int row);
+  const DataSchedule& Schedule() const { return schedule_; }
+  const DataSchedule::Batch& LastBatch() const { return last_; }
+  const std::vector<float>& LastNoise() const { return h_noise_; }  // width offsets | height offsets | mirror bits
+
+ private:
+  static constexpr int kRing = 4;
+  DataSchedule schedule_;
+  int channels_, isy_, isx_, gy_, gx_, target_dims_, batch_;
+  bool translate_, flip_;
+  const float* images_;
+  const int* labels_;
+  const float* targets_;
+  uint64_t rng_;
+  int cur_ = 0;                                    // which of the chunk buffers is resident
+  float* d_images_[2] = {nullptr, nullptr};
+  int* d_labels_[2] = {nullptr, nullptr};
+  float* d_targets_[2] = {nullptr, nullptr};
+  int* d_perm_ = nullptr;
+  float* d_noise_ = nullptr;                       // 3 x batch
+  float* pinned_noise_ = nullptr;                  // kRing blocks of 3 x batch floats
+  int* pinned_perm_ = nullptr;                     // kRing blocks of chunk ints
+  cudaEvent_t noise_done_[kRing], perm_done_[kRing], loaded_[2], consumed_[2];
+  int noise_slot_ = 0, perm_slot_ = 0;
+  bool staged_ = false;                            // the schedule's preload has been issued into buffer 1 - cur_
+  cudaStream_t copy_stream_ = nullptr;            // with two chunk buffers only
+  DataSchedule::Batch last_;
+  std::vector<float> h_noise_;
+  void CopyRows(const std::vector<int>& rows, int buf, cudaStream_t s);
+  void UploadPermutation();
+  void SampleNoise(int multiplicity_id);
 };
 
 }  // namespace cnbhost

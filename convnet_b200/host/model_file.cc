@@ -558,6 +558,32 @@ class Mapper {
       const std::string why = FrozenError(chain_edges, k, &at);
       if (!why.empty()) Fail(*edges[out[chain[at]]]->msg->Get("block_backprop"), EdgeName(*edges[out[chain[k]]]->msg), why);
     }
+    // the data sets' batch order, and the crop of the data stream that feeds the input layer (DataHandler); not written
+    // back by model_text
+    for (auto [field, spec] : {std::pair{"train_dataset", &m.train_dataset}, std::pair{"valid_dataset", &m.valid_dataset}}) {
+      const Entry* d = model.Get(field);
+      if (!d) continue;
+      const Msg& ds = *d->msg;
+      DatasetOrder& o = spec->order;
+      spec->present = true;
+      o.batch_size = (int)ds.Int("batch_size", 1);
+      o.chunk_size = (int)ds.Int("chunk_size", 0);
+      o.max_reuse_count = (int)ds.Int("max_reuse_count", 0);
+      o.pipeline_loads = ds.Bool("pipeline_loads", false);
+      o.randomize_cpu = ds.Bool("randomize_cpu", false);
+      o.randomize_gpu = ds.Bool("randomize_gpu", false);
+      o.random_access_chunk_size = (int)ds.Int("random_access_chunk_size", 1);
+      o.multiplicity = (int)ds.Int("multiplicity", 1);
+      for (const Entry* s : ds.All("data_config")) {
+        const Msg& dc = *s->msg;
+        if (dc.Get("layer_name")->s != m.layer.front().name) continue;
+        spec->translate = dc.Bool("can_translate", false);
+        spec->flip = dc.Bool("can_flip", false);
+        spec->gpu_image_size_y = (int)dc.Int("gpu_image_size_y", 0);
+        spec->gpu_image_size_x = (int)dc.Int("gpu_image_size_x", 0);
+        break;
+      }
+    }
     return m;
   }
 

@@ -41,6 +41,28 @@ class OptimizerConfig(ct.Structure):
         return {f[0]: getattr(self, f[0]) for f in self._fields_}
 
 
+class DatasetOrder(ct.Structure):
+    """host/data.h DatasetOrder: the batch-order fields of the reference's DatasetConfig (proto/convnet_config.proto:371-382),
+    same names, same defaults."""
+    _fields_ = [("batch_size", ct.c_int), ("chunk_size", ct.c_int), ("max_reuse_count", ct.c_int),
+                ("pipeline_loads", ct.c_int), ("randomize_cpu", ct.c_int), ("randomize_gpu", ct.c_int),
+                ("random_access_chunk_size", ct.c_int), ("multiplicity", ct.c_int)]
+    DEFAULTS = {"batch_size": 1, "random_access_chunk_size": 1, "multiplicity": 1}
+
+    @classmethod
+    def from_dict(cls, d):
+        c = cls(**cls.DEFAULTS)
+        names = [f[0] for f in cls._fields_]
+        for k, v in d.items():
+            if k not in names:
+                raise KeyError("unsupported dataset field %r (known: %s)" % (k, ", ".join(names)))
+            setattr(c, k, int(v))
+        return c
+
+    def to_dict(self):
+        return {f[0]: getattr(self, f[0]) for f in self._fields_}
+
+
 HOST_LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "libconvnet_b200_host.so")
 _host = None
 
@@ -104,6 +126,15 @@ def load_host():
             "cnb_net_frozen_edges": ([vp, ct.POINTER(ll)], i),
             "cnb_model_frozen": ([ct.c_char_p, i, ct.c_char_p, ct.c_char_p], i),
             "cnb_model_flops": ([ct.c_char_p, i, ct.POINTER(d), ct.POINTER(d)], i),
+            "cnb_schedule_create": ([ct.POINTER(DatasetOrder), i, ct.c_ulonglong], vp), "cnb_schedule_destroy": ([vp], None),
+            "cnb_schedule_chunk_size": ([vp], i),
+            "cnb_schedule_next": ([vp, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i)], i),
+            "cnb_schedule_seek": ([vp, i], i),
+            "cnb_handler_create": ([ct.POINTER(DatasetOrder), i, i, i, i, i, i, i, i, vp, vp, vp, i, ct.c_ulonglong], vp),
+            "cnb_handler_destroy": ([vp], None), "cnb_handler_get_batch": ([vp, vp], i), "cnb_handler_seek": ([vp, i], i),
+            "cnb_handler_last": ([vp, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(f)], i),
+            "cnb_model_dataset": ([ct.c_char_p, i, ct.POINTER(DatasetOrder), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i),
+                                   ct.POINTER(i)], i),
         }
         for name, (args, res) in sig.items():
             fn = getattr(H, name)
@@ -674,6 +705,133 @@ def view_offset(multiplicity_id, max_offset_x, max_offset_y):
     w, h = ct.c_int(0), ct.c_int(0)
     H.cnb_data_view_offset(multiplicity_id, max_offset_x, max_offset_y, ct.byref(w), ct.byref(h))
     return w.value, h.value
+
+
+class DataHandler:
+    """The reference's DataHandler (src/datahandler.cc; host/data.h) over a data set already in host memory: float pixels
+    `images` [N, channels, rows, cols] (a CPU float32 tensor, pinned for copies that overlap the step), integer `labels`
+    [N] and / or float `targets` [N, features].  It keeps a chunk of chunk_size images on the GPU (the whole data set when
+    chunk_size is 0 or larger), and get_batch(net) writes the next minibatch into the net's input layer, randomly cropped
+    to gpu_image_size (when `translate`; else the centre / corner view of multiplicity_id) and mirrored (when `flip`; else
+    views 5..9), together with the labels or the targets the net's output layer trains on, in one kernel launch.
+
+    The order follows the reference's rules: a chunk is reused max_reuse_count times before the next one is loaded,
+    randomize_gpu reshuffles the chunk's order for every pass, randomize_cpu loads chunks of random_access_chunk_size-row
+    blocks from random places (else consecutive rows, wrapping around), every batch is served `multiplicity` times with
+    multiplicity_id 0, 1, ..., and pipeline_loads copies the next chunk while the net trains.  dataset_schedule() gives
+    the same order without a GPU.  The tensors must outlive the handler (it keeps references)."""
+
+    def __init__(self, images, labels=None, targets=None, *, batch_size, chunk_size=0, gpu_image_size=None, translate=False,
+                 flip=False, randomize_gpu=False, randomize_cpu=False, random_access_chunk_size=1, max_reuse_count=0,
+                 multiplicity=1, pipeline_loads=False, seed=1):
+        import torch
+        self.H = load_host()
+        self.h = None
+        assert images.dtype == torch.float32 and images.device.type == "cpu" and images.dim() == 4
+        n, c, isy, isx = images.shape
+        gy, gx = ((isy, isx) if gpu_image_size is None else
+                  (gpu_image_size, gpu_image_size) if isinstance(gpu_image_size, int) else gpu_image_size)
+        self._images = images.contiguous()
+        self._labels = None if labels is None else labels.to(torch.int32).contiguous()
+        self._targets = None if targets is None else targets.to(torch.float32).reshape(n, -1).contiguous()
+        for t in (self._labels, self._targets):
+            assert t is None or (t.device.type == "cpu" and t.shape[0] == n), "labels / targets: one row per image, on the host"
+        self.order = DatasetOrder.from_dict(dict(
+            batch_size=batch_size, chunk_size=chunk_size, max_reuse_count=max_reuse_count, pipeline_loads=pipeline_loads,
+            randomize_cpu=randomize_cpu, randomize_gpu=randomize_gpu, random_access_chunk_size=random_access_chunk_size,
+            multiplicity=multiplicity))
+        self.batch_size = batch_size
+        ptr = lambda t: None if t is None else t.data_ptr()
+        self.h = self.H.cnb_handler_create(
+            ct.byref(self.order), n, c, isy, isx, gy, gx, int(translate), int(flip), ptr(self._images), ptr(self._labels),
+            ptr(self._targets), 0 if self._targets is None else self._targets.shape[1], seed)
+        if not self.h:
+            raise ValueError(self.H.cnb_last_error().decode())
+
+    @classmethod
+    def from_model(cls, model, images, labels=None, which="train_dataset", *, targets=None, net=None, seed=1):
+        """a handler configured by a model file's train_dataset or valid_dataset: its batch order, and the crop
+        (gpu_image_size_y / _x), can_translate and can_flip of the data stream whose layer_name is the input layer.
+        ValueError when the model has no such block, or when its batch_size differs from `net`'s."""
+        cfg = model_dataset(model, which)
+        if cfg is None:
+            raise ValueError("model %r has no %s" % (model, which))
+        if net is not None and cfg["batch_size"] != net.batch_size:
+            raise ValueError("%s of %r has batch_size %d and the net %d" % (which, model, cfg["batch_size"], net.batch_size))
+        gy, gx = cfg.pop("gpu_image_size_y"), cfg.pop("gpu_image_size_x")
+        gy, gx = gy or images.shape[2], gx or images.shape[3]
+        return cls(images, labels, targets, gpu_image_size=(gy, gx), seed=seed, **cfg)
+
+    def close(self):
+        if self.h:
+            self.H.cnb_handler_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        self.close()
+
+    def get_batch(self, net):
+        """the next minibatch into net's input layer, and its labels or targets into labels_tensor() / targets_tensor()"""
+        if net.batch_size != self.batch_size:
+            raise ValueError("the net's batch size is %d and the handler's %d" % (net.batch_size, self.batch_size))
+        if self.H.cnb_handler_get_batch(self.h, net.h) != 0:
+            raise ValueError(self.H.cnb_last_error().decode())
+
+    def seek(self, row):
+        """restart the schedule at data set row `row` (DataHandler::Seek): the next batch loads a chunk from there"""
+        if self.H.cnb_handler_seek(self.h, row) != 0:
+            raise ValueError(self.H.cnb_last_error().decode())
+
+    def last_indices(self):
+        """{"start", "multiplicity_id", "rows": the data set row of each image of the last batch, "width_offset",
+        "height_offset", "flip": its jitter}"""
+        b = self.batch_size
+        start, mid, rows, noise = ct.c_int(0), ct.c_int(0), (ct.c_int * b)(), (ct.c_float * (3 * b))()
+        self.H.cnb_handler_last(self.h, ct.byref(start), ct.byref(mid), rows, noise)
+        v = list(noise)
+        return {"start": start.value, "multiplicity_id": mid.value, "rows": list(rows), "width_offset": v[:b],
+                "height_offset": v[b:2 * b], "flip": v[2 * b:]}
+
+
+def dataset_schedule(config, dataset_size, steps, seed=1, seeks=None):
+    """the order a DataHandler with batch-order fields `config` (a dict of DatasetConfig names) and seed `seed` serves a
+    data set of dataset_size images in (host logic only, no GPU): for each of `steps` minibatches a tuple (rows, start,
+    multiplicity_id, permutation): rows is the list of data set rows of the chunk loaded for that batch (None when the
+    resident chunk is kept), and batch image n is chunk column permutation[start + n].  seeks: {step: row} calls seek(row)
+    before that step.  ValueError for a configuration the handler refuses."""
+    H = load_host()
+    order = DatasetOrder.from_dict(config)
+    s = H.cnb_schedule_create(ct.byref(order), dataset_size, seed)
+    if not s:
+        raise ValueError(H.cnb_last_error().decode())
+    try:
+        chunk = H.cnb_schedule_chunk_size(s)
+        rows, perm, start, mid, out = (ct.c_int * chunk)(), (ct.c_int * chunk)(), ct.c_int(0), ct.c_int(0), []
+        for k in range(steps):
+            if seeks and k in seeks and H.cnb_schedule_seek(s, seeks[k]) != 0:
+                raise ValueError(H.cnb_last_error().decode())
+            loaded = H.cnb_schedule_next(s, ct.byref(start), ct.byref(mid), rows, perm)
+            out.append((list(rows) if loaded else None, start.value, mid.value, list(perm)))
+        return out
+    finally:
+        H.cnb_schedule_destroy(s)
+
+
+def model_dataset(model, which="train_dataset"):
+    """a model's train_dataset or valid_dataset block (host-only): None when it has none, else its batch-order fields
+    (DatasetOrder names) with translate, flip, gpu_image_size_y and gpu_image_size_x (0: not set) of the data stream that
+    feeds the input layer"""
+    o, v = DatasetOrder(), [ct.c_int(0) for _ in range(4)]
+    rc = load_host().cnb_model_dataset(model.encode(), {"train_dataset": 0, "valid_dataset": 1}[which], ct.byref(o),
+                                       *[ct.byref(x) for x in v])
+    if rc < 0:
+        raise ValueError("cannot build model %r (see stderr)" % model)
+    if rc == 0:
+        return None
+    d = {k: (bool(x) if k in ("pipeline_loads", "randomize_cpu", "randomize_gpu") else x) for k, x in o.to_dict().items()}
+    d.update(zip(("translate", "flip", "gpu_image_size_y", "gpu_image_size_x"), (bool(v[0].value), bool(v[1].value),
+                                                                                   v[2].value, v[3].value)))
+    return d
 
 
 Net.model_output_layer = staticmethod(model_output_layer)

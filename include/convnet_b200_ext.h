@@ -315,6 +315,20 @@ void cnb_polyak_average(float* out, const float* queue, long long n, long long s
 int convnet_b200_extract_patches(cudamat* images, cudamat* patches, cudamat* width_offset, cudamat* height_offset,
                                  cudamat* flip, int img_width, int img_height, int patch_width, int patch_height);
 
+/* The same crop through a permutation of the chunk, with the batch's labels and targets gathered in the same launch
+ * (DataHandler, host/data.h).  Batch image n reads chunk column index[n] (device ints, each < the chunk's image count):
+ *   patches[n + N*(x + pw*(y + ph*c))] = images[sx + W*(height_offset[n] + y + H*(c + C*index[n]))]
+ * with sx as above, so the pixels are bit-identical to convnet_b200_extract_patches on a chunk whose column n is column
+ * index[n] of this one.  The shuffle costs one index read per image instead of a rewrite of the chunk.
+ *   labels_dst[n] = labels_src[index[n]]                                  (one int per chunk image)
+ *   targets_dst[n + N*j] = targets_src[target_dims*index[n] + j]          (one row of target_dims floats per chunk image)
+ * labels_src / labels_dst and targets_src / targets_dst are both NULL or both set.  The crop must fit the image
+ * (pw <= W, ph <= H).  0 ok, -1 bad arguments, -3 launch error.  Runs on the library's stream. */
+int cnb_extract_patches_indexed(const float* images, float* patches, const int* index, const float* width_offset,
+                                const float* height_offset, const float* flip, int N, int C, int W, int H, int pw, int ph,
+                                const int* labels_src, int* labels_dst, const float* targets_src, float* targets_dst,
+                                int target_dims);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -70,7 +70,8 @@ struct TcParams {
   // (bank_bytes = Cin * x_yblocks * BN * 128), filled from the caller's filters `xw` ([c][ty][tx][o], o contiguous)
   const float* xw;
   uint32_t bank_bytes;              // 0: the B half of the ring follows the A ring
-  uint32_t epi_bytes;               // fprop / dgrad: the staging tile (BM x BN fp32) after the ring or bank; wgrad: 0
+  uint32_t epi_bytes;               // fprop / dgrad: the staging tile (BM x BN fp32) after the ring or bank; wgrad: the
+                                    // consumer warps' transpose areas (kWgradStageBytes), or 0 for the scalar stores
   uint32_t b_tx_bytes;              // bytes the B-operand TMA(s) of one stage actually deliver
   // merged requests: when N % 128 == 0 (2-D) the chunks of an m-tile are one box over a (chunk, ..., N/chunk, ...) view
   // of the tensor; when Cout % chunk == 0 the BN/chunk filter chunks are one box likewise.
@@ -302,6 +303,17 @@ __device__ __forceinline__ void xmode_fprop_mma(float (&acc)[16][4], const TcPar
 // then hits 32 distinct banks, and a store warp's ld.shared.v4 of one column reads 512 contiguous bytes.
 __device__ __forceinline__ uint32_t epi_off(int row, int col) {
   return (uint32_t)(col * (BM * 4) + ((((row >> 2) ^ col) & 7) << 4) + (((row >> 2) & ~7) << 4) + ((row & 3) << 2));
+}
+
+// ---- wgrad epilogue: each consumer warp writes its 16 rows x BN columns of dW, 32 columns at a time, through a 2 KiB
+// area of its own: column-major, 64 bytes per column, the 16-byte unit row / 4 XORed with (col / 2) & 3.  A lane then
+// reads 4 consecutive rows (output features o, dW's contiguous axis) of one column with one ld.shared.v4 and writes them
+// with one 16-byte store, where a store straight from the accumulators moves 4 bytes per lane.
+constexpr int kWgradPassCols = 32;
+constexpr uint32_t kWgradWarpBytes = 16 * kWgradPassCols * 4;
+constexpr uint32_t kWgradStageBytes = kConsumerWarps * kWgradWarpBytes;
+__device__ __forceinline__ uint32_t wgrad_stage_off(int row, int col) {
+  return (uint32_t)(col * 64 + ((((row >> 2) ^ (col >> 1)) & 3) << 4) + ((row & 3) << 2));
 }
 
 __device__ __forceinline__ float4 ld4(const float* a, bool vec) {
@@ -784,6 +796,53 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
       __syncwarp();
       if (lane == 0) ptx::mbar_arrive(&ctl->epi_full);
       epi_phase ^= 1;
+    } else if (p.epi_bytes) {
+      // wgrad, not x-mode, Cout % 4 == 0, dW 16-byte aligned: through this warp's transpose area (wgrad_stage_off).
+      // Lane l reads column l / 4 + 8 i of the pass, rows 4 (l & 3) .. + 3: all valid or all not.
+      const uint32_t stg = ptx::smem_u32(smemE) + (uint32_t)warp * kWgradWarpBytes;
+      const int r4 = 4 * (lane & 3);
+      const int o = tile.o_tile * BM + warp * 16 + r4;
+      const long long col_stride = (long long)p.Cout * p.taps;
+      float* const rp = p.out + (long long)tile.split * p.Cout * p.taps * p.Cin + o + (long long)p.Cout * tile.tap +
+                        col_stride * ((long long)tile.c_tile * p.BN);
+      const int ncols_valid = min(p.BN, p.Cin - tile.c_tile * p.BN);
+      const bool direct_scale = (p.splits == 1) || p.untied;
+      const float so_eff = direct_scale ? p.so : 1.f;
+      const bool rmw = direct_scale && p.st != 0.f;
+#pragma unroll
+      for (int pass = 0; pass < BN_MAX / kWgradPassCols; pass++) {
+        if (pass * kWgradPassCols >= p.BN) break;
+#pragma unroll
+        for (int jj = 0; jj < kWgradPassCols / 8; jj++)
+#pragma unroll
+          for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int e = 0; e < 2; e++)
+              ptx::sts32(stg + wgrad_stage_off(g + 8 * h, 8 * jj + 2 * tq + e), acc[pass * (kWgradPassCols / 8) + jj][2 * h + e]);
+        __syncwarp();
+#pragma unroll
+        for (int i = 0; i < kWgradPassCols / 8; i++) {
+          const int cl = (lane >> 2) + 8 * i, col = pass * kWgradPassCols + cl;
+          const float4 a = ptx::lds128(stg + wgrad_stage_off(r4, cl));
+          if (o >= p.Cout || col >= ncols_valid) continue;
+          float* const dst = rp + col_stride * col;
+          const float av[4] = {a.x, a.y, a.z, a.w};
+          float ov[4] = {0.f, 0.f, 0.f, 0.f};
+          if (rmw) {
+            const float4 old = *reinterpret_cast<const float4*>(dst);
+            ov[0] = old.x; ov[1] = old.y; ov[2] = old.z; ov[3] = old.w;
+          }
+          float v[4];
+#pragma unroll
+          for (int k = 0; k < 4; k++) {
+            float r = so_eff * av[k];
+            if (rmw) r += p.st * ov[k];
+            v[k] = r;
+          }
+          *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+        }
+        __syncwarp();                                // the next pass rewrites the area
+      }
     } else {
       // wgrad: dW[o, tap, c] straight from the registers
       float* rowp[2] = {nullptr, nullptr};
@@ -926,11 +985,15 @@ void launch_one(const CUtensorMap& a, const CUtensorMap& b, const TcParams& p, s
 
 template <int OP>
 void launch(const CUtensorMap& a, const CUtensorMap& b, TcParams& p) {
-  p.epi_bytes = OP == kWgrad ? 0u : epi_bytes_for(p.BN);
+  auto aligned = [](const void* q, uintptr_t a) { return (reinterpret_cast<uintptr_t>(q) & (a - 1)) == 0; };
+  // wgrad writes dW 16 bytes per lane through the consumer warps' transpose areas wherever 4 consecutive output
+  // features are one aligned float4 (not the x-mode scatter): its tiles carry few k-blocks, and 4-byte stores from the
+  // accumulators held fc6's 302 MB dW to 0.9 TB/s on an H100.  The areas cost the ring one of its seven stages.
+  if (OP == kWgrad) p.epi_bytes = (!p.x_mode && p.Cout % 4 == 0 && aligned(p.out, 16)) ? kWgradStageBytes : 0u;
+  else p.epi_bytes = epi_bytes_for(p.BN);
   p.stages = pick_stages(p.bank_bytes, p.epi_bytes);
   const size_t smem = smem_bytes_for(p.stages, p.bank_bytes, p.epi_bytes);
   // the store warps move 4 rows (16 bytes of out / mask, 8 of out16) per access where the pointers allow it
-  auto aligned = [](const void* q, uintptr_t a) { return (reinterpret_cast<uintptr_t>(q) & (a - 1)) == 0; };
   p.vec = aligned(p.out, 16) && aligned(p.mask, 16) && aligned(p.out16, 8) ? 1 : 0;
   const bool sig = p.act == kActLogistic || (p.mask && p.mask_act == kActLogistic);
   CNB_REQUIRE(OP != kWgrad || !sig, "tc_conv: wgrad has no activation epilogue");

@@ -63,82 +63,6 @@ void Layer::AllocateMemory(int batch_size) {               // layer.cc:228-262 (
   }
 }
 
-std::string EdgeShapeError(const Edge& e, int source_channels, int dest_channels) {
-  const int my = e.GetNumModulesY(), mx = e.GetNumModulesX(), mt = e.GetNumModulesT();
-  if (my < 1 || mx < 1 || mt < 1)
-    return "its kernel, stride and padding leave no output (" + std::to_string(my) + " x " + std::to_string(mx) + " x " +
-           std::to_string(mt) + " modules in y, x, t)";
-  const EdgeType t = e.Config().edge_type;
-  if ((t == MAXPOOL || t == AVGPOOL || t == RESPONSE_NORM) && source_channels != dest_channels)
-    return "pooling and response normalisation keep the channel count, but the source layer has " +
-           std::to_string(source_channels) + " channels and the destination " + std::to_string(dest_channels);
-  if ((t == CONVOLUTIONAL || t == LOCAL) && e.Config().padding_t != 0)
-    return "padding_t " + std::to_string(e.Config().padding_t) + " is not supported on a convolution (the 3-D kernels "
-           "fold the frames into channels)";
-  return "";
-}
-
-std::string SampleEdgeError(const Edge& e, int source_channels, int dest_channels, bool on_input, bool into_output) {
-  const EdgeType t = e.Config().edge_type;
-  if (t != UPSAMPLE && t != DOWNSAMPLE && t != RGBTOYUV) return "";
-  const std::string name = kEdgeTypeNames[t], f = std::to_string(e.Config().sample_factor);
-  if (t != RGBTOYUV && e.Config().sample_factor < 1) return "field 'sample_factor': " + f + " is below 1";
-  if (source_channels != dest_channels)
-    return "field 'edge_type': " + name + " keeps the channel count, but the source layer has " +
-           std::to_string(source_channels) + " channels and the destination " + std::to_string(dest_channels);
-  const int y = e.GetImageSizeY(), x = e.GetImageSizeX();
-  if (t == DOWNSAMPLE && (y % e.Config().sample_factor || x % e.Config().sample_factor))
-    return "field 'sample_factor': DOWNSAMPLE by " + f + " needs image sizes divisible by " + f + ", and the source layer is " +
-           std::to_string(y) + " x " + std::to_string(x);
-  if (t == RGBTOYUV) {
-    if (!on_input) return "field 'edge_type': RGBTOYUV runs only on the input layer's outgoing edge (it has no backward pass)";
-    if (source_channels != 3)
-      return "field 'edge_type': RGBTOYUV maps 3 colour channels to 3, and the layers have " + std::to_string(source_channels);
-    if (e.GetImageSizeT() != 1) return "field 'edge_type': RGBTOYUV is not supported on 3-D layers (image_size_t > 1)";
-    if (into_output)
-      return "field 'edge_type': RGBTOYUV cannot write the output layer (the layer it writes receives no derivative, and the "
-             "loss needs one)";
-  }
-  return "";
-}
-
-std::string TieError(const std::vector<const Edge*>& edges, size_t i) {
-  const EdgeConfig& c = edges[i]->Config();
-  if (c.tied_to.empty()) return "";
-  const std::string f = "field 'tied_to': ", owner = "edge '" + c.tied_to + "'";
-  size_t k = 0;
-  while (k < edges.size() && edges[k]->GetName() != c.tied_to) k++;
-  if (k == edges.size()) return f + "the net has no edge '" + c.tied_to + "'";
-  if (k == i) return f + "an edge cannot be tied to itself";
-  const EdgeConfig& o = edges[k]->Config();
-  if (!o.tied_to.empty()) return f + owner + " is itself tied (to '" + o.tied_to + "'): tie to '" + o.tied_to + "' instead";
-  if (edges[k]->HasNoParameters()) return f + owner + " has no parameters";
-  if (o.edge_type != c.edge_type)
-    return f + owner + " is " + kEdgeTypeNames[o.edge_type] + ", this edge " + kEdgeTypeNames[c.edge_type] +
-           " (a tie joins edges of one edge_type)";
-  const EdgeWithWeight *w = dynamic_cast<const EdgeWithWeight*>(edges[i]), *ow = dynamic_cast<const EdgeWithWeight*>(edges[k]);
-  auto shape = [](const Shape4D& s) {
-    return "(" + std::to_string(s.shape[0]) + ", " + std::to_string(s.shape[1]) + ", " + std::to_string(s.shape[2]) + ", " +
-           std::to_string(s.shape[3]) + ")";
-  };
-  const Shape4D a = w->GetWeightShape(), b = ow->GetWeightShape();
-  if (memcmp(&a, &b, sizeof(a)) != 0)
-    return f + "the weights of this edge have shape " + shape(a) + ", those of " + owner + " " + shape(b);
-  auto bias = [](const EdgeWithWeight* e) {
-    const EdgeConfig& x = e->Config();
-    if (x.has_no_bias) return std::string("none (has_no_bias)");
-    return std::to_string(e->GetNumOutputChannels()) + " x " + std::to_string(e->GetBiasCols()) +
-           (x.edge_type == CONVOLUTIONAL ? (x.shared_bias ? " (shared_bias)" : " (one per output position)") : "");
-  };
-  if (bias(w) != bias(ow)) return f + "the bias of this edge is " + bias(w) + ", that of " + owner + " " + bias(ow);
-  // every contribution to the shared bias gradient must come from one stream: a 3-D conv sums its bias on the main stream,
-  // a 2-D one on the side lane
-  if (c.edge_type == CONVOLUTIONAL && (edges[i]->GetImageSizeT() == 1) != (edges[k]->GetImageSizeT() == 1))
-    return f + "a tie joins a 3-D and a 2-D convolution";
-  if (c.grad_check) return f + "grad_check on a tied edge (set it on " + owner + ", which checks the shared tensors)";
-  return "";
-}
-
 int FrozenEdges(const std::vector<EdgeConfig>& edges) {
   int n = 0;
   for (size_t i = 0; i < edges.size(); i++)
@@ -146,33 +70,143 @@ int FrozenEdges(const std::vector<EdgeConfig>& edges) {
   return n;
 }
 
-std::string FrozenError(const std::vector<const Edge*>& edges, size_t i, size_t* at) {
+// ---- the checks of ConvNet::Refuse.  Each returns why it refuses (empty: it does not) and the fields it objects to, in
+// order of preference (ModelRefused::fields)
+namespace {
+struct Objection {
+  std::string why;
+  std::vector<std::string> fields;
+};
+
+// edge `e`, once SetImageSize has run, between layers of `source_channels` and `dest_channels`: it gives its destination at
+// least one module in y, x and t, a pooling or response-norm edge keeps the channel count, and a convolution has no
+// temporal padding (the 3-D kernels fold the frames into channels).  The edge as a whole
+Objection EdgeShapeError(const Edge& e, int source_channels, int dest_channels) {
+  const int my = e.GetNumModulesY(), mx = e.GetNumModulesX(), mt = e.GetNumModulesT();
+  if (my < 1 || mx < 1 || mt < 1)
+    return {"its kernel, stride and padding leave no output (" + std::to_string(my) + " x " + std::to_string(mx) + " x " +
+            std::to_string(mt) + " modules in y, x, t)"};
+  const EdgeType t = e.Config().edge_type;
+  if ((t == MAXPOOL || t == AVGPOOL || t == RESPONSE_NORM) && source_channels != dest_channels)
+    return {"pooling and response normalisation keep the channel count, but the source layer has " +
+            std::to_string(source_channels) + " channels and the destination " + std::to_string(dest_channels)};
+  if ((t == CONVOLUTIONAL || t == LOCAL) && e.Config().padding_t != 0)
+    return {"padding_t " + std::to_string(e.Config().padding_t) + " is not supported on a convolution (the 3-D kernels "
+            "fold the frames into channels)"};
+  return {};
+}
+
+// an UPSAMPLE, DOWNSAMPLE or RGBTOYUV edge `e` (SetImageSize has run) between layers of `source_channels` and
+// `dest_channels`, its source being the input layer when `on_input` and its destination the output layer when
+// `into_output`.  A factor is at least 1, the three keep the channel count, a DOWNSAMPLE's image size is divisible by its
+// factor, and RGBTOYUV maps the 3 channels of a 2-D input layer to a hidden layer (the layer it writes receives no
+// derivative, and an output layer needs one for its loss).  sample_factor or edge_type
+Objection SampleEdgeError(const Edge& e, int source_channels, int dest_channels, bool on_input, bool into_output) {
+  const EdgeType t = e.Config().edge_type;
+  if (t != UPSAMPLE && t != DOWNSAMPLE && t != RGBTOYUV) return {};
+  auto refuse = [](const std::string& field, const std::string& why) {
+    return Objection{"field '" + field + "': " + why, {field}};
+  };
+  const std::string name = kEdgeTypeNames[t], f = std::to_string(e.Config().sample_factor);
+  if (t != RGBTOYUV && e.Config().sample_factor < 1) return refuse("sample_factor", f + " is below 1");
+  if (source_channels != dest_channels)
+    return refuse("edge_type", name + " keeps the channel count, but the source layer has " + std::to_string(source_channels) +
+                  " channels and the destination " + std::to_string(dest_channels));
+  const int y = e.GetImageSizeY(), x = e.GetImageSizeX();
+  if (t == DOWNSAMPLE && (y % e.Config().sample_factor || x % e.Config().sample_factor))
+    return refuse("sample_factor", "DOWNSAMPLE by " + f + " needs image sizes divisible by " + f +
+                  ", and the source layer is " + std::to_string(y) + " x " + std::to_string(x));
+  if (t == RGBTOYUV) {
+    if (!on_input)
+      return refuse("edge_type", "RGBTOYUV runs only on the input layer's outgoing edge (it has no backward pass)");
+    if (source_channels != 3)
+      return refuse("edge_type",
+                    "RGBTOYUV maps 3 colour channels to 3, and the layers have " + std::to_string(source_channels));
+    if (e.GetImageSizeT() != 1) return refuse("edge_type", "RGBTOYUV is not supported on 3-D layers (image_size_t > 1)");
+    if (into_output)
+      return refuse("edge_type", "RGBTOYUV cannot write the output layer (the layer it writes receives no derivative, and the "
+                    "loss needs one)");
+  }
+  return {};
+}
+
+// edge `i` of a chain (every edge's SetImageSize has run), if tied, may run with and train the parameters of the edge its
+// tied_to names.  The owner must exist, be another edge, be untied itself, have parameters of the same edge_type and the
+// same weight and bias shapes, and sum its bias gradient on the same stream; a tied edge may not ask for grad_check (its
+// owner checks the shared tensors).  tied_to
+Objection TieError(const std::vector<const Edge*>& edges, size_t i) {
+  const EdgeConfig& c = edges[i]->Config();
+  if (c.tied_to.empty()) return {};
+  auto refuse = [](const std::string& why) { return Objection{"field 'tied_to': " + why, {"tied_to"}}; };
+  const std::string owner = "edge '" + c.tied_to + "'";
+  size_t k = 0;
+  while (k < edges.size() && edges[k]->GetName() != c.tied_to) k++;
+  if (k == edges.size()) return refuse("the net has no edge '" + c.tied_to + "'");
+  if (k == i) return refuse("an edge cannot be tied to itself");
+  const EdgeConfig& o = edges[k]->Config();
+  if (!o.tied_to.empty())
+    return refuse(owner + " is itself tied (to '" + o.tied_to + "'): tie to '" + o.tied_to + "' instead");
+  if (edges[k]->HasNoParameters()) return refuse(owner + " has no parameters");
+  if (o.edge_type != c.edge_type)
+    return refuse(owner + " is " + kEdgeTypeNames[o.edge_type] + ", this edge " + kEdgeTypeNames[c.edge_type] +
+                  " (a tie joins edges of one edge_type)");
+  const EdgeWithWeight *w = dynamic_cast<const EdgeWithWeight*>(edges[i]), *ow = dynamic_cast<const EdgeWithWeight*>(edges[k]);
+  auto shape = [](const Shape4D& s) {
+    return "(" + std::to_string(s.shape[0]) + ", " + std::to_string(s.shape[1]) + ", " + std::to_string(s.shape[2]) + ", " +
+           std::to_string(s.shape[3]) + ")";
+  };
+  const Shape4D a = w->GetWeightShape(), b = ow->GetWeightShape();
+  if (memcmp(&a, &b, sizeof(a)) != 0)
+    return refuse("the weights of this edge have shape " + shape(a) + ", those of " + owner + " " + shape(b));
+  auto bias = [](const EdgeWithWeight* e) {
+    const EdgeConfig& x = e->Config();
+    if (x.has_no_bias) return std::string("none (has_no_bias)");
+    return std::to_string(e->GetNumOutputChannels()) + " x " + std::to_string(e->GetBiasCols()) +
+           (x.edge_type == CONVOLUTIONAL ? (x.shared_bias ? " (shared_bias)" : " (one per output position)") : "");
+  };
+  if (bias(w) != bias(ow)) return refuse("the bias of this edge is " + bias(w) + ", that of " + owner + " " + bias(ow));
+  // every contribution to the shared bias gradient must come from one stream: a 3-D conv sums its bias on the main stream,
+  // a 2-D one on the side lane
+  if (c.edge_type == CONVOLUTIONAL && (edges[i]->GetImageSizeT() == 1) != (edges[k]->GetImageSizeT() == 1))
+    return refuse("a tie joins a 3-D and a 2-D convolution");
+  if (c.grad_check) return refuse("grad_check on a tied edge (set it on " + owner + ", which checks the shared tensors)");
+  return {};
+}
+
+// edge `i` of a chain (shapes known, ties accepted by TieError) may be frozen or trained as its block_backprop says.  A
+// weighted edge below a blocked one must be blocked itself, the edges of a tie group agree, and a frozen edge may not ask
+// for grad_check.  block_backprop of the blocked edge *at
+Objection FrozenError(const std::vector<const Edge*>& edges, size_t i, size_t* at) {
   const Edge& e = *edges[i];
-  const std::string f = "field 'block_backprop': ";
+  auto refuse = [](const std::string& why) { return Objection{"field 'block_backprop': " + why, {"block_backprop"}}; };
   for (size_t k = 0; k < edges.size() && !e.Config().tied_to.empty(); k++)
     if (edges[k]->GetName() == e.Config().tied_to && edges[k]->IsBackPropBlocked() != e.IsBackPropBlocked()) {
       const Edge& blocked = e.IsBackPropBlocked() ? e : *edges[k];
       const Edge& open = e.IsBackPropBlocked() ? *edges[k] : e;
       *at = e.IsBackPropBlocked() ? i : k;
-      return f + "edge '" + blocked.GetName() + "' is blocked and edge '" + open.GetName() + "' of its tie group is not (a "
-             "tie group is frozen or trained as a whole)";
+      return refuse("edge '" + blocked.GetName() + "' is blocked and edge '" + open.GetName() + "' of its tie group is not (a "
+                    "tie group is frozen or trained as a whole)");
     }
   size_t above = i;                                  // the nearest blocked edge at or above this one
   while (above < edges.size() && !edges[above]->IsBackPropBlocked()) above++;
-  if (above == edges.size() || e.HasNoParameters()) return "";
+  if (above == edges.size() || e.HasNoParameters()) return {};
   *at = above;
   if (above != i)
-    return f + "this edge has weights and lies below the blocked edge '" + edges[above]->GetName() + "', so no derivative "
-           "reaches it and nothing would train it: set block_backprop on it too";
-  if (e.Config().grad_check) return f + "grad_check on a frozen edge (its parameters get no gradient)";
-  return "";
+    return refuse("this edge has weights and lies below the blocked edge '" + edges[above]->GetName() + "', so no derivative "
+                  "reaches it and nothing would train it: set block_backprop on it too");
+  if (e.Config().grad_check) return refuse("grad_check on a frozen edge (its parameters get no gradient)");
+  return {};
 }
 
-std::string LayerConfigError(const LayerConfig& c) {
+// the activation, loss function and performance metric of `c` can run.  The loss function or performance metric that
+// fails, else the activation
+Objection LayerConfigError(const LayerConfig& c) {
   const bool softmax = c.activation == SOFTMAX || c.activation == SOFTMAX_DIST;
   if (!c.is_output) {
-    if (softmax) return "SOFTMAX / SOFTMAX_DIST is an output activation (back-propagation through a softmax is not implemented)";
-    return "";
+    if (softmax)
+      return {"SOFTMAX / SOFTMAX_DIST is an output activation (back-propagation through a softmax is not implemented)",
+              {"activation"}};
+    return {};
   }
   auto name = [](int f) -> std::string {
     static const char* n[] = {"SQUARED_ERROR", "LINEAR_ERROR", "CROSS_ENTROPY_MULTINOMIAL", "CROSS_ENTROPY_BINARY",
@@ -183,16 +217,18 @@ std::string LayerConfigError(const LayerConfig& c) {
   const std::string target = TakesLabels(c.activation) ? "integer labels" : "a float target per feature";
   for (int which = 0; which < 2; which++) {
     const int f = which ? c.performance_metric : c.loss_function;
-    const std::string field = which ? "performance_metric " : "loss_function ";
-    if (f < SQUARED_ERROR || f > CLASSIFICATION_BINARY) return field + name(f) + " is not supported";
+    const std::string field = which ? "performance_metric" : "loss_function";
+    auto refuse = [&](const std::string& why) { return Objection{field + " " + name(f) + why, {field, "activation"}}; };
+    if (f < SQUARED_ERROR || f > CLASSIFICATION_BINARY) return refuse(" is not supported");
     if (!which && (f == CLASSIFICATION_MULTINOMIAL || f == CLASSIFICATION_BINARY))
-      return field + name(f) + " has no derivative to train with";
+      return refuse(" has no derivative to train with");
     if (ReadsLabels(f) != TakesLabels(c.activation))
-      return field + name(f) + " reads " + (ReadsLabels(f) ? "integer labels" : "a float target per feature") +
-             ", but this output layer's activation has " + target;
+      return refuse(std::string(" reads ") + (ReadsLabels(f) ? "integer labels" : "a float target per feature") +
+                    ", but this output layer's activation has " + target);
   }
-  return "";
+  return {};
 }
+}  // namespace
 
 // `emit`: this call is the last writer of the tensor and the next conv edge reads it as bf16 (see LastStateWriter)
 void Layer::ApplyActivation(bool emit) {
@@ -409,8 +445,7 @@ ConvNet::ConvNet(const ModelConfig& model, int batch_size) : model_(model), batc
     edges_[i]->SetImageSize(layers_[i]->GetSizeY(), layers_[i]->GetSizeX(), layers_[i]->GetSizeT());
     layers_[i + 1]->SetSize(edges_[i]->GetNumModulesY(), edges_[i]->GetNumModulesX(), edges_[i]->GetNumModulesT());
   }
-  const std::string why = Refusal();
-  if (!why.empty()) throw std::invalid_argument(why);
+  Refuse();
   frozen_ = FrozenEdges(model.edge);
   for (size_t i = 0; i < edges_.size(); i++)
     if (model.edge[i].edge_type == RGBTOYUV || ((int)i < frozen_ && !layers_[i + 1]->IsOutput())) layers_[i + 1]->SetNoDeriv();
@@ -441,48 +476,48 @@ bool ConvNet::Grouped(size_t i) const {
   return owner_[i] >= 0 && std::count(owner_.begin(), owner_.end(), owner_[i]) > 1;
 }
 
-std::string ConvNet::Refusal() const {
-  for (const LayerConfig& lc : model_.layer) {       // activations, loss functions and metrics this class cannot run
-    const std::string why = LayerConfigError(lc);
-    if (!why.empty()) return "layer '" + lc.name + "': " + why;
-  }
+void ConvNet::Refuse() const {
+  // `o`, if it objects, as the refusal of layer or edge `at`, its message after `where`
+  auto check = [](const std::string& where, bool edge, size_t at, const Objection& o) {
+    if (!o.why.empty()) throw ModelRefused(where + ": " + o.why, edge, at, o.fields);
+  };
+  for (size_t i = 0; i < layers_.size(); i++)        // activations, loss functions and metrics this class cannot run
+    check("layer '" + layers_[i]->GetName() + "'", false, i, LayerConfigError(model_.layer[i]));
   std::vector<const Edge*> chain;
   for (const auto& e : edges_) chain.push_back(e.get());
   for (size_t i = 0; i < edges_.size(); i++) {
-    const std::string sample =
-        SampleEdgeError(*edges_[i], layers_[i]->GetNumChannels(), layers_[i + 1]->GetNumChannels(), layers_[i]->IsInput(),
-                        layers_[i + 1]->IsOutput());
-    if (!sample.empty()) return "edge '" + edges_[i]->GetName() + "': " + sample;
-    const std::string shape = EdgeShapeError(*edges_[i], layers_[i]->GetNumChannels(), layers_[i + 1]->GetNumChannels());
-    if (!shape.empty()) return "edge '" + edges_[i]->GetName() + "': " + shape;
-    const std::string tie = TieError(chain, i);
-    if (!tie.empty()) return "edge '" + edges_[i]->GetName() + "': " + tie;
-    size_t at;
-    const std::string frozen = FrozenError(chain, i, &at);
-    if (!frozen.empty()) return "edge '" + edges_[i]->GetName() + "': " + frozen;
+    const std::string where = "edge '" + edges_[i]->GetName() + "'";
+    const int from = layers_[i]->GetNumChannels(), to = layers_[i + 1]->GetNumChannels();
+    check(where, true, i, SampleEdgeError(*edges_[i], from, to, layers_[i]->IsInput(), layers_[i + 1]->IsOutput()));
+    check(where, true, i, EdgeShapeError(*edges_[i], from, to));
+    check(where, true, i, TieError(chain, i));
+    size_t at = i;
+    const Objection frozen = FrozenError(chain, i, &at);
+    check(where, true, at, frozen);
     if (model_.edge[i].edge_type == LOCAL && layers_[i]->GetSizeT() != 1)     // the untied conv kernels are 2-D only
-      return "edge '" + edges_[i]->GetName() + "': LOCAL is not supported on 3-D layers (image_size_t > 1)";
+      check(where, true, i, {"LOCAL is not supported on 3-D layers (image_size_t > 1)", {"edge_type"}});
     const int init = model_.edge[i].initialization;
     if (!model_.edge[i].tied_to.empty()) continue;                          // (its initialisation is never used)
     if (!edges_[i]->HasNoParameters() && init != DENSE_GAUSSIAN && init != DENSE_GAUSSIAN_SQRT_FAN_IN &&
         init != DENSE_UNIFORM && init != DENSE_UNIFORM_SQRT_FAN_IN && init != CONSTANT && init != PRETRAINED)
-      return "edge '" + edges_[i]->GetName() + "': initialization " + std::to_string(init) + " is not implemented";
-    if (!edges_[i]->HasNoParameters() && init == PRETRAINED && model_.edge[i].pretrained_model.empty())
-      return "edge '" + edges_[i]->GetName() + "': initialization PRETRAINED without pretrained_model";
+      check(where, true, i, {"initialization " + std::to_string(init) + " is not implemented", {"initialization"}});
   }
   for (size_t i = 0; i < layers_.size(); i++) {      // what the batch-norm passes cannot run
     const Layer* l = layers_[i].get();
     if (!l->BatchNormalize()) continue;
+    const std::string where = "layer '" + l->GetName() + "'";
     std::string why;
-    if (l->IsInput() || l->IsOutput()) why = "is not supported on the input or output layer";
-    else if (model_.edge[i - 1].edge_type == RGBTOYUV) why = "is not supported on the layer RGBTOYUV writes (it receives no derivative)";
-    else if (l->GetSizeT() > 1) why = "is not supported on 3-D layers (image_size_t > 1)";
-    for (int which = 0; which < 2 && why.empty(); which++)
-      if (const char* err = BnOptimizerConfigError(which ? model_.layer[i].beta_optimizer : model_.layer[i].gamma_optimizer))
-        why = std::string(which ? "beta" : "gamma") + "_optimizer: " + err;
-    if (!why.empty()) return "layer '" + l->GetName() + "': batch_normalize " + why;
+    if (l->IsInput() || l->IsOutput()) why = "batch_normalize is not supported on the input or output layer";
+    else if (model_.edge[i - 1].edge_type == RGBTOYUV)
+      why = "field 'batch_normalize': not supported on the layer RGBTOYUV writes (it receives no derivative)";
+    else if (l->GetSizeT() > 1) why = "batch_normalize is not supported on 3-D layers (image_size_t > 1)";
+    check(where, false, i, {why, {"batch_normalize"}});
+    const LayerConfig& c = model_.layer[i];
+    for (const auto& [f, o] :
+         {std::pair{"gamma_optimizer", &c.gamma_optimizer}, std::pair{"beta_optimizer", &c.beta_optimizer}})
+      if (const char* err = BnOptimizerConfigError(*o))
+        check(where, false, i, {std::string("batch_normalize ") + f + ": " + err, {f, "batch_normalize"}});
   }
-  return "";
 }
 
 // Epilogue fusion of the layers' activation (ReLU, logistic), its derivative and the dropout into the neighbouring

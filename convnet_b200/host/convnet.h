@@ -10,7 +10,9 @@
 #pragma once
 #include <map>
 #include <memory>
+#include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "data.h"
@@ -52,34 +54,22 @@ struct LayerConfig {
 
 // nullptr if `c` can train gamma or beta, else why not: OptimizerConfigError, or a norm rule (refused, DESIGN.md §5)
 const char* BnOptimizerConfigError(const OptimizerConfig& c);
-// "" if the activation, loss function and performance metric of `c` can run, else why not
-std::string LayerConfigError(const LayerConfig& c);
-// "" if edge `e`, once SetImageSize has run, can run between layers of `source_channels` and `dest_channels`: it gives
-// its destination at least one module in y, x and t, a pooling or response-norm edge keeps the channel count, and a
-// convolution has no temporal padding (the 3-D kernels fold the frames into channels); else why not
-std::string EdgeShapeError(const Edge& e, int source_channels, int dest_channels);
-// "" if `e` is not an UPSAMPLE, DOWNSAMPLE or RGBTOYUV edge, or (SetImageSize has run) can run between layers of
-// `source_channels` and `dest_channels`, its source being the input layer when `on_input` and its destination the output
-// layer when `into_output`; else why not, starting with the field it objects to ("field 'sample_factor': " or
-// "field 'edge_type': ").  A factor is at least 1, the three keep the channel count, a DOWNSAMPLE's image size is divisible
-// by its factor, and RGBTOYUV maps the 3 channels of a 2-D input layer to a hidden layer (the layer it writes receives no
-// derivative, and an output layer needs one for its loss)
-std::string SampleEdgeError(const Edge& e, int source_channels, int dest_channels, bool on_input, bool into_output);
-// "" if edge `i` of a chain (every edge's SetImageSize has run) is untied, or may run with and train the parameters of the
-// edge its tied_to names; else why not, starting with "field 'tied_to': ".  The owner must exist, be another edge, be
-// untied itself, have parameters of the same edge_type and the same weight and bias shapes, and sum its bias gradient on
-// the same stream; a tied edge may not ask for grad_check (its owner checks the shared tensors)
-std::string TieError(const std::vector<const Edge*>& edges, size_t i);
 // Fine-tuning (EdgeConfig::block_backprop): an edge is frozen if it is blocked or lies below a blocked edge, so the frozen
 // edges of a chain are [0, FrozenEdges).  They run their forward pass only: no weight gradient, no derivative into their
 // source, no optimizer step.  The hidden layers they write receive no derivative (the output layer keeps the one its
 // loss writes)
 int FrozenEdges(const std::vector<EdgeConfig>& edges);
-// "" if edge `i` of a chain (shapes known, ties accepted by TieError) may be frozen or trained as its block_backprop says,
-// else why not, starting with "field 'block_backprop': ", and in *at the blocked edge whose field the message is about.
-// A weighted edge below a blocked one must be blocked itself, the edges of a tie group agree, and a frozen edge may not
-// ask for grad_check
-std::string FrozenError(const std::vector<const Edge*>& edges, size_t i, size_t* at);
+
+// What ConvNet's constructor throws for a model it cannot run.  what() names the layer or edge and says why; `edge` and
+// `index` say which layer or edge of the chain holds what it objects to, and `fields` which of its fields, in order of
+// preference (none: the layer or edge as a whole).  The model-file reader reports the refusal at that field's line
+struct ModelRefused : std::invalid_argument {
+  ModelRefused(const std::string& what, bool edge, size_t index, std::vector<std::string> fields)
+      : std::invalid_argument(what), edge(edge), index(index), fields(std::move(fields)) {}
+  bool edge;
+  size_t index;
+  std::vector<std::string> fields;
+};
 
 struct ModelConfig {
   std::string name;
@@ -263,7 +253,7 @@ std::vector<Bucket> PlanBuckets(const std::vector<size_t>& edge_offset, const st
 
 class ConvNet {
  public:
-  ConvNet(const ModelConfig& model, int batch_size);            // std::invalid_argument: a model this class cannot run
+  ConvNet(const ModelConfig& model, int batch_size);            // ModelRefused: a model this class cannot run
   virtual ~ConvNet();
   // the layout of the flat parameter buffer (host only): each edge's slice padded to 128 floats, followed by the
   // [gamma | beta] slice, also padded, of the layer the edge writes when that layer is batch-normalised; and the table of
@@ -346,11 +336,11 @@ class ConvNet {
   int batch_size_;
   std::vector<std::unique_ptr<Layer>> layers_;
   std::vector<std::unique_ptr<Edge>> edges_;    // edges_[i]: layers_[i] -> layers_[i+1]
-  std::string Refusal() const;                  // "" if this class can run the model, else why not
+  void Refuse() const;                          // throws ModelRefused if this class cannot run the model
   // which passes of the neighbouring layers ride in each edge's kernels (Edge::FusionPlan), once the shapes are known;
   // also tells each layer whether its activation / derivative pass is left to do (Layer::SetActivationFused / SetDerivFused)
   void PlanFusion();
-  // tie groups (EdgeConfig::tied_to), resolved once Refusal has accepted them: per edge, owner_ is the edge whose parameters
+  // tie groups (EdgeConfig::tied_to), resolved once Refuse has accepted them: per edge, owner_ is the edge whose parameters
   // it runs with (itself when untied, -1 without parameters) and home_ the group's lowest edge, where the parameters sit in
   // the flat buffer.  Back-propagation reaches that edge last, so its bucket becomes final after every contribution to
   // the shared gradients and every read of the shared weights

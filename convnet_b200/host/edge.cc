@@ -256,7 +256,7 @@ std::vector<float> EdgeWithWeight::InitialWeights(unsigned seed) const {
     std::normal_distribution<float> g(0.f, 1.f);
     const float scale = init == DENSE_GAUSSIAN ? init_wt : init_wt / std::sqrt((float)WeightCols());
     for (size_t i = 0; i < n; i++) h[i] = g(gen) * scale;
-  } else {                                                   // CONSTANT (ConvNet::Refusal admits no other rule)
+  } else {                                                   // CONSTANT (ConvNet::Refuse admits no other rule)
     for (size_t i = 0; i < n; i++) h[i] = init_wt;
   }
   return h;

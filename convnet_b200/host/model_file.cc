@@ -514,50 +514,7 @@ class Mapper {
 
     for (size_t k = 0; k < chain.size(); k++)
       m.layer.push_back(MapLayer(*layers[chain[k]], k == 0, k + 1 == chain.size()));
-    // the image sizes along the chain, as ConvNet propagates them: each edge type's own SetImageSize, so that an edge
-    // ConvNet::Refusal would refuse (EdgeShapeError) is refused here with its line
-    int y = m.layer[0].image_size_y, x = m.layer[0].image_size_x, t = m.layer[0].image_size_t;
-    std::vector<std::unique_ptr<Edge>> built;
-    for (size_t k = 0; k + 1 < chain.size(); k++) {
-      const Entry& at = *edges[out[chain[k]]];
-      m.edge.push_back(MapEdge(at, m.layer[k]));
-      built.emplace_back(Edge::ChooseEdgeClass(m.edge[k]));
-      Edge* e = built.back().get();
-      e->SetInputChannels(m.layer[k].num_channels);
-      e->SetOutputChannels(m.layer[k + 1].num_channels);
-      e->SetImageSize(y, x, t);
-      // at the line of the field the message names (sample_factor, else edge_type)
-      const std::string sample = SampleEdgeError(*e, m.layer[k].num_channels, m.layer[k + 1].num_channels, k == 0,
-                                                 k + 2 == chain.size());
-      if (!sample.empty()) {
-        const Msg& em = *at.msg;
-        const char* field = sample.rfind("field 'sample_factor'", 0) == 0 ? "sample_factor" : "edge_type";
-        Fail(em.Has(field) ? *em.Get(field) : at, EdgeName(em), sample);
-      }
-      const std::string why = EdgeShapeError(*e, m.layer[k].num_channels, m.layer[k + 1].num_channels);
-      if (!why.empty()) Fail(at, EdgeName(*at.msg), why);
-      if (check_pretrained_ && m.edge[k].initialization == PRETRAINED && !e->HasNoParameters() && m.edge[k].tied_to.empty())
-        CheckPretrained(*at.msg, *dynamic_cast<EdgeWithWeight*>(e), m.edge[k]);
-      y = e->GetNumModulesY(); x = e->GetNumModulesX(); t = e->GetNumModulesT();
-      const Msg& dest = *layers[chain[k + 1]]->msg;
-      if (m.edge[k].edge_type == RGBTOYUV && m.layer[k + 1].batch_normalize)
-        Fail(*dest.Get("batch_normalize"), "layer '" + m.layer[k + 1].name + "'",
-             "field 'batch_normalize': not supported on the layer RGBTOYUV writes (it receives no derivative)");
-    }
-    // ties, once every edge knows its shapes (ConvNet::Refusal runs the same checks), at the line of tied_to
-    std::vector<const Edge*> chain_edges;
-    for (const auto& e : built) chain_edges.push_back(e.get());
-    for (size_t k = 0; k < built.size(); k++) {
-      const std::string why = TieError(chain_edges, k);
-      const Msg& e = *edges[out[chain[k]]]->msg;
-      if (!why.empty()) Fail(*e.Get("tied_to"), EdgeName(e), why);
-    }
-    // block_backprop (ConvNet::Refusal runs the same checks), at the line of the blocked edge's field
-    for (size_t k = 0; k < built.size(); k++) {
-      size_t at = k;
-      const std::string why = FrozenError(chain_edges, k, &at);
-      if (!why.empty()) Fail(*edges[out[chain[at]]]->msg->Get("block_backprop"), EdgeName(*edges[out[chain[k]]]->msg), why);
-    }
+    for (size_t k = 0; k + 1 < chain.size(); k++) m.edge.push_back(MapEdge(*edges[out[chain[k]]], m.layer[k]));
     // the data sets' batch order, and the crop of the data stream that feeds the input layer (DataHandler); not written
     // back by model_text
     for (auto [field, spec] : {std::pair{"train_dataset", &m.train_dataset}, std::pair{"valid_dataset", &m.valid_dataset}}) {
@@ -583,6 +540,23 @@ class Mapper {
         spec->gpu_image_size_x = (int)dc.Int("gpu_image_size_x", 0);
         break;
       }
+    }
+    // what needs the whole chain: ConvNet's checks, at the line of the first field the refusal names that the layer or edge
+    // block sets (else of the block), then the checkpoints of the PRETRAINED edges
+    std::unique_ptr<ConvNet> net;
+    try {
+      net = std::make_unique<ConvNet>(m, 1);               // host only: no device memory
+    } catch (const ModelRefused& r) {
+      const Entry& block = r.edge ? *edges[out[chain[r.index]]] : *layers[chain[r.index]];
+      const Entry* at = &block;
+      for (const std::string& f : r.fields)
+        if (const Entry* e = block.msg->Get(f)) { at = e; break; }
+      Fail(*at, "", r.what());
+    }
+    for (size_t k = 0; check_pretrained_ && k < m.edge.size(); k++) {
+      const Edge& e = *net->Edges()[k];
+      if (m.edge[k].initialization == PRETRAINED && !e.HasNoParameters() && m.edge[k].tied_to.empty())
+        CheckPretrained(*edges[out[chain[k]]]->msg, dynamic_cast<const EdgeWithWeight&>(e), m.edge[k]);
     }
     return m;
   }
@@ -818,19 +792,6 @@ class Mapper {
       for (const char* f : {"gamma_optimizer", "beta_optimizer"}) if (const Entry* e = l.Get(f)) CheckOptimizer(*e, where);
       c.gamma_optimizer = Merge(def_w_, l.Get("gamma_optimizer"), where);
       c.beta_optimizer = Merge(def_b_, l.Get("beta_optimizer"), where);
-      for (int which = 0; which < 2; which++)
-        if (const char* err = BnOptimizerConfigError(which ? c.beta_optimizer : c.gamma_optimizer)) {
-          const Entry* e = l.Get(which ? "beta_optimizer" : "gamma_optimizer");
-          Fail(e ? *e : *l.Get("batch_normalize"), where,
-               std::string("batch_normalize ") + (which ? "beta" : "gamma") + "_optimizer: " + err);
-        }
-    }
-    const std::string why = LayerConfigError(c);           // its message starts with the field it objects to
-    if (!why.empty()) {
-      const Entry* e = l.Get("activation");
-      for (const char* f : {"performance_metric", "loss_function"})
-        if (why.rfind(f, 0) == 0 && l.Has(f)) e = l.Get(f);
-      Fail(e ? *e : at, where, why);
     }
     return c;
   }
@@ -846,10 +807,10 @@ class Mapper {
     const int t = HostValue(kEdgeTypeNames, type);
     if (t < 0) Fail(*e.Get("edge_type"), where, "field 'edge_type': " + type + " is not supported");
     c.edge_type = (EdgeType)t;
-    if (const Entry* tie = e.Get("tied_to")) c.tied_to = tie->s;      // checked with the whole chain (TieError)
+    if (const Entry* tie = e.Get("tied_to")) c.tied_to = tie->s;
     RefuseMessage(e, "source_slice", "layer slices are not supported", where);
     RefuseMessage(e, "dest_slice", "layer slices are not supported", where);
-    c.block_backprop = e.Bool("block_backprop", false);     // checked with the whole chain (FrozenError)
+    c.block_backprop = e.Bool("block_backprop", false);
     if (e.Int("gpu_id", 0) != 0) Fail(*e.Get("gpu_id"), where, "field 'gpu_id': one GPU per model (data parallelism replicates it)");
 
     // geometry: the *_y / *_x fields fall back to kernel_size / stride / padding only when absent (src/edge.cc:87-106)
@@ -871,7 +832,7 @@ class Mapper {
         if (v <= 0)
           Fail(e.Has(f) ? *e.Get(f) : e.Has("stride") ? *e.Get("stride") : at, where,
                std::string("field '") + f + "' must be positive");
-      // a pooling window <= 0 is "global" (MaxPoolEdge::SetImageSize); a conv or local kernel needs a size
+      // a pooling window <= 0 is "global" (MaxPoolEdge pools the whole image); a conv or local kernel needs a size
       if (c.edge_type == CONVOLUTIONAL || c.edge_type == LOCAL)
         for (const auto& [f, v] : {std::make_pair("kernel_size_y", c.kernel_size_y),
                                    std::make_pair("kernel_size_x", c.kernel_size_x),
@@ -890,8 +851,6 @@ class Mapper {
     c.has_no_bias = e.Bool("has_no_bias", false);
     c.scale_gradients = e.Float("scale_gradients", 1.f);
     c.sample_factor = (int)e.Int("sample_factor", 1);
-    if (IsSampling(c.edge_type) && c.sample_factor < 1)
-      Fail(*e.Get("sample_factor"), where, "field 'sample_factor': " + std::to_string(c.sample_factor) + " is below 1");
     c.response_norm_in_blocks = e.Bool("response_norm_in_blocks", false);
     c.add_scale = e.Float("add_scale", 0.f);
     c.pow_scale = e.Float("pow_scale", 0.f);

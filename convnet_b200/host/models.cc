@@ -249,34 +249,6 @@ ModelConfig BuildTiedCheckNet() {
   return m;
 }
 
-// NOT a model: a deliberately invalid config (a 3-D clip net with a LOCAL edge) that the tests of the host's refusals
-// build by the name "invalid:local3d" — ConvNet refuses it, the untied kernels being 2-D
-ModelConfig BuildLocal3DNet() {
-  ModelConfig m; m.name = "invalid:local3d";
-  LayerConfig in = L("input", 3); in.is_input = true; in.image_size_y = in.image_size_x = 16; in.image_size_t = 4;
-  m.layer = {in, L("conv1", 16, RECTIFIED_LINEAR), L("local2", 16, RECTIFIED_LINEAR), L("output", 10, SOFTMAX)};
-  m.layer.back().is_output = true;
-  m.edge = {Conv(3, 2, 1), E(LOCAL, 3, 1, 1), E(FC)};
-  finish(m);
-  return m;
-}
-
-// NOT models: deliberately invalid output configs on the tiny net ("invalid:<what>") that the tests of ConvNet's refusals
-// build (LayerConfigError); false for an unknown <what>
-static bool BuildInvalidOutputNet(const std::string& what, ModelConfig* m) {
-  *m = BuildTinyNet();
-  LayerConfig& out = m->layer.back();
-  if (what == "hidden-softmax") m->layer[4].activation = SOFTMAX;                           // nin1
-  else if (what == "hinge-loss") out.loss_function = HINGE_LINEAR;
-  else if (what == "hinge-metric") out.performance_metric = HINGE_QUADRATIC;
-  else if (what == "loss-target") out.loss_function = SQUARED_ERROR;                        // labels output, per-feature loss
-  else if (what == "metric-target") { out.activation = LOGISTIC; out.loss_function = CROSS_ENTROPY_BINARY; }  // default metric
-  else if (what == "classification-loss") { out.activation = LOGISTIC; out.loss_function = CLASSIFICATION_BINARY; }
-  else return false;
-  m->name = "invalid:" + what;
-  return true;
-}
-
 // "<model>+ref-optimizer": the optimizer blocks of the model's pbtxt exactly (BuildAlexNet / BuildLeNet keep the constant
 // momentum and leave out the norm rules and the FC l2_decay)
 static void UseReferenceOptimizers(const std::string& base, ModelConfig& m) {
@@ -439,9 +411,6 @@ ModelConfig BuildModel(const std::string& name) {
   if (name == "localcheck") return BuildLocalCheckNet();
   if (name == "updown") return BuildUpDownNet();
   if (name == "updowncheck") return BuildUpDownCheckNet();
-  if (name == "invalid:local3d") return BuildLocal3DNet();     // test-only, refused by ConvNet (see above)
-  ModelConfig invalid;
-  if (name.rfind("invalid:", 0) == 0 && BuildInvalidOutputNet(name.substr(8), &invalid)) return invalid;
   throw std::invalid_argument("unknown model '" + name + "'");
 }
 

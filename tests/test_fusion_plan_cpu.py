@@ -54,6 +54,13 @@ def test_fusion_plan_does_not_depend_on_the_batch_or_the_optimizer():
         assert N.model_fusion(model, batch=128) == N.model_fusion(same)
 
 
-def test_fusion_plan_refuses_what_the_net_refuses():
+def test_fusion_plan_refuses_what_the_net_refuses(tmp_path, capfd):
+    # c3d with its first conv edge LOCAL (the untied kernels are 2-D only)
+    lines = N.model_text("c3d").splitlines(keepends=True)
+    line = lines.index("  edge_type: CONVOLUTIONAL\n") + 1
+    lines[line - 1] = "  edge_type: LOCAL\n"
+    path = tmp_path / "local3d.pbtxt"
+    path.write_text("".join(lines))
     with pytest.raises(ValueError):
-        N.model_fusion("invalid:local3d")
+        N.model_fusion(str(path))
+    assert "%s:%d: edge 'input:conv1a': LOCAL" % (path, line) in capfd.readouterr().err

@@ -53,10 +53,15 @@ def test_local_gradcheck_net_shapes():
     assert N.model_edge_params("localcheck") == [8 * (36 * 64 + 64), 0, 8 * (72 * 9 + 9), 5 * (72 + 1)]
 
 
-def test_local_on_3d_layers_is_refused(capfd):
-    # "invalid:local3d": a test-only clip net whose second weighted edge is LOCAL; the net construction refuses it
+def test_local_on_3d_layers_is_refused_at_its_line(tmp_path, capfd):
+    # c3d with its first conv edge LOCAL: the net construction refuses it at the line of edge_type
+    lines = N.model_text("c3d").splitlines(keepends=True)
+    line = lines.index("  edge_type: CONVOLUTIONAL\n") + 1
+    lines[line - 1] = "  edge_type: LOCAL\n"
+    path = tmp_path / "local3d.pbtxt"
+    path.write_text("".join(lines))
     with pytest.raises(ValueError):
-        N.model_edge_params("invalid:local3d")
-    assert "LOCAL is not supported on 3-D layers" in capfd.readouterr().err
+        N.model_edge_params(str(path))
+    assert "%s:%d: edge 'input:conv1a': LOCAL is not supported on 3-D layers" % (path, line) in capfd.readouterr().err
     with pytest.raises(ValueError):
-        N.model_param_layout("invalid:local3d")
+        N.model_param_layout(str(path))

@@ -68,19 +68,43 @@ def test_logcheck_is_gradcheck_with_logistic_units():
     ("tiny+binary-ce+soft-targets", "one output suffix only"),
     ("lenet+squared-error+squared-error", "one output suffix only"),
     ("gradcheck+logistic", "+logistic finds no RECTIFIED_LINEAR hidden layer"),
-    ("tiny+logistic+logistic", "+logistic finds no RECTIFIED_LINEAR hidden layer"),
-    ("invalid:hidden-softmax", "layer 'nin1': SOFTMAX / SOFTMAX_DIST is an output activation"),
-    ("invalid:hinge-loss", "layer 'output': loss_function HINGE_LINEAR is not supported"),
-    ("invalid:hinge-metric", "layer 'output': performance_metric HINGE_QUADRATIC is not supported"),
-    ("invalid:loss-target", "loss_function SQUARED_ERROR reads a float target per feature, but this output layer's "
-                            "activation has integer labels"),
-    ("invalid:metric-target", "performance_metric CLASSIFICATION_MULTINOMIAL reads integer labels, but this output "
-                              "layer's activation has a float target per feature"),
-    ("invalid:classification-loss", "loss_function CLASSIFICATION_BINARY has no derivative to train with")])
+    ("tiny+logistic+logistic", "+logistic finds no RECTIFIED_LINEAR hidden layer")])
 def test_refusals(model, message, capfd):
     with pytest.raises(ValueError):
         N.model_param_layout(model)
     assert message in capfd.readouterr().err
+
+
+# tiny's model text with fields of one layer changed; the refusal names the line of `field`
+@pytest.mark.parametrize("layer,changes,field,message", [
+    ("nin1", {"activation": "SOFTMAX"}, "activation", "layer 'nin1': SOFTMAX / SOFTMAX_DIST is an output activation"),
+    ("output", {"loss_function": "HINGE_LINEAR"}, "loss_function",
+     "layer 'output': loss_function HINGE_LINEAR is not supported"),
+    ("output", {"performance_metric": "HINGE_QUADRATIC"}, "performance_metric",
+     "layer 'output': performance_metric HINGE_QUADRATIC is not supported"),
+    # a labels output with a per-feature loss; a per-feature output with the labels metric
+    ("output", {"loss_function": "SQUARED_ERROR"}, "loss_function",
+     "layer 'output': loss_function SQUARED_ERROR reads a float target per feature, but this output layer's activation "
+     "has integer labels"),
+    ("output", {"activation": "LOGISTIC", "loss_function": "CROSS_ENTROPY_BINARY"}, "performance_metric",
+     "layer 'output': performance_metric CLASSIFICATION_MULTINOMIAL reads integer labels, but this output layer's "
+     "activation has a float target per feature"),
+    ("output", {"activation": "LOGISTIC", "loss_function": "CLASSIFICATION_BINARY"}, "loss_function",
+     "layer 'output': loss_function CLASSIFICATION_BINARY has no derivative to train with")])
+def test_refusals_in_a_model_file(tmp_path, capfd, layer, changes, field, message):
+    lines = N.model_text("tiny").splitlines(keepends=True)
+    k, at = lines.index('  name: "%s"\n' % layer), {}
+    while lines[k] != "}\n":
+        name = lines[k].split(":")[0].strip()
+        if name in changes:
+            lines[k] = "  %s: %s\n" % (name, changes[name])
+        at[name] = k + 1
+        k += 1
+    path = tmp_path / "tiny.pbtxt"
+    path.write_text("".join(lines))
+    with pytest.raises(ValueError):
+        N.model_param_layout(str(path))
+    assert "%s:%d: %s" % (path, at[field], message) in capfd.readouterr().err
 
 
 def test_loss_codes_follow_the_proto():

@@ -24,8 +24,6 @@ void reduce_partials(const float* part, float* out, long long elems, int groups,
 struct ConvOutcome { int path = kPathNone; bool emitted = false, dropped = false; };
 ConvOutcome tc_conv_up(const ConvGeom& g, const float* images, const float* filters, float* targets,
                        float scaleTargets, float scaleOutput, const Fuse& fuse, __nv_bfloat16* targets_bf16);
-int extract_patches(const float* images, float* patches, const float* width_offset, const float* height_offset, const float* flip,
-                    int N, int W, int H, int pw, int ph, int C);                                          // elementwise.cu
 void dropout_apply(float* x, long long n, float dropprob, float scale, unsigned long long seed, __nv_bfloat16* out16);   // elementwise.cu
 void tc_conv_down_prestage(const ConvGeom& g, const float* derivs, const float* filters);   // builds the dgrad filter banks, if that path will run
 ConvOutcome tc_conv_down(const ConvGeom& g, const float* derivs, const float* filters, float* targets,

@@ -113,8 +113,9 @@ int convnet_b200_extract_patches(cudamat* images, cudamat* patches, cudamat* wid
   if (width_offset->size[0] * width_offset->size[1] != num_images) return -1;
   if (height_offset->size[0] * height_offset->size[1] != num_images) return -1;
   if (flip->size[0] * flip->size[1] != num_images) return -1;
-  return extract_patches(images->data_device, patches->data_device, width_offset->data_device, height_offset->data_device,
-                         flip->data_device, num_images, img_width, img_height, patch_width, patch_height, num_colors);
+  return cnb_extract_patches(images->data_device, patches->data_device, nullptr, width_offset->data_device,
+                             height_offset->data_device, flip->data_device, num_images, num_colors, img_width, img_height,
+                             patch_width, patch_height, nullptr, nullptr, nullptr, nullptr, 0);
 }
 void convnet_b200_fuse_next_dropout(float dropprob, float scale, unsigned long long seed) {
   Fuse& f = state().fuse;

@@ -417,17 +417,15 @@ API void cnb_data_get_batch(void* d, void* net, int start, int multiplicity_id) 
 }
 // the jitter of the last minibatch (host copies): out = {width offsets, height offsets, mirror bits}, 3 x batch floats
 API int cnb_data_last_noise(void* d, float* out, int cap) {
-  DataIterator* it = (DataIterator*)d;
-  const int n = (int)it->LastWidthOffsets().size();
+  const NoiseStage& noise = ((DataIterator*)d)->Noise();
+  const int n = noise.LastBatch();
   if (cap < 3 * n) return -1;
-  memcpy(out, it->LastWidthOffsets().data(), sizeof(float) * n);
-  memcpy(out + n, it->LastHeightOffsets().data(), sizeof(float) * n);
-  memcpy(out + 2 * n, it->LastFlipBits().data(), sizeof(float) * n);
+  memcpy(out, noise.Last(), sizeof(float) * 3 * n);
   return n;
 }
 // pure host logic (no GPU): offset of deterministic view `multiplicity_id` for a free range of (max_x, max_y) pixels
 API void cnb_data_view_offset(int multiplicity_id, int max_offset_x, int max_offset_y, int* w, int* h) {
-  DataIterator::ViewOffset(multiplicity_id, max_offset_x, max_offset_y, w, h);
+  Jitter::ViewOffset(multiplicity_id, max_offset_x, max_offset_y, w, h);
 }
 
 // ---- the data set feed (data.h): DataSchedule is the pure host state machine, DataHandler runs it on the GPU.  A refused
@@ -476,10 +474,10 @@ API int cnb_handler_seek(void* h, int row) {
 API int cnb_handler_last(void* p, int* start, int* multiplicity_id, int* rows, float* noise) {
   DataHandler* h = (DataHandler*)p;
   const DataSchedule& s = h->Schedule();
-  const int n = (int)h->LastNoise().size() / 3;
+  const int n = h->Noise().LastBatch();
   *start = h->LastBatch().start; *multiplicity_id = h->LastBatch().multiplicity_id;
   for (int i = 0; i < n; i++) rows[i] = s.Rows()[s.Permutation()[h->LastBatch().start + i]];
-  memcpy(noise, h->LastNoise().data(), sizeof(float) * 3 * n);
+  memcpy(noise, h->Noise().Last(), sizeof(float) * 3 * n);
   return n;
 }
 // a model's train_dataset (which 0) or valid_dataset (1): 1 and its fields, 0 when the model has none, -1 unknown model

@@ -2,7 +2,11 @@
 // one image per column, and per minibatch a crop + mirror + transpose into the input layer (src/datahandler.cc:146-200
 // DataHandler::GetBatch, :520-531 DataIterator::AddNoise, :533-568 DataIterator::SampleNoise).  Reading the data set from
 // disk (HDF5 / image lists) stays with the caller: it hands over float pixels in the reference's (colour, row, column)
-// order through Upload().
+// order, to DataIterator::Upload or in host memory to DataHandler.
+// The two feeds share the per-minibatch work: Jitter draws the offsets and mirror bits, NoiseStage carries them to the
+// device, and one crop launch cuts the batch (DataIterator: cnb_extract_patches on a contiguous slice of its chunk;
+// DataHandler: cnb_extract_patches_indexed through a permutation, gathering the labels or targets in the same launch).
+// What each owns apart from that is its chunk and how it fills it.
 #pragma once
 #include <cstdint>
 #include <vector>
@@ -13,40 +17,70 @@ namespace cnbhost {
 
 class ConvNet;
 
-// splitmix64: the generator behind the jitter of DataIterator and DataHandler and the shuffles of DataSchedule
+// splitmix64: the generator behind the jitter and the shuffles of DataSchedule
 uint64_t SplitMix64(uint64_t& state);
+
+// :533-568 — the jitter of one minibatch: random offsets when `translate`, else the centre / corner crop number
+// multiplicity_id % 5; random mirror bits when `flip`, else multiplicity_id / 5.  Per image the height offset is drawn
+// before the width offset, and the mirror bits after all offsets.
+class Jitter {
+ public:
+  Jitter(int image_size_y, int image_size_x, int gpu_image_size_y, int gpu_image_size_x, bool translate, bool flip,
+         uint64_t seed);
+  // out[0, 3 * batch_size): width offsets | height offsets | mirror bits (mirrored when > 0.5)
+  void Sample(int batch_size, int multiplicity_id, float* out);
+  // the deterministic (translate == false) views of :547-556: centre, top-left, top-right, bottom-right, bottom-left
+  static void ViewOffset(int multiplicity_id, int max_offset_x, int max_offset_y, int* w, int* h);
+
+ private:
+  int max_offset_y_, max_offset_x_;
+  bool translate_, flip_;
+  uint64_t rng_;
+  float Uniform();                                // [0, 1)
+};
+
+// The jitter on its way to the crop: kRing pinned blocks that Jitter fills in place, each reused only after the event
+// recorded behind its last copy, so no batch waits for the stream, and one device block of 3 x batch floats that the copy
+// lands in and the crop reads.  A batch larger than any before grows both, once the stream has drained.
+class NoiseStage {
+ public:
+  NoiseStage();
+  ~NoiseStage();
+  // draws a batch's jitter and copies it on Matrix::Stream(); returns the device block
+  const float* Stage(Jitter& jitter, int batch_size, int multiplicity_id);
+  const float* Last() const { return last_; }     // host copy of the last batch's jitter, 3 x LastBatch() floats
+  int LastBatch() const { return last_batch_; }   // 0 before the first
+
+ private:
+  static constexpr int kRing = 4;
+  float* pinned_ = nullptr;                       // kRing blocks of 3 x cap_ floats
+  float* device_ = nullptr;                       // 3 x cap_
+  const float* last_ = nullptr;
+  int cap_ = 0, last_batch_ = 0, slot_ = 0;
+  cudaEvent_t done_[kRing];
+};
 
 class DataIterator {
  public:
   // images of image_size_y x image_size_x x channels, `chunk_size` of them on the GPU; the net sees gpu_image_size_* crops
   DataIterator(int chunk_size, int channels, int image_size_y, int image_size_x, int gpu_image_size_y, int gpu_image_size_x,
                bool translate, bool flip, uint64_t seed);
-  ~DataIterator();
   int ChunkSize() const { return chunk_size_; }
   int NumDims() const { return channels_ * image_size_y_ * image_size_x_; }
   // host pixels of images [first, first + count) of the chunk, image-major, each image (colour, row, column); async
   void Upload(const float* host, int first, int count);
-  // :533-568 — the jitter of one minibatch: random offsets when `translate`, else the centre / corner crop number
-  // multiplicity_id % 5; random mirror bits when `flip`, else multiplicity_id / 5
-  void SampleNoise(int batch_size, int multiplicity_id);
-  // the deterministic (translate == false) views of :547-556: centre, top-left, top-right, bottom-right, bottom-left
-  static void ViewOffset(int multiplicity_id, int max_offset_x, int max_offset_y, int* w, int* h);
+  // the jitter of the next minibatch of batch_size images (Jitter::Sample), staged for AddNoise
+  void SampleNoise(int batch_size, int multiplicity_id) { d_noise_ = noise_.Stage(jitter_, batch_size, multiplicity_id); }
   // :520-531 + GetBatch's slice: images [start, start + batch) of the chunk -> dest (batch x C*gy*gx, image fastest)
   void AddNoise(int start, Matrix& dest);
-  const std::vector<float>& LastWidthOffsets() const { return h_wo_; }
-  const std::vector<float>& LastHeightOffsets() const { return h_ho_; }
-  const std::vector<float>& LastFlipBits() const { return h_flip_; }
+  const NoiseStage& Noise() const { return noise_; }
 
  private:
   int chunk_size_, channels_, image_size_y_, image_size_x_, gpu_image_size_y_, gpu_image_size_x_;
-  bool translate_, flip_;
-  uint64_t rng_;
-  Matrix data_, width_offset_, height_offset_, flip_bit_;
-  std::vector<float> h_wo_, h_ho_, h_flip_;
-  float* pinned_ = nullptr;                       // 3 x batch floats, the staging area of the three vectors
-  int pinned_cap_ = 0;
-  uint64_t NextRand();
-  float Uniform();                                // [0, 1)
+  Matrix data_;
+  Jitter jitter_;
+  NoiseStage noise_;
+  const float* d_noise_ = nullptr;
 };
 
 // The fields of the reference's DatasetConfig (proto/convnet_config.proto:371-382) that decide the batch order, with the
@@ -104,8 +138,8 @@ class DataSchedule {
 // Streams: chunk copies without pipeline_loads, the jitter and permutation uploads, and the crop run on the library
 // stream.  With pipeline_loads (and a data set larger than a chunk) the next chunk is copied into a second buffer on a
 // copy stream of its own; that copy waits for an event recorded after the last crop that read the buffer, and the crop
-// after the swap waits for the copy's event.  Jitter and permutations reach the device through rings of pinned blocks,
-// each reused only after the event recorded behind its last copy: no stream is synchronised per batch.
+// after the swap waits for the copy's event.  Jitter (NoiseStage) and permutations reach the device through rings of
+// pinned blocks, each reused only after the event recorded behind its last copy: no stream is synchronised per batch.
 class DataHandler {
  public:
   DataHandler(const DatasetOrder& c, int dataset_size, int channels, int image_size_y, int image_size_x,
@@ -119,34 +153,30 @@ class DataHandler {
   void Seek(int row);
   const DataSchedule& Schedule() const { return schedule_; }
   const DataSchedule::Batch& LastBatch() const { return last_; }
-  const std::vector<float>& LastNoise() const { return h_noise_; }  // width offsets | height offsets | mirror bits
+  const NoiseStage& Noise() const { return noise_; }
 
  private:
   static constexpr int kRing = 4;
   DataSchedule schedule_;
   int channels_, isy_, isx_, gy_, gx_, target_dims_, batch_;
-  bool translate_, flip_;
   const float* images_;
   const int* labels_;
   const float* targets_;
-  uint64_t rng_;
+  Jitter jitter_;
+  NoiseStage noise_;
   int cur_ = 0;                                    // which of the chunk buffers is resident
   float* d_images_[2] = {nullptr, nullptr};
   int* d_labels_[2] = {nullptr, nullptr};
   float* d_targets_[2] = {nullptr, nullptr};
   int* d_perm_ = nullptr;
-  float* d_noise_ = nullptr;                       // 3 x batch
-  float* pinned_noise_ = nullptr;                  // kRing blocks of 3 x batch floats
   int* pinned_perm_ = nullptr;                     // kRing blocks of chunk ints
-  cudaEvent_t noise_done_[kRing], perm_done_[kRing], loaded_[2], consumed_[2];
-  int noise_slot_ = 0, perm_slot_ = 0;
+  cudaEvent_t perm_done_[kRing], loaded_[2], consumed_[2];
+  int perm_slot_ = 0;
   bool staged_ = false;                            // the schedule's preload has been issued into buffer 1 - cur_
   cudaStream_t copy_stream_ = nullptr;            // with two chunk buffers only
   DataSchedule::Batch last_;
-  std::vector<float> h_noise_;
   void CopyRows(const std::vector<int>& rows, int buf, cudaStream_t s);
   void UploadPermutation();
-  void SampleNoise(int multiplicity_id);
 };
 
 }  // namespace cnbhost

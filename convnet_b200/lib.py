@@ -110,13 +110,14 @@ SIGNATURES = {
     "cnb_bn_apply": [FP, FP, ct.c_longlong, I, FP, FP, FP, FP, I],
     "cnb_bn_backward": [FP, FP, ct.c_longlong, I, FP, FP, FP, I, FP, FP],
     "cnb_polyak_average": [FP, FP, ct.c_longlong, ct.c_longlong, I],
+    "cnb_extract_patches": [FP, FP, ct.c_void_p, FP, FP, FP, I, I, I, I, I, I, ct.c_void_p, ct.c_void_p, FP, FP, I],
     "cnb_extract_patches_indexed": [FP, FP, ct.c_void_p, FP, FP, FP, I, I, I, I, I, I, ct.c_void_p, ct.c_void_p, FP, FP, I],
 }
 RESTYPES = {
     "convnet_b200_version": I, "convnet_b200_get_stream": ct.c_void_p,
     "convnet_b200_get_conv_precision": I, "convnet_b200_last_conv_path": I, "convnet_b200_bf16_is_staged": I,
     "convnet_b200_launch_count": ct.c_ulonglong, "convnet_b200_extract_patches": I,
-    "convnet_b200_dgrad_bank_builds": ct.c_ulonglong, "cnb_extract_patches_indexed": I,
+    "convnet_b200_dgrad_bank_builds": ct.c_ulonglong, "cnb_extract_patches": I, "cnb_extract_patches_indexed": I,
 }
 
 _lib = None

@@ -68,7 +68,7 @@ def build(force=False, verbose=False):
 
 HOST = os.path.join(HERE, "host")
 HOST_LIB = os.path.join(LIBDIR, "libconvnet_b200_host.so")
-HOST_SOURCES = ["matrix.cc", "edge.cc", "convnet.cc", "models.cc", "model_file.cc", "checkpoint.cc", "data.cc", "capi.cc"]
+HOST_SOURCES = ["matrix.cc", "edge.cc", "convnet.cc", "models.cc", "model_file.cc", "checkpoint.cc", "train.cc", "data.cc", "capi.cc"]
 
 
 def build_host(force=False):

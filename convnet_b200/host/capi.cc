@@ -16,6 +16,7 @@ struct NetHandle {
   ConvNet* net = nullptr;
   GradChecker* checker = nullptr;
   DataParallelSync* dp = nullptr;
+  std::vector<TrainEvent> events;                          // of the last cnb_net_train
 };
 
 // BuildModel for the C API: an unknown name gives false and the reason on stderr instead of an exception
@@ -490,3 +491,74 @@ API int cnb_model_dataset(const char* model, int which, DatasetOrder* order, int
   *gpu_image_size_y = d.gpu_image_size_y; *gpu_image_size_x = d.gpu_image_size_x;
   return d.present ? 1 : 0;
 }
+
+// ---- the training loop (train.cc).  Host only: a model's schedule, CheckReduceLearningRate and the loop's decisions
+// static description of a model's training schedule: ints = {max_iter, print_after, validate_after, save_after,
+// reduce_lr_num_steps, reduce_lr_max, smaller_is_better}, floats = {reduce_lr_factor, reduce_lr_threshold}, and the
+// NUL-terminated strings reduce_lr_layer_name and checkpoint_dir (up to 4096 bytes each).  0 ok, -1 unknown model
+API int cnb_model_schedule(const char* model, int* ints, float* floats, char* layer_name, char* checkpoint_dir) {
+  ModelConfig m;
+  if (!TryBuildModel(model, &m)) return -1;
+  const int v[] = {m.max_iter, m.print_after, m.validate_after, m.save_after, m.reduce_lr_num_steps, m.reduce_lr_max,
+                   m.smaller_is_better ? 1 : 0};
+  memcpy(ints, v, sizeof(v));
+  floats[0] = m.reduce_lr_factor; floats[1] = m.reduce_lr_threshold;
+  snprintf(layer_name, 4096, "%s", m.reduce_lr_layer_name.c_str());
+  snprintf(checkpoint_dir, 4096, "%s", m.checkpoint_dir.c_str());
+  return 0;
+}
+API int cnb_reduce_lr_due(const float* history, int len, int num_steps, float threshold, int smaller_is_better) {
+  return ReduceLrDue(std::vector<float>(history, history + len), num_steps, threshold, smaller_is_better != 0) ? 1 : 0;
+}
+// ConvNet::Train's decisions without a net, from TrainOneBatch call `start` + 1 to max_iter: per iteration with an action,
+// iters[k] and actions[k] (TrainSchedule::Action bits, plus 16: the learning rate is reduced after this validation, 32:
+// this validation runs on the Polyak average), and for the save after the loop a last record (max_iter, 8 | 64).  The
+// validations take the values values[0, n_values) in order.  Returns the number of records (writes up to `cap`); -1 with
+// the reason in cnb_last_error(): a refused schedule or model, or more validations than values
+API long long cnb_train_dry_run(const char* model, long long start, int lr_reduce_counter, int validation_set,
+                                const float* values, int n_values, long long cap, long long* iters, int* actions) {
+  long long n = 0;
+  const int rc = Guard([&] {
+    const ModelConfig m = BuildModel(model);
+    TrainSchedule s(m, lr_reduce_counter);
+    auto put = [&](long long it, int a) { if (n < cap) { iters[n] = it; actions[n] = a; } n++; };
+    int validated = 0;
+    long long inserted = 0;
+    for (long long it = start + 1; it <= m.max_iter; it++) {
+      int a = s.Actions(it, validation_set != 0);
+      if (a & TrainSchedule::INSERT) inserted++;
+      if (a & TrainSchedule::VALIDATE) {
+        if (validated == n_values) throw std::invalid_argument("more validations than values");
+        if (PolyakOn(m) && inserted > 0) a |= 32;
+        if (s.Validated(values[validated++])) a |= 16;
+      }
+      if (a) put(it, a);
+    }
+    if (s.FinalSave()) put(m.max_iter, TrainSchedule::SAVE | 64);
+  });
+  return rc ? -1 : n;
+}
+
+API int cnb_net_validate(void* p, void* handler, float* out) {
+  return Guard([&] { *out = ((NetHandle*)p)->net->Validate(*(DataHandler*)handler); });
+}
+// ConvNet::Train; valid, checkpoint_dir and run_name may be NULL.  Returns the number of events (cnb_net_train_event), or
+// -1 with the reason in cnb_last_error()
+API int cnb_net_train(void* p, void* train, void* valid, const char* checkpoint_dir, const char* run_name) {
+  NetHandle* h = (NetHandle*)p;
+  h->events.clear();
+  const int rc = Guard([&] {
+    h->events = h->net->Train(*(DataHandler*)train, (DataHandler*)valid, checkpoint_dir ? checkpoint_dir : "",
+                              run_name ? run_name : "");
+  });
+  return rc ? -1 : (int)h->events.size();
+}
+// event k of the last cnb_net_train: *kind 0 train, 1 valid.  0 ok, -1 k out of range
+API int cnb_net_train_event(void* p, int k, long long* iteration, int* kind, float* value, int* lr_reduced, int* polyak) {
+  const std::vector<TrainEvent>& e = ((NetHandle*)p)->events;
+  if (k < 0 || k >= (int)e.size()) return -1;
+  *iteration = e[k].iteration; *kind = e[k].kind; *value = e[k].value;
+  *lr_reduced = e[k].lr_reduced; *polyak = e[k].polyak;
+  return 0;
+}
+API int cnb_net_lr_reduce_counter(void* p) { return ((NetHandle*)p)->net->LrReduceCounter(); }

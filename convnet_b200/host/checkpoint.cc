@@ -201,6 +201,7 @@ void ConvNet::Save(const std::string& path) {
     w.Text("__model__", ModelText(m));
     w.Int("__current_iter__", (long long)step_);
     w.Int("__seed__", (long long)model_.seed);
+    if (lr_reduce_counter_) w.Int("__lr_reduce_counter__", lr_reduce_counter_);   // (a net the loop never reduced: no record)
     std::vector<OptimizerConfig> opt;
     for (const TrainedTensor& t : tensors_) opt.push_back(t.opt);
     for (const CheckpointEntry& e : CheckpointEntries(opt)) {
@@ -265,7 +266,15 @@ void ConvNet::Load(const std::string& path) {
   std::vector<OptimizerConfig> configs;
   for (const TrainedTensor& t : tensors_) configs.push_back(ModelOptimizer(opt, t));
   const std::vector<CheckpointEntry> entries = CheckpointEntries(configs);
-  std::set<std::string> known = {"__model__", "__current_iter__", "__seed__"};
+  // optional: the reductions of the learning rate ConvNet::Train applied.  Unlike the reference's Load (src/convnet.cc:
+  // 745-748) they are not applied again: __model__ already holds the epsilons they left
+  long long lr_reduce_counter = 0;
+  if (f.Has("__lr_reduce_counter__")) {
+    const std::string why = f.Check("__lr_reduce_counter__", CheckpointFile::INT64, 1);
+    if (!why.empty()) throw std::invalid_argument(why);
+    memcpy(&lr_reduce_counter, f.Read("__lr_reduce_counter__").data(), 8);
+  }
+  std::set<std::string> known = {"__model__", "__current_iter__", "__seed__", "__lr_reduce_counter__"};
   for (const CheckpointEntry& e : entries) {
     const bool step = e.buffer == CheckpointEntry::STEP;
     const std::string why = f.Check(e.name, step ? CheckpointFile::INT64 : CheckpointFile::FLOAT32, e.n);
@@ -296,6 +305,7 @@ void ConvNet::Load(const std::string& path) {
     }
   }
   step_ = (unsigned long long)iter;
+  lr_reduce_counter_ = (int)lr_reduce_counter;
   model_.seed = (unsigned)seed;
   if (salted_) SaltDropout();                        // the file's seed, this net's rank
   CKPT_CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));   // (the host buffers go away)

@@ -746,10 +746,13 @@ float ConvNet::GetLoss() {                                   // Layer::GetLoss: 
   return out.LossWeight() * loss_sum_.ReadValue(0);
 }
 float ConvNet::GetPerformanceMetric() {
+  SumPerformanceMetric(loss_sum_.GetDevData() + 1);
+  return loss_sum_.ReadValue(1);
+}
+void ConvNet::SumPerformanceMetric(float* dst) {
   Layer& out = OutputLayer();
   out.ComputePerformanceMetric();
-  cnb_sum(out.GetMetricPerImage(), loss_sum_.GetDevData() + 1, batch_size_);
-  return loss_sum_.ReadValue(1);
+  cnb_sum(out.GetMetricPerImage(), dst, batch_size_);
 }
 
 void ConvNet::Bprop() {                                      // convnet.cc:390-405 + 362-375

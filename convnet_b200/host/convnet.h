@@ -79,6 +79,12 @@ struct ModelConfig {
   // Polyak averaging (proto Model fields, same defaults): on when polyak_after and polyak_queue_size are both > 0; its
   // insertion rule (PolyakDue) also reads validate_after and save_after
   int polyak_after = 0, polyak_queue_size = 0, validate_after = -1, save_after = -1;
+  // the rest of the training schedule ConvNet::Train runs (TrainSchedule; proto Model fields, same defaults).  ModelText
+  // writes none of them, nor validate_after / save_after without Polyak: a checkpoint's __model__ carries no schedule
+  int max_iter = -1, print_after = -1, reduce_lr_num_steps = 0, reduce_lr_max = 0;
+  float reduce_lr_factor = 1.f, reduce_lr_threshold = 0.f;
+  bool smaller_is_better = false;
+  std::string reduce_lr_layer_name, checkpoint_dir;
   // train_dataset / valid_dataset: the batch order and, from the data stream of the input layer, its crop (gpu_image_size
   // 0: the whole image) and jitter
   struct Dataset {
@@ -92,6 +98,46 @@ inline bool PolyakOn(const ModelConfig& m) { return m.polyak_after > 0 && m.poly
 // checkpoint.cc: whether the reference's training loop inserts the parameters into the Polyak queue after TrainOneBatch call
 // number `iteration` (src/convnet.cc:881-883, 965-967 with i + 1 = iteration; C++'s truncating %).  False with Polyak off
 bool PolyakDue(const ModelConfig& m, long long iteration);
+
+// train.cc: the reference's CheckReduceLearningRate (src/convnet.cc:788-818): false while `history` holds fewer than
+// num_steps values; else the float running means of the first num_steps / 2 and of the other values among the last
+// num_steps, and true when (smaller_is_better ? first - second : second - first) < threshold
+bool ReduceLrDue(const std::vector<float>& history, int num_steps, float threshold, bool smaller_is_better);
+
+// train.cc: the schedule of the reference's Train loop (src/convnet.cc:921-1006) without a net, so that a dry run and
+// ConvNet::Train take their decisions from the same code.  Periods are C++'s truncating %: an action with period p runs
+// after TrainOneBatch call `iteration` when iteration % p == 0, so p = -1 (the proto default of print_after and
+// save_after) runs it after every call, and -p acts as p.  The constructor refuses (std::invalid_argument naming the
+// field) what the reference divides by zero or exits on: print_after or save_after 0, and a reduce_lr_layer_name that
+// is not the output layer's
+class TrainSchedule {
+ public:
+  TrainSchedule(const ModelConfig& m, int lr_reduce_counter);
+  enum Action { PRINT = 1, INSERT = 2, VALIDATE = 4, SAVE = 8 };
+  // the actions after TrainOneBatch call `iteration` (i + 1 in the reference's loop), in the order they run;
+  // VALIDATE only when there is a validation set
+  int Actions(long long iteration, bool validation_set) const;
+  bool FinalSave() const { return m_.max_iter % m_.save_after != 0; }       // :1003, after the last step
+  // :978-994 for a new validation value: true when the learning rate is to be reduced now (the counters have moved)
+  bool Validated(float value);
+  int LrReduceCounter() const { return lr_reduce_counter_; }
+  const ModelConfig& Model() const { return m_; }
+
+ private:
+  ModelConfig m_;
+  std::vector<float> history_;
+  int lr_reduce_counter_, dont_reduce_lr_ = 0;
+};
+
+// one line of ConvNet::Train's log: the training metric of a print (TRAIN) or a validation value (VALID)
+struct TrainEvent {
+  enum Kind { TRAIN, VALID };
+  long long iteration;
+  Kind kind;
+  float value;
+  bool lr_reduced = false;        // VALID: the learning rate was reduced after it
+  bool polyak = false;            // VALID: measured on the Polyak average (false: on the current weights)
+};
 
 // checkpoint.cc: a checkpoint file (DESIGN.md §5 "Checkpoints"): an 8-byte magic, a u32 version, then records until EOF,
 // each a u32 name length, the name, a u8 type, a u64 element count and the payload, little-endian.  The constructor reads
@@ -276,6 +322,25 @@ class ConvNet {
   void TrainOneBatch(float* loss_out);                          // convnet.cc:475-485
   float GetLoss();                                              // loss_function_weight * the batch's loss (synchronises)
   float GetPerformanceMetric();                                 // sum of the per-image performance metric (synchronises)
+  // the same sum into device float `dst`, on the main stream, without a host wait
+  void SumPerformanceMetric(float* dst);
+
+  // ---- the reference's Validate and Train (train.cc)
+  // src/convnet.cc:571-589: Seek(0), then dataset_size / batch_size batches (the rest is dropped) of GetBatch, Fprop(false)
+  // and the output layer's metric; the float running mean total = total * k / (k + 1) + e / (batch * (k + 1)).  One host
+  // wait, at the end.  std::invalid_argument: the handler's batch size is not the net's
+  float Validate(DataHandler& data);
+  // src/convnet.cc:866-1006 from Iteration() to max_iter (TrainSchedule).  The run is named run_name ("" : <model
+  // name>_<timestamp>); under checkpoint_dir ("" : the model's, and "." if it has none; created if missing) it writes
+  // <run>.pbtxt, <run>_train.log, <run>_valid.log, <run>.ckpt and, with Polyak, <run>.ckptpolyak.  Validation with
+  // Polyak on runs on LoadPolyakWeights() and training continues from the average, as in the reference; where the queue
+  // is still empty (the reference divides by zero) it runs on the current weights, and the log says so.
+  // std::invalid_argument: the schedule (TrainSchedule), a handler of another batch size, a data-parallel net
+  std::vector<TrainEvent> Train(DataHandler& train, DataHandler* valid, const std::string& checkpoint_dir,
+                                const std::string& run_name);
+  // reductions of the learning rate the loop has applied to this net; a checkpoint keeps it (record
+  // __lr_reduce_counter__, written when it is not 0), and Load restores it without applying them again
+  int LrReduceCounter() const { return lr_reduce_counter_; }
   void SetDataParallel(DataParallelSync* dp, size_t bucket_floats);
   void SetBucketFloats(size_t bucket_floats);                   // re-plan the buckets (also used without data parallelism)
   void BroadcastParameters();
@@ -399,6 +464,8 @@ class ConvNet {
   void PrestageAll();                                           // every prestaging edge rebuilds its dgrad banks (main stream)
   float* polyak_ = nullptr;                                     // polyak_queue_size slots, then the backup
   int polyak_index_ = 0;
+  int lr_reduce_counter_ = 0;
+  void SaveWithPolyak(const std::string& path);                 // train.cc: the reference's Save() (:659-667)
   bool polyak_full_ = false, polyak_backup_ = false;
 };
 

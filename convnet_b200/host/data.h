@@ -112,6 +112,8 @@ class DataSchedule {
   Batch Next();                    // DataHandler::GetBatch, :146-200
   void Seek(int row);              // DataHandler::Seek, :124-133
   int ChunkSize() const { return chunk_size_; }
+  int DatasetSize() const { return dataset_size_; }
+  int BatchSize() const { return c_.batch_size; }
   bool FitsOnGpu() const { return fits_on_gpu_; }
   bool Pipelined() const { return c_.pipeline_loads != 0; }
   const std::vector<int>& Rows() const { return rows_; }            // the resident chunk's data set rows

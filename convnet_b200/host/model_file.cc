@@ -462,7 +462,17 @@ class Mapper {
       for (const char* f : {"validate_after", "save_after"})
         if (model.Int(f, -1) == 0) Fail(*model.Get(f), "", std::string("field '") + f + "': 0 with Polyak averaging on "
                                         "(its insertion rule takes the iteration modulo " + f + ")");
-    def_w_ = model.Get("default_weight_optimizer");
+    // the rest of the training schedule (ConvNet::Train checks it when a run starts)
+    m.max_iter = (int)model.Int("max_iter", -1);
+    m.print_after = (int)model.Int("print_after", -1);
+    m.reduce_lr_factor = model.Float("reduce_lr_factor", 1.f);
+    m.reduce_lr_threshold = model.Float("reduce_lr_threshold", 0.f);
+    m.reduce_lr_num_steps = (int)model.Int("reduce_lr_num_steps", 0);
+    m.reduce_lr_max = (int)model.Int("reduce_lr_max", 0);
+    m.smaller_is_better = model.Bool("smaller_is_better", false);
+    if (const Entry* e = model.Get("reduce_lr_layer_name")) m.reduce_lr_layer_name = e->s;
+    if (const Entry* e = model.Get("checkpoint_dir")) m.checkpoint_dir = e->s;
+    def_w_ =model.Get("default_weight_optimizer");
     def_b_ = model.Get("default_bias_optimizer");
     for (const Entry* d : {def_w_, def_b_}) if (d) CheckOptimizer(*d, "");
 

@@ -135,6 +135,13 @@ def load_host():
             "cnb_handler_last": ([vp, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(f)], i),
             "cnb_model_dataset": ([ct.c_char_p, i, ct.POINTER(DatasetOrder), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i),
                                    ct.POINTER(i)], i),
+            "cnb_model_schedule": ([ct.c_char_p, ct.POINTER(i), ct.POINTER(f), ct.c_char_p, ct.c_char_p], i),
+            "cnb_reduce_lr_due": ([ct.POINTER(f), i, i, f, i], i),
+            "cnb_train_dry_run": ([ct.c_char_p, ll, i, i, ct.POINTER(f), i, ll, ct.POINTER(ll), ct.POINTER(i)], ll),
+            "cnb_net_validate": ([vp, vp, ct.POINTER(f)], i),
+            "cnb_net_train": ([vp, vp, vp, ct.c_char_p, ct.c_char_p], i),
+            "cnb_net_train_event": ([vp, i, ct.POINTER(ll), ct.POINTER(i), ct.POINTER(f), ct.POINTER(i), ct.POINTER(i)], i),
+            "cnb_net_lr_reduce_counter": ([vp], i),
         }
         for name, (args, res) in sig.items():
             fn = getattr(H, name)
@@ -418,6 +425,42 @@ class Net:
     def load_current_weights(self):
         """restore the parameters load_polyak_weights kept aside"""
         self._check(self.H.cnb_net_load_current_weights(self.h))
+
+    lr_reduce_counter = property(lambda s: s.H.cnb_net_lr_reduce_counter(s.h),
+                                 doc="learning-rate reductions train() has applied (kept by save, restored by load)")
+
+    # --- the reference's Validate and Train loop (host/train.cc)
+    def validate(self, handler):
+        """the output layer's performance metric per image over the DataHandler `handler` (ConvNet::Validate): seek(0),
+        then dataset_size // batch_size test-mode batches (the rest is dropped), averaged as the reference's float running
+        mean.  ValueError for a handler of another batch size."""
+        v = ct.c_float(0)
+        self._check(self.H.cnb_net_validate(self.h, handler.h, ct.byref(v)))
+        return v.value
+
+    def train(self, train, valid=None, *, checkpoint_dir=None, run_name=None):
+        """train to the model's schedule (ConvNet::Train, the reference's Train loop) from DataHandler `train`, validating
+        on DataHandler `valid` if given, from `iteration` to max_iter.  The schedule is the model's: model_schedule(model)
+        for the fields; the periods act where the iteration modulo the period is 0, so an unset print_after or save_after
+        (-1) prints or checkpoints after every step.  Files go under checkpoint_dir (default: the model's, else "."), named
+        after run_name (default "<model name>_<timestamp>"): <run>.pbtxt, <run>_train.log ("iteration seconds value"
+        per print), <run>_valid.log ("iteration value" per validation), <run>.ckpt and with Polyak <run>.ckptpolyak.
+        Validation with Polyak on loads the average and training continues from it, as in the reference; with the queue
+        still empty it runs on the current weights.  Returns the events, in order: {"iteration", "kind": "train" (the
+        metric per image since the last print) | "valid", "value", "lr_reduced", "polyak" (validated on the average)}.
+        ValueError for a schedule the loop refuses, a handler of another batch size or a data-parallel net."""
+        n = self.H.cnb_net_train(self.h, train.h, valid.h if valid is not None else None,
+                                 None if checkpoint_dir is None else os.fsencode(checkpoint_dir),
+                                 None if run_name is None else run_name.encode())
+        if n < 0:
+            raise ValueError(self.H.cnb_last_error().decode())
+        out = []
+        for k in range(n):
+            it, kind, v, red, pol = ct.c_longlong(0), ct.c_int(0), ct.c_float(0), ct.c_int(0), ct.c_int(0)
+            self.H.cnb_net_train_event(self.h, k, ct.byref(it), ct.byref(kind), ct.byref(v), ct.byref(red), ct.byref(pol))
+            out.append({"iteration": it.value, "kind": ("train", "valid")[kind.value], "value": v.value,
+                        "lr_reduced": bool(red.value), "polyak": bool(pol.value)})
+        return out
 
     def train_step(self, want_loss=True):
         if want_loss:
@@ -832,6 +875,59 @@ def model_dataset(model, which="train_dataset"):
     d.update(zip(("translate", "flip", "gpu_image_size_y", "gpu_image_size_x"), (bool(v[0].value), bool(v[1].value),
                                                                                    v[2].value, v[3].value)))
     return d
+
+
+SCHEDULE_INTS = ("max_iter", "print_after", "validate_after", "save_after", "reduce_lr_num_steps", "reduce_lr_max",
+                 "smaller_is_better")
+
+
+def model_schedule(model):
+    """a model's training schedule (host-only), the fields Net.train reads, at the proto's defaults where unset:
+    {"max_iter", "print_after", "validate_after", "save_after", "reduce_lr_factor", "reduce_lr_threshold",
+    "reduce_lr_num_steps", "reduce_lr_max", "smaller_is_better", "reduce_lr_layer_name", "checkpoint_dir"}"""
+    ints, floats = (ct.c_int * 7)(), (ct.c_float * 2)()
+    layer, cdir = ct.create_string_buffer(4096), ct.create_string_buffer(4096)
+    if load_host().cnb_model_schedule(model.encode(), ints, floats, layer, cdir):
+        raise ValueError("cannot build model %r (see stderr)" % model)
+    out = dict(zip(SCHEDULE_INTS, ints))
+    out["smaller_is_better"] = bool(out["smaller_is_better"])
+    out.update(reduce_lr_factor=floats[0], reduce_lr_threshold=floats[1], reduce_lr_layer_name=layer.value.decode(),
+               checkpoint_dir=os.fsdecode(cdir.value))
+    return out
+
+
+def reduce_lr_due(history, num_steps, threshold, smaller_is_better):
+    """the reference's CheckReduceLearningRate, the test Net.train applies after each validation: False while `history`
+    (validation values, oldest first) holds fewer than num_steps values; else whether the float running mean of the
+    second half of its last num_steps values (the larger half when num_steps is odd) improves on the first half's by less
+    than `threshold` (improves: is smaller when smaller_is_better, else larger)"""
+    h = (ct.c_float * max(1, len(history)))(*history)
+    return bool(load_host().cnb_reduce_lr_due(h, len(history), num_steps, threshold, int(smaller_is_better)))
+
+
+TRAIN_ACTIONS = ("print", "insert", "validate", "save", "lr_reduced", "polyak", "final")
+
+
+def train_dry_run(model, valid_values=None, *, iteration=0, lr_reduce_counter=0):
+    """what Net.train does with `model`'s schedule from train_step number `iteration` + 1 to max_iter, without a GPU
+    (host/train.cc TrainSchedule, the code Net.train decides with): a list of (iteration, set of actions) for every
+    iteration with an action, in order; actions are "print", "insert" (into the Polyak queue), "validate", "save",
+    "lr_reduced" (after this validation), "polyak" (this validation runs on the Polyak average).  The checkpoint after
+    the loop is a last record (max_iter, {"save", "final"}).  valid_values: the validation values, in order (None: no
+    validation set).  ValueError for a schedule Net.train refuses, or fewer values than validations."""
+    H = load_host()
+    vals = list(valid_values or [])
+    fv = (ct.c_float * max(1, len(vals)))(*vals)
+    cap = 1024
+    while True:
+        its, acts = (ct.c_longlong * cap)(), (ct.c_int * cap)()
+        n = H.cnb_train_dry_run(model.encode(), iteration, lr_reduce_counter, int(valid_values is not None), fv, len(vals),
+                                cap, its, acts)
+        if n < 0:
+            raise ValueError(H.cnb_last_error().decode())
+        if n <= cap:
+            return [(its[k], {a for b, a in enumerate(TRAIN_ACTIONS) if acts[k] >> b & 1}) for k in range(n)]
+        cap = n
 
 
 Net.model_output_layer = staticmethod(model_output_layer)

@@ -19,39 +19,57 @@ struct NetHandle {
   std::vector<TrainEvent> events;                          // of the last cnb_net_train
 };
 
-// BuildModel for the C API: an unknown name gives false and the reason on stderr instead of an exception
-static bool TryBuildModel(const char* name, ModelConfig* m) {
-  try { *m = BuildModel(name); return true; }
-  catch (const std::invalid_argument& e) { fprintf(stderr, "convnet_b200 host: %s\n", e.what()); return false; }
+static std::string g_last_error;
+// the message of the last refusal (of a model, a checkpoint, a data set configuration or the training loop)
+API const char* cnb_last_error() { return g_last_error.c_str(); }
+// runs f: 0, or -1 with what it threw in cnb_last_error() and on stderr
+template <class F>
+static int Guard(F f) {
+  try {
+    f();
+    return 0;
+  } catch (const std::exception& e) {
+    g_last_error = e.what();
+    fprintf(stderr, "convnet_b200 host: %s\n", e.what());
+    return -1;
+  }
 }
 
-// NULL: unknown model name, or a model the host cannot run (the reason is printed on stderr)
-API void* cnb_net_create(const char* model, int batch_size, unsigned seed, int grad_checker) {
-  ModelConfig m;
-  if (!TryBuildModel(model, &m)) return nullptr;
-  m.seed = seed;
+// a handle on the ConvNet (GradChecker when grad_checker) of a built-in name or model file, with its seed replaced unless
+// `seed` is NULL; no device memory yet.  NULL: an unknown name, or a model that cannot be read or run (cnb_last_error)
+static NetHandle* Open(const char* model, int batch, const unsigned* seed, bool grad_checker) {
   NetHandle* h = new NetHandle;
-  try {
-    if (grad_checker) { h->checker = new GradChecker(m, batch_size); h->net = h->checker; }
-    else h->net = new ConvNet(m, batch_size);
-  } catch (const std::invalid_argument& e) {
-    fprintf(stderr, "convnet_b200 host: %s\n", e.what());
-    delete h;
-    return nullptr;
-  }
-  try {
-    h->net->AllocateMemory();                                  // (reads the checkpoints of PRETRAINED edges)
-  } catch (const std::exception& e) {
-    fprintf(stderr, "convnet_b200 host: %s\n", e.what());
-    delete h->net;
+  if (Guard([&] {
+        ModelConfig m = BuildModel(model);
+        if (seed) m.seed = *seed;
+        if (grad_checker) h->net = h->checker = new GradChecker(m, batch);
+        else h->net = new ConvNet(m, batch);
+      })) {
     delete h;
     return nullptr;
   }
   return h;
 }
+// a host-only handle: the net built and its parameters planned, nothing allocated on the device.  The cnb_net_* calls that
+// read no device memory describe the model through it: edges, layers, the parameter layout, the fusion plan, FLOPs, the
+// trained tensors' optimizers, and the model-level settings below (cnb_net_model_text ... cnb_net_train_dry_run)
+API void* cnb_model_open(const char* model, int batch) {
+  NetHandle* h = Open(model, batch, nullptr, false);
+  if (h) h->net->PlanParameters();
+  return h;
+}
 API void cnb_net_destroy(void* p) {
   NetHandle* h = (NetHandle*)p;
   delete h->net; delete h->dp; delete h;
+}
+// a net to run: NULL as for cnb_model_open, or when its memory cannot be set up (the checkpoints of PRETRAINED edges)
+API void* cnb_net_create(const char* model, int batch_size, unsigned seed, int grad_checker) {
+  NetHandle* h = Open(model, batch_size, &seed, grad_checker != 0);
+  if (h && Guard([&] { h->net->AllocateMemory(); })) {
+    cnb_net_destroy(h);
+    return nullptr;
+  }
+  return h;
 }
 API long long cnb_net_num_params(void* p) { return (long long)((NetHandle*)p)->net->NumParameters(); }
 API int cnb_net_num_edges(void* p) { return (int)((NetHandle*)p)->net->Edges().size(); }
@@ -60,6 +78,21 @@ API double cnb_net_edge_flops(void* p, int i) { return ((NetHandle*)p)->net->Edg
 // where edge i's parameters begin in the flat buffers (a tied edge: its owner's), and how many floats it owns (0 if tied)
 API long long cnb_net_edge_offset(void* p, int i) { return (long long)((NetHandle*)p)->net->ParamOffset(i); }
 API long long cnb_net_edge_size(void* p, int i) { return (long long)((NetHandle*)p)->net->Edges()[i]->GetParameterMemoryRequirement(); }
+// where the slice placed at edge position i begins (ConvNet::EdgeOffsets: a tie group's slice sits at its lowest edge)
+API long long cnb_net_edge_slice(void* p, int i) { return (long long)((NetHandle*)p)->net->EdgeOffsets()[i]; }
+// the epilogue fusion ConvNet::PlanFusion decided for edge i: *up_act / *down_act the CNB_ACT_* code ComputeUp applies and
+// the one whose derivative ComputeDown applies; returns the Edge::FusionPlan flags (bit 0 dropout_up, 1 scale_down,
+// 2 sums_bias_below, 3 offers_bias_grad)
+API int cnb_net_edge_fusion(void* p, int i, int* up_act, int* down_act) {
+  const Edge::FusionPlan& f = ((NetHandle*)p)->net->Edges()[i]->Plan();
+  *up_act = f.up_act; *down_act = f.down_act;
+  return f.dropout_up | f.scale_down << 1 | f.sums_bias_below << 2 | f.offers_bias_grad << 3;
+}
+// the passes left to layer i after fusion: bit 0 a separate activation pass, bit 1 a separate derivative pass
+API int cnb_net_layer_passes(void* p, int i) {
+  const Layer& l = *((NetHandle*)p)->net->Layers()[i];
+  return l.HasSeparateActivationPass() | l.HasSeparateDerivPass() << 1;
+}
 // the edge whose parameters edge i runs with ("" when untied)
 API const char* cnb_net_edge_tied_to(void* p, int i) { return ((NetHandle*)p)->net->Edges()[i]->Config().tied_to.c_str(); }
 // the frozen edges are [0, n) (ConvNet::NumFrozenEdges); their parameters the prefix [0, *trained_offset) of the buffers
@@ -112,13 +145,16 @@ API int cnb_net_set_optimizer(void* p, const char* tensor, const OptimizerConfig
 // the adaptive optimizer state (cnb_net_num_params floats, carved like the parameters); NULL while no optimizer of the
 // net is ADAGRAD_SGD or RMSPROP_SGD
 API float* cnb_net_adaptive_state(void* p) { return ((NetHandle*)p)->net->AdaptiveState(); }
-// the step count of one optimizer and the (epsilon, momentum) its next update uses.  0 ok, -1 no such tensor
-API int cnb_net_get_optimizer_state(void* p, const char* tensor, long long* step, float* epsilon, float* momentum) {
+// the step count of one optimizer, the (epsilon, momentum) its next update uses and, unless `config` is NULL, its
+// settings.  Returns the tensor's floats (0: the bias of a has_no_bias edge), -1 no such tensor
+API long long cnb_net_get_optimizer_state(void* p, const char* tensor, long long* step, float* epsilon, float* momentum,
+                                          OptimizerConfig* config) {
   const TrainedTensor* t = Tensor(p, tensor);
   if (!t) return -1;
   *step = t->step;
   OptimizerSchedule(t->opt, *step, epsilon, momentum);
-  return 0;
+  if (config) *config = t->opt;
+  return t->n;
 }
 // pure host logic: (epsilon, momentum) of the update after `step` earlier ones.  0 ok, -2 invalid config
 API int cnb_optimizer_schedule(const OptimizerConfig* c, long long step, float* epsilon, float* momentum) {
@@ -134,6 +170,11 @@ static Layer* BnLayer(void* p, int layer) {
 }
 API const char* cnb_net_layer_name(void* p, int i) { return ((NetHandle*)p)->net->Layers()[i]->GetName().c_str(); }
 API int cnb_net_layer_channels(void* p, int i) { return ((NetHandle*)p)->net->Layers()[i]->GetNumChannels(); }
+// the running-average factor and the variance epsilon of layer i's batch normalisation (the model's, used or not)
+API void cnb_net_layer_bn(void* p, int i, float* bn_f, float* bn_epsilon) {
+  const LayerConfig& l = ((NetHandle*)p)->net->Model().layer[i];
+  *bn_f = l.bn_f; *bn_epsilon = l.bn_epsilon;
+}
 // offset of the layer's [gamma | beta] (2 x channels floats) in the flat parameter / gradient buffers; -1: not batch-normalised
 API long long cnb_net_bn_offset(void* p, int layer) { return BnLayer(p, layer) ? ((NetHandle*)p)->net->BnOffsets()[layer] : -1; }
 // device vector of `channels` floats: which 0 running mean, 1 running sigma, 2 batch mean, 3 batch sigma (of the last
@@ -155,15 +196,12 @@ API long long cnb_net_targets_floats(void* p) { return (long long)((NetHandle*)p
 // loss_function_weight * the batch's loss (ConvNet::GetLoss) and the summed performance metric (GetPerformanceMetric)
 API float cnb_net_loss(void* p) { return ((NetHandle*)p)->net->GetLoss(); }
 API float cnb_net_metric(void* p) { return ((NetHandle*)p)->net->GetPerformanceMetric(); }
-// static description of a model's output layer (no device memory): 0 ok, -1 unknown model.  *activation: the Activation
-// enum of convnet.h; *loss / *metric: proto LossFunction numbers; *labels: 1 trained on integer labels, 0 on float targets
-API int cnb_model_output_layer(const char* model, int* activation, int* loss, int* metric, float* weight, int* labels) {
-  ModelConfig m;
-  if (!TryBuildModel(model, &m)) return -1;
-  const LayerConfig& l = m.layer.back();
+// the model's output layer.  *activation: the Activation enum of convnet.h; *loss / *metric: proto LossFunction numbers;
+// *labels: 1 trained on integer labels, 0 on float targets
+API void cnb_net_output_layer(void* p, int* activation, int* loss, int* metric, float* weight, int* labels) {
+  const LayerConfig& l = ((NetHandle*)p)->net->Model().layer.back();
   *activation = l.activation; *loss = l.loss_function; *metric = l.performance_metric; *weight = l.loss_function_weight;
   *labels = TakesLabels(l.activation) ? 1 : 0;
-  return 0;
 }
 // one training step; *loss (may be NULL) receives the batch's loss as cnb_net_loss gives it (one scalar D2H)
 API void cnb_net_train_step(void* p, float* loss) { ((NetHandle*)p)->net->TrainOneBatch(loss); }
@@ -209,129 +247,10 @@ API int cnb_plan_buckets(int n_edges, const long long* offsets, const long long*
   for (const Bucket& k : b) { if (n >= cap) break; lo[n] = (long long)k.lo; hi[n] = (long long)k.hi; trigger[n] = k.trigger; n++; }
   return n;
 }
-// a host-only ConvNet (no device memory) of a model, or nullptr with the reason on stderr
-static ConvNet* TryBuildNet(const char* model, int batch) {
-  ModelConfig m;
-  if (!TryBuildModel(model, &m)) return nullptr;
-  try { return new ConvNet(m, batch); }
-  catch (const std::invalid_argument& e) { fprintf(stderr, "convnet_b200 host: %s\n", e.what()); return nullptr; }
-}
-// static description of a model (no device memory): per-edge parameter count, for planning / reporting
-API int cnb_model_edge_params(const char* model, int batch, int cap, long long* sizes) {
-  ConvNet* net = TryBuildNet(model, batch);
-  if (!net) return -1;
-  int n = 0;
-  for (auto& e : net->Edges()) { if (n >= cap) break; sizes[n++] = (long long)e->GetParameterMemoryRequirement(); }
-  delete net;
-  return n;
-}
-// static description of a model: the FLOPs of one forward pass and of one training step at `batch` (FlopsFprop,
-// FlopsTrainStep).  0 ok, -1 unknown model
-API int cnb_model_flops(const char* model, int batch, double* fprop, double* train) {
-  ConvNet* net = TryBuildNet(model, batch);
-  if (!net) return -1;
-  *fprop = net->FlopsFprop();
-  *train = net->FlopsTrainStep();
-  delete net;
-  return 0;
-}
-// static description of a model: the flat parameter buffer (ConvNet::PlanParameters).  Returns the number of edges E
-// (-1: unknown model); fills edge_offsets[0, E) and, per layer, bn_offsets[0, E] (-1: not batch-normalised), each up to
-// `cap` entries, and *total (floats, padding included)
-API int cnb_model_param_layout(const char* model, int batch, int cap, long long* edge_offsets, long long* bn_offsets,
-                               long long* total) {
-  ConvNet* net = TryBuildNet(model, batch);
-  if (!net) return -1;
-  net->PlanParameters();
-  const int n = (int)net->Edges().size();
-  for (int i = 0; i < n && i < cap; i++) edge_offsets[i] = (long long)net->EdgeOffsets()[i];
-  for (int i = 0; i <= n && i < cap; i++) bn_offsets[i] = net->BnOffsets()[i];
-  *total = (long long)net->NumParameters();
-  delete net;
-  return n;
-}
-// static description of a model: the epilogue fusion ConvNet::PlanFusion decides.  Returns the number of edges E (-1:
-// unknown model); fills, up to `cap` entries each, per edge up_act / down_act[0, E) (the CNB_ACT_* code ComputeUp applies,
-// and the one whose derivative ComputeDown applies) and flags[0, E) (Edge::FusionPlan: bit 0 dropout_up, 1 scale_down,
-// 2 sums_bias_below, 3 offers_bias_grad), and per layer passes[0, E] (bit 0: a separate activation pass remains, bit 1:
-// a separate derivative pass remains)
-API int cnb_model_fusion(const char* model, int batch, int cap, int* up_act, int* down_act, int* flags, int* passes) {
-  ConvNet* net = TryBuildNet(model, batch);
-  if (!net) return -1;
-  const int n = (int)net->Edges().size();
-  for (int i = 0; i < n && i < cap; i++) {
-    const Edge::FusionPlan& p = net->Edges()[i]->Plan();
-    up_act[i] = p.up_act; down_act[i] = p.down_act;
-    flags[i] = p.dropout_up | p.scale_down << 1 | p.sums_bias_below << 2 | p.offers_bias_grad << 3;
-  }
-  for (int i = 0; i <= n && i < cap; i++)
-    passes[i] = net->Layers()[i]->HasSeparateActivationPass() | net->Layers()[i]->HasSeparateDerivPass() << 1;
-  delete net;
-  return n;
-}
-// static description of a model's layer `layer`: 1 batch-normalised (then *channels, *bn_f, *bn_epsilon and the gamma /
-// beta optimizers are filled), 0 not, -1 unknown model, -2 layer out of range.  name: 64 bytes, the layer's name
-API int cnb_model_bn_layer(const char* model, int layer, char* name, int* channels, float* bn_f, float* bn_epsilon,
-                           OptimizerConfig* gamma, OptimizerConfig* beta) {
-  ModelConfig m;
-  if (!TryBuildModel(model, &m)) return -1;
-  if (layer < 0 || layer >= (int)m.layer.size()) return -2;
-  const LayerConfig& l = m.layer[layer];
-  strncpy(name, l.name.c_str(), 63); name[63] = 0;
-  if (!l.batch_normalize) return 0;
-  *channels = l.num_channels; *bn_f = l.bn_f; *bn_epsilon = l.bn_epsilon;
-  *gamma = l.gamma_optimizer; *beta = l.beta_optimizer;
-  return 1;
-}
-// static description of a model: the optimizer config of edge `edge` (which: 0 weights, 1 bias).  0 ok, -1 unknown model,
-// -2 edge out of range or without parameters of its own (a tied edge trains with its owner's optimizers)
-API int cnb_model_edge_optimizer(const char* model, int edge, int which, OptimizerConfig* out) {
-  ModelConfig m;
-  if (!TryBuildModel(model, &m)) return -1;
-  if (edge < 0 || edge >= (int)m.edge.size() || which < 0 || which > 1) return -2;
-  const EdgeConfig& e = m.edge[edge];
-  if (e.edge_type == MAXPOOL || e.edge_type == AVGPOOL || e.edge_type == RESPONSE_NORM || (which == 1 && e.has_no_bias) ||
-      !e.tied_to.empty())
-    return -2;
-  *out = which ? e.bias_optimizer : e.weight_optimizer;
-  return 0;
-}
-
-// static description of a model: the name of edge `edge` and, if it is tied, the edge whose parameters it uses (both
-// NUL-terminated, up to 256 bytes).  1 tied, 0 untied, -1 unknown model, -2 edge out of range
-API int cnb_model_tie(const char* model, int edge, char* name, char* owner) {
-  ModelConfig m;
-  if (!TryBuildModel(model, &m)) return -1;
-  if (edge < 0 || edge >= (int)m.edge.size()) return -2;
-  const EdgeConfig& e = m.edge[edge];
-  snprintf(name, 256, "%s", e.name.c_str());
-  snprintf(owner, 256, "%s", e.tied_to.c_str());
-  return e.tied_to.empty() ? 0 : 1;
-}
-
-// static description of a model: frozen edge `edge` (block_backprop, FrozenEdges) and the layer it writes, unless that is the
-// output layer (names NUL-terminated, up to 256 bytes; layer "" for the output).  1 frozen, 0 trained, -1 unknown model
-// or one the host cannot run, -2 edge out of range
-API int cnb_model_frozen(const char* model, int edge, char* name, char* layer) {
-  ConvNet* net = TryBuildNet(model, 1);
-  if (!net) return -1;
-  const int n = (int)net->Edges().size(), frozen = net->NumFrozenEdges();
-  int rc = edge < 0 || edge >= n ? -2 : edge < frozen ? 1 : 0;
-  if (rc == 1) {
-    Layer& l = *net->Layers()[edge + 1];
-    snprintf(name, 256, "%s", net->Edges()[edge]->GetName().c_str());
-    snprintf(layer, 256, "%s", l.IsOutput() ? "" : l.GetName().c_str());
-  }
-  delete net;
-  return rc;
-}
-
-// a model's resolved ModelConfig as a config::Model text proto (ModelText).  Returns its length in bytes (-1: unknown
-// model or unreadable file, the reason on stderr) and writes up to cap - 1 of them and a terminating NUL into buf
-API long long cnb_model_text(const char* model, char* buf, long long cap) {
-  ModelConfig m;
-  if (!TryBuildModel(model, &m)) return -1;
-  const std::string t = ModelText(m);
+// the model as a config::Model text proto (ModelText).  Returns its length in bytes and writes up to cap - 1 of them
+// and a terminating NUL into buf
+API long long cnb_net_model_text(void* p, char* buf, long long cap) {
+  const std::string t = ModelText(((NetHandle*)p)->net->Model());
   if (cap > 0) {
     const size_t n = std::min((size_t)(cap - 1), t.size());
     memcpy(buf, t.data(), n);
@@ -340,45 +259,25 @@ API long long cnb_model_text(const char* model, char* buf, long long cap) {
   return (long long)t.size();
 }
 
-// static description of a model: the initial weights of edge `edge` under RNG seed `seed` (EdgeWithWeight::InitialWeights;
-// the net seeds edge i with its seed + 17 i), or a PRETRAINED edge's weights from its checkpoint.  Returns their number
-// (writes up to `cap`); -1 unknown model or unreadable checkpoint, -2 edge out of range or without parameters of its own
-API long long cnb_model_initial_weights(const char* model, int edge, unsigned seed, float* out, long long cap) {
-  ConvNet* net = TryBuildNet(model, 1);
-  if (!net) return -1;
+// the initial weights of edge `edge` under RNG seed `seed` (EdgeWithWeight::InitialWeights; the net seeds edge i with its
+// seed + 17 i), or a PRETRAINED edge's weights from its checkpoint.  Returns their number (writes up to `cap`); -1 an
+// unreadable checkpoint (cnb_last_error), -2 edge out of range or without parameters of its own
+API long long cnb_net_initial_weights(void* p, int edge, unsigned seed, float* out, long long cap) {
+  ConvNet* net = ((NetHandle*)p)->net;
   EdgeWithWeight* e = edge >= 0 && edge < (int)net->Edges().size() ? dynamic_cast<EdgeWithWeight*>(net->Edges()[edge].get()) : nullptr;
-  long long n = -2;
-  if (e && !e->Tied()) {
-    std::vector<float> w;
-    try {
-      w = e->Config().initialization == PRETRAINED ? PretrainedWeights(e->Config(), e->WeightCount()) : e->InitialWeights(seed);
-    } catch (const std::exception& x) {
-      fprintf(stderr, "convnet_b200 host: %s\n", x.what());
-      delete net;
-      return -1;
-    }
-    n = (long long)w.size();
-    if (cap > 0) memcpy(out, w.data(), sizeof(float) * (size_t)std::min(n, cap));
-  }
-  delete net;
+  if (!e || e->Tied()) return -2;
+  std::vector<float> w;
+  if (Guard([&] {
+        w = e->Config().initialization == PRETRAINED ? PretrainedWeights(e->Config(), e->WeightCount()) : e->InitialWeights(seed);
+      }))
+    return -1;
+  const long long n = (long long)w.size();
+  if (cap > 0) memcpy(out, w.data(), sizeof(float) * (size_t)std::min(n, cap));
   return n;
 }
 
 // ---- checkpoints and Polyak averaging (checkpoint.cc).  Each returns 0, or -1 with the message on stderr and in
 // cnb_last_error()
-static std::string g_last_error;
-API const char* cnb_last_error() { return g_last_error.c_str(); }
-template <class F>
-static int Guard(F f) {
-  try {
-    f();
-    return 0;
-  } catch (const std::exception& e) {
-    g_last_error = e.what();
-    fprintf(stderr, "convnet_b200 host: %s\n", e.what());
-    return -1;
-  }
-}
 API int cnb_net_save(void* p, const char* path) { return Guard([&] { ((NetHandle*)p)->net->Save(path); }); }
 API int cnb_net_load(void* p, const char* path) { return Guard([&] { ((NetHandle*)p)->net->Load(path); }); }
 API long long cnb_net_iteration(void* p) { return (long long)((NetHandle*)p)->net->Iteration(); }
@@ -386,20 +285,14 @@ API int cnb_net_polyak_insert(void* p) { return Guard([&] { ((NetHandle*)p)->net
 API int cnb_net_load_polyak_weights(void* p) { return Guard([&] { ((NetHandle*)p)->net->LoadPolyakWeights(); }); }
 API int cnb_net_load_current_weights(void* p) { return Guard([&] { ((NetHandle*)p)->net->LoadCurrentWeights(); }); }
 API int cnb_net_polyak_count(void* p) { return ((NetHandle*)p)->net->PolyakCount(); }
-// static description of a model: its Polyak settings.  1 Polyak on, 0 off, -1 unknown model
-API int cnb_model_polyak(const char* model, int* after, int* queue_size, int* validate_after, int* save_after) {
-  ModelConfig m;
-  if (!TryBuildModel(model, &m)) return -1;
+// the model's Polyak settings.  1 Polyak on, 0 off
+API int cnb_net_polyak(void* p, int* after, int* queue_size, int* validate_after, int* save_after) {
+  const ModelConfig& m = ((NetHandle*)p)->net->Model();
   *after = m.polyak_after; *queue_size = m.polyak_queue_size; *validate_after = m.validate_after; *save_after = m.save_after;
   return PolyakOn(m) ? 1 : 0;
 }
-// pure host logic: 1 if the reference's loop inserts into the Polyak queue after TrainOneBatch call `iteration` (PolyakDue),
-// 0 if not, -1 unknown model
-API int cnb_polyak_due(const char* model, long long iteration) {
-  ModelConfig m;
-  if (!TryBuildModel(model, &m)) return -1;
-  return PolyakDue(m, iteration) ? 1 : 0;
-}
+// 1 if the reference's loop inserts into the Polyak queue after TrainOneBatch call `iteration` (PolyakDue), else 0
+API int cnb_net_polyak_due(void* p, long long iteration) { return PolyakDue(((NetHandle*)p)->net->Model(), iteration) ? 1 : 0; }
 
 // ---- the device side of the input pipeline (data.h): a GPU-resident chunk + per-minibatch crop / mirror into the net's input
 API void* cnb_data_create(int chunk_size, int channels, int image_size_y, int image_size_x, int gpu_image_size_y,
@@ -481,11 +374,10 @@ API int cnb_handler_last(void* p, int* start, int* multiplicity_id, int* rows, f
   memcpy(noise, h->Noise().Last(), sizeof(float) * 3 * n);
   return n;
 }
-// a model's train_dataset (which 0) or valid_dataset (1): 1 and its fields, 0 when the model has none, -1 unknown model
-API int cnb_model_dataset(const char* model, int which, DatasetOrder* order, int* translate, int* flip, int* gpu_image_size_y,
-                          int* gpu_image_size_x) {
-  ModelConfig m;
-  if (!TryBuildModel(model, &m)) return -1;
+// the model's train_dataset (which 0) or valid_dataset (1): 1 and its fields, 0 when the model has none
+API int cnb_net_dataset(void* p, int which, DatasetOrder* order, int* translate, int* flip, int* gpu_image_size_y,
+                        int* gpu_image_size_x) {
+  const ModelConfig& m = ((NetHandle*)p)->net->Model();
   const ModelConfig::Dataset& d = which ? m.valid_dataset : m.train_dataset;
   *order = d.order; *translate = d.translate; *flip = d.flip;
   *gpu_image_size_y = d.gpu_image_size_y; *gpu_image_size_x = d.gpu_image_size_x;
@@ -493,33 +385,31 @@ API int cnb_model_dataset(const char* model, int which, DatasetOrder* order, int
 }
 
 // ---- the training loop (train.cc).  Host only: a model's schedule, CheckReduceLearningRate and the loop's decisions
-// static description of a model's training schedule: ints = {max_iter, print_after, validate_after, save_after,
-// reduce_lr_num_steps, reduce_lr_max, smaller_is_better}, floats = {reduce_lr_factor, reduce_lr_threshold}, and the
-// NUL-terminated strings reduce_lr_layer_name and checkpoint_dir (up to 4096 bytes each).  0 ok, -1 unknown model
-API int cnb_model_schedule(const char* model, int* ints, float* floats, char* layer_name, char* checkpoint_dir) {
-  ModelConfig m;
-  if (!TryBuildModel(model, &m)) return -1;
+// the model's training schedule: ints = {max_iter, print_after, validate_after, save_after, reduce_lr_num_steps,
+// reduce_lr_max, smaller_is_better}, floats = {reduce_lr_factor, reduce_lr_threshold}, and reduce_lr_layer_name and
+// checkpoint_dir (NUL-terminated, owned by the handle)
+API void cnb_net_schedule(void* p, int* ints, float* floats, const char** layer_name, const char** checkpoint_dir) {
+  const ModelConfig& m = ((NetHandle*)p)->net->Model();
   const int v[] = {m.max_iter, m.print_after, m.validate_after, m.save_after, m.reduce_lr_num_steps, m.reduce_lr_max,
                    m.smaller_is_better ? 1 : 0};
   memcpy(ints, v, sizeof(v));
   floats[0] = m.reduce_lr_factor; floats[1] = m.reduce_lr_threshold;
-  snprintf(layer_name, 4096, "%s", m.reduce_lr_layer_name.c_str());
-  snprintf(checkpoint_dir, 4096, "%s", m.checkpoint_dir.c_str());
-  return 0;
+  *layer_name = m.reduce_lr_layer_name.c_str();
+  *checkpoint_dir = m.checkpoint_dir.c_str();
 }
 API int cnb_reduce_lr_due(const float* history, int len, int num_steps, float threshold, int smaller_is_better) {
   return ReduceLrDue(std::vector<float>(history, history + len), num_steps, threshold, smaller_is_better != 0) ? 1 : 0;
 }
-// ConvNet::Train's decisions without a net, from TrainOneBatch call `start` + 1 to max_iter: per iteration with an action,
+// ConvNet::Train's decisions for the model, from TrainOneBatch call `start` + 1 to max_iter: per iteration with an action,
 // iters[k] and actions[k] (TrainSchedule::Action bits, plus 16: the learning rate is reduced after this validation, 32:
 // this validation runs on the Polyak average), and for the save after the loop a last record (max_iter, 8 | 64).  The
 // validations take the values values[0, n_values) in order.  Returns the number of records (writes up to `cap`); -1 with
-// the reason in cnb_last_error(): a refused schedule or model, or more validations than values
-API long long cnb_train_dry_run(const char* model, long long start, int lr_reduce_counter, int validation_set,
-                                const float* values, int n_values, long long cap, long long* iters, int* actions) {
+// the reason in cnb_last_error(): a refused schedule, or more validations than values
+API long long cnb_net_train_dry_run(void* p, long long start, int lr_reduce_counter, int validation_set,
+                                    const float* values, int n_values, long long cap, long long* iters, int* actions) {
   long long n = 0;
   const int rc = Guard([&] {
-    const ModelConfig m = BuildModel(model);
+    const ModelConfig& m = ((NetHandle*)p)->net->Model();
     TrainSchedule s(m, lr_reduce_counter);
     auto put = [&](long long it, int a) { if (n < cap) { iters[n] = it; actions[n] = a; } n++; };
     int validated = 0;

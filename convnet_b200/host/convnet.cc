@@ -569,8 +569,10 @@ ConvNet::~ConvNet() {
   for (cudaEvent_t e : {trace_.t0, trace_.fwd, trace_.bwd, trace_.end}) if (e) cudaEventDestroy(e);
   for (std::vector<cudaEvent_t>* v : {&trace_.c0, &trace_.c1, &trace_.s1}) for (cudaEvent_t e : *v) cudaEventDestroy(e);
   if (polyak_) cudaFree(polyak_);
-  convnet_b200_reserve_sms(0);
-  convnet_b200_bf16_invalidate(nullptr);                     // the buffers go away; a later net may get the same addresses
+  if (allocated_) {
+    convnet_b200_reserve_sms(0);
+    convnet_b200_bf16_invalidate(nullptr);                   // the buffers go away; a later net may get the same addresses
+  }
 }
 
 // AllocateEdgeMemory (convnet.cc:272-298): one flat buffer, each edge's slice padded to 128 floats.  The [gamma | beta]
@@ -623,6 +625,7 @@ void ConvNet::PlanParameters() {
 }
 
 void ConvNet::AllocateMemory() {
+  allocated_ = true;
   for (auto& l : layers_) l->AllocateMemory(batch_size_);
   PlanParameters();
   size_t total = num_params_;

@@ -353,6 +353,7 @@ class ConvNet {
   // the staged bf16 copies and dgrad banks coherent.  std::runtime_error: an I/O failure
   void Save(const std::string& path);
   void Load(const std::string& path);
+  const ModelConfig& Model() const { return model_; }           // the model the net was built from (Load: its seed)
   ModelConfig CurrentModel() const;                             // the model with the optimizer settings now in force
   unsigned long long Iteration() const { return step_; }        // TrainOneBatch calls so far (the dropout step)
   // the keep-mask seed the next training Fprop gives layer i; 0 for a layer without dropout
@@ -414,6 +415,9 @@ class ConvNet {
   void ResolveTies();
   bool Grouped(size_t i) const;                 // edge i shares its parameters with another edge
   bool prestage_ = true;                       // rebuild the dgrad banks behind each optimizer step (PrestageDown)
+  // AllocateMemory has begun: the net may own staged bf16 copies and an SM reservation, which its destructor drops.  A
+  // host-only net (no AllocateMemory) leaves the library's state to the nets that run
+  bool allocated_ = false;
   Matrix parameters_, grad_parameters_, history_, loss_sum_, state_;
   std::vector<TrainedTensor> tensors_;
   void AllocateAdaptiveState();                 // state_, each tensor's slice initialised for its optimizer

@@ -76,9 +76,12 @@ def load_host():
         H = ct.CDLL(HOST_LIB_PATH)
         vp, i, ll, d, f = ct.c_void_p, ct.c_int, ct.c_longlong, ct.c_double, ct.c_float
         sig = {
+            "cnb_model_open": ([ct.c_char_p, i], vp),
             "cnb_net_create": ([ct.c_char_p, i, ct.c_uint, i], vp), "cnb_net_destroy": ([vp], None),
             "cnb_net_num_params": ([vp], ll), "cnb_net_num_edges": ([vp], i), "cnb_net_edge_name": ([vp, i], ct.c_char_p),
             "cnb_net_edge_flops": ([vp, i], d), "cnb_net_edge_offset": ([vp, i], ll), "cnb_net_edge_size": ([vp, i], ll),
+            "cnb_net_edge_slice": ([vp, i], ll), "cnb_net_edge_fusion": ([vp, i, ct.POINTER(i), ct.POINTER(i)], i),
+            "cnb_net_layer_passes": ([vp, i], i),
             "cnb_net_flops_fprop": ([vp], d), "cnb_net_flops_train": ([vp], d),
             "cnb_net_input": ([vp], vp), "cnb_net_input_floats": ([vp], ll), "cnb_net_labels": ([vp], vp),
             "cnb_net_output": ([vp], vp), "cnb_net_num_classes": ([vp], i), "cnb_net_params": ([vp], vp),
@@ -93,39 +96,31 @@ def load_host():
             "cnb_data_view_offset": ([i, i, i, ct.POINTER(i), ct.POINTER(i)], None),
             "cnb_dp_unique_id": ([ct.c_char_p], i), "cnb_net_dp_init": ([vp, i, i, ct.c_char_p, ll], i),
             "cnb_plan_buckets": ([i, ct.POINTER(ll), ct.POINTER(ll), ll, i, ct.POINTER(ll), ct.POINTER(ll), ct.POINTER(i)], i),
-            "cnb_model_edge_params": ([ct.c_char_p, i, i, ct.POINTER(ll)], i),
             "cnb_net_reduce_learning_rate": ([vp, f], None),
             "cnb_net_set_optimizer": ([vp, ct.c_char_p, ct.POINTER(OptimizerConfig)], i),
             "cnb_net_adaptive_state": ([vp], vp),
-            "cnb_net_get_optimizer_state": ([vp, ct.c_char_p, ct.POINTER(ll), ct.POINTER(f), ct.POINTER(f)], i),
+            "cnb_net_get_optimizer_state": ([vp, ct.c_char_p, ct.POINTER(ll), ct.POINTER(f), ct.POINTER(f),
+                                             ct.POINTER(OptimizerConfig)], ll),
             "cnb_optimizer_schedule": ([ct.POINTER(OptimizerConfig), ll, ct.POINTER(f), ct.POINTER(f)], i),
-            "cnb_model_edge_optimizer": ([ct.c_char_p, i, i, ct.POINTER(OptimizerConfig)], i),
             "cnb_net_grad_check": ([vp, ct.c_uint, i, ct.c_char_p, ct.POINTER(f), ct.POINTER(f), ct.POINTER(f)], i),
             "cnb_net_layer_name": ([vp, i], ct.c_char_p), "cnb_net_layer_channels": ([vp, i], i),
+            "cnb_net_layer_bn": ([vp, i, ct.POINTER(f), ct.POINTER(f)], None),
             "cnb_net_bn_offset": ([vp, i], ll), "cnb_net_bn_stat": ([vp, i, i], vp),
             "cnb_bn_optimizer_check": ([ct.POINTER(OptimizerConfig)], i),
-            "cnb_model_param_layout": ([ct.c_char_p, i, i, ct.POINTER(ll), ct.POINTER(ll), ct.POINTER(ll)], i),
-            "cnb_model_fusion": ([ct.c_char_p, i, i, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i)], i),
-            "cnb_model_bn_layer": ([ct.c_char_p, i, ct.c_char_p, ct.POINTER(i), ct.POINTER(f), ct.POINTER(f),
-                                    ct.POINTER(OptimizerConfig), ct.POINTER(OptimizerConfig)], i),
             "cnb_net_targets": ([vp], vp), "cnb_net_targets_floats": ([vp], ll), "cnb_net_metric": ([vp], f),
-            "cnb_model_output_layer": ([ct.c_char_p, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(f),
-                                        ct.POINTER(i)], i),
-            "cnb_model_text": ([ct.c_char_p, ct.c_char_p, ll], ll),
-            "cnb_model_initial_weights": ([ct.c_char_p, i, ct.c_uint, ct.POINTER(f), ll], ll),
+            "cnb_net_output_layer": ([vp, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(f), ct.POINTER(i)], None),
+            "cnb_net_model_text": ([vp, ct.c_char_p, ll], ll),
+            "cnb_net_initial_weights": ([vp, i, ct.c_uint, ct.POINTER(f), ll], ll),
             "cnb_net_history": ([vp], vp), "cnb_last_error": ([], ct.c_char_p), "cnb_net_save": ([vp, ct.c_char_p], i),
             "cnb_net_load": ([vp, ct.c_char_p], i), "cnb_net_iteration": ([vp], ll),
             "cnb_net_polyak_insert": ([vp], i), "cnb_net_load_polyak_weights": ([vp], i),
             "cnb_net_load_current_weights": ([vp], i), "cnb_net_polyak_count": ([vp], i),
-            "cnb_model_polyak": ([ct.c_char_p, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i)], i),
-            "cnb_polyak_due": ([ct.c_char_p, ll], i),
+            "cnb_net_polyak": ([vp, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i)], i),
+            "cnb_net_polyak_due": ([vp, ll], i),
             "cnb_net_edge_tied_to": ([vp, i], ct.c_char_p),
             "cnb_net_layer_deriv": ([vp, i], vp),
-            "cnb_model_tie": ([ct.c_char_p, i, ct.c_char_p, ct.c_char_p], i),
             "cnb_net_dropout_seed": ([vp, i], ct.c_ulonglong),
             "cnb_net_frozen_edges": ([vp, ct.POINTER(ll)], i),
-            "cnb_model_frozen": ([ct.c_char_p, i, ct.c_char_p, ct.c_char_p], i),
-            "cnb_model_flops": ([ct.c_char_p, i, ct.POINTER(d), ct.POINTER(d)], i),
             "cnb_schedule_create": ([ct.POINTER(DatasetOrder), i, ct.c_ulonglong], vp), "cnb_schedule_destroy": ([vp], None),
             "cnb_schedule_chunk_size": ([vp], i),
             "cnb_schedule_next": ([vp, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i)], i),
@@ -133,11 +128,11 @@ def load_host():
             "cnb_handler_create": ([ct.POINTER(DatasetOrder), i, i, i, i, i, i, i, i, vp, vp, vp, i, ct.c_ulonglong], vp),
             "cnb_handler_destroy": ([vp], None), "cnb_handler_get_batch": ([vp, vp], i), "cnb_handler_seek": ([vp, i], i),
             "cnb_handler_last": ([vp, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(f)], i),
-            "cnb_model_dataset": ([ct.c_char_p, i, ct.POINTER(DatasetOrder), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i),
-                                   ct.POINTER(i)], i),
-            "cnb_model_schedule": ([ct.c_char_p, ct.POINTER(i), ct.POINTER(f), ct.c_char_p, ct.c_char_p], i),
+            "cnb_net_dataset": ([vp, i, ct.POINTER(DatasetOrder), ct.POINTER(i), ct.POINTER(i), ct.POINTER(i),
+                                 ct.POINTER(i)], i),
+            "cnb_net_schedule": ([vp, ct.POINTER(i), ct.POINTER(f), ct.POINTER(ct.c_char_p), ct.POINTER(ct.c_char_p)], None),
             "cnb_reduce_lr_due": ([ct.POINTER(f), i, i, f, i], i),
-            "cnb_train_dry_run": ([ct.c_char_p, ll, i, i, ct.POINTER(f), i, ll, ct.POINTER(ll), ct.POINTER(i)], ll),
+            "cnb_net_train_dry_run": ([vp, ll, i, i, ct.POINTER(f), i, ll, ct.POINTER(ll), ct.POINTER(i)], ll),
             "cnb_net_validate": ([vp, vp, ct.POINTER(f)], i),
             "cnb_net_train": ([vp, vp, vp, ct.c_char_p, ct.c_char_p], i),
             "cnb_net_train_event": ([vp, i, ct.POINTER(ll), ct.POINTER(i), ct.POINTER(f), ct.POINTER(i), ct.POINTER(i)], i),
@@ -150,7 +145,80 @@ def load_host():
     return _host
 
 
-class Net:
+class Model:
+    """A model's chain built on the host only, for describing it: its edges, layers, parameter layout, fusion plan and
+    FLOPs at `batch`, without device memory.  `model` is a built-in name or a model file, with suffixes, as for Net.  A
+    model that cannot be read or run raises ValueError with the reason (for a file: its line and field)."""
+
+    def __init__(self, model, batch=1):
+        self._open(model, batch, load_host().cnb_model_open(model.encode(), batch))
+
+    def _open(self, model, batch, h):
+        self.H, self.h, self.model, self.batch_size = load_host(), h, model, batch
+        if not h:
+            raise ValueError(self.H.cnb_last_error().decode())
+
+    def close(self):
+        if self.h:
+            self.H.cnb_net_destroy(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    num_params = property(lambda s: s.H.cnb_net_num_params(s.h))
+    flops_fprop = property(lambda s: s.H.cnb_net_flops_fprop(s.h))
+    flops_train = property(lambda s: s.H.cnb_net_flops_train(s.h))
+
+    def _frozen(self):
+        off = ct.c_longlong(0)
+        return self.H.cnb_net_frozen_edges(self.h, ct.byref(off)), off.value
+
+    trained_offset = property(lambda s: s._frozen()[1],
+                              doc="floats at the start of params_tensor() held by frozen edges and layers, which nothing trains")
+
+    def edges(self):
+        return [(self.H.cnb_net_edge_name(self.h, i).decode(), self.H.cnb_net_edge_flops(self.h, i),
+                 self.H.cnb_net_edge_offset(self.h, i), self.H.cnb_net_edge_size(self.h, i))
+                for i in range(self.H.cnb_net_num_edges(self.h))]
+
+    def _edge_name(self, edge):
+        """the name of `edge` (index or name); "" for an index out of range, whose tensors the host then does not find.
+        ValueError for a tied edge, whose optimizers are its owner's"""
+        names = [e[0] for e in self.edges()]
+        if isinstance(edge, str):
+            if edge not in names:
+                raise KeyError("no edge %r (edges: %s)" % (edge, ", ".join(names)))
+            i = names.index(edge)
+        elif 0 <= int(edge) < len(names):
+            i = int(edge)
+        else:
+            return ""
+        owner = self.H.cnb_net_edge_tied_to(self.h, i).decode()
+        if owner:
+            raise ValueError("edge %r is tied to %r: its weights, bias and optimizers are those of %r" % (edge, owner, owner))
+        return names[i]
+
+    def bn_layers(self):
+        """[(layer index, name, channels, offset of [gamma | beta] in params_tensor())] of the batch-normalised layers"""
+        out = []
+        for i in range(self.H.cnb_net_num_layers(self.h)):
+            off = self.H.cnb_net_bn_offset(self.h, i)
+            if off >= 0:
+                out.append((i, self.H.cnb_net_layer_name(self.h, i).decode(), self.H.cnb_net_layer_channels(self.h, i), off))
+        return out
+
+    def _optimizer_config(self, tensor):
+        """the optimizer settings (a dict) of trained tensor `tensor`; None when there is none or it holds no floats"""
+        c, step, v = OptimizerConfig(), ct.c_longlong(0), ct.c_float(0)
+        n = self.H.cnb_net_get_optimizer_state(self.h, tensor.encode(), ct.byref(step), ct.byref(v), ct.byref(v), ct.byref(c))
+        return c.to_dict() if n > 0 else None
+
+
+class Net(Model):
     """A chain ConvNet built natively, from a built-in name ("alexnet" | "lenet" | "c3d" | "tiny" | "lcnet" | "gradcheck" |
     "logcheck" | "localcheck" | "tiednet" | "tiedcheck" | "updown" | "updowncheck") or from a model file: any name ending in ".pbtxt" is the path of a config::Model text proto
     as the reference writes them (examples/*/net.pbtxt), read with the proto's defaults (model_text() prints any model
@@ -170,7 +238,7 @@ class Net:
     One output suffix at most: "+squared-error" (LINEAR output, SQUARED_ERROR), "+binary-ce" (LOGISTIC output,
     CROSS_ENTROPY_BINARY, metric CLASSIFICATION_BINARY), "+soft-targets" (SOFTMAX_DIST, CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED);
     such outputs train on targets_tensor() instead of labels_tensor().  "logcheck": the gradcheck net with logistic units.
-    A model that cannot be read or run raises ValueError; the reason (for a file: its line and field) is on stderr.
+    A model that cannot be read or run raises ValueError with the reason (for a file: its line and field), as Model does.
 
     Tied edges (the reference's Edge.tied_to, see model_ties()) run with their owner's weights and bias and add their
     gradients to the owner's: they own no parameters (edges() reports size 0 and the owner's offset), and the owner's
@@ -194,36 +262,10 @@ class Net:
     trained trunk."""
 
     def __init__(self, model, batch_size, seed=42, grad_checker=False):
-        self.H = load_host()
-        self.h = self.H.cnb_net_create(model.encode(), batch_size, seed, int(grad_checker))
-        if not self.h:
-            raise ValueError("cannot build model %r (see stderr)" % model)
-        self.batch_size = batch_size
-        self.model = model
+        self._open(model, batch_size, load_host().cnb_net_create(model.encode(), batch_size, seed, int(grad_checker)))
 
-    def close(self):
-        if self.h:
-            self.H.cnb_net_destroy(self.h)
-            self.h = None
-
-    # --- sizes
-    num_params = property(lambda s: s.H.cnb_net_num_params(s.h))
     num_classes = property(lambda s: s.H.cnb_net_num_classes(s.h))
     input_floats = property(lambda s: s.H.cnb_net_input_floats(s.h))
-    flops_fprop = property(lambda s: s.H.cnb_net_flops_fprop(s.h))
-    flops_train = property(lambda s: s.H.cnb_net_flops_train(s.h))
-
-    def _frozen(self):
-        off = ct.c_longlong(0)
-        return self.H.cnb_net_frozen_edges(self.h, ct.byref(off)), off.value
-
-    trained_offset = property(lambda s: s._frozen()[1],
-                              doc="floats at the start of params_tensor() held by frozen edges and layers, which nothing trains")
-
-    def edges(self):
-        return [(self.H.cnb_net_edge_name(self.h, i).decode(), self.H.cnb_net_edge_flops(self.h, i),
-                 self.H.cnb_net_edge_offset(self.h, i), self.H.cnb_net_edge_size(self.h, i))
-                for i in range(self.H.cnb_net_num_edges(self.h))]
 
     # --- device buffers as torch tensors (zero-copy views)
     def _view(self, ptr, n, dtype):
@@ -310,25 +352,8 @@ class Net:
 
     def _optimizer_state(self, tensor):
         step, eps, mom = ct.c_longlong(0), ct.c_float(0), ct.c_float(0)
-        rc = self.H.cnb_net_get_optimizer_state(self.h, tensor.encode(), ct.byref(step), ct.byref(eps), ct.byref(mom))
-        return {"step": step.value, "epsilon": eps.value, "momentum": mom.value} if rc == 0 else None
-
-    def _edge_name(self, edge):
-        """the name of `edge` (index or name); "" for an index out of range, whose tensors the host then does not find.
-        ValueError for a tied edge, whose optimizers are its owner's"""
-        names = [e[0] for e in self.edges()]
-        if isinstance(edge, str):
-            if edge not in names:
-                raise KeyError("no edge %r (edges: %s)" % (edge, ", ".join(names)))
-            i = names.index(edge)
-        elif 0 <= int(edge) < len(names):
-            i = int(edge)
-        else:
-            return ""
-        owner = self.H.cnb_net_edge_tied_to(self.h, i).decode()
-        if owner:
-            raise ValueError("edge %r is tied to %r: its weights, bias and optimizers are those of %r" % (edge, owner, owner))
-        return names[i]
+        n = self.H.cnb_net_get_optimizer_state(self.h, tensor.encode(), ct.byref(step), ct.byref(eps), ct.byref(mom), None)
+        return {"step": step.value, "epsilon": eps.value, "momentum": mom.value} if n >= 0 else None
 
     def set_optimizer(self, edge, weights=None, bias=None):
         """replace the settings of the weight and / or bias optimizer of `edge` (index or name) with the optimizer block
@@ -358,15 +383,6 @@ class Net:
         self.H.cnb_net_reduce_learning_rate(self.h, factor)
 
     # --- batch normalisation (Layer::ApplyBatchNormalization, src/layer.cc:452-510)
-    def bn_layers(self):
-        """[(layer index, name, channels, offset of [gamma | beta] in params_tensor())] of the batch-normalised layers"""
-        out = []
-        for i in range(self.H.cnb_net_num_layers(self.h)):
-            off = self.H.cnb_net_bn_offset(self.h, i)
-            if off >= 0:
-                out.append((i, self.H.cnb_net_layer_name(self.h, i).decode(), self.H.cnb_net_layer_channels(self.h, i), off))
-        return out
-
     def _bn_layer(self, layer):
         for entry in self.bn_layers():
             if layer in (entry[0], entry[1]):
@@ -500,40 +516,31 @@ class Net:
 
 def model_edge_params(model, batch=1):
     """parameter count of every edge of a model (host-only: no device memory is touched)."""
-    H = load_host()
-    buf = (ct.c_longlong * 64)()
-    n = H.cnb_model_edge_params(model.encode(), batch, 64, buf)
-    if n < 0:
-        raise ValueError("unknown model %r (see stderr)" % model)
-    return [buf[k] for k in range(n)]
+    with Model(model, batch) as m:
+        return [e[3] for e in m.edges()]
 
 
 def model_edge_optimizer(model, edge, which="weights"):
     """the optimizer config (dict of proto field names) a model gives edge `edge` (host-only); None for an edge without
     parameters"""
-    c = OptimizerConfig()
-    rc = load_host().cnb_model_edge_optimizer(model.encode(), edge, {"weights": 0, "bias": 1}[which], ct.byref(c))
-    if rc == -1:
-        raise ValueError("unknown model %r (see stderr)" % model)
-    return c.to_dict() if rc == 0 else None
+    kind = {"weights": ":weight", "bias": ":bias"}[which]
+    with Model(model) as m:
+        names = [e[0] for e in m.edges()]
+        return m._optimizer_config(names[edge] + kind) if 0 <= edge < len(names) else None
 
 
 def model_bn_layers(model):
     """the batch-normalised layers of a model (host-only): [{"layer", "name", "channels", "bn_f", "bn_epsilon",
     "gamma_optimizer", "beta_optimizer"}] in chain order"""
-    H, out, i = load_host(), [], 0
-    while True:
-        name, ch, f_, eps = ct.create_string_buffer(64), ct.c_int(0), ct.c_float(0), ct.c_float(0)
-        g, b = OptimizerConfig(), OptimizerConfig()
-        rc = H.cnb_model_bn_layer(model.encode(), i, name, ct.byref(ch), ct.byref(f_), ct.byref(eps), ct.byref(g), ct.byref(b))
-        if rc == -1:
-            raise ValueError("unknown model %r (see stderr)" % model)
-        if rc == -2:
-            return out
-        if rc == 1:
-            out.append({"layer": i, "name": name.value.decode(), "channels": ch.value, "bn_f": f_.value,
-                        "bn_epsilon": eps.value, "gamma_optimizer": g.to_dict(), "beta_optimizer": b.to_dict()})
-        i += 1
+    out = []
+    with Model(model) as m:
+        for i, name, channels, _ in m.bn_layers():
+            f_, eps = ct.c_float(0), ct.c_float(0)
+            m.H.cnb_net_layer_bn(m.h, i, ct.byref(f_), ct.byref(eps))
+            out.append({"layer": i, "name": name, "channels": channels, "bn_f": f_.value, "bn_epsilon": eps.value,
+                        "gamma_optimizer": m._optimizer_config(name + ":gamma"),
+                        "beta_optimizer": m._optimizer_config(name + ":beta")})
+    return out
 
 
 ACTIVATIONS = ("LINEAR", "RECTIFIED_LINEAR", "SOFTMAX", "LOGISTIC", "SOFTMAX_DIST")
@@ -546,8 +553,8 @@ def model_output_layer(model):
     """the output layer a model configures (host-only): {"activation", "loss_function", "performance_metric" (names),
     "loss_function_weight", "labels" (True: trained on integer labels, False: on float targets)}"""
     a, lf, pm, lab, w = ct.c_int(0), ct.c_int(0), ct.c_int(0), ct.c_int(0), ct.c_float(0)
-    if load_host().cnb_model_output_layer(model.encode(), ct.byref(a), ct.byref(lf), ct.byref(pm), ct.byref(w), ct.byref(lab)):
-        raise ValueError("unknown model %r (see stderr)" % model)
+    with Model(model) as m:
+        m.H.cnb_net_output_layer(m.h, ct.byref(a), ct.byref(lf), ct.byref(pm), ct.byref(w), ct.byref(lab))
     return {"activation": ACTIVATIONS[a.value], "loss_function": LOSS_FUNCTIONS[lf.value],
             "performance_metric": LOSS_FUNCTIONS[pm.value], "loss_function_weight": w.value, "labels": bool(lab.value)}
 
@@ -556,101 +563,73 @@ def model_text(model):
     """the resolved configuration of a model (built-in, suffixed or file) as a config::Model text proto: every field the
     host reads for each layer and edge explicit, floats printed so that they read back bit-exactly.  Written to a file
     ending in ".pbtxt", it builds the same model."""
-    H, cap = load_host(), 1 << 16
-    while True:
-        buf = ct.create_string_buffer(cap)
-        n = H.cnb_model_text(model.encode(), buf, cap)
-        if n < 0:
-            raise ValueError("cannot read model %r (see stderr)" % model)
-        if n < cap:
-            return buf.value.decode()
-        cap = n + 1
+    with Model(model) as m:
+        n = m.H.cnb_net_model_text(m.h, None, 0)
+        buf = ct.create_string_buffer(n + 1)
+        m.H.cnb_net_model_text(m.h, buf, n + 1)
+    return buf.value.decode()
 
 
 def model_initial_weights(model, edge, seed=42):
     """the initial weights (a list of floats, without the bias) of edge `edge` of a model under RNG seed `seed`
     (host-only; the net seeds edge i with its seed + 17 i), or a PRETRAINED edge's weights from its checkpoint; None for
     an edge without parameters of its own (a tied edge starts from its owner's)"""
-    H = load_host()
-    n = H.cnb_model_initial_weights(model.encode(), edge, seed, None, 0)
-    if n == -1:
-        raise ValueError("cannot build model %r (see stderr)" % model)
-    if n < 0:
-        return None
-    buf = (ct.c_float * n)()
-    H.cnb_model_initial_weights(model.encode(), edge, seed, buf, n)
+    with Model(model) as m:
+        n = m.H.cnb_net_initial_weights(m.h, edge, seed, None, 0)
+        if n == -1:
+            raise ValueError(m.H.cnb_last_error().decode())
+        if n < 0:
+            return None
+        buf = (ct.c_float * n)()
+        m.H.cnb_net_initial_weights(m.h, edge, seed, buf, n)
     return list(buf)
 
 
 def model_ties(model):
     """the tied edges of a model (host-only): {tied edge name: the name of the edge whose parameters it uses}"""
-    H, out, i = load_host(), {}, 0
-    while True:
-        name, owner = ct.create_string_buffer(256), ct.create_string_buffer(256)
-        rc = H.cnb_model_tie(model.encode(), i, name, owner)
-        if rc == -1:
-            raise ValueError("cannot build model %r (see stderr)" % model)
-        if rc == -2:
-            return out
-        if rc == 1:
-            out[name.value.decode()] = owner.value.decode()
-        i += 1
+    with Model(model) as m:
+        owners = [(e[0], m.H.cnb_net_edge_tied_to(m.h, i).decode()) for i, e in enumerate(m.edges())]
+    return {name: owner for name, owner in owners if owner}
 
 
 def model_flops(model, batch):
     """{"fprop", "train"}: the FLOPs of one forward pass and of one training step of a model at `batch` (host-only; the
     flops_fprop / flops_train of a Net)"""
-    fprop, train = ct.c_double(0), ct.c_double(0)
-    if load_host().cnb_model_flops(model.encode(), batch, ct.byref(fprop), ct.byref(train)):
-        raise ValueError("cannot build model %r (see stderr)" % model)
-    return {"fprop": fprop.value, "train": train.value}
+    with Model(model, batch) as m:
+        return {"fprop": m.flops_fprop, "train": m.flops_train}
 
 
 def model_frozen(model):
     """the frozen part of a model (host-only): {"edges": the blocked edges and those below them, "layers": the hidden layers
     they write}, in chain order"""
-    H, out, i = load_host(), {"edges": [], "layers": []}, 0
-    while True:
-        name, layer = ct.create_string_buffer(256), ct.create_string_buffer(256)
-        rc = H.cnb_model_frozen(model.encode(), i, name, layer)
-        if rc == -1:
-            raise ValueError("cannot build model %r (see stderr)" % model)
-        if rc != 1:
-            return out
-        out["edges"].append(name.value.decode())
-        if layer.value:
-            out["layers"].append(layer.value.decode())
-        i += 1
+    with Model(model) as m:
+        n, layers = m._frozen()[0], m.H.cnb_net_num_layers(m.h)
+        return {"edges": [e[0] for e in m.edges()[:n]],
+                "layers": [m.H.cnb_net_layer_name(m.h, i).decode() for i in range(1, n + 1) if i < layers - 1]}
 
 
 def model_polyak(model):
     """a model's Polyak averaging (host-only): None when it is off, else {"polyak_after", "polyak_queue_size",
     "validate_after", "save_after"}"""
     v = [ct.c_int(0) for _ in range(4)]
-    rc = load_host().cnb_model_polyak(model.encode(), *[ct.byref(x) for x in v])
-    if rc < 0:
-        raise ValueError("cannot build model %r (see stderr)" % model)
-    return dict(zip(("polyak_after", "polyak_queue_size", "validate_after", "save_after"), (x.value for x in v))) if rc else None
+    with Model(model) as m:
+        on = m.H.cnb_net_polyak(m.h, *[ct.byref(x) for x in v])
+    return dict(zip(("polyak_after", "polyak_queue_size", "validate_after", "save_after"), (x.value for x in v))) if on else None
 
 
 def polyak_due(model, iteration):
     """whether the reference's training loop inserts into the Polyak queue after train_step number `iteration`"""
-    rc = load_host().cnb_polyak_due(model.encode(), iteration)
-    if rc < 0:
-        raise ValueError("cannot build model %r (see stderr)" % model)
-    return bool(rc)
+    with Model(model) as m:
+        return bool(m.H.cnb_net_polyak_due(m.h, iteration))
 
 
 def model_param_layout(model, batch=1):
     """the flat parameter buffer of a model (host-only): {"edge_offsets": [...], "bn_offsets": per layer (None: not
     batch-normalised), "total": floats with padding}"""
-    cap = 256
-    eo, bo, total = (ct.c_longlong * cap)(), (ct.c_longlong * cap)(), ct.c_longlong(0)
-    n = load_host().cnb_model_param_layout(model.encode(), batch, cap, eo, bo, ct.byref(total))
-    if n < 0:
-        raise ValueError("cannot build model %r (see stderr)" % model)
-    return {"edge_offsets": [eo[k] for k in range(n)], "bn_offsets": [bo[k] if bo[k] >= 0 else None for k in range(n + 1)],
-            "total": total.value}
+    with Model(model, batch) as m:
+        bn = [m.H.cnb_net_bn_offset(m.h, i) for i in range(m.H.cnb_net_num_layers(m.h))]
+        return {"edge_offsets": [m.H.cnb_net_edge_slice(m.h, i) for i in range(m.H.cnb_net_num_edges(m.h))],
+                "bn_offsets": [off if off >= 0 else None for off in bn], "total": m.num_params}
 
 
 FUSION_FLAGS = ("dropout_up", "scale_down", "sums_bias_below", "offers_bias_grad")
@@ -660,15 +639,15 @@ def model_fusion(model, batch=1):
     """the epilogue fusion plan of a model (host-only): {"edges": per edge {"up_act", "down_act" (CNB_ACT_* codes: 0 none,
     1 ReLU, 2 logistic), "dropout_up", "scale_down", "sums_bias_below", "offers_bias_grad"}, "layers": per layer
     {"activation_pass", "deriv_pass"} (True: a separate pass remains)}"""
-    cap = 256
-    up, down, flags, passes = [(ct.c_int * cap)() for _ in range(4)]
-    n = load_host().cnb_model_fusion(model.encode(), batch, cap, up, down, flags, passes)
-    if n < 0:
-        raise ValueError("cannot build model %r (see stderr)" % model)
-    edges = [dict(up_act=up[k], down_act=down[k], **{f: bool(flags[k] >> b & 1) for b, f in enumerate(FUSION_FLAGS)})
-             for k in range(n)]
-    layers = [{"activation_pass": bool(passes[k] & 1), "deriv_pass": bool(passes[k] & 2)} for k in range(n + 1)]
-    return {"edges": edges, "layers": layers}
+    edges = []
+    with Model(model, batch) as m:
+        for i in range(m.H.cnb_net_num_edges(m.h)):
+            up, down = ct.c_int(0), ct.c_int(0)
+            flags = m.H.cnb_net_edge_fusion(m.h, i, ct.byref(up), ct.byref(down))
+            edges.append(dict(up_act=up.value, down_act=down.value,
+                              **{f: bool(flags >> b & 1) for b, f in enumerate(FUSION_FLAGS)}))
+        passes = [m.H.cnb_net_layer_passes(m.h, i) for i in range(m.H.cnb_net_num_layers(m.h))]
+    return {"edges": edges, "layers": [{"activation_pass": bool(p & 1), "deriv_pass": bool(p & 2)} for p in passes]}
 
 
 def check_bn_optimizer(config):
@@ -865,11 +844,10 @@ def model_dataset(model, which="train_dataset"):
     (DatasetOrder names) with translate, flip, gpu_image_size_y and gpu_image_size_x (0: not set) of the data stream that
     feeds the input layer"""
     o, v = DatasetOrder(), [ct.c_int(0) for _ in range(4)]
-    rc = load_host().cnb_model_dataset(model.encode(), {"train_dataset": 0, "valid_dataset": 1}[which], ct.byref(o),
-                                       *[ct.byref(x) for x in v])
-    if rc < 0:
-        raise ValueError("cannot build model %r (see stderr)" % model)
-    if rc == 0:
+    with Model(model) as m:
+        present = m.H.cnb_net_dataset(m.h, {"train_dataset": 0, "valid_dataset": 1}[which], ct.byref(o),
+                                      *[ct.byref(x) for x in v])
+    if not present:
         return None
     d = {k: (bool(x) if k in ("pipeline_loads", "randomize_cpu", "randomize_gpu") else x) for k, x in o.to_dict().items()}
     d.update(zip(("translate", "flip", "gpu_image_size_y", "gpu_image_size_x"), (bool(v[0].value), bool(v[1].value),
@@ -885,14 +863,14 @@ def model_schedule(model):
     """a model's training schedule (host-only), the fields Net.train reads, at the proto's defaults where unset:
     {"max_iter", "print_after", "validate_after", "save_after", "reduce_lr_factor", "reduce_lr_threshold",
     "reduce_lr_num_steps", "reduce_lr_max", "smaller_is_better", "reduce_lr_layer_name", "checkpoint_dir"}"""
-    ints, floats = (ct.c_int * 7)(), (ct.c_float * 2)()
-    layer, cdir = ct.create_string_buffer(4096), ct.create_string_buffer(4096)
-    if load_host().cnb_model_schedule(model.encode(), ints, floats, layer, cdir):
-        raise ValueError("cannot build model %r (see stderr)" % model)
+    ints, floats, layer, cdir = (ct.c_int * 7)(), (ct.c_float * 2)(), ct.c_char_p(), ct.c_char_p()
+    with Model(model) as m:
+        m.H.cnb_net_schedule(m.h, ints, floats, ct.byref(layer), ct.byref(cdir))
+        layer, cdir = layer.value, cdir.value
     out = dict(zip(SCHEDULE_INTS, ints))
     out["smaller_is_better"] = bool(out["smaller_is_better"])
-    out.update(reduce_lr_factor=floats[0], reduce_lr_threshold=floats[1], reduce_lr_layer_name=layer.value.decode(),
-               checkpoint_dir=os.fsdecode(cdir.value))
+    out.update(reduce_lr_factor=floats[0], reduce_lr_threshold=floats[1], reduce_lr_layer_name=layer.decode(),
+               checkpoint_dir=os.fsdecode(cdir))
     return out
 
 
@@ -915,19 +893,19 @@ def train_dry_run(model, valid_values=None, *, iteration=0, lr_reduce_counter=0)
     "lr_reduced" (after this validation), "polyak" (this validation runs on the Polyak average).  The checkpoint after
     the loop is a last record (max_iter, {"save", "final"}).  valid_values: the validation values, in order (None: no
     validation set).  ValueError for a schedule Net.train refuses, or fewer values than validations."""
-    H = load_host()
     vals = list(valid_values or [])
     fv = (ct.c_float * max(1, len(vals)))(*vals)
     cap = 1024
-    while True:
-        its, acts = (ct.c_longlong * cap)(), (ct.c_int * cap)()
-        n = H.cnb_train_dry_run(model.encode(), iteration, lr_reduce_counter, int(valid_values is not None), fv, len(vals),
-                                cap, its, acts)
-        if n < 0:
-            raise ValueError(H.cnb_last_error().decode())
-        if n <= cap:
-            return [(its[k], {a for b, a in enumerate(TRAIN_ACTIONS) if acts[k] >> b & 1}) for k in range(n)]
-        cap = n
+    with Model(model) as m:
+        while True:
+            its, acts = (ct.c_longlong * cap)(), (ct.c_int * cap)()
+            n = m.H.cnb_net_train_dry_run(m.h, iteration, lr_reduce_counter, int(valid_values is not None), fv, len(vals),
+                                          cap, its, acts)
+            if n < 0:
+                raise ValueError(m.H.cnb_last_error().decode())
+            if n <= cap:
+                return [(its[k], {a for b, a in enumerate(TRAIN_ACTIONS) if acts[k] >> b & 1}) for k in range(n)]
+            cap = n
 
 
 Net.model_output_layer = staticmethod(model_output_layer)

@@ -36,12 +36,13 @@ def write(tmp_path, text, name="net.pbtxt"):
 def refused(tmp_path, capfd, text, line, *words):
     path = write(tmp_path, text)
     capfd.readouterr()
-    with pytest.raises(ValueError):
+    with pytest.raises(ValueError) as e:
         N.model_text(path)
     err = capfd.readouterr().err
-    assert "%s:%d:" % (path, line) in err, err
-    for w in words:
-        assert w in err, (w, err)
+    for text in (err, str(e.value)):
+        assert "%s:%d:" % (path, line) in text, text
+        for w in words:
+            assert w in text, (w, text)
 
 
 # ------------------------------------------------------------------------------------------------------ Polyak

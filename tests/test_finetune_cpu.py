@@ -38,12 +38,13 @@ def edge_blocks(text):
 
 def refused(tmp_path, capfd, path, file, line, *words):
     capfd.readouterr()
-    with pytest.raises(ValueError):
+    with pytest.raises(ValueError) as e:
         N.model_text(path)
     err = capfd.readouterr().err
-    assert "%s:%d:" % (file, line) in err, err
-    for w in words:
-        assert w in err, (w, err)
+    for text in (err, str(e.value)):
+        assert "%s:%d:" % (file, line) in text, text
+        for w in words:
+            assert w in text, (w, text)
 
 
 # ------------------------------------------------------------------------------------------------ built-in models

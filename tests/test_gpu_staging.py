@@ -240,3 +240,27 @@ def test_prestaged_dgrad_banks_are_used_and_dropped_on_weight_writes():
     finally:
         L.convnet_b200_bf16_invalidate(None)
         lib.set_precision("fp32")
+
+
+def test_describing_a_model_keeps_a_live_nets_copies():
+    """a host-only Model (here through model_flops) touches no library state: the bf16 copies of the weights that a
+    training step staged for the next forward pass stay staged."""
+    from convnet_b200 import lib
+    from convnet_b200 import net as N
+    L = lib.load()
+    lib.set_precision("bf16")
+    net = N.Net("alexnet", 32, seed=3)
+    try:
+        base = net.params_tensor().data_ptr()                   # (taking the pointer drops the copies: before the step)
+        net.input_tensor().normal_()
+        net.labels_tensor().zero_()
+        net.train_step(False)
+        staged = lambda: [name for name, _, off, size in net.edges() if size and L.convnet_b200_bf16_is_staged(base + 4 * off, 1)]
+        before = staged()
+        assert before
+        N.model_flops("alexnet", 32)
+        assert staged() == before
+    finally:
+        net.close()
+        L.convnet_b200_bf16_invalidate(None)
+        lib.set_precision("fp32")

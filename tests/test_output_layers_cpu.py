@@ -70,9 +70,10 @@ def test_logcheck_is_gradcheck_with_logistic_units():
     ("gradcheck+logistic", "+logistic finds no RECTIFIED_LINEAR hidden layer"),
     ("tiny+logistic+logistic", "+logistic finds no RECTIFIED_LINEAR hidden layer")])
 def test_refusals(model, message, capfd):
-    with pytest.raises(ValueError):
+    with pytest.raises(ValueError) as e:
         N.model_param_layout(model)
     assert message in capfd.readouterr().err
+    assert message in str(e.value)
 
 
 # tiny's model text with fields of one layer changed; the refusal names the line of `field`
@@ -102,9 +103,10 @@ def test_refusals_in_a_model_file(tmp_path, capfd, layer, changes, field, messag
         k += 1
     path = tmp_path / "tiny.pbtxt"
     path.write_text("".join(lines))
-    with pytest.raises(ValueError):
+    with pytest.raises(ValueError) as e:
         N.model_param_layout(str(path))
     assert "%s:%d: %s" % (path, at[field], message) in capfd.readouterr().err
+    assert "%s:%d: %s" % (path, at[field], message) in str(e.value)
 
 
 def test_loss_codes_follow_the_proto():

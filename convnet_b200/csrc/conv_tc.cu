@@ -28,6 +28,7 @@
 #include <cudaTypedefs.h>
 
 #include <algorithm>
+#include <type_traits>
 #include <vector>
 
 #include "conv_kernels.h"
@@ -404,79 +405,89 @@ __device__ __forceinline__ void store_tiles(const TcParams& p, SmemCtl* ctl, uin
     if (batches > 0) load_batch(0);
     ptx::mbar_wait(&ctl->epi_full, phase);
     if (batches == 0 && lane == 0) ptx::mbar_arrive(&ctl->epi_empty);
-    for (int b = 0; b < batches; b++) {
-      const int c0 = sw + kStoreWarps * kEpiCols * b;
-      float bv[kEpiCols];
+    // The batches, compiled twice: LEAN, the plain writes of a forward pass (no old target, mask or dropout;
+    // 16-byte aligned), and every other call.  Branches on work a call does not do, inside the loop over the
+    // elements, cost the store warps a third of conv1 fprop's time on an H100 (DESIGN.md §6).
+    auto drain = [&](auto lean) {
+      constexpr bool LEAN = decltype(lean)::value;
+      for (int b = 0; b < batches; b++) {
+        const int c0 = sw + kStoreWarps * kEpiCols * b;
+        float bv[kEpiCols];
 #pragma unroll
-      for (int k = 0; k < kEpiCols; k++) {
-        const int col = c0 + kStoreWarps * k;
-        acc[k] = col < ncols ? ptx::lds128(stg + epi_off(lr, col)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      if (b == batches - 1) {                         // the last read of the staging tile: the consumers may refill it
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&ctl->epi_empty);
-      }
-      if (OP == kFprop && bias) {
-#pragma unroll
-        for (int k = 0; k < kEpiCols; k++) {          // column c0 + SW k is this warp's (kEpiCols b + k)-th
-          const int j = kEpiCols * b + k;
-          bv[k] = __shfl_sync(0xffffffffu, (kBiasHi && j >= 32) ? bias_hi : bias_lo, j & 31);
+        for (int k = 0; k < kEpiCols; k++) {
+          const int col = c0 + kStoreWarps * k;
+          acc[k] = col < ncols ? ptx::lds128(stg + epi_off(lr, col)) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
-      }
-      if (row < 0) continue;
+        if (b == batches - 1) {                         // the last read of the staging tile: the consumers may refill it
+          __syncwarp();
+          if (lane == 0) ptx::mbar_arrive(&ctl->epi_empty);
+        }
+        if (OP == kFprop && bias) {
 #pragma unroll
-      for (int k = 0; k < kEpiCols; k++) {            // the results replace the accumulators in acc
-        const int col = c0 + kStoreWarps * k;
-        if (col >= ncols) continue;
-        const long long idx = row + col_stride * col;
-        const float a[4] = {acc[k].x, acc[k].y, acc[k].z, acc[k].w};
-        const float o[4] = {old[k].x, old[k].y, old[k].z, old[k].w};
-        const float m[4] = {msk[k].x, msk[k].y, msk[k].z, msk[k].w};
-        float v[4];
-#pragma unroll
-        for (int e = 0; e < 4; e++) {
-          float r = so_eff * a[e];
-          if (rmw) r += p.st * o[e];
-          if (OP == kFprop) {
-            if (bias) r += bv[k];
-            if (SIG) { if (p.act) r = act_apply(r, p.act); }
-            else if (p.act) r = fmaxf(r, 0.f);
-            if (p.drop_scale != 0.f) r *= dropout_keep(p.drop_seed + (unsigned long long)(idx + e), p.drop_prob, p.drop_scale);
+          for (int k = 0; k < kEpiCols; k++) {          // column c0 + SW k is this warp's (kEpiCols b + k)-th
+            const int j = kEpiCols * b + k;
+            bv[k] = __shfl_sync(0xffffffffu, (kBiasHi && j >= 32) ? bias_hi : bias_lo, j & 31);
           }
-          if (SIG) { if (p.mask) r = act_deriv(r, m[e], p.mask_act); }
-          else if (p.mask && !(m[e] > 0.f)) r = 0.f;
-          v[e] = r;
         }
-        acc[k] = make_float4(v[0], v[1], v[2], v[3]);
-      }
-      if ((rmw || p.mask) && b + 1 < batches) load_batch(b + 1);
+        if (row < 0) continue;
 #pragma unroll
-      for (int k = 0; k < kEpiCols; k++) {
-        const int col = c0 + kStoreWarps * k;
-        if (col >= ncols) continue;
-        const long long idx = row + col_stride * col;
-        const float v[4] = {acc[k].x, acc[k].y, acc[k].z, acc[k].w};
-        float* const dst = p.out + idx;
-        if (vec) {
-          *reinterpret_cast<float4*>(dst) = acc[k];
-        } else {
+        for (int k = 0; k < kEpiCols; k++) {            // the results replace the accumulators in acc
+          const int col = c0 + kStoreWarps * k;
+          if (col >= ncols) continue;
+          const long long idx = row + col_stride * col;
+          const float a[4] = {acc[k].x, acc[k].y, acc[k].z, acc[k].w};
+          const float o[4] = {old[k].x, old[k].y, old[k].z, old[k].w};
+          const float m[4] = {msk[k].x, msk[k].y, msk[k].z, msk[k].w};
+          float v[4];
 #pragma unroll
-          for (int e = 0; e < 4; e++) dst[e] = v[e];
+          for (int e = 0; e < 4; e++) {
+            float r = so_eff * a[e];
+            if (!LEAN && rmw) r += p.st * o[e];
+            if (OP == kFprop) {
+              if (bias) r += bv[k];
+              if (SIG) { if (p.act) r = act_apply(r, p.act); }
+              else if (p.act) r = fmaxf(r, 0.f);
+              if (!LEAN && p.drop_scale != 0.f) r *= dropout_keep(p.drop_seed + (unsigned long long)(idx + e), p.drop_prob, p.drop_scale);
+            }
+            if (!LEAN) {
+              if (SIG) { if (p.mask) r = act_deriv(r, m[e], p.mask_act); }
+              else if (p.mask && !(m[e] > 0.f)) r = 0.f;
+            }
+            v[e] = r;
+          }
+          acc[k] = make_float4(v[0], v[1], v[2], v[3]);
         }
-        if (p.out16) {
-          __nv_bfloat16* const d16 = p.out16 + idx;
-          const __nv_bfloat162 lo = __floats2bfloat162_rn(v[0], v[1]), hi = __floats2bfloat162_rn(v[2], v[3]);
-          if (vec) {
-            uint2 w;
-            w.x = *reinterpret_cast<const uint32_t*>(&lo);
-            w.y = *reinterpret_cast<const uint32_t*>(&hi);
-            *reinterpret_cast<uint2*>(d16) = w;
+        if (!LEAN && (rmw || p.mask) && b + 1 < batches) load_batch(b + 1);
+#pragma unroll
+        for (int k = 0; k < kEpiCols; k++) {
+          const int col = c0 + kStoreWarps * k;
+          if (col >= ncols) continue;
+          const long long idx = row + col_stride * col;
+          const float v[4] = {acc[k].x, acc[k].y, acc[k].z, acc[k].w};
+          float* const dst = p.out + idx;
+          if (LEAN || vec) {
+            *reinterpret_cast<float4*>(dst) = acc[k];
           } else {
-            d16[0] = lo.x; d16[1] = lo.y; d16[2] = hi.x; d16[3] = hi.y;
+#pragma unroll
+            for (int e = 0; e < 4; e++) dst[e] = v[e];
+          }
+          if (p.out16) {
+            __nv_bfloat16* const d16 = p.out16 + idx;
+            const __nv_bfloat162 lo = __floats2bfloat162_rn(v[0], v[1]), hi = __floats2bfloat162_rn(v[2], v[3]);
+            if (LEAN || vec) {
+              uint2 w;
+              w.x = *reinterpret_cast<const uint32_t*>(&lo);
+              w.y = *reinterpret_cast<const uint32_t*>(&hi);
+              *reinterpret_cast<uint2*>(d16) = w;
+            } else {
+              d16[0] = lo.x; d16[1] = lo.y; d16[2] = hi.x; d16[3] = hi.y;
+            }
           }
         }
       }
-    }
+    };
+    if (!rmw && !p.mask && !(OP == kFprop && p.drop_scale != 0.f) && vec) drain(std::true_type{});
+    else drain(std::false_type{});
     phase ^= 1;
   }
 }

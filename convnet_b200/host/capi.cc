@@ -1,4 +1,11 @@
 // capi.cc — plain C doors onto the host C++ (ConvNet / GradChecker / DataParallelSync) for ctypes.
+//
+// Every entry that can fail runs its body in Guard and reports one way: a status (0, or a count where the entry returns
+// one), -1 when the library refused (an invalid_argument, a logic_error, a file it cannot read or write), -2 when a CUDA
+// or NCCL call failed (DeviceError), and NULL for the entries that create an object.  The reason is in cnb_last_error()
+// and on stderr as "convnet_b200 host: <reason>"; cnb_last_status() tells a NULL's -1 from its -2.  After a -2 in the
+// middle of a step the net's state is undefined: the only safe call left on it is cnb_net_destroy.  The entries that only
+// read fields cannot fail and return their value.
 #include <algorithm>
 #include <cstdio>
 #include <cstring>
@@ -20,32 +27,48 @@ struct NetHandle {
 };
 
 static std::string g_last_error;
-// the message of the last refusal (of a model, a checkpoint, a data set configuration or the training loop)
+static int g_last_status = 0;
+// the reason and the status (-1 or -2) of the last failure
 API const char* cnb_last_error() { return g_last_error.c_str(); }
-// runs f: 0, or -1 with what it threw in cnb_last_error() and on stderr
+API int cnb_last_status() { return g_last_status; }
+static int Fail(const std::exception& e, int status) {
+  g_last_error = e.what();
+  g_last_status = status;
+  fprintf(stderr, "convnet_b200 host: %s\n", e.what());
+  return status;
+}
+// runs f: 0, or the status of what it threw (-2 a DeviceError, -1 any other exception)
 template <class F>
 static int Guard(F f) {
   try {
     f();
     return 0;
+  } catch (const DeviceError& e) {
+    return Fail(e, -2);
   } catch (const std::exception& e) {
-    g_last_error = e.what();
-    fprintf(stderr, "convnet_b200 host: %s\n", e.what());
-    return -1;
+    return Fail(e, -1);
   }
 }
 
+API void cnb_net_destroy(void* p) {
+  NetHandle* h = (NetHandle*)p;
+  delete h->net; delete h->dp; delete h;
+}
 // a handle on the ConvNet (GradChecker when grad_checker) of a built-in name or model file, with its seed replaced unless
-// `seed` is NULL; no device memory yet.  NULL: an unknown name, or a model that cannot be read or run (cnb_last_error)
-static NetHandle* Open(const char* model, int batch, const unsigned* seed, bool grad_checker) {
+// `seed` is NULL, and its device memory allocated when `allocate` (else its parameters only planned).  NULL: an unknown
+// name, a model that cannot be read or run, or memory that cannot be set up (the checkpoints of PRETRAINED edges, the
+// device)
+static void* Open(const char* model, int batch, const unsigned* seed, bool grad_checker, bool allocate) {
   NetHandle* h = new NetHandle;
   if (Guard([&] {
         ModelConfig m = BuildModel(model);
         if (seed) m.seed = *seed;
         if (grad_checker) h->net = h->checker = new GradChecker(m, batch);
         else h->net = new ConvNet(m, batch);
+        if (allocate) h->net->AllocateMemory();
+        else h->net->PlanParameters();
       })) {
-    delete h;
+    cnb_net_destroy(h);
     return nullptr;
   }
   return h;
@@ -53,23 +76,10 @@ static NetHandle* Open(const char* model, int batch, const unsigned* seed, bool 
 // a host-only handle: the net built and its parameters planned, nothing allocated on the device.  The cnb_net_* calls that
 // read no device memory describe the model through it: edges, layers, the parameter layout, the fusion plan, FLOPs, the
 // trained tensors' optimizers, and the model-level settings below (cnb_net_model_text ... cnb_net_train_dry_run)
-API void* cnb_model_open(const char* model, int batch) {
-  NetHandle* h = Open(model, batch, nullptr, false);
-  if (h) h->net->PlanParameters();
-  return h;
-}
-API void cnb_net_destroy(void* p) {
-  NetHandle* h = (NetHandle*)p;
-  delete h->net; delete h->dp; delete h;
-}
-// a net to run: NULL as for cnb_model_open, or when its memory cannot be set up (the checkpoints of PRETRAINED edges)
+API void* cnb_model_open(const char* model, int batch) { return Open(model, batch, nullptr, false, false); }
+// a net to run
 API void* cnb_net_create(const char* model, int batch_size, unsigned seed, int grad_checker) {
-  NetHandle* h = Open(model, batch_size, &seed, grad_checker != 0);
-  if (h && Guard([&] { h->net->AllocateMemory(); })) {
-    cnb_net_destroy(h);
-    return nullptr;
-  }
-  return h;
+  return Open(model, batch_size, &seed, grad_checker != 0, true);
 }
 API long long cnb_net_num_params(void* p) { return (long long)((NetHandle*)p)->net->NumParameters(); }
 API int cnb_net_num_edges(void* p) { return (int)((NetHandle*)p)->net->Edges().size(); }
@@ -121,9 +131,11 @@ API float* cnb_net_device_loss(void* p) { return ((NetHandle*)p)->net->DeviceLos
 // the seed of the dropout mask the next training-mode Fprop draws for layer i (0: the layer has no dropout)
 API unsigned long long cnb_net_dropout_seed(void* p, int i) { return ((NetHandle*)p)->net->NextDropoutSeed((size_t)i); }
 
-API void cnb_net_fprop(void* p, int train) { ((NetHandle*)p)->net->Fprop(train != 0); }
-API void cnb_net_bprop(void* p) { ((NetHandle*)p)->net->ComputeDeriv(); ((NetHandle*)p)->net->Bprop(); }
-API void cnb_net_update(void* p) { ((NetHandle*)p)->net->UpdateWeights(); }
+API int cnb_net_fprop(void* p, int train) { return Guard([&] { ((NetHandle*)p)->net->Fprop(train != 0); }); }
+API int cnb_net_bprop(void* p) {
+  return Guard([&] { ((NetHandle*)p)->net->ComputeDeriv(); ((NetHandle*)p)->net->Bprop(); });
+}
+API int cnb_net_update(void* p) { return Guard([&] { ((NetHandle*)p)->net->UpdateWeights(); }); }
 API void cnb_net_reduce_learning_rate(void* p, float factor) { ((NetHandle*)p)->net->ReduceLearningRate(factor); }
 
 // ---- optimizer settings (edge.h OptimizerConfig: proto Optimizer, SGD fields) of one trained tensor, named as its
@@ -133,14 +145,15 @@ static TrainedTensor* Tensor(void* p, const char* name) {
     if (t.name == name) return &t;
   return nullptr;
 }
-// replaces the settings of one optimizer (its step count and momentum history stay).  0 ok, -1 no such tensor, -2 a
-// config this tensor cannot train with (OptimizerConfigError; BnOptimizerConfigError for gamma / beta; on stderr)
+// replaces the settings of one optimizer (its step count and momentum history stay).  Refused: no such tensor, or a
+// config this tensor cannot train with (OptimizerConfigError; BnOptimizerConfigError for gamma / beta)
 API int cnb_net_set_optimizer(void* p, const char* tensor, const OptimizerConfig* c) {
-  TrainedTensor* t = Tensor(p, tensor);
-  if (!t) return -1;
-  if (const char* err = t->ConfigError(*c)) { fprintf(stderr, "convnet_b200 host: %s\n", err); return -2; }
-  ((NetHandle*)p)->net->SetOptimizer(*t, *c);
-  return 0;
+  return Guard([&] {
+    TrainedTensor* t = Tensor(p, tensor);
+    if (!t) throw std::invalid_argument(std::string("no trained tensor '") + tensor + "'");
+    if (const char* err = t->ConfigError(*c)) throw std::invalid_argument(std::string(t->name) + ": " + err);
+    ((NetHandle*)p)->net->SetOptimizer(*t, *c);
+  });
 }
 // the adaptive optimizer state (cnb_net_num_params floats, carved like the parameters); NULL while no optimizer of the
 // net is ADAGRAD_SGD or RMSPROP_SGD
@@ -156,11 +169,13 @@ API long long cnb_net_get_optimizer_state(void* p, const char* tensor, long long
   if (config) *config = t->opt;
   return t->n;
 }
-// pure host logic: (epsilon, momentum) of the update after `step` earlier ones.  0 ok, -2 invalid config
+// pure host logic: (epsilon, momentum) of the update after `step` earlier ones.  Refused: a config OptimizerConfigError
+// objects to
 API int cnb_optimizer_schedule(const OptimizerConfig* c, long long step, float* epsilon, float* momentum) {
-  if (OptimizerConfigError(*c)) return -2;
-  OptimizerSchedule(*c, step, epsilon, momentum);
-  return 0;
+  return Guard([&] {
+    if (const char* err = OptimizerConfigError(*c)) throw std::invalid_argument(err);
+    OptimizerSchedule(*c, step, epsilon, momentum);
+  });
 }
 
 // ---- batch normalisation (convnet.h Layer).  layer: index into the chain (0 = input).  which: 0 gamma, 1 beta.
@@ -183,19 +198,20 @@ API float* cnb_net_bn_stat(void* p, int layer, int which) {
   Layer* l = BnLayer(p, layer);
   return l && which >= 0 && which < 4 ? l->BnStat(which) : nullptr;
 }
-// pure host logic: 0 if `c` can train gamma / beta, -2 if not (the reason on stderr)
+// pure host logic: 0 if `c` can train gamma / beta, refused if not
 API int cnb_bn_optimizer_check(const OptimizerConfig* c) {
-  if (const char* err = BnOptimizerConfigError(*c)) { fprintf(stderr, "convnet_b200 host: %s\n", err); return -2; }
-  return 0;
+  return Guard([&] {
+    if (const char* err = BnOptimizerConfigError(*c)) throw std::invalid_argument(err);
+  });
 }
 
 // the output layer's float targets ([batch x state columns], column-major, written by the caller); NULL / 0 for an output
 // layer trained on labels (cnb_net_labels)
 API float* cnb_net_targets(void* p) { return ((NetHandle*)p)->net->OutputLayer().GetTargets().GetDevData(); }
 API long long cnb_net_targets_floats(void* p) { return (long long)((NetHandle*)p)->net->OutputLayer().GetTargets().GetNumEls(); }
-// loss_function_weight * the batch's loss (ConvNet::GetLoss) and the summed performance metric (GetPerformanceMetric)
-API float cnb_net_loss(void* p) { return ((NetHandle*)p)->net->GetLoss(); }
-API float cnb_net_metric(void* p) { return ((NetHandle*)p)->net->GetPerformanceMetric(); }
+// *out: loss_function_weight * the batch's loss (ConvNet::GetLoss) / the summed performance metric (GetPerformanceMetric)
+API int cnb_net_loss(void* p, float* out) { return Guard([&] { *out = ((NetHandle*)p)->net->GetLoss(); }); }
+API int cnb_net_metric(void* p, float* out) { return Guard([&] { *out = ((NetHandle*)p)->net->GetPerformanceMetric(); }); }
 // the model's output layer.  *activation: the Activation enum of convnet.h; *loss / *metric: proto LossFunction numbers;
 // *labels: 1 trained on integer labels, 0 on float targets
 API void cnb_net_output_layer(void* p, int* activation, int* loss, int* metric, float* weight, int* labels) {
@@ -204,30 +220,36 @@ API void cnb_net_output_layer(void* p, int* activation, int* loss, int* metric, 
   *labels = TakesLabels(l.activation) ? 1 : 0;
 }
 // one training step; *loss (may be NULL) receives the batch's loss as cnb_net_loss gives it (one scalar D2H)
-API void cnb_net_train_step(void* p, float* loss) { ((NetHandle*)p)->net->TrainOneBatch(loss); }
+API int cnb_net_train_step(void* p, float* loss) { return Guard([&] { ((NetHandle*)p)->net->TrainOneBatch(loss); }); }
 // one traced training step (ConvNet::TraceStep); returns the number of floats the full record has, writes min(cap, that)
 API int cnb_net_trace_step(void* p, float* out, int cap) {
-  const std::vector<float> t = ((NetHandle*)p)->net->TraceStep();
+  std::vector<float> t;
+  const int rc = Guard([&] { t = ((NetHandle*)p)->net->TraceStep(); });
   for (int i = 0; i < cap && i < (int)t.size(); i++) out[i] = t[i];
-  return (int)t.size();
+  return rc ? rc : (int)t.size();
 }
 
 // data parallel: rank 0 calls cnb_dp_unique_id, the launcher broadcasts the 128 bytes, every rank calls cnb_net_dp_init
-API int cnb_dp_unique_id(char* out128) { return DataParallelSync::GetUniqueId(out128) ? 0 : -1; }
+API int cnb_dp_unique_id(char* out128) { return Guard([&] { DataParallelSync::GetUniqueId(out128); }); }
 API int cnb_net_dp_init(void* p, int rank, int world, const char* id128, long long bucket_floats) {
   NetHandle* h = (NetHandle*)p;
-  h->dp = new DataParallelSync();
-  if (!h->dp->Init(rank, world, id128)) return -1;
-  h->net->SetDataParallel(h->dp, (size_t)bucket_floats);
-  h->net->BroadcastParameters();
-  return 0;
+  return Guard([&] {
+    h->dp = new DataParallelSync();
+    h->dp->Init(rank, world, id128);
+    h->net->SetDataParallel(h->dp, (size_t)bucket_floats);
+    h->net->BroadcastParameters();
+  });
 }
 
-// grad check: fills up to `cap` results; returns the number of checked edges
+// grad check: fills up to `cap` results; returns the number of checked edges.  Refused on a net not created as a checker
 API int cnb_net_grad_check(void* p, unsigned seed, int cap, char* names /*cap x 64*/, float* eps, float* diff_w, float* diff_b) {
   NetHandle* h = (NetHandle*)p;
-  if (!h->checker) return -1;
-  std::vector<GradCheckResult> r = h->checker->Run(seed);
+  std::vector<GradCheckResult> r;
+  const int rc = Guard([&] {
+    if (!h->checker) throw std::invalid_argument("grad_check: the net was not created as a grad checker");
+    r = h->checker->Run(seed);
+  });
+  if (rc) return rc;
   int n = 0;
   for (const GradCheckResult& g : r) {
     if (n >= cap) break;
@@ -260,24 +282,23 @@ API long long cnb_net_model_text(void* p, char* buf, long long cap) {
 }
 
 // the initial weights of edge `edge` under RNG seed `seed` (EdgeWithWeight::InitialWeights; the net seeds edge i with its
-// seed + 17 i), or a PRETRAINED edge's weights from its checkpoint.  Returns their number (writes up to `cap`); -1 an
-// unreadable checkpoint (cnb_last_error), -2 edge out of range or without parameters of its own
+// seed + 17 i), or a PRETRAINED edge's weights from its checkpoint.  Returns their number (writes up to `cap`), 0 for an
+// edge out of range or without parameters of its own; refused: an unreadable checkpoint
 API long long cnb_net_initial_weights(void* p, int edge, unsigned seed, float* out, long long cap) {
   ConvNet* net = ((NetHandle*)p)->net;
   EdgeWithWeight* e = edge >= 0 && edge < (int)net->Edges().size() ? dynamic_cast<EdgeWithWeight*>(net->Edges()[edge].get()) : nullptr;
-  if (!e || e->Tied()) return -2;
+  if (!e || e->Tied()) return 0;
   std::vector<float> w;
-  if (Guard([&] {
+  if (const int rc = Guard([&] {
         w = e->Config().initialization == PRETRAINED ? PretrainedWeights(e->Config(), e->WeightCount()) : e->InitialWeights(seed);
       }))
-    return -1;
+    return rc;
   const long long n = (long long)w.size();
   if (cap > 0) memcpy(out, w.data(), sizeof(float) * (size_t)std::min(n, cap));
   return n;
 }
 
-// ---- checkpoints and Polyak averaging (checkpoint.cc).  Each returns 0, or -1 with the message on stderr and in
-// cnb_last_error()
+// ---- checkpoints and Polyak averaging (checkpoint.cc)
 API int cnb_net_save(void* p, const char* path) { return Guard([&] { ((NetHandle*)p)->net->Save(path); }); }
 API int cnb_net_load(void* p, const char* path) { return Guard([&] { ((NetHandle*)p)->net->Load(path); }); }
 API long long cnb_net_iteration(void* p) { return (long long)((NetHandle*)p)->net->Iteration(); }
@@ -297,17 +318,25 @@ API int cnb_net_polyak_due(void* p, long long iteration) { return PolyakDue(((Ne
 // ---- the device side of the input pipeline (data.h): a GPU-resident chunk + per-minibatch crop / mirror into the net's input
 API void* cnb_data_create(int chunk_size, int channels, int image_size_y, int image_size_x, int gpu_image_size_y,
                           int gpu_image_size_x, int translate, int flip, unsigned long long seed) {
-  return new DataIterator(chunk_size, channels, image_size_y, image_size_x, gpu_image_size_y, gpu_image_size_x,
-                          translate != 0, flip != 0, seed);
+  DataIterator* d = nullptr;
+  Guard([&] {
+    d = new DataIterator(chunk_size, channels, image_size_y, image_size_x, gpu_image_size_y, gpu_image_size_x,
+                         translate != 0, flip != 0, seed);
+  });
+  return d;
 }
 API void cnb_data_destroy(void* d) { delete (DataIterator*)d; }
-API void cnb_data_upload(void* d, const float* host, int first, int count) { ((DataIterator*)d)->Upload(host, first, count); }
+API int cnb_data_upload(void* d, const float* host, int first, int count) {
+  return Guard([&] { ((DataIterator*)d)->Upload(host, first, count); });
+}
 // DataHandler::GetBatch for the input layer of `net`: sample the jitter, then cut images [start, start + batch) into it
-API void cnb_data_get_batch(void* d, void* net, int start, int multiplicity_id) {
-  DataIterator* it = (DataIterator*)d;
-  Matrix& dest = ((NetHandle*)net)->net->InputLayer().GetState();
-  it->SampleNoise(dest.GetRows(), multiplicity_id);
-  it->AddNoise(start, dest);
+API int cnb_data_get_batch(void* d, void* net, int start, int multiplicity_id) {
+  return Guard([&] {
+    DataIterator* it = (DataIterator*)d;
+    Matrix& dest = ((NetHandle*)net)->net->InputLayer().GetState();
+    it->SampleNoise(dest.GetRows(), multiplicity_id);
+    it->AddNoise(start, dest);
+  });
 }
 // the jitter of the last minibatch (host copies): out = {width offsets, height offsets, mirror bits}, 3 x batch floats
 API int cnb_data_last_noise(void* d, float* out, int cap) {
@@ -322,11 +351,11 @@ API void cnb_data_view_offset(int multiplicity_id, int max_offset_x, int max_off
   Jitter::ViewOffset(multiplicity_id, max_offset_x, max_offset_y, w, h);
 }
 
-// ---- the data set feed (data.h): DataSchedule is the pure host state machine, DataHandler runs it on the GPU.  A refused
-// configuration gives NULL / -1 and the reason in cnb_last_error()
+// ---- the data set feed (data.h): DataSchedule is the pure host state machine, DataHandler runs it on the GPU
 API void* cnb_schedule_create(const DatasetOrder* c, int dataset_size, unsigned long long seed) {
-  try { return new DataSchedule(*c, dataset_size, seed); }
-  catch (const std::invalid_argument& e) { g_last_error = e.what(); return nullptr; }
+  DataSchedule* s = nullptr;
+  Guard([&] { s = new DataSchedule(*c, dataset_size, seed); });
+  return s;
 }
 API void cnb_schedule_destroy(void* s) { delete (DataSchedule*)s; }
 API int cnb_schedule_chunk_size(void* s) { return ((DataSchedule*)s)->ChunkSize(); }
@@ -340,29 +369,22 @@ API int cnb_schedule_next(void* p, int* start, int* multiplicity_id, int* rows, 
   if (b.loaded) memcpy(rows, s->Rows().data(), sizeof(int) * s->ChunkSize());
   return b.loaded ? 1 : 0;
 }
-API int cnb_schedule_seek(void* s, int row) {
-  try { ((DataSchedule*)s)->Seek(row); return 0; }
-  catch (const std::invalid_argument& e) { g_last_error = e.what(); return -1; }
-}
+API int cnb_schedule_seek(void* s, int row) { return Guard([&] { ((DataSchedule*)s)->Seek(row); }); }
 // images: dataset_size x channels*y*x floats, labels: dataset_size ints (or NULL), targets: dataset_size x target_dims
 // floats (or NULL), all in host memory that outlives the handler
 API void* cnb_handler_create(const DatasetOrder* c, int dataset_size, int channels, int image_size_y, int image_size_x,
                              int gpu_image_size_y, int gpu_image_size_x, int translate, int flip, const float* images,
                              const int* labels, const float* targets, int target_dims, unsigned long long seed) {
-  try {
-    return new DataHandler(*c, dataset_size, channels, image_size_y, image_size_x, gpu_image_size_y, gpu_image_size_x,
-                           translate != 0, flip != 0, images, labels, targets, target_dims, seed);
-  } catch (const std::invalid_argument& e) { g_last_error = e.what(); return nullptr; }
+  DataHandler* h = nullptr;
+  Guard([&] {
+    h = new DataHandler(*c, dataset_size, channels, image_size_y, image_size_x, gpu_image_size_y, gpu_image_size_x,
+                        translate != 0, flip != 0, images, labels, targets, target_dims, seed);
+  });
+  return h;
 }
 API void cnb_handler_destroy(void* h) { delete (DataHandler*)h; }
-API int cnb_handler_get_batch(void* h, void* net) {
-  try { ((DataHandler*)h)->GetBatch(*((NetHandle*)net)->net); return 0; }
-  catch (const std::invalid_argument& e) { g_last_error = e.what(); return -1; }
-}
-API int cnb_handler_seek(void* h, int row) {
-  try { ((DataHandler*)h)->Seek(row); return 0; }
-  catch (const std::invalid_argument& e) { g_last_error = e.what(); return -1; }
-}
+API int cnb_handler_get_batch(void* h, void* net) { return Guard([&] { ((DataHandler*)h)->GetBatch(*((NetHandle*)net)->net); }); }
+API int cnb_handler_seek(void* h, int row) { return Guard([&] { ((DataHandler*)h)->Seek(row); }); }
 // the last minibatch (host copies): *start, *multiplicity_id, the data set row of each image (rows[batch]) and its jitter
 // (noise[3 x batch]: width offsets, height offsets, mirror bits); returns the batch size
 API int cnb_handler_last(void* p, int* start, int* multiplicity_id, int* rows, float* noise) {
@@ -403,8 +425,8 @@ API int cnb_reduce_lr_due(const float* history, int len, int num_steps, float th
 // ConvNet::Train's decisions for the model, from TrainOneBatch call `start` + 1 to max_iter: per iteration with an action,
 // iters[k] and actions[k] (TrainSchedule::Action bits, plus 16: the learning rate is reduced after this validation, 32:
 // this validation runs on the Polyak average), and for the save after the loop a last record (max_iter, 8 | 64).  The
-// validations take the values values[0, n_values) in order.  Returns the number of records (writes up to `cap`); -1 with
-// the reason in cnb_last_error(): a refused schedule, or more validations than values
+// validations take the values values[0, n_values) in order.  Returns the number of records (writes up to `cap`); refused:
+// a schedule the loop refuses, or more validations than values
 API long long cnb_net_train_dry_run(void* p, long long start, int lr_reduce_counter, int validation_set,
                                     const float* values, int n_values, long long cap, long long* iters, int* actions) {
   long long n = 0;
@@ -426,14 +448,13 @@ API long long cnb_net_train_dry_run(void* p, long long start, int lr_reduce_coun
     }
     if (s.FinalSave()) put(m.max_iter, TrainSchedule::SAVE | 64);
   });
-  return rc ? -1 : n;
+  return rc ? rc : n;
 }
 
 API int cnb_net_validate(void* p, void* handler, float* out) {
   return Guard([&] { *out = ((NetHandle*)p)->net->Validate(*(DataHandler*)handler); });
 }
-// ConvNet::Train; valid, checkpoint_dir and run_name may be NULL.  Returns the number of events (cnb_net_train_event), or
-// -1 with the reason in cnb_last_error()
+// ConvNet::Train; valid, checkpoint_dir and run_name may be NULL.  Returns the number of events (cnb_net_train_event)
 API int cnb_net_train(void* p, void* train, void* valid, const char* checkpoint_dir, const char* run_name) {
   NetHandle* h = (NetHandle*)p;
   h->events.clear();
@@ -441,7 +462,7 @@ API int cnb_net_train(void* p, void* train, void* valid, const char* checkpoint_
     h->events = h->net->Train(*(DataHandler*)train, (DataHandler*)valid, checkpoint_dir ? checkpoint_dir : "",
                               run_name ? run_name : "");
   });
-  return rc ? -1 : (int)h->events.size();
+  return rc ? rc : (int)h->events.size();
 }
 // event k of the last cnb_net_train: *kind 0 train, 1 valid.  0 ok, -1 k out of range
 API int cnb_net_train_event(void* p, int k, long long* iteration, int* kind, float* value, int* lr_reduced, int* polyak) {

@@ -23,12 +23,6 @@ const uint32_t kVersion = 1;
 const char* const kTypeNames[] = {"float32", "int64", "text"};
 const size_t kTypeBytes[] = {4, 8, 1};
 
-#define CKPT_CUDA_CHECK(expr)                                                                          \
-  do {                                                                                                 \
-    cudaError_t _e = (expr);                                                                           \
-    if (_e != cudaSuccess) throw std::runtime_error(std::string(#expr) + ": " + cudaGetErrorString(_e)); \
-  } while (0)
-
 std::string Errno() { return strerror(errno); }
 
 // little-endian scalars (the hosts this runs on are little-endian; the format fixes the byte order)
@@ -54,7 +48,7 @@ class RecordWriter {
   void Floats(const std::string& name, const float* dev, long long n) {
     Header(name, CheckpointFile::FLOAT32, (uint64_t)n);
     std::vector<float> h((size_t)n);
-    if (n) CKPT_CUDA_CHECK(cudaMemcpy(h.data(), dev, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    if (n) CUDA_CHECK(cudaMemcpy(h.data(), dev, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
     Write(h.data(), sizeof(float) * h.size());
   }
 
@@ -176,8 +170,8 @@ ModelConfig ConvNet::CurrentModel() const {
 }
 
 void ConvNet::WaitAllStreams() {
-  CKPT_CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
-  for (cudaStream_t s : {side_, comm_, opt_}) if (s) CKPT_CUDA_CHECK(cudaStreamSynchronize(s));
+  CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
+  for (cudaStream_t s : {side_, comm_, opt_}) if (s) CUDA_CHECK(cudaStreamSynchronize(s));
 }
 
 // after a bulk write of the parameters: the dgrad banks are rebuilt now, on the main stream, rather than inside the next
@@ -300,15 +294,15 @@ void ConvNet::Load(const std::string& path) {
     if (e.buffer == CheckpointEntry::STEP) {
       memcpy(&tensors_[e.tensor].step, data[k].data(), 8);
     } else if (e.n) {
-      CKPT_CUDA_CHECK(cudaMemcpyAsync(EntryData(e), data[k].data(), sizeof(float) * (size_t)e.n, cudaMemcpyHostToDevice,
-                                      Matrix::Stream()));
+      CUDA_CHECK(cudaMemcpyAsync(EntryData(e), data[k].data(), sizeof(float) * (size_t)e.n, cudaMemcpyHostToDevice,
+                                 Matrix::Stream()));
     }
   }
   step_ = (unsigned long long)iter;
   lr_reduce_counter_ = (int)lr_reduce_counter;
   model_.seed = (unsigned)seed;
   if (salted_) SaltDropout();                        // the file's seed, this net's rank
-  CKPT_CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));   // (the host buffers go away)
+  CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));        // (the host buffers go away)
   // 5. the staged copies of the old weights: dropped, and the dgrad banks rebuilt
   InvalidateStaging();
   PrestageAll();
@@ -335,7 +329,7 @@ void ConvNet::LoadPretrained(size_t i) {
     if (!why.empty()) throw std::invalid_argument("edge '" + edge + "' (PRETRAINED): " + why);
     for (const auto& [name, dev] : tensors) {
       const std::vector<char> h = f.Read(name);
-      CKPT_CUDA_CHECK(cudaMemcpy(dev, h.data(), h.size(), cudaMemcpyHostToDevice));
+      CUDA_CHECK(cudaMemcpy(dev, h.data(), h.size(), cudaMemcpyHostToDevice));
     }
     memcpy(&t.step, f.Read(prefix + "_step").data(), 8);
   }
@@ -372,10 +366,10 @@ void ConvNet::InsertPolyak() {
     }
   }
   // after the optimizer stream's pending updates, without a host wait; the next step's updates wait for the main stream
-  CKPT_CUDA_CHECK(cudaEventRecord(ev_opt_, opt_));
-  CKPT_CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), ev_opt_, 0));
-  CKPT_CUDA_CHECK(cudaMemcpyAsync(polyak_ + (size_t)polyak_index_ * n, parameters_.GetDevData(), sizeof(float) * n,
-                                  cudaMemcpyDeviceToDevice, Matrix::Stream()));
+  CUDA_CHECK(cudaEventRecord(ev_opt_, opt_));
+  CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), ev_opt_, 0));
+  CUDA_CHECK(cudaMemcpyAsync(polyak_ + (size_t)polyak_index_ * n, parameters_.GetDevData(), sizeof(float) * n,
+                             cudaMemcpyDeviceToDevice, Matrix::Stream()));
   if (++polyak_index_ == model_.polyak_queue_size) { polyak_index_ = 0; polyak_full_ = true; }
 }
 
@@ -383,10 +377,10 @@ void ConvNet::LoadPolyakWeights() {
   if (!PolyakOn(model_)) throw std::invalid_argument("the model has no Polyak averaging (polyak_after, polyak_queue_size)");
   if (PolyakCount() == 0) throw std::invalid_argument("LoadPolyakWeights: nothing has been inserted into the Polyak queue");
   const size_t n = num_params_;
-  CKPT_CUDA_CHECK(cudaEventRecord(ev_opt_, opt_));
-  CKPT_CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), ev_opt_, 0));
+  CUDA_CHECK(cudaEventRecord(ev_opt_, opt_));
+  CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), ev_opt_, 0));
   float* backup = polyak_ + (size_t)model_.polyak_queue_size * n;
-  CKPT_CUDA_CHECK(cudaMemcpyAsync(backup, parameters_.GetDevData(), sizeof(float) * n, cudaMemcpyDeviceToDevice, Matrix::Stream()));
+  CUDA_CHECK(cudaMemcpyAsync(backup, parameters_.GetDevData(), sizeof(float) * n, cudaMemcpyDeviceToDevice, Matrix::Stream()));
   // the kernel's write drops the staged copies of the old weights (bf16 twins and dgrad banks) itself.  Only the trained
   // range: the frozen parameters are equal in every slot, and their average could still round (DESIGN.md §5)
   const size_t lo = TrainedOffset();
@@ -398,8 +392,8 @@ void ConvNet::LoadPolyakWeights() {
 void ConvNet::LoadCurrentWeights() {
   if (!polyak_backup_) throw std::invalid_argument("LoadCurrentWeights without an earlier LoadPolyakWeights");
   const size_t n = num_params_;
-  CKPT_CUDA_CHECK(cudaMemcpyAsync(parameters_.GetDevData(), polyak_ + (size_t)model_.polyak_queue_size * n, sizeof(float) * n,
-                                  cudaMemcpyDeviceToDevice, Matrix::Stream()));
+  CUDA_CHECK(cudaMemcpyAsync(parameters_.GetDevData(), polyak_ + (size_t)model_.polyak_queue_size * n, sizeof(float) * n,
+                             cudaMemcpyDeviceToDevice, Matrix::Stream()));
   InvalidateStaging();
   PrestageAll();
 }

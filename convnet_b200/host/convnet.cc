@@ -18,15 +18,6 @@
 
 namespace cnbhost {
 
-#define HOST_CUDA_CHECK(expr)                                                                         \
-  do {                                                                                                \
-    cudaError_t _e = (expr);                                                                          \
-    if (_e != cudaSuccess) {                                                                          \
-      fprintf(stderr, "%s(%d) : CUDA error : %s : %s\n", __FILE__, __LINE__, #expr, cudaGetErrorString(_e)); \
-      exit(EXIT_FAILURE);                                                                             \
-    }                                                                                                 \
-  } while (0)
-
 // =================================================================== Layer
 Layer::~Layer() { if (labels_) cudaFree(labels_); }
 
@@ -52,8 +43,8 @@ void Layer::AllocateMemory(int batch_size) {               // layer.cc:228-262 (
     bn_stats_.AllocateGPUMemory(1, 4 * config_.num_channels);
   }
   if (config_.is_output) {
-    HOST_CUDA_CHECK(cudaMalloc((void**)&labels_, sizeof(int) * batch_size));
-    HOST_CUDA_CHECK(cudaMemset(labels_, 0, sizeof(int) * batch_size));
+    CUDA_CHECK(cudaMalloc((void**)&labels_, sizeof(int) * batch_size));
+    CUDA_CHECK(cudaMemset(labels_, 0, sizeof(int) * batch_size));
     loss_per_image_.AllocateGPUMemory(batch_size, 1);
     metric_per_image_.AllocateGPUMemory(batch_size, 1);
     if (!TakesLabels(config_.activation)) {                // layer.cc:530-602: data_ shaped like the state
@@ -333,7 +324,7 @@ struct NcclApi {
   ncclResult_t (*AllReduce)(const void*, void*, size_t, ncclDataType_t, ncclRedOp_t, ncclComm_t, cudaStream_t) = nullptr;
   ncclResult_t (*Bcast)(const void*, void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
   const char* (*GetErrorString)(ncclResult_t) = nullptr;
-  bool ok = false;
+  std::string error;                                         // why it cannot be used ("": it can)
 };
 NcclApi& nccl() {
   static NcclApi api;
@@ -342,26 +333,26 @@ NcclApi& nccl() {
     tried = true;
     // torch's bundled libnccl.so.2 is already mapped when the launcher imported torch; otherwise the loader path is used
     api.handle = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
-    if (!api.handle) { fprintf(stderr, "convnet_b200 host: cannot load libnccl.so.2: %s\n", dlerror()); return api; }
+    if (!api.handle) { api.error = std::string("cannot load libnccl.so.2: ") + dlerror(); return api; }
 #define LOAD(field, sym) api.field = reinterpret_cast<decltype(api.field)>(dlsym(api.handle, sym))
     LOAD(GetUniqueId, "ncclGetUniqueId"); LOAD(CommInitRank, "ncclCommInitRank"); LOAD(CommDestroy, "ncclCommDestroy");
     LOAD(CommInitRankConfig, "ncclCommInitRankConfig");
     LOAD(AllReduce, "ncclAllReduce"); LOAD(Bcast, "ncclBroadcast"); LOAD(GetErrorString, "ncclGetErrorString");
 #undef LOAD
-    api.ok = api.GetUniqueId && api.CommInitRank && api.AllReduce && api.Bcast;
+    if (!api.GetUniqueId || !api.CommInitRank || !api.AllReduce || !api.Bcast)
+      api.error = "libnccl.so.2 lacks ncclGetUniqueId, ncclCommInitRank, ncclAllReduce or ncclBroadcast";
   }
   return api;
 }
-#define NCCL_CHECK(expr)                                                                               \
-  do {                                                                                                 \
-    ncclResult_t _r = (expr);                                                                          \
-    if (_r != ncclSuccess) {                                                                           \
-      fprintf(stderr, "%s(%d) : NCCL error : %s : %s\n", __FILE__, __LINE__, #expr,                    \
-              nccl().GetErrorString ? nccl().GetErrorString(_r) : "?");                                \
-      exit(EXIT_FAILURE);                                                                              \
-    }                                                                                                  \
-  } while (0)
+NcclApi& RequireNccl() {
+  if (!nccl().error.empty()) throw DeviceError("NCCL is not available: " + nccl().error);
+  return nccl();
+}
 }  // namespace
+
+const char* NcclErrorString(int result) {
+  return nccl().GetErrorString ? nccl().GetErrorString((ncclResult_t)result) : "unknown NCCL error";
+}
 
 DataParallelSync::DataParallelSync() {}
 DataParallelSync::~DataParallelSync() {
@@ -370,16 +361,14 @@ DataParallelSync::~DataParallelSync() {
   if (ready_) cudaEventDestroy(ready_);
   if (done_) cudaEventDestroy(done_);
 }
-bool DataParallelSync::GetUniqueId(char out[128]) {
-  if (!nccl().ok) return false;
+void DataParallelSync::GetUniqueId(char out[128]) {
   ncclUniqueId id;
   static_assert(sizeof(ncclUniqueId) == 128, "ncclUniqueId is 128 bytes");
-  NCCL_CHECK(nccl().GetUniqueId(&id));
+  NCCL_CHECK(RequireNccl().GetUniqueId(&id));
   memcpy(out, &id, 128);
-  return true;
 }
-bool DataParallelSync::Init(int rank, int world, const char idbytes[128]) {
-  if (!nccl().ok) return false;
+void DataParallelSync::Init(int rank, int world, const char idbytes[128]) {
+  RequireNccl();
   rank_ = rank; world_ = world;
   ncclUniqueId id;
   memcpy(&id, idbytes, 128);
@@ -407,18 +396,17 @@ bool DataParallelSync::Init(int rank, int world, const char idbytes[128]) {
     NCCL_CHECK(nccl().CommInitRank(&c, world, id, rank));
   }
   comm_ = c;
-  HOST_CUDA_CHECK(cudaStreamCreateWithFlags(&comm_stream_, cudaStreamNonBlocking));
-  HOST_CUDA_CHECK(cudaEventCreateWithFlags(&ready_, cudaEventDisableTiming));
-  HOST_CUDA_CHECK(cudaEventCreateWithFlags(&done_, cudaEventDisableTiming));
-  return true;
+  CUDA_CHECK(cudaStreamCreateWithFlags(&comm_stream_, cudaStreamNonBlocking));
+  CUDA_CHECK(cudaEventCreateWithFlags(&ready_, cudaEventDisableTiming));
+  CUDA_CHECK(cudaEventCreateWithFlags(&done_, cudaEventDisableTiming));
 }
 void DataParallelSync::Broadcast(float* buf, size_t count) {
   if (world_ <= 1) return;
-  HOST_CUDA_CHECK(cudaEventRecord(ready_, Matrix::Stream()));
-  HOST_CUDA_CHECK(cudaStreamWaitEvent(comm_stream_, ready_, 0));
+  CUDA_CHECK(cudaEventRecord(ready_, Matrix::Stream()));
+  CUDA_CHECK(cudaStreamWaitEvent(comm_stream_, ready_, 0));
   NCCL_CHECK(nccl().Bcast(buf, buf, count, ncclFloat, 0, (ncclComm_t)comm_, comm_stream_));
-  HOST_CUDA_CHECK(cudaEventRecord(done_, comm_stream_));
-  HOST_CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), done_, 0));
+  CUDA_CHECK(cudaEventRecord(done_, comm_stream_));
+  CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), done_, 0));
 }
 void DataParallelSync::AllReduceAverageAsync(float* buf, size_t offset, size_t count, cudaStream_t comm) {
   if (world_ <= 1 || count == 0) return;
@@ -428,7 +416,9 @@ void DataParallelSync::AllReduceAverageAsync(float* buf, size_t offset, size_t c
 // =================================================================== ConvNet
 ConvNet::ConvNet(const ModelConfig& model, int batch_size) : model_(model), batch_size_(batch_size) {
   // BuildNet (convnet.cc:150-270), restricted to chains: edge i connects layer i to layer i+1
-  if (model.layer.size() != model.edge.size() + 1) { fprintf(stderr, "ConvNet: model must be a chain\n"); exit(1); }
+  if (model.layer.size() != model.edge.size() + 1)
+    throw std::invalid_argument("ConvNet: the model must be a chain (" + std::to_string(model.layer.size()) + " layers, " +
+                                std::to_string(model.edge.size()) + " edges)");
   for (const LayerConfig& lc : model.layer) layers_.emplace_back(new Layer(lc));
   for (size_t i = 0; i < model.edge.size(); i++) {
     edges_.emplace_back(Edge::ChooseEdgeClass(model.edge[i]));
@@ -659,18 +649,18 @@ void ConvNet::AllocateMemory() {
   // so the edge takes the history, the step and the adaptive state from the file too
   for (size_t i = 0; i < edges_.size(); i++)
     if (owner_[i] == (int)i && model_.edge[i].initialization == PRETRAINED) LoadPretrained(i);
-  HOST_CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
+  CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
   InvalidateStaging();
-  HOST_CUDA_CHECK(cudaStreamCreateWithFlags(&side_, cudaStreamNonBlocking));
-  HOST_CUDA_CHECK(cudaStreamCreateWithFlags(&opt_, cudaStreamNonBlocking));
-  HOST_CUDA_CHECK(cudaEventCreateWithFlags(&ev_opt_, cudaEventDisableTiming));
-  HOST_CUDA_CHECK(cudaStreamCreateWithFlags(&comm_, cudaStreamNonBlocking));
-  HOST_CUDA_CHECK(cudaEventCreateWithFlags(&ev_comm_, cudaEventDisableTiming));
-  HOST_CUDA_CHECK(cudaEventCreateWithFlags(&ev_main_, cudaEventDisableTiming));
-  HOST_CUDA_CHECK(cudaEventCreateWithFlags(&ev_side_, cudaEventDisableTiming));
+  CUDA_CHECK(cudaStreamCreateWithFlags(&side_, cudaStreamNonBlocking));
+  CUDA_CHECK(cudaStreamCreateWithFlags(&opt_, cudaStreamNonBlocking));
+  CUDA_CHECK(cudaEventCreateWithFlags(&ev_opt_, cudaEventDisableTiming));
+  CUDA_CHECK(cudaStreamCreateWithFlags(&comm_, cudaStreamNonBlocking));
+  CUDA_CHECK(cudaEventCreateWithFlags(&ev_comm_, cudaEventDisableTiming));
+  CUDA_CHECK(cudaEventCreateWithFlags(&ev_main_, cudaEventDisableTiming));
+  CUDA_CHECK(cudaEventCreateWithFlags(&ev_side_, cudaEventDisableTiming));
   SetBucketFloats((size_t)8 << 20);
   lane_.stream = side_;
-  HOST_CUDA_CHECK(cudaEventCreateWithFlags(&lane_.ready, cudaEventDisableTiming));
+  CUDA_CHECK(cudaEventCreateWithFlags(&lane_.ready, cudaEventDisableTiming));
   for (auto& e : edges_)
     if (EdgeWithWeight* w = dynamic_cast<EdgeWithWeight*>(e.get())) w->SetSideLane(&lane_);
 }
@@ -789,14 +779,14 @@ void ConvNet::Bprop() {                                      // convnet.cc:390-4
         if (b.trigger != i - 1) continue;
         if (!comm_pending_) convnet_b200_reserve_sms(dp_->reserved_sms());
         // the bucket's gradients: weight gradients on the main stream, bias gradients (column sums) on the side stream
-        HOST_CUDA_CHECK(cudaEventRecord(ev_main_, Matrix::Stream()));
-        HOST_CUDA_CHECK(cudaStreamWaitEvent(comm_, ev_main_, 0));
-        HOST_CUDA_CHECK(cudaEventRecord(ev_side_, side_));
-        HOST_CUDA_CHECK(cudaStreamWaitEvent(comm_, ev_side_, 0));
-        if (trace_.on) HOST_CUDA_CHECK(cudaEventRecord(trace_.c0[bi], comm_));
+        CUDA_CHECK(cudaEventRecord(ev_main_, Matrix::Stream()));
+        CUDA_CHECK(cudaStreamWaitEvent(comm_, ev_main_, 0));
+        CUDA_CHECK(cudaEventRecord(ev_side_, side_));
+        CUDA_CHECK(cudaStreamWaitEvent(comm_, ev_side_, 0));
+        if (trace_.on) CUDA_CHECK(cudaEventRecord(trace_.c0[bi], comm_));
         dp_->AllReduceAverageAsync(grad_parameters_.GetDevData(), b.lo, b.hi - b.lo, comm_);
-        HOST_CUDA_CHECK(cudaEventRecord(ev_reduced_[bi], comm_));
-        if (trace_.on) HOST_CUDA_CHECK(cudaEventRecord(trace_.c1[bi], comm_));
+        CUDA_CHECK(cudaEventRecord(ev_reduced_[bi], comm_));
+        if (trace_.on) CUDA_CHECK(cudaEventRecord(trace_.c1[bi], comm_));
         comm_pending_ = true;
       }
     if (in->ReceivesDeriv()) {
@@ -813,9 +803,9 @@ void ConvNet::Bprop() {                                      // convnet.cc:390-4
     if (eager_update_)
       for (size_t bi = 0; bi < buckets_.size(); bi++)
         if (buckets_[bi].trigger == i - 1) {
-          if (dp_ && dp_->world() > 1) HOST_CUDA_CHECK(cudaStreamWaitEvent(opt_, ev_reduced_[bi], 0));   // SGD after its all-reduce
+          if (dp_ && dp_->world() > 1) CUDA_CHECK(cudaStreamWaitEvent(opt_, ev_reduced_[bi], 0));        // SGD after its all-reduce
           IssueBucketUpdate(buckets_[bi]);
-          if (trace_.on) HOST_CUDA_CHECK(cudaEventRecord(trace_.s1[bi], opt_));
+          if (trace_.on) CUDA_CHECK(cudaEventRecord(trace_.s1[bi], opt_));
         }
   }
   if (!eager_update_ && !(dp_ && dp_->world() > 1)) WaitSide();   // stand-alone Bprop: the gradients are complete on return
@@ -828,10 +818,10 @@ void ConvNet::IssueBucketUpdate(const Bucket& b) {
   std::vector<CnbOptTensorEx> tensors;
   AppendUpdates(b.trigger, b.last, tensors);
   if (tensors.empty()) return;
-  HOST_CUDA_CHECK(cudaEventRecord(ev_main_, Matrix::Stream()));
-  HOST_CUDA_CHECK(cudaStreamWaitEvent(opt_, ev_main_, 0));
-  HOST_CUDA_CHECK(cudaEventRecord(ev_side_, side_));
-  HOST_CUDA_CHECK(cudaStreamWaitEvent(opt_, ev_side_, 0));
+  CUDA_CHECK(cudaEventRecord(ev_main_, Matrix::Stream()));
+  CUDA_CHECK(cudaStreamWaitEvent(opt_, ev_main_, 0));
+  CUDA_CHECK(cudaEventRecord(ev_side_, side_));
+  CUDA_CHECK(cudaStreamWaitEvent(opt_, ev_side_, 0));
   void* main_stream = convnet_b200_get_stream();
   convnet_b200_set_stream(opt_);
   // the update, and the rescale of the rows of norm-limited tensors: both before the banks below are rebuilt from the weights
@@ -850,19 +840,19 @@ void ConvNet::IssueBucketUpdate(const Bucket& b) {
 void ConvNet::WaitSide() {
   if (lane_.used) { side_pending_ = true; lane_.used = false; }
   if (comm_pending_) {                                       // every all-reduce of the step (the SGD steps on side_ wait for theirs too)
-    HOST_CUDA_CHECK(cudaEventRecord(ev_comm_, comm_));
-    HOST_CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), ev_comm_, 0));
+    CUDA_CHECK(cudaEventRecord(ev_comm_, comm_));
+    CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), ev_comm_, 0));
     comm_pending_ = false;
     convnet_b200_reserve_sms(0);
   }
   if (opt_pending_) {
-    HOST_CUDA_CHECK(cudaEventRecord(ev_opt_, opt_));
-    HOST_CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), ev_opt_, 0));
+    CUDA_CHECK(cudaEventRecord(ev_opt_, opt_));
+    CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), ev_opt_, 0));
     opt_pending_ = false;
   }
   if (!side_pending_) return;
-  HOST_CUDA_CHECK(cudaEventRecord(ev_side_, side_));
-  HOST_CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), ev_side_, 0));
+  CUDA_CHECK(cudaEventRecord(ev_side_, side_));
+  CUDA_CHECK(cudaStreamWaitEvent(Matrix::Stream(), ev_side_, 0));
   side_pending_ = false;
 }
 
@@ -891,37 +881,37 @@ void ConvNet::ReduceLearningRate(float factor) {             // convnet.cc:820-8
 }
 
 void ConvNet::TrainOneBatch(float* loss_out) {               // convnet.cc:475-485 (GetBatch is the caller's H2D copy)
-  if (trace_.on) HOST_CUDA_CHECK(cudaEventRecord(trace_.t0, Matrix::Stream()));
+  if (trace_.on) CUDA_CHECK(cudaEventRecord(trace_.t0, Matrix::Stream()));
   Fprop(true);
   ComputeDeriv();
-  if (trace_.on) HOST_CUDA_CHECK(cudaEventRecord(trace_.fwd, Matrix::Stream()));
+  if (trace_.on) CUDA_CHECK(cudaEventRecord(trace_.fwd, Matrix::Stream()));
   if (loss_out) {                                            // GetLoss: one scalar D2H per step, like the reference
     cnb_sum(OutputLayer().GetLossPerImage(), loss_sum_.GetDevData(), batch_size_);
   }
   eager_update_ = true;
   Bprop();
-  if (trace_.on) HOST_CUDA_CHECK(cudaEventRecord(trace_.bwd, Matrix::Stream()));
+  if (trace_.on) CUDA_CHECK(cudaEventRecord(trace_.bwd, Matrix::Stream()));
   updated_in_bprop_ = true;
   eager_update_ = false;
   UpdateWeights();
-  if (trace_.on) HOST_CUDA_CHECK(cudaEventRecord(trace_.end, Matrix::Stream()));
+  if (trace_.on) CUDA_CHECK(cudaEventRecord(trace_.end, Matrix::Stream()));
   if (loss_out) *loss_out = OutputLayer().LossWeight() * loss_sum_.ReadValue(0);
   step_++;
 }
 
 std::vector<float> ConvNet::TraceStep() {
-  auto make = [](cudaEvent_t* e) { if (!*e) HOST_CUDA_CHECK(cudaEventCreate(e)); };
+  auto make = [](cudaEvent_t* e) { if (!*e) CUDA_CHECK(cudaEventCreate(e)); };
   make(&trace_.t0); make(&trace_.fwd); make(&trace_.bwd); make(&trace_.end);
   for (std::vector<cudaEvent_t>* v : {&trace_.c0, &trace_.c1, &trace_.s1})
     while (v->size() < buckets_.size()) { cudaEvent_t e = nullptr; make(&e); v->push_back(e); }
-  HOST_CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
+  CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
   trace_.on = true;
   TrainOneBatch(nullptr);
   trace_.on = false;
-  HOST_CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
-  HOST_CUDA_CHECK(cudaStreamSynchronize(side_));
-  HOST_CUDA_CHECK(cudaStreamSynchronize(opt_));
-  HOST_CUDA_CHECK(cudaStreamSynchronize(comm_));
+  CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
+  CUDA_CHECK(cudaStreamSynchronize(side_));
+  CUDA_CHECK(cudaStreamSynchronize(opt_));
+  CUDA_CHECK(cudaStreamSynchronize(comm_));
   auto since = [&](cudaEvent_t e) { float ms = -1.f; return cudaEventElapsedTime(&ms, trace_.t0, e) == cudaSuccess ? ms : -1.f; };
   std::vector<float> out = {since(trace_.fwd), since(trace_.bwd), since(trace_.end), (float)buckets_.size()};
   const bool multi = dp_ && dp_->world() > 1;
@@ -972,7 +962,7 @@ void ConvNet::SetBucketFloats(size_t bucket_floats) {
   buckets_ = PlanBuckets(edge_offset_, trained, bucket_floats);
   while (ev_reduced_.size() < buckets_.size()) {
     cudaEvent_t e;
-    HOST_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     ev_reduced_.push_back(e);
   }
 }
@@ -1003,8 +993,8 @@ double GradChecker::LossAtD(Matrix& w, size_t index, float value) {
   Layer& out = OutputLayer();
   out.ComputeDeriv();
   std::vector<float> h(batch_size_);
-  HOST_CUDA_CHECK(cudaMemcpyAsync(h.data(), out.GetLossPerImage(), sizeof(float) * batch_size_, cudaMemcpyDeviceToHost, Matrix::Stream()));
-  HOST_CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
+  CUDA_CHECK(cudaMemcpyAsync(h.data(), out.GetLossPerImage(), sizeof(float) * batch_size_, cudaMemcpyDeviceToHost, Matrix::Stream()));
+  CUDA_CHECK(cudaStreamSynchronize(Matrix::Stream()));
   double s = 0;
   for (float v : h) s += v;
   return (double)out.LossWeight() * s;
@@ -1021,7 +1011,7 @@ std::vector<GradCheckResult> GradChecker::Run(unsigned seed) {
   std::vector<int> hl(batch_size_);
   const int classes = OutputLayer().GetState().GetCols();
   for (int& v : hl) v = (int)(gen() % classes);
-  HOST_CUDA_CHECK(cudaMemcpy(OutputLayer().GetLabels(), hl.data(), sizeof(int) * batch_size_, cudaMemcpyHostToDevice));
+  CUDA_CHECK(cudaMemcpy(OutputLayer().GetLabels(), hl.data(), sizeof(int) * batch_size_, cudaMemcpyHostToDevice));
   Matrix& t = OutputLayer().GetTargets();                     // a per-feature target: one the loss function accepts
   if (t.GetNumEls()) {
     const int rows = t.GetRows(), cols = t.GetCols();

@@ -271,8 +271,8 @@ class DataParallelSync {
  public:
   DataParallelSync();
   ~DataParallelSync();
-  static bool GetUniqueId(char out[128]);                       // rank 0; bytes are broadcast by the launcher
-  bool Init(int rank, int world, const char id[128]);
+  static void GetUniqueId(char out[128]);                       // rank 0; bytes are broadcast by the launcher
+  void Init(int rank, int world, const char id[128]);
   int world() const { return world_; }
   int rank() const { return rank_; }
   void Broadcast(float* buf, size_t count);                     // initial parameters from rank 0 (convnet.cc:300-309)

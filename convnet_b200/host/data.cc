@@ -1,8 +1,6 @@
 // data.cc — see data.h.
 #include "data.h"
 
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <stdexcept>
 #include <string>
@@ -11,16 +9,16 @@
 
 namespace cnbhost {
 
-#define DATA_CUDA_CHECK(expr)                                                                          \
-  do {                                                                                                 \
-    cudaError_t _e = (expr);                                                                           \
-    if (_e != cudaSuccess) { fprintf(stderr, "%s(%d): %s: %s\n", __FILE__, __LINE__, #expr, cudaGetErrorString(_e)); exit(1); } \
-  } while (0)
-
 uint64_t SplitMix64(uint64_t& state) {
   uint64_t z = (state += 0x9E3779B97F4A7C15ULL);
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL; z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
   return z ^ (z >> 31);
+}
+
+// the status of a crop launch: 0 ok, -1 shapes or pointers it cannot crop with, -3 the launch failed
+static void CheckCrop(const char* call, int rc) {
+  if (rc == -3) throw DeviceError(std::string(call) + ": the launch failed");
+  if (rc != 0) throw std::invalid_argument(std::string(call) + " cannot crop with these shapes or pointers");
 }
 
 // ---------------------------------------------------------------- Jitter
@@ -57,12 +55,9 @@ void Jitter::Sample(int batch_size, int multiplicity_id, float* out) {
 }
 
 // ---------------------------------------------------------------- NoiseStage
-NoiseStage::NoiseStage() {
-  for (int k = 0; k < kRing; k++) DATA_CUDA_CHECK(cudaEventCreateWithFlags(&done_[k], cudaEventDisableTiming));
-}
-
 NoiseStage::~NoiseStage() {
-  if (pinned_) cudaStreamSynchronize(Matrix::Stream());      // copies may still read the ring, crops the device block
+  if (!pinned_) return;                                      // nothing staged yet: nothing was created
+  cudaStreamSynchronize(Matrix::Stream());                   // copies may still read the ring, crops the device block
   for (int k = 0; k < kRing; k++) cudaEventDestroy(done_[k]);
   cudaFree(device_); cudaFreeHost(pinned_);
 }
@@ -71,18 +66,20 @@ const float* NoiseStage::Stage(Jitter& jitter, int batch_size, int multiplicity_
   const cudaStream_t s = Matrix::Stream();
   if (batch_size > cap_) {
     if (pinned_) {
-      DATA_CUDA_CHECK(cudaStreamSynchronize(s));
-      DATA_CUDA_CHECK(cudaFree(device_)); DATA_CUDA_CHECK(cudaFreeHost(pinned_));
+      CUDA_CHECK(cudaStreamSynchronize(s));
+      CUDA_CHECK(cudaFree(device_)); CUDA_CHECK(cudaFreeHost(pinned_));
+    } else {
+      for (int k = 0; k < kRing; k++) CUDA_CHECK(cudaEventCreateWithFlags(&done_[k], cudaEventDisableTiming));
     }
-    DATA_CUDA_CHECK(cudaMalloc((void**)&device_, sizeof(float) * 3 * (size_t)batch_size));
-    DATA_CUDA_CHECK(cudaMallocHost((void**)&pinned_, sizeof(float) * 3 * (size_t)batch_size * kRing));
+    CUDA_CHECK(cudaMalloc((void**)&device_, sizeof(float) * 3 * (size_t)batch_size));
+    CUDA_CHECK(cudaMallocHost((void**)&pinned_, sizeof(float) * 3 * (size_t)batch_size * kRing));
     cap_ = batch_size;
   }
   float* block = pinned_ + (size_t)slot_ * 3 * cap_;
-  DATA_CUDA_CHECK(cudaEventSynchronize(done_[slot_]));      // kRing batches ago: long done
+  CUDA_CHECK(cudaEventSynchronize(done_[slot_]));           // kRing batches ago: long done
   jitter.Sample(batch_size, multiplicity_id, block);
-  DATA_CUDA_CHECK(cudaMemcpyAsync(device_, block, sizeof(float) * 3 * batch_size, cudaMemcpyHostToDevice, s));
-  DATA_CUDA_CHECK(cudaEventRecord(done_[slot_], s));
+  CUDA_CHECK(cudaMemcpyAsync(device_, block, sizeof(float) * 3 * batch_size, cudaMemcpyHostToDevice, s));
+  CUDA_CHECK(cudaEventRecord(done_[slot_], s));
   slot_ = (slot_ + 1) % kRing;
   last_ = block;
   last_batch_ = batch_size;
@@ -95,31 +92,33 @@ DataIterator::DataIterator(int chunk_size, int channels, int image_size_y, int i
     : chunk_size_(chunk_size), channels_(channels), image_size_y_(image_size_y), image_size_x_(image_size_x),
       gpu_image_size_y_(gpu_image_size_y), gpu_image_size_x_(gpu_image_size_x),
       jitter_(image_size_y, image_size_x, gpu_image_size_y, gpu_image_size_x, translate, flip, seed) {
-  if (gpu_image_size_y > image_size_y || gpu_image_size_x > image_size_x || chunk_size <= 0 || channels <= 0) {
-    fprintf(stderr, "DataIterator: the crop must fit the image\n"); exit(1);
-  }
+  if (chunk_size <= 0 || channels <= 0) throw std::invalid_argument("DataIterator: chunk_size and channels must be positive");
+  if (gpu_image_size_y > image_size_y || gpu_image_size_x > image_size_x)
+    throw std::invalid_argument("DataIterator: the crop (gpu_image_size " + std::to_string(gpu_image_size_y) + " x " +
+                                std::to_string(gpu_image_size_x) + ") must fit the image (image_size " +
+                                std::to_string(image_size_y) + " x " + std::to_string(image_size_x) + ")");
   data_.AllocateGPUMemory(NumDims(), chunk_size);          // one image per column (src/datahandler.cc:60-75)
 }
 
 void DataIterator::Upload(const float* host, int first, int count) {
-  if (first < 0 || count < 0 || first + count > chunk_size_) { fprintf(stderr, "DataIterator::Upload: out of range\n"); exit(1); }
-  DATA_CUDA_CHECK(cudaMemcpyAsync(data_.GetDevData() + (size_t)first * NumDims(), host, sizeof(float) * (size_t)count * NumDims(),
-                                  cudaMemcpyHostToDevice, Matrix::Stream()));
+  if (first < 0 || count < 0 || first + count > chunk_size_)
+    throw std::invalid_argument("DataIterator::Upload: images [" + std::to_string(first) + ", " + std::to_string(first + count) +
+                                ") are outside the chunk of " + std::to_string(chunk_size_));
+  CUDA_CHECK(cudaMemcpyAsync(data_.GetDevData() + (size_t)first * NumDims(), host, sizeof(float) * (size_t)count * NumDims(),
+                             cudaMemcpyHostToDevice, Matrix::Stream()));
 }
 
 void DataIterator::AddNoise(int start, Matrix& dest) {
   const int batch_size = dest.GetRows();
-  if (start < 0 || start + batch_size > chunk_size_ || noise_.LastBatch() != batch_size) {
-    fprintf(stderr, "DataIterator::AddNoise: slice out of range, or SampleNoise was not called for this batch size\n"); exit(1);
-  }
-  if (dest.GetCols() != channels_ * gpu_image_size_y_ * gpu_image_size_x_) {
-    fprintf(stderr, "DataIterator::AddNoise: dest is not batch x channels * crop\n"); exit(1);
-  }
+  if (start < 0 || start + batch_size > chunk_size_ || noise_.LastBatch() != batch_size)
+    throw std::invalid_argument("DataIterator::AddNoise: slice out of range, or SampleNoise was not called for this batch size");
+  if (dest.GetCols() != channels_ * gpu_image_size_y_ * gpu_image_size_x_)
+    throw std::invalid_argument("DataIterator::AddNoise: dest is not batch x channels * crop");
   // (the reference copies with CopyTranspose when there is neither crop nor mirror; the same kernel covers that case)
   const int rc = cnb_extract_patches(data_.GetDevData() + (size_t)start * NumDims(), dest.GetDevData(), nullptr, d_noise_,
                                      d_noise_ + batch_size, d_noise_ + 2 * batch_size, batch_size, channels_, image_size_x_,
                                      image_size_y_, gpu_image_size_x_, gpu_image_size_y_, nullptr, nullptr, nullptr, nullptr, 0);
-  if (rc != 0) { fprintf(stderr, "Error extracting patches (%d)\n", rc); exit(1); }
+  CheckCrop("DataIterator::AddNoise: cnb_extract_patches", rc);
 }
 
 // ---------------------------------------------------------------- DataSchedule
@@ -231,18 +230,18 @@ DataHandler::DataHandler(const DatasetOrder& c, int dataset_size, int channels, 
   const size_t chunk = (size_t)schedule_.ChunkSize(), dims = (size_t)channels * isy_ * isx_;
   const int nbuf = schedule_.Pipelined() && !schedule_.FitsOnGpu() ? 2 : 1;
   for (int b = 0; b < nbuf; b++) {
-    DATA_CUDA_CHECK(cudaMalloc((void**)&d_images_[b], sizeof(float) * chunk * dims));
-    if (labels_) DATA_CUDA_CHECK(cudaMalloc((void**)&d_labels_[b], sizeof(int) * chunk));
-    if (targets_) DATA_CUDA_CHECK(cudaMalloc((void**)&d_targets_[b], sizeof(float) * chunk * target_dims_));
+    CUDA_CHECK(cudaMalloc((void**)&d_images_[b], sizeof(float) * chunk * dims));
+    if (labels_) CUDA_CHECK(cudaMalloc((void**)&d_labels_[b], sizeof(int) * chunk));
+    if (targets_) CUDA_CHECK(cudaMalloc((void**)&d_targets_[b], sizeof(float) * chunk * target_dims_));
   }
-  DATA_CUDA_CHECK(cudaMalloc((void**)&d_perm_, sizeof(int) * chunk));
-  DATA_CUDA_CHECK(cudaMallocHost((void**)&pinned_perm_, sizeof(int) * chunk * kRing));
-  for (int k = 0; k < kRing; k++) DATA_CUDA_CHECK(cudaEventCreateWithFlags(&perm_done_[k], cudaEventDisableTiming));
+  CUDA_CHECK(cudaMalloc((void**)&d_perm_, sizeof(int) * chunk));
+  CUDA_CHECK(cudaMallocHost((void**)&pinned_perm_, sizeof(int) * chunk * kRing));
+  for (int k = 0; k < kRing; k++) CUDA_CHECK(cudaEventCreateWithFlags(&perm_done_[k], cudaEventDisableTiming));
   for (int b = 0; b < 2; b++) {
-    DATA_CUDA_CHECK(cudaEventCreateWithFlags(&loaded_[b], cudaEventDisableTiming));
-    DATA_CUDA_CHECK(cudaEventCreateWithFlags(&consumed_[b], cudaEventDisableTiming));
+    CUDA_CHECK(cudaEventCreateWithFlags(&loaded_[b], cudaEventDisableTiming));
+    CUDA_CHECK(cudaEventCreateWithFlags(&consumed_[b], cudaEventDisableTiming));
   }
-  if (nbuf == 2) DATA_CUDA_CHECK(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
+  if (nbuf == 2) CUDA_CHECK(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
   UploadPermutation();                                              // the identity, until a pass reshuffles it
 }
 
@@ -265,12 +264,12 @@ void DataHandler::CopyRows(const std::vector<int>& rows, int buf, cudaStream_t s
     size_t run = 1;
     while (i + run < rows.size() && rows[i + run] == rows[i] + (int)run) run++;
     const size_t r = (size_t)rows[i];
-    DATA_CUDA_CHECK(cudaMemcpyAsync(d_images_[buf] + i * dims, images_ + r * dims, sizeof(float) * run * dims,
-                                    cudaMemcpyHostToDevice, s));
-    if (labels_) DATA_CUDA_CHECK(cudaMemcpyAsync(d_labels_[buf] + i, labels_ + r, sizeof(int) * run, cudaMemcpyHostToDevice, s));
+    CUDA_CHECK(cudaMemcpyAsync(d_images_[buf] + i * dims, images_ + r * dims, sizeof(float) * run * dims,
+                               cudaMemcpyHostToDevice, s));
+    if (labels_) CUDA_CHECK(cudaMemcpyAsync(d_labels_[buf] + i, labels_ + r, sizeof(int) * run, cudaMemcpyHostToDevice, s));
     if (targets_)
-      DATA_CUDA_CHECK(cudaMemcpyAsync(d_targets_[buf] + i * target_dims_, targets_ + r * target_dims_,
-                                      sizeof(float) * run * target_dims_, cudaMemcpyHostToDevice, s));
+      CUDA_CHECK(cudaMemcpyAsync(d_targets_[buf] + i * target_dims_, targets_ + r * target_dims_,
+                                 sizeof(float) * run * target_dims_, cudaMemcpyHostToDevice, s));
     i += run;
   }
 }
@@ -280,10 +279,10 @@ void DataHandler::UploadPermutation() {
   perm_slot_ = (perm_slot_ + 1) % kRing;
   const std::vector<int>& perm = schedule_.Permutation();
   int* block = pinned_perm_ + (size_t)slot * perm.size();
-  DATA_CUDA_CHECK(cudaEventSynchronize(perm_done_[slot]));          // the block's last copy has left it
+  CUDA_CHECK(cudaEventSynchronize(perm_done_[slot]));               // the block's last copy has left it
   memcpy(block, perm.data(), sizeof(int) * perm.size());
-  DATA_CUDA_CHECK(cudaMemcpyAsync(d_perm_, block, sizeof(int) * perm.size(), cudaMemcpyHostToDevice, Matrix::Stream()));
-  DATA_CUDA_CHECK(cudaEventRecord(perm_done_[slot], Matrix::Stream()));
+  CUDA_CHECK(cudaMemcpyAsync(d_perm_, block, sizeof(int) * perm.size(), cudaMemcpyHostToDevice, Matrix::Stream()));
+  CUDA_CHECK(cudaEventRecord(perm_done_[slot], Matrix::Stream()));
 }
 
 void DataHandler::Seek(int row) {
@@ -305,18 +304,18 @@ void DataHandler::GetBatch(Matrix& input, int* labels_out, float* targets_out) {
     } else {                                                        // WaitForPreload: swap in the staged chunk
       const int next = 1 - cur_;
       if (!staged_) {                                               // a preload begun within this GetBatch (a restart)
-        DATA_CUDA_CHECK(cudaStreamWaitEvent(copy_stream_, consumed_[next], 0));
+        CUDA_CHECK(cudaStreamWaitEvent(copy_stream_, consumed_[next], 0));
         CopyRows(schedule_.Rows(), next, copy_stream_);
-        DATA_CUDA_CHECK(cudaEventRecord(loaded_[next], copy_stream_));
+        CUDA_CHECK(cudaEventRecord(loaded_[next], copy_stream_));
       }
-      DATA_CUDA_CHECK(cudaStreamWaitEvent(s, loaded_[next], 0));
-      DATA_CUDA_CHECK(cudaEventRecord(consumed_[cur_], s));         // behind the last crop that read the old chunk
+      CUDA_CHECK(cudaStreamWaitEvent(s, loaded_[next], 0));
+      CUDA_CHECK(cudaEventRecord(consumed_[cur_], s));              // behind the last crop that read the old chunk
       cur_ = next;
       staged_ = false;
       if (!schedule_.PreloadRows().empty()) {                       // StartPreload: the next chunk into the free buffer
-        DATA_CUDA_CHECK(cudaStreamWaitEvent(copy_stream_, consumed_[1 - cur_], 0));
+        CUDA_CHECK(cudaStreamWaitEvent(copy_stream_, consumed_[1 - cur_], 0));
         CopyRows(schedule_.PreloadRows(), 1 - cur_, copy_stream_);
-        DATA_CUDA_CHECK(cudaEventRecord(loaded_[1 - cur_], copy_stream_));
+        CUDA_CHECK(cudaEventRecord(loaded_[1 - cur_], copy_stream_));
         staged_ = true;
       }
     }
@@ -327,7 +326,7 @@ void DataHandler::GetBatch(Matrix& input, int* labels_out, float* targets_out) {
                                              noise + batch_, noise + 2 * batch_, batch_, channels_, isx_, isy_, gx_, gy_,
                                              labels_out ? d_labels_[cur_] : nullptr, labels_out,
                                              targets_out ? d_targets_[cur_] : nullptr, targets_out, target_dims_);
-  if (rc != 0) { fprintf(stderr, "DataHandler::GetBatch: cnb_extract_patches_indexed returned %d\n", rc); exit(1); }
+  CheckCrop("DataHandler::GetBatch: cnb_extract_patches_indexed", rc);
 }
 
 void DataHandler::GetBatch(ConvNet& net) {

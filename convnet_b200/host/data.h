@@ -44,7 +44,7 @@ class Jitter {
 // lands in and the crop reads.  A batch larger than any before grows both, once the stream has drained.
 class NoiseStage {
  public:
-  NoiseStage();
+  NoiseStage() = default;                         // creates nothing on the device: the first Stage does
   ~NoiseStage();
   // draws a batch's jitter and copies it on Matrix::Stream(); returns the device block
   const float* Stage(Jitter& jitter, int batch_size, int multiplicity_id);
@@ -57,7 +57,7 @@ class NoiseStage {
   float* device_ = nullptr;                       // 3 x cap_
   const float* last_ = nullptr;
   int cap_ = 0, last_batch_ = 0, slot_ = 0;
-  cudaEvent_t done_[kRing];
+  cudaEvent_t done_[kRing] = {};
 };
 
 class DataIterator {

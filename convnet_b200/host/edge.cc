@@ -2,9 +2,9 @@
 #include "edge.h"
 
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
 #include <random>
+#include <stdexcept>
+#include <string>
 #include <vector>
 
 namespace cnbhost {
@@ -17,6 +17,11 @@ Edge::Edge(const EdgeConfig& c)
     : config_(c), name_(c.name.empty() ? c.source + ":" + c.dest : c.name), source_(nullptr), dest_(nullptr),
       num_input_channels_(0), num_output_channels_(0), image_size_y_(0), image_size_x_(0), image_size_t_(1),
       num_modules_y_(1), num_modules_x_(1), num_modules_t_(1), batch_size_(0) {}
+
+// a chain has one edge into each layer, so every edge overwrites its output: the accumulating paths are not implemented
+static void NotOverwrite(const char* what) {
+  throw std::logic_error(std::string(what) + ": another edge writes this edge's output, which is not implemented");
+}
 
 Edge* Edge::ChooseEdgeClass(const EdgeConfig& c) {          // src/edge.cc:17-60
   switch (c.edge_type) {
@@ -31,8 +36,7 @@ Edge* Edge::ChooseEdgeClass(const EdgeConfig& c) {          // src/edge.cc:17-60
     case DOWNSAMPLE: return new DownSampleEdge(c);
     case RGBTOYUV: return new RgbToYuvEdge(c);
   }
-  fprintf(stderr, "Error: Undefined edge type.\n");
-  exit(1);
+  throw std::logic_error("Edge::ChooseEdgeClass: edge type " + std::to_string((int)c.edge_type) + " is not defined");
 }
 
 ConvDesc Edge::GetConvDesc(const EdgeConfig& c) {           // src/edge.cc:87-106
@@ -418,10 +422,7 @@ void MaxPoolEdge::SetImageSize(int y, int x, int t) {        // maxpool_edge.cc:
   Edge::SetImageSize(y, x, t, conv_desc_);
 }
 void MaxPoolEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) {   // :50-58
-  if (!overwrite) {
-    fprintf(stderr, " In MaxPoolEdge::ComputeUp() : some other layer is writing to this maxpool layer's output. Not implemented.\n");
-    exit(1);
-  }
+  if (!overwrite) NotOverwrite("MaxPoolEdge::ComputeUp()");
   ArmUp(nullptr, up_req_.emit);
   // training: have the kernel record which window elements equal the maximum; ComputeDown then reads those masks instead of
   // re-reading and comparing input and output (nothing between the two calls writes either tensor except through the library,
@@ -434,7 +435,7 @@ void MaxPoolEdge::ComputeDown(Matrix& deriv_output, Matrix& input, Matrix& outpu
   Matrix::ConvMaxPoolUndo(input, deriv_output, output, deriv_input, conv_desc_, overwrite ? 0 : 1);
 }
 void AvgPoolEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool train) {   // avgpool_edge.cc:50-58
-  if (!overwrite) { fprintf(stderr, " In AvgPoolEdge::ComputeUp() : not implemented for non-overwrite.\n"); exit(1); }
+  if (!overwrite) NotOverwrite("AvgPoolEdge::ComputeUp()");
   ArmUp(nullptr, up_req_.emit);
   Matrix::ConvAvgPool(input, output, conv_desc_);
 }
@@ -472,10 +473,6 @@ ConvDesc SampleEdge::Desc() const {
   d.padding_y = d.padding_x = d.padding_t = 0;
   d.num_input_channels = d.num_output_channels = d.input_channel_end = d.output_channel_end = num_input_channels_ * image_size_t_;
   return d;
-}
-static void NotOverwrite(const char* what) {
-  fprintf(stderr, " In %s : some other layer is writing to this layer. Not implemented.\n", what);
-  exit(1);
 }
 
 void UpSampleEdge::SetImageSize(int y, int x, int t) {        // upsample_edge.cc:17-22
@@ -517,8 +514,7 @@ void RgbToYuvEdge::ComputeUp(Matrix& input, Matrix& output, bool overwrite, bool
   Matrix::ConvRGBToYUV(input, output);
 }
 void RgbToYuvEdge::ComputeDown(Matrix&, Matrix&, Matrix&, Matrix&, bool) {
-  fprintf(stderr, "RgbToYuvEdge::ComputeDown: RGBTOYUV has no backward pass\n");
-  exit(1);
+  throw std::logic_error("RgbToYuvEdge::ComputeDown: RGBTOYUV has no backward pass");
 }
 
 }  // namespace cnbhost

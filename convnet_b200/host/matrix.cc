@@ -3,19 +3,11 @@
 
 #include "../../include/convnet_b200_conv.h"
 
-#include <cstdio>
-#include <cstdlib>
+#include <stdexcept>
+#include <string>
+#include <vector>
 
 namespace cnbhost {
-
-#define HOST_CUDA_CHECK(expr)                                                                         \
-  do {                                                                                                \
-    cudaError_t _e = (expr);                                                                          \
-    if (_e != cudaSuccess) {                                                                          \
-      fprintf(stderr, "%s(%d) : CUDA error : %s : %s\n", __FILE__, __LINE__, #expr, cudaGetErrorString(_e)); \
-      exit(EXIT_FAILURE);                                                                             \
-    }                                                                                                 \
-  } while (0)
 
 cudaStream_t Matrix::Stream() { return (cudaStream_t)convnet_b200_get_stream(); }
 
@@ -31,11 +23,11 @@ Matrix::~Matrix() {
 }
 
 void Matrix::AllocateGPUMemory(int rows, int cols) {
-  if (owns_ && mat_.data_device) { HOST_CUDA_CHECK(cudaFree(mat_.data_device)); mat_.data_device = nullptr; }
+  if (owns_ && mat_.data_device) { CUDA_CHECK(cudaFree(mat_.data_device)); mat_.data_device = nullptr; }
   const size_t n = (size_t)rows * cols;
   if (n > 0) {
-    HOST_CUDA_CHECK(cudaMalloc((void**)&mat_.data_device, n * sizeof(float)));
-    HOST_CUDA_CHECK(cudaMemsetAsync(mat_.data_device, 0, n * sizeof(float), Stream()));   // the reference calloc's + uploads
+    CUDA_CHECK(cudaMalloc((void**)&mat_.data_device, n * sizeof(float)));
+    CUDA_CHECK(cudaMemsetAsync(mat_.data_device, 0, n * sizeof(float), Stream()));        // the reference calloc's + uploads
   }
   owns_ = true; mat_.owns_data = 1;
   mat_.size[0] = rows; mat_.size[1] = cols;
@@ -54,7 +46,9 @@ void Matrix::Reshape(int rows, int cols) {
   const size_t n = GetNumEls();
   if (rows < 0) rows = (int)(n / cols);
   if (cols < 0) cols = (int)(n / rows);
-  if ((size_t)rows * cols != n) { fprintf(stderr, "Matrix::Reshape: size mismatch\n"); abort(); }
+  if ((size_t)rows * cols != n)
+    throw std::logic_error("Matrix::Reshape: " + std::to_string(rows) + " x " + std::to_string(cols) + " for " +
+                           std::to_string(n) + " elements");
   mat_.size[0] = rows; mat_.size[1] = cols;
 }
 
@@ -63,30 +57,28 @@ void Matrix::SetShape4D(int d1, int d2, int d3, int d4) {
 }
 
 void Matrix::Set(float v) {
-  if (v == 0.f) { HOST_CUDA_CHECK(cudaMemsetAsync(mat_.data_device, 0, GetNumEls() * sizeof(float), Stream())); return; }
+  if (v == 0.f) { CUDA_CHECK(cudaMemsetAsync(mat_.data_device, 0, GetNumEls() * sizeof(float), Stream())); return; }
   // rare path (non-zero constants): host staging
-  float* tmp = (float*)malloc(GetNumEls() * sizeof(float));
-  for (size_t i = 0; i < GetNumEls(); i++) tmp[i] = v;
-  HOST_CUDA_CHECK(cudaMemcpyAsync(mat_.data_device, tmp, GetNumEls() * sizeof(float), cudaMemcpyHostToDevice, Stream()));
-  HOST_CUDA_CHECK(cudaStreamSynchronize(Stream()));
-  free(tmp);
+  const std::vector<float> tmp(GetNumEls(), v);
+  CUDA_CHECK(cudaMemcpyAsync(mat_.data_device, tmp.data(), GetNumEls() * sizeof(float), cudaMemcpyHostToDevice, Stream()));
+  CUDA_CHECK(cudaStreamSynchronize(Stream()));
 }
 void Matrix::CopyFromHost(const float* src, size_t n) {
-  HOST_CUDA_CHECK(cudaMemcpyAsync(mat_.data_device, src, n * sizeof(float), cudaMemcpyHostToDevice, Stream()));
+  CUDA_CHECK(cudaMemcpyAsync(mat_.data_device, src, n * sizeof(float), cudaMemcpyHostToDevice, Stream()));
 }
 void Matrix::CopyToHost(float* dst, size_t n) {
-  HOST_CUDA_CHECK(cudaMemcpyAsync(dst, mat_.data_device, n * sizeof(float), cudaMemcpyDeviceToHost, Stream()));
-  HOST_CUDA_CHECK(cudaStreamSynchronize(Stream()));
+  CUDA_CHECK(cudaMemcpyAsync(dst, mat_.data_device, n * sizeof(float), cudaMemcpyDeviceToHost, Stream()));
+  CUDA_CHECK(cudaStreamSynchronize(Stream()));
 }
 float Matrix::ReadValue(size_t index) {
   float v;
-  HOST_CUDA_CHECK(cudaMemcpyAsync(&v, mat_.data_device + index, sizeof(float), cudaMemcpyDeviceToHost, Stream()));
-  HOST_CUDA_CHECK(cudaStreamSynchronize(Stream()));
+  CUDA_CHECK(cudaMemcpyAsync(&v, mat_.data_device + index, sizeof(float), cudaMemcpyDeviceToHost, Stream()));
+  CUDA_CHECK(cudaStreamSynchronize(Stream()));
   return v;
 }
 void Matrix::WriteValue(size_t index, float v) {
-  HOST_CUDA_CHECK(cudaMemcpyAsync(mat_.data_device + index, &v, sizeof(float), cudaMemcpyHostToDevice, Stream()));
-  HOST_CUDA_CHECK(cudaStreamSynchronize(Stream()));
+  CUDA_CHECK(cudaMemcpyAsync(mat_.data_device + index, &v, sizeof(float), cudaMemcpyHostToDevice, Stream()));
+  CUDA_CHECK(cudaStreamSynchronize(Stream()));
 }
 
 void Matrix::AddRowVec(Matrix& v) { cnb_add_channel_bias(mat_.data_device, v.GetDevData(), GetRows(), GetCols()); }
@@ -175,6 +167,6 @@ void Matrix::ConvResponseNormCrossMapUndo3D(Matrix& outGrads, Matrix& inputs, Ma
                                  powScale, blocked, image_size_t);
 }
 
-void Matrix::SetupCUDADevice(int board) { HOST_CUDA_CHECK(cudaSetDevice(board)); }
+void Matrix::SetupCUDADevice(int board) { CUDA_CHECK(cudaSetDevice(board)); }
 
 }  // namespace cnbhost

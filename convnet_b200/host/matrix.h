@@ -14,6 +14,7 @@
 
 #include "../../include/convnet_b200_conv_gemm.h"
 #include "../../include/convnet_b200_ext.h"
+#include "check.h"
 
 namespace cnbhost {
 

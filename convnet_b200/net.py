@@ -87,11 +87,11 @@ def load_host():
             "cnb_net_output": ([vp], vp), "cnb_net_num_classes": ([vp], i), "cnb_net_params": ([vp], vp),
             "cnb_net_grads": ([vp], vp), "cnb_net_layer_state": ([vp, i], vp), "cnb_net_layer_floats": ([vp, i], ll),
             "cnb_net_num_layers": ([vp], i), "cnb_net_device_loss": ([vp], vp),
-            "cnb_net_fprop": ([vp, i], None), "cnb_net_bprop": ([vp], None), "cnb_net_update": ([vp], None),
-            "cnb_net_loss": ([vp], f), "cnb_net_train_step": ([vp, ct.POINTER(f)], None),
+            "cnb_net_fprop": ([vp, i], i), "cnb_net_bprop": ([vp], i), "cnb_net_update": ([vp], i),
+            "cnb_net_loss": ([vp, ct.POINTER(f)], i), "cnb_net_train_step": ([vp, ct.POINTER(f)], i),
             "cnb_net_trace_step": ([vp, ct.POINTER(f), i], i),
             "cnb_data_create": ([i, i, i, i, i, i, i, i, ct.c_ulonglong], vp), "cnb_data_destroy": ([vp], None),
-            "cnb_data_upload": ([vp, vp, i, i], None), "cnb_data_get_batch": ([vp, vp, i, i], None),
+            "cnb_data_upload": ([vp, vp, i, i], i), "cnb_data_get_batch": ([vp, vp, i, i], i),
             "cnb_data_last_noise": ([vp, ct.POINTER(f), i], i),
             "cnb_data_view_offset": ([i, i, i, ct.POINTER(i), ct.POINTER(i)], None),
             "cnb_dp_unique_id": ([ct.c_char_p], i), "cnb_net_dp_init": ([vp, i, i, ct.c_char_p, ll], i),
@@ -107,11 +107,12 @@ def load_host():
             "cnb_net_layer_bn": ([vp, i, ct.POINTER(f), ct.POINTER(f)], None),
             "cnb_net_bn_offset": ([vp, i], ll), "cnb_net_bn_stat": ([vp, i, i], vp),
             "cnb_bn_optimizer_check": ([ct.POINTER(OptimizerConfig)], i),
-            "cnb_net_targets": ([vp], vp), "cnb_net_targets_floats": ([vp], ll), "cnb_net_metric": ([vp], f),
+            "cnb_net_targets": ([vp], vp), "cnb_net_targets_floats": ([vp], ll), "cnb_net_metric": ([vp, ct.POINTER(f)], i),
             "cnb_net_output_layer": ([vp, ct.POINTER(i), ct.POINTER(i), ct.POINTER(i), ct.POINTER(f), ct.POINTER(i)], None),
             "cnb_net_model_text": ([vp, ct.c_char_p, ll], ll),
             "cnb_net_initial_weights": ([vp, i, ct.c_uint, ct.POINTER(f), ll], ll),
-            "cnb_net_history": ([vp], vp), "cnb_last_error": ([], ct.c_char_p), "cnb_net_save": ([vp, ct.c_char_p], i),
+            "cnb_net_history": ([vp], vp), "cnb_last_error": ([], ct.c_char_p), "cnb_last_status": ([], i),
+            "cnb_net_save": ([vp, ct.c_char_p], i),
             "cnb_net_load": ([vp, ct.c_char_p], i), "cnb_net_iteration": ([vp], ll),
             "cnb_net_polyak_insert": ([vp], i), "cnb_net_load_polyak_weights": ([vp], i),
             "cnb_net_load_current_weights": ([vp], i), "cnb_net_polyak_count": ([vp], i),
@@ -145,6 +146,19 @@ def load_host():
     return _host
 
 
+def _check(rc):
+    """the result of a host call that can fail: a status, count or handle passes through; a failure raises, with the host's
+    reason (cnb_last_error) as its message: ValueError for a refusal (-1), RuntimeError for a failed CUDA or NCCL call
+    (-2), and for a NULL handle whichever of the two cnb_last_status() names.  After a RuntimeError in the middle of a
+    step the net's state is undefined, and close() is the only safe call left on it."""
+    H = load_host()
+    if rc is None:
+        rc = H.cnb_last_status()
+    if rc >= 0:
+        return rc
+    raise (RuntimeError if rc == -2 else ValueError)(H.cnb_last_error().decode())
+
+
 class Model:
     """A model's chain built on the host only, for describing it: its edges, layers, parameter layout, fusion plan and
     FLOPs at `batch`, without device memory.  `model` is a built-in name or a model file, with suffixes, as for Net.  A
@@ -154,9 +168,8 @@ class Model:
         self._open(model, batch, load_host().cnb_model_open(model.encode(), batch))
 
     def _open(self, model, batch, h):
-        self.H, self.h, self.model, self.batch_size = load_host(), h, model, batch
-        if not h:
-            raise ValueError(self.H.cnb_last_error().decode())
+        self.H, self.h, self.model, self.batch_size = load_host(), None, model, batch
+        self.h = _check(h)
 
     def close(self):
         if self.h:
@@ -238,7 +251,8 @@ class Net(Model):
     One output suffix at most: "+squared-error" (LINEAR output, SQUARED_ERROR), "+binary-ce" (LOGISTIC output,
     CROSS_ENTROPY_BINARY, metric CLASSIFICATION_BINARY), "+soft-targets" (SOFTMAX_DIST, CROSS_ENTROPY_MULTINOMIAL_DISTRIBUTED);
     such outputs train on targets_tensor() instead of labels_tensor().  "logcheck": the gradcheck net with logistic units.
-    A model that cannot be read or run raises ValueError with the reason (for a file: its line and field), as Model does.
+    A model that cannot be read or run raises ValueError with the reason (for a file: its line and field), as Model does;
+    a device that cannot hold it (or no device) RuntimeError with the CUDA error.
 
     Tied edges (the reference's Edge.tied_to, see model_ties()) run with their owner's weights and bias and add their
     gradients to the owner's: they own no parameters (edges() reports size 0 and the owner's offset), and the owner's
@@ -327,28 +341,31 @@ class Net(Model):
 
     # --- compute
     def fprop(self, train=False):
-        self.H.cnb_net_fprop(self.h, int(train))
+        _check(self.H.cnb_net_fprop(self.h, int(train)))
 
     def bprop(self):
-        self.H.cnb_net_bprop(self.h)
+        _check(self.H.cnb_net_bprop(self.h))
 
     def update(self):
-        self.H.cnb_net_update(self.h)
+        _check(self.H.cnb_net_update(self.h))
 
     def loss(self):
         """loss_function_weight times the batch's loss under the output layer's loss function (after fprop)"""
-        return self.H.cnb_net_loss(self.h)
+        v = ct.c_float(0)
+        _check(self.H.cnb_net_loss(self.h, ct.byref(v)))
+        return v.value
 
     def metric(self):
         """the output layer's performance metric summed over the batch (after fprop): correct images for
         CLASSIFICATION_MULTINOMIAL, the per-image share of correct features for CLASSIFICATION_BINARY, or a loss"""
-        return self.H.cnb_net_metric(self.h)
+        v = ct.c_float(0)
+        _check(self.H.cnb_net_metric(self.h, ct.byref(v)))
+        return v.value
 
     # --- optimizer (SGDOptimizer, src/optimizer.cc): one per trained tensor, named "<edge>:weight", "<edge>:bias",
     # "<layer>:gamma", "<layer>:beta" as in checkpoints
     def _set_optimizer(self, tensor, d):
-        """0, -1 (no such tensor) or -2 (config refused, the reason on stderr)"""
-        return self.H.cnb_net_set_optimizer(self.h, tensor.encode(), ct.byref(OptimizerConfig.from_dict(d)))
+        _check(self.H.cnb_net_set_optimizer(self.h, tensor.encode(), ct.byref(OptimizerConfig.from_dict(d))))
 
     def _optimizer_state(self, tensor):
         step, eps, mom = ct.c_longlong(0), ct.c_float(0), ct.c_float(0)
@@ -362,13 +379,9 @@ class Net(Model):
         name = self._edge_name(edge)
         if name and [e[0] for e in self.edges()].index(name) < self._frozen()[0]:
             raise ValueError("edge %r is blocked (block_backprop): it is frozen, and no optimizer trains it" % (name,))
-        for key, kind, d in (("weights", ":weight", weights), ("bias", ":bias", bias)):
-            if d is None:
-                continue
-            rc = self._set_optimizer(name + kind, d)
-            if rc != 0:
-                raise ValueError("set_optimizer(%r, %s): %s" % (edge, key, "no such weighted edge" if rc == -1
-                                                                else "config not supported (see stderr)"))
+        for kind, d in ((":weight", weights), (":bias", bias)):
+            if d is not None:
+                self._set_optimizer(name + kind, d)
 
     def optimizer_state(self, edge):
         """{"weights": {...}, "bias": {...}}: updates counted so far ("step") and the epsilon / momentum of the next one"""
@@ -405,8 +418,8 @@ class Net(Model):
         set_optimizer; norm rules are refused).  Step counts and momentum histories are kept."""
         name = self._bn_layer(layer)[1]
         for key, d in (("gamma", gamma), ("beta", beta)):
-            if d is not None and self._set_optimizer(name + ":" + key, d) != 0:
-                raise ValueError("set_bn_optimizer(%r, %s): config not supported (see stderr)" % (layer, key))
+            if d is not None:
+                self._set_optimizer(name + ":" + key, d)
 
     def bn_optimizer_state(self, layer):
         """{"gamma": {...}, "beta": {...}}: updates counted so far ("step") and the epsilon / momentum of the next one"""
@@ -414,33 +427,29 @@ class Net(Model):
         return {key: self._optimizer_state(name + ":" + key) for key in ("gamma", "beta")}
 
     # --- checkpoints and Polyak averaging (ConvNet::Save / Load / InsertPolyak / LoadPolyakWeights / LoadCurrentWeights)
-    def _check(self, rc):
-        if rc != 0:
-            raise ValueError(self.H.cnb_last_error().decode())
-
     def save(self, path):
         """write the net's state to `path` (through path + "temp", fsynced and renamed), after every pending step"""
-        self._check(self.H.cnb_net_save(self.h, os.fsencode(path)))
+        _check(self.H.cnb_net_save(self.h, os.fsencode(path)))
 
     def load(self, path):
         """restore the state `save` wrote from a net of the same model: ValueError (naming the record) if the file does not
         fit this net, which is then unchanged"""
-        self._check(self.H.cnb_net_load(self.h, os.fsencode(path)))
+        _check(self.H.cnb_net_load(self.h, os.fsencode(path)))
 
     iteration = property(lambda s: s.H.cnb_net_iteration(s.h), doc="train_step calls so far (restored by load)")
     polyak_count = property(lambda s: s.H.cnb_net_polyak_count(s.h), doc="filled slots of the Polyak queue")
 
     def polyak_insert(self):
         """copy the parameters into the next slot of the Polyak queue (a ring of polyak_queue_size slots)"""
-        self._check(self.H.cnb_net_polyak_insert(self.h))
+        _check(self.H.cnb_net_polyak_insert(self.h))
 
     def load_polyak_weights(self):
         """keep the parameters aside and replace them with the average of the filled queue slots"""
-        self._check(self.H.cnb_net_load_polyak_weights(self.h))
+        _check(self.H.cnb_net_load_polyak_weights(self.h))
 
     def load_current_weights(self):
         """restore the parameters load_polyak_weights kept aside"""
-        self._check(self.H.cnb_net_load_current_weights(self.h))
+        _check(self.H.cnb_net_load_current_weights(self.h))
 
     lr_reduce_counter = property(lambda s: s.H.cnb_net_lr_reduce_counter(s.h),
                                  doc="learning-rate reductions train() has applied (kept by save, restored by load)")
@@ -451,7 +460,7 @@ class Net(Model):
         then dataset_size // batch_size test-mode batches (the rest is dropped), averaged as the reference's float running
         mean.  ValueError for a handler of another batch size."""
         v = ct.c_float(0)
-        self._check(self.H.cnb_net_validate(self.h, handler.h, ct.byref(v)))
+        _check(self.H.cnb_net_validate(self.h, handler.h, ct.byref(v)))
         return v.value
 
     def train(self, train, valid=None, *, checkpoint_dir=None, run_name=None):
@@ -465,11 +474,9 @@ class Net(Model):
         still empty it runs on the current weights.  Returns the events, in order: {"iteration", "kind": "train" (the
         metric per image since the last print) | "valid", "value", "lr_reduced", "polyak" (validated on the average)}.
         ValueError for a schedule the loop refuses, a handler of another batch size or a data-parallel net."""
-        n = self.H.cnb_net_train(self.h, train.h, valid.h if valid is not None else None,
-                                 None if checkpoint_dir is None else os.fsencode(checkpoint_dir),
-                                 None if run_name is None else run_name.encode())
-        if n < 0:
-            raise ValueError(self.H.cnb_last_error().decode())
+        n = _check(self.H.cnb_net_train(self.h, train.h, valid.h if valid is not None else None,
+                                        None if checkpoint_dir is None else os.fsencode(checkpoint_dir),
+                                        None if run_name is None else run_name.encode()))
         out = []
         for k in range(n):
             it, kind, v, red, pol = ct.c_longlong(0), ct.c_int(0), ct.c_float(0), ct.c_int(0), ct.c_int(0)
@@ -481,16 +488,16 @@ class Net(Model):
     def train_step(self, want_loss=True):
         if want_loss:
             v = ct.c_float(0)
-            self.H.cnb_net_train_step(self.h, ct.byref(v))
+            _check(self.H.cnb_net_train_step(self.h, ct.byref(v)))
             return v.value
-        self.H.cnb_net_train_step(self.h, None)
+        _check(self.H.cnb_net_train_step(self.h, None))
         return None
 
     def trace_step(self):
         """One extra training step with timing events on the three streams (ConvNet::TraceStep): device milliseconds since
         the step began of the pipeline's milestones, and per gradient bucket its size, exchange window and SGD end."""
         buf = (ct.c_float * 512)()
-        n = min(512, self.H.cnb_net_trace_step(self.h, buf, 512))
+        n = min(512, _check(self.H.cnb_net_trace_step(self.h, buf, 512)))
         v = [buf[k] for k in range(n)]
         out = {"fprop_end_ms": v[0], "bprop_compute_end_ms": v[1], "step_end_ms": v[2], "buckets": []}
         for b in range(int(v[3])):
@@ -499,15 +506,14 @@ class Net(Model):
         return out
 
     def dp_init(self, rank, world, id_bytes, bucket_floats=32 << 20):
+        """join the data-parallel group: RuntimeError when NCCL cannot be loaded or initialised"""
         assert len(id_bytes) == 128
-        rc = self.H.cnb_net_dp_init(self.h, rank, world, bytes(id_bytes), bucket_floats)
-        if rc != 0:
-            raise RuntimeError("NCCL initialisation failed (libnccl.so.2 not loadable?)")
+        _check(self.H.cnb_net_dp_init(self.h, rank, world, bytes(id_bytes), bucket_floats))
 
     def grad_check(self, seed=1, cap=64):
         names = ct.create_string_buffer(64 * cap)
         eps, dw, db = (ct.c_float * cap)(), (ct.c_float * cap)(), (ct.c_float * cap)()
-        n = self.H.cnb_net_grad_check(self.h, seed, cap, names, eps, dw, db)
+        n = _check(self.H.cnb_net_grad_check(self.h, seed, cap, names, eps, dw, db))
         out = []
         for k in range(n):
             out.append((names.raw[64 * k:64 * (k + 1)].split(b"\0")[0].decode(), eps[k], dw[k], db[k]))
@@ -575,10 +581,8 @@ def model_initial_weights(model, edge, seed=42):
     (host-only; the net seeds edge i with its seed + 17 i), or a PRETRAINED edge's weights from its checkpoint; None for
     an edge without parameters of its own (a tied edge starts from its owner's)"""
     with Model(model) as m:
-        n = m.H.cnb_net_initial_weights(m.h, edge, seed, None, 0)
-        if n == -1:
-            raise ValueError(m.H.cnb_last_error().decode())
-        if n < 0:
+        n = _check(m.H.cnb_net_initial_weights(m.h, edge, seed, None, 0))
+        if n == 0:
             return None
         buf = (ct.c_float * n)()
         m.H.cnb_net_initial_weights(m.h, edge, seed, buf, n)
@@ -652,15 +656,14 @@ def model_fusion(model, batch=1):
 
 def check_bn_optimizer(config):
     """raise ValueError if the optimizer block `config` (a dict) cannot train gamma / beta"""
-    if load_host().cnb_bn_optimizer_check(ct.byref(OptimizerConfig.from_dict(config))) != 0:
-        raise ValueError("optimizer config not supported for gamma / beta: %r (see stderr)" % (config,))
+    _check(load_host().cnb_bn_optimizer_check(ct.byref(OptimizerConfig.from_dict(config))))
 
 
 def optimizer_schedule(config, step):
     """(epsilon, momentum) of the update after `step` earlier ones under the optimizer block `config` (a dict)"""
     eps, mom = ct.c_float(0), ct.c_float(0)
-    if load_host().cnb_optimizer_schedule(ct.byref(OptimizerConfig.from_dict(config)), step, ct.byref(eps), ct.byref(mom)):
-        raise ValueError("optimizer config not supported: %r" % (config,))
+    c = OptimizerConfig.from_dict(config)
+    _check(load_host().cnb_optimizer_schedule(ct.byref(c), step, ct.byref(eps), ct.byref(mom)))
     return eps.value, mom.value
 
 
@@ -681,21 +684,21 @@ def plan_buckets(edge_sizes, bucket_floats):
 
 def dp_unique_id():
     buf = ct.create_string_buffer(128)
-    if load_host().cnb_dp_unique_id(buf) != 0:
-        raise RuntimeError("ncclGetUniqueId failed")
+    _check(load_host().cnb_dp_unique_id(buf))
     return buf.raw
 
 
 class DataIterator:
     """Device side of the reference's input pipeline (host/data.h; src/datahandler.cc:146-200, 520-568): a chunk of images
-    resident on the GPU, and per minibatch a random (or centre / corner) crop + mirror into the net's input layer."""
+    resident on the GPU, and per minibatch a random (or centre / corner) crop + mirror into the net's input layer.
+    ValueError for a crop larger than the image, or a chunk_size or channels below 1."""
 
     def __init__(self, chunk_size, channels, image_size, gpu_image_size, translate=True, flip=True, seed=1):
-        self.H = load_host()
+        self.H, self.h = load_host(), None
         isy, isx = (image_size, image_size) if isinstance(image_size, int) else image_size
         gy, gx = (gpu_image_size, gpu_image_size) if isinstance(gpu_image_size, int) else gpu_image_size
         self.chunk_size, self.dims = chunk_size, channels * isy * isx
-        self.h = self.H.cnb_data_create(chunk_size, channels, isy, isx, gy, gx, int(translate), int(flip), seed)
+        self.h = _check(self.H.cnb_data_create(chunk_size, channels, isy, isx, gy, gx, int(translate), int(flip), seed))
 
     def close(self):
         if self.h:
@@ -707,11 +710,11 @@ class DataIterator:
         import torch
         t = host_tensor.contiguous()
         assert t.dtype == torch.float32 and t.device.type == "cpu" and t[0].numel() == self.dims
-        self.H.cnb_data_upload(self.h, t.data_ptr(), first, t.shape[0])
+        _check(self.H.cnb_data_upload(self.h, t.data_ptr(), first, t.shape[0]))
         self._keep = t                                   # the copy is asynchronous
 
     def get_batch(self, net, start=0, multiplicity_id=0):
-        self.H.cnb_data_get_batch(self.h, net.h, start, multiplicity_id)
+        _check(self.H.cnb_data_get_batch(self.h, net.h, start, multiplicity_id))
 
     def last_noise(self, batch):
         buf = (ct.c_float * (3 * batch))()
@@ -764,11 +767,9 @@ class DataHandler:
             multiplicity=multiplicity))
         self.batch_size = batch_size
         ptr = lambda t: None if t is None else t.data_ptr()
-        self.h = self.H.cnb_handler_create(
+        self.h = _check(self.H.cnb_handler_create(
             ct.byref(self.order), n, c, isy, isx, gy, gx, int(translate), int(flip), ptr(self._images), ptr(self._labels),
-            ptr(self._targets), 0 if self._targets is None else self._targets.shape[1], seed)
-        if not self.h:
-            raise ValueError(self.H.cnb_last_error().decode())
+            ptr(self._targets), 0 if self._targets is None else self._targets.shape[1], seed))
 
     @classmethod
     def from_model(cls, model, images, labels=None, which="train_dataset", *, targets=None, net=None, seed=1):
@@ -796,13 +797,11 @@ class DataHandler:
         """the next minibatch into net's input layer, and its labels or targets into labels_tensor() / targets_tensor()"""
         if net.batch_size != self.batch_size:
             raise ValueError("the net's batch size is %d and the handler's %d" % (net.batch_size, self.batch_size))
-        if self.H.cnb_handler_get_batch(self.h, net.h) != 0:
-            raise ValueError(self.H.cnb_last_error().decode())
+        _check(self.H.cnb_handler_get_batch(self.h, net.h))
 
     def seek(self, row):
         """restart the schedule at data set row `row` (DataHandler::Seek): the next batch loads a chunk from there"""
-        if self.H.cnb_handler_seek(self.h, row) != 0:
-            raise ValueError(self.H.cnb_last_error().decode())
+        _check(self.H.cnb_handler_seek(self.h, row))
 
     def last_indices(self):
         """{"start", "multiplicity_id", "rows": the data set row of each image of the last batch, "width_offset",
@@ -823,15 +822,13 @@ def dataset_schedule(config, dataset_size, steps, seed=1, seeks=None):
     before that step.  ValueError for a configuration the handler refuses."""
     H = load_host()
     order = DatasetOrder.from_dict(config)
-    s = H.cnb_schedule_create(ct.byref(order), dataset_size, seed)
-    if not s:
-        raise ValueError(H.cnb_last_error().decode())
+    s = _check(H.cnb_schedule_create(ct.byref(order), dataset_size, seed))
     try:
         chunk = H.cnb_schedule_chunk_size(s)
         rows, perm, start, mid, out = (ct.c_int * chunk)(), (ct.c_int * chunk)(), ct.c_int(0), ct.c_int(0), []
         for k in range(steps):
-            if seeks and k in seeks and H.cnb_schedule_seek(s, seeks[k]) != 0:
-                raise ValueError(H.cnb_last_error().decode())
+            if seeks and k in seeks:
+                _check(H.cnb_schedule_seek(s, seeks[k]))
             loaded = H.cnb_schedule_next(s, ct.byref(start), ct.byref(mid), rows, perm)
             out.append((list(rows) if loaded else None, start.value, mid.value, list(perm)))
         return out
@@ -899,10 +896,8 @@ def train_dry_run(model, valid_values=None, *, iteration=0, lr_reduce_counter=0)
     with Model(model) as m:
         while True:
             its, acts = (ct.c_longlong * cap)(), (ct.c_int * cap)()
-            n = m.H.cnb_net_train_dry_run(m.h, iteration, lr_reduce_counter, int(valid_values is not None), fv, len(vals),
-                                          cap, its, acts)
-            if n < 0:
-                raise ValueError(m.H.cnb_last_error().decode())
+            n = _check(m.H.cnb_net_train_dry_run(m.h, iteration, lr_reduce_counter, int(valid_values is not None), fv,
+                                                 len(vals), cap, its, acts))
             if n <= cap:
                 return [(its[k], {a for b, a in enumerate(TRAIN_ACTIONS) if acts[k] >> b & 1}) for k in range(n)]
             cap = n

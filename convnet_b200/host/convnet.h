@@ -5,8 +5,8 @@
 // Accumulate + Broadcast (src/convnet.cc:407-438) with in-place NCCL all-reduce over NVLink.
 //
 // Layers form a chain (every BASELINE net is one: Appendix B of SURVEY.md).  The model comes
-// from a ModelConfig struct: built by name in models.cc, or read from the reference's config::Model
-// text proto (a net.pbtxt file) in model_file.cc.
+// from a ModelConfig struct that model_file.cc reads from the reference's config::Model text proto:
+// a net.pbtxt file, or the text of a built-in model, which models.cc holds by name.
 #pragma once
 #include <map>
 #include <memory>
@@ -488,16 +488,8 @@ class GradChecker : public ConvNet {
   double LossAtD(Matrix& w, size_t index, float value);
 };
 
-// models.cc
-ModelConfig BuildAlexNet();     // examples/imagenet/CLS_net_20140801232522.pbtxt
-ModelConfig BuildLeNet();       // examples/mnist-conv/net.pbtxt
-ModelConfig BuildC3D();         // SURVEY.md §8(d) cfg4
-ModelConfig BuildTinyNet();     // small conv+pool+rnorm+1x1+fc net for tests / grad check
-ModelConfig BuildLogCheckNet(); // the gradcheck net with logistic hidden units
-ModelConfig BuildUpDownNet();   // encoder-decoder with RGBTOYUV, DOWNSAMPLE and UPSAMPLE edges (bench size)
-ModelConfig BuildUpDownCheckNet();  // run_grad_check net for the sampling edges
-// a built-in name, a path ending in ".pbtxt" (ReadModelFile), either with suffixes ("+bn", "+rmsprop", ...).
-// std::invalid_argument: unknown name, unreadable or refused file
+// models.cc: a built-in name (its model text, read by ReadModelText), a path ending in ".pbtxt" (ReadModelFile), either
+// with suffixes ("+bn", "+rmsprop", ...).  std::invalid_argument: unknown name, unreadable or refused file
 ModelConfig BuildModel(const std::string& name);
 
 // model_file.cc: the reference's config::Model text proto (src/util.cc ReadPbtxt, proto/convnet_config.proto).

@@ -1,6 +1,7 @@
 // model_file.cc — the reference's config::Model text protos (examples/*/net.pbtxt, read by ReadPbtxt, src/util.cc:87):
-// ReadModelFile parses one as protobuf's TextFormat does for these messages and maps it onto a ModelConfig with the
-// reference's semantics; ModelText prints any ModelConfig as one.  Protobuf is not a dependency: the schema below is
+// ReadModelText parses one as protobuf's TextFormat does for these messages and maps it onto a ModelConfig with the
+// reference's semantics, for a model file (ReadModelFile) and for the text of a built-in model (models.cc) alike;
+// ModelText prints any ModelConfig as one.  Protobuf is not a dependency: the schema below is
 // proto/convnet_config.proto's field names, types and presence rules.
 #include <algorithm>
 #include <cctype>

@@ -7,7 +7,7 @@ from convnet_b200 import net as N
 
 pad = lambda v: (v + 127) // 128 * 128
 
-# lcnet (models.cc BuildLcNet): conv1, pool1, conv2, pool2, local3, local4, fc5, output
+# lcnet (its text in models.cc): conv1, pool1, conv2, pool2, local3, local4, fc5, output
 LCNET_EDGES = [64 * (5 * 5 * 3 + 1), 0, 128 * (3 * 3 * 64 + 1), 0,
                128 * (1152 * 144 + 144),          # local3: 12 x 12 modules, K = 3*3*128, one bias per output feature
                128 * (1152 * 100 + 100),          # local4: 10 x 10 modules

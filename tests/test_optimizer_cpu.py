@@ -69,7 +69,7 @@ def test_invalid_configs_are_refused():
 
 
 # examples/imagenet/CLS_net_20140801232522.pbtxt: every weight / bias optimizer has epsilon 0.01 and momentum 0.5 -> 0.9
-# over 2000 steps (e.g. :148-158); the extra weight settings by edge index of BuildAlexNet's chain
+# over 2000 steps (e.g. :148-158); the extra weight settings by edge index of the alexnet chain
 RAMP = {"epsilon": f32(0.01), "initial_momentum": f32(0.5), "final_momentum": f32(0.9), "momentum_transition_timescale": 2000}
 ALEX_WEIGHTS = {
     0: {},                                             # input -> hidden1_conv, :148-153

@@ -21,7 +21,7 @@ from convnet_b200 import lib  # noqa: E402
 from convnet_b200.abi import GetConvDesc  # noqa: E402
 from convnet_b200.matrix import CUDAMatrix  # noqa: E402
 
-# AlexNet (BuildAlexNet): input side, Cin, Cout, kernel, stride, padding -> output side
+# AlexNet (the alexnet text in models.cc): input side, Cin, Cout, kernel, stride, padding -> output side
 LAYERS = {"conv2": (55, 96, 256, 5, 2, 1), "conv3": (14, 256, 384, 3, 1, 1), "conv4": (14, 768, 384, 3, 1, 1),
           "conv5": (14, 384, 512, 3, 1, 0), "fc6": (1, 512 * 36, 4096, 1, 1, 0)}
 ACT = {"relu": 1, "logistic": 2}

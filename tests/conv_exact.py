@@ -86,7 +86,7 @@ PATH_MODEL = {"cuda-core-fp32": "fp32", "tc-tf32": "tf32", "tc-bf16": "bf16"}
 
 def conv_path(op, g, mode):
     """'cuda-core-fp32', 'tc-tf32' or 'tc-bf16': the path of a conv call in precision `mode`"""
-    x_mode = g.Cin * g.kt < 8
+    x_mode = g.Cin * g.kt < 8           # (a 3-D call folds its kt frames into Cin * kt channels)
     rows = g.N * g.modX * g.modY * g.modT
     if mode == "fp32" or (x_mode and (g.kx > 8 or g.ky > 8)):
         return "cuda-core-fp32"
@@ -94,11 +94,11 @@ def conv_path(op, g, mode):
         tc = g.N % 4 == 0 and g.Cout % 4 == 0
         bf = not x_mode and g.N % 8 == 0 and g.Cout % 8 == 0
     elif op == "dgrad":
-        tc = g.N % 4 == 0 and g.Cout % 4 == 0 and g.Cout >= 8 and g.Cin >= 8 and g.kx <= 32 and g.ky <= 32
+        tc = g.N % 4 == 0 and g.Cout % 4 == 0 and g.Cout >= 8 and g.Cin * g.kt >= 8 and g.kx <= 32 and g.ky <= 32
         bf = g.N % 8 == 0 and g.Cout % 8 == 0
     else:
         tc = g.N % 4 == 0 and g.Cout >= 8
-        bf = not x_mode and g.N % 8 == 0 and (rows >= 1024 or (g.T == 1 and g.N % 128 == 0 and g.Cin % 32 == 0))
+        bf = not x_mode and g.N % 8 == 0 and (rows >= 1024 or (g.modT == 1 and g.N % 128 == 0 and g.Cin * g.kt % 32 == 0))
     if not tc:
         return "cuda-core-fp32"
     return "tc-bf16" if mode == "bf16" and bf else "tc-tf32"
@@ -342,13 +342,12 @@ def expect(op, g, a, b, kind, t0=None, st=0.0, so=1.0, bias=None, relu=False, ma
             S = torch.where(written, S + (st * t).abs(), S)
     elif op == "dgrad":
         keep = torch.zeros_like(keep)  # scaleTargets 0 clears the whole target
-    if bias is not None:
-        assert op == "fprop" and g.modT == 1
-        bb = bias.to(torch.float64).view(1, -1, 1)
-        shape = (g.CoutT, g.modY * g.modX, g.N)
+    if bias is not None:             # one bias per output channel, added to every output frame
+        assert op == "fprop"
+        shape = (g.modT, g.CoutT, g.modY * g.modX, g.N)
         full = torch.zeros(g.CoutT, dtype=torch.float64, device=dev)
-        full[g.cout0:g.cout0 + g.Cout] = bb.view(-1)
-        fb = full.view(-1, 1, 1).expand(shape).reshape(-1)
+        full[g.cout0:g.cout0 + g.Cout] = bias.to(torch.float64).view(-1)
+        fb = full.view(1, -1, 1, 1).expand(shape).reshape(-1)
         ref = torch.where(written, ref + fb, ref)
         S = torch.where(written, S + fb.abs(), S)
     if relu:

@@ -51,6 +51,11 @@ Frozen trunks (block_backprop): frozen edges get fprop rows only.  Their slice o
 state is bit-identical after the step, their slice of the gradient buffer still holds the sentinel, and the hidden
 layers they write have no derivative.
 
+3-D layers (c3d): frames stack as channel blocks (channel c + C*t).  A 3-D conv is conv_exact's 3-D Geo (T, kt, st_t:
+frame window f reads frames [f st_t, f st_t + kt)), its bias added to every output frame and its bias gradient the sum of
+one column sum per output frame (the first writing, the others adding, as in a tie group); max / average pools are
+pool_exact's 3-D PG (kernel_size / kernel_size_t 0: the whole image / clip), and an FC edge reads every frame.
+
 Dropout is checked inside the fprop of the layer that draws it: the keep mask of element i is
 float32(hash(seed + i)) * 2^-32 >= p with the seed the net reported for the step (Net.dropout_seed), whether the edge's
 epilogue applies it or a separate pass does (then the pass's product adds one rounding, far inside the bar).
@@ -60,8 +65,7 @@ Tensor-core calls are also controls: their output must FAIL against the wrong op
 
 Not audited, raising Unsupported: batch-normalised layers, LOCAL edges and CONVOLUTIONAL edges with an unshared bias,
 dropout on non-ReLU layers (its keep mask cannot be read back from the state), other output layers and optimizers, nets
-that are not chains, and 3-D layers (c3d: no small 3-D model exists, and the
-3-D pool and conv paths have exact tests of their own).
+that are not chains, and on 3-D layers every edge but CONVOLUTIONAL, MAXPOOL, AVERAGE_POOL and FC.
 """
 import dataclasses
 import math
@@ -137,9 +141,10 @@ class LayerGeo:
     act: str
     dropprob: float
     cfg: dict
+    T: int = 1                    # frames (3-D layers stack them as channel blocks, channel c + C*t)
 
     def floats(self, N):
-        return N * self.W * self.H * self.C
+        return N * self.W * self.H * self.C * self.T
 
 
 @dataclasses.dataclass
@@ -169,8 +174,6 @@ class Model:
         if len(layers) != len(edges) + 1:
             raise Unsupported("%s: not a chain" % name)
         inp = layers[0]
-        if int(inp.get("image_size_t", 1)) != 1:
-            raise Unsupported("%s: 3-D layers" % name)
         for lc in layers:
             if lc.get("batch_normalize"):
                 raise Unsupported("%s: layer %s is batch-normalised" % (name, lc["name"]))
@@ -184,25 +187,29 @@ class Model:
             raise Unsupported("%s: output layer %s / %s" % (name, out["activation"], out.get("loss_function")))
         self.loss_weight = f32(out.get("loss_function_weight", 1.0))
         W, H = int(inp["image_size_x"]), int(inp["image_size_y"])
-        self.layers = [LayerGeo(inp["name"], int(inp["num_channels"]), W, H, inp["activation"], 0.0, inp)]
+        self.layers = [LayerGeo(inp["name"], int(inp["num_channels"]), W, H, inp["activation"], 0.0, inp,
+                                int(inp.get("image_size_t", 1)))]
         self.edges = []
         for i, e in enumerate(edges):
             kind = e["edge_type"]
             if kind not in WEIGHTED + ("MAXPOOL", "AVERAGE_POOL", "RESPONSE_NORM") + SAMPLING:
                 raise Unsupported("%s: edge type %s" % (name, kind))
-            if int(e.get("kernel_size_t", 1)) != 1 or int(e.get("padding_t", 0)) != 0:
-                raise Unsupported("%s: 3-D edge" % name)
             if kind == "CONVOLUTIONAL" and not e.get("shared_bias", True):
                 raise Unsupported("%s: unshared conv bias" % name)
             lc = layers[i + 1]
             src = self.layers[i]
+            if src.T > 1 and kind not in ("CONVOLUTIONAL", "FC", "MAXPOOL", "AVERAGE_POOL"):
+                raise Unsupported("%s: %s edge on the 3-D layer %s" % (name, kind, src.name))
+            t = src.T
             if kind == "FC":
-                w, h = 1, 1
+                w, h, t = 1, 1, 1
             elif kind in ("CONVOLUTIONAL", "MAXPOOL", "AVERAGE_POOL"):
                 ky = int(e["kernel_size_y"]) if e["kernel_size_y"] > 0 else src.H
                 kx = int(e["kernel_size_x"]) if e["kernel_size_x"] > 0 else src.W
                 w = num_modules(src.W, kx, int(e["stride_x"]), int(e["padding_x"]))
                 h = num_modules(src.H, ky, int(e["stride_y"]), int(e["padding_y"]))
+                kt = int(e.get("kernel_size_t", 1)) if e.get("kernel_size_t", 1) > 0 else src.T
+                t = num_modules(src.T, kt, int(e.get("stride_t", 1)), int(e.get("padding_t", 0)))
             elif kind == "UPSAMPLE":
                 f = int(e.get("sample_factor", 1))
                 w, h = src.W * f, src.H * f
@@ -212,7 +219,7 @@ class Model:
             else:
                 w, h = src.W, src.H
             self.layers.append(LayerGeo(lc["name"], int(lc["num_channels"]), w, h, lc["activation"],
-                                        float(lc.get("dropprob", 0.0)), lc))
+                                        float(lc.get("dropprob", 0.0)), lc, t))
             self.edges.append(EdgeGeo(e.get("name") or "%s:%s" % (e["source"], e["dest"]), kind, e, i, i + 1))
         # tie groups: owner[k] is the edge whose parameters weighted edge k uses (tied_to names it), and the group's
         # parameters sit at the slice of its lowest member (Net.model_ties)
@@ -232,11 +239,12 @@ class Model:
         s, d = self.layers[e.src], self.layers[e.dst]
         c = e.cfg
         if e.kind == "FC":
-            return cx.Geo(N, 1, 1, s.W * s.H * s.C, d.C, 1, 1)
+            return cx.Geo(N, 1, 1, s.W * s.H * s.C * s.T, d.C, 1, 1)
         if e.kind == "CONV_ONETOONE":
             return cx.Geo(N, s.W, s.H, s.C, d.C, 1, 1)
         return cx.Geo(N, s.W, s.H, s.C, d.C, int(c["kernel_size_y"]), int(c["kernel_size_x"]), int(c["stride_y"]),
-                      int(c["stride_x"]), int(c["padding_y"]), int(c["padding_x"]))
+                      int(c["stride_x"]), int(c["padding_y"]), int(c["padding_x"]), T=s.T,
+                      kt=int(c.get("kernel_size_t", 1)), st_t=int(c.get("stride_t", 1)))
 
     def group(self, k):
         """the weighted edges that share edge k's parameters (edge k alone when untied), in chain order"""
@@ -257,8 +265,9 @@ class Model:
         s, c = self.layers[e.src], e.cfg
         ky = int(c["kernel_size_y"]) if c["kernel_size_y"] > 0 else s.H
         kx = int(c["kernel_size_x"]) if c["kernel_size_x"] > 0 else s.W
+        kt = int(c.get("kernel_size_t", 1)) if c.get("kernel_size_t", 1) > 0 else s.T    # (0: the whole clip)
         return px.PG(N, s.W, s.H, s.C, ky, kx, int(c["stride_y"]), int(c["stride_x"]), int(c["padding_y"]),
-                     int(c["padding_x"]))
+                     int(c["padding_x"]), s.T, kt, int(c.get("stride_t", 1)), int(c.get("padding_t", 0)))
 
     def weight_slices(self, k, N):
         """(weights, bias) index ranges of weighted edge k in the flat buffers"""
@@ -437,22 +446,25 @@ class Auditor:
         y = s.grads[bs[0]:bs[1]]
         zero = torch.zeros(dst.C, dtype=torch.float32, device=y.device)
         above = m.edges[e.dst] if e.dst < len(m.edges) else None
-        if len(m.group(k)) > 1:
-            # a tie group: the library keeps every member's column sum on the side lane, in back-propagation order (no
-            # member hands its bias gradient to a pool undo, ConvNet::PlanFusion).  Each later member adds its sum to
-            # the stored partial (st = 1): its bar covers that addition (the st * b0 term), and the partial's own error
-            # carries over unscaled, so the bars add
-            assert not any(m.plan[j]["offers_bias_grad"] for j in m.group(k)), "a tie member offers its bias gradient"
+        if len(m.group(k)) > 1 or dst.T > 1:
+            # a tie group or a 3-D layer: one column sum per member (in back-propagation order) and per output frame,
+            # on the side lane (no such edge hands its bias gradient to a pool undo, ConvNet::PlanFusion), the first
+            # writing the gradient and each later one adding to the stored partial (st = 1): its bar covers that
+            # addition (the st * b0 term), and the partial's own error carries over unscaled, so the bars add
+            assert not any(m.plan[j]["offers_bias_grad"] for j in m.group(k)), "%s offers its bias gradient" % e.name
             exp = None
             for j in m.group(k)[::-1]:
                 ej = m.edges[j]
                 dj = m.layers[ej.dst]
                 soj = f32(f32(ej.cfg.get("scale_gradients", 1.0)) / s.N)
-                b0 = zero if exp is None else exp.ref.to(torch.float32)
-                x = ex.bias_grad(s.derivs[ej.dst], s.N * dj.W * dj.H, dj.C, b0, 0.0 if exp is None else 1.0, soj)
-                exp = x if exp is None else px.Expect(exp.ref + (x.ref - b0.to(torch.float64)), exp.bar + x.bar,
-                                                      x.exact)
-            how = "tie group sum"
+                per = s.N * dj.W * dj.H
+                for t in range(dj.T):
+                    b0 = zero if exp is None else exp.ref.to(torch.float32)
+                    x = ex.bias_grad(s.derivs[ej.dst][t * per * dj.C:(t + 1) * per * dj.C], per, dj.C, b0,
+                                     0.0 if exp is None else 1.0, soj)
+                    exp = x if exp is None else px.Expect(exp.ref + (x.ref - b0.to(torch.float64)), exp.bar + x.bar,
+                                                          x.exact)
+            how = "tie group sum" if len(m.group(k)) > 1 else "sum over %d frames" % dst.T
         elif above is not None and m.plan[e.dst]["sums_bias_below"] and m.plan[k]["offers_bias_grad"]:
             relu = m.plan[e.dst]["down_act"] == 1
             if above.kind == "UPSAMPLE":          # the block sum is a forward average pool on the big image
@@ -783,6 +795,34 @@ def sample_dropout_text():
         j = t.index("dropprob: 0", i)
         t = t[:j] + "dropprob: 0.25" + t[j + len("dropprob: 0"):]
     return t
+
+
+def video_text():
+    """a small 3-D net as a model-file text: 16 x 16 clips of 8 frames and 4 channels; conv1 (kt 2) and a 2 x 2 max pool
+    within frames, conv2 with frame windows of 3 at stride_t 2 (overlapping: its dgrad sums two windows on every second
+    frame), a 2 x 2 average pool with overlapping frame windows of 2 at stride_t 1 and c3d's global max pool
+    (kernel_size 0, kernel_size_t 0) under an FC softmax.  At N 16 every conv call of bf16 mode takes the bf16 tensor
+    cores."""
+    return """name: "video"
+seed: 42
+default_weight_optimizer { epsilon: 0.01 final_momentum: 0.9 }
+default_bias_optimizer { epsilon: 0.01 final_momentum: 0.9 }
+layer { name: "input" num_channels: 4 image_size_y: 16 image_size_x: 16 image_size_t: 8 }
+layer { name: "conv1" num_channels: 16 activation: RECTIFIED_LINEAR }
+layer { name: "pool1" num_channels: 16 }
+layer { name: "conv2" num_channels: 32 activation: RECTIFIED_LINEAR }
+layer { name: "pool2" num_channels: 32 }
+layer { name: "pool3" num_channels: 32 }
+layer { name: "output" num_channels: 10 activation: SOFTMAX }
+edge { source: "input" dest: "conv1" edge_type: CONVOLUTIONAL kernel_size: 3 padding: 1 kernel_size_t: 2
+       shared_bias: true initialization: DENSE_UNIFORM_SQRT_FAN_IN }
+edge { source: "conv1" dest: "pool1" edge_type: MAXPOOL kernel_size: 2 stride: 2 }
+edge { source: "pool1" dest: "conv2" edge_type: CONVOLUTIONAL kernel_size: 3 padding: 1 kernel_size_t: 3 stride_t: 2
+       shared_bias: true initialization: DENSE_UNIFORM_SQRT_FAN_IN }
+edge { source: "conv2" dest: "pool2" edge_type: AVERAGE_POOL kernel_size: 2 stride: 2 kernel_size_t: 2 }
+edge { source: "pool2" dest: "pool3" edge_type: MAXPOOL kernel_size: 0 kernel_size_t: 0 }
+edge { source: "pool3" dest: "output" edge_type: FC initialization: DENSE_UNIFORM_SQRT_FAN_IN }
+"""
 
 
 def _sgd_config(model, edge):

@@ -5,7 +5,8 @@ NaN guard zones.
 Each branch case names the branch it targets and asserts the path the call took and the kernels it launched, with the
 operands pre-staged in bf16 mode so that no conversion pass is counted.  The launch count tells the branch apart:
 split-K and wgrad reduction splits add a reduction launch, dgrad in fprop form launches once per stride phase plus once
-for the first build of its filter banks, 3-D dgrad once per frame.  Every tensor-core case is also a control: the same
+for the first build of its filter banks, 3-D dgrad once per output frame (frame windows stride_t frames apart, which
+overlap when kt > stride_t and leave frames unread when kt < stride_t).  Every tensor-core case is also a control: the same
 output must FAIL the bar against the wrong operand models of its precision (conv_exact.CONTROLS), or the case is too weak
 to see a rounding fault.
 """
@@ -239,6 +240,10 @@ CASES = [
          "N%8!=0 in bf16 mode: tf32", ("bf16",), path={"bf16": "tc-tf32"}, launches={"bf16": 1}),
     Case("fp_3d_cin9", "fprop", Geo(32, 10, 10, 3, 16, 3, 3, 1, 1, 1, 1, T=5, kt=3),
          "3-D: Cin 9 folded from 3 x kt 3, 3 frames", TC, launches={"tf32": 1, "bf16": 1}),
+    Case("fp_3d_st2_kt3", "fprop", Geo(32, 8, 8, 4, 16, 3, 3, 1, 1, 1, 1, T=7, kt=3, st_t=2),
+         "3-D, stride_t 2 < kt 3: 3 overlapping frame windows", TC, launches={"tf32": 1, "bf16": 1}),
+    Case("fp_3d_st2_kt1", "fprop", Geo(32, 8, 8, 8, 16, 3, 3, 1, 1, 1, 1, T=7, kt=1, st_t=2),
+         "3-D, kt 1 < stride_t 2: frames 1, 3, 5 read by no window", TC, launches={"tf32": 1, "bf16": 1}),
     Case("fp_subrange", "fprop", Geo(32, 8, 8, 32, 32, 3, 3, 1, 1, 1, 1, cin0=16, CinT=48, cout0=16, CoutT=64),
          "channel sub-ranges, scaleTargets 0.5", TC, launches={"tf32": 1, "bf16": 1}, st=0.5),
     Case("fp_unaligned_operand", "fprop", Geo(32, 8, 8, 16, 16, 3, 3, 1, 1, 1, 1),
@@ -278,6 +283,12 @@ CASES = [
          launches={m: 4 + (st not in (0.0, 1.0)) for m in TC}, st=st)
     for st in (0.0, 0.5, 1.0)
 ] + [
+    Case("dg_3d_st2_kt%d" % kt, "dgrad", Geo(32, 8, 8, cin, 16, 3, 3, 1, 1, 1, 1, T=T, kt=kt, st_t=2),
+         "3-D, stride_t 2, kt %d (%s): one launch per output frame" % (kt, why), TC,
+         launches={m: (T - kt) // 2 + 1 for m in TC})
+    for kt, cin, T, why in ((3, 4, 7, "windows overlap on every second frame"), (2, 4, 8, "windows tile the frames"),
+                            (1, 8, 7, "frames 1, 3, 5 read by no window: exactly 0"))
+] + [
     Case("dg_subrange", "dgrad", Geo(32, 8, 8, 32, 32, 3, 3, 1, 1, 1, 1, cin0=16, CinT=48, cout0=8, CoutT=48),
          "channel sub-ranges, scaleTargets 1", TC, launches={"tf32": 1, "bf16": 1}, st=1.0),
     # ---- wgrad
@@ -291,6 +302,10 @@ CASES = [
          "x-mode, ky 7: two channels per tile, two tiles", TC, path={"bf16": "tc-tf32"}),
     Case("wg_3d", "wgrad", Geo(32, 6, 6, 8, 16, 3, 3, 1, 1, 1, 1, T=5, kt=2),
          "3-D, 4 frames", TC),
+    Case("wg_3d_st2_kt3", "wgrad", Geo(32, 8, 8, 4, 16, 3, 3, 1, 1, 1, 1, T=7, kt=3, st_t=2),
+         "3-D, stride_t 2 < kt 3: 3 overlapping frame windows", TC),
+    Case("wg_3d_st2_kt2", "wgrad", Geo(32, 8, 8, 8, 16, 3, 3, 1, 1, 1, 1, T=8, kt=2, st_t=2),
+         "3-D, kt == stride_t 2: 4 frame windows that tile the frames", TC),
     Case("wg_st_so", "wgrad", Geo(32, 8, 8, 32, 32, 3, 3, 1, 1, 1, 1),
          "scaleTargets 0.5, scaleOutput 0.25", TC, st=0.5, so=0.25),
     Case("wg_fc_bf16", "wgrad", Geo(128, 1, 1, 512, 256, 1, 1),
@@ -348,7 +363,8 @@ def _check_twin(env, c, out):
 # persistent grids smaller than the GPU: the multi-tile walk and the ring-phase wrap
 # ---------------------------------------------------------------------------------------------------------------------
 SMALL_GRID = [("dg_gather_k1_s2", "bf16"), ("dg_gather_k1_s2", "tf32"), ("wg_dead_taps", "tf32"),
-              ("wg_dead_taps", "bf16"), ("fp_x_cin3_k7_merged", "tf32"), ("dg_fpform_s2_odd", "bf16")]
+              ("wg_dead_taps", "bf16"), ("fp_x_cin3_k7_merged", "tf32"), ("dg_fpform_s2_odd", "bf16"),
+              ("fp_3d_st2_kt3", "bf16"), ("dg_3d_st2_kt3", "tf32"), ("dg_3d_st2_kt1", "bf16"), ("wg_3d_st2_kt3", "bf16")]
 
 
 @pytest.mark.parametrize("name,mode", SMALL_GRID)

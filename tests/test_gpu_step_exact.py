@@ -11,8 +11,10 @@ fail against the weights after it, or the audit could not tell a filter bank reb
 Beyond AlexNet's kind of net the cases cover logistic units (tiny+logistic, logcheck), the LINEAR / squared-error,
 LOGISTIC / binary cross-entropy and SOFTMAX_DIST / soft-target output layers on float targets, Adagrad and RMSProp, tied
 edges (tiednet: one conv filter bank at three geometries, an FC pair whose slice sits at the lower edge), the sampling
-and colour edges (updown, updowncheck, and updowncheck with dropout around its sampling edges) and fine-tuning on a frozen trunk (whose parameters, history and adaptive state must keep their bits, whose gradients must
-keep the sentinel and whose hidden layers have no derivative)."""
+and colour edges (updown, updowncheck, and updowncheck with dropout around its sampling edges), fine-tuning on a frozen
+trunk (whose parameters, history and adaptive state must keep their bits, whose gradients must keep the sentinel and whose
+hidden layers have no derivative) and 3-D layers (c3d, and a small 3-D net with a stride_t 2 conv and 3-D max, average and
+global pools)."""
 import os
 import subprocess
 import sys
@@ -70,6 +72,9 @@ CASES += [("tiny+logistic", 32, "bf16", 0), ("tiny+logistic", 32, "bf16", 3), ("
           ("alexnet+finetune", 128, "bf16", 3), ("tiny+logistic+adagrad+finetune", 32, "bf16", 3),
           ("tiednet", 64, "bf16", 0), ("tiednet", 64, "bf16", 3), ("tiednet", 64, "fp32", 3),
           ("updown", 128, "bf16", 0), ("updowncheck", 32, "fp32", 3), ("updowncheck", 32, "bf16", 3)]
+# 3-D layers: c3d at batch 8 and at the bench's cfg4 batch of 32 (its float64 restatement of conv1a's output, 360 M
+# elements at batch 32, is the largest of the file)
+CASES += [("c3d", 8, "bf16", 0), ("c3d", 8, "bf16", 3), ("c3d", 32, "bf16", 0)]
 # (updown is audited on its first step: its loss sums the squared error of 49,152 outputs per image, and on N(0, 1)
 # targets at the model's learning rate the warm-up steps diverge; updowncheck audits the sampling edges warmed up)
 
@@ -93,6 +98,19 @@ def test_sampling_dropout_step(tmp_path, mode):
         f.write(se.sample_dropout_text())
     rows, left, _ = se.audit_case(path, 32, mode, 3)
     _record("updowncheck+dropout/32/%s/step3" % mode, mode, rows, left, t0)
+
+
+@pytest.mark.parametrize("mode,warmup", [("fp32", 3), ("tf32", 3), ("bf16", 0), ("bf16", 3)])
+def test_video_step(tmp_path, mode, warmup):
+    """the small 3-D net of step_exact.video_text: a conv with frame windows of 3 at stride_t 2, 3-D max, average and
+    global max pools, at N 16 (every conv call of bf16 mode on the bf16 tensor cores)"""
+    t0 = time.time()
+    torch.cuda.reset_peak_memory_stats()
+    path = str(tmp_path / "video.pbtxt")
+    with open(path, "w") as f:
+        f.write(se.video_text())
+    rows, left, _ = se.audit_case(path, 16, mode, warmup)
+    _record("video/16/%s/step%d" % (mode, warmup), mode, rows, left, t0)
 
 
 def test_step_without_fusions():

@@ -1,6 +1,6 @@
 """The step auditor (tests/step_exact.py) without a GPU: it passes a float32 torch step of `tiny` and `gradcheck` (and
 of `tiny` with dropout on its 1x1 layer, with logistic units, with each target-trained output layer, with Adagrad or
-RMSProp, on a frozen trunk, and of `logcheck` and `tiednet`), and it fails every single injected fault, naming the layer
+RMSProp, on a frozen trunk, and of `logcheck`, `tiednet` and a small 3-D net), and it fails every single injected fault, naming the layer
 and quantity.
 
 The snapshot is made the way the net makes one: torch float32 forward and autograd backward in the library's layouts,
@@ -27,6 +27,18 @@ def _nchw(flat, N, C, H, W):
     return cx._act(flat, N, W, H, C)
 
 
+def _frames(h, T):
+    """(N, C*T, H, W) with frames as channel blocks -> (N, C, T, H, W)"""
+    N, CT, H, W = h.shape
+    return h.view(N, T, CT // T, H, W).transpose(1, 2)
+
+
+def _unframes(z):
+    """(N, C, T, H, W) -> (N, C*T, H, W), frame t at channels [C*t, C*t + C)"""
+    N, C, T, H, W = z.shape
+    return z.transpose(1, 2).reshape(N, T * C, H, W)
+
+
 def _flat(t):
     return cx._unact(t).contiguous()
 
@@ -51,7 +63,9 @@ def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None, fa
     """a Snapshot of one float32 step of `model` (a step_exact.Model).  seeds: per layer dropout seed (default: drawn);
     fprop_operands: {edge index: operand-model kind} rounds that edge's fprop operands like a tensor-core path;
     fault: 'relu_deriv' takes ReLU' instead of sigma' at every logistic layer, 'labels_deriv' makes a soft-target
-    output derivative against one-hot labels, 'adagrad_twice' adds the squared gradient to the Adagrad state twice"""
+    output derivative against one-hot labels, 'adagrad_twice' adds the squared gradient to the Adagrad state twice,
+    'frame_offset' starts the frame windows of every 3-D conv one frame apart instead of stride_t, 'drop_last_window'
+    leaves the last frame window of every 3-D pool unwritten (0)"""
     g = torch.Generator().manual_seed(seed)
     m = model
     L = len(m.layers)
@@ -78,7 +92,7 @@ def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None, fa
 
     P = params.clone().requires_grad_(True)
     states, zs = [x], [None]
-    h = _nchw(x, N, l0.C, l0.H, l0.W)
+    h = _nchw(x, N, l0.C * l0.T, l0.H, l0.W)
     for k, e in enumerate(m.edges):
         s, d = m.layers[e.src], m.layers[e.dst]
         if e.kind in se.WEIGHTED:
@@ -92,6 +106,11 @@ def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None, fa
                 xin = cx.MODELS[kind](h.detach()) + (h - h.detach())
             if e.kind == "FC":
                 z = (_flat(xin).view(-1, N).t() @ W.view(gg.K, gg.Cout) + b).view(N, d.C, 1, 1)
+            elif s.T > 1:                   # filter column c + Cin*dt: channel c of window frame dt
+                wt = W.view(gg.kt, gg.Cin, gg.ky, gg.kx, gg.Cout).permute(4, 1, 0, 2, 3)
+                st_t = 1 if fault == "frame_offset" else gg.st_t
+                z = tF.conv3d(_frames(xin, s.T), wt, b, stride=(st_t, gg.sy, gg.sx), padding=(0, gg.py, gg.px))
+                z = _unframes(z[:, :, :d.T])
             else:
                 wt = W.view(gg.Cin, gg.ky, gg.kx, gg.Cout).permute(3, 0, 1, 2)
                 z = tF.conv2d(xin, wt, b, stride=(gg.sy, gg.sx), padding=(gg.py, gg.px))
@@ -103,6 +122,16 @@ def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None, fa
         elif e.kind == "DOWNSAMPLE":
             f = int(e.cfg["sample_factor"])
             z = tF.avg_pool2d(h, f, f)
+        elif e.kind in ("MAXPOOL", "AVERAGE_POOL") and s.T > 1:
+            pg = m.pool_geo(e, N)
+            win = dict(kernel_size=(pg.kt, pg.ky, pg.kx), stride=(pg.st_t, pg.sy, pg.sx), padding=(pg.pt, pg.py, pg.px))
+            assert e.kind == "AVERAGE_POOL" or not any(win["padding"]) and all(          # windows that do not overlap
+                st == k or k == n for st, k, n in zip(win["stride"], win["kernel_size"], (s.T, s.H, s.W)))
+            z = (_MaxPool3dTies.apply(_frames(h, s.T), win["kernel_size"]) if e.kind == "MAXPOOL" else
+                 tF.avg_pool3d(_frames(h, s.T), count_include_pad=False, **win))
+            if fault == "drop_last_window":         # the last frame window never computed
+                z = torch.cat([z[:, :, :-1], torch.zeros_like(z[:, :, -1:])], 2)
+            z = _unframes(z)
         elif e.kind == "MAXPOOL":
             pg = m.pool_geo(e, N)
             z = tF.max_pool2d(h, (pg.ky, pg.kx), (pg.sy, pg.sx), (pg.py, pg.px))
@@ -129,7 +158,7 @@ def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None, fa
         if d.dropprob > 0:
             kept = cx.dropout_kept(d.floats(N), np.float32(d.dropprob), seeds[e.dst])
             mask = torch.from_numpy(kept).float() * se.dropout_scale(d.dropprob)
-            h = h * _nchw(mask, N, d.C, d.H, d.W)
+            h = h * _nchw(mask, N, d.C * d.T, d.H, d.W)
         states.append(_flat(h.detach()))
     C = m.layers[-1].floats(N) // N           # output features (units x pixels), image fastest like the targets
     p = _flat(h.detach()).view(C, N).t()
@@ -144,7 +173,7 @@ def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None, fa
     _, _, v, _ = lr.loss_ref(m.loss, p.double().numpy(), t=None if targets is None else targets.view(C, N).t().numpy(),
                              labels=labels.numpy(), weight=m.loss_weight)
     loss = float(m.loss_weight * v.sum())
-    zs[-1].backward(_nchw(dz.t().reshape(-1), N, m.layers[-1].C, m.layers[-1].H, m.layers[-1].W))
+    zs[-1].backward(_nchw(dz.t().reshape(-1), N, m.layers[-1].C * m.layers[-1].T, m.layers[-1].H, m.layers[-1].W))
     derivs = [None] + [_flat(z.grad) if m.receives_deriv(i + 1) else None for i, z in enumerate(zs[1:])]
     grads = torch.full((m.total,), float("nan"))
     grads.view(torch.int32).fill_(se.SENTINEL)
@@ -183,6 +212,25 @@ def simulate(model, N, seed=0, seeds=None, lr_scale=1.0, fprop_operands=None, fa
                 s_after[a:b] = torch.from_numpy(st)
     return se.Snapshot(N, labels, states, derivs, params, hist, grads, p_after, h_after, loss, seeds, opt_state,
                        targets, s_before, s_after)
+
+
+class _MaxPool3dTies(torch.autograd.Function):
+    """3-D max pooling over non-overlapping windows whose backward gives the gradient to EVERY element equal to its
+    window's maximum, as the reference's undo does (torch's picks one; ReLU layers tie at 0, often a whole window)"""
+
+    @staticmethod
+    def forward(ctx, x, k):
+        z = tF.max_pool3d(x, k, k)
+        ctx.save_for_backward(x, z)
+        ctx.k = k
+        return z
+
+    @staticmethod
+    def backward(ctx, dz):
+        x, z = ctx.saved_tensors
+        up = lambda t: t.repeat_interleave(ctx.k[0], 2).repeat_interleave(ctx.k[1], 3).repeat_interleave(  # noqa: E731
+            ctx.k[2], 4)[:, :, :x.shape[2], :x.shape[3], :x.shape[4]]
+        return torch.where(x == up(z), up(dz), torch.zeros_like(x)), None
 
 
 class _LogisticReluDeriv(torch.autograd.Function):
@@ -543,7 +591,40 @@ def test_tie_group_bias_missing_a_member():
     _caught(m, s, m.edges[o].name, "bias_grad")
 
 
-@pytest.mark.parametrize("name", ["tiny+bn", "lcnet", "c3d", "tiedcheck", "localcheck"])
+@pytest.fixture(scope="module")
+def video_model(tmp_path_factory):
+    path = str(tmp_path_factory.mktemp("model") / "video.pbtxt")
+    with open(path, "w") as f:
+        f.write(se.video_text())
+    return se.load_model(path, 4)
+
+
+def test_auditor_passes_3d_step(video_model):
+    """the small 3-D net: a conv with frame windows of 2, one of 3 at stride_t 2, 3-D max, average and global pools"""
+    m = video_model
+    assert [l.T for l in m.layers] == [8, 7, 7, 3, 2, 1, 1]
+    rows = _audit(m, simulate(m, 4))
+    assert not se.failures(rows), "\n".join(map(str, se.failures(rows)))
+    got = {(r.layer, r.quantity) for r in rows}
+    assert {("conv2", "fprop"), ("pool1", "dgrad"), ("pool1:conv2", "wgrad"), ("pool1:conv2", "bias_grad"),
+            ("pool2", "fprop"), ("conv2", "undo"), ("pool3", "fprop"), ("pool2", "undo")} <= got
+    assert "sum over 3 frames" in [r for r in rows if (r.layer, r.quantity) == ("pool1:conv2", "bias_grad")][0].detail
+
+
+def test_3d_conv_frame_offset_without_stride_t(video_model):
+    """conv2's frame windows started one frame apart instead of stride_t = 2 frames"""
+    _caught(video_model, simulate(video_model, 4, fault="frame_offset"), "conv2", "fprop")
+
+
+def test_3d_pool_drops_its_last_frame_window(video_model):
+    """the last frame window of the 3-D max pool (pool1: 7 frames) and average pool (pool2: 2 windows of 2 frames)
+    never written"""
+    s = simulate(video_model, 4, fault="drop_last_window")
+    _caught(video_model, s, "pool1", "fprop")
+    _caught(video_model, s, "pool2", "fprop")
+
+
+@pytest.mark.parametrize("name", ["tiny+bn", "lcnet", "tiedcheck", "localcheck"])
 def test_unsupported_models_raise(name):
     with pytest.raises(se.Unsupported):
         se.load_model(name, 32)
